@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py - headline benchmark of the B200-native RePlay sequential-recommender hot path.
+"""bench.py - headline benchmark of the H100-native RePlay sequential-recommender hot path.
 
-    python bench.py --gpus N --steps K --warmup W [--config 2|3|5]     # this repo's CUDA path (torchrun launches N>1)
+    python bench.py --gpus N --steps K --warmup W [--config 2|3|5] [--dump-outputs DIR]   # this repo's CUDA path (torchrun launches N>1)
     python bench.py --impl reference --gpus N --steps K ... [--config]  # the reference's CPU algorithm (oracle port), host cores
 
 --config 2 (default, BASELINE.json configs[1]): SASRec seq_len=200 d=128 H=2 2 blocks |items|=50 000, full-catalog CE, Adam,
@@ -16,7 +16,12 @@ One step = forward + backward + gradient all-reduce + Adam over one batch.  `val
 replays (replay_b200.trainer.Trainer).  `e2e`: the same step through the reference-facing Lightning mirror
 (`LightningModule.training_step` / legacy `Bert4Rec.training_step`) with PINNED HOST batches, host->device copies and a
 device->host read of the loss inside the timed region.  Timing: CUDA events on the launching stream, barrier + synchronize on
-both sides, max over ranks; every step works on > L2 of activations (no L2 flush needed; stated in `config`).
+both sides, max over ranks; every step works on > L2 of activations (no L2 flush needed; stated in `config`).  Every timed
+window of the training legs is --steps steps long.
+
+--dump-outputs DIR writes, after the timed steps, what the timed step computed in its last step (the loss, a fixed seeded
+sample of the updated fp32 parameters and of Adam's first moment - the running mean of the gradients the steps applied;
+the gradient buffer itself is zeroed by the optimizer) and the last scoring call's top-K as DIR/<name>.npy; the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -46,26 +51,13 @@ SCORE_CFG = dict(n_items=500_000, d=128, seq_len=200, k=10, users_per_call=4096,
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as fh:
-            z = json.load(fh)
-        return dict(hbm=z["hbm_gbs"], tc_burst=z["bf16_tflops"], tc_sustained=z["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, tc_burst=1590.0, tc_sustained=1400.0, src="fallback")
-
-
-def measured_traffic(key: str):
-    """dram__bytes_read + dram__bytes_write per launch of the named kernel from the committed ncu capture of THIS shape
-    (profiles/r2_traffic.json, written by tools/extract_traffic.py from the .ncu-rep); None if no capture exists for it."""
-    p = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    if not os.path.exists(p):
-        return None
-    with open(p) as fh:
-        return json.load(fh).get(key)
+    """Denominators of the roofline fractions: NVIDIA's data sheet of the H100 SXM (700 W): 3.35 TB/s HBM3, 989 TFLOP/s
+    dense bf16.  A data-sheet rate, not one this card reached: a lower power limit lowers the clocks (see `clocks`)."""
+    return dict(hbm=3350.0, tc=989.0, src="H100 SXM data sheet (700 W)")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index: int):
         self.rows, self.proc, self.index = [], None, index
@@ -116,7 +108,7 @@ def workload_string(c):
                 f"mask_prob {c['mask_prob']}, full-catalog CE over masked positions + Adam, dropout {c['dropout']}, synthetic windows "
                 "(activations per step > L2)")
     return (f"{c['name']}: SASRec L={c['seq_len']} d={c['d']} H={c['heads']} blocks={c['blocks']} |I|={c['n_items']}, full-catalog CE + Adam, "
-            f"dropout {c['dropout']}, MovieLens-shaped synthetic windows (inputs > L2: activations per step exceed the 126 MB L2)")
+            f"dropout {c['dropout']}, MovieLens-shaped synthetic windows (inputs > L2: activations per step exceed the 50 MB L2)")
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -213,13 +205,13 @@ def run_reference(args):
     if rank != 0:
         return
     c = CONFIGS[args.config]
-    n_timed = max(1, min(args.steps, 5 if args.config == 2 else 2))  # bounded sample: a CPU step of this workload takes seconds
-    v, med, _ = cpu_train_seq_per_s(c, steps=n_timed, warmup=1)
+    n_timed = max(1, args.steps)
+    v, med, _ = cpu_train_seq_per_s(c, steps=n_timed, warmup=max(0, args.warmup))
     cores = torch.get_num_threads()
     metric = "bert4rec_train_seq_per_s" if c["kind"] == "bert" else "sasrec_train_seq_per_s"
     line = {
         "impl": "reference", "metric": metric, "value": v, "unit": "seq/s", "n_gpus": args.gpus,
-        "steps": args.steps, "warmup": args.warmup, "ms_per_step": med * 1e3, "higher_is_better": True, "scaling": "weak",
+        "steps": n_timed, "warmup": max(0, args.warmup), "ms_per_step": med * 1e3, "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": workload_string(c) + " - CPU oracle port of the reference algorithm",
                    **{k: c[k] for k in ("seq_len", "d", "heads", "blocks", "n_items")}, "global_batch": c["cpu_batch"]},
@@ -346,6 +338,14 @@ def run_ours(args):
     ms, loss = timed(step_dev, K)
     clocks = sampler.stop() if rank == 0 else None
     final_loss = float(loss[0].item())
+    if args.dump_outputs and rank == 0:
+        # what the last timed step computed: its loss, and a fixed seeded sample of the parameters it updated and of Adam's
+        # first moment, which carries the gradients (the step's Adam launch zeroes the gradient buffer itself).  The full flat
+        # buffers are up to GBs; 1 M elements each keep the dump far below 64 MB.
+        n = eng.p32.numel()
+        pick = torch.randperm(n, generator=torch.Generator().manual_seed(0))[: min(n, 1 << 20)].sort().values.to(dev)
+        dump_outputs(args.dump_outputs, train_loss=loss[:1], params_sample=eng.p32[pick], adam_m_sample=eng.adam_m[pick],
+                     sample_index=pick)
     # ---- (N > 1) the gradient exchange alone: 20 back-to-back calls on the staged gradient, ranks in lock step
     exchange = None
     if world > 1:
@@ -356,10 +356,10 @@ def run_ours(args):
         exchange = {"kind": "rp_peer_allreduce (in-graph NVLink kernel)" if tr.peer is not None else "ncclAllReduce (eager, between two graphs)",
                     "ms": ms_x / 20, "bytes": int(eng.g32.numel() * 4), "balanced_batches": not args.no_balance}
         eng.g32.zero_()
-    # ---- sustained: the same step for >= 2 s (power / thermal steady state), clocks sampled over the whole window
+    # ---- sustained: the same steps once more right behind the first window, clocks sampled over the whole window
     sustained = None
     if not args.no_sustained:
-        n_sus = max(K, int(2500.0 / (ms / K)))
+        n_sus = K
         s2 = ClockSampler(local)
         if rank == 0:
             s2.start()
@@ -408,8 +408,8 @@ def run_ours(args):
         torch.cuda.synchronize()
         return a.elapsed_time(b) / iters
 
-    # ---- roofline of the dominant kernels: the tcgen05 CE-head kernels, timed live with CUDA events (standalone, same
-    # buffers as the last step; each launch streams > L2 worth of operands through TMEM/SMEM)
+    # ---- roofline of the dominant kernels: the CE-head kernels, timed live with CUDA events (standalone, same buffers as
+    # the last step; each launch streams > L2 worth of operands through shared memory)
     step_dev(0)
     torch.cuda.synchronize()
     n_valid = int(eng.n_valid.item())
@@ -428,17 +428,14 @@ def run_ours(args):
     ce_ms = t_fwd + t_bwd
     fused = bool(eng.fused_ce and d <= 256)
     n_exec = 4 if fused else 5  # GEMM-equivalents executed: fused fwd+dH (S, dH) + dE pass (S, dE); un-fused: S twice more
-    traffic = measured_traffic(f"ce_head_c{args.config}_b{B}")
     roof = {
         "bound": "tensor",
         "kernel": ("ce_bwd_kernel<FUSED> (fwd+dH) + ce_bwd_kernel<COL> (dE)" if fused else "ce_fwd_kernel + materialised-G GEMMs (d = 512)")
                   + ": logits GEMM + softmax-CE, fwd+bwd",
-        "achieved": 3 * gemm_flops / (ce_ms * 1e-3) / 1e12, "peak": PK["tc_burst"], "unit": "TFLOP/s",
-        "frac": 3 * gemm_flops / (ce_ms * 1e-3) / 1e12 / PK["tc_burst"],
-        # dram__bytes_read + dram__bytes_write per launch of the two passes (committed ncu capture of THIS shape), else null
-        "traffic": traffic,
+        "achieved": 3 * gemm_flops / (ce_ms * 1e-3) / 1e12, "peak": PK["tc"], "unit": "TFLOP/s",
+        "frac": 3 * gemm_flops / (ce_ms * 1e-3) / 1e12 / PK["tc"],
         "algorithmic_bytes": 2 * (I * d * 2 + n_valid * d * 2) + I * d * 4 + n_valid * d * 2,
-        "peak_source": PK["src"] + " burst (kernels timed alone)",
+        "peak_source": PK["src"] + " (kernels timed alone)",
         "detail": {"ce_fwd_ms": t_fwd, "ce_bwd_ms": t_bwd, "n_valid_targets": n_valid,
                    "algorithmic_flops_per_launch_pair": 3 * gemm_flops,
                    "executed_tflops": n_exec * gemm_flops / (ce_ms * 1e-3) / 1e12, "fused_fwd_dh": fused,
@@ -475,7 +472,7 @@ def run_ours(args):
                    "parallelism": f"dp{world}", "valid_targets_per_seq": valid_per_seq, "cuda_graph": not args.no_graph,
                    "batch_sharding": ("one rank" if world == 1 else
                                       ("index" if args.no_balance else "global batch dealt to the ranks by valid-target count")),
-                   "l2": "no flush: every step streams > 126 MB of activations / table"},
+                   "l2": "no flush: every step streams > 50 MB of activations / table"},
         "e2e": {"value": world * B * K / ms_e2e * 1e3, "unit": "seq/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4,
                 "ms_per_step": ms_e2e / K,
                 "path": ("LightningModule(SasRec).training_step" if c["kind"] == "sasrec" else "Bert4Rec.training_step")
@@ -486,8 +483,8 @@ def run_ours(args):
         "clocks": clocks,
         "roofline": roof,
         "step_roofline": {"credited_flops_per_seq": fl_seq, "achieved_tflops_per_gpu": step_tflops,
-                          "peak": PK["tc_sustained"], "frac": step_tflops / PK["tc_sustained"],
-                          "note": "whole step vs sustained bf16 peak; FLOPs per SURVEY 8d (valid targets only, x3 for train)"},
+                          "peak": PK["tc"], "frac": step_tflops / PK["tc"],
+                          "note": "whole step vs the data-sheet bf16 peak; FLOPs per SURVEY 8d (valid targets only, x3 for train)"},
         "cpu_baseline": cpu,
         "scoring": scoring,
         "final_loss": final_loss,
@@ -555,10 +552,12 @@ def run_scoring(args, dev, rank, world, PK, barrier, time_kernel):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for i in range(n_calls):
-            call_dev(i)
+            out = call_dev(i)
         e1.record()
         barrier()
         ms_dev = maxr(e0.elapsed_time(e1))
+        if args.dump_outputs and rank == 0 and Bu == sc["users_per_call"]:   # the headline call size: its last call's top-K
+            dump_outputs(args.dump_outputs, topk_ids=out[0], topk_scores=out[1])
         # end to end through the reference-facing callback
         cb = TorchTopItemsCallback(top_k=K, query_column="query_id", item_column="item_id",
                                    postprocessors=[SeenItemsFilter(item_count=I, seen_items_column="seen_ids")])
@@ -625,10 +624,21 @@ def run_scoring(args, dev, rank, world, PK, barrier, time_kernel):
             "value": cpu_predict_users_per_s(), "unit": "users/s", "cores": torch.get_num_threads(), "kind": "port",
             "sample": "64 users, 3 timed calls: oracle body + full logits + seen filter + torch.topk, torch fp32 CPU"},
         "roofline": {"bound": "tensor", "kernel": "score_topk_kernel", "achieved": head_flops / (t_head * 1e-3) / 1e12,
-                     "peak": PK["tc_burst"], "unit": "TFLOP/s", "frac": head_flops / (t_head * 1e-3) / 1e12 / PK["tc_burst"],
-                     "head_ms": t_head, "head_users_per_s": Bu / t_head * 1e3, "traffic": measured_traffic(f"score_topk_b{Bu}"),
+                     "peak": PK["tc"], "unit": "TFLOP/s", "frac": head_flops / (t_head * 1e-3) / 1e12 / PK["tc"],
+                     "head_ms": t_head, "head_users_per_s": Bu / t_head * 1e3,
                      "algorithmic_bytes": I * d * 2 + Bu * d * 2 + Bu * L * 4 + Bu * K * 12},
     }
+
+
+def dump_outputs(out_dir, **arrays):
+    """DIR/<name>.npy for every array: floating point as float32, integers (ids, indices) as float64 (exact below 2^53)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        a = t.double().numpy() if not t.is_floating_point() else t.float().numpy()
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def main():
@@ -648,6 +658,9 @@ def main():
     ap.add_argument("--batch", type=int, default=None, help="sequences per GPU and step (SURVEY 8d sweeps {128, 256, 512} at config 2)")
     ap.add_argument("--dropout", type=float, default=None, help="diagnostic override of the workload's dropout; "
                     "a run with this flag is not the benchmark configuration")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's loss, seeded samples of the updated parameters and of "
+                         "Adam's first moment, and the last scoring call's top-K as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,4 +1,4 @@
-/* rp_b200.h - C ABI of librp_b200.so: the B200 (sm_100a) kernels behind RePlay's sequential-recommender hot path.
+/* rp_b200.h - C ABI of librp_b200.so: the H100 (sm_90a) kernels behind RePlay's sequential-recommender hot path.
  *
  * The reference (sb-ai-lab/RePlay @ b4e051e8) has NO FFI on this path: its extension points are Python protocols and
  * Lightning hooks (SURVEY.md §8b).  Each entry point below therefore cites the reference *Python* call it replaces;
@@ -28,7 +28,7 @@ extern "C" {
 #define RP_EDRIVER (-4)    /* CUDA driver entry point unavailable / tensor-map encode failed */
 #define RP_EWORKSPACE (-5) /* workspace too small */
 
-/* library / build info: returns a static string such as "rp_b200 0.1 sm_100a" */
+/* library / build info: returns a static string such as "rp_b200 0.1 sm_90a" */
 const char* rp_version(void);
 
 /* ---------------------------------------------------------------------------------------------------------------
@@ -87,8 +87,8 @@ int rp_ce_head_fwd(const void* hc, const void* table, const float* bias, const i
 /* gradients of the mean CE for d(loss) = 1:  d_hc bf16 [capacity, d] (rows < *n_valid; already produced by the forward when
  * `fused` != 0 and the bound held, otherwise computed here); d_table fp32 [n_items, d] is OVERWRITTEN (softmax part) and
  * then atomically corrected by the one-hot part; d_bias fp32 [n_items] likewise iff bias.  `fused` must equal
- * (d_hc != NULL) of the matching forward call and then needs the same workspace.  d in {64,128,256}: fused tcgen05 passes
- * (logits never leave TMEM).  d = 512 (bias == NULL only): S plus a [128 x 512] fp32 accumulator exceed the 512 TMEM columns, so
+ * (d_hc != NULL) of the matching forward call and then needs the same workspace.  d in {64,128,256}: fused wgmma passes
+ * (logits never leave the registers).  d = 512 (bias == NULL only): a [128 x 512] fp32 accumulator does not fit them, so
  * the softmax numerators of a token chunk are materialised in bf16 inside the workspace (chunk sized by RP_CE_WIDE_G_BYTES,
  * default 8 GiB) and three GEMMs per chunk produce dH and dE; the workspace is then always required.
  * n_valid_hint: host estimate of *n_valid (0 = unknown), load-balance only. */
@@ -111,7 +111,7 @@ int rp_ce_head_bwd(const void* hc, const void* table, const float* bias, const i
  * Transformer body.  All activations are token-major bf16 [T = B*L, d]; weights are the bf16 shadow of the fp32 masters.
  * ------------------------------------------------------------------------------------------------------------- */
 
-/* Generic batched GEMM  C[m,n] = epilogue(alpha * sum_k A(m,k) B(n,k))  on tcgen05.
+/* Generic batched GEMM  C[m,n] = epilogue(alpha * sum_k A(m,k) B(n,k))  on wgmma.
  *   replaces  torch.nn.MultiheadAttention in/out projections   replay/nn/sequential/sasrec/transformer.py:36-46,99-106
  *             Conv1d(d,d,1) / Linear FFN layers                  replay/nn/ffn.py:43-57 ; models/nn/sequential/sasrec/model.py:490-506
  *                                                                models/nn/sequential/bert4rec/model.py:516-527
@@ -174,8 +174,8 @@ typedef struct rp_attn_desc {
 int rp_attn_fwd(const rp_attn_desc* a, void* stream);
 
 /* Fused attention backward (L <= 256, head_dim 64), one CTA per (sequence, head): recomputes S^T = K.Q^T and
- * dP^T = V.dO^T on tcgen05, forms P / dS in registers from the forward's row statistics (m_save, inv_sum) and accumulates
- * dV = Pd^T.dO, dK = dS^T.Q, dQ = dS.K with the bf16 operands staged in TMEM / swizzled shared memory - the [B*H, L, L]
+ * dP^T = V.dO^T on wgmma, forms P / dS in registers from the forward's row statistics (m_save, inv_sum) and accumulates
+ * dV = Pd^T.dO, dK = dS^T.Q, dQ = dS.K with the bf16 operands as register A operands (deterministic) - the [B*H, L, L]
  * matrices of the un-fused path are never written.  Replaces autograd's backward of the SDPA core of
  * torch.nn.MultiheadAttention (replay/nn/sequential/sasrec/transformer.py:99-106 ; bert4rec/model.py:494).
  * q/k/v/d_out/out: token-major 2-D bf16 arrays; dq/dk/dv: outputs (rows b*L + i, columns x_c0 + h*64). */
@@ -264,7 +264,7 @@ int rp_gather_rows(const void* src, const int32_t* idx, int n_max, const int32_t
                    void* stream);
 
 /* Inference / predict(): the whole point-wise FFN in one pass  out = relu(y W1^T + b1) W2^T + b2 + y  (weights resident in shared
- * memory, hidden activation kept in TMEM, residual read from the staged y tile): y is read once and out written once.
+ * memory, hidden activation kept in registers, residual read from the staged y tile): y is read once and out written once.
  *   replaces (eval)  SasRecPointWiseFeedForward.forward  replay/models/nn/sequential/sasrec/model.py:496-506 ; replay/nn/ffn.py:43-57
  * y, out bf16 [T, d] (no aliasing), w1 / w2 bf16 [d, d], b1 / b2 fp32 [d], rowmask optional uint8 [T] (0 -> zero row), d in {64,128}. */
 int rp_ffn_fused(const void* y, const void* w1, const float* b1, const void* w2, const float* b2, const uint8_t* rowmask, int T,
@@ -320,7 +320,7 @@ int rp_pre_attn_bwd(const void* dQ, const void* dKV, const void* dh, const void*
 
 /* ALL weight and bias gradients of one transformer block in one launch (+ one deterministic reduction launch):
  *   dW_i[n_out_i, n_in_i] (+)= dY_i[T, n_out_i]^T . X_i[T, n_in_i] ;  db_i[n_out_i] (+)= column sums of dY_i      i < n_pairs <= 8
- * dY_i / X_i are read in place (MN-major tcgen05 operands, contraction over the tokens); the bias gradient is one extra N = 16
+ * dY_i / X_i are read in place (MN-major wgmma operands, contraction over the tokens); the bias gradient is one extra N = 16
  * MMA per k-step against a tile of ones.  n_out, n_in multiples of 64; at most 48 output tiles of 128 x 128 in one call.
  *   replaces  autograd's weight / bias gradients of  replay/nn/sequential/sasrec/transformer.py:36-46,99-110 ;
  *             replay/nn/ffn.py:43-57 ; replay/models/nn/sequential/sasrec/model.py:407-414,490-506 ; bert4rec/model.py:471-527 */
@@ -406,15 +406,15 @@ int rp_build_batch(const int64_t* offsets, const int32_t* items, long long n_seq
                    uint8_t* pad_mask, int64_t* labels, uint8_t* aux_mask, int64_t* query_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * Bring-up self test of the tcgen05 operand encodings (used by tests/, not by the product path).
- * A, B: bf16 [128,128]; D: fp32 [128,128].  mode bit0: B given as Bt[K,N]; bit1: A staged through TMEM;
+ * Bring-up self test of the wgmma operand encodings (used by tests/, not by the product path).
+ * A, B: bf16 [128,128]; D: fp32 [128,128].  mode bit0: B given as Bt[K,N]; bit1: A read into registers;
  * bit2: A given as At[K,M].  D = A . B^T in every mode.
  * ------------------------------------------------------------------------------------------------------------- */
-int rp_selftest_umma(int mode, const void* A, const void* B, float* D, void* stream);
+int rp_selftest_mma(int mode, const void* A, const void* B, float* D, void* stream);
 /* TMA feed-rate probe (tools/probe_tma.py): every CTA streams `tiles` [box_rows x d] row tiles of a K-major bf16 table through
  * an 8-stage ring with no consumer. */
-/* tcgen05.mma issue-rate probe (tools/probe_mma.py): mode bit0 B MN-major, bit1 A from TMEM, bit2 A MN-major; every CTA issues
- * iters x 8 MMAs (128x128x16 bf16) and writes its elapsed SM cycles to cycles_out[blockIdx.x]. */
+/* wgmma issue-rate probe (tools/probe_mma.py): mode bit0 B MN-major, bit1 A from registers, bit2 A MN-major, bits 3-4 N = 128 /
+ * 256 / 64; one warpgroup per CTA issues iters x 8 MMAs (64xNx16 bf16) and writes its elapsed SM cycles to cycles_out[blockIdx.x]. */
 int rp_selftest_mma_probe(int mode, int iters, int grid, long long* cycles_out, void* stream);
 int rp_selftest_tma_probe(const void* table, long long rows, int d, int box_rows, int tiles, int same_tile, int grid,
                           void* stream);

@@ -7,7 +7,7 @@ import os
 from ctypes import c_char_p, c_float, c_int, c_int32, c_int64, c_size_t, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# RP_B200_LIB: load another build of the SAME C ABI (A/B timing of kernel variants inside one GPU call, tools/ab_env.sh)
+# RP_B200_LIB: load another build of the SAME C ABI (A/B timing of two builds of the kernels in one process)
 LIB_PATH = os.environ.get("RP_B200_LIB") or os.path.join(_HERE, "librp_b200.so")
 
 _lib = None
@@ -42,13 +42,13 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RpError(
-            f"{LIB_PATH} is missing: build it with `python -m replay_b200.build` (nvcc, sm_100a). "
+            f"{LIB_PATH} is missing: build it with `python -m replay_b200.build` (nvcc, sm_90a). "
             "replay_b200 has no CPU fallback."
         )
     L = ctypes.CDLL(LIB_PATH)
     P = c_void_p
     _sig(L.rp_version, c_char_p, [])
-    _sig(L.rp_selftest_umma, c_int, [c_int, P, P, P, P])
+    _sig(L.rp_selftest_mma, c_int, [c_int, P, P, P, P])
     _sig(L.rp_seen_prepare, c_int, [P, c_int, c_int, c_int, P, P, P])
     _sig(L.rp_score_topk_workspace, c_size_t, [c_int, c_int, c_int, c_int])
     _sig(L.rp_score_topk, c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, P, P, P, P, c_size_t, P])

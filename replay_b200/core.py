@@ -287,9 +287,8 @@ class SasRecCore(torch.nn.Module):
     # evaluated on the last W positions alone - same position embeddings (right-aligned), same result, W / L of the body work.
     # MovieLens-shaped histories at L = 200: ~1/3 of the users fit 64 positions, ~2/3 fit 128: the body of a 4096-user call
     # shrinks by a third.  One host read (bucket sizes + a left-padding check) and one extra pass of launches per bucket per
-    # call: measured through predict_step + TopItemsCallback (bench25, r2) it pays for large calls only - 32768 users per
-    # call 14.7 -> 12.5 ms, 4096 users 2.08 -> 2.25 ms (launch-bound) - so it engages from ``predict_bucket_min_batch`` users
-    # per call.  RP_PREDICT_BUCKETS=0 turns it off.
+    # call: it pays for large calls only (small calls are launch-bound), so it engages from ``predict_bucket_min_batch``
+    # users per call.  RP_PREDICT_BUCKETS=0 turns it off.
     predict_buckets = tuple(int(v) for v in os.environ.get("RP_PREDICT_BUCKETS", "64,128").split(",") if v and int(v) > 0)
     predict_bucket_min_users = 1024    # smaller buckets join the next wider one
     predict_bucket_min_batch = 8192    # calls with fewer users take the single full-window pass

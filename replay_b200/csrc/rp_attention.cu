@@ -1,6 +1,6 @@
 // rp_attention.cu - padded-sequence multi-head attention for L <= 512 (L > 256: head_dim 64 only) (SASRec causal + key-padding, BERT4Rec key-padding):
-// fused forward on tcgen05 (S = Q.K^T in TMEM -> masked softmax in registers -> P bf16 back into TMEM -> O = P.V),
-// and the row-wise softmax backward that sits between the batched backward GEMMs (rp_gemm).
+// fused forward on wgmma (S = Q.K^T in registers -> masked softmax in registers -> P bf16 as the register A operand of O = P.V),
+// the row-wise softmax backward that sits between the batched backward GEMMs (rp_gemm), and the fused backward (below).
 //
 // Replaces torch.nn.MultiheadAttention's scaled-dot-product core as configured by the reference:
 //   replay/nn/sequential/sasrec/transformer.py:36-46,99-106 + replay/nn/mask.py:18-51 (float [B*H,L,L] mask never built)
@@ -9,7 +9,7 @@
 // Fully masked query rows produce a zero output (torch >= 2.5 safe-softmax semantics of the training path).
 #include "rp_host.h"
 #include "rp_philox.cuh"
-#include "rp_sm100.cuh"
+#include "rp_sm90.cuh"
 
 namespace rp {
 
@@ -31,16 +31,15 @@ struct AttnParams {
 
 static constexpr float kLog2eA = 1.4426950408889634f;
 
-static constexpr int kAfThreads = 32 + 8 * 32;  // issuer warp + 8 softmax warps (lane quarter x even / odd 32-key chunks)
+static constexpr int kAfThreads = 256;  // two warpgroups: query rows [0, 64) and [64, 128) of the tile
 
-// KB = number of 256-key blocks the CTA keeps resident (1: L <= 256, 2: L <= 512).  S [128 x 256*KB] fp32 fills 256*KB
-// TMEM columns; P (bf16) is written back over its first half and O accumulates behind it.
-// A query row is shared by TWO threads (even / odd 32-key chunks; row max and row sum meet in shared memory): 8 softmax
-// warps per CTA, 16 per SM - the kernel is bound by the integer / exp work of the element-wise passes, not by the MMAs, and
-// 4 warps per CTA left the ALU pipe half idle (ncu r2c).  Warps whose 32 rows lie beyond L do nothing; 32 x 32 chunks above
-// the causal diagonal are zero-filled without loads, exponentials or dropout draws.
+// KB = number of 256-key blocks the CTA keeps resident (1: L <= 256, 2: L <= 512).  Q, K and V of the tile stay in shared
+// memory; each warpgroup walks the visible keys in 64-key chunks twice: pass 1 takes the row max of S = Q.K^T, pass 2
+// recomputes the chunk, forms P = exp(S - max) in registers (saved un-dropped to p_save if asked, then dropped) and
+// accumulates O += P.V with P as the register A operand.  Chunks entirely above the causal diagonal of a warpgroup's rows
+// are skipped (their P is zero).
 template <int HD, int KB>
-__global__ void __launch_bounds__(kAfThreads, 2)
+__global__ void __launch_bounds__(kAfThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
   constexpr int HC = HD / 64;                 // 64-wide head-dim chunks
@@ -53,19 +52,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   uint8_t* sK = sQ + Q_BYTES;
   uint8_t* sV = sK + KV_BYTES;
   __shared__ __align__(16) uint32_t s_colkey[256 * KB];   // dropout key of every key position
-  __shared__ float s_red[2][2][128];                        // [max | sum][chunk parity][row]
-  __shared__ uint64_t bar_load, bar_v, bar_s, bar_p, bar_o;
-  __shared__ uint64_t bar_pair[4][2][2];                    // [lane quarter][chunk parity of the loader][iteration parity]
-  __shared__ uint32_t tmem_slot;
+  __shared__ uint8_t s_keyok[256 * KB];                    // key position is real (j < L, and not padding if masked)
+  __shared__ uint64_t bar_load;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
   const int bz = b * p.H + h;
   const int L = p.L;
   // Inference: a query tile whose rows are ALL padding (left-padded windows: the first tile of every user with at most L - 128
-  // items, ~40 % of the MovieLens-shaped users at L = 200) produces nothing anybody reads - the new path masks pad positions as
-  // keys and never queries them, the legacy path zeroes pad rows after the block.  Such a CTA writes zeros and leaves before
-  // any load or MMA.  (Training keeps the rows: the backward reads their saved statistics.)
+  // items) produces nothing anybody reads - the new path masks pad positions as keys and never queries them, the legacy
+  // path zeroes pad rows after the block.  Such a CTA writes zeros and leaves before any load or MMA.  (Training keeps the
+  // rows: the backward reads their saved statistics.)
   if (p.pad_mask && p.inv_sum == nullptr && p.p_save == nullptr && p.m_save == nullptr) {
     const int r = q0 + (int)threadIdx.x;
     const int live = (threadIdx.x < 128 && r < L) ? (p.pad_mask[(size_t)b * L + r] != 0) : 0;
@@ -80,256 +76,158 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       return;
     }
   }
-  int nk = p.causal ? min(L, q0 + 128) : L;        // keys that can be visible to this query tile
-  const int nk32 = (nk + 31) & ~31;                // MMA N / K extent (<= 256 per block, KB blocks)
+  const int nk = p.causal ? min(L, q0 + 128) : L;  // keys that can be visible to this query tile
+  const int nk32 = (nk + 31) & ~31;                // extent of the saved probability rows
   const int n_boxes = (nk32 + 127) / 128;
+  const int n64 = (nk32 + 63) / 64;
 
   if (threadIdx.x == 0) {
     mbar_init(&bar_load, 1);
-    mbar_init(&bar_v, 1);
-    mbar_init(&bar_s, 1);
-    mbar_init(&bar_p, 8);
-    mbar_init(&bar_o, 1);
-    for (int t = 0; t < 16; ++t) mbar_init(&bar_pair[0][0][0] + t, 1);
     fence_barrier_init();
     const int row0 = b * L;
-    mbar_arrive_expect_tx(&bar_load, HC * 128 * 128 + HC * n_boxes * 128 * 128);
-    mbar_arrive_expect_tx(&bar_v, HC * n_boxes * 128 * 128);
+    mbar_arrive_expect_tx(&bar_load, HC * 128 * 128 + 2 * HC * n_boxes * 128 * 128);
     for (int c = 0; c < HC; ++c) {
       tma_load_2d(sQ + c * 16384, &tmQ, &bar_load, p.q_c0 + h * HD + c * 64, row0 + q0);
-      for (int bx = 0; bx < n_boxes; ++bx)
+      for (int bx = 0; bx < n_boxes; ++bx) {
         tma_load_2d(sK + c * KV_CHUNK + bx * 16384, &tmK, &bar_load, p.k_c0 + h * HD + c * 64, row0 + bx * 128);
+        tma_load_2d(sV + c * KV_CHUNK + bx * 16384, &tmV, &bar_load, p.v_c0 + h * HD + c * 64, row0 + bx * 128);
+      }
     }
-    for (int c = 0; c < HC; ++c)
-      for (int bx = 0; bx < n_boxes; ++bx)
-        tma_load_2d(sV + c * KV_CHUNK + bx * 16384, &tmV, &bar_v, p.v_c0 + h * HD + c * 64, row0 + bx * 128);
   }
-  if (warp == 0) {
-    __syncwarp();
-    tmem_alloc(&tmem_slot, 256 * KB);
-  } else if (p.drop_p > 0.f) {
-    for (int j = threadIdx.x - 32; j < 256 * KB; j += 256) s_colkey[j] = drop_col_key((uint32_t)j);
+  for (int j = threadIdx.x; j < 256 * KB; j += kAfThreads) {
+    s_colkey[j] = p.drop_p > 0.f ? drop_col_key((uint32_t)j) : 0u;
+    s_keyok[j] = (j < L) && (!p.mask_pad_keys || p.pad_mask[(size_t)b * L + j] != 0);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t tmem_o = tmem + 128 * KB;   // reuses the S columns behind the packed P once P is complete
 
-  if (warp == 0) {
-    if (elect_one()) {
-      mbar_wait(&bar_load, 0);
-      tc_fence_after();
+  const int t = threadIdx.x & 127, wg = threadIdx.x >> 7;
+  const int fr = frag_row(t), fc = frag_col(t);
+  const int ia = q0 + 64 * wg + fr, ib = ia + 8;   // the two query rows of this thread
+  const int wg_last = q0 + 64 * wg + 63;           // last query row of the warpgroup
+  const int n_live = p.causal ? min(n64, wg_last / 64 + 1) : n64;  // chunks with a visible key for some row of the warpgroup
+  const float sl2 = p.scale * kLog2eA;
+  const bool drop = p.drop_p > 0.f;
+  const uint32_t thr = drop ? (uint32_t)(p.drop_p * 4294967296.0) : 0u;
+  const float ks_drop = drop ? 1.f / (1.f - p.drop_p) : 1.f;
+  const unsigned long long seed_eff = p.seed + ((drop && p.seed_ptr) ? *p.seed_ptr : 0ull);
+  const uint32_t rk_a = drop ? drop_row_key(seed_eff, p.drop_off, (unsigned long long)bz * p.Lp + (unsigned long long)ia) : 0u;
+  const uint32_t rk_b = drop ? drop_row_key(seed_eff, p.drop_off, (unsigned long long)bz * p.Lp + (unsigned long long)ib) : 0u;
+  auto visible = [&](int key, int i) -> bool { return s_keyok[key] && (!p.causal || key <= i); };
+  const uint32_t q_base = smem_u32(sQ) + wg * 8192;
+  auto qk_chunk = [&](float (&sacc)[32], int j0) {
+    wg_fence();
 #pragma unroll
-      for (int kb = 0; kb < KB; ++kb) {           // one MMA N extent is at most 256 keys
-        const int nb = min(256, nk32 - kb * 256);
-        if (nb <= 0) break;
-        const uint32_t idesc1 = umma_idesc_bf16(128, nb);
+    for (int c = 0; c < HC; ++c)
 #pragma unroll
-        for (int c = 0; c < HC; ++c)
+      for (int ks = 0; ks < 4; ++ks)
+        WgmmaSS<64>::template run<0, 0>(sacc, desc_k(q_base + c * 16384 + ks * 32),
+                                        desc_k(smem_u32(sK) + c * KV_CHUNK + j0 * 128 + ks * 32), (c | ks) != 0);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(sacc);
+  };
+  mbar_wait(&bar_load, 0);
+
+  // ---- pass 1: row max over the visible keys
+  float mxa = -INFINITY, mxb = -INFINITY;
+  for (int ch = 0; ch < n_live; ++ch) {
+    float sacc[32];
+    qk_chunk(sacc, ch * 64);
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks)
-            umma_ss(tmem + kb * 256, umma_desc_sw128(smem_u32(sQ) + c * 16384 + ks * 32, 16, 1024),
-                    umma_desc_sw128(smem_u32(sK) + c * KV_CHUNK + kb * 32768 + ks * 32, 16, 1024), idesc1, (c | ks) != 0);
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int key = ch * 64 + 8 * j + fc + e;
+        if (visible(key, ia)) mxa = fmaxf(mxa, sacc[4 * j + e]);
+        if (visible(key, ib)) mxb = fmaxf(mxb, sacc[4 * j + 2 + e]);
       }
-      umma_commit(&bar_s);
-      // ---- second GEMM once the softmax warps have written P
-      mbar_wait(&bar_v, 0);
-      mbar_wait(&bar_p, 0);
-      tc_fence_after();
-      constexpr uint32_t idesc2 = umma_idesc_bf16(128, HD, false, true);
-      for (int ks = 0; ks < nk32 / 16; ++ks)
-        umma_ts(tmem_o, tmem + ks * 8, umma_desc_sw128(smem_u32(sV) + ks * 2048, KV_CHUNK, 1024), idesc2, ks != 0);
-      umma_commit(&bar_o);
+  }
+#pragma unroll
+  for (int o = 1; o <= 2; o <<= 1) {
+    mxa = fmaxf(mxa, __shfl_xor_sync(0xffffffffu, mxa, o));
+    mxb = fmaxf(mxb, __shfl_xor_sync(0xffffffffu, mxb, o));
+  }
+  const float moa = (mxa == -INFINITY) ? 0.f : mxa * sl2, mob = (mxb == -INFINITY) ? 0.f : mxb * sl2;
+
+  // ---- pass 2: P = exp2(S * scale * log2e - max), row sums, optional copy of the un-dropped P, O += P.V
+  __nv_bfloat16* pa = (p.p_save && ia < L) ? p.p_save + ((size_t)bz * p.Lp + ia) * p.Lp : nullptr;
+  __nv_bfloat16* pb = (p.p_save && ib < L) ? p.p_save + ((size_t)bz * p.Lp + ib) * p.Lp : nullptr;
+  float oacc[HD / 2];
+  acc_zero(oacc);
+  float suma = 0.f, sumb = 0.f;
+  for (int ch = 0; ch < n_live; ++ch) {
+    float sacc[32];
+    qk_chunk(sacc, ch * 64);
+    uint32_t pk[16];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int key = ch * 64 + 8 * j + fc;
+      float ea[2], eb[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        ea[e] = visible(key + e, ia) ? ex2f(fmaf(sacc[4 * j + e], sl2, -moa)) : 0.f;
+        eb[e] = visible(key + e, ib) ? ex2f(fmaf(sacc[4 * j + 2 + e], sl2, -mob)) : 0.f;
+        suma += ea[e];
+        sumb += eb[e];
+      }
+      if (key < nk32) {
+        if (pa) *reinterpret_cast<uint32_t*>(pa + key) = pack_bf16(ea[0], ea[1]);
+        if (pb) *reinterpret_cast<uint32_t*>(pb + key) = pack_bf16(eb[0], eb[1]);
+      }
+      if (drop) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const uint32_t ck = s_colkey[key + e];
+          ea[e] = drop_mix(rk_a, ck) >= thr ? ea[e] * ks_drop : 0.f;
+          eb[e] = drop_mix(rk_b, ck) >= thr ? eb[e] * ks_drop : 0.f;
+        }
+      }
+      pk[2 * j] = pack_bf16(ea[0], ea[1]);
+      pk[2 * j + 1] = pack_bf16(eb[0], eb[1]);
     }
-  } else {
-    // ------------------------------------------------ softmax warps: thread = (query row, chunk parity)
-    const int quarter = warp & 3, par = (warp - 1) >> 2;
-    const int row = quarter * 32 + lane;
-    const int i = q0 + row;                 // query position inside the sequence
-    const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;
-    const bool warp_live = q0 + quarter * 32 < L;        // some row of this warp is a real query
-    const int n_chunks = nk32 / 32;
-    // chunks at or below the causal diagonal of this warp's LAST row; the rest of the tile's key extent is masked for
-    // every row of the warp
-    const int n_vis = p.causal ? min(n_chunks, (q0 + quarter * 32 + 31) / 32 + 1) : n_chunks;
-    // key-visibility bit masks of this thread's chunks (chunk c = 2 t + par), 32 keys per word
-    uint32_t kmask[4 * KB];
-    {
-      uint8_t pm[4 * KB];   // all loads first: a ballot per load serialises their latencies
+    wg_fence();
 #pragma unroll
-      for (int t = 0; t < 4 * KB; ++t) {
-        const int j = (2 * t + par) * 32 + lane;
-        pm[t] = (j < L && p.mask_pad_keys) ? p.pad_mask[(size_t)b * L + j] : (uint8_t)(j < L);
-      }
-#pragma unroll
-      for (int t = 0; t < 4 * KB; ++t) kmask[t] = __ballot_sync(0xffffffffu, pm[t] != 0);
+    for (int kk = 0; kk < 4; ++kk) {  // 16 keys per step: A fragment = P columns [16 kk, 16 kk + 16) of the chunk
+      const uint32_t a[4] = {pk[4 * kk], pk[4 * kk + 1], pk[4 * kk + 2], pk[4 * kk + 3]};
+      WgmmaRS<HD>::template run<1>(oacc, a, desc_mn(smem_u32(sV) + (ch * 4 + kk) * 2048, KV_CHUNK), 1);
     }
-    const float sl2 = p.scale * kLog2eA;
-    const bool drop = p.drop_p > 0.f;
-    const uint32_t thr = drop ? (uint32_t)(p.drop_p * 4294967296.0) : 0u;
-    const float ks_drop = drop ? 1.f / (1.f - p.drop_p) : 1.f;
-    const unsigned long long seed_eff = p.seed + ((drop && p.seed_ptr) ? *p.seed_ptr : 0ull);
-    const uint32_t row_key = drop ? drop_row_key(seed_eff, p.drop_off, (unsigned long long)bz * p.Lp + (unsigned long long)i) : 0u;
-    auto vis_mask = [&](int c) -> uint32_t {
-      uint32_t m = 0;
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(oacc);
+  }
+  // probability rows of the chunks above the diagonal of this warpgroup are zero
+  for (int ch = n_live; ch < n64; ++ch)
 #pragma unroll
-      for (int t = 0; t < 4 * KB; ++t)
-        if (2 * t + par == c) m = kmask[t];
-      if (p.causal) {
-        const int rel = i - c * 32;
-        const uint32_t cm = rel >= 31 ? 0xffffffffu : (rel < 0 ? 0u : ((2u << rel) - 1u));
-        m &= cm;
-      }
-      return m;
-    };
-    mbar_wait_relaxed(&bar_s, 0);
-    tc_fence_after();
-    // pass 1: row max over the visible keys of this thread's chunks
-    float mx = -INFINITY;
-    if (warp_live) {
-      for (int c = par; c < n_vis; c += 2) {
-        const uint32_t vm = vis_mask(c);
-        if (__all_sync(0xffffffffu, vm == 0u)) continue;
-        uint32_t raw[32];
-        tmem_ld32(tmem + lane_base + c * 32, raw);
-        tmem_ld_wait();
-        if (vm == 0xffffffffu) {  // chunk entirely visible (the common case below the diagonal): no per-element selects
-          float m0 = __uint_as_float(raw[0]), m1 = __uint_as_float(raw[1]), m2 = __uint_as_float(raw[2]), m3 = __uint_as_float(raw[3]);
-#pragma unroll
-          for (int q = 4; q < 32; q += 4) {
-            m0 = fmaxf(m0, __uint_as_float(raw[q]));
-            m1 = fmaxf(m1, __uint_as_float(raw[q + 1]));
-            m2 = fmaxf(m2, __uint_as_float(raw[q + 2]));
-            m3 = fmaxf(m3, __uint_as_float(raw[q + 3]));
-          }
-          mx = fmaxf(mx, fmaxf(fmaxf(m0, m1), fmaxf(m2, m3)));
-        } else if (vm != 0u) {
-#pragma unroll
-          for (int q = 0; q < 32; ++q)
-            if (vm & (1u << q)) mx = fmaxf(mx, __uint_as_float(raw[q]));
-        }
+    for (int j = 0; j < 8; ++j) {
+      const int key = ch * 64 + 8 * j + fc;
+      if (key < nk32) {
+        if (pa) *reinterpret_cast<uint32_t*>(pa + key) = 0u;
+        if (pb) *reinterpret_cast<uint32_t*>(pb + key) = 0u;
       }
     }
-    s_red[0][par][row] = mx;
-    named_bar_sync(1 + quarter, 64);   // the two warps of this lane quarter
-    mx = fmaxf(mx, s_red[0][par ^ 1][row]);
-    const float moff = (mx == -INFINITY) ? 0.f : mx * sl2;
-    // pass 2: exponentials, row sum, P (bf16) back into TMEM over S, optional copy of the un-dropped P to global
-    float sum = 0.f;
-    __nv_bfloat16* prow =
-        (p.p_save && i < L) ? p.p_save + ((size_t)bz * p.Lp + i) * p.Lp : nullptr;
-    // The packed P chunk c lands on columns [16 c, 16 c + 16) = inside S chunk c / 2, which belongs to this row's OTHER
-    // thread for every second chunk.  S chunk t is loaded in iteration t / 2 and stored over in iteration t, so each warp
-    // announces "my loads of iteration t are done" (mbarrier, before its exponentials) and checks the partner warp's
-    // announcement of the same iteration right before its store - by then it has long been made.  Two mbarriers per
-    // direction alternate by iteration: a warp can be at most one announcement ahead of its partner's check.
-    for (int t = 0; 2 * t < n_chunks; ++t) {
-      const int c = 2 * t + par;
-      const bool active = warp_live && c < n_chunks;
-      const uint32_t vm = (active && c < n_vis) ? vis_mask(c) : 0u;
-      const bool blank = !active || __all_sync(0xffffffffu, vm == 0u);  // masked for the whole warp: nothing loaded or drawn
-      uint32_t raw[32];
-      if (!blank) {
-        tmem_ld32(tmem + lane_base + c * 32, raw);
-        tmem_ld_wait();
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_pair[quarter][par][t & 1]);
-      if (!active) continue;
-      uint32_t pk[16];
-      if (blank) {
 #pragma unroll
-        for (int q = 0; q < 16; ++q) pk[q] = 0u;
-        if (prow) {
-#pragma unroll
-          for (int q = 0; q < 32; q += 8) *reinterpret_cast<uint4*>(prow + c * 32 + q) = make_uint4(0u, 0u, 0u, 0u);
-        }
-      } else {
-        float e[32];
-        if (vm == 0xffffffffu) {
-#pragma unroll
-          for (int q = 0; q < 32; ++q) {
-            e[q] = ex2f(fmaf(__uint_as_float(raw[q]), sl2, -moff));
-            sum += e[q];
-          }
-        } else {
-#pragma unroll
-          for (int q = 0; q < 32; ++q) {
-            const float v = ex2f(fmaf(__uint_as_float(raw[q]), sl2, -moff));
-            e[q] = (vm & (1u << q)) ? v : 0.f;
-            sum += e[q];
-          }
-        }
-        if (prow) {
-#pragma unroll
-          for (int q = 0; q < 32; q += 8) {
-            uint4 w;
-            w.x = pack_bf16(e[q], e[q + 1]);
-            w.y = pack_bf16(e[q + 2], e[q + 3]);
-            w.z = pack_bf16(e[q + 4], e[q + 5]);
-            w.w = pack_bf16(e[q + 6], e[q + 7]);
-            *reinterpret_cast<uint4*>(prow + c * 32 + q) = w;
-          }
-        }
-        if (drop) {
-          const uint4* ck = reinterpret_cast<const uint4*>(s_colkey + c * 32);
-#pragma unroll
-          for (int q = 0; q < 32; q += 4) {
-            const uint4 k4 = ck[q >> 2];
-            e[q] = drop_mix(row_key, k4.x) >= thr ? e[q] * ks_drop : 0.f;
-            e[q + 1] = drop_mix(row_key, k4.y) >= thr ? e[q + 1] * ks_drop : 0.f;
-            e[q + 2] = drop_mix(row_key, k4.z) >= thr ? e[q + 2] * ks_drop : 0.f;
-            e[q + 3] = drop_mix(row_key, k4.w) >= thr ? e[q + 3] * ks_drop : 0.f;
-          }
-        }
-#pragma unroll
-        for (int q = 0; q < 32; q += 2) pk[q >> 1] = pack_bf16(e[q], e[q + 1]);
-      }
-      mbar_wait(&bar_pair[quarter][par ^ 1][t & 1], (t >> 1) & 1);
-      tc_fence_after();
-      tmem_st16(tmem + lane_base + c * 16, pk);
+  for (int o = 1; o <= 2; o <<= 1) {
+    suma += __shfl_xor_sync(0xffffffffu, suma, o);
+    sumb += __shfl_xor_sync(0xffffffffu, sumb, o);
+  }
+  const float inva = suma > 0.f ? 1.f / suma : 0.f, invb = sumb > 0.f ? 1.f / sumb : 0.f;
+  if (fc == 0) {
+    if (ia < L) {
+      if (p.inv_sum) p.inv_sum[(size_t)bz * p.Lp + ia] = inva;
+      if (p.m_save) p.m_save[(size_t)bz * p.Lp + ia] = moa;
     }
-    if (warp_live) tmem_st_wait();
-    s_red[1][par][row] = sum;
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&bar_p);
-    named_bar_sync(1 + quarter, 64);   // the two warps of this lane quarter
-    sum += s_red[1][par ^ 1][row];
-    const float inv = sum > 0.f ? 1.f / sum : 0.f;
-    if (par == 0 && i < L) {
-      if (p.inv_sum) p.inv_sum[(size_t)bz * p.Lp + i] = inv;
-      if (p.m_save) p.m_save[(size_t)bz * p.Lp + i] = moff;
-    }
-    // ---- O = (P.V) / sum : chunk parity 0 stores the even 32-column groups of the head, parity 1 the odd ones
-    mbar_wait_relaxed(&bar_o, 0);
-    tc_fence_after();
-    if (warp_live) {
-#pragma unroll
-      for (int c = par * 32; c < HD; c += 64) {
-        uint32_t raw[32];
-        tmem_ld32(tmem_o + lane_base + c, raw);
-        tmem_ld_wait();
-        if (i < L) {
-          __nv_bfloat16* o = p.out + ((size_t)b * L + i) * p.ldo + h * HD + c;
-#pragma unroll
-          for (int q = 0; q < 32; q += 8) {
-            uint4 w;
-            w.x = pack_bf16(__uint_as_float(raw[q]) * inv, __uint_as_float(raw[q + 1]) * inv);
-            w.y = pack_bf16(__uint_as_float(raw[q + 2]) * inv, __uint_as_float(raw[q + 3]) * inv);
-            w.z = pack_bf16(__uint_as_float(raw[q + 4]) * inv, __uint_as_float(raw[q + 5]) * inv);
-            w.w = pack_bf16(__uint_as_float(raw[q + 6]) * inv, __uint_as_float(raw[q + 7]) * inv);
-            *reinterpret_cast<uint4*>(o + q) = w;
-          }
-        }
-      }
+    if (ib < L) {
+      if (p.inv_sum) p.inv_sum[(size_t)bz * p.Lp + ib] = invb;
+      if (p.m_save) p.m_save[(size_t)bz * p.Lp + ib] = mob;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem, 256 * KB);
+  // ---- O = (P.V) / sum
+#pragma unroll
+  for (int j = 0; j < HD / 8; ++j) {
+    const int c = h * HD + 8 * j + fc;
+    if (ia < L) *reinterpret_cast<uint32_t*>(p.out + ((size_t)b * L + ia) * p.ldo + c) = pack_bf16(oacc[4 * j] * inva, oacc[4 * j + 1] * inva);
+    if (ib < L) *reinterpret_cast<uint32_t*>(p.out + ((size_t)b * L + ib) * p.ldo + c) = pack_bf16(oacc[4 * j + 2] * invb, oacc[4 * j + 3] * invb);
+  }
 }
 
 // Row-wise softmax backward between the batched GEMMs.  One warp per (batch*head, query) row.
@@ -611,6 +509,302 @@ RP_API int rp_attn_softmax_bwd(void* p_save, void* dpd, const float* inv_sum, in
     attn_softmax_bwd_kernel<2><<<(int)blocks, 256, 0, stream>>>(reinterpret_cast<__nv_bfloat16*>(p_save),
                                                                 reinterpret_cast<__nv_bfloat16*>(dpd), inv_sum, BH, L, Lp, scale,
                                                                 drop_p, seed, drop_off, seed_ptr);
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+// ==================================================================================================================
+// Fused attention backward on wgmma for L <= 256, head_dim 64: one CTA per (sequence, head).
+//
+// Replaces autograd's backward of torch.nn.MultiheadAttention's SDPA core
+// (replay/nn/sequential/sasrec/transformer.py:99-106, models/nn/sequential/sasrec/model.py:435, bert4rec/model.py:494)
+// without materialising the [B*H, L, L] probability / gradient matrices the un-fused path needs.
+//
+// Q, K, V, dO and O of the (sequence, head) stay in shared memory.  The two warpgroups work on 64-row blocks:
+//   phase 1, rows = keys (block kb):   for every 64-query step qs
+//     S^T = K_kb . Q_qs^T, dP^T = V_kb . dO_qs^T       (registers)
+//     P = exp2(s*sl2 - m_i) * inv_i (masked), dS = P * (dP * dropmask/keep - delta_i) * scale, Pd = P * dropmask/keep
+//     dV_kb += Pd^T . dO_qs,  dK_kb += dS^T . Q_qs    (bf16 Pd^T / dS^T as register A operands)
+//   phase 2, rows = queries (block qb): for every 64-key block kb the same S, dP, dS (recomputed), dQ_qb += dS . K_kb
+// Every gradient element is summed by one warpgroup in a fixed order (deterministic, no atomics); causally empty blocks
+// are skipped.  Row statistics m_i (max in exp2 units) and inv_i (1/rowsum) come from the forward; delta_i = sum_c dO[i,c] O[i,c].
+
+namespace rp {
+
+struct AttnBwdParams {
+  int B, H, L, Lp;
+  int causal, mask_pad_keys;
+  float scale;
+  const uint8_t* pad_mask;
+  const float* m_save;         // [B*H, Lp]
+  const float* inv_sum;        // [B*H, Lp]
+  __nv_bfloat16* dQ; int ld_dq, dq_c0;   // outputs: rows b*L + i, columns x_c0 + h*64
+  __nv_bfloat16* dK; int ld_dk, dk_c0;
+  __nv_bfloat16* dV; int ld_dv, dv_c0;
+  int q_c0, k_c0, v_c0;        // column offsets of head 0 inside the Q / K / V arrays (tensor maps)
+  float drop_p;
+  unsigned long long seed, drop_off;
+  const unsigned long long* seed_ptr;
+};
+
+static constexpr int kAbThreads = 256;   // two warpgroups
+
+// the five 3-D tensor maps [B][L][columns] (box 128 rows x 64 columns, rows >= L out of bounds: zero-filled)
+struct AttnBwdMaps {
+  CUtensorMap q, k, v, d_o, o;
+};
+
+// dS and Pd of the 64 x 64 block held as an accumulator fragment pair (S, dP).  KEYS_ROWS: fragment rows are keys, columns
+// queries (phase 1); otherwise rows are queries, columns keys (phase 2).  r0 / c0: first row / column position of the block.
+// Results packed as bf16 A fragments: pk_s = dS, pk_p = Pd (element order of the accumulator).
+template <bool KEYS_ROWS>
+__device__ __forceinline__ void attn_bwd_block(const float (&sa)[32], const float (&dpa)[32], uint32_t (&pk_s)[16], uint32_t (&pk_p)[16],
+                                               const float4* __restrict__ s_stat, const uint8_t* __restrict__ s_keyok,
+                                               const uint32_t* __restrict__ s_colkey, int r0, int c0, int L, bool causal,
+                                               float sl2, float scale, bool drop, uint32_t thr, float ks_drop) {
+  const int t = threadIdx.x & 127;
+  const int fr = frag_row(t), fc = frag_col(t);
+  const float keep_s = ks_drop * scale;
+#pragma unroll
+  for (int q = 0; q < 8; ++q)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {   // h: fragment row fr (0) or fr + 8 (1)
+      float ds2[2], pd2[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int rr = r0 + fr + 8 * h, cc = c0 + 8 * q + fc + e;
+        const int i = KEYS_ROWS ? cc : rr, j = KEYS_ROWS ? rr : cc;   // query, key
+        const float4 st = s_stat[i];   // m, 1/sum, delta * scale, row key (bits)
+        const float pr = ex2f(fmaf(sa[4 * q + 2 * h + e], sl2, -st.x)) * st.y;
+        float kp = ks_drop, kps = keep_s;
+        if (drop) {
+          const bool keep = drop_mix(__float_as_uint(st.w), s_colkey[j]) >= thr;
+          kp = keep ? ks_drop : 0.f;
+          kps = keep ? keep_s : 0.f;
+        }
+        const bool vis = s_keyok[j] && i < L && (!causal || j <= i);
+        ds2[e] = vis ? pr * fmaf(dpa[4 * q + 2 * h + e], kps, -st.z) : 0.f;
+        pd2[e] = vis ? pr * kp : 0.f;
+      }
+      pk_s[2 * q + h] = pack_bf16(ds2[0], ds2[1]);
+      pk_p[2 * q + h] = pack_bf16(pd2[0], pd2[1]);
+    }
+}
+
+__global__ void __launch_bounds__(kAbThreads, 1)
+attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
+  constexpr int HD = 64;
+  constexpr int TILE = 128 * 128;  // bytes of one [128 rows x 64 bf16] swizzled tile; 64-row block b at + b * 8192
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem;               // 2 tiles each (rows 0-127, 128-255)
+  uint8_t* sdO = sQ + 2 * TILE;
+  uint8_t* sK = sdO + 2 * TILE;
+  uint8_t* sV = sK + 2 * TILE;
+  uint8_t* sO = sV + 2 * TILE;
+  __shared__ float4 s_stat[256];    // per query: m, 1/sum, delta * scale, dropout row key
+  __shared__ uint8_t s_keyok[256];
+  __shared__ __align__(16) uint32_t s_colkey[256];
+  __shared__ uint64_t bar_load;
+
+  const int h = blockIdx.x % p.H, b = blockIdx.x / p.H;
+  const int bz = b * p.H + h;
+  const int L = p.L;
+  const int n_t = (L + 127) / 128;  // 128-row tiles
+  const int n_blk = (L + 63) / 64;  // 64-row blocks
+  const bool drop = p.drop_p > 0.f;
+
+  if (threadIdx.x == 0) {
+    mbar_init(&bar_load, 1);
+    fence_barrier_init();
+    mbar_arrive_expect_tx(&bar_load, 5 * n_t * TILE);
+    for (int t = 0; t < n_t; ++t) {
+      tma_load_3d(sK + t * TILE, &tm.k, &bar_load, p.k_c0 + h * HD, t * 128, b);
+      tma_load_3d(sQ + t * TILE, &tm.q, &bar_load, p.q_c0 + h * HD, t * 128, b);
+      tma_load_3d(sV + t * TILE, &tm.v, &bar_load, p.v_c0 + h * HD, t * 128, b);
+      tma_load_3d(sdO + t * TILE, &tm.d_o, &bar_load, h * HD, t * 128, b);
+      tma_load_3d(sO + t * TILE, &tm.o, &bar_load, h * HD, t * 128, b);
+    }
+  }
+  __syncthreads();
+  {
+    // row statistics of this (sequence, head): m, 1/sum from the forward, delta = sum_c dO[i,c] O[i,c], the dropout keys
+    const int i = threadIdx.x, ti = i >> 7, r = i & 127;
+    const unsigned long long seed_eff = p.seed + ((drop && p.seed_ptr) ? *p.seed_ptr : 0ull);
+    float m = 0.f, inv = 0.f, dl = 0.f;
+    if (i < L) {
+      m = p.m_save[(size_t)bz * p.Lp + i];
+      inv = p.inv_sum[(size_t)bz * p.Lp + i];
+    }
+    const uint32_t rk = drop_row_key(seed_eff, p.drop_off, (unsigned long long)bz * p.Lp + (unsigned long long)i);
+    s_keyok[i] = i < L && (!p.mask_pad_keys || p.pad_mask[(size_t)b * L + i] != 0);
+    s_colkey[i] = drop_col_key((uint32_t)i);
+    mbar_wait(&bar_load, 0);
+    if (ti < n_t) {
+#pragma unroll
+      for (int c = 0; c < HD / 8; ++c) {
+        const uint4 ov = *reinterpret_cast<const uint4*>(sO + ti * TILE + sw128_off((uint32_t)r, (uint32_t)c));
+        const uint4 dv = *reinterpret_cast<const uint4*>(sdO + ti * TILE + sw128_off((uint32_t)r, (uint32_t)c));
+        const __nv_bfloat162* o2 = reinterpret_cast<const __nv_bfloat162*>(&ov);
+        const __nv_bfloat162* d2 = reinterpret_cast<const __nv_bfloat162*>(&dv);
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+          const float2 a = __bfloat1622float2(o2[t]), g = __bfloat1622float2(d2[t]);
+          dl = fmaf(a.x, g.x, fmaf(a.y, g.y, dl));
+        }
+      }
+    }
+    s_stat[i] = make_float4(m, inv, dl * p.scale, __uint_as_float(rk));
+  }
+  __syncthreads();
+
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  const int fr = frag_row(t), fc = frag_col(t);
+  const float sl2 = p.scale * kLog2eA;
+  const uint32_t thr = drop ? (uint32_t)(p.drop_p * 4294967296.0) : 0u;
+  const float ks_drop = drop ? 1.f / (1.f - p.drop_p) : 1.f;
+  const uint32_t aQ = smem_u32(sQ), adO = smem_u32(sdO), aK = smem_u32(sK), aV = smem_u32(sV);
+  // S-type products of two 64-row blocks: X_x . Y_y^T (both K-major over the 64 head dims)
+  auto qk = [&](float (&acc)[32], uint32_t x, uint32_t y) {
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) WgmmaSS<64>::template run<0, 0>(acc, desc_k(x + ks * 32), desc_k(y + ks * 32), ks != 0);
+  };
+  auto store_rows = [&](const float (&acc)[32], __nv_bfloat16* base, int ld, int c0, int r0) {
+    const int ra = r0 + fr, rb = ra + 8;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int c = c0 + h * HD + 8 * j + fc;
+      if (ra < L) *reinterpret_cast<uint32_t*>(base + ((size_t)b * L + ra) * ld + c) = pack_bf16(acc[4 * j], acc[4 * j + 1]);
+      if (rb < L) *reinterpret_cast<uint32_t*>(base + ((size_t)b * L + rb) * ld + c) = pack_bf16(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+  };
+  // blocks of this warpgroup: wg and 3 - wg (balances the causal triangle)
+#pragma unroll 1
+  for (int u = 0; u < 2; ++u) {
+    const int kb = u == 0 ? wg : 3 - wg;
+    if (kb >= n_blk) continue;
+    // ---- phase 1: rows = keys of block kb
+    float dk[32], dv[32];
+    acc_zero(dk);
+    acc_zero(dv);
+#pragma unroll 1
+    for (int qs = p.causal ? kb : 0; qs < n_blk; ++qs) {
+      float sa[32], dpa[32];
+      wg_fence();
+      qk(sa, aK + kb * 8192, aQ + qs * 8192);
+      qk(dpa, aV + kb * 8192, adO + qs * 8192);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(sa);
+      wg_fence_acc(dpa);
+      uint32_t pk_s[16], pk_p[16];
+      attn_bwd_block<true>(sa, dpa, pk_s, pk_p, s_stat, s_keyok, s_colkey, kb * 64, qs * 64, L, p.causal, sl2, p.scale, drop, thr,
+                           ks_drop);
+      wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {   // contraction over the 64 queries of the step
+        const uint32_t ap[4] = {pk_p[4 * kk], pk_p[4 * kk + 1], pk_p[4 * kk + 2], pk_p[4 * kk + 3]};
+        const uint32_t as[4] = {pk_s[4 * kk], pk_s[4 * kk + 1], pk_s[4 * kk + 2], pk_s[4 * kk + 3]};
+        WgmmaRS<64>::template run<1>(dv, ap, desc_mn(adO + qs * 8192 + kk * 2048, 8192), 1);
+        WgmmaRS<64>::template run<1>(dk, as, desc_mn(aQ + qs * 8192 + kk * 2048, 8192), 1);
+      }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(dk);
+      wg_fence_acc(dv);
+    }
+    store_rows(dk, p.dK, p.ld_dk, p.dk_c0, kb * 64);
+    store_rows(dv, p.dV, p.ld_dv, p.dv_c0, kb * 64);
+  }
+#pragma unroll 1
+  for (int u = 0; u < 2; ++u) {
+    const int qb = u == 0 ? wg : 3 - wg;
+    if (qb >= n_blk) continue;
+    // ---- phase 2: rows = queries of block qb
+    float dq[32];
+    acc_zero(dq);
+    const int kb_end = p.causal ? qb + 1 : n_blk;
+#pragma unroll 1
+    for (int kb = 0; kb < kb_end; ++kb) {
+      float sa[32], dpa[32];
+      wg_fence();
+      qk(sa, aQ + qb * 8192, aK + kb * 8192);
+      qk(dpa, adO + qb * 8192, aV + kb * 8192);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(sa);
+      wg_fence_acc(dpa);
+      uint32_t pk_s[16], pk_p[16];
+      attn_bwd_block<false>(sa, dpa, pk_s, pk_p, s_stat, s_keyok, s_colkey, qb * 64, kb * 64, L, p.causal, sl2, p.scale, drop, thr,
+                            ks_drop);
+      wg_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {   // contraction over the 64 keys of the block
+        const uint32_t as[4] = {pk_s[4 * kk], pk_s[4 * kk + 1], pk_s[4 * kk + 2], pk_s[4 * kk + 3]};
+        WgmmaRS<64>::template run<1>(dq, as, desc_mn(aK + kb * 8192 + kk * 2048, 8192), 1);
+      }
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(dq);
+    }
+    store_rows(dq, p.dQ, p.ld_dq, p.dq_c0, qb * 64);
+  }
+}
+
+}  // namespace rp
+
+using namespace rp;
+
+struct rp_attn_bwd_desc {
+  const void* q; long long q_rows, q_cols, ldq; int q_c0;
+  const void* k; long long k_rows, k_cols, ldk; int k_c0;
+  const void* v; long long v_rows, v_cols, ldv; int v_c0;
+  const void* d_out; long long do_rows, do_cols, ld_do;
+  const void* out; int ldo;
+  int B, H, L, head_dim;
+  int causal, mask_pad_keys;
+  const uint8_t* pad_mask;
+  const float* m_save; const float* inv_sum;
+  void* dq; int ld_dq, dq_c0;
+  void* dk; int ld_dk, dk_c0;
+  void* dv; int ld_dv, dv_c0;
+  float drop_p; unsigned long long seed, drop_off; const unsigned long long* seed_ptr;
+  float scale;
+};
+
+RP_API int rp_attn_bwd(const rp_attn_bwd_desc* a, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!a || !a->q || !a->k || !a->v || !a->d_out || !a->out || !a->pad_mask || !a->m_save || !a->inv_sum || !a->dq || !a->dk ||
+      !a->dv)
+    return RP_EINVAL;
+  if (a->L <= 0 || a->L > 256 || a->B <= 0 || a->H <= 0 || a->head_dim != 64) return RP_ESHAPE;
+  if ((a->ld_dq & 7) || (a->ld_dk & 7) || (a->ld_dv & 7) || (a->ldo & 7) || (a->ld_do & 7) || (a->dq_c0 & 7) || (a->dk_c0 & 7) ||
+      (a->dv_c0 & 7))
+    return RP_EALIGN;
+  AttnBwdParams p;
+  p.B = a->B; p.H = a->H; p.L = a->L; p.Lp = (a->L + 63) & ~63;
+  p.causal = a->causal; p.mask_pad_keys = a->mask_pad_keys;
+  p.scale = a->scale > 0.f ? a->scale : 1.f / sqrtf((float)a->head_dim);
+  p.pad_mask = a->pad_mask;
+  p.m_save = a->m_save; p.inv_sum = a->inv_sum;
+  p.dQ = reinterpret_cast<__nv_bfloat16*>(a->dq); p.ld_dq = a->ld_dq; p.dq_c0 = a->dq_c0;
+  p.dK = reinterpret_cast<__nv_bfloat16*>(a->dk); p.ld_dk = a->ld_dk; p.dk_c0 = a->dk_c0;
+  p.dV = reinterpret_cast<__nv_bfloat16*>(a->dv); p.ld_dv = a->ld_dv; p.dv_c0 = a->dv_c0;
+  p.q_c0 = a->q_c0; p.k_c0 = a->k_c0; p.v_c0 = a->v_c0;
+  p.drop_p = a->drop_p; p.seed = a->seed; p.drop_off = a->drop_off; p.seed_ptr = a->seed_ptr;
+  AttnBwdMaps tm;
+  int rc;
+  const uint64_t B = (uint64_t)a->B, L = (uint64_t)a->L;
+  if ((uint64_t)a->q_rows < B * L || (uint64_t)a->k_rows < B * L || (uint64_t)a->v_rows < B * L || (uint64_t)a->do_rows < B * L)
+    return RP_ESHAPE;
+  if ((rc = make_tmap_bf16_seq(&tm.q, a->q, B, L, a->q_cols, a->ldq, 128)) != RP_OK) return rc;
+  if ((rc = make_tmap_bf16_seq(&tm.k, a->k, B, L, a->k_cols, a->ldk, 128)) != RP_OK) return rc;
+  if ((rc = make_tmap_bf16_seq(&tm.v, a->v, B, L, a->v_cols, a->ldv, 128)) != RP_OK) return rc;
+  if ((rc = make_tmap_bf16_seq(&tm.d_o, a->d_out, B, L, a->do_cols, a->ld_do, 128)) != RP_OK) return rc;
+  if ((rc = make_tmap_bf16_seq(&tm.o, a->out, B, L, (uint64_t)a->H * 64, a->ldo, 128)) != RP_OK) return rc;
+  const int smem = 10 * 128 * 128 + 1024;
+  RP_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  attn_bwd_kernel<<<a->B * a->H, kAbThreads, smem, stream>>>(tm, p);
   RP_LAUNCH_CHECK();
   return RP_OK;
 }

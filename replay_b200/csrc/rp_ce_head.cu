@@ -8,11 +8,11 @@
 // Inputs are the COMPACTED valid-target rows Hc[T_v, d] (bf16, capacity T rows; T_v lives in device memory so the whole
 // step stays CUDA-graph capturable), the item table E[I, d] (bf16) and labels[T_v].
 //
-//   ce_fwd_kernel      CTA = 128 tokens x an item split.  S = Hc.E^T tile by tile in TMEM; epilogue keeps an online
-//                      (max, sum-exp) per row and picks the target logit.                      -> partial (m, s), z_y
+//   ce_fwd_kernel      CTA = 128 tokens x an item split.  S = Hc.E^T tile by tile (wgmma, registers); an online
+//                      (max, sum-exp) per row.                                                  -> partial (m, s)
 //   ce_finalize_kernel lse, loss = mean(lse - z_y), per-token exponent offset c_t = -lse*log2e + log2(1/T_v)
-//   ce_bwd_kernel<ROW> CTA = 128 tokens, loops over item tiles:   G = exp2(S*log2e + c_row) (bf16, written back into
-//                      TMEM over S), dH += G . E_tile  (A from TMEM, B = the same smem tile, MN-major)
+//   ce_bwd_kernel<ROW> CTA = 128 tokens, loops over item tiles:   G = exp2(S*log2e + c_row) (bf16, kept in registers as
+//                      the A operand), dH += G . E_tile  (B = the same smem tile, MN-major)
 //                      final: dH[t] -= E[y_t] / T_v                                             -> dHc bf16 [T_v, d]
 //   ce_bwd_kernel<COL> CTA = 128 items, loops over token tiles:   S^T = E_tile . Hc^T, G = exp2(S^T*log2e + c_col),
 //                      dE += G . Hc_tile                                                          -> dE fp32 [I, d] (=)
@@ -21,7 +21,7 @@
 
 #include "rp_host.h"
 #include "rp_gemm_desc.h"
-#include "rp_sm100.cuh"
+#include "rp_sm90.cuh"
 
 namespace rp {
 
@@ -29,100 +29,10 @@ static constexpr int kT = 128;                  // tile edge (rows per CTA, colu
 static constexpr int kChunk = 128 * 128;        // bytes of one [128 rows x 64 bf16] swizzled chunk
 static constexpr float kLog2e = 1.4426950408889634f;
 static constexpr float kLn2 = 0.6931471805599453f;
-static constexpr int kEpiWarps = 8;
-static constexpr int kThreads = 64 + kEpiWarps * 32;
-// backward / fused kernels: RP_CE_BWD_CG column groups per TMEM lane quarter -> 4*CG epilogue warps (16 by default): the
-// knob kept for experiments: 16 warps (CG = 4) measured ~8 % slower than 8 (CG = 2) on B200, see profiles/r1_ce_variants.md
-#ifndef RP_CE_BWD_CG
-#define RP_CE_BWD_CG 2
-#endif
-#ifndef RP_CE_ABLATE
-#define RP_CE_ABLATE 0
-#endif
-#ifndef RP_CE_NSTAGE_D128
-#define RP_CE_NSTAGE_D128 4   // B-tile ring depth of the backward / fused kernels at d = 128 (32 KB per stage)
-#endif
-static constexpr int kBwdCG = RP_CE_BWD_CG;
-static constexpr int kBwdEpiWarps = 4 * kBwdCG;
-static constexpr int kBwdThreads = 64 + kBwdEpiWarps * 32;
-// RP_CE_GROUPS = 2 (d = 128): TWO such sets of epilogue warps, one per S buffer (even / odd column tiles).  One set works in
-// lock step - wait, tcgen05.ld, 64 exponentials per thread, tcgen05.st, arrive - so the MUFU pipe (the 16 384 exponentials of
-// a tile need >= 1024 of the ~1170 tensor cycles of the tile) idles through every load / store / barrier phase; two sets on
-// different tiles fill each other's gaps (r2 ncu: MUFU 61-65 % and tensor 69-74 % busy with one set).
-#ifndef RP_CE_GROUPS
-#define RP_CE_GROUPS 1   /* r2 A/B (profiles/r2_ce_variants.md): two sets measured 3-5 % SLOWER than one - kept as a knob */
-#endif
-static constexpr int kCeMaxGroups = 2;
-
-// tuning knobs (measured on B200, see profiles/): every RP_CE_POLY_EVERY-th exponential goes to the FMA-pipe polynomial
-// instead of MUFU.EX2 (0 = MUFU only); RP_CE_NBUF3 = 1 triple-buffers S in TMEM for d <= 128.
-#ifndef RP_CE_POLY_EVERY
-#define RP_CE_POLY_EVERY 4   /* forward: 25 % of the exponentials on the FMA pipe (measured best, profiles/r1_ce_variants.md) */
-#endif
-#ifndef RP_CE_POLY_EVERY_BWD
-#define RP_CE_POLY_EVERY_BWD 0   /* backward / fused passes: MUFU only (r2 A/B with the in-order issue: 0 beats 12.5 % by 2-8 %, profiles/r2_ce_variants.md) */
-#endif
-#ifndef RP_CE_NBUF3
-#define RP_CE_NBUF3 1
-#endif
-#ifndef RP_CE_A_TMEM
-#define RP_CE_A_TMEM 1
-#endif
-// MMA issue order of the backward / fused kernels (profiles/r2_ce_issue_order.md):
-//   0  round-1 order: S tile j+NBUF-1 is issued right behind the second GEMM of tile j-1 and has to wait for it (its TMEM
-//      buffer is the one that GEMM reads G from): the tensor pipe drains once per tile
-//   1  (d <= 128) two S buffers, row tile in TMEM, S tile j+2 issued right BEHIND the second GEMM of tile j without a
-//      barrier in between: tcgen05.mma instructions of one CTA execute in issue order, so the overwrite of the buffer cannot
-//      overtake the reads of G; the issuing thread never waits on work it has just queued
-//   2  three S buffers (row tile in shared memory), prefetch distance 1: every wait is for a GEMM issued two groups earlier
-#ifndef RP_CE_ORDER
-#define RP_CE_ORDER 1
-#endif
-#ifndef RP_CE_TN64
-#define RP_CE_TN64 0      /* d <= 128: 64-wide column tiles in four S buffers (0 = 128-wide in two) */
-#endif
-#ifndef RP_CE_TN64_GROUPS
-#define RP_CE_TN64_GROUPS 2   /* TN = 64: two epilogue warp sets on alternating tiles (1 = all 8 warps on every tile) */
-#endif
-#ifndef RP_CE_RELAXED_WAITS
-#define RP_CE_RELAXED_WAITS 0   /* the MMA / TMA threads sleep between polls of their (long) waits: they share a sub-partition with two epilogue warps */
-#endif
-#ifndef RP_CE_PACE_DEPTH
-#define RP_CE_PACE_DEPTH 0   /* pairs of tcgen05.mma in flight before the issuing thread waits for a completion (0 = issue at will) */
-#endif
-#ifndef RP_CE_NO_EMPTY
-#define RP_CE_NO_EMPTY 1   /* in-order issue: stages are released by the S-complete barrier of tile j + NBUF (one commit per tile less) */
-#endif
-#ifndef RP_CE_PRESCALE
-#define RP_CE_PRESCALE 0   /* fused pass: log2(e) folded into the TMEM row tile (one instruction less per logit; measured: no gain, 1.061 vs 1.050 ms, and the extra bf16 rounding breaks the 1e-2 gradient tolerance of test_ce_head at d = 64) */
-#endif
-#ifndef RP_CE_POLY_EVERY_Q1
-#define RP_CE_POLY_EVERY_Q1 RP_CE_POLY_EVERY_BWD   /* polynomial share of lane quarter 1's epilogue warps (see the chunk lambda) */
-#endif
-#ifndef RP_CE_ISSUE_GROUP
-#define RP_CE_ISSUE_GROUP 0      /* > 0: the issuing thread sleeps RP_CE_ISSUE_SLEEP_NS after every so many tcgen05.mma */
-#endif
-#ifndef RP_CE_ISSUE_SLEEP_NS
-#define RP_CE_ISSUE_SLEEP_NS 150
-#endif
-#ifndef RP_CE_ISSUERS
-#define RP_CE_ISSUERS 1   /* MMA-issuing threads of the backward / fused kernels (1 = warp 1 alone) */
-#endif
-#ifndef RP_CE_PERSIST
-#define RP_CE_PERSIST 1   /* dE pass: one CTA per SM over balanced slices of the (item tile, token tile) pairs; 0 = one CTA per item tile */
-#endif
-#ifdef RP_CE_TRACE  // diagnostic build (-DRP_CE_TRACE): timeline of CTA 0 - 8 event kinds x the first 256 column tiles
-__device__ unsigned long long g_ce_trace[2][16 * 256];   // [0]: fused forward / dH pass, [1]: dE pass; kinds 8..15: hand-over time of epilogue warp 0..7
-#define RP_CTR(k, j) do { if (blockIdx.x == 0 && (j) < 256) g_ce_trace[MODE == 1][(k) * 256 + (j)] = clock64(); } while (0)
-#else
-#define RP_CTR(k, j) do { } while (0)
-#endif
-template <int DEG, int EVERY>
-__device__ __forceinline__ float ce_ex2(float x, int q) {
-  if (EVERY > 0 && (q % (EVERY > 0 ? EVERY : 1)) == 1) return ex2_poly<DEG>(x);
-  return ex2f(x);
-}
-
+// CTA layout of the head kernels: warpgroups 0 / 1 own rows [0, 64) / [64, 128) of the row tile; thread 0 also feeds the TMA
+// ring (a separate producer warp would cap the registers of the accumulating threads)
+static constexpr int kThreads = 256;
+static constexpr int kTN = 64;                  // column tile of the backward / fused kernels
 // ----------------------------------------------------------------------------------------------------------------
 // forward
 // ----------------------------------------------------------------------------------------------------------------
@@ -130,16 +40,15 @@ template <int KCH, int NSTAGE>
 __global__ void __launch_bounds__(kThreads, 1)
 ce_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
               const int32_t* __restrict__ n_valid_ptr, int n_items, int n_splits, const float* __restrict__ bias,
-              float2* __restrict__ part /* [T, n_splits, 2] (m in log2 units, s) */,
+              float2* __restrict__ part /* [T, n_splits] (m in log2 units, s) */,
               const int32_t* __restrict__ skip_if_safe) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + KCH * kChunk;
-  __shared__ uint64_t bar_a, bar_full[NSTAGE], bar_empty[NSTAGE], bar_tfull[2], bar_tempty[2];
-  __shared__ uint32_t tmem_slot;
+  __shared__ uint64_t bar_a, bar_full[NSTAGE], bar_empty[NSTAGE];
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   const int tok_tile = blockIdx.x / n_splits, split = blockIdx.x % n_splits;
   if (skip_if_safe && *skip_if_safe != 0) return;  // the fused pass covers this step
   const int n_valid = *n_valid_ptr;
@@ -153,119 +62,93 @@ ce_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     mbar_init(&bar_a, 1);
     for (int i = 0; i < NSTAGE; ++i) {
       mbar_init(&bar_full[i], 1);
-      mbar_init(&bar_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bar_tfull[i], 1);
-      mbar_init(&bar_tempty[i], kEpiWarps);
+      mbar_init(&bar_empty[i], 8);
     }
     fence_barrier_init();
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == 1) tmem_alloc(&tmem_slot, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-
-  if (warp == 0) {
-    if (elect_one()) {
-      mbar_arrive_expect_tx(&bar_a, KCH * kChunk);
-      for (int kc = 0; kc < KCH; ++kc) tma_load_2d(sA + kc * kChunk, &tmA, &bar_a, kc * 64, t0);
-      uint32_t it = 0;
-      for (int j = j_begin; j < j_end; ++j)
-        for (int kc = 0; kc < KCH; ++kc, ++it) {
-          const uint32_t s = it % NSTAGE, ph = (it / NSTAGE) & 1;
-          mbar_wait(&bar_empty[s], ph ^ 1);
-          mbar_arrive_expect_tx(&bar_full[s], kChunk);
-          tma_load_2d(sB + s * kChunk, &tmB, &bar_full[s], kc * 64, j * kT);
-        }
-    }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(kT, kT);
-      mbar_wait(&bar_a, 0);
-      tc_fence_after();
-      uint32_t it = 0;
-      for (int j = j_begin, n = 0; j < j_end; ++j, ++n) {
-        const uint32_t as = n & 1, aph = (n >> 1) & 1;
-        mbar_wait(&bar_tempty[as], aph ^ 1);
-        tc_fence_after();
-        const uint32_t dcol = tmem + as * kT;
-        for (int kc = 0; kc < KCH; ++kc, ++it) {
-          const uint32_t s = it % NSTAGE, ph = (it / NSTAGE) & 1;
-          mbar_wait(&bar_full[s], ph);
-          tc_fence_after();
-          const uint32_t a0 = smem_u32(sA + kc * kChunk), b0 = smem_u32(sB + s * kChunk);
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks)
-            umma_ss(dcol, umma_desc_sw128(a0 + ks * 32, 16, 1024), umma_desc_sw128(b0 + ks * 32, 16, 1024), idesc,
-                    (kc | ks) != 0);
-          umma_commit(&bar_empty[s]);
-        }
-        umma_commit(&bar_tfull[as]);
-      }
-    }
-  } else {
-    const int ew = warp - 2, quarter = warp & 3, half = ew >> 2;
-    const int row = quarter * 32 + lane;
-    const int t = t0 + row;
-    float m = -1e30f, ssum = 0.f;  // m in log2 units
-    for (int j = j_begin, n = 0; j < j_end; ++j, ++n) {
-      const uint32_t as = n & 1, aph = (n >> 1) & 1;
-      mbar_wait(&bar_tfull[as], aph);
-      tc_fence_after();
-      const uint32_t tbase = tmem + ((uint32_t)(quarter * 32) << 16) + as * kT + half * 64;
-      uint32_t raw[64];
-      tmem_ld32(tbase, *reinterpret_cast<uint32_t(*)[32]>(&raw[0]));
-      tmem_ld32(tbase + 32, *reinterpret_cast<uint32_t(*)[32]>(&raw[32]));
-      tmem_ld_wait();
-      // the accumulator stage is free as soon as its values sit in registers
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_tempty[as]);
-      const int col0 = j * kT + half * 64;
-      if (bias) {  // untied / biased head (BERT4Rec): logits = h.W^T + b ; warp-uniform 16-byte loads (bias is padded to 128)
-#pragma unroll
-        for (int q = 0; q < 64; q += 4) {
-          const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + col0 + q));
-          raw[q + 0] = __float_as_uint(__uint_as_float(raw[q + 0]) + b4.x);
-          raw[q + 1] = __float_as_uint(__uint_as_float(raw[q + 1]) + b4.y);
-          raw[q + 2] = __float_as_uint(__uint_as_float(raw[q + 2]) + b4.z);
-          raw[q + 3] = __float_as_uint(__uint_as_float(raw[q + 3]) + b4.w);
-        }
-      }
-      if (col0 + 64 > n_items) {  // ragged last tile
-#pragma unroll
-        for (int q = 0; q < 64; ++q)
-          if (col0 + q >= n_items) raw[q] = 0xff800000u;  // -inf
-      }
-      float cm0 = __uint_as_float(raw[0]), cm1 = __uint_as_float(raw[1]);
-#pragma unroll
-      for (int q = 2; q < 64; q += 2) {
-        cm0 = fmaxf(cm0, __uint_as_float(raw[q]));
-        cm1 = fmaxf(cm1, __uint_as_float(raw[q + 1]));
-      }
-      const float mn = fmaxf(m, fmaxf(cm0, cm1) * kLog2e);
-      ssum *= ex2f(m - mn);
-      m = mn;
-      // half of the exponentials on MUFU, half on the FMA pipe
-      float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll
-      for (int q = 0; q < 64; q += 4) {
-        a0 += ce_ex2<4, RP_CE_POLY_EVERY>(fmaf(__uint_as_float(raw[q + 0]), kLog2e, -mn), q + 0);
-        a1 += ce_ex2<4, RP_CE_POLY_EVERY>(fmaf(__uint_as_float(raw[q + 1]), kLog2e, -mn), q + 1);
-        a2 += ce_ex2<4, RP_CE_POLY_EVERY>(fmaf(__uint_as_float(raw[q + 2]), kLog2e, -mn), q + 2);
-        a3 += ce_ex2<4, RP_CE_POLY_EVERY>(fmaf(__uint_as_float(raw[q + 3]), kLog2e, -mn), q + 3);
-      }
-      ssum += (a0 + a1) + (a2 + a3);
-    }
-    if (t < n_valid) part[((size_t)t * n_splits + split) * 2 + half] = make_float2(m, ssum);
+  const int n_chunks = (j_end - j_begin) * KCH;
+  auto issue = [&](int i) {   // thread 0: chunk i of the item tiles -> stage i % NSTAGE
+    const uint32_t s = i % NSTAGE;
+    mbar_wait(&bar_empty[s], ((i / NSTAGE) & 1) ^ 1);
+    mbar_arrive_expect_tx(&bar_full[s], kChunk);
+    tma_load_2d(sB + s * kChunk, &tmB, &bar_full[s], (i % KCH) * 64, (j_begin + i / KCH) * kT);
+  };
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(&bar_a, KCH * kChunk);
+    for (int kc = 0; kc < KCH; ++kc) tma_load_2d(sA + kc * kChunk, &tmA, &bar_a, kc * 64, t0);
+    for (int i = 0; i < NSTAGE && i < n_chunks; ++i) issue(i);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 256);
+  const int t = threadIdx.x & 127, wg = threadIdx.x >> 7;
+  const int fc = frag_col(t);
+  const int ta = t0 + 64 * wg + frag_row(t), tb = ta + 8;   // the two token rows of this thread
+  float ma = -1e30f, sa = 0.f, mb = -1e30f, sb = 0.f;      // m in log2 units
+  mbar_wait(&bar_a, 0);
+  uint32_t it = 0;
+  for (int j = j_begin; j < j_end; ++j) {
+    float acc[kT / 2];
+    for (int kc = 0; kc < KCH; ++kc, ++it) {
+      const uint32_t s = it % NSTAGE, ph = (it / NSTAGE) & 1;
+      mbar_wait(&bar_full[s], ph);
+      const uint32_t a0 = smem_u32(sA + kc * kChunk) + wg * 8192, b0 = smem_u32(sB + s * kChunk);
+      wg_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) WgmmaSS<kT>::template run<0, 0>(acc, desc_k(a0 + ks * 32), desc_k(b0 + ks * 32), (kc | ks) != 0);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bar_empty[s]);
+      if (threadIdx.x == 0 && (int)it + NSTAGE < n_chunks) issue((int)it + NSTAGE);
+    }
+    const int col0 = j * kT + fc;
+#pragma unroll
+    for (int q = 0; q < kT / 8; ++q)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = col0 + 8 * q + e;
+        const float b = (bias && col < n_items) ? __ldg(bias + col) : 0.f;   // untied / biased head (BERT4Rec)
+        const bool in = col < n_items;                                        // ragged last tile
+        acc[4 * q + e] = in ? acc[4 * q + e] + b : -INFINITY;
+        acc[4 * q + 2 + e] = in ? acc[4 * q + 2 + e] + b : -INFINITY;
+      }
+    float cma = -INFINITY, cmb = -INFINITY;
+#pragma unroll
+    for (int q = 0; q < kT / 8; ++q) {
+      cma = fmaxf(cma, fmaxf(acc[4 * q], acc[4 * q + 1]));
+      cmb = fmaxf(cmb, fmaxf(acc[4 * q + 2], acc[4 * q + 3]));
+    }
+    const float mna = fmaxf(ma, cma * kLog2e), mnb = fmaxf(mb, cmb * kLog2e);
+    sa *= ex2f(ma - mna);
+    sb *= ex2f(mb - mnb);
+    ma = mna;
+    mb = mnb;
+    float xa = 0.f, xb = 0.f;
+#pragma unroll
+    for (int q = 0; q < kT / 8; ++q) {
+      xa += ex2f(fmaf(acc[4 * q], kLog2e, -mna)) + ex2f(fmaf(acc[4 * q + 1], kLog2e, -mna));
+      xb += ex2f(fmaf(acc[4 * q + 2], kLog2e, -mnb)) + ex2f(fmaf(acc[4 * q + 3], kLog2e, -mnb));
+    }
+    sa += xa;
+    sb += xb;
+  }
+  // the four threads of a quad hold the same rows: merge their (max, sum) pairs
+#pragma unroll
+  for (int o = 1; o <= 2; o <<= 1) {
+    const float oma = __shfl_xor_sync(0xffffffffu, ma, o), osa = __shfl_xor_sync(0xffffffffu, sa, o);
+    const float omb = __shfl_xor_sync(0xffffffffu, mb, o), osb = __shfl_xor_sync(0xffffffffu, sb, o);
+    const float na = fmaxf(ma, oma), nb = fmaxf(mb, omb);
+    sa = sa * ex2f(ma - na) + osa * ex2f(oma - na);
+    sb = sb * ex2f(mb - nb) + osb * ex2f(omb - nb);
+    ma = na;
+    mb = nb;
+  }
+  if (fc == 0) {
+    if (ta < n_valid) part[(size_t)ta * n_splits + split] = make_float2(ma, sa);
+    if (tb < n_valid) part[(size_t)tb * n_splits + split] = make_float2(mb, sb);
+  }
 }
 
 // Per-row variants of the full-catalog head (all single positive label per position):
@@ -382,6 +265,11 @@ struct CeDirect {
                          // forward) instead of the fixed reference 0, so G is the softmax itself (z ~ 1) whatever |logit| is
 };
 
+// exponent offset of row r in the fused pass (log2 units): 0, or -lse[r] behind the two-pass forward; -inf beyond T_v
+__device__ __forceinline__ float crow_of(const CeDirect& d, int r, int n_valid) {
+  return r < n_valid ? (d.use_lse_off ? -d.lse[r] * kLog2e : 0.f) : -INFINITY;
+}
+
 // loss = mean over the valid targets of row_loss, deterministic (fixed partition + tree); also publishes 1 / T_v
 __global__ void __launch_bounds__(1024) ce_loss_reduce_kernel(const float* __restrict__ row_loss, const int32_t* __restrict__ n_valid_ptr,
                                                               const int32_t* __restrict__ safe_flag, float* __restrict__ loss_out,
@@ -414,52 +302,14 @@ __global__ void __launch_bounds__(1024) ce_loss_reduce_kernel(const float* __res
 // MODE 2: rows = tokens, FUSED forward+backward: G~ = exp(s + b) with reference max 0 (valid while |s| is bounded, see
 //         ce_bound_kernel), per-row sum of G~ and un-normalised dH~ = sum_i G~ E_i over this CTA's column split
 //                                                                                      -> out = partial dH~ fp32, zpart
-// One SEGMENT of a CTA's work = one row tile against a contiguous run of column tiles.  The per-row-tile launches (fused
-// forward / two-pass dH: grid = row tiles x column splits) have exactly one segment per CTA.  The dE pass is PERSISTENT: the
-// grid is one CTA per SM and CTA c owns the slice [W c / G, W (c+1) / G) of the W = row tiles x column tiles linearised
-// (row tile, column tile) pairs - up to a few segments, every SM busy to the last tile (391 item tiles as one CTA each were
-// 2.64 waves on 148 SMs: 12 % of the pass was an idle tail).  A segment that does not cover its row tile's whole column
-// range adds its partial accumulator to the (zeroed) output with vector reductions.
-struct CeSeg {
-  long long w, w_end;
-  int n_ct_all, row_tile, j0, n;
-  bool valid;
-  __device__ void set() {
-    valid = w < w_end;
-    row_tile = (int)(w / n_ct_all);
-    j0 = (int)(w - (long long)row_tile * n_ct_all);
-    const long long left = w_end - w;
-    n = (n_ct_all - j0 < left) ? n_ct_all - j0 : (int)left;
-  }
-  __device__ void advance() {
-    w += n;
-    set();
-  }
-};
-
-// TN = width of a column tile (= of one S buffer in TMEM).  TN = 64 with FOUR S buffers (d <= 128): the chain
-//   first GEMM (S) -> epilogue (G over S) -> second GEMM (reads G) -> first GEMM of the tile that reuses the buffer
-// is serial per buffer, so with two 128-wide buffers a tile took (tensor time + epilogue time + hand-off latencies) / 2 =
-// ~1535 cycles although the tensor pipe and the MUFU pipe were each busy for only 1024 of them (ncu r2i: both 67 %).  Four
-// 64-wide buffers use the same 256 TMEM columns, keep four such chains in flight, and leave S of the next tile complete long
-// before the epilogue gets to it (so its first TMEM load can be issued ahead of time).
-// CG / GROUPS = how the 8 epilogue warps divide the work.  TN = 128: CG = 2 column groups per TMEM lane quarter, all 8 warps
-// on every tile.  TN = 64: TWO warp SETS (GROUPS = 2) of one warp per lane quarter (CG = 1), set g owns the tiles j = g mod 2.
-// The timeline of a CTA (tools/trace_ce.py, profiles/r2_ce_timeline.md) shows ~450 cycles per tile in the epilogue that are
-// not exponentials - waking up on the S barrier, the first TMEM load, the drain of the last exponentials into the TMEM store,
-// the hand-over - next to 16 cycles per column of MUFU time (two warps share a sub-partition's MUFU).  With one set these
-// phases are serial (1500 cycles per 128 columns, MUFU 67 % busy); with two sets on different tiles the sub-partition's two
-// warps are out of phase and the other warp's exponentials fill them.
-// NI = number of MMA-issuing threads (warp 1 and the warps behind the epilogue warps, one per SM sub-partition).  Issuing a
-// tile's 16 tcgen05.mma keeps the issuing thread's sub-partition from issuing anything else for ~700 cycles (timeline: the
-// two epilogue warps that share warp 1's sub-partition handed their G over 700-900 cycles after the other six, and the tile
-// pace followed them).  NI = 3 issuers take the tiles round-robin, so sub-partitions 1-3 lose a third of that each (sub-
-// partition 0 hosts the TMA thread); an mbarrier token passes the right to issue from tile to tile, which keeps the
-// instructions in tile order in the (in-order) tensor pipe.
-template <int KCH, int NSTAGE, int MODE, int NBUF, bool A_TMEM, bool INORDER, bool HAS_BIAS, int GROUPS, bool PERSIST, int TN, int CG, int NI>
-__global__ void __launch_bounds__(64 + GROUPS * 4 * CG * 32 + (NI - 1) * 32, 1)
+// CTA = one 128-row tile against the column tiles [j0, j0 + n_ct) (64 columns each).  Per column tile: S = A_tile . B_tile^T
+// (wgmma, registers), G = exp2(S log2e + offset) in registers, acc += G . B_tile with G as the register A operand and the
+// same shared-memory B tile read MN-major.  At the end the [128 x D] accumulator goes through shared memory to the row-wise
+// epilogue (thread = row, warpgroup = half of the D columns).
+template <int KCH, int NSTAGE, int MODE, bool HAS_BIAS>
+__global__ void __launch_bounds__(kThreads, 1)
 ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-              const __nv_bfloat16* __restrict__ a_rows /* the row-side matrix (tmA) as a plain pointer, for A_TMEM */,
+              const __nv_bfloat16* __restrict__ a_rows /* the row-side matrix (tmA) as a plain pointer */,
               const float* __restrict__ cvec /* [T] exponent offsets per token */, const int32_t* __restrict__ labels,
               const __nv_bfloat16* __restrict__ table, const float* __restrict__ loss_inv /* [1] = 1/T_v */,
               const int32_t* __restrict__ n_valid_ptr, int n_items, const float* __restrict__ bias,
@@ -467,613 +317,266 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
               int n_splits, int capacity, float* __restrict__ zpart, const CeDirect direct) {
   constexpr bool COLCONST = (MODE == 1);
   constexpr bool FUSED = (MODE == 2);
-  constexpr int kW = TN / CG;  // S columns owned by one epilogue warp (its bf16 G lands in the first kW/2 of them)
-  constexpr int kChunkB = TN * 128;   // bytes of one [TN rows x 64 bf16] swizzled chunk of a column tile
-  // fused pass with the row tile in TMEM and no bias: the tile is multiplied by log2(e) on its way into TMEM, so a logit's
-  // exponential is ONE instruction (ex2 of the accumulator word: live rows have offset 0) instead of FFMA + ex2 - the
-  // epilogue warps next to the MMA-issuing thread are short of issue slots (profiles/r2_ce_timeline.md)
-  constexpr bool PRESCALE = FUSED && A_TMEM && !HAS_BIAS && (RP_CE_PRESCALE != 0);
-  constexpr int kEW = 4 * CG * GROUPS;   // epilogue warps in total
-  constexpr int kSlots = CG * GROUPS;      // column slots of the accumulator read-out / of the row-sum partials
-  static_assert(GROUPS == 1 || (GROUPS == 2 && NBUF % 2 == 0), "two epilogue warp sets: even / odd S buffers");
-  static_assert(NBUF * TN + KCH * 64 + (A_TMEM ? KCH * 32 : 0) <= 512, "TMEM: S buffers + accumulator + row tile");
   constexpr int D = KCH * 64;
-  if (safe_flag && (*safe_flag != 0) != (run_if_safe != 0)) return;  // fused path vs two-pass fallback (uniform)
+  constexpr int kChunkB = kTN * 128;      // bytes of one [64 rows x 64 bf16] swizzled chunk of a column tile
   constexpr int kStage = KCH * kChunkB;   // one column tile in shared memory
-  constexpr int kATile = KCH * kChunk;    // the row tile (when it is not in TMEM)
+  constexpr int PITCH = D + 4;            // fp32 accumulator stage (over the ring once the column tiles are done)
+  constexpr int kSlots = 2, DW = D / kSlots;
+  if (safe_flag && (*safe_flag != 0) != (run_if_safe != 0)) return;  // fused path vs two-pass fallback (uniform)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // A_TMEM: the resident row tile lives in TMEM (K-major, two bf16 per 32-bit column) and the first GEMM reads it from
-  // there, which halves that GEMM's shared-memory traffic - M=128 x N=128 SS MMAs need the full 128 B/clk of smem.
   uint8_t* sA = smem;
-  uint8_t* sB = smem + (A_TMEM ? 0 : kATile);
-  __shared__ __align__(16) float s_cc[NSTAGE][TN];
-  __shared__ float s_gsum[kSlots][kT];
-  __shared__ float s_dot[FUSED ? kSlots : 1][kT];
-  // S-complete barriers form a ring over the smem STAGES (not the NBUF TMEM buffers): the TMA thread, which runs up to
-  // NSTAGE tiles ahead, can then wait for one particular tile's first GEMM without its phase being lapped (see NO_EMPTY)
-  __shared__ uint64_t bar_a, bar_full[NSTAGE], bar_empty[NSTAGE], bar_sfull[NSTAGE], bar_sfree[NBUF], bar_pfull[NBUF], bar_acc, bar_tok[NI], bar_pace[8];
-  // NO_EMPTY: with the in-order issue a tile's smem stage is free once the first GEMM of tile j + NBUF has completed (it is
-  // queued right behind the second GEMM of tile j, the stage's last reader) - the S-complete barrier of that tile doubles as
-  // the stage-free signal and the tcgen05.commit on bar_empty (~50 cycles per tile, profiles/r2_ce_timeline.md) goes away
-  constexpr bool NO_EMPTY = INORDER && NI == 1 && (NSTAGE > NBUF + 1) && (RP_CE_NO_EMPTY != 0);
-  __shared__ uint32_t tmem_slot;
+  uint8_t* sB = smem + KCH * kChunk;
+  __shared__ float s_row[kT];             // per-row sum of G (FUSED) / of G before the item factor (COLCONST with bias)
+  __shared__ float s_dot[kSlots][kT];
+  __shared__ uint64_t bar_a, bar_full[NSTAGE], bar_empty[NSTAGE];
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   const int n_valid = *n_valid_ptr;
-  static_assert(!PERSIST || (COLCONST && A_TMEM), "persistent work slices: dE pass with the row tile in TMEM");
   const int split = FUSED ? blockIdx.x % n_splits : 0;
   const int n_rows = COLCONST ? n_items : n_valid;
   const int n_cols = COLCONST ? n_valid : n_items;
-  const int n_ct_all = (n_cols + TN - 1) / TN;              // column tiles of the whole problem
-  const int jg0 = FUSED ? (int)(((long long)n_ct_all * split) / n_splits) : 0;        // first column tile of this CTA
-  CeSeg seg0;
-  seg0.n_ct_all = n_ct_all > 0 ? n_ct_all : 1;
-  if (PERSIST) {
-    const long long W = (long long)((n_rows + kT - 1) / kT) * n_ct_all;
-    seg0.w = W * blockIdx.x / gridDim.x;
-    seg0.w_end = W * (blockIdx.x + 1) / gridDim.x;
-    seg0.set();
-    if (!seg0.valid) return;   // (uniform) nothing to do: the output was zeroed by the host side
-  } else {
-    seg0.row_tile = FUSED ? blockIdx.x / n_splits : blockIdx.x;
-    seg0.j0 = jg0;
-    seg0.n = FUSED ? (int)(((long long)n_ct_all * (split + 1)) / n_splits) - jg0 : n_ct_all;
-    seg0.w = 0;
-    seg0.w_end = seg0.n;       // advance() ends the iteration after this one segment (n = 0 included)
-    seg0.valid = true;
-    if (seg0.row_tile * kT >= n_rows) return;
-  }
+  const int n_ct_all = (n_cols + kTN - 1) / kTN;
+  const int row_tile = FUSED ? blockIdx.x / n_splits : blockIdx.x;
+  const int j0 = FUSED ? (int)(((long long)n_ct_all * split) / n_splits) : 0;
+  const int n_ct = FUSED ? (int)(((long long)n_ct_all * (split + 1)) / n_splits) - j0 : n_ct_all;
+  const int r0 = row_tile * kT;
+  if (r0 >= n_rows) return;
 
   if (threadIdx.x == 0) {
-    mbar_init(&bar_a, A_TMEM ? kEW : 1);
+    mbar_init(&bar_a, 1);
     for (int i = 0; i < NSTAGE; ++i) {
       mbar_init(&bar_full[i], 1);
-      mbar_init(&bar_empty[i], 1);
+      mbar_init(&bar_empty[i], 8);
     }
-    for (int i = 0; i < NSTAGE; ++i) mbar_init(&bar_sfull[i], 1);
-    for (int i = 0; i < NBUF; ++i) {
-      mbar_init(&bar_sfree[i], 1);
-      mbar_init(&bar_pfull[i], 4 * CG);
-    }
-    mbar_init(&bar_acc, 1);
-    for (int i = 0; i < NI; ++i) mbar_init(&bar_tok[i], 1);
-    for (int i = 0; i < 8; ++i) mbar_init(&bar_pace[i], 1);
     fence_barrier_init();
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == 1) tmem_alloc(&tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t tmem_acc = tmem + NBUF * TN;   // S buffers first, then the [128 x D] accumulator
-  const uint32_t tmem_a = tmem_acc + D;         // A_TMEM: [128 x D] bf16 operand, D/2 columns
-
-  if (warp == 0) {
-    if (elect_one()) {
-      if (!A_TMEM) {
-        mbar_arrive_expect_tx(&bar_a, kATile);
-        for (int kc = 0; kc < KCH; ++kc) tma_load_2d(sA + kc * kChunk, &tmA, &bar_a, kc * 64, seg0.row_tile * kT);
-      }
-      // the column-tile ring runs on a tile counter that continues across segments: the loads of the next segment's first
-      // tiles are already in flight while the current segment drains
-      uint32_t g = 0;
-      for (CeSeg sg = seg0; sg.valid; sg.advance())
-        for (int jl = 0; jl < sg.n; ++jl, ++g) {
-          const uint32_t s = g % NSTAGE, ph = (g / NSTAGE) & 1;
-          const int jc = sg.j0 + jl;   // column tile
-          if (NO_EMPTY) {
-            // stage s was last used by tile g - NSTAGE; it is free when S of tile g - NSTAGE + NBUF is complete
-            if (g >= (uint32_t)NSTAGE) {
-              const uint32_t w = g - NSTAGE + NBUF;
-              mbar_wait(&bar_sfull[w % NSTAGE], (w / NSTAGE) & 1);
-            }
-          } else {
-#if RP_CE_RELAXED_WAITS
-            mbar_wait_relaxed(&bar_empty[s], ph ^ 1);
-#else
-            mbar_wait(&bar_empty[s], ph ^ 1);
-#endif
+  auto issue = [&](int jl) {   // thread 0: column tile jl -> stage jl % NSTAGE
+    const uint32_t s = jl % NSTAGE;
+    mbar_wait(&bar_empty[s], ((jl / NSTAGE) & 1) ^ 1);
+    mbar_arrive_expect_tx(&bar_full[s], kStage);
+    for (int kc = 0; kc < KCH; ++kc) tma_load_2d(sB + s * kStage + kc * kChunkB, &tmB, &bar_full[s], kc * 64, (j0 + jl) * kTN);
+  };
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(&bar_a, KCH * kChunk);
+    for (int kc = 0; kc < KCH; ++kc) tma_load_2d(sA + kc * kChunk, &tmA, &bar_a, kc * 64, r0);
+    for (int jl = 0; jl < NSTAGE && jl < n_ct; ++jl) issue(jl);
+  }
+  const int t = threadIdx.x & 127, wg = threadIdx.x >> 7;
+  const int fc = frag_col(t);
+  const int rla = 64 * wg + frag_row(t), rlb = rla + 8;   // this thread's rows inside the tile
+  float crow_a = 0.f, crow_b = 0.f;
+  if (MODE == 0) {
+    crow_a = (r0 + rla < n_valid) ? cvec[r0 + rla] : -INFINITY;
+    crow_b = (r0 + rlb < n_valid) ? cvec[r0 + rlb] : -INFINITY;
+  }
+  if (FUSED) {
+    crow_a = (r0 + rla < n_valid) ? (direct.use_lse_off ? -direct.lse[r0 + rla] * kLog2e : 0.f) : -INFINITY;
+    crow_b = (r0 + rlb < n_valid) ? (direct.use_lse_off ? -direct.lse[r0 + rlb] * kLog2e : 0.f) : -INFINITY;
+  }
+  float za = 0.f, zb = 0.f;   // FUSED: row sums of G~; COLCONST with bias: row sums of G (bias gradient)
+  float acc[D / 2];
+  acc_zero(acc);
+  mbar_wait(&bar_a, 0);
+  const uint32_t a_base = smem_u32(sA) + wg * 8192;
+  for (int jl = 0; jl < n_ct; ++jl) {
+    const uint32_t s = jl % NSTAGE, ph = (jl / NSTAGE) & 1;
+    mbar_wait(&bar_full[s], ph);
+    const uint32_t b0 = smem_u32(sB + s * kStage);
+    float sacc[kTN / 2];
+    wg_fence();
+#pragma unroll
+    for (int kc = 0; kc < KCH; ++kc)
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks)
+        WgmmaSS<kTN>::template run<0, 0>(sacc, desc_k(a_base + kc * kChunk + ks * 32), desc_k(b0 + kc * kChunkB + ks * 32),
+                                         (kc | ks) != 0);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(sacc);
+    // G = exp2(S log2e + offset) -> bf16 A fragments
+    const int col0 = (j0 + jl) * kTN + fc;
+    uint32_t pk[kTN / 4];
+#pragma unroll
+    for (int q = 0; q < kTN / 8; ++q) {
+      float g[4];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = col0 + 8 * q + e;
+        float va = sacc[4 * q + e], vb = sacc[4 * q + 2 + e];
+        if (COLCONST) {
+          const float cc = __ldg(cvec + col);   // -inf beyond the valid tokens (the buffer is padded to 128 rows)
+          g[e] = ex2f(fmaf(va, kLog2e, cc));
+          g[2 + e] = ex2f(fmaf(vb, kLog2e, cc));
+        } else {
+          const bool in = col < n_items;
+          if (HAS_BIAS && in) {
+            const float bb = __ldg(bias + col);
+            va += bb;
+            vb += bb;
           }
-          mbar_arrive_expect_tx(&bar_full[s], kStage + (COLCONST ? TN * 4 : 0));
-          for (int kc = 0; kc < KCH; ++kc)
-            tma_load_2d(sB + s * kStage + kc * kChunkB, &tmB, &bar_full[s], kc * 64, jc * TN);
-          if (COLCONST) {
-            asm volatile(
-                "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                    smem_u32(&s_cc[s][0])),
-                "l"(cvec + (size_t)jc * TN), "r"(TN * 4), "r"(smem_u32(&bar_full[s]))
-                : "memory");
-          }
+          g[e] = in ? ex2f(fmaf(va, kLog2e, crow_a)) : 0.f;
+          g[2 + e] = in ? ex2f(fmaf(vb, kLog2e, crow_b)) : 0.f;
         }
+      }
+      if (FUSED || (COLCONST && HAS_BIAS)) {
+        za += g[0] + g[1];
+        zb += g[2] + g[3];
+      }
+      pk[2 * q] = pack_bf16(g[0], g[1]);
+      pk[2 * q + 1] = pack_bf16(g[2], g[3]);
     }
-  } else if (warp == 1 || warp >= 2 + kEW) {
-    const int ii = warp == 1 ? 0 : warp - (2 + kEW) + 1;   // issuer index: tiles with (ring position) % NI == ii are mine
-    if (elect_one()) {
-      constexpr uint32_t idesc1 = umma_idesc_bf16(kT, TN);
-      constexpr uint32_t idesc2 = umma_idesc_bf16(kT, D, false, true);
-      // PRE S tiles are in flight ahead of the second GEMM.  INORDER: tile j+NBUF follows the second GEMM of tile j through
-      // the in-order tensor pipe (no barrier); otherwise tile j+PRE is issued before it and waits for the second GEMM of
-      // tile j+PRE-NBUF (RP_CE_ORDER 0: the one issued last -> pipe drain; 2: two groups back)
-      constexpr int PRE = INORDER ? NBUF : ((RP_CE_ORDER == 2 && NBUF >= 3) ? NBUF - 2 : NBUF - 1);
-      uint32_t g0 = 0, nseg = 0;   // ring position of the segment's first tile (S buffers, smem stages); segment count
-      uint32_t n_tok = 0;          // tokens this issuer has consumed (parity of its token barrier)
-      // Issue pacing.  The tensor pipe's instruction queue holds ~6 tcgen05.mma; a further one does not just make this thread
-      // wait - it stalls the DISPATCH of this thread's SM sub-partition, and the two epilogue warps that live there with it
-      // (timeline, tools/trace_ce.py: their hand-over came 700-900 cycles after the other six warps', whichever sub-partition
-      // the issuer was moved to).  So instructions go out in pairs, each pair committed to a ring of eight mbarriers, and pair
-      // m is only issued once pair m - DEPTH has completed: the waiting happens on an mbarrier (harmless) instead of in the
-      // dispatch stage, and the pipe still has 2 (DEPTH - 1) .. 2 DEPTH instructions queued.
-      constexpr uint32_t DEPTH = RP_CE_PACE_DEPTH;
-      uint32_t n_pair = 0, n_half = 0;
-      // Open-loop variant (RP_CE_ISSUE_GROUP / RP_CE_ISSUE_SLEEP_NS): after every GROUP instructions the issuing thread
-      // sleeps (nanosleep deschedules the warp: the sub-partition's dispatch is free) for about the time the pipe needs to
-      // drain them, instead of sitting in the dispatch stage until the queue has room.
-      uint32_t n_issued = 0;
-      auto pace = [&]() {          // call right before every tcgen05.mma
-        if (RP_CE_ISSUE_GROUP > 0 && NI == 1) {
-          if (n_issued != 0 && n_issued % RP_CE_ISSUE_GROUP == 0) __nanosleep(RP_CE_ISSUE_SLEEP_NS);
-          ++n_issued;
-        }
-        if (DEPTH == 0 || NI > 1) return;
-        if ((n_half & 1) == 0 && n_pair >= DEPTH) {
-          const uint32_t m = n_pair - DEPTH;
-          mbar_wait(&bar_pace[m & 7], (m >> 3) & 1);
-        }
-      };
-      auto paced = [&]() {         // call right after every tcgen05.mma
-        if (DEPTH == 0 || NI > 1) return;
-        if (n_half & 1) {
-          umma_commit(&bar_pace[n_pair & 7]);
-          ++n_pair;
-        }
-        ++n_half;
-      };
-      for (CeSeg sg = seg0; sg.valid; sg.advance(), ++nseg) {
-        const int n_ct = sg.n;
-        auto issue_mma1 = [&](int jl) {
-          const uint32_t g = g0 + jl, s = g % NSTAGE, ph = (g / NSTAGE) & 1;
-          mbar_wait(&bar_full[s], ph);
-          if (!INORDER && g >= NBUF) mbar_wait(&bar_sfree[g % NBUF], ((g / NBUF) - 1) & 1);
-          tc_fence_after();
-          const uint32_t dcol = tmem + (g % NBUF) * TN;
+    wg_fence();
 #pragma unroll
-          for (int kc = 0; kc < KCH; ++kc) {
-            const uint32_t a0 = smem_u32(sA + kc * kChunk), b0 = smem_u32(sB + s * kStage + kc * kChunkB);
+    for (int kk = 0; kk < kTN / 16; ++kk) {
+      const uint32_t af[4] = {pk[4 * kk], pk[4 * kk + 1], pk[4 * kk + 2], pk[4 * kk + 3]};
+      WgmmaRS<D>::template run<1>(acc, af, desc_mn(b0 + kk * 2048, kChunkB), 1);
+    }
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bar_empty[s]);
+    if (threadIdx.x == 0 && jl + NSTAGE < n_ct) issue(jl + NSTAGE);
+  }
+  // ---- row sums (the quad's threads share rows) and the accumulator stage
 #pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              pace();
-              if (A_TMEM)
-                umma_ts(dcol, tmem_a + kc * 32 + ks * 8, umma_desc_sw128(b0 + ks * 32, 16, 1024), idesc1, (kc | ks) != 0);
-              else
-                umma_ss(dcol, umma_desc_sw128(a0 + ks * 32, 16, 1024), umma_desc_sw128(b0 + ks * 32, 16, 1024), idesc1,
-                        (kc | ks) != 0);
-              paced();
-            }
-          }
-          umma_commit(&bar_sfull[g % NSTAGE]);
-        };
-        for (int jl = 0; jl < n_ct; ++jl) {
-          const uint32_t g = g0 + jl, s = g % NSTAGE;
-          if (NI > 1) {
-            if ((int)(g % NI) != ii) continue;
-            if (g > 0) {   // the right to issue: the issuer of tile g-1 has queued all of its instructions
-              mbar_wait(&bar_tok[ii], n_tok & 1);
-              ++n_tok;
-              tc_fence_after();
-            }
-          }
-          if (jl == 0) {
-            // the row tile of this segment is in place (TMEM: written by the epilogue warps after they drained the previous
-            // segment's accumulator, so the accumulator may be overwritten as well); the segment's first S tiles go first
-            mbar_wait(&bar_a, nseg & 1);
-            tc_fence_after();
-            for (int q = 0; q < PRE && q < n_ct; ++q) issue_mma1(q);
-          }
-          if (!INORDER && jl + PRE < n_ct) issue_mma1(jl + PRE);
-          RP_CTR(4, g);   // MMA thread starts waiting for G of tile g
-#if RP_CE_RELAXED_WAITS
-          mbar_wait_relaxed(&bar_pfull[g % NBUF], (g / NBUF) & 1);
-#else
-          mbar_wait(&bar_pfull[g % NBUF], (g / NBUF) & 1);
-#endif
-          RP_CTR(5, g);   // ... G of tile g is there
-          tc_fence_after();
-          const uint32_t pcol = tmem + (g % NBUF) * TN;  // G (bf16 pairs) lives over S, kW/2 packed columns per column group
-          const uint32_t b0 = smem_u32(sB + s * kStage);
-#pragma unroll
-          for (int ks = 0; ks < TN / 16; ++ks) {
-            pace();
-            umma_ts(tmem_acc, pcol + ((ks * 16) / kW) * kW + ((ks * 16) % kW) / 2, umma_desc_sw128(b0 + ks * 2048, kChunkB, 1024),
-                    idesc2, (jl | ks) != 0);
-            paced();
-          }
-          if (!NO_EMPTY) umma_commit(&bar_empty[s]);
-          if (INORDER) {
-            if (jl + PRE < n_ct) issue_mma1(jl + PRE);
-          } else {
-            umma_commit(&bar_sfree[g % NBUF]);
-          }
-          if (jl == n_ct - 1) umma_commit(&bar_acc);   // (in-order pipe: everything issued before it has completed as well)
-          RP_CTR(6, g);   // second GEMM of tile g and first GEMM of tile g + PRE are queued
-          if (NI > 1) {
-            tc_fence_before();
-            mbar_arrive(&bar_tok[(g + 1) % NI]);
-          }
-        }
-        if (n_ct == 0 && ii == 0) {   // (single-segment launches only) nothing to multiply: release the epilogue's final wait
-          mbar_wait(&bar_a, nseg & 1);
-          umma_commit(&bar_acc);
-        }
-        g0 += n_ct;
+  for (int o = 1; o <= 2; o <<= 1) {
+    za += __shfl_xor_sync(0xffffffffu, za, o);
+    zb += __shfl_xor_sync(0xffffffffu, zb, o);
+  }
+  if (fc == 0) {
+    s_row[rla] = za;
+    s_row[rlb] = zb;
+  }
+  named_bar_sync(1, 256);   // both warpgroups are done with the ring
+  float* stage = reinterpret_cast<float*>(sB);
+  acc_to_stage(acc, stage, PITCH, 64 * wg, 0);
+  named_bar_sync(1, 256);
+  // ---- final: thread = row, warpgroup = slot of DW accumulator columns
+  const int row = t, slot = wg;
+  const int r = r0 + row;
+  const float* arow = stage + row * PITCH + slot * DW;
+  if (COLCONST) {
+    float* o = reinterpret_cast<float*>(out);
+    // biased head: G carries a per-item factor e^{b_i}; it was left out of the loop and is applied to the row here
+    const float rs = (HAS_BIAS && r < n_items) ? __expf(bias[r]) : 1.f;
+    if (HAS_BIAS && slot == 0 && r < n_items) d_bias[r] = s_row[row] * rs;
+    if (r < n_items) {
+      float4* dst = reinterpret_cast<float4*>(o + (size_t)r * D + slot * DW);
+#pragma unroll 4
+      for (int c = 0; c < DW; c += 4) {
+        const float4 v = *reinterpret_cast<const float4*>(arow + c);
+        dst[c >> 2] = make_float4(v.x * rs, v.y * rs, v.z * rs, v.w * rs);
       }
+    }
+  } else if (FUSED && direct.d_hc != nullptr) {
+    // ---- no column splits: finish here.  z_t = row sum of G~; dH = acc / (z T_v) - E[y] / T_v
+    const float z = s_row[row];
+    const bool live = r < n_valid;
+    const float inv_n = n_valid > 0 ? 1.f / (float)n_valid : 0.f;
+    const int y = live ? labels[r] : 0;
+    float wg_ = (live && direct.row.w_ext) ? direct.row.w_ext[r] : 1.f;   // gradient weight of the row
+    if (direct.row.kind == 1) {
+      // LogInCE: the weight needs the target logit before the gradient can be scaled - one extra pass over h . E[y]
+      float dp = 0.f;
+      if (live) {
+        const uint4* ey = reinterpret_cast<const uint4*>(table + (size_t)y * D + slot * DW);
+        const uint4* hr = reinterpret_cast<const uint4*>(a_rows + (size_t)r * D + slot * DW);
+#pragma unroll 4
+        for (int q = 0; q < DW / 8; ++q) {
+          const uint4 e = __ldg(ey + q), hh = __ldg(hr + q);
+          const __nv_bfloat162* e2 = reinterpret_cast<const __nv_bfloat162*>(&e);
+          const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&hh);
+#pragma unroll
+          for (int pp = 0; pp < 4; ++pp) {
+            const float2 ef = __bfloat1622float2(e2[pp]), hf = __bfloat1622float2(h2[pp]);
+            dp = fmaf(hf.x, ef.x, fmaf(hf.y, ef.y, dp));
+          }
+        }
+      }
+      s_dot[slot][row] = dp;
+      named_bar_sync(1, 256);
+      float zy0 = s_dot[0][row] + s_dot[1][row];
+      if (HAS_BIAS) zy0 += bias[y];
+      named_bar_sync(1, 256);   // s_dot is written again below
+      float rl_unused;
+      if (live) ce_row_terms(direct.row, r, __logf(z) - crow_of(direct, r, n_valid) * kLn2, zy0, rl_unused, wg_);
+    }
+    const float scale = live ? wg_ * inv_n / z : 0.f;
+    const float lab = wg_ * inv_n;
+    float dot = 0.f;
+    if (live) {
+      const uint4* ey = reinterpret_cast<const uint4*>(table + (size_t)y * D + slot * DW);
+      const uint4* hr = reinterpret_cast<const uint4*>(a_rows + (size_t)r * D + slot * DW);
+      uint4* dst = reinterpret_cast<uint4*>(direct.d_hc + (size_t)r * D + slot * DW);
+#pragma unroll 4
+      for (int q = 0; q < DW / 8; ++q) {
+        const uint4 e = __ldg(ey + q), hh = __ldg(hr + q);
+        const __nv_bfloat162* e2 = reinterpret_cast<const __nv_bfloat162*>(&e);
+        const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&hh);
+        uint4 w;
+        uint32_t* w32 = reinterpret_cast<uint32_t*>(&w);
+#pragma unroll
+        for (int pp = 0; pp < 4; ++pp) {
+          const float2 ef = __bfloat1622float2(e2[pp]), hf = __bfloat1622float2(h2[pp]);
+          dot = fmaf(hf.x, ef.x, fmaf(hf.y, ef.y, dot));
+          w32[pp] = pack_bf16(arow[8 * q + 2 * pp] * scale - lab * ef.x, arow[8 * q + 2 * pp + 1] * scale - lab * ef.y);
+        }
+        dst[q] = w;
+      }
+    }
+    s_dot[slot][row] = dot;
+    named_bar_sync(1, 256);
+    if (slot == 0 && r < capacity) {
+      if (live) {
+        float zy = s_dot[0][row] + s_dot[1][row];
+        if (HAS_BIAS) zy += bias[y];
+        const float lse2 = log2f(z) - crow_of(direct, r, n_valid);   // (the offset is 0 unless the pass runs behind the two-pass forward)
+        float rl, wg2;
+        ce_row_terms(direct.row, r, lse2 * kLn2, zy, rl, wg2);
+        direct.lse[r] = lse2 * kLn2;
+        direct.cvec[r] = -lse2 + log2f(wg2 * inv_n);
+        direct.row_loss[r] = rl;
+        if (direct.row.roww) direct.row.roww[r] = wg2;
+      } else {
+        direct.cvec[r] = -INFINITY;  // rows beyond T_v contribute nothing to the dE pass
+      }
+    }
+  } else if (FUSED) {
+    // partial (this column split) un-normalised gradient and row sums; ce_fused_finalize_kernel reduces the splits
+    float* o = reinterpret_cast<float*>(out) + (size_t)split * capacity * D;
+    if (r < n_valid) {
+      if (slot == 0) zpart[(size_t)split * capacity + r] = s_row[row];
+      float4* dst = reinterpret_cast<float4*>(o + (size_t)r * D + slot * DW);
+#pragma unroll 4
+      for (int c = 0; c < DW; c += 4) dst[c >> 2] = *reinterpret_cast<const float4*>(arow + c);
     }
   } else {
-    const int ew = warp - 2, quarter = warp & 3;                 // lane quarter
-    const int grp = ew / (4 * CG), cg = (ew % (4 * CG)) >> 2, slot = grp * CG + cg;   // warp set, column group
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;
-    uint32_t g0 = 0, nseg = 0;   // ring position of the segment's first tile; segment count (parity of bar_a / bar_acc)
-    for (CeSeg sg = seg0; sg.valid; g0 += sg.n, ++nseg, sg.advance()) {
-    const int r0 = sg.row_tile * kT, n_ct = sg.n, jg0 = sg.j0;   // first row (token or item), column tiles [jg0, jg0 + n_ct)
-    const bool partial = PERSIST && n_ct != n_ct_all;            // other CTAs hold the rest of this row tile's columns
-    float crow = 0.f;
-    if (MODE == 0) crow = (r0 + row < n_valid) ? cvec[r0 + row] : -INFINITY;
-    if (FUSED) crow = (r0 + row < n_valid) ? (direct.use_lse_off ? -direct.lse[r0 + row] * kLog2e : 0.f) : -INFINITY;
-    float zacc = 0.f;  // FUSED: sum of G~ over this thread's columns
-    float gsum = 0.f;  // COL mode with bias: sum over tokens of G (before the e^{b_i} row factor) -> bias gradient
-    if (A_TMEM) {
-      // thread (row, column group) copies its slice of the row tile from global memory into TMEM: K elements
-      // [cg*D/CG, (cg+1)*D/CG) of row r0+row -> packed columns [cg*D/(2CG), ...); rows beyond the matrix read as zero
-      constexpr int WORDS = D / 2 / kSlots;  // 32-bit words per thread
-      static_assert(WORDS % 16 == 0, "row-tile copy works in 16-word TMEM stores");
-      const bool in = (r0 + row) < n_rows;
-      const uint4* src = reinterpret_cast<const uint4*>(a_rows + (size_t)(in ? r0 + row : 0) * D + slot * (D / kSlots));
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
+    if (r < n_valid) {
+      const float inv_n = loss_inv[0] * (direct.row.roww ? direct.row.roww[r] : 1.f);
+      const int y = labels[r];
+      const uint4* ey = reinterpret_cast<const uint4*>(table + (size_t)y * D + slot * DW);
+      uint4* dst = reinterpret_cast<uint4*>(o + (size_t)r * D + slot * DW);
+#pragma unroll 4
+      for (int q = 0; q < DW / 8; ++q) {
+        const uint4 e = ey[q];
+        const __nv_bfloat162* e2 = reinterpret_cast<const __nv_bfloat162*>(&e);
+        uint4 w;
+        uint32_t* w32 = reinterpret_cast<uint32_t*>(&w);
 #pragma unroll
-      for (int c = 0; c < WORDS; c += 16) {
-        uint32_t v[16];
-#pragma unroll
-        for (int q = 0; q < 16; q += 4) {
-          const uint4 t4 = in ? __ldg(src + ((c + q) >> 2)) : make_uint4(0u, 0u, 0u, 0u);
-          v[q] = t4.x; v[q + 1] = t4.y; v[q + 2] = t4.z; v[q + 3] = t4.w;
+        for (int pp = 0; pp < 4; ++pp) {
+          const float2 ef = __bfloat1622float2(e2[pp]);
+          w32[pp] = pack_bf16(arow[8 * q + 2 * pp] - inv_n * ef.x, arow[8 * q + 2 * pp + 1] - inv_n * ef.y);
         }
-        if (PRESCALE) {   // fused pass: the row tile carries log2(e), so S comes out of the tensor core in log2 units
-#pragma unroll
-          for (int q = 0; q < 16; ++q) {
-            const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&v[q]));
-            v[q] = pack_bf16(f.x * kLog2e, f.y * kLog2e);
-          }
-        }
-        tmem_st16(tmem_a + lane_base + slot * WORDS + c, v);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_a);
-    }
-    // Software pipeline over CW-column chunks of this warp's kW = 64 columns: while the exponentials of one chunk run, the
-    // tcgen05.ld of the next chunk of the SAME tile is in flight.  A warp-wide load occupies the quarter's TMEM read port for
-    // ~2 cycles per column (256 cycles per tile and SM sub-partition); with load-everything -> wait -> compute that time was
-    // MUFU idle time (ncu r2b: MUFU 61-65 % busy, ~1400 cycles per tile against 1024 of MUFU work and 1168 of tensor work).
-    // The pipeline does NOT reach into the next tile: S of tile j+1 only completes one tile of tensor work after the G of tile
-    // j-1 was handed over (two S buffers, in-order issue), i.e. about when this tile's epilogue ends - a prefetch placed
-    // before this tile's last chunk waited ~500 cycles for it (measured r2i: 1.02 -> 1.44 ms).
-    constexpr int CW = 16, NCH = kW / CW;
-    static_assert(NCH >= 2 && NCH % 2 == 0, "chunk pipeline: pairs of 16-column chunks");
-    // the first chunk of the NEXT tile is fetched before this tile's last chunk is exponentiated - only with >= 3 S buffers:
-    // with two, S of tile j+1 completes about when the epilogue of tile j ends (measured r2i: such a prefetch costs 40 %)
-    // (a set's next tile is j + GROUPS; its S is issued behind the second GEMM of tile j + GROUPS - NBUF, which must not
-    //  depend on THIS tile's G: NBUF > GROUPS)
-    constexpr bool PREFETCH = (NBUF >= 3) && (NBUF > GROUPS);
-    auto s_wait = [&](int j) {   // j: tile of this segment; g0 + j: its position in the S-buffer / smem rings
-      mbar_wait(&bar_sfull[(g0 + j) % NSTAGE], ((g0 + j) / NSTAGE) & 1);
-      tc_fence_after();
-    };
-    auto s_addr = [&](int j) -> uint32_t { return tmem + lane_base + (uint32_t)((g0 + j) % NBUF) * TN + cg * kW; };
-    uint32_t rawA[CW], rawB[CW];
-#if RP_CE_ABLATE == 4
-#pragma unroll
-    for (int q = 0; q < CW; ++q) rawA[q] = rawB[q] = __float_as_uint(-1.f - 0.01f * (lane + q));
-#endif
-    for (int j = grp; j < n_ct; j += GROUPS) {   // two warp sets: this one owns every GROUPS-th column tile (= one S buffer)
-      const uint32_t b = (g0 + j) % NBUF, s = (g0 + j) % NSTAGE;
-      if (COLCONST) mbar_wait(&bar_full[s], ((g0 + j) / NSTAGE) & 1);  // s_cc[s] was written by the async proxy
-      if (threadIdx.x == 64) RP_CTR(0, g0 + j);   // epilogue arrives at tile
-      if (!PREFETCH || j == grp || RP_CE_ABLATE == 2) s_wait(j);
-      if (threadIdx.x == 64) RP_CTR(1, g0 + j);   // S observed complete
-#if RP_CE_ABLATE == 2  // diagnostic build (tools/ce_variants.sh): no epilogue work at all -> MMA + TMA pipeline alone
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_pfull[b]);
-      continue;
-#endif
-      const uint32_t sbase = s_addr(j);
-      // G = exp2(S*log2e + offset) of one CW-column chunk -> CW/2 packed bf16 pairs, written in place over the warp's own
-      // (already consumed) S columns: chunk k lands in packed columns [k CW/2, (k+1) CW/2)
-      auto chunk_e = [&](const uint32_t (&raw)[CW], int k, auto every_c) {
-        constexpr int EVERY = decltype(every_c)::value;
-        uint32_t pk[CW / 2];
-        const int col0 = (jg0 + j) * TN + cg * kW + k * CW;
-        if (COLCONST) {
-          const float4* cc = reinterpret_cast<const float4*>(&s_cc[s][cg * kW + k * CW]);
-#pragma unroll
-          for (int q = 0; q < CW; q += 4) {
-            const float4 o = cc[q >> 2];
-            const float g0_ = ce_ex2<3, EVERY>(fmaf(__uint_as_float(raw[q + 0]), kLog2e, o.x), q + 0);
-            const float g1_ = ce_ex2<3, EVERY>(fmaf(__uint_as_float(raw[q + 1]), kLog2e, o.y), q + 1);
-            const float g2_ = ce_ex2<3, EVERY>(fmaf(__uint_as_float(raw[q + 2]), kLog2e, o.z), q + 2);
-            const float g3_ = ce_ex2<3, EVERY>(fmaf(__uint_as_float(raw[q + 3]), kLog2e, o.w), q + 3);
-            if (HAS_BIAS) gsum += (g0_ + g1_) + (g2_ + g3_);
-            pk[(q >> 1) + 0] = pack_bf16(g0_, g1_);
-            pk[(q >> 1) + 1] = pack_bf16(g2_, g3_);
-          }
-        } else {
-          float sv[CW];
-#pragma unroll
-          for (int q = 0; q < CW; ++q) sv[q] = __uint_as_float(raw[q]);
-          if (HAS_BIAS) {  // per-column bias: s + b before the exponential (warp-uniform 16-byte loads)
-#pragma unroll
-            for (int q = 0; q < CW; q += 4) {
-              const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + col0 + q));
-              sv[q + 0] += b4.x;
-              sv[q + 1] += b4.y;
-              sv[q + 2] += b4.z;
-              sv[q + 3] += b4.w;
-            }
-          }
-          if (col0 + CW <= n_items) {  // (warp-uniform) every column of this chunk exists: no per-element masking in the hot loop
-            float z0 = 0.f, z1 = 0.f;
-#pragma unroll
-            for (int q = 0; q < CW; q += 2) {
-              const float g0_ = PRESCALE ? ce_ex2<3, EVERY>(sv[q + 0], q + 0) : ce_ex2<3, EVERY>(fmaf(sv[q + 0], kLog2e, crow), q + 0);
-              const float g1_ = PRESCALE ? ce_ex2<3, EVERY>(sv[q + 1], q + 1) : ce_ex2<3, EVERY>(fmaf(sv[q + 1], kLog2e, crow), q + 1);
-              if (FUSED) {
-                z0 += g0_;
-                z1 += g1_;
-              }
-              pk[q >> 1] = pack_bf16(g0_, g1_);
-            }
-            if (FUSED) zacc += z0 + z1;
-          } else {  // ragged last tile of the catalog: columns beyond it do not exist
-#pragma unroll
-            for (int q = 0; q < CW; q += 2) {
-              float g0_ = PRESCALE ? ex2f(sv[q + 0]) : ex2f(fmaf(sv[q + 0], kLog2e, crow));
-              float g1_ = PRESCALE ? ex2f(sv[q + 1]) : ex2f(fmaf(sv[q + 1], kLog2e, crow));
-              if (col0 + q >= n_items) g0_ = 0.f;
-              if (col0 + q + 1 >= n_items) g1_ = 0.f;
-              if (FUSED) zacc += g0_ + g1_;
-              pk[q >> 1] = pack_bf16(g0_, g1_);
-            }
-          }
-        }
-#if RP_CE_ABLATE == 1  // diagnostic build: keep the TMEM traffic, drop the exponentials (G = bf16(S))
-#pragma unroll
-        for (int q = 0; q < CW; q += 2) pk[q >> 1] = pack_bf16(__uint_as_float(raw[q]), __uint_as_float(raw[q + 1]));
-#endif
-#if RP_CE_ABLATE == 3   // diagnostic: exponentials without the TMEM store of G
-        if (pk[0] == 0x12345678u && pk[CW / 2 - 1] == 0x9abcdef0u) tmem_st8(sbase + k * (CW / 2), pk);
-#else
-        tmem_st8(sbase + k * (CW / 2), pk);
-#endif
-      };
-      // the two epilogue warps that share the MMA-issuing thread's sub-partition (lane quarter 1) lose ~700 cycles per tile to
-      // its blocked dispatch: RP_CE_POLY_EVERY_Q1 moves a share of THEIR exponentials to the FMA pipe
-      auto chunk = [&](const uint32_t (&raw)[CW], int k) {
-        if (RP_CE_POLY_EVERY_Q1 != RP_CE_POLY_EVERY_BWD && quarter == 1)
-          chunk_e(raw, k, std::integral_constant<int, RP_CE_POLY_EVERY_Q1>{});
-        else
-          chunk_e(raw, k, std::integral_constant<int, RP_CE_POLY_EVERY_BWD>{});
-      };
-#if RP_CE_ABLATE == 4   // diagnostic: no TMEM loads (the exponentials run on whatever the registers hold)
-#define tmem_ld16(a, r) asm volatile("" : "+r"(r[0]), "+r"(r[5]), "+r"(r[10]), "+r"(r[15]))
-#endif
-      if (!PREFETCH || j == grp) tmem_ld16(sbase, rawA);
-#pragma unroll
-      for (int k = 0; k < NCH; k += 2) {
-        tmem_ld_wait();                                   // chunk k has landed in rawA
-        tmem_ld16(sbase + (k + 1) * CW, rawB);            // chunk k+1 is on its way while chunk k is exponentiated
-        chunk(rawA, k);
-        tmem_ld_wait();                                   // chunk k+1 has landed in rawB
-        if (k + 2 < NCH) {
-          tmem_ld16(sbase + (k + 2) * CW, rawA);
-        } else if (PREFETCH && j + GROUPS < n_ct) {       // S of the set's next tile was issued long ago: normally complete
-          s_wait(j + GROUPS);
-          tmem_ld16(s_addr(j + GROUPS), rawA);
-        }
-        chunk(rawB, k + 1);
-      }
-#if RP_CE_ABLATE == 4
-#undef tmem_ld16
-#endif
-      if (threadIdx.x == 64) RP_CTR(2, g0 + j);   // exponentials done, stores issued
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_pfull[b]);
-      if (threadIdx.x == 64) RP_CTR(3, g0 + j);   // G handed to the MMA thread
-      if (lane == 0) RP_CTR(8 + (ew & 7), g0 + j);
-    }
-    // ---- final: accumulator -> global; this warp owns accumulator columns [cg*D/CG, (cg+1)*D/CG), 16 at a time
-    mbar_wait(&bar_acc, nseg & 1);
-    tc_fence_after();
-    const int r = r0 + row;
-    constexpr int DW = D / kSlots;
-    const uint32_t abase = tmem_acc + lane_base + slot * DW;
-    if (COLCONST) {
-      float* o = reinterpret_cast<float*>(out);
-      // biased head: G carries a per-item factor e^{b_i}; it was left out of the loop and is applied to the row here
-      const float rs = (HAS_BIAS && r < n_items) ? __expf(bias[r]) : 1.f;
-      if (HAS_BIAS) {
-        s_gsum[slot][row] = gsum;
-        asm volatile("bar.sync 1, %0;" ::"r"(kEW * 32) : "memory");  // epilogue warps only
-        if (slot == 0 && r < n_items) {
-          float tot = 0.f;
-#pragma unroll
-          for (int k = 0; k < kSlots; ++k) tot += s_gsum[k][row];
-          if (partial) atomicAdd(d_bias + r, tot * rs); else d_bias[r] = tot * rs;
-        }
-        if (PERSIST) asm volatile("bar.sync 1, %0;" ::"r"(kEW * 32) : "memory");  // s_gsum is rewritten by the next segment
-      }
-#pragma unroll 1
-      for (int c = 0; c < DW; c += 16) {
-        uint32_t a16[16];
-        tmem_ld16(abase + c, a16);
-        tmem_ld_wait();
-        if (r < n_items) {
-          float4* dst = reinterpret_cast<float4*>(o + (size_t)r * D + slot * DW + c);
-#pragma unroll
-          for (int q = 0; q < 16; q += 4) {
-            const float4 v = make_float4(__uint_as_float(a16[q]) * rs, __uint_as_float(a16[q + 1]) * rs,
-                                         __uint_as_float(a16[q + 2]) * rs, __uint_as_float(a16[q + 3]) * rs);
-            // a slice of the row tile's columns: 16-byte vector reduction into the zeroed output (at most two CTAs share a
-            // row tile while a CTA's slice is longer than one row tile's column range, so the sum does not depend on order)
-            if (partial) atomicAdd(dst + (q >> 2), v); else dst[q >> 2] = v;
-          }
-        }
-      }
-      // the accumulator / row-tile columns are handed back to the MMA thread by the next segment's bar_a arrivals
-      tc_fence_before();
-    } else if (FUSED && direct.d_hc != nullptr) {
-      // ---- no column splits: finish here.  z_t = sum of the four slots' row sums; dH = acc / (z T_v) - E[y] / T_v
-      s_gsum[slot][row] = zacc;
-      asm volatile("bar.sync 1, %0;" ::"r"(kEW * 32) : "memory");
-      float z = 0.f;
-#pragma unroll
-      for (int k = 0; k < kSlots; ++k) z += s_gsum[k][row];
-      const bool live = r < n_valid;
-      const float inv_n = n_valid > 0 ? 1.f / (float)n_valid : 0.f;
-      const int y = live ? labels[r] : 0;
-      float wg = (live && direct.row.w_ext) ? direct.row.w_ext[r] : 1.f;   // gradient weight of the row
-      if (direct.row.kind == 1) {
-        // LogInCE: the weight needs the target logit before the gradient can be scaled - one extra pass over h . E[y]
-        float dp = 0.f;
-        if (live) {
-          const uint4* ey = reinterpret_cast<const uint4*>(table + (size_t)y * D + slot * DW);
-          const uint4* hr = reinterpret_cast<const uint4*>(a_rows + (size_t)r * D + slot * DW);
-#pragma unroll
-          for (int q = 0; q < DW / 8; ++q) {
-            const uint4 e = __ldg(ey + q), hh = __ldg(hr + q);
-            const __nv_bfloat162* e2 = reinterpret_cast<const __nv_bfloat162*>(&e);
-            const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&hh);
-#pragma unroll
-            for (int pp = 0; pp < 4; ++pp) {
-              const float2 ef = __bfloat1622float2(e2[pp]), hf = __bfloat1622float2(h2[pp]);
-              dp = fmaf(hf.x, ef.x, fmaf(hf.y, ef.y, dp));
-            }
-          }
-        }
-        s_dot[slot][row] = dp;
-        asm volatile("bar.sync 1, %0;" ::"r"(kEW * 32) : "memory");
-        float zy0 = 0.f;
-#pragma unroll
-        for (int k = 0; k < kSlots; ++k) zy0 += s_dot[k][row];
-        if (HAS_BIAS) zy0 += bias[y];
-        asm volatile("bar.sync 1, %0;" ::"r"(kEW * 32) : "memory");   // s_dot is written again below
-        float rl_unused;
-        if (live) ce_row_terms(direct.row, r, __logf(z) - crow * kLn2, zy0, rl_unused, wg);
-      }
-      const float scale = live ? wg * inv_n / z : 0.f;
-      const float lab = wg * inv_n;
-      float dot = 0.f;
-#pragma unroll 1
-      for (int c = 0; c < DW; c += 16) {
-        uint32_t a16[16];
-        tmem_ld16(abase + c, a16);
-        tmem_ld_wait();
-        if (live) {
-          const uint4* ey = reinterpret_cast<const uint4*>(table + (size_t)y * D + slot * DW + c);
-          const uint4* hr = reinterpret_cast<const uint4*>(a_rows + (size_t)r * D + slot * DW + c);
-          uint4* dst = reinterpret_cast<uint4*>(direct.d_hc + (size_t)r * D + slot * DW + c);
-#pragma unroll
-          for (int q = 0; q < 16; q += 8) {
-            const uint4 e = __ldg(ey + (q >> 3)), hh = __ldg(hr + (q >> 3));
-            const __nv_bfloat162* e2 = reinterpret_cast<const __nv_bfloat162*>(&e);
-            const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&hh);
-            uint4 w;
-            uint32_t* w32 = reinterpret_cast<uint32_t*>(&w);
-#pragma unroll
-            for (int pp = 0; pp < 4; ++pp) {
-              const float2 ef = __bfloat1622float2(e2[pp]), hf = __bfloat1622float2(h2[pp]);
-              dot = fmaf(hf.x, ef.x, fmaf(hf.y, ef.y, dot));
-              w32[pp] = pack_bf16(__uint_as_float(a16[q + 2 * pp]) * scale - lab * ef.x,
-                                  __uint_as_float(a16[q + 2 * pp + 1]) * scale - lab * ef.y);
-            }
-            dst[q >> 3] = w;
-          }
-        }
-      }
-      s_dot[slot][row] = dot;
-      asm volatile("bar.sync 1, %0;" ::"r"(kEW * 32) : "memory");
-      if (slot == 0 && r < capacity) {
-        if (live) {
-          float zy = 0.f;
-#pragma unroll
-          for (int k = 0; k < kSlots; ++k) zy += s_dot[k][row];
-          if (HAS_BIAS) zy += bias[y];
-          const float lse2 = log2f(z) - crow;   // (crow = 0 unless the pass runs behind the two-pass forward)
-          float rl, wg2;
-          ce_row_terms(direct.row, r, lse2 * kLn2, zy, rl, wg2);
-          direct.lse[r] = lse2 * kLn2;
-          direct.cvec[r] = -lse2 + log2f(wg2 * inv_n);
-          direct.row_loss[r] = rl;
-          if (direct.row.roww) direct.row.roww[r] = wg2;
-        } else {
-          direct.cvec[r] = -INFINITY;  // rows beyond T_v contribute nothing to the dE pass
-        }
-      }
-    } else if (FUSED) {
-      // partial (this column split) un-normalised gradient and row sums; ce_fused_finalize_kernel reduces the splits
-      float* o = reinterpret_cast<float*>(out) + (size_t)split * capacity * D;
-      if (r < n_valid) zpart[((size_t)split * kSlots + slot) * capacity + r] = zacc;
-#pragma unroll 1
-      for (int c = 0; c < DW; c += 16) {
-        uint32_t a16[16];
-        tmem_ld16(abase + c, a16);
-        tmem_ld_wait();
-        if (r < n_valid) {
-          float4* dst = reinterpret_cast<float4*>(o + (size_t)r * D + slot * DW + c);
-#pragma unroll
-          for (int q = 0; q < 16; q += 4)
-            dst[q >> 2] = make_float4(__uint_as_float(a16[q]), __uint_as_float(a16[q + 1]), __uint_as_float(a16[q + 2]),
-                                      __uint_as_float(a16[q + 3]));
-        }
-      }
-    } else {
-      __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
-      const float inv_n = loss_inv[0] * ((direct.row.roww && r < n_valid) ? direct.row.roww[r] : 1.f);
-      const int y = (r < n_valid) ? labels[r] : 0;
-#pragma unroll 1
-      for (int c = 0; c < DW; c += 16) {
-        uint32_t a16[16];
-        tmem_ld16(abase + c, a16);
-        tmem_ld_wait();
-        if (r < n_valid) {
-          const uint4* ey = reinterpret_cast<const uint4*>(table + (size_t)y * D + slot * DW + c);
-          uint4* dst = reinterpret_cast<uint4*>(o + (size_t)r * D + slot * DW + c);
-#pragma unroll
-          for (int q = 0; q < 16; q += 8) {
-            const uint4 e = ey[q >> 3];
-            const __nv_bfloat162* e2 = reinterpret_cast<const __nv_bfloat162*>(&e);
-            uint4 w;
-            uint32_t* w32 = reinterpret_cast<uint32_t*>(&w);
-#pragma unroll
-            for (int p = 0; p < 4; ++p) {
-              const float2 ef = __bfloat1622float2(e2[p]);
-              w32[p] = pack_bf16(__uint_as_float(a16[q + 2 * p]) - inv_n * ef.x,
-                                 __uint_as_float(a16[q + 2 * p + 1]) - inv_n * ef.y);
-            }
-            dst[q >> 3] = w;
-          }
-        }
+        dst[q] = w;
       }
     }
-    }  // segments
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 512);
 }
 
 // dE[y_t, :] -= Hc[t, :] / T_v   (fp32 atomics; several tokens may share a label)
@@ -1277,7 +780,7 @@ __global__ void ce_dh_reduce_kernel(const float* __restrict__ part, int n_splits
   }
 }
 
-// d = 512: S and the [128 x 512] fp32 gradient accumulator do not fit the 512 TMEM columns together, so the backward
+// d = 512: the [128 x 512] fp32 gradient accumulator does not fit the registers of the two warpgroups, so the backward
 // materialises the softmax numerators G (bf16) for a chunk of tokens at a time and runs three plain GEMMs per chunk.
 // Chunk rows: as many as fit the G budget (RP_CE_WIDE_G_BYTES, default 8 GiB), multiple of 128.
 static long long wide_ldg(int n_items) { return ((long long)n_items + 63) / 64 * 64; }
@@ -1320,7 +823,7 @@ static const int kMaxSplitsFwd = 32;   // two-pass forward: only (max, sum) pair
 static const int kWideSplitK = 16;     // d = 512 backward: split-K partials of the dH GEMM
 
 static size_t ce_ws_base_bytes(int cap, int d) {
-  return (size_t)cap * kMaxSplitsFwd * 2 * sizeof(float2) + 4096 + 64 + (size_t)kMaxSplits * kBwdCG * kCeMaxGroups * cap * 4 +
+  return (size_t)cap * kMaxSplitsFwd * 2 * sizeof(float2) + 4096 + 64 + (size_t)kMaxSplits * cap * 4 +
          (size_t)(cap + 3) / 4 * 16 + (d <= 256 ? (size_t)kMaxSplits * cap * d * 4 : 0) + 256;
 }
 static size_t ce_ws_bytes(int cap, int n_items, int d) {
@@ -1344,21 +847,13 @@ static CeWs ce_ws(void* workspace, int cap, int d) {
   r.flag = reinterpret_cast<int32_t*>(r.ticket + 4);
   w += 64;
   r.zpart = reinterpret_cast<float*>(w);
-  w += (size_t)kMaxSplits * kBwdCG * kCeMaxGroups * cap * 4;
+  w += (size_t)kMaxSplits * cap * 4;
   r.roww = reinterpret_cast<float*>(w);   // gradient weight per row (CeRowOpts), written by every forward finalisation
   w += (size_t)(cap + 3) / 4 * 16;
   r.part_dh = reinterpret_cast<float*>(w);
   (void)d;
   return r;
 }
-
-#ifdef RP_CE_TRACE
-RP_API int rp_debug_ce_trace(unsigned long long* host_out, int n_words) {
-  RP_CUDA_CHECK(cudaDeviceSynchronize());
-  RP_CUDA_CHECK(cudaMemcpyFromSymbol(host_out, rp::g_ce_trace, sizeof(unsigned long long) * (size_t)n_words));
-  return RP_OK;
-}
-#endif
 
 RP_API size_t rp_ce_head_workspace(int capacity_tokens, int n_items, int d) {
   if (capacity_tokens <= 0 || n_items <= 0 || d <= 0) return 0;
@@ -1377,55 +872,25 @@ static int launch_ce_fwd(const CUtensorMap& tmA, const CUtensorMap& tmB, const i
   return RP_OK;
 }
 
-// two epilogue warp sets: d = 128 with two S buffers (the row-tile copy and the accumulator read-out split 4 ways there)
-constexpr int ce_groups_of(int kch, int nbuf) { return (RP_CE_GROUPS == 2 && kch == 2 && nbuf == 2) ? 2 : 1; }
-static int ce_z_slots(int d) {
-  constexpr bool a_tmem = (RP_CE_A_TMEM != 0) && (RP_CE_ORDER == 1);
-  const int nbuf = (d <= 128 && a_tmem) ? 2 : ((RP_CE_NBUF3 && d <= 128) ? 3 : 2);
-  if (d <= 128 && a_tmem && RP_CE_TN64 != 0) return RP_CE_TN64_GROUPS == 2 ? 2 : kBwdCG;
-  return kBwdCG * ce_groups_of(d / 64, nbuf);
-}
-
 template <int KCH, int NSTAGE, int MODE>
 static int launch_ce_bwd(const CUtensorMap& tmA, const void* b_mat, int b_rows, const void* a_rows, const float* cvec,
                          const int32_t* labels,
                          const void* table, const float* loss_inv, const int32_t* n_valid, int n_items, const float* bias,
                          float* d_bias, void* out, int grid, const int32_t* safe_flag, int run_if_safe, int n_splits,
                          int capacity, float* zpart, cudaStream_t stream, const CeDirect& direct = CeDirect{nullptr, nullptr, nullptr, nullptr, CeRowOpts{nullptr, nullptr, 0, 0.f, 0.f}, 0}) {
-  // d <= 128: the row tile goes to TMEM (2 S buffers + accumulator + operand = 448 columns) and its 32 KB of smem become
-  // an extra pipeline stage; d = 256: row tile in smem, 2 S buffers + accumulator = 512 columns
-  // RP_CE_ORDER 1: both directions keep the row tile in TMEM (two S buffers suffice once the issue order no longer drains the
-  // pipe); otherwise round 1's choice (measured then: the TMEM row tile paid for the dE pass only, because it forces 2 buffers)
-  constexpr bool A_TMEM = (RP_CE_A_TMEM != 0) && KCH <= 2 && (MODE == 1 || RP_CE_ORDER == 1);
-  // column tiles: 64 wide in four S buffers when the row tile is in TMEM and the issue order is the in-order one (see the
-  // kernel's header comment), else 128 wide in two (three without the TMEM row tile)
-  constexpr int TN = (A_TMEM && RP_CE_ORDER == 1 && RP_CE_TN64 != 0) ? 64 : 128;
-  constexpr int NBUF = TN == 64 ? 4 : (A_TMEM ? 2 : ((RP_CE_NBUF3 && KCH <= 2) ? 3 : 2));
-  constexpr bool INORDER = (RP_CE_ORDER == 1) && (NBUF == 2 || TN == 64);
-  constexpr int NST = (NSTAGE + (A_TMEM ? 1 : 0)) * (128 / TN);   // the same bytes of column tiles in flight
-  const int smem = (A_TMEM ? 0 : 1) * KCH * kChunk + NST * KCH * TN * 128 + 1024;
-  CUtensorMap tmB;   // column-side matrix, one [TN rows x 64 columns] box per chunk
+  // row tile + a ring of NSTAGE column tiles; the fp32 accumulator stage reuses the ring at the end
+  const int ring = NSTAGE * KCH * kTN * 128, stage = 128 * (KCH * 64 + 4) * 4;
+  const int smem = KCH * kChunk + (ring > stage ? ring : stage) + 1024;
+  CUtensorMap tmB;   // column-side matrix, one [64 rows x 64 columns] box per chunk
   {
-    const int rc = make_tmap_bf16(&tmB, b_mat, b_rows, KCH * 64, KCH * 64, TN);
+    const int rc = make_tmap_bf16(&tmB, b_mat, b_rows, KCH * 64, KCH * 64, kTN);
     if (rc != RP_OK) return rc;
   }
   // the biased head (BERT4Rec) is a separate instantiation: its per-column adds / row sums cost an instruction per logit
-  constexpr int GROUPS = TN == 64 ? RP_CE_TN64_GROUPS : ce_groups_of(KCH, NBUF);
-  constexpr int CG = (TN == 64 && GROUPS == 2) ? 1 : kBwdCG;
-  // dE pass with the row tile in TMEM: persistent work slices (see CeSeg) - `grid` row tiles become one CTA per SM, the
-  // output is zeroed first because slices that end inside a row tile add their part with reductions
-  constexpr bool PERSIST = (MODE == 1) && A_TMEM && (RP_CE_PERSIST != 0);
-  constexpr int NI = (INORDER && RP_CE_ISSUERS > 1) ? RP_CE_ISSUERS : 1;
-  auto kern = bias ? ce_bwd_kernel<KCH, NST, MODE, NBUF, A_TMEM, INORDER, true, GROUPS, PERSIST, TN, CG, NI>
-                   : ce_bwd_kernel<KCH, NST, MODE, NBUF, A_TMEM, INORDER, false, GROUPS, PERSIST, TN, CG, NI>;
+  auto kern = bias ? ce_bwd_kernel<KCH, NSTAGE, MODE, true> : ce_bwd_kernel<KCH, NSTAGE, MODE, false>;
   RP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  if (PERSIST) {
-    RP_CUDA_CHECK(cudaMemsetAsync(out, 0, (size_t)n_items * KCH * 64 * sizeof(float), stream));
-    if (d_bias) RP_CUDA_CHECK(cudaMemsetAsync(d_bias, 0, (size_t)n_items * sizeof(float), stream));
-    if (grid > sm_count()) grid = sm_count();
-  }
-  kern<<<grid, 64 + GROUPS * 4 * CG * 32 + (NI - 1) * 32, smem, stream>>>(tmA, tmB, reinterpret_cast<const __nv_bfloat16*>(a_rows), cvec, labels,
-                                            reinterpret_cast<const __nv_bfloat16*>(table), loss_inv,
+  kern<<<grid, kThreads, smem, stream>>>(tmA, tmB, reinterpret_cast<const __nv_bfloat16*>(a_rows), cvec, labels,
+                                         reinterpret_cast<const __nv_bfloat16*>(table), loss_inv,
                                          n_valid, n_items, bias, d_bias, out, safe_flag, run_if_safe, n_splits, capacity, zpart, direct);
   RP_LAUNCH_CHECK();
   return RP_OK;
@@ -1439,13 +904,13 @@ static int dispatch_ce_bwd(int d, const CUtensorMap& tmA, const void* b_mat, int
                            int capacity, float* zpart, cudaStream_t stream, const CeDirect& direct = CeDirect{nullptr, nullptr, nullptr, nullptr, CeRowOpts{nullptr, nullptr, 0, 0.f, 0.f}, 0}) {
   switch (d) {
     case 64:
-      return launch_ce_bwd<1, 6, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
+      return launch_ce_bwd<1, 8, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
                                        safe_flag, run_if_safe, n_splits, capacity, zpart, stream, direct);
     case 128:
-      return launch_ce_bwd<2, RP_CE_NSTAGE_D128, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
+      return launch_ce_bwd<2, 6, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
                                        safe_flag, run_if_safe, n_splits, capacity, zpart, stream, direct);
     case 256:
-      return launch_ce_bwd<4, 2, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
+      return launch_ce_bwd<4, 4, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
                                        safe_flag, run_if_safe, n_splits, capacity, zpart, stream, direct);
     default:
       return RP_ESHAPE;
@@ -1519,7 +984,7 @@ RP_API int rp_ce_head_fwd_w(const void* hc, const void* table, const float* bias
     } else
     ce_fused_finalize_kernel<<<blocks, 256, 0, stream>>>(ws.part_dh, ws.zpart, reinterpret_cast<const __nv_bfloat16*>(hc),
                                                          reinterpret_cast<const __nv_bfloat16*>(table), labels, bias, n_valid,
-                                                         ws.flag, P, ce_z_slots(d), capacity, d, lse, cvec,
+                                                         ws.flag, P, 1, capacity, d, lse, cvec,
                                                          reinterpret_cast<__nv_bfloat16*>(d_hc), ws.block_sums, ws.ticket, loss_out,
                                                          CeRowOpts{row_weight, ws.roww, loss_kind, log_eps, clamp}, 0, 1);
     RP_LAUNCH_CHECK();
@@ -1527,7 +992,7 @@ RP_API int rp_ce_head_fwd_w(const void* hc, const void* table, const float* bias
   }
   int P2 = pick_splits(hint_tiles, n_item_tiles, kMaxSplitsFwd);
   if (fused) {  // two-pass fallback behind the fused pass: it only runs when the bound failed; launching (and retiring) tens of
-                // thousands of CTAs that exit at once cost ~40 us per step, so keep it at about two waves
+                // thousands of CTAs that exit at once is not free, so keep it at about two waves
     const int cap = (2 * sm_count() + n_tok_tiles - 1) / n_tok_tiles;
     if (P2 > cap) P2 = cap;
   }
@@ -1539,7 +1004,7 @@ RP_API int rp_ce_head_fwd_w(const void* hc, const void* table, const float* bias
   }
   if (rc != RP_OK) return rc;
   ce_finalize_kernel<<<blocks, 256, 0, stream>>>(ws.part, reinterpret_cast<const __nv_bfloat16*>(hc),
-                                                 reinterpret_cast<const __nv_bfloat16*>(table), labels, bias, n_valid, P2 * 2,
+                                                 reinterpret_cast<const __nv_bfloat16*>(table), labels, bias, n_valid, P2,
                                                  capacity, d, lse, cvec, ws.block_sums, ws.ticket, loss_out, skip,
                                                  CeRowOpts{row_weight, ws.roww, loss_kind, log_eps, clamp});
   RP_LAUNCH_CHECK();
@@ -1564,7 +1029,7 @@ RP_API int rp_ce_head_fwd_w(const void* hc, const void* table, const float* bias
     } else {
       ce_fused_finalize_kernel<<<blocks, 256, 0, stream>>>(ws.part_dh, ws.zpart, reinterpret_cast<const __nv_bfloat16*>(hc),
                                                            reinterpret_cast<const __nv_bfloat16*>(table), labels, bias, n_valid,
-                                                           ws.flag, P, ce_z_slots(d), capacity, d, lse, cvec,
+                                                           ws.flag, P, 1, capacity, d, lse, cvec,
                                                            reinterpret_cast<__nv_bfloat16*>(d_hc), ws.block_sums, ws.ticket, loss_out,
                                                            CeRowOpts{row_weight, ws.roww, loss_kind, log_eps, clamp}, 1, 0);
     }

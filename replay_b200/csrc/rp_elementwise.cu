@@ -8,7 +8,7 @@
 // replay/models/nn/optimizer_utils/optimizer_factory.py:71-87 (torch.optim.Adam).
 #include "rp_host.h"
 #include "rp_philox.cuh"
-#include "rp_sm100.cuh"
+#include "rp_sm90.cuh"
 
 namespace rp {
 

@@ -1,4 +1,4 @@
-// rp_gemm.cu - generic batched bf16 GEMM on tcgen05 with a fused epilogue; the workhorse of the transformer body.
+// rp_gemm.cu - generic batched bf16 GEMM on wgmma with a fused epilogue; the workhorse of the transformer body.
 //
 //   C[m, n] = epilogue( alpha * sum_k A(m, k) * B(n, k) )            (per batch element)
 //
@@ -8,12 +8,9 @@
 //   (replay/nn/sequential/sasrec/transformer.py:36-46,99-106 ; replay/nn/ffn.py:43-57 ;
 //    replay/models/nn/sequential/sasrec/model.py:407-414,490-506 ; replay/models/nn/sequential/bert4rec/model.py:471-527).
 //
-// CTA = one 128 x BN output tile (x one K split).  warp 0: TMA producer, warp 1: MMA issuer, warps 2-5: epilogue.
-#include <stdlib.h>
-
 #include "rp_host.h"
 #include "rp_philox.cuh"
-#include "rp_sm100.cuh"
+#include "rp_sm90.cuh"
 
 namespace rp {
 
@@ -51,7 +48,7 @@ struct GemmParams {
   int k_limit_base;
 };
 
-// Epilogue of one [1 row x 32 columns] strip held in registers (shared by the tile kernel and the persistent kernel).
+// Epilogue of one [1 row x 32 columns] strip held in registers.
 struct EpiRow {
   long long c_base;   // element offset of this output row in C
   long long drop_row; // row index of the activation dropout stream (rp_philox.cuh): element (drop_row, column)
@@ -196,7 +193,9 @@ __device__ __forceinline__ void gemm_epilogue_chunk(const GemmParams& p, const f
       }
 }
 
-static constexpr int kGemmThreads = 192;
+// CTA = one 128 x BN output tile (x one K split).  Warpgroups 0 / 1: wgmma over rows [0, 64) / [64, 128) of the tile, then
+// the epilogue (thread = output row, warpgroup = column half); warp 8: TMA producer.
+static constexpr int kGemmThreads = 288;
 
 template <int BN, bool A_MN, bool B_MN, int NSTAGE>
 __global__ void __launch_bounds__(kGemmThreads, 1)
@@ -204,15 +203,19 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   constexpr int A_BYTES = 128 * 128;       // [128 x 64] bf16
   constexpr int B_BYTES = BN * 128;        // [BN x 64] bf16
   constexpr int STAGE = A_BYTES + B_BYTES;
+  constexpr int PITCH = BN + 4;            // fp32 accumulator stage, placed over the operand ring once the contraction ends
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ uint64_t bar_full[NSTAGE], bar_empty[NSTAGE], bar_acc;
-  __shared__ uint32_t tmem_slot;
+  __shared__ uint64_t bar_full[NSTAGE], bar_empty[NSTAGE];
   __shared__ __align__(16) float s_bias[BN];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_tile = blockIdx.x;
-  const int m_tile = blockIdx.y / p.split_k, ksplit = blockIdx.y % p.split_k;
+  // one linear grid dimension (no 65535 limit on the row tiles of tall GEMMs): n tile fastest, then K split, then m tile -
+  // CTAs launched side by side share their A rows in L2
+  const int n_tiles = (p.N + BN - 1) / BN;
+  const int n_tile = (int)(blockIdx.x % n_tiles);
+  const int mk = (int)(blockIdx.x / n_tiles);
+  const int m_tile = mk / p.split_k, ksplit = mk % p.split_k;
   const int bz = blockIdx.z, outer = bz / p.inner, in = bz % p.inner;
   const int m0 = m_tile * 128, n0 = n_tile * BN;
   if (p.m_limit_dev != nullptr && m0 + p.m_limit_base >= *p.m_limit_dev) return;  // whole tile beyond the dynamic row count
@@ -227,23 +230,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (threadIdx.x == 0) {
     for (int i = 0; i < NSTAGE; ++i) {
       mbar_init(&bar_full[i], 1);
-      mbar_init(&bar_empty[i], 1);
+      mbar_init(&bar_empty[i], 8);
     }
-    mbar_init(&bar_acc, 1);
     fence_barrier_init();
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == 1) tmem_alloc(&tmem_slot, BN < 32 ? 32 : BN);
-  if (p.bias != nullptr && threadIdx.x >= 64) {
-    for (int i = threadIdx.x - 64; i < BN; i += 128) s_bias[i] = (n0 + i < p.N) ? p.bias[n0 + i] : 0.f;
+  if (p.bias != nullptr && threadIdx.x < 256) {
+    for (int i = threadIdx.x; i < BN; i += 256) s_bias[i] = (n0 + i < p.N) ? p.bias[n0 + i] : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (elect_one()) {
       for (int kc = kc_begin, it = 0; kc < kc_end; ++kc, ++it) {
         const uint32_t s = it % NSTAGE, ph = (it / NSTAGE) & 1;
@@ -266,409 +264,75 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128, BN, A_MN, B_MN);
-      for (int kc = kc_begin, it = 0; kc < kc_end; ++kc, ++it) {
-        const uint32_t s = it % NSTAGE, ph = (it / NSTAGE) & 1;
-        mbar_wait(&bar_full[s], ph);
-        tc_fence_after();
-        const uint32_t a0 = smem_u32(smem + s * STAGE), b0 = a0 + A_BYTES;
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          const uint64_t ad = A_MN ? umma_desc_sw128(a0 + ks * 2048, 8192, 1024) : umma_desc_sw128(a0 + ks * 32, 16, 1024);
-          const uint64_t bd = B_MN ? umma_desc_sw128(b0 + ks * 2048, 8192, 1024) : umma_desc_sw128(b0 + ks * 32, 16, 1024);
-          umma_ss(tmem, ad, bd, idesc, (it | ks) != 0);
-        }
-        umma_commit(&bar_empty[s]);
-      }
-      umma_commit(&bar_acc);
-    }
-  } else {
-    // ------------------------------------------------ epilogue: thread = output row
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const int m = m0 + row;
-    mbar_wait(&bar_acc, 0);
-    tc_fence_after();
-    const bool row_ok = m < p.M;
-    const long long c_base = p.c_off0 + (long long)outer * p.c_oo + (long long)in * p.c_oi + (long long)m * p.ldc +
-                             (p.out_mode == 3 ? (long long)ksplit * p.c_split_stride : 0ll);
-    float rm = 1.f;
-    if (p.rowmask && row_ok) rm = p.rowmask[p.rowmask_off0 + (long long)outer * p.rowmask_oo + m] ? 1.f : 0.f;
-    EpiRow er;
-    er.c_base = c_base;
-    er.drop_row = (long long)bz * p.M + m;
-    er.rm = rm;
-    er.exp_off = (p.act == 3 && row_ok) ? p.row_exp2_offset[m] : 0.f;
-    er.keep_scale = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
-    er.drop_thr = p.drop_p > 0.f ? (uint32_t)(p.drop_p * 4294967296.0) : 0u;
-    er.seed_eff = p.seed + ((p.drop_p > 0.f && p.seed_ptr) ? *p.seed_ptr : 0ull);
-#pragma unroll 1
-    for (int c = 0; c < BN; c += 32) {
-      uint32_t raw[32];
-      tmem_ld32(tmem + ((uint32_t)(quarter * 32) << 16) + c, raw);
-      tmem_ld_wait();
-      if (!row_ok || n0 + c >= p.N) continue;
-      if (kc_begin >= kc_end) {  // empty contraction (dynamic K limit): the accumulator was never written
-#pragma unroll
-        for (int q = 0; q < 32; ++q) raw[q] = 0u;
-      }
-      gemm_epilogue_chunk(p, s_bias, er, raw, n0, c);
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, BN < 32 ? 32 : BN);
+  // ------------------------------------------------ warpgroup wg: rows [64 wg, 64 wg + 64) of the tile
+  const int wg = warp >> 2;
+  float acc[BN / 2];
+  acc_zero(acc);  // an empty contraction (dynamic K limit) leaves zeros
+  for (int kc = kc_begin, it = 0; kc < kc_end; ++kc, ++it) {
+    const uint32_t s = it % NSTAGE, ph = (it / NSTAGE) & 1;
+    mbar_wait(&bar_full[s], ph);
+    const uint32_t a0 = smem_u32(smem + s * STAGE) + wg * 8192, b0 = smem_u32(smem + s * STAGE + A_BYTES);
+    wg_fence_acc(acc);
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      const uint64_t ad = A_MN ? desc_mn(a0 + ks * 2048, 8192) : desc_k(a0 + ks * 32);
+      const uint64_t bd = B_MN ? desc_mn(b0 + ks * 2048, 8192) : desc_k(b0 + ks * 32);
+      WgmmaSS<BN>::template run<A_MN, B_MN>(acc, ad, bd, 1);
+    }
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bar_empty[s]);
+  }
+  named_bar_sync(1, 256);  // both warpgroups are done reading the ring
+  float* stage = reinterpret_cast<float*>(smem);
+  acc_to_stage(acc, stage, PITCH, wg * 64, 0);
+  named_bar_sync(1, 256);
+  // ------------------------------------------------ epilogue: thread = output row, warpgroup = column half
+  const int row = threadIdx.x & 127;
+  const int m = m0 + row;
+  const bool row_ok = m < p.M;
+  const long long c_base = p.c_off0 + (long long)outer * p.c_oo + (long long)in * p.c_oi + (long long)m * p.ldc +
+                           (p.out_mode == 3 ? (long long)ksplit * p.c_split_stride : 0ll);
+  float rm = 1.f;
+  if (p.rowmask && row_ok) rm = p.rowmask[p.rowmask_off0 + (long long)outer * p.rowmask_oo + m] ? 1.f : 0.f;
+  EpiRow er;
+  er.c_base = c_base;
+  er.drop_row = (long long)bz * p.M + m;
+  er.rm = rm;
+  er.exp_off = (p.act == 3 && row_ok) ? p.row_exp2_offset[m] : 0.f;
+  er.keep_scale = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
+  er.drop_thr = p.drop_p > 0.f ? (uint32_t)(p.drop_p * 4294967296.0) : 0u;
+  er.seed_eff = p.seed + ((p.drop_p > 0.f && p.seed_ptr) ? *p.seed_ptr : 0ull);
+  if (!row_ok) return;
+#pragma unroll 1
+  for (int c = wg * (BN / 2); c < (wg + 1) * (BN / 2); c += 32) {
+    if (n0 + c >= p.N) break;
+    uint32_t raw[32];
+    stage_ld32(stage + row * PITCH + c, raw);
+    gemm_epilogue_chunk(p, s_bias, er, raw, n0, c);
+  }
 }
 
 template <int BN, bool A_MN, bool B_MN, int NSTAGE>
 static int launch_gemm_n(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int batch, cudaStream_t st) {
-  const int smem = NSTAGE * (128 * 128 + BN * 128) + 1024;
+  const int ring = NSTAGE * (128 * 128 + BN * 128), stage = 128 * (BN + 4) * 4;
+  const int smem = (ring > stage ? ring : stage) + 1024;
   auto kern = gemm_kernel<BN, A_MN, B_MN, NSTAGE>;
   RP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  dim3 grid((p.N + BN - 1) / BN, ((p.M + 127) / 128) * p.split_k, batch);
+  const long long ctas = (long long)((p.N + BN - 1) / BN) * ((p.M + 127) / 128) * p.split_k;
+  if (ctas > 0x7fffffffll) return RP_ESHAPE;
+  dim3 grid((unsigned)ctas, 1, batch);
   kern<<<grid, kGemmThreads, smem, st>>>(tmA, tmB, p);
   RP_LAUNCH_CHECK();
   return RP_OK;
 }
 
-
-// ------------------------------------------------------------------------------------------------------------------
-// Weight-stationary persistent variant for the tall-skinny projections of the body (M = tokens, N, K <= 256):
-// the CTA keeps its [BN x K] slice of the weight in shared memory, streams 128-row activation tiles through a TMA ring,
-// double-buffers the accumulator in TMEM and overlaps the epilogue of tile i with the loads + MMAs of tile i+1.
-// grid = (ctas_per_n_tile, n_tiles); CTA x handles M tiles x, x + gridDim.x, ...
-// ------------------------------------------------------------------------------------------------------------------
-static constexpr int kWsEpiWarps = 8;
-static constexpr int kWsThreads = 64 + kWsEpiWarps * 32;
-
-template <int BN, int KCH, bool B_MN, int NA>
-__global__ void __launch_bounds__(kWsThreads, 1)
-gemm_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  constexpr int A_STAGE = KCH * 128 * 128;          // [128 x K]
-  constexpr int B_BYTES = KCH * BN * 128;           // [BN x K]
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sB = smem;
-  uint8_t* sA = smem + B_BYTES;
-  __shared__ uint64_t bar_b, bar_full[NA], bar_empty[NA], bar_tfull[2], bar_tempty[2];
-  __shared__ uint32_t tmem_slot;
-  __shared__ __align__(16) float s_bias[BN];
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n0 = blockIdx.y * BN;
-  const int m_tiles = (p.M + 127) / 128;
-
-  if (threadIdx.x == 0) {
-    mbar_init(&bar_b, 1);
-    for (int i = 0; i < NA; ++i) {
-      mbar_init(&bar_full[i], 1);
-      mbar_init(&bar_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bar_tfull[i], 1);
-      mbar_init(&bar_tempty[i], kWsEpiWarps);
-    }
-    fence_barrier_init();
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1) tmem_alloc(&tmem_slot, 2 * BN);
-  if (p.bias != nullptr && threadIdx.x >= 64)
-    for (int i = threadIdx.x - 64; i < BN; i += kWsEpiWarps * 32) s_bias[i] = (n0 + i < p.N) ? p.bias[n0 + i] : 0.f;
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-
-  if (warp == 0) {
-    if (elect_one()) {
-      mbar_arrive_expect_tx(&bar_b, B_BYTES);
-      for (int kc = 0; kc < KCH; ++kc) {
-        if (B_MN) {
-#pragma unroll
-          for (int c = 0; c < BN / 64; ++c)
-            tma_load_2d(sB + kc * (BN * 128) + c * 8192, &tmB, &bar_b, p.b_c0 + n0 + c * 64, p.b_r0 + kc * 64);
-        } else {
-          tma_load_2d(sB + kc * (BN * 128), &tmB, &bar_b, p.b_c0 + kc * 64, p.b_r0 + n0);
-        }
-      }
-      int it = 0;
-      for (int mt = blockIdx.x; mt < m_tiles; mt += gridDim.x, ++it) {
-        const uint32_t s = it % NA, ph = (it / NA) & 1;
-        mbar_wait(&bar_empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&bar_full[s], A_STAGE);
-        for (int kc = 0; kc < KCH; ++kc)
-          tma_load_2d(sA + s * A_STAGE + kc * 16384, &tmA, &bar_full[s], p.a_c0 + kc * 64, p.a_r0 + mt * 128);
-      }
-    }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128, BN, false, B_MN);
-      mbar_wait(&bar_b, 0);
-      int it = 0;
-      for (int mt = blockIdx.x; mt < m_tiles; mt += gridDim.x, ++it) {
-        const uint32_t s = it % NA, ph = (it / NA) & 1, as = it & 1, aph = (it >> 1) & 1;
-        mbar_wait(&bar_tempty[as], aph ^ 1);
-        mbar_wait(&bar_full[s], ph);
-        tc_fence_after();
-        const uint32_t a0 = smem_u32(sA + s * A_STAGE), b0 = smem_u32(sB);
-#pragma unroll
-        for (int kc = 0; kc < KCH; ++kc)
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t ad = umma_desc_sw128(a0 + kc * 16384 + ks * 32, 16, 1024);
-            const uint64_t bd = B_MN ? umma_desc_sw128(b0 + kc * (BN * 128) + ks * 2048, 8192, 1024)
-                                     : umma_desc_sw128(b0 + kc * (BN * 128) + ks * 32, 16, 1024);
-            umma_ss(tmem + as * BN, ad, bd, idesc, (kc | ks) != 0);
-          }
-        umma_commit(&bar_empty[s]);
-        umma_commit(&bar_tfull[as]);
-      }
-    }
-  } else {
-    // ------------------------------------------------ epilogue: 8 warps, warp%4 = lane quarter, (warp-2)/4 = column half
-    const int ew = warp - 2, quarter = warp & 3, half = ew >> 2;
-    const int row = quarter * 32 + lane;
-    constexpr int HALF = BN / 2;
-    EpiRow er;
-    er.keep_scale = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
-    er.drop_thr = p.drop_p > 0.f ? (uint32_t)(p.drop_p * 4294967296.0) : 0u;
-    er.seed_eff = p.seed + ((p.drop_p > 0.f && p.seed_ptr) ? *p.seed_ptr : 0ull);
-    int it = 0;
-    for (int mt = blockIdx.x; mt < m_tiles; mt += gridDim.x, ++it) {
-      const uint32_t as = it & 1, aph = (it >> 1) & 1;
-      const int m = mt * 128 + row;
-      const bool row_ok = m < p.M;
-      er.c_base = p.c_off0 + (long long)m * p.ldc;
-      er.drop_row = m;
-      er.rm = 1.f;
-      er.exp_off = 0.f;
-      if (p.rowmask && row_ok) er.rm = p.rowmask[p.rowmask_off0 + m] ? 1.f : 0.f;
-      mbar_wait(&bar_tfull[as], aph);
-      tc_fence_after();
-      const uint32_t tbase = tmem + ((uint32_t)(quarter * 32) << 16) + as * BN + half * HALF;
-      if (HALF == 128) {   // BN = 256 (both halves of a fused K | V projection in one pass over the activations)
-        uint32_t r0[32], r1[32];
-        tmem_ld32(tbase, r0);
-        tmem_ld32(tbase + 32, r1);
-        tmem_ld_wait();
-        if (row_ok && n0 + half * HALF < p.N) gemm_epilogue_chunk(p, s_bias, er, r0, n0, half * HALF);
-        if (row_ok && n0 + half * HALF + 32 < p.N) gemm_epilogue_chunk(p, s_bias, er, r1, n0, half * HALF + 32);
-        tmem_ld32(tbase + 64, r0);
-        tmem_ld32(tbase + 96, r1);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_tempty[as]);
-        if (row_ok && n0 + half * HALF + 64 < p.N) gemm_epilogue_chunk(p, s_bias, er, r0, n0, half * HALF + 64);
-        if (row_ok && n0 + half * HALF + 96 < p.N) gemm_epilogue_chunk(p, s_bias, er, r1, n0, half * HALF + 96);
-      } else if (HALF == 64) {
-        uint32_t r0[32], r1[32];
-        tmem_ld32(tbase, r0);
-        tmem_ld32(tbase + 32, r1);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_tempty[as]);  // accumulator stage is free once its values sit in registers
-        if (row_ok && n0 + half * HALF < p.N) gemm_epilogue_chunk(p, s_bias, er, r0, n0, half * HALF);
-        if (row_ok && n0 + half * HALF + 32 < p.N) gemm_epilogue_chunk(p, s_bias, er, r1, n0, half * HALF + 32);
-      } else {
-        uint32_t r0[32];
-        tmem_ld32(tbase, r0);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar_tempty[as]);
-        if (row_ok && n0 + half * HALF < p.N) gemm_epilogue_chunk(p, s_bias, er, r0, n0, half * HALF);
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 2 * BN);
-}
-
-template <int BN, int KCH, bool B_MN>
-static int launch_gemm_ws(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
-  constexpr int NA = 2;  // B + 2 A stages: <= 96 KB for K <= 128 so that two CTAs share an SM
-  const int smem = KCH * BN * 128 + NA * KCH * 128 * 128 + 1024;
-  auto kern = gemm_ws_kernel<BN, KCH, B_MN, NA>;
-  RP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  const int n_tiles = (p.N + BN - 1) / BN, m_tiles = (p.M + 127) / 128;
-  int per_n = ((KCH <= 2 && BN <= 128) ? 2 : 1) * sm_count() / n_tiles;
-  if (per_n < 1) per_n = 1;
-  if (per_n > m_tiles) per_n = m_tiles;
-  dim3 grid(per_n, n_tiles);
-  kern<<<grid, kWsThreads, smem, st>>>(tmA, tmB, p);
-  RP_LAUNCH_CHECK();
-  return RP_OK;
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Persistent streaming variant for mid-size and large single GEMMs (BERT4Rec's d -> 4d FFN, the d = 512 CE backward,
-// predict-sized projections): one CTA per SM walks 128 x 128 output tiles (n fastest, so that CTAs running side by side
-// share the A rows in L2); A and B k-chunks stream through an NSTAGE-deep TMA ring; FOUR accumulator stages in TMEM
-// (4 x 128 = 512 columns) let the 8 epilogue warps trail the tensor core by up to three tiles, so short-K tiles with heavy
-// epilogues (bias + GELU + dropout) and long-K tiles both keep the MMA pipe fed.  batch == 1, split_k == 1.
-// ------------------------------------------------------------------------------------------------------------------
-static constexpr int kPsEpiWarps = 8;
-static constexpr int kPsThreads = 64 + kPsEpiWarps * 32;
-
-// BN = 128: four accumulator stages; BN = 256 (wide outputs): two stages, and an M=128 x N=256 MMA reads 12 KB of shared
-// memory per 128 tensor-core cycles instead of 8 KB per 64, i.e. it is no longer shared-memory-bandwidth bound.
-template <int BN, bool A_MN, bool B_MN, int NSTAGE>
-__global__ void __launch_bounds__(kPsThreads, 1)
-gemm_ps_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  constexpr int kPsAcc = 512 / BN;
-  constexpr int A_BYTES = 128 * 128, B_BYTES = BN * 128, STAGE = A_BYTES + B_BYTES;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  __shared__ uint64_t bar_full[NSTAGE], bar_empty[NSTAGE], bar_tfull[kPsAcc], bar_tempty[kPsAcc];
-  __shared__ uint32_t tmem_slot;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int m_eff = p.M, k_eff = p.K;
-  if (p.m_limit_dev != nullptr) m_eff = max(0, min(p.M, *p.m_limit_dev - p.m_limit_base));
-  if (p.k_limit_dev != nullptr) k_eff = max(0, min(p.K, *p.k_limit_dev - p.k_limit_base));
-  const int m_tiles = (m_eff + 127) / 128, n_tiles = (p.N + BN - 1) / BN;
-  const int k_chunks = (k_eff + 63) / 64;
-  const long long total = (long long)m_tiles * n_tiles;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < NSTAGE; ++i) {
-      mbar_init(&bar_full[i], 1);
-      mbar_init(&bar_empty[i], 1);
-    }
-    for (int i = 0; i < kPsAcc; ++i) {
-      mbar_init(&bar_tfull[i], 1);
-      mbar_init(&bar_tempty[i], kPsEpiWarps);
-    }
-    fence_barrier_init();
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-  }
-  if (warp == 1) tmem_alloc(&tmem_slot, kPsAcc * BN);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-
-  if (warp == 0) {
-    if (elect_one()) {
-      uint32_t it = 0;
-      for (long long t = blockIdx.x; t < total; t += gridDim.x) {
-        const int m0 = (int)(t / n_tiles) * 128, n0 = (int)(t % n_tiles) * BN;
-        for (int kc = 0; kc < k_chunks; ++kc, ++it) {
-          const uint32_t s = it % NSTAGE, ph = (it / NSTAGE) & 1;
-          mbar_wait(&bar_empty[s], ph ^ 1);
-          mbar_arrive_expect_tx(&bar_full[s], STAGE);
-          uint8_t* sa = smem + s * STAGE;
-          uint8_t* sb = sa + A_BYTES;
-          if (A_MN) {
-            tma_load_2d(sa, &tmA, &bar_full[s], p.a_c0 + m0, p.a_r0 + kc * 64);
-            tma_load_2d(sa + 8192, &tmA, &bar_full[s], p.a_c0 + m0 + 64, p.a_r0 + kc * 64);
-          } else {
-            tma_load_2d(sa, &tmA, &bar_full[s], p.a_c0 + kc * 64, p.a_r0 + m0);
-          }
-          if (B_MN) {
-#pragma unroll
-            for (int c = 0; c < BN / 64; ++c)
-              tma_load_2d(sb + c * 8192, &tmB, &bar_full[s], p.b_c0 + n0 + c * 64, p.b_r0 + kc * 64);
-          } else {
-            tma_load_2d(sb, &tmB, &bar_full[s], p.b_c0 + kc * 64, p.b_r0 + n0);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128, BN, A_MN, B_MN);
-      uint32_t it = 0, tile = 0;
-      for (long long t = blockIdx.x; t < total; t += gridDim.x, ++tile) {
-        const uint32_t as = tile % kPsAcc, aph = (tile / kPsAcc) & 1;
-        mbar_wait(&bar_tempty[as], aph ^ 1);
-        tc_fence_after();
-        for (int kc = 0; kc < k_chunks; ++kc, ++it) {
-          const uint32_t s = it % NSTAGE, ph = (it / NSTAGE) & 1;
-          mbar_wait(&bar_full[s], ph);
-          tc_fence_after();
-          const uint32_t a0 = smem_u32(smem + s * STAGE), b0 = a0 + A_BYTES;
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t ad = A_MN ? umma_desc_sw128(a0 + ks * 2048, 8192, 1024) : umma_desc_sw128(a0 + ks * 32, 16, 1024);
-            const uint64_t bd = B_MN ? umma_desc_sw128(b0 + ks * 2048, 8192, 1024) : umma_desc_sw128(b0 + ks * 32, 16, 1024);
-            umma_ss(tmem + as * BN, ad, bd, idesc, (kc | ks) != 0);
-          }
-          umma_commit(&bar_empty[s]);
-        }
-        umma_commit(&bar_tfull[as]);
-      }
-    }
-  } else {
-    // ------------------------------------------------ epilogue: 8 warps, warp%4 = lane quarter, (warp-2)/4 = column half
-    const int ew = warp - 2, quarter = warp & 3, half = ew >> 2;
-    const int row = quarter * 32 + lane;
-    constexpr int HALF = BN / 2;
-    EpiRow er;
-    er.keep_scale = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
-    er.drop_thr = p.drop_p > 0.f ? (uint32_t)(p.drop_p * 4294967296.0) : 0u;
-    er.seed_eff = p.seed + ((p.drop_p > 0.f && p.seed_ptr) ? *p.seed_ptr : 0ull);
-    uint32_t tile = 0;
-    for (long long t = blockIdx.x; t < total; t += gridDim.x, ++tile) {
-      const uint32_t as = tile % kPsAcc, aph = (tile / kPsAcc) & 1;
-      const int m = (int)(t / n_tiles) * 128 + row, n0 = (int)(t % n_tiles) * BN;
-      const bool row_ok = m < p.M;
-      er.c_base = p.c_off0 + (long long)m * p.ldc;
-      er.drop_row = m;
-      er.rm = 1.f;
-      if (p.rowmask && row_ok) er.rm = p.rowmask[p.rowmask_off0 + m] ? 1.f : 0.f;
-      er.exp_off = (p.act == 3 && row_ok) ? p.row_exp2_offset[m] : 0.f;
-      mbar_wait(&bar_tfull[as], aph);
-      tc_fence_after();
-      const uint32_t tbase = tmem + ((uint32_t)(quarter * 32) << 16) + as * BN + half * HALF;
-      const float* bias_n0 = p.bias ? p.bias + n0 : nullptr;  // N % 32 == 0 is required with a bias (launcher)
-#pragma unroll 1
-      for (int c0 = 0; c0 < HALF; c0 += 64) {  // 64 columns per round
-        uint32_t r0[32], r1[32];
-        tmem_ld32(tbase + c0, r0);
-        tmem_ld32(tbase + c0 + 32, r1);
-        tmem_ld_wait();
-        if (c0 + 64 == HALF) {  // accumulator stage is free once its last values sit in registers
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&bar_tempty[as]);
-        }
-        if (k_chunks == 0) {  // empty contraction (dynamic K limit): the accumulator was never written
-#pragma unroll
-          for (int q = 0; q < 32; ++q) r0[q] = r1[q] = 0u;
-        }
-        const int c = half * HALF + c0;
-        if (row_ok && n0 + c < p.N) gemm_epilogue_chunk(p, bias_n0, er, r0, n0, c);
-        if (row_ok && n0 + c + 32 < p.N) gemm_epilogue_chunk(p, bias_n0, er, r1, n0, c + 32);
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, kPsAcc * BN);
-}
-
-template <int BN, bool A_MN, bool B_MN>
-static int launch_gemm_ps(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t st) {
-  constexpr int NSTAGE = BN == 128 ? 6 : 4;
-  const int smem = NSTAGE * (128 * 128 + BN * 128) + 1024;
-  auto kern = gemm_ps_kernel<BN, A_MN, B_MN, NSTAGE>;
-  RP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  const long long tiles = (long long)((p.M + 127) / 128) * ((p.N + BN - 1) / BN);
-  const int grid = (int)(tiles < sm_count() ? tiles : sm_count());
-  kern<<<grid, kPsThreads, smem, st>>>(tmA, tmB, p);
-  RP_LAUNCH_CHECK();
-  return RP_OK;
-}
-
-// short-K problems (the body's d x d projections) use 2 stages so that 3 CTAs share an SM and their prologues,
+// short-K problems (the body's d x d projections) use 2 stages so that several CTAs share an SM and their prologues,
 // main loops and epilogues overlap; long-K problems (weight gradients) use a 4-deep ring.
 template <int BN, bool A_MN, bool B_MN>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int batch, cudaStream_t st) {
@@ -713,52 +377,6 @@ RP_API int rp_gemm(const rp_gemm_desc* g, void* stream_) {
   const int bn = (g->N <= 64) ? 64 : 128;
   if ((rc = make_tmap_bf16(&tmA, g->A, g->a_rows, g->a_cols, g->lda, g->a_mn ? 64 : 128)) != RP_OK) return rc;
   if ((rc = make_tmap_bf16(&tmB, g->B, g->b_rows, g->b_cols, g->ldb, g->b_mn ? 64 : bn)) != RP_OK) return rc;
-  // weight-stationary persistent kernel: activation [M, K] K-major, K in {64,128,256}, one batch, no split-K
-  static const int ws_min_m = getenv("RP_GEMM_WS_MIN_M") ? atoi(getenv("RP_GEMM_WS_MIN_M")) : 131072;  // measured: pays for M >~ 100K rows (predict), neutral at 51K
-  const bool ws_ok = g->act != 3 && g->out_mode != 4 && !g->m_limit_dev && !g->k_limit_dev && g->M >= ws_min_m && !g->a_mn && g->batch == 1 && g->split_k == 1 && g->M >= 1024 && g->N >= 64 &&
-                     (g->K == 64 || g->K == 128 || g->K == 256) && g->a_ro == 0 && g->a_ri == 0 && g->b_ro == 0 && g->b_ri == 0 &&
-                     g->a_co == 0 && g->a_ci == 0 && g->b_co == 0 && g->b_ci == 0 && g->c_oo == 0 && g->c_oi == 0;
-  if (ws_ok && bn == 128 && g->N == 256 && !g->b_mn && g->K <= 128 && !getenv("RP_GEMM_WS_NO_WIDE")) {
-    // both 128-column halves in one CTA: the activations are read once (two n-tiles each streamed the whole [M, K] matrix:
-    // 421 MB of DRAM reads for a 210 MB input in the predict body's K | V projection, ncu r2j)
-    if ((rc = make_tmap_bf16(&tmB, g->B, g->b_rows, g->b_cols, g->ldb, 256)) != RP_OK) return rc;
-    return g->K == 64 ? launch_gemm_ws<256, 1, false>(tmA, tmB, p, stream) : launch_gemm_ws<256, 2, false>(tmA, tmB, p, stream);
-  }
-  if (ws_ok && bn == 128) {
-#define RP_WS_CASE(KCH_)                                                             \
-  return g->b_mn ? launch_gemm_ws<128, KCH_, true>(tmA, tmB, p, stream) : launch_gemm_ws<128, KCH_, false>(tmA, tmB, p, stream)
-    if (g->K == 64) { RP_WS_CASE(1); }
-    if (g->K == 128) { RP_WS_CASE(2); }
-    RP_WS_CASE(4);
-#undef RP_WS_CASE
-  }
-  // persistent streaming kernel: single GEMMs with enough tiles for every SM and a contraction / width beyond the body's
-  // d x d projections (those are launch/latency-bound and stay on the tile kernel, which co-schedules 3 CTAs per SM)
-  static const long long ps_min_flop = getenv("RP_GEMM_PS_MIN_FLOP") ? atoll(getenv("RP_GEMM_PS_MIN_FLOP")) : 4000000000ll;
-  static const bool ps_small = getenv("RP_GEMM_PS_SMALL") && atoi(getenv("RP_GEMM_PS_SMALL")) != 0;  // experiment: d x d projections too
-  const long long tiles = (long long)((g->M + 127) / 128) * ((g->N + 127) / 128);
-  const bool ps_ok = g->batch == 1 && g->split_k == 1 && g->out_mode != 1 && g->out_mode != 3 && bn == 128 &&
-                     tiles >= sm_count() && 2ll * g->M * g->N * g->K >= ps_min_flop && (g->K > 128 || g->N > 128 || ps_small) &&
-                     (!g->bias || g->N % 32 == 0) && g->a_ro == 0 && g->a_ri == 0 && g->b_ro == 0 && g->b_ri == 0 &&
-                     g->a_co == 0 && g->a_ci == 0 && g->b_co == 0 && g->b_ci == 0 && g->c_oo == 0 && g->c_oi == 0 &&
-                     g->rowmask_oo == 0;
-  if (ps_ok) {
-    // wide outputs: 128 x 256 tiles when they still give every SM a tile
-    const bool wide = g->N >= 256 && (long long)((g->M + 127) / 128) * ((g->N + 255) / 256) >= sm_count();
-    if (wide && !g->b_mn) {  // K-major B: the TMA box grows to 256 rows
-      if ((rc = make_tmap_bf16(&tmB, g->B, g->b_rows, g->b_cols, g->ldb, 256)) != RP_OK) return rc;
-    }
-#define RP_PS_CASE(BN_)                                                                                  \
-  do {                                                                                                   \
-    if (!g->a_mn && !g->b_mn) return launch_gemm_ps<BN_, false, false>(tmA, tmB, p, stream);             \
-    if (!g->a_mn && g->b_mn) return launch_gemm_ps<BN_, false, true>(tmA, tmB, p, stream);               \
-    if (g->a_mn && !g->b_mn) return launch_gemm_ps<BN_, true, false>(tmA, tmB, p, stream);               \
-    return launch_gemm_ps<BN_, true, true>(tmA, tmB, p, stream);                                         \
-  } while (0)
-    if (wide) RP_PS_CASE(256);
-    RP_PS_CASE(128);
-#undef RP_PS_CASE
-  }
 #define RP_GEMM_CASE(BN_, AMN_, BMN_) return launch_gemm<BN_, AMN_, BMN_>(tmA, tmB, p, g->batch, stream)
   if (bn == 64) {
     if (!g->a_mn && !g->b_mn) RP_GEMM_CASE(64, false, false);

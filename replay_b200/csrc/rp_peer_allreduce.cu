@@ -3,7 +3,7 @@
 //
 // Replaces  the bucketed gradient all-reduce Lightning's DDP runs under `loss.backward()` for the reference
 //           (replay/nn/lightning/module.py:62-75 under Trainer(strategy="ddp"); SURVEY.md 2.1 / 8e)
-// and round 1's eager ncclAllReduce between two graph replays (launch gaps on both sides of it, 0.4 ms of a 4.1 ms step).
+// and an eager ncclAllReduce between two graph replays (launch gaps on both sides of it).
 //
 // Every rank holds the gradient in a buffer of the SAME symmetric allocation (torch.distributed._symmetric_memory does the
 // cuMem export / import - plumbing); the kernel gets the W peer pointers by value.  Two-shot scheme:

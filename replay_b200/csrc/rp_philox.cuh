@@ -36,10 +36,9 @@ __host__ __device__ __forceinline__ uint32_t fmix32(uint32_t h) {  // murmur3 fi
 }
 
 // Dropout draws.  The attention forward walks the [query, key] matrix by query rows, the fused backward by key rows, the
-// activation kernels by token rows - so the mask must be computable per element in any order - and it was the dominant
-// integer cost of those kernels (a murmur finaliser per attention probability kept the ALU pipe ~55 % busy; the previous
-// activation generator, 6 finalisers per 4 elements, was ~45 % of the instructions of the fused post-attention kernel; ncu
-// r2c).  The draw for element (row r, column j) of a site is
+// activation kernels by token rows - so the mask must be computable per element in any order - and it is a large integer
+// cost of those kernels (a full hash finaliser per element would dominate them): a row key and a column key are hashed
+// once each and mixed cheaply per element.  The draw for element (row r, column j) of a site is
 //   drop_mix(drop_row_key(seed, site offset, r), drop_col_key(j))
 // (attention probabilities: r = (batch*head)*Lp + query, j = key; activations [T, d]: r = token row, j = feature column)
 // with the two well-mixed 32-bit keys computed once per row / per key (shared-memory tables) and a two-multiply mix per

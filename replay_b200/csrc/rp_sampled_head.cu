@@ -14,7 +14,7 @@
 // bound: each (token, negative) pair reads one table row) whose backward scatters with fp32 atomics.
 #include "rp_host.h"
 #include "rp_gemm_desc.h"
-#include "rp_sm100.cuh"
+#include "rp_sm90.cuh"
 
 namespace rp {
 

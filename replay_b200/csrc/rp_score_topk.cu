@@ -7,13 +7,13 @@
 // without ever materialising the [B, |I|] logits.
 //
 // Kernel 1 (score_topk_kernel): one CTA = 128 users x a contiguous range of 128-item tiles.
-//   warp 0   TMA producer: user tile A (resident in smem) + ring of item-table K-chunks [128 items x 64]
-//   warp 1   tcgen05.mma issuer: S[128x128] fp32 in TMEM, double buffered (2 x 128 columns)
-//   warps 2-5 epilogue: tcgen05.ld 32 columns at a time, thread = user row, seen-mask via a cursor into the user's
-//            sorted seen list, running top-K (sorted, registers), partial top-K written per (user, item split)
+//   thread 0    TMA: user tile A (resident in smem) + ring of item-table K-chunks [128 items x 64]
+//   warpgroups  wgmma: S[128x128] fp32 in registers (warpgroup g: users [64 g, 64 g + 64)); each 64-column half of the
+//   0 and 1     tile goes through a shared-memory stage, then thread = (user row, 32-column part): seen-mask via a cursor
+//               into the user's sorted seen list, running top-K (sorted, registers), partial top-K per (user, split, part)
 // Kernel 2 (topk_merge_kernel): one warp per user merges the per-split partial lists (score desc, column asc).
 #include "rp_host.h"
-#include "rp_sm100.cuh"
+#include "rp_sm90.cuh"
 
 namespace rp {
 
@@ -61,15 +61,13 @@ __device__ __forceinline__ float key2f(uint32_t k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
-static constexpr int kEpiWarps = 16;   // lane quarter x 32-column part of the 128-column tile: 4 warps per SM sub-partition hide the
-                                       // tcgen05.ld / shared-memory / insert-chain latencies of each other (measured: the epilogue,
-                                       // not the MMA or the TMA feed, bounds this kernel)
-static constexpr int kColParts = kEpiWarps / 4;
-static constexpr int kAccMax = 4;    // accumulator stages in TMEM: 4 x 128 columns, or 3 when the user tile itself lives in TMEM
-static constexpr int kThreads = 64 + kEpiWarps * 32;
+static constexpr int kEpiThreads = 256;   // the two warpgroups
+static constexpr int kColParts = 2;       // 32-column parts of each 64-column half: one running top-K per (row, part)
+static constexpr int kThreads = kEpiThreads;
+static constexpr int kStagePitch = 64 + 4;
 
 // One 32-column chunk of one row (thread).  FAST PATH: the maxima of the four 8-column groups against the admission threshold -
-// the values are never modified or copied (they stay in the registers tcgen05.ld filled).  Seen / out-of-catalog columns are
+// the values are never modified or copied.  Seen / out-of-catalog columns are
 // NOT masked here: a masked column only matters if it would be admitted, and then the slow path drops it from the hit mask (a
 // spurious slow-path entry costs about what masking every chunk that holds a seen item would).  SLOW PATH (a group maximum
 // beats the threshold): stage that group's 8 values in shared memory so that ONE insert site serves a runtime column index,
@@ -96,14 +94,14 @@ __device__ __forceinline__ void score_chunk(const uint32_t (&raw)[32], uint32_t 
         uint32_t hit = 0;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          sc[i * (kEpiWarps * 32)] = __uint_as_float(raw[8 * k + i]);
+          sc[i * kEpiThreads] = __uint_as_float(raw[8 * k + i]);
           hit |= (__uint_as_float(raw[8 * k + i]) > thr) ? (1u << i) : 0u;
         }
         hit &= ~(kill >> (8 * k));
         while (hit) {
           const int i = __ffs(hit) - 1;
           hit &= hit - 1;
-          const float val = sc[i * (kEpiWarps * 32)];
+          const float val = sc[i * kEpiThreads];
           if (val > fmaxf(top.thr(), gthr)) top.insert(val, col0 + 8 * k + i);
         }
       }
@@ -119,162 +117,116 @@ __global__ void __launch_bounds__(kThreads, 1)
 score_topk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const int32_t* __restrict__ seen_sorted, int S, int n_users, int n_items, int K, int n_splits,
                   const float* __restrict__ bias, float* __restrict__ part_vals, int32_t* __restrict__ part_ids,
-                  uint32_t* __restrict__ row_thr /* [n_users] shared K-th-best keys, zero-filled */,
-                  const __nv_bfloat16* __restrict__ hq_rows /* the user matrix as a plain pointer (A_TMEM) */) {
+                  uint32_t* __restrict__ row_thr /* [n_users] shared K-th-best keys, zero-filled */) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;                          // KCH chunks of 16 KB
   uint8_t* sB = smem + KCH * kChunkBytes;      // NSTAGE chunks of 16 KB
-  // d = 128 / 256: the resident user tile Hq goes to TMEM (packed bf16, d/2 columns) and the MMA takes its A operand from
-  // there: 73 instead of 102 cycles per 128x128x16 MMA (profiles/r1_mma_probe.md); three accumulator stages remain
-  constexpr bool A_TMEM = (KCH == 2 || KCH == 4);
-  constexpr int kAcc = A_TMEM ? 3 : 4;
-  __shared__ uint64_t bar_a, bar_full[NSTAGE], bar_empty[NSTAGE], bar_tfull[kAccMax], bar_tempty[kAccMax];
-  __shared__ uint32_t tmem_slot;
-  __shared__ float s_scratch[8 * kEpiWarps * 32];  // [i][epilogue thread]: one 8-column group staged for the insert path
+  float* stage = reinterpret_cast<float*>(sB + NSTAGE * kChunkBytes);   // [128 x kStagePitch] fp32: one 64-column half
+  __shared__ uint64_t bar_a, bar_full[NSTAGE], bar_empty[NSTAGE];
+  __shared__ float s_scratch[8 * kEpiThreads];  // [i][thread]: one 8-column group staged for the insert path
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   const int user_tile = blockIdx.x / n_splits, split = blockIdx.x % n_splits;
   const int u0 = user_tile * kTileM;
   const int n_tiles_total = (n_items + kTileN - 1) / kTileN;
   const int t_begin = (int)(((long long)n_tiles_total * split) / n_splits);
   const int t_end = (int)(((long long)n_tiles_total * (split + 1)) / n_splits);
-  const int n_ct = t_end - t_begin;
 
   if (threadIdx.x == 0) {
-    mbar_init(&bar_a, A_TMEM ? kEpiWarps : 1);
+    mbar_init(&bar_a, 1);
     for (int i = 0; i < NSTAGE; ++i) {
       mbar_init(&bar_full[i], 1);
-      mbar_init(&bar_empty[i], 1);
-    }
-    for (int i = 0; i < kAcc; ++i) {
-      mbar_init(&bar_tfull[i], 1);
-      mbar_init(&bar_tempty[i], kEpiWarps);  // one arrive per epilogue warp
+      mbar_init(&bar_empty[i], 8);
     }
     fence_barrier_init();
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == 1) tmem_alloc(&tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-
-  if (warp == 0) {
-    // ------------------------------------------------ TMA producer
-    if (elect_one()) {
-      if (!A_TMEM) {
-        mbar_arrive_expect_tx(&bar_a, KCH * kChunkBytes);
-        for (int kc = 0; kc < KCH; ++kc) tma_load_2d(sA + kc * kChunkBytes, &tmA, &bar_a, kc * 64, u0);
-      }
-      uint32_t it = 0;
-      for (int t = t_begin; t < t_end; ++t) {
-        for (int kc = 0; kc < KCH; ++kc, ++it) {
-          const uint32_t s = it % NSTAGE, ph = (it / NSTAGE) & 1;
-          mbar_wait(&bar_empty[s], ph ^ 1);
-          mbar_arrive_expect_tx(&bar_full[s], kChunkBytes);
-          tma_load_2d(sB + s * kChunkBytes, &tmB, &bar_full[s], kc * 64, t * kTileN);
-        }
-      }
+  // the ring of item-table chunks is fed by thread 0: chunk i -> stage i % NSTAGE once the 8 warps released its previous use
+  const int n_chunks = (t_end - t_begin) * KCH;
+  auto issue = [&](int i) {
+    const uint32_t s = i % NSTAGE;
+    mbar_wait(&bar_empty[s], ((i / NSTAGE) & 1) ^ 1);
+    mbar_arrive_expect_tx(&bar_full[s], kChunkBytes);
+    tma_load_2d(sB + s * kChunkBytes, &tmB, &bar_full[s], (i % KCH) * 64, (t_begin + i / KCH) * kTileN);
+  };
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(&bar_a, KCH * kChunkBytes);
+    for (int kc = 0; kc < KCH; ++kc) tma_load_2d(sA + kc * kChunkBytes, &tmA, &bar_a, kc * 64, u0);
+    for (int i = 0; i < NSTAGE && i < n_chunks; ++i) issue(i);
+  }
+  const int wg = threadIdx.x >> 7, ft = threadIdx.x & 127;
+  const int fr = frag_row(ft), fc = frag_col(ft);
+  // row-wise part: thread = (user row, 32-column part of the staged half)
+  const int row = ft, part = wg;
+  const int u = u0 + row;
+  const bool live = u < n_users;
+  float* sc = s_scratch + threadIdx.x;  // element q of this thread at sc[q * kEpiThreads]
+  TopK<KMAX> top;
+  top.init(K);
+  // cursor into this user's sorted seen list (ascending, kNoId = padding).  The next entry is prefetched one step ahead
+  // so that the (rare, per thread) advance never waits on a dependent global load inside the tile loop.
+  const int32_t* sp = seen_sorted ? seen_sorted + (size_t)(live ? u : 0) * S : nullptr;
+  int ci = 0;
+  int next_seen = kNoId, pre_seen = kNoId;
+  if (sp && live) {
+    const int first_col = t_begin * kTileN;
+    int lo = 0, hi = S;  // lower_bound(first_col), once per CTA
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (sp[mid] < first_col) lo = mid + 1; else hi = mid;
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------ MMA issuer
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(kTileM, kTileN);
-      mbar_wait(&bar_a, 0);
-      tc_fence_after();
-      uint32_t it = 0;
-      for (int j = 0; j < n_ct; ++j) {
-        const uint32_t as = j % kAcc, aph = (j / kAcc) & 1;
-        mbar_wait(&bar_tempty[as], aph ^ 1);
-        tc_fence_after();
-        const uint32_t dcol = tmem + as * kTileN;
-        for (int kc = 0; kc < KCH; ++kc, ++it) {
-          const uint32_t s = it % NSTAGE, ph = (it / NSTAGE) & 1;
-          mbar_wait(&bar_full[s], ph);
-          tc_fence_after();
-          const uint32_t a0 = smem_u32(sA + kc * kChunkBytes), b0 = smem_u32(sB + s * kChunkBytes);
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            if (A_TMEM)
-              umma_ts(dcol, tmem + kAcc * kTileN + kc * 32 + ks * 8, umma_desc_sw128(b0 + ks * 32, 16, 1024), idesc, (kc | ks) != 0);
-            else
-              umma_ss(dcol, umma_desc_sw128(a0 + ks * 32, 16, 1024), umma_desc_sw128(b0 + ks * 32, 16, 1024), idesc,
-                      (kc | ks) != 0);
-          }
-          umma_commit(&bar_empty[s]);
-        }
-        umma_commit(&bar_tfull[as]);
-      }
+    ci = lo;
+    next_seen = ci < S ? sp[ci] : kNoId;
+    pre_seen = ci + 1 < S ? sp[ci + 1] : kNoId;
+  }
+  // K-th best already secured for this row by ANY thread / CTA working on it (other column parts and item splits):
+  // anything strictly below it cannot reach the final top-K, so it never enters the insert path.  The shared value is
+  // read one tile AHEAD (a stale threshold is only weaker, never wrong), so its L2 round trip is off the per-tile path.
+  uint32_t gk = live ? *reinterpret_cast<volatile uint32_t*>(row_thr + u) : 0u;
+  float gthr = -INFINITY;
+  mbar_wait(&bar_a, 0);
+  uint32_t it = 0;
+  for (int t = t_begin, j = 0; t < t_end; ++t, ++j) {
+    if ((j & 3) == 0) {  // refresh every 4th tile: the shared threshold moves slowly once the lists are full
+      gthr = gk != 0u ? key2f(gk - 1u) : -INFINITY;  // largest value strictly below the shared K-th best
+      if (live) gk = *reinterpret_cast<volatile uint32_t*>(row_thr + u);  // lands long before its use 4 tiles later
     }
-  } else {
-    // ------------------------------------------------ epilogue: 16 warps; warp%4 = TMEM lane quarter, (warp-2)/4 = 32-column part
-    const int ew = warp - 2, quarter = warp & 3, part = ew >> 2;
-    const int row = quarter * 32 + lane;
-    const int u = u0 + row;
-    const bool live = u < n_users;
-    float* sc = s_scratch + ew * 32 + lane;  // element q of this thread at sc[q * (kEpiWarps*32)]
-    if (A_TMEM) {
-      // thread (row, part) copies K elements [part*D/4, (part+1)*D/4) of its user row from global memory into TMEM
-      constexpr int D = KCH * 64, WORDS = D / 8;   // 32-bit words (bf16 pairs) per thread
-      const uint4* src = reinterpret_cast<const uint4*>(hq_rows + (size_t)(live ? u : 0) * D + part * (D / 4));
+    float acc[kTileN / 2];
+    for (int kc = 0; kc < KCH; ++kc, ++it) {
+      const uint32_t s = it % NSTAGE, ph = (it / NSTAGE) & 1;
+      mbar_wait(&bar_full[s], ph);
+      const uint32_t a0 = smem_u32(sA + kc * kChunkBytes) + wg * 8192, b0 = smem_u32(sB + s * kChunkBytes);
+      wg_fence();
 #pragma unroll
-      for (int c = 0; c < WORDS; c += 16) {
-        uint32_t v[16];
-#pragma unroll
-        for (int q = 0; q < 16; q += 4) {
-          const uint4 t4 = live ? __ldg(src + ((c + q) >> 2)) : make_uint4(0u, 0u, 0u, 0u);
-          v[q] = t4.x; v[q + 1] = t4.y; v[q + 2] = t4.z; v[q + 3] = t4.w;
-        }
-        tmem_st16(tmem + ((uint32_t)(quarter * 32) << 16) + kAcc * kTileN + part * WORDS + c, v);
-      }
-      tmem_st_wait();
-      tc_fence_before();
+      for (int ks = 0; ks < 4; ++ks)
+        WgmmaSS<kTileN>::template run<0, 0>(acc, desc_k(a0 + ks * 32), desc_k(b0 + ks * 32), (kc | ks) != 0);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(acc);
       __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_a);
+      if (lane == 0) mbar_arrive(&bar_empty[s]);
+      if (threadIdx.x == 0 && (int)it + NSTAGE < n_chunks) issue((int)it + NSTAGE);
     }
-    TopK<KMAX> top;
-    top.init(K);
-    // cursor into this user's sorted seen list (ascending, kNoId = padding).  The next entry is prefetched one step ahead
-    // so that the (rare, per thread) advance never waits on a dependent global load inside the tile loop.
-    const int32_t* sp = seen_sorted ? seen_sorted + (size_t)(live ? u : 0) * S : nullptr;
-    int ci = 0;
-    int next_seen = kNoId, pre_seen = kNoId;
-    if (sp && live) {
-      const int first_col = t_begin * kTileN;
-      int lo = 0, hi = S;  // lower_bound(first_col), once per CTA
-      while (lo < hi) {
-        const int mid = (lo + hi) >> 1;
-        if (sp[mid] < first_col) lo = mid + 1; else hi = mid;
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      named_bar_sync(1, kEpiThreads);   // the stage's previous readers are done
+      {
+        const int r = 64 * wg + fr;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+          const int jj = 8 * half + q;
+          *reinterpret_cast<float2*>(stage + r * kStagePitch + 8 * q + fc) = make_float2(acc[4 * jj], acc[4 * jj + 1]);
+          *reinterpret_cast<float2*>(stage + (r + 8) * kStagePitch + 8 * q + fc) = make_float2(acc[4 * jj + 2], acc[4 * jj + 3]);
+        }
       }
-      ci = lo;
-      next_seen = ci < S ? sp[ci] : kNoId;
-      pre_seen = ci + 1 < S ? sp[ci + 1] : kNoId;
-    }
-    // K-th best already secured for this row by ANY thread / CTA working on it (other column halves and item splits):
-    // anything strictly below it cannot reach the final top-K, so it never enters the insert path.  The shared value is
-    // read one tile AHEAD (a stale threshold is only weaker, never wrong), so its L2 round trip is off the per-tile path.
-    uint32_t gk = live ? *reinterpret_cast<volatile uint32_t*>(row_thr + u) : 0u;
-    float gthr = -INFINITY;
-    for (int t = t_begin, j = 0; t < t_end; ++t, ++j) {
-      const uint32_t as = j % kAcc, aph = (j / kAcc) & 1;
-      if ((j & 3) == 0) {  // refresh every 4th tile: the shared threshold moves slowly once the lists are full
-        gthr = gk != 0u ? key2f(gk - 1u) : -INFINITY;  // largest value strictly below the shared K-th best
-        if (live) gk = *reinterpret_cast<volatile uint32_t*>(row_thr + u);  // lands long before its use 4 tiles later
-      }
-      mbar_wait(&bar_tfull[as], aph);
-      tc_fence_after();
-      const uint32_t tbase = tmem + ((uint32_t)(quarter * 32) << 16) + as * kTileN + part * 32;
+      named_bar_sync(1, kEpiThreads);
       uint32_t raw[32];
-      tmem_ld32(tbase, raw);
-      tmem_ld_wait();
-      // the accumulator stage can be reused as soon as its values sit in registers
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_tempty[as]);
-      const int col0 = t * kTileN + part * 32;
-      // seen items of this 32-column chunk as a bit mask (also skips entries that belong to the other column parts);
+      stage_ld32(stage + row * kStagePitch + part * 32, raw);
+      const int col0 = t * kTileN + half * 64 + part * 32;
+      // seen items of this 32-column chunk as a bit mask (also skips entries that belong to the other column part);
       // columns beyond the catalog (ragged last tile) are "seen" too
       uint32_t kill = 0;
       while (next_seen < col0 + 32) {
@@ -288,32 +240,28 @@ score_topk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (bias == nullptr) {
         score_chunk(raw, kill, thr, gthr, col0, top, sc, live, row_thr + u);
       } else {  // biased head (BERT4Rec): warp-uniform 16-byte loads, bias padded to a multiple of 128 entries
-        uint32_t xb[32];
 #pragma unroll
         for (int q = 0; q < 32; q += 4) {
           const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + col0 + q));
-          xb[q] = __float_as_uint(__uint_as_float(raw[q]) + b4.x);
-          xb[q + 1] = __float_as_uint(__uint_as_float(raw[q + 1]) + b4.y);
-          xb[q + 2] = __float_as_uint(__uint_as_float(raw[q + 2]) + b4.z);
-          xb[q + 3] = __float_as_uint(__uint_as_float(raw[q + 3]) + b4.w);
+          raw[q] = __float_as_uint(__uint_as_float(raw[q]) + b4.x);
+          raw[q + 1] = __float_as_uint(__uint_as_float(raw[q + 1]) + b4.y);
+          raw[q + 2] = __float_as_uint(__uint_as_float(raw[q + 2]) + b4.z);
+          raw[q + 3] = __float_as_uint(__uint_as_float(raw[q + 3]) + b4.w);
         }
-        score_chunk(xb, kill, thr, gthr, col0, top, sc, live, row_thr + u);
+        score_chunk(raw, kill, thr, gthr, col0, top, sc, live, row_thr + u);
       }
     }
-    if (live) {
-      float* pv = part_vals + (((size_t)u * n_splits + split) * kColParts + part) * K;
-      int32_t* pi = part_ids + (((size_t)u * n_splits + split) * kColParts + part) * K;
-#pragma unroll
-      for (int i = 0; i < KMAX; ++i)
-        if (i >= KMAX - K) {
-          pv[i - (KMAX - K)] = top.v[i];
-          pi[i - (KMAX - K)] = top.id[i];
-        }
-    }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 512);
+  if (live) {
+    float* pv = part_vals + (((size_t)u * n_splits + split) * kColParts + part) * K;
+    int32_t* pi = part_ids + (((size_t)u * n_splits + split) * kColParts + part) * K;
+#pragma unroll
+    for (int i = 0; i < KMAX; ++i)
+      if (i >= KMAX - K) {
+        pv[i - (KMAX - K)] = top.v[i];
+        pi[i - (KMAX - K)] = top.id[i];
+      }
+  }
 }
 
 // one warp per user: merge n_splits sorted partial lists -> final top-K; ties: smaller column first.
@@ -439,21 +387,21 @@ static int choose_splits(int n_user_tiles, int n_item_tiles) {
 template <int KCH, int NSTAGE>
 static int launch_score_topk(const CUtensorMap& tmA, const CUtensorMap& tmB, const int32_t* seen_sorted, int S, int B,
                              int I, int K, int n_splits, const float* bias, float* pv, int32_t* pi, uint32_t* row_thr,
-                             const __nv_bfloat16* hq_rows, cudaStream_t stream) {
-  const int smem = (KCH + NSTAGE) * kChunkBytes + 1024;
+                             cudaStream_t stream) {
+  const int smem = (KCH + NSTAGE) * kChunkBytes + 128 * kStagePitch * 4 + 1024;
   const int grid = ((B + kTileM - 1) / kTileM) * n_splits;
   if (K <= 10) {
     auto kern = score_topk_kernel<KCH, NSTAGE, 10>;
     RP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    kern<<<grid, kThreads, smem, stream>>>(tmA, tmB, seen_sorted, S, B, I, K, n_splits, bias, pv, pi, row_thr, hq_rows);
+    kern<<<grid, kThreads, smem, stream>>>(tmA, tmB, seen_sorted, S, B, I, K, n_splits, bias, pv, pi, row_thr);
   } else if (K <= 16) {
     auto kern = score_topk_kernel<KCH, NSTAGE, 16>;
     RP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    kern<<<grid, kThreads, smem, stream>>>(tmA, tmB, seen_sorted, S, B, I, K, n_splits, bias, pv, pi, row_thr, hq_rows);
+    kern<<<grid, kThreads, smem, stream>>>(tmA, tmB, seen_sorted, S, B, I, K, n_splits, bias, pv, pi, row_thr);
   } else {
     auto kern = score_topk_kernel<KCH, NSTAGE, 32>;
     RP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    kern<<<grid, kThreads, smem, stream>>>(tmA, tmB, seen_sorted, S, B, I, K, n_splits, bias, pv, pi, row_thr, hq_rows);
+    kern<<<grid, kThreads, smem, stream>>>(tmA, tmB, seen_sorted, S, B, I, K, n_splits, bias, pv, pi, row_thr);
   }
   RP_LAUNCH_CHECK();
   return RP_OK;
@@ -504,14 +452,10 @@ RP_API int rp_score_topk(const void* hq, const void* table, const float* bias, c
   if ((rc = make_tmap_bf16(&tmA, hq, n_users, d, d, 128)) != RP_OK) return rc;
   if ((rc = make_tmap_bf16(&tmB, table, n_items, d, d, 128)) != RP_OK) return rc;
   switch (d) {
-    case 64: rc = launch_score_topk<1, 8>(tmA, tmB, seen_sorted, S, n_users, n_items, K, p, bias, pv, pi, row_thr,
-                                            reinterpret_cast<const __nv_bfloat16*>(hq), stream); break;
-    case 128: rc = launch_score_topk<2, 8>(tmA, tmB, seen_sorted, S, n_users, n_items, K, p, bias, pv, pi, row_thr,
-                                            reinterpret_cast<const __nv_bfloat16*>(hq), stream); break;
-    case 256: rc = launch_score_topk<4, 6>(tmA, tmB, seen_sorted, S, n_users, n_items, K, p, bias, pv, pi, row_thr,
-                                            reinterpret_cast<const __nv_bfloat16*>(hq), stream); break;
-    default: rc = launch_score_topk<8, 3>(tmA, tmB, seen_sorted, S, n_users, n_items, K, p, bias, pv, pi, row_thr,
-                                            reinterpret_cast<const __nv_bfloat16*>(hq), stream); break;
+    case 64: rc = launch_score_topk<1, 8>(tmA, tmB, seen_sorted, S, n_users, n_items, K, p, bias, pv, pi, row_thr, stream); break;
+    case 128: rc = launch_score_topk<2, 8>(tmA, tmB, seen_sorted, S, n_users, n_items, K, p, bias, pv, pi, row_thr, stream); break;
+    case 256: rc = launch_score_topk<4, 6>(tmA, tmB, seen_sorted, S, n_users, n_items, K, p, bias, pv, pi, row_thr, stream); break;
+    default: rc = launch_score_topk<8, 3>(tmA, tmB, seen_sorted, S, n_users, n_items, K, p, bias, pv, pi, row_thr, stream); break;
   }
   if (rc != RP_OK) return rc;
   const int threads = 128;

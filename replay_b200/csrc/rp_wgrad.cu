@@ -8,7 +8,7 @@
 // that round 1 ran as 5-6 split-K GEMM launches + as many reduction launches + a column-sum launch per block.
 //
 // The contraction runs over the tokens, so both operands are read IN PLACE as MN-major tiles (rows = 64 tokens of the
-// row-major activation, TMA -> 128B-swizzled shared memory -> tcgen05).  Work unit = one 128 x BN tile of one dW and one
+// row-major activation, TMA -> 128B-swizzled shared memory -> wgmma).  Work unit = one 128 x BN tile of one dW and one
 // slab of the tokens; the grid is ~one CTA per SM (units x token splits).  The bias gradient rides on the tensor core too:
 // one extra N = 16 MMA per k-step against a resident tile of ones gives the column sums of the dY tile that is already in
 // shared memory (no extra pass over dY, no float atomics).  Every CTA stores its fp32 partial tile; `wgrad_reduce_kernel` adds
@@ -16,13 +16,13 @@
 #include <string.h>
 
 #include "rp_host.h"
-#include "rp_sm100.cuh"
+#include "rp_sm90.cuh"
 
 namespace rp {
 
 static constexpr int kWgMaxPairs = 8;
 static constexpr int kWgMaxUnits = 48;
-static constexpr int kWgThreads = 192;
+static constexpr int kWgThreads = 256;   // warpgroup g: output rows [64 g, 64 g + 64) of the tile; thread 0 feeds the ring
 static constexpr int kWgStages = 5;
 
 struct WgradParams {
@@ -41,12 +41,11 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_group_kernel(const __grid
   constexpr int STAGE = A_BYTES + B_BYTES;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sOnes = smem;                       // [64 x 64] bf16 ones (8 KB): B operand of the bias MMA
+  uint8_t* sOnes = smem;                       // bf16 ones (8 KB): K-major B operand [16 x 64] of the bias MMA
   uint8_t* sRing = smem + 8192;
-  __shared__ uint64_t bar_full[kWgStages], bar_empty[kWgStages], bar_acc;
-  __shared__ uint32_t tmem_slot;
+  __shared__ uint64_t bar_full[kWgStages], bar_empty[kWgStages];
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31;
   const int unit = blockIdx.x / p.splits, split = blockIdx.x % p.splits;
   const int pair = p.unit_pair[unit], m0 = p.unit_m0[unit], n0 = p.unit_n0[unit];
   const bool do_bias = (n0 == 0);              // exactly one column tile per dY row block carries the bias gradient
@@ -59,86 +58,68 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_group_kernel(const __grid
   if (threadIdx.x == 0) {
     for (int i = 0; i < kWgStages; ++i) {
       mbar_init(&bar_full[i], 1);
-      mbar_init(&bar_empty[i], 1);
+      mbar_init(&bar_empty[i], 8);
     }
-    mbar_init(&bar_acc, 1);
     fence_barrier_init();
     tma_prefetch_desc(tmA);
     tma_prefetch_desc(tmB);
   }
-  if (warp == 1) tmem_alloc(&tmem_slot, 256);  // accumulator BN (<= 128) columns + 16 for the bias column sums
   for (int i = threadIdx.x; i < 8192 / 4; i += kWgThreads) reinterpret_cast<uint32_t*>(sOnes)[i] = 0x3F803F80u;  // bf16 1.0 x 2
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t tmem_b = tmem + 128;
+  const int n_it = c_end - c_begin;
+  auto issue = [&](int it) {   // thread 0: token chunk c_begin + it -> stage it % kWgStages
+    const uint32_t s = it % kWgStages;
+    mbar_wait(&bar_empty[s], ((it / kWgStages) & 1) ^ 1);
+    mbar_arrive_expect_tx(&bar_full[s], STAGE);
+    uint8_t* sa = sRing + s * STAGE;
+    uint8_t* sb = sa + A_BYTES;
+    const int c = c_begin + it;
+    tma_load_2d(sa, tmA, &bar_full[s], m0, c * 64);
+    tma_load_2d(sa + 8192, tmA, &bar_full[s], m0 + 64, c * 64);
+#pragma unroll
+    for (int q = 0; q < BN / 64; ++q) tma_load_2d(sb + q * 8192, tmB, &bar_full[s], n0 + q * 64, c * 64);
+  };
+  if (threadIdx.x == 0)
+    for (int it = 0; it < kWgStages && it < n_it; ++it) issue(it);
 
-  if (warp == 0) {
-    if (elect_one()) {
-      for (int c = c_begin, it = 0; c < c_end; ++c, ++it) {
-        const uint32_t s = it % kWgStages, ph = (it / kWgStages) & 1;
-        mbar_wait(&bar_empty[s], ph ^ 1);
-        mbar_arrive_expect_tx(&bar_full[s], STAGE);
-        uint8_t* sa = sRing + s * STAGE;
-        uint8_t* sb = sa + A_BYTES;
-        tma_load_2d(sa, tmA, &bar_full[s], m0, c * 64);
-        tma_load_2d(sa + 8192, tmA, &bar_full[s], m0 + 64, c * 64);
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
+  float acc[BN / 2], accb[8];
+  acc_zero(acc);   // (more splits than token chunks: the partial is zero)
+  acc_zero(accb);
+  const uint32_t ones = smem_u32(sOnes);
+  for (int it = 0; it < n_it; ++it) {
+    const uint32_t s = it % kWgStages, ph = (it / kWgStages) & 1;
+    mbar_wait(&bar_full[s], ph);
+    const uint32_t a0 = smem_u32(sRing + s * STAGE) + wg * 8192, b0 = smem_u32(sRing + s * STAGE + A_BYTES);
+    wg_fence();
 #pragma unroll
-        for (int q = 0; q < BN / 64; ++q) tma_load_2d(sb + q * 8192, tmB, &bar_full[s], n0 + q * 64, c * 64);
-      }
+    for (int ks = 0; ks < 4; ++ks) {  // 16 tokens per k-step = 16 rows x 128 B of every [64 x 64] box
+      const uint64_t ad = desc_mn(a0 + ks * 2048, 8192);
+      WgmmaSS<BN>::template run<1, 1>(acc, ad, desc_mn(b0 + ks * 2048, 8192), 1);
+      if (do_bias) WgmmaSS<16>::template run<1, 0>(accb, ad, desc_k(ones + ks * 32), 1);
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128, BN, true, true);
-      constexpr uint32_t idesc_b = umma_idesc_bf16(128, 16, true, true);
-      const uint32_t ones = smem_u32(sOnes);
-      for (int c = c_begin, it = 0; c < c_end; ++c, ++it) {
-        const uint32_t s = it % kWgStages, ph = (it / kWgStages) & 1;
-        mbar_wait(&bar_full[s], ph);
-        tc_fence_after();
-        const uint32_t a0 = smem_u32(sRing + s * STAGE), b0 = a0 + A_BYTES;
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {  // 16 tokens per k-step = 16 rows x 128 B of every [64 x 64] box
-          const uint64_t ad = umma_desc_sw128(a0 + ks * 2048, 8192, 1024);
-          umma_ss(tmem, ad, umma_desc_sw128(b0 + ks * 2048, 8192, 1024), idesc, (it | ks) != 0);
-          if (do_bias) umma_ss(tmem_b, ad, umma_desc_sw128(ones + ks * 2048, 8192, 1024), idesc_b, (it | ks) != 0);
-        }
-        umma_commit(&bar_empty[s]);
-      }
-      umma_commit(&bar_acc);
-    }
-  } else {
-    // ------------------------------------------------ epilogue: thread = one output feature row of the dW tile
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    mbar_wait(&bar_acc, 0);
-    tc_fence_after();
-    const bool empty = c_begin >= c_end;  // (more splits than token chunks): the accumulator was never written
-    float* o = p.part + ((size_t)(unit * p.splits + split) * 128 + row) * BN;
-#pragma unroll 1
-    for (int c = 0; c < BN; c += 32) {
-      uint32_t raw[32];
-      tmem_ld32(tmem + ((uint32_t)(quarter * 32) << 16) + c, raw);
-      tmem_ld_wait();
-#pragma unroll
-      for (int q = 0; q < 32; q += 4)
-        *reinterpret_cast<float4*>(o + c + q) =
-            empty ? make_float4(0.f, 0.f, 0.f, 0.f)
-                  : make_float4(__uint_as_float(raw[q]), __uint_as_float(raw[q + 1]), __uint_as_float(raw[q + 2]),
-                                __uint_as_float(raw[q + 3]));
-    }
-    if (do_bias) {
-      uint32_t rb[16];
-      tmem_ld16(tmem_b + ((uint32_t)(quarter * 32) << 16), rb);
-      tmem_ld_wait();
-      p.part_b[(size_t)(unit * p.splits + split) * 128 + row] = empty ? 0.f : __uint_as_float(rb[0]);
-    }
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(acc);
+    wg_fence_acc(accb);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bar_empty[s]);
+    if (threadIdx.x == 0 && it + kWgStages < n_it) issue(it + kWgStages);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem, 256);
+  // ------------------------------------------------ partial tile: rows 64 wg + frag_row (+ 8), fp32
+  const int ra = 64 * wg + frag_row(t), fc = frag_col(t);
+  float* oa = p.part + ((size_t)(unit * p.splits + split) * 128 + ra) * BN;
+  float* ob = oa + 8 * BN;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    *reinterpret_cast<float2*>(oa + 8 * j + fc) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2*>(ob + 8 * j + fc) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+  }
+  if (do_bias && fc == 0) {   // every column of the ones product holds the row's sum
+    p.part_b[(size_t)(unit * p.splits + split) * 128 + ra] = accb[0];
+    p.part_b[(size_t)(unit * p.splits + split) * 128 + ra + 8] = accb[2];
+  }
 }
 
 struct WgradReduceParams {

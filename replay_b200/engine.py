@@ -1,5 +1,5 @@
-"""Execution engine of the SASRec hot path on B200: owns the flat parameter / gradient / optimizer buffers and the
-activation workspace, and sequences the hand-written sm_100a kernels (librp_b200.so, include/rp_b200.h) for
+"""Execution engine of the SASRec hot path on H100: owns the flat parameter / gradient / optimizer buffers and the
+activation workspace, and sequences the hand-written sm_90a kernels (librp_b200.so, include/rp_b200.h) for
 
     train step  = batch prep -> embedding -> N x [LN, QKV GEMMs, fused attention, out-proj, LN, FFN] -> final LN with
                   valid-target compaction -> fused CE head  -> full backward -> (gradient all-reduce) -> Adam
@@ -87,7 +87,7 @@ def _ru(x, m):
 
 
 class _CountingLib:
-    """Proxy over the ctypes library that counts the sm_100a kernel launches issued through it (bench.py reports them)."""
+    """Proxy over the ctypes library that counts the sm_90a kernel launches issued through it (bench.py reports them)."""
 
     KERNELS = {"rp_gemm": 1, "rp_attn_fwd": 1, "rp_attn_bwd": 1, "rp_attn_last": 1, "rp_attn_softmax_bwd": 1, "rp_prepare_batch": 2, "rp_embed_fwd": 1,
                "rp_embed_bwd": 2, "rp_layernorm_fwd": 1, "rp_layernorm_bwd": 1, "rp_dropout_bwd": 1, "rp_colsum": 1, "rp_colsum_multi": 1,
@@ -151,7 +151,7 @@ class SasRecEngine:
         self.rng_counter = torch.zeros(1, device=self.dev, dtype=torch.int64)
         self.seed = seed & 0xFFFFFFFFFFFF
         self.training = with_grad
-        # fused tcgen05 attention backward: head_dim 64, L <= 256; otherwise saved probabilities + batched GEMMs
+        # fused attention backward: head_dim 64, L <= 256; otherwise saved probabilities + batched GEMMs
         self.fused_attn_bwd = cfg.head_slot == 64 and seq_len <= 256
         self.sampled = None       # full-catalog CE unless set_loss() selects a sampled head
         self._loss_args = None
@@ -375,7 +375,7 @@ class SasRecEngine:
             self.s["dKV"] = torch.zeros(T, 2 * d, **bf)
             if not self.fused_attn_bwd:
                 self.s["dpd"] = torch.zeros(BH, self.Lp, self.Lp, **bf)
-            self.wg_ws = torch.zeros(148 * 4 * d * d, **f32)  # split-K partials of the weight-gradient GEMMs
+            self.wg_ws = torch.zeros(self.n_sm * 4 * d * d, **f32)  # split-K partials of the weight-gradient GEMMs
             self._wgrad_ws = None  # workspace of rp_wgrad_group, sized on first use
 
     def _stream(self):
@@ -437,6 +437,11 @@ class SasRecEngine:
         g.c_split_stride = c_split_stride
         check(self.lib.rp_gemm(ctypes.byref(g), self._stream()), "rp_gemm")
 
+    @property
+    def n_sm(self) -> int:
+        """Streaming multiprocessors of the engine's GPU (sizes the split-K waves of the weight gradients)."""
+        return torch.cuda.get_device_properties(self.dev).multi_processor_count
+
     def _wgrad(self, dY, X, dW, n_out, n_in):
         """dW[n_out, n_in] += dY[T, n_out]^T . X[T, n_in]: both operands read MN-major in place; split-K over about one wave
         of CTAs, each storing its fp32 partial tile (no atomics: 100+ CTAs hammering the same 16 K addresses serialise in
@@ -445,14 +450,14 @@ class SasRecEngine:
         chunks = (self.T + 63) // 64
         n = n_out * n_in
         per = int(os.environ.get("RP_WGRAD_CHUNKS", "8"))
-        split = max(1, min(chunks // per, (148 + tiles - 1) // tiles, self.wg_ws.numel() // n))
+        split = max(1, min(chunks // per, (self.n_sm + tiles - 1) // tiles, self.wg_ws.numel() // n))
         self._gemm(dY, X, self.wg_ws, n_out, n_in, self.T, a_mn=True, b_mn=True, out_mode=3, split_k=split,
                    c_geom=(n_in, 0, 0, 0), c_split_stride=n)
         check(self.lib.rp_reduce_splits(self.wg_ws.data_ptr(), split, n, n, dW.data_ptr(), 1, self._stream()), "rp_reduce_splits")
 
     def _wgrad_group(self, pairs):
         """[(dY bf16 [T, n_out], X bf16 [T, n_in], dW fp32 [n_out, n_in], db fp32 [n_out] | None), ...]: every weight and bias
-        gradient of a block in one tcgen05 launch + one deterministic reduction launch (csrc/rp_wgrad.cu).  Gradients are
+        gradient of a block in one wgmma launch + one deterministic reduction launch (csrc/rp_wgrad.cu).  Gradients are
         accumulated (+=) like the un-fused path does."""
         n = len(pairs)
         arr = (WgradPair * n)()
@@ -612,7 +617,7 @@ class SasRecEngine:
                 self._gemm(lb["q_in"], in_w[:d], lb["Q"], Bq, d, d, bias=in_b[:d])
                 if self.fused_pre_attn:
                     # [K | V] of ALL tokens through the fused pre-attention kernel in its K | V-only mode (activations read
-                    # once, TMA-store epilogue): 227 -> ~120 us per 4096-user call against the weight-stationary GEMM
+                    # once, both halves from one resident weight)
                     check(self.lib.rp_ln_qkv_fused(x.data_ptr(), None, None, 1e-8, in_w.data_ptr(), in_b.data_ptr(), T, d, None,
                                                    None, a["KV"].data_ptr(), None, None, hdv, self._stream()), "rp_ln_qkv_fused")
                 else:
@@ -662,7 +667,7 @@ class SasRecEngine:
             ad.drop_p, ad.seed, ad.drop_off, ad.seed_ptr = drop, self.seed, self._site(i, 0) << 40, self.rng_counter.data_ptr()
             check(self.lib.rp_attn_fwd(ctypes.byref(ad), self._stream()), "rp_attn_fwd")
             if not training and d <= 128 and self.fused_post_attn_eval:
-                # inference: out-projection + residual + LayerNorm + FFN in one pass over the tokens (csrc/rp_ffn.cu)
+                # inference: out-projection + residual + LayerNorm + FFN in one pass over the tokens (csrc/rp_block_fused.cu)
                 check(self.lib.rp_post_attn_fused(a["O"].data_ptr(), a["q_in"].data_ptr(), w("out_w").data_ptr(),
                                                   f("out_b").data_ptr(), f("ln2_w").data_ptr(), f("ln2_b").data_ptr(), 1e-8,
                                                   w("w1").data_ptr(), f("b1").data_ptr(), w("w2").data_ptr(), f("b2").data_ptr(),
@@ -683,7 +688,7 @@ class SasRecEngine:
             self._gemm(a["O"], w("out_w"), a["h"], T, d, d, bias=f("out_b"), residual=a["q_in"])
             self._ln_fwd(a["h"], f("ln2_w"), f("ln2_b"), 1e-8, a["y"], a["mean2"], a["rstd2"], T)
             if not training and d <= 128 and self.fused_ffn_eval:
-                # inference: both FFN GEMMs in one pass, the hidden activation never leaves the SM (csrc/rp_ffn.cu)
+                # inference: both FFN GEMMs in one pass, the hidden activation never leaves the SM (csrc/rp_block_fused.cu)
                 check(self.lib.rp_ffn_fused(a["y"].data_ptr(), w("w1").data_ptr(), f("b1").data_ptr(), w("w2").data_ptr(),
                                             f("b2").data_ptr(), pad.data_ptr() if legacy else None, T, d,
                                             self.x[i + 1].data_ptr(), self._stream()), "rp_ffn_fused")

@@ -1,4 +1,4 @@
-"""BERT4Rec on the B200 engine (replay/models/nn/sequential/bert4rec/model.py:10-527, lightning.py:332-351):
+"""BERT4Rec on the H100 engine (replay/models/nn/sequential/bert4rec/model.py:10-527, lightning.py:332-351):
 pre-LN transformer blocks with exact-erf GELU 4d FFN, a single <MASK> embedding, key-padding-only attention, no final
 LayerNorm, and an untied ``Linear(d, |I|)`` head with bias (default) or the tied item table + ``out_bias``.  The loss is the
 full-catalog CE over the positions that are real AND masked.  Same kernels as SASRec (rp_gemm / rp_attn_fwd / fused CE head),
@@ -33,7 +33,7 @@ class BertConfig:
         if self.d not in (64, 128, 256):
             raise ValueError("hidden size must be one of 64/128/256 for BERT4Rec (CE-backward tile constraint)")
         if self.d % self.n_heads or self.d // self.n_heads not in (64, 128):
-            raise ValueError("head_dim must be 64 or 128 (tcgen05 128B-swizzle tile constraint)")
+            raise ValueError("head_dim must be 64 or 128 (128B-swizzle tile constraint of the kernels)")
 
 
     # the shared engine code asks every config for its feature-slot geometry; BERT4Rec has no padded layout (head_dim 64 / 128)
@@ -199,7 +199,7 @@ class Bert4RecEngine(SasRecEngine):
             self.s["dQKV"] = torch.zeros(T, 3 * d, **bf)
             if not self.fused_attn_bwd:
                 self.s["dpd"] = torch.zeros(BH, self.Lp, self.Lp, **bf)
-            self.wg_ws = torch.zeros(148 * 4 * d * d, **f32)  # split-K partials of the weight-gradient GEMMs
+            self.wg_ws = torch.zeros(self.n_sm * 4 * d * d, **f32)  # split-K partials of the weight-gradient GEMMs
 
     # ------------------------------------------------------------------------------------------------ batch
     def set_batch(self, ids, pad_mask, token_mask, labels=None):

@@ -1,4 +1,4 @@
-"""Mirror of the legacy ``replay.models.nn.sequential.bert4rec`` modules on the B200 engine: ``Bert4RecModel``
+"""Mirror of the legacy ``replay.models.nn.sequential.bert4rec`` modules on the H100 engine: ``Bert4RecModel``
 (bert4rec/model.py:10-170) and the Lightning module ``Bert4Rec`` (bert4rec/lightning.py:15-683), plus the host-side
 input-layout helpers (uniform masker dataset.py:55-92, predict shift dataset.py:322-345)."""
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""Mirror of the legacy ``replay.models.nn.sequential.sasrec`` modules on the B200 engine:
+"""Mirror of the legacy ``replay.models.nn.sequential.sasrec`` modules on the H100 engine:
 ``SasRecModel`` (model.py:15-197) and the Lightning module ``SasRec`` (lightning.py:22-658).  Legacy semantics: causal mask
 only (pad keys are NOT masked), pad rows zeroed after the embedding and after every block, final LayerNorm eps 1e-8,
 sequence length must equal ``max_len`` (predict batches are left-padded up to it, lightning.py:624-658)."""
@@ -32,7 +32,7 @@ class SasRecModel(torch.nn.Module):
                  dropout: float = 0.2, ti_modification: bool = False, time_span: int = 256, device=None, seed: int = 0):
         super().__init__()
         if ti_modification:
-            raise NotImplementedError("TiSASRec is outside the B200 hot-path scope (SURVEY.md §2)")
+            raise NotImplementedError("TiSASRec is outside the hot-path scope (SURVEY.md §2)")
         name, card, pad, _ = item_feature_of(schema)
         self.schema = schema
         self.item_feature_name = name

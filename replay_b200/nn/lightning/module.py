@@ -13,7 +13,7 @@ class OptimizerFactory:
     def __init__(self, optimizer: str = "adam", learning_rate: float = 0.001, weight_decay: float = 0.0,
                  betas: tuple = (0.9, 0.98)):
         if optimizer != "adam" or weight_decay != 0.0:
-            raise NotImplementedError("the fused B200 path implements Adam without weight decay (the reference default)")
+            raise NotImplementedError("the fused path implements Adam without weight decay (the reference default)")
         self.learning_rate, self.betas = learning_rate, betas
 
     def create(self, parameters):

@@ -1,4 +1,4 @@
-"""Mirror of ``replay.nn.sequential.SasRec`` (replay/nn/sequential/sasrec/model.py:116-378) backed by the B200 engine.
+"""Mirror of ``replay.nn.sequential.SasRec`` (replay/nn/sequential/sasrec/model.py:116-378) backed by the H100 engine.
 
 Same construction (``from_params``), same ``forward`` signature and train / inference output contracts, same
 ``state_dict`` key names (SURVEY.md Appendix B); the computation is the fused CUDA path (``replay_b200.core``)."""

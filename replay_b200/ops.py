@@ -1,5 +1,5 @@
 """Tensor-level wrappers over the C ABI (include/rp_b200.h).  torch is used for device memory and streams only; every
-function launches hand-written sm_100a kernels from librp_b200.so on the current CUDA stream."""
+function launches hand-written sm_90a kernels from librp_b200.so on the current CUDA stream."""
 from __future__ import annotations
 
 import torch
@@ -22,11 +22,11 @@ def _need(t, dtype, name):
         raise ValueError(f"{name}: expected contiguous CUDA tensor of {dtype}, got {t.dtype} on {t.device}")
 
 
-def selftest_umma(mode: int, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+def selftest_mma(mode: int, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     _need(a, torch.bfloat16, "a")
     _need(b, torch.bfloat16, "b")
     d = torch.empty(128, 128, device=a.device, dtype=torch.float32)
-    check(lib().rp_selftest_umma(mode, _ptr(a), _ptr(b), _ptr(d), _stream()), "rp_selftest_umma")
+    check(lib().rp_selftest_mma(mode, _ptr(a), _ptr(b), _ptr(d), _stream()), "rp_selftest_mma")
     return d
 
 

@@ -18,9 +18,9 @@ class Trainer:
         self.engine = engine
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         self.use_graph = use_graph
-        # RP_DDP_ONE_GRAPH=1 (experimental, off): capture ncclAllReduce inside the step graph.  With torch 2.11 / NCCL 2.28 on
-        # the B200 boxes the capture hangs (also in "thread_local" capture-error mode, measured r2 on 2 GPUs), so the NCCL
-        # fallback keeps round 1's scheme: graph (forward + backward), eager all-reduce, graph (Adam).
+        # RP_DDP_ONE_GRAPH=1 (experimental, off): capture ncclAllReduce inside the step graph.  With torch 2.11 / NCCL 2.28 the
+        # capture has been seen to hang (also in "thread_local" capture-error mode), so the NCCL path runs graph (forward +
+        # backward), eager all-reduce, graph (Adam).
         self.one_graph = (os.environ.get("RP_DDP_ONE_GRAPH", "0") != "0") if one_graph is None else one_graph
         if self.world > 1 and dist.get_backend() != "nccl":
             self.one_graph = False   # gloo stages CUDA tensors through the host: not capturable

@@ -8,13 +8,10 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")
-# exercise the weight-stationary persistent GEMM on the small test shapes too (its production threshold is M >= 131072)
-os.environ.setdefault("RP_GEMM_WS_MIN_M", "1024")
-os.environ.setdefault("RP_GEMM_PS_MIN_FLOP", "50000000")  # route mid-size test GEMMs through the persistent streaming kernel
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90a) GPU")
 
 
 @pytest.fixture(scope="session")

@@ -179,7 +179,7 @@ def test_last_position_shortcut_equals_full_body(golden_dir, cuda, name, variant
 
 @pytest.mark.parametrize("dropout", [0.0, 0.2])
 def test_fused_attention_backward_matches_unfused(golden_dir, cuda, dropout):
-    """The fused tcgen05 attention backward and the un-fused path (batched GEMMs + softmax-backward kernel) share the forward
+    """The fused attention backward and the un-fused path (batched GEMMs + softmax-backward kernel) share the forward
     (same dropout masks): their parameter gradients must agree to bf16 round-off."""
     from oracle import sasrec as osr
     from replay_b200.engine import EncoderConfig, SasRecEngine

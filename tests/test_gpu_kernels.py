@@ -1,4 +1,4 @@
-"""GPU parity tests of the individual sm_100a kernels, called through the C ABI (ctypes), against the CPU oracle."""
+"""GPU parity tests of the individual sm_90a kernels, called through the C ABI (ctypes), against the CPU oracle."""
 import pytest
 import torch
 
@@ -15,15 +15,15 @@ def ops():
 
 
 @pytest.mark.parametrize("mode", [0, 1, 2, 3, 4, 5])
-def test_umma_operand_modes(ops, mode):
-    """tcgen05 descriptor encodings: K-major / MN-major smem operands, A from TMEM."""
+def test_mma_operand_modes(ops, mode):
+    """wgmma descriptor encodings: K-major / MN-major smem operands, A from registers."""
     g = torch.Generator().manual_seed(mode)
     a = torch.randn(128, 128, generator=g).to(torch.bfloat16)
     b = torch.randn(128, 128, generator=g).to(torch.bfloat16)
     ref = a.double() @ b.double().T
     a_in = a.T.contiguous() if mode & 4 else a
     b_in = b.T.contiguous() if mode & 1 else b
-    d = ops.selftest_umma(mode, a_in.cuda(), b_in.cuda()).cpu().double()
+    d = ops.selftest_mma(mode, a_in.cuda(), b_in.cuda()).cpu().double()
     err = (d - ref).abs().max().item()
     assert err < 1e-3, f"mode {mode}: max err {err}"
 
@@ -157,8 +157,7 @@ def test_ce_head_fused_falls_back_when_logits_are_unbounded(ops):
                                         (1500, 384, 64, True), (2048, 128, 128, True), (4096, 512, 128, False),
                                         (300, 128, 128, False), (257, 192, 128, True)])
 def test_gemm_matches_matmul(ops, M, N, K, b_mn, monkeypatch):
-    """rp_gemm (tile kernel and the weight-stationary persistent kernel, forced on here for M >= 1024) with the fused
-    epilogue: bias + ReLU + residual, K-major and MN-major weights."""
+    """rp_gemm with the fused epilogue: bias + ReLU + residual, K-major and MN-major weights, N beyond one tile."""
     g = torch.Generator().manual_seed(M + N + K)
     A = torch.randn(M, K, generator=g).to(torch.bfloat16)
     W = (torch.randn(N, K, generator=g) * 0.2).to(torch.bfloat16)
@@ -277,9 +276,9 @@ def test_activation_dropout_generator_statistics(ops):
 
 
 @pytest.mark.parametrize("a_mn,b_mn", [(False, False), (False, True), (True, False), (True, True)])
-def test_persistent_streaming_gemm(ops, a_mn, b_mn):
-    """gemm_ps_kernel (tiles >= #SMs, K = 512 so the weight-stationary kernel does not take it): all four operand layouts,
-    fused epilogue (bias + GELU + residual, bf16 out), fp32 store and accumulate, N not a multiple of the tile."""
+def test_gemm_more_tiles_than_sms_all_layouts(ops, a_mn, b_mn):
+    """A GEMM with more tiles than SMs and K = 512: all four operand layouts, fused epilogue (bias + GELU + residual,
+    bf16 out), fp32 store and accumulate, N not a multiple of the tile."""
     g = torch.Generator().manual_seed(int(a_mn) * 2 + int(b_mn))
     M, N, K = 2504, 1184, 512          # 20 x 10 tiles, ragged last M and N tile (pitches stay 16-byte multiples)
     A = (torch.randn(M, K, generator=g) * 0.5).to(torch.bfloat16)
@@ -312,9 +311,9 @@ def test_persistent_streaming_gemm(ops, a_mn, b_mn):
     assert (Ck.cpu().double() - zk).abs().max().item() < 5e-3
 
 
-def test_ce_head_wide_hidden_large_enough_for_the_persistent_gemm(ops):
-    """d = 512 CE backward at a size whose G / dE GEMMs run on gemm_ps_kernel (exp2 epilogue + device-side row limit, MN-major
-    operands + device-side contraction limit)."""
+def test_ce_head_wide_hidden_gemms_with_more_tiles_than_sms(ops):
+    """d = 512 CE backward at a size whose G / dE GEMMs span more tiles than SMs (exp2 epilogue + device-side row limit,
+    MN-major operands + device-side contraction limit)."""
     T, n_valid, I, d = 1536, 1300, 5000, 512
     g = torch.Generator().manual_seed(11)
     hc = (torch.randn(T, d, generator=g) * 0.7).to(torch.bfloat16)
@@ -568,12 +567,12 @@ def test_post_attn_bwd_matches_formula(ops, T, d, drop, masked):
     assert float(((db.cpu().double() + 1.0) - dy.sum(0)).norm() / dy.sum(0).norm()) < 1e-2
 
 
-def test_gemm_weight_stationary_wide_tile_matches_matmul(ops):
-    """The predict body's K | V projection shape (M >= 131072 rows, N = 256, K = 128, bias): gemm_ws_kernel<256> keeps both
-    128-column halves of the weight in one CTA so the activations are read once; against a fp32 matmul of the same bf16 data."""
+def test_gemm_tall_kv_projection_beyond_65535_row_tiles(ops):
+    """The predict body's K | V projection shape (N = 256, K = 128, bias) with more than 65535 row tiles (8.4 M rows: predict
+    at L = 512 with > 16 K users per call), against a fp32 matmul of the same bf16 data on the first and last rows."""
     cuda = torch.device("cuda")
     g = torch.Generator(device="cuda").manual_seed(5)
-    M, N, K = 131072 + 300, 256, 128
+    M, N, K = 128 * 65536 + 300, 256, 128
     A = (torch.randn(M, K, device=cuda, generator=g) * 0.5).bfloat16()
     W = (torch.randn(N, K, device=cuda, generator=g) * 0.2).bfloat16()
     b = torch.randn(N, device=cuda, generator=g)

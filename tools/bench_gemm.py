@@ -22,7 +22,8 @@ def t(fn, n=10):
 
 shapes = [(25600, 1024, 256, False, "bert ffn1 fwd"), (25600, 256, 1024, False, "bert ffn2 fwd"), (25600, 768, 256, False, "bert qkv"),
           (25600, 256, 1024, True, "bert ffn1 dgrad (B MN-major)"), (51200, 128, 128, False, "c2 proj"),
-          (16384, 512, 512, False, "c5 proj"), (1408, 200_000, 512, False, "c5 G gemm slice (N=200K)")]
+          (16384, 512, 512, False, "c5 proj"), (1408, 200_000, 512, False, "c5 G gemm slice (N=200K)"),
+          (819200, 256, 128, False, "predict K|V projection (4096 x 200)")]
 for M, N, K, b_mn, name in shapes:
     A = torch.randn(M, K, device="cuda").to(torch.bfloat16)
     W = (torch.randn(N, K, device="cuda") * 0.1).to(torch.bfloat16)

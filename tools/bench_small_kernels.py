@@ -20,11 +20,11 @@ for M in (128, 1024, 12800, 51200, 204800):
     t0 = bench(lambda: ops.gemm(A, W, C, M, 128, 128))
     t1 = bench(lambda: ops.gemm(A, W, C, M, 128, 128, bias=bias, act=1, residual=R))
     t2 = bench(lambda: ops.gemm(A, W, C, M, 128, 128, b_mn=True))
-    print(f"gemm M={M:7d} N=K=128: plain {t0:6.1f} us | bias+relu+residual {t1:6.1f} us | B MN-major {t2:6.1f} us | ideal HBM {(M*128*2*2)/6.5e6:5.1f} us")
+    print(f"gemm M={M:7d} N=K=128: plain {t0:6.1f} us | bias+relu+residual {t1:6.1f} us | B MN-major {t2:6.1f} us | data-sheet HBM time {(M*128*2*2)/3.35e6:5.1f} us")
 T = 51200
 dY = torch.randn(T, 128, device=dev).bfloat16(); X = torch.randn(T, 128, device=dev).bfloat16()
 dW = torch.zeros(128, 128, device=dev)
-for split in (1, 8, 33, 74, 148):
+for split in (1, 8, 33, 66, 132):
     t = bench(lambda: ops.gemm(dY, X, dW, 128, 128, T, a_mn=True, b_mn=True, out_mode=1, split_k=split))
     print(f"wgrad T={T} split={split:3d}: {t:6.1f} us")
 x = torch.randn(T, 128, device=dev).bfloat16()

@@ -13,7 +13,7 @@ st = torch.cuda.current_stream().cuda_stream
 for rows, d, name in ((50_000, 128, "50K x 128 (12.8 MB, L2-resident)"), (500_000, 128, "500K x 128 (128 MB)")):
     tab = torch.randn(rows, d, device="cuda").to(torch.bfloat16)
     for box_rows in (128, 256):
-        for grid in (1, 148):
+        for grid in (1, torch.cuda.get_device_properties(0).multi_processor_count):
             for same in (0, 1):
                 tiles = 2000
                 f = lambda: check(L.rp_selftest_tma_probe(tab.data_ptr(), rows, d, box_rows, tiles, same, grid, st), "probe")

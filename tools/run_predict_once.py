@@ -1,4 +1,4 @@
-"""One predict() call at the scoring leg's shape (4096 users, L=200, d=128, |I|=500K) for ncu launch lists."""
+"""One predict() call at the scoring leg's shape (4096 users, L=200, d=128, |I|=500K), e.g. to trace with torch.profiler."""
 import os
 import sys
 
