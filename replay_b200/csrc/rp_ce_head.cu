@@ -32,7 +32,7 @@ static constexpr float kLn2 = 0.6931471805599453f;
 // CTA layout of the head kernels: warpgroups 0 / 1 own rows [0, 64) / [64, 128) of the row tile; thread 0 also feeds the TMA
 // ring (a separate producer warp would cap the registers of the accumulating threads)
 static constexpr int kThreads = 256;
-static constexpr int kTN = 64;                  // column tile of the backward / fused kernels
+static constexpr int kTN = 64;                  // grid of the column splits of the fused pass (ce_bwd_kernel tiles: TN)
 // ----------------------------------------------------------------------------------------------------------------
 // forward
 // ----------------------------------------------------------------------------------------------------------------
@@ -302,11 +302,13 @@ __global__ void __launch_bounds__(1024) ce_loss_reduce_kernel(const float* __res
 // MODE 2: rows = tokens, FUSED forward+backward: G~ = exp(s + b) with reference max 0 (valid while |s| is bounded, see
 //         ce_bound_kernel), per-row sum of G~ and un-normalised dH~ = sum_i G~ E_i over this CTA's column split
 //                                                                                      -> out = partial dH~ fp32, zpart
-// CTA = one 128-row tile against the column tiles [j0, j0 + n_ct) (64 columns each).  Per column tile: S = A_tile . B_tile^T
-// (wgmma, registers), G = exp2(S log2e + offset) in registers, acc += G . B_tile with G as the register A operand and the
-// same shared-memory B tile read MN-major.  At the end the [128 x D] accumulator goes through shared memory to the row-wise
-// epilogue (thread = row, warpgroup = half of the D columns).
-template <int KCH, int NSTAGE, int MODE, bool HAS_BIAS>
+// CTA = one 128-row tile against the columns [c_begin, c_end) in n_ct tiles of TN columns.  Per column tile: S = A_tile .
+// B_tile^T (wgmma, registers), G = exp2(S log2e + offset) in registers, acc += G . B_tile with G as the register A operand
+// and the same shared-memory B tile read MN-major.  At the end the [128 x D] accumulator goes through shared memory to the
+// row-wise epilogue (thread = row, warpgroup = half of the D columns).
+// TN = 128 halves how often the A tile is read from shared memory per column (the S wgmma at N = 64 needs as many bytes per
+// cycle as shared memory delivers); d = 256 keeps TN = 64 because a 128-column S does not fit next to its accumulator.
+template <int KCH, int NSTAGE, int TN, int MODE, bool HAS_BIAS>
 __global__ void __launch_bounds__(kThreads, 1)
 ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
               const __nv_bfloat16* __restrict__ a_rows /* the row-side matrix (tmA) as a plain pointer */,
@@ -318,7 +320,7 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   constexpr bool COLCONST = (MODE == 1);
   constexpr bool FUSED = (MODE == 2);
   constexpr int D = KCH * 64;
-  constexpr int kChunkB = kTN * 128;      // bytes of one [64 rows x 64 bf16] swizzled chunk of a column tile
+  constexpr int kChunkB = TN * 128;       // bytes of one [TN rows x 64 bf16] swizzled chunk of a column tile
   constexpr int kStage = KCH * kChunkB;   // one column tile in shared memory
   constexpr int PITCH = D + 4;            // fp32 accumulator stage (over the ring once the column tiles are done)
   constexpr int kSlots = 2, DW = D / kSlots;
@@ -336,10 +338,13 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   const int split = FUSED ? blockIdx.x % n_splits : 0;
   const int n_rows = COLCONST ? n_items : n_valid;
   const int n_cols = COLCONST ? n_valid : n_items;
-  const int n_ct_all = (n_cols + kTN - 1) / kTN;
+  // column split of the fused pass on a grid of kTN columns whatever TN is, so the splits (and the order in which their
+  // partial sums are added) do not depend on the tile size; a split's last tile is masked at c_end
+  const int n_grid = (n_cols + kTN - 1) / kTN;
   const int row_tile = FUSED ? blockIdx.x / n_splits : blockIdx.x;
-  const int j0 = FUSED ? (int)(((long long)n_ct_all * split) / n_splits) : 0;
-  const int n_ct = FUSED ? (int)(((long long)n_ct_all * (split + 1)) / n_splits) - j0 : n_ct_all;
+  const int c_begin = FUSED ? (int)(((long long)n_grid * split) / n_splits) * kTN : 0;
+  const int c_end = FUSED ? min(n_cols, (int)(((long long)n_grid * (split + 1)) / n_splits) * kTN) : n_cols;
+  const int n_ct = c_end > c_begin ? (c_end - c_begin + TN - 1) / TN : 0;
   const int r0 = row_tile * kT;
   if (r0 >= n_rows) return;
 
@@ -358,7 +363,7 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     const uint32_t s = jl % NSTAGE;
     mbar_wait(&bar_empty[s], ((jl / NSTAGE) & 1) ^ 1);
     mbar_arrive_expect_tx(&bar_full[s], kStage);
-    for (int kc = 0; kc < KCH; ++kc) tma_load_2d(sB + s * kStage + kc * kChunkB, &tmB, &bar_full[s], kc * 64, (j0 + jl) * kTN);
+    for (int kc = 0; kc < KCH; ++kc) tma_load_2d(sB + s * kStage + kc * kChunkB, &tmB, &bar_full[s], kc * 64, c_begin + jl * TN);
   };
   if (threadIdx.x == 0) {
     mbar_arrive_expect_tx(&bar_a, KCH * kChunk);
@@ -386,22 +391,22 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     const uint32_t s = jl % NSTAGE, ph = (jl / NSTAGE) & 1;
     mbar_wait(&bar_full[s], ph);
     const uint32_t b0 = smem_u32(sB + s * kStage);
-    float sacc[kTN / 2];
+    float sacc[TN / 2];
     wg_fence();
 #pragma unroll
     for (int kc = 0; kc < KCH; ++kc)
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks)
-        WgmmaSS<kTN>::template run<0, 0>(sacc, desc_k(a_base + kc * kChunk + ks * 32), desc_k(b0 + kc * kChunkB + ks * 32),
-                                         (kc | ks) != 0);
+        WgmmaSS<TN>::template run<0, 0>(sacc, desc_k(a_base + kc * kChunk + ks * 32), desc_k(b0 + kc * kChunkB + ks * 32),
+                                        (kc | ks) != 0);
     wg_commit();
     wg_wait<0>();
     wg_fence_acc(sacc);
     // G = exp2(S log2e + offset) -> bf16 A fragments
-    const int col0 = (j0 + jl) * kTN + fc;
-    uint32_t pk[kTN / 4];
+    const int col0 = c_begin + jl * TN + fc;
+    uint32_t pk[TN / 4];
 #pragma unroll
-    for (int q = 0; q < kTN / 8; ++q) {
+    for (int q = 0; q < TN / 8; ++q) {
       float g[4];
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
@@ -412,7 +417,7 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
           g[e] = ex2f(fmaf(va, kLog2e, cc));
           g[2 + e] = ex2f(fmaf(vb, kLog2e, cc));
         } else {
-          const bool in = col < n_items;
+          const bool in = col < c_end;
           if (HAS_BIAS && in) {
             const float bb = __ldg(bias + col);
             va += bb;
@@ -431,7 +436,7 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     }
     wg_fence();
 #pragma unroll
-    for (int kk = 0; kk < kTN / 16; ++kk) {
+    for (int kk = 0; kk < TN / 16; ++kk) {
       const uint32_t af[4] = {pk[4 * kk], pk[4 * kk + 1], pk[4 * kk + 2], pk[4 * kk + 3]};
       WgmmaRS<D>::template run<1>(acc, af, desc_mn(b0 + kk * 2048, kChunkB), 1);
     }
@@ -872,22 +877,22 @@ static int launch_ce_fwd(const CUtensorMap& tmA, const CUtensorMap& tmB, const i
   return RP_OK;
 }
 
-template <int KCH, int NSTAGE, int MODE>
+template <int KCH, int NSTAGE, int TN, int MODE>
 static int launch_ce_bwd(const CUtensorMap& tmA, const void* b_mat, int b_rows, const void* a_rows, const float* cvec,
                          const int32_t* labels,
                          const void* table, const float* loss_inv, const int32_t* n_valid, int n_items, const float* bias,
                          float* d_bias, void* out, int grid, const int32_t* safe_flag, int run_if_safe, int n_splits,
                          int capacity, float* zpart, cudaStream_t stream, const CeDirect& direct = CeDirect{nullptr, nullptr, nullptr, nullptr, CeRowOpts{nullptr, nullptr, 0, 0.f, 0.f}, 0}) {
   // row tile + a ring of NSTAGE column tiles; the fp32 accumulator stage reuses the ring at the end
-  const int ring = NSTAGE * KCH * kTN * 128, stage = 128 * (KCH * 64 + 4) * 4;
+  const int ring = NSTAGE * KCH * TN * 128, stage = 128 * (KCH * 64 + 4) * 4;
   const int smem = KCH * kChunk + (ring > stage ? ring : stage) + 1024;
-  CUtensorMap tmB;   // column-side matrix, one [64 rows x 64 columns] box per chunk
+  CUtensorMap tmB;   // column-side matrix, one [TN rows x 64 columns] box per chunk
   {
-    const int rc = make_tmap_bf16(&tmB, b_mat, b_rows, KCH * 64, KCH * 64, kTN);
+    const int rc = make_tmap_bf16(&tmB, b_mat, b_rows, KCH * 64, KCH * 64, TN);
     if (rc != RP_OK) return rc;
   }
   // the biased head (BERT4Rec) is a separate instantiation: its per-column adds / row sums cost an instruction per logit
-  auto kern = bias ? ce_bwd_kernel<KCH, NSTAGE, MODE, true> : ce_bwd_kernel<KCH, NSTAGE, MODE, false>;
+  auto kern = bias ? ce_bwd_kernel<KCH, NSTAGE, TN, MODE, true> : ce_bwd_kernel<KCH, NSTAGE, TN, MODE, false>;
   RP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   kern<<<grid, kThreads, smem, stream>>>(tmA, tmB, reinterpret_cast<const __nv_bfloat16*>(a_rows), cvec, labels,
                                          reinterpret_cast<const __nv_bfloat16*>(table), loss_inv,
@@ -904,13 +909,13 @@ static int dispatch_ce_bwd(int d, const CUtensorMap& tmA, const void* b_mat, int
                            int capacity, float* zpart, cudaStream_t stream, const CeDirect& direct = CeDirect{nullptr, nullptr, nullptr, nullptr, CeRowOpts{nullptr, nullptr, 0, 0.f, 0.f}, 0}) {
   switch (d) {
     case 64:
-      return launch_ce_bwd<1, 8, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
+      return launch_ce_bwd<1, 8, 128, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
                                        safe_flag, run_if_safe, n_splits, capacity, zpart, stream, direct);
     case 128:
-      return launch_ce_bwd<2, 6, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
+      return launch_ce_bwd<2, 4, 128, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
                                        safe_flag, run_if_safe, n_splits, capacity, zpart, stream, direct);
     case 256:
-      return launch_ce_bwd<4, 4, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
+      return launch_ce_bwd<4, 4, 64, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
                                        safe_flag, run_if_safe, n_splits, capacity, zpart, stream, direct);
     default:
       return RP_ESHAPE;
