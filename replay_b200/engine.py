@@ -650,22 +650,7 @@ class SasRecEngine:
                 self._ln_fwd(x, f("ln1_w"), f("ln1_b"), 1e-8, a["q_in"], a["mean1"], a["rstd1"], T)
                 self._gemm(a["q_in"], in_w[:d], a["Q"], T, d, d, bias=in_b[:d])
                 self._gemm(x, in_w[d:], a["KV"], T, 2 * d, d, bias=in_b[d:])
-            ad = AttnDesc()
-            ad.q, ad.q_rows, ad.q_cols, ad.ldq, ad.q_c0 = a["Q"].data_ptr(), T, d, d, 0
-            ad.k, ad.k_rows, ad.k_cols, ad.ldk, ad.k_c0 = a["KV"].data_ptr(), T, 2 * d, 2 * d, 0
-            ad.v, ad.v_rows, ad.v_cols, ad.ldv, ad.v_c0 = a["KV"].data_ptr(), T, 2 * d, 2 * d, d
-            ad.B, ad.H, ad.L, ad.head_dim = self.B, H, L, hd
-            ad.causal, ad.mask_pad_keys = 1, int(not legacy)
-            ad.scale = att_scale
-            ad.pad_mask = pad.data_ptr()
-            ad.out, ad.ldo = a["O"].data_ptr(), d
-            if training and self.with_grad:
-                ad.p_save = None if self.fused_attn_bwd else a["P"].data_ptr()
-                ad.inv_sum, ad.m_save = a["inv_sum"].data_ptr(), a["m2"].data_ptr()
-            else:
-                ad.p_save, ad.inv_sum, ad.m_save = None, None, None
-            ad.drop_p, ad.seed, ad.drop_off, ad.seed_ptr = drop, self.seed, self._site(i, 0) << 40, self.rng_counter.data_ptr()
-            check(self.lib.rp_attn_fwd(ctypes.byref(ad), self._stream()), "rp_attn_fwd")
+            self._attention_forward(i, training)
             if not training and d <= 128 and self.fused_post_attn_eval:
                 # inference: out-projection + residual + LayerNorm + FFN in one pass over the tokens (csrc/rp_block_fused.cu)
                 check(self.lib.rp_post_attn_fused(a["O"].data_ptr(), a["q_in"].data_ptr(), w("out_w").data_ptr(),
@@ -697,6 +682,73 @@ class SasRecEngine:
             self._gemm(a["u"], w("w2"), self.x[i + 1], T, d, d, bias=f("b2"), drop_p=drop, drop_site=self._site(i, 2),
                        residual=a["y"], rowmask=pad if legacy else None)
 
+    def _attention_forward(self, i: int, training: bool):
+        """Attention core of block ``i``: O = softmax(Q.K^T * scale, causal + pad-key mask) . V over act[i]'s Q and packed
+        [K | V] (one [T, 2d] array), saving the row statistics (and P on the un-fused path) when training with gradients."""
+        cfg, T, d, L = self.cfg, self.T, self.cfg.dp, self.L
+        H, a = cfg.n_heads, self.act[i]
+        ad = AttnDesc()
+        ad.q, ad.q_rows, ad.q_cols, ad.ldq, ad.q_c0 = a["Q"].data_ptr(), T, d, d, 0
+        ad.k, ad.k_rows, ad.k_cols, ad.ldk, ad.k_c0 = a["KV"].data_ptr(), T, 2 * d, 2 * d, 0
+        ad.v, ad.v_rows, ad.v_cols, ad.ldv, ad.v_c0 = a["KV"].data_ptr(), T, 2 * d, 2 * d, d
+        ad.B, ad.H, ad.L, ad.head_dim = self.B, H, L, d // H
+        ad.causal, ad.mask_pad_keys = 1, int(cfg.variant != "legacy")
+        ad.scale = 1.0 / math.sqrt(cfg.head_dim)
+        ad.pad_mask = self.in_pad.data_ptr()
+        ad.out, ad.ldo = a["O"].data_ptr(), d
+        if training and self.with_grad:
+            ad.p_save = None if self.fused_attn_bwd else a["P"].data_ptr()
+            ad.inv_sum, ad.m_save = a["inv_sum"].data_ptr(), a["m2"].data_ptr()
+        else:
+            ad.p_save, ad.inv_sum, ad.m_save = None, None, None
+        ad.drop_p = cfg.dropout if training else 0.0
+        ad.seed, ad.drop_off, ad.seed_ptr = self.seed, self._site(i, 0) << 40, self.rng_counter.data_ptr()
+        check(self.lib.rp_attn_fwd(ctypes.byref(ad), self._stream()), "rp_attn_fwd")
+
+    def _attention_backward(self, i: int):
+        """dQ (into s["dQ"]) and packed [dK | dV] (into s["dKV"]) of block ``i``'s attention core from s["d_o"] and what
+        ``_attention_forward(i, True)`` saved: the fused kernel for head slot 64 at L <= 256, otherwise dPd = dO.V^T, the
+        row-wise softmax backward over the saved probabilities, and three batched GEMMs."""
+        cfg, T, d, L, Lp = self.cfg, self.T, self.cfg.dp, self.L, self.Lp
+        H, a, s, st = cfg.n_heads, self.act[i], self.s, self._stream
+        hd, BH = d // H, self.B * H
+        att_scale, drop = 1.0 / math.sqrt(cfg.head_dim), cfg.dropout
+        KV, Q = a["KV"], a["Q"]
+        if self.fused_attn_bwd:
+            bd = AttnBwdDesc()
+            bd.q, bd.q_rows, bd.q_cols, bd.ldq, bd.q_c0 = Q.data_ptr(), T, d, d, 0
+            bd.k, bd.k_rows, bd.k_cols, bd.ldk, bd.k_c0 = KV.data_ptr(), T, 2 * d, 2 * d, 0
+            bd.v, bd.v_rows, bd.v_cols, bd.ldv, bd.v_c0 = KV.data_ptr(), T, 2 * d, 2 * d, d
+            bd.d_out, bd.do_rows, bd.do_cols, bd.ld_do = s["d_o"].data_ptr(), T, d, d
+            bd.out, bd.ldo = a["O"].data_ptr(), d
+            bd.B, bd.H, bd.L, bd.head_dim = self.B, H, L, hd
+            bd.causal, bd.mask_pad_keys = 1, int(cfg.variant != "legacy")
+            bd.scale = att_scale
+            bd.pad_mask = self.in_pad.data_ptr()
+            bd.m_save, bd.inv_sum = a["m2"].data_ptr(), a["inv_sum"].data_ptr()
+            bd.dq, bd.ld_dq, bd.dq_c0 = s["dQ"].data_ptr(), d, 0
+            bd.dk, bd.ld_dk, bd.dk_c0 = s["dKV"].data_ptr(), 2 * d, 0
+            bd.dv, bd.ld_dv, bd.dv_c0 = s["dKV"].data_ptr(), 2 * d, d
+            bd.drop_p, bd.seed, bd.drop_off, bd.seed_ptr = drop, self.seed, self._site(i, 0) << 40, self.rng_counter.data_ptr()
+            check(self.lib.rp_attn_bwd(ctypes.byref(bd), st()), "rp_attn_bwd")
+            return
+        P, dpd = a["P"].view(BH * Lp, Lp), s["dpd"].view(BH * Lp, Lp)
+        # dPd = dO . V^T
+        self._gemm(s["d_o"], KV, dpd, L, L, hd, batch=BH, inner=H, a_off=(0, L, 0, 0, 0, hd), b_off=(0, L, 0, d, 0, hd),
+                   c_geom=(Lp, 0, H * Lp * Lp, Lp * Lp))
+        check(self.lib.rp_attn_softmax_bwd(P.data_ptr(), dpd.data_ptr(), a["inv_sum"].data_ptr(), BH, L,
+                                           att_scale, drop, self.seed, self._site(i, 0) << 40,
+                                           self.rng_counter.data_ptr(), st()), "rp_attn_softmax_bwd")
+        # dQ = dS . K      (A = dS [BH*Lp, Lp] K-major, B = K MN-major)
+        self._gemm(dpd, KV, s["dQ"], L, hd, L, b_mn=True, batch=BH, inner=H, a_off=(0, H * Lp, Lp, 0, 0, 0),
+                   b_off=(0, L, 0, 0, 0, hd), c_geom=(d, 0, L * d, hd))
+        # dK = dS^T . Q    (A = dS MN-major, B = Q MN-major)
+        self._gemm(dpd, Q, s["dKV"], L, hd, L, a_mn=True, b_mn=True, batch=BH, inner=H, a_off=(0, H * Lp, Lp, 0, 0, 0),
+                   b_off=(0, L, 0, 0, 0, hd), c_geom=(2 * d, 0, L * 2 * d, hd))
+        # dV = Pd^T . dO
+        self._gemm(P, s["d_o"], s["dKV"], L, hd, L, a_mn=True, b_mn=True, batch=BH, inner=H,
+                   a_off=(0, H * Lp, Lp, 0, 0, 0), b_off=(0, L, 0, 0, 0, hd), c_geom=(2 * d, d, L * 2 * d, hd))
+
     def forward_train(self):
         """Loss of the staged batch (device fp32 [2] view: mean CE over the valid targets, 1/n_valid)."""
         cfg, T = self.cfg, self.T
@@ -723,13 +775,11 @@ class SasRecEngine:
     # ------------------------------------------------------------------------------------------------ backward
     def backward(self):
         cfg, T, d, L = self.cfg, self.T, self.cfg.dp, self.L
-        hdv, att_scale = cfg.hd_valid, 1.0 / math.sqrt(cfg.head_dim)
+        hdv = cfg.hd_valid
         p16, prm, G, s = self.params16, self.params, self.grads, self.s
         legacy = cfg.variant == "legacy"
         drop = cfg.dropout
         ks = 1.0 / (1.0 - drop) if drop > 0 else 1.0
-        H, hd, Lp = cfg.n_heads, d // cfg.n_heads, self.Lp
-        BH = self.B * H
         st = self._stream
         from .ops import ce_head_bwd
 
@@ -800,42 +850,7 @@ class SasRecEngine:
                 if not fw:
                     self._wgrad(s["dh"], a["O"], g("out_w"), d, d)
                 bias_grads.append((s["dh"], g("out_b")))
-            # ---- attention backward
-            KV, Q = a["KV"], a["Q"]
-            if self.fused_attn_bwd:
-                bd = AttnBwdDesc()
-                bd.q, bd.q_rows, bd.q_cols, bd.ldq, bd.q_c0 = Q.data_ptr(), T, d, d, 0
-                bd.k, bd.k_rows, bd.k_cols, bd.ldk, bd.k_c0 = KV.data_ptr(), T, 2 * d, 2 * d, 0
-                bd.v, bd.v_rows, bd.v_cols, bd.ldv, bd.v_c0 = KV.data_ptr(), T, 2 * d, 2 * d, d
-                bd.d_out, bd.do_rows, bd.do_cols, bd.ld_do = s["d_o"].data_ptr(), T, d, d
-                bd.out, bd.ldo = a["O"].data_ptr(), d
-                bd.B, bd.H, bd.L, bd.head_dim = self.B, H, L, hd
-                bd.causal, bd.mask_pad_keys = 1, int(not legacy)
-                bd.scale = att_scale
-                bd.pad_mask = self.in_pad.data_ptr()
-                bd.m_save, bd.inv_sum = a["m2"].data_ptr(), a["inv_sum"].data_ptr()
-                bd.dq, bd.ld_dq, bd.dq_c0 = s["dQ"].data_ptr(), d, 0
-                bd.dk, bd.ld_dk, bd.dk_c0 = s["dKV"].data_ptr(), 2 * d, 0
-                bd.dv, bd.ld_dv, bd.dv_c0 = s["dKV"].data_ptr(), 2 * d, d
-                bd.drop_p, bd.seed, bd.drop_off, bd.seed_ptr = drop, self.seed, self._site(i, 0) << 40, self.rng_counter.data_ptr()
-                check(self.lib.rp_attn_bwd(ctypes.byref(bd), st()), "rp_attn_bwd")
-            else:
-                P, dpd = a["P"].view(BH * Lp, Lp), s["dpd"].view(BH * Lp, Lp)
-                # dPd = dO . V^T
-                self._gemm(s["d_o"], KV, dpd, L, L, hd, batch=BH, inner=H, a_off=(0, L, 0, 0, 0, hd), b_off=(0, L, 0, d, 0, hd),
-                           c_geom=(Lp, 0, H * Lp * Lp, Lp * Lp))
-                check(self.lib.rp_attn_softmax_bwd(P.data_ptr(), dpd.data_ptr(), a["inv_sum"].data_ptr(), BH, L,
-                                                   att_scale, drop, self.seed, self._site(i, 0) << 40,
-                                                   self.rng_counter.data_ptr(), st()), "rp_attn_softmax_bwd")
-                # dQ = dS . K      (A = dS [BH*Lp, Lp] K-major, B = K MN-major)
-                self._gemm(dpd, KV, s["dQ"], L, hd, L, b_mn=True, batch=BH, inner=H, a_off=(0, H * Lp, Lp, 0, 0, 0),
-                           b_off=(0, L, 0, 0, 0, hd), c_geom=(d, 0, L * d, hd))
-                # dK = dS^T . Q    (A = dS MN-major, B = Q MN-major)
-                self._gemm(dpd, Q, s["dKV"], L, hd, L, a_mn=True, b_mn=True, batch=BH, inner=H, a_off=(0, H * Lp, Lp, 0, 0, 0),
-                           b_off=(0, L, 0, 0, 0, hd), c_geom=(2 * d, 0, L * 2 * d, hd))
-                # dV = Pd^T . dO
-                self._gemm(P, s["d_o"], s["dKV"], L, hd, L, a_mn=True, b_mn=True, batch=BH, inner=H,
-                           a_off=(0, H * Lp, Lp, 0, 0, 0), b_off=(0, L, 0, 0, 0, hd), c_geom=(2 * d, d, L * 2 * d, hd))
+            self._attention_backward(i)
             # ---- projections
             in_w = w("in_w")
             if self.fused_pre_attn:
