@@ -768,7 +768,7 @@ RP_API int rp_colsum_multi(int n, const void* const* dy, const int* cols, const 
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (n <= 0 || n > 6 || !dy || !cols || !ld || !db || rows <= 0) return RP_EINVAL;
   ColsumBatch b;
-  int max_cols = 0, min_cols = 1 << 30;
+  int max_cols = 0, red_floats = 0;
   for (int i = 0; i < n; ++i) {
     if (!dy[i] || !db[i] || cols[i] <= 0 || (cols[i] & 3) || cols[i] > 1024 || (ld[i] & 3)) return RP_EINVAL;
     b.dy[i] = reinterpret_cast<const __nv_bfloat16*>(dy[i]);
@@ -776,15 +776,18 @@ RP_API int rp_colsum_multi(int n, const void* const* dy, const int* cols, const 
     b.ld[i] = ld[i];
     b.cols[i] = cols[i];
     max_cols = cols[i] > max_cols ? cols[i] : max_cols;
-    min_cols = cols[i] < min_cols ? cols[i] : min_cols;
+    // tensor i reduces through [rlanes_i][cols_i] floats (<= 1024): size the buffer for the largest of these products, not
+    // for max rlanes x max cols (64 KB when widths 64 and 1024 share a launch: over the default limit, the launch failed)
+    const int red = (256 / (cols[i] / 4)) * cols[i];
+    red_floats = red > red_floats ? red : red_floats;
   }
   b.rows = rows;
-  const int rlanes_max = 256 / (min_cols / 4), rlanes_min = 256 / (max_cols / 4);
+  const int rlanes_min = 256 / (max_cols / 4);
   if (rlanes_min < 1) return RP_ESHAPE;
   int gx = sm_count() * 4 / n;
   if (gx < 1) gx = 1;
   if (gx > (rows + rlanes_min - 1) / rlanes_min) gx = (rows + rlanes_min - 1) / rlanes_min;
-  const size_t smem = (size_t)(rlanes_max > rlanes_min ? rlanes_max : rlanes_min) * max_cols * sizeof(float);
+  const size_t smem = (size_t)red_floats * sizeof(float);
   colsum_multi_kernel<<<dim3(gx, n), 256, smem, stream>>>(b);
   RP_LAUNCH_CHECK();
   return RP_OK;
