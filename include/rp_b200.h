@@ -107,6 +107,22 @@ int rp_ce_head_bwd(const void* hc, const void* table, const float* bias, const i
                    int capacity, int n_items, int d, const float* loss_out, const float* cvec, void* d_hc, float* d_table,
                    float* d_bias, int fused, int n_valid_hint, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Full-catalog BCE head, single positive label per position, over the same buffers (workspace: rp_ce_head_workspace):
+ *   replaces  BCEWithLogitsLoss(reduction="sum")(logits, onehot(y)) / T_v     replay/nn/loss/bce.py:10-95
+ *                                                   replay/models/nn/sequential/bert4rec/lightning.py:273-305
+ *   loss_out fp32 [2] = { sum_t [sum_i softplus(x_ti) - x_t,y_t] / T_v, 1 / T_v },  x = hc . table^T (+ bias).
+ * The sigmoid is bounded: no log-sum-exp, no bound guard, no second pass.  d_hc (optional, d <= 256) enables the fused
+ * forward + dH pass; loss and d_hc are bitwise reproducible.  The backward overwrites d_table (and d_bias iff bias) with
+ * (sigmoid - onehot)^T . hc / T_v and its column sums; `fused` must equal (d_hc != NULL && d <= 256) of the forward.
+ * d in {64,128,256} with or without bias, 512 without bias (materialised sigmoid chunks, rp_gemm act 4).  The BCE head reads
+ * bias entries < n_items only, so a bias of exactly n_items entries is enough here. */
+int rp_bce_head_fwd(const void* hc, const void* table, const float* bias, const int32_t* labels, const int32_t* n_valid,
+                    int capacity, int n_items, int d, float* loss_out, void* d_hc, int n_valid_hint, void* workspace,
+                    size_t workspace_bytes, void* stream);
+int rp_bce_head_bwd(const void* hc, const void* table, const float* bias, const int32_t* labels, const int32_t* n_valid,
+                    int capacity, int n_items, int d, const float* loss_out, void* d_hc, float* d_table, float* d_bias,
+                    int fused, int n_valid_hint, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Transformer body.  All activations are token-major bf16 [T = B*L, d]; weights are the bf16 shadow of the fp32 masters.
  * ------------------------------------------------------------------------------------------------------------- */
@@ -122,7 +138,8 @@ int rp_ce_head_bwd(const void* hc, const void* table, const float* bias, const i
  * out_mode 0: bf16 store, 1: fp32 atomic add (split_k >= 1), 2: fp32 store, 3: fp32 store of the split-K partial at
  * C + ksplit * c_split_stride (deterministic two-stage split-K; reduce with rp_reduce_splits), 4: fp32 C += x as a plain
  * read-modify-write (split_k == 1, every element has one owner).
- * Epilogue order: alpha, bias[N], act (0 none, 1 ReLU, 2 GELU-erf, 3 exp2 with a per-row offset), Philox dropout(drop_p; seed + *seed_ptr, drop_offset +
+ * Epilogue order: alpha, bias[N], act (0 none, 1 ReLU, 2 GELU-erf, 3 exp2 with a per-row offset, 4 sigmoid times 2^(per-row
+ * offset): x = sigmoid(x) * exp2(row_exp2_offset[m]), exactly 0 where the offset is -inf), Philox dropout(drop_p; seed + *seed_ptr, drop_offset +
  * element offset in C), gate (x *= gate != 0 ? gate_scale : 0, same geometry as C), residual (bf16, same geometry as C),
  * post-residual dropout (post_drop_p, post_drop_offset), rowmask[rowmask_off0 + outer*rowmask_oo + m].
  * C2 (optional, bf16, geometry of C) receives the value after the bias and before the activation; gate_mode 1 multiplies
@@ -141,7 +158,7 @@ typedef struct rp_gemm_desc {
   const void* gate; float gate_scale;
   void* C2; int gate_mode; float post_drop_p; unsigned long long post_drop_offset;
   long long c_split_stride;
-  const float* row_exp2_offset;                    /* act 3: x = exp2(x * log2(e) + row_exp2_offset[m]) */
+  const float* row_exp2_offset;                    /* act 3: x = exp2(x * log2(e) + row_exp2_offset[m]); act 4: see above */
   const int32_t* m_limit_dev; int m_limit_base;    /* device scalar: 128-row tiles with m0 + base >= *limit are skipped */
   const int32_t* k_limit_dev; int k_limit_base;    /* device scalar: the contraction stops at *limit - base, rounded up to
                                                       a whole 64-element chunk (operands beyond the limit must be finite) */

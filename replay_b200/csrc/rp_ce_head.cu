@@ -17,6 +17,15 @@
 //   ce_bwd_kernel<COL> CTA = 128 items, loops over token tiles:   S^T = E_tile . Hc^T, G = exp2(S^T*log2e + c_col),
 //                      dE += G . Hc_tile                                                          -> dE fp32 [I, d] (=)
 //   ce_label_scatter   dE[y_t] -= Hc[t] / T_v   (the one-hot part of softmax - onehot, sparse)
+//
+// The full-catalog BCE head (rp_bce_head_*) runs on the same tile loops:
+//   loss = (1/T_v) sum_t [ sum_i softplus(x_ti) - x_t,y_t ],  x = s + b,  dx = (sigmoid(x) - onehot) / T_v
+// replacing  BCEWithLogitsLoss(sum) / T_v            replay/nn/loss/bce.py:10-95 ; bert4rec/lightning.py:273-305
+//   ce_bwd_kernel<3>   rows = tokens: G = sigmoid(S + b) (bf16 A operand), dH += G . E_tile, row sums of softplus
+//   ce_bwd_kernel<4>   rows = items: G = sigmoid(S^T + b_row) over the valid tokens, dE = G . Hc / T_v, d_bias = rowsum / T_v
+//   ce_fwd_kernel<BCE> row sums of softplus only (the un-fused forward, and the loss at d = 512)
+// The sigmoid is bounded, so there is no log-sum-exp, no bound guard and no second pass; rows past T_v and columns past the
+// split end are masked explicitly (sigmoid(0) = 1/2 would leak where CE's exp(-inf) = 0 does not).
 #include <type_traits>
 
 #include "rp_host.h"
@@ -33,10 +42,21 @@ static constexpr float kLn2 = 0.6931471805599453f;
 // ring (a separate producer warp would cap the registers of the accumulating threads)
 static constexpr int kThreads = 256;
 static constexpr int kTN = 64;                  // grid of the column splits of the fused pass (ce_bwd_kernel tiles: TN)
+
+// BCE per logit x, with e = exp(-|x|):  sigmoid = (x >= 0 ? 1 : e) / (1 + e),  softplus = max(x, 0) + log1p(e).
+// The log1p terms are summed as lg2 of the product of a column tile's (1 + e) factors (at most 32 per thread and row, each in
+// (1, 2], so the product stays below 2^32): a logit costs two special-function operations (ex2, rcp) instead of three.
+__device__ __forceinline__ float bce_sigmoid(float x, float& one_plus_e) {
+  const float e = ex2f(-fabsf(x) * kLog2e);
+  one_plus_e = 1.f + e;
+  return __fdividef(x >= 0.f ? 1.f : e, one_plus_e);
+}
 // ----------------------------------------------------------------------------------------------------------------
 // forward
 // ----------------------------------------------------------------------------------------------------------------
-template <int KCH, int NSTAGE>
+// BCE = true: per (row, split) sum of softplus(s + b) over the split's columns instead of the (max, sum-exp) pair; `part` then
+// holds floats, element (t, split) at [t * n_splits + split].
+template <int KCH, int NSTAGE, bool BCE = false>
 __global__ void __launch_bounds__(kThreads, 1)
 ce_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
               const int32_t* __restrict__ n_valid_ptr, int n_items, int n_splits, const float* __restrict__ bias,
@@ -114,6 +134,22 @@ ce_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         acc[4 * q + e] = in ? acc[4 * q + e] + b : -INFINITY;
         acc[4 * q + 2 + e] = in ? acc[4 * q + 2 + e] + b : -INFINITY;
       }
+    if constexpr (BCE) {   // softplus(-inf) = max(-inf, 0) + lg2(1 + 0) = 0: the masked columns add nothing
+      float pa = 1.f, pb = 1.f, xa = 0.f, xb = 0.f;
+#pragma unroll
+      for (int q = 0; q < kT / 8; ++q)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float va = acc[4 * q + e], vb = acc[4 * q + 2 + e];
+          xa += fmaxf(va, 0.f);
+          xb += fmaxf(vb, 0.f);
+          pa *= 1.f + ex2f(-fabsf(va) * kLog2e);
+          pb *= 1.f + ex2f(-fabsf(vb) * kLog2e);
+        }
+      sa += xa + __log2f(pa) * kLn2;
+      sb += xb + __log2f(pb) * kLn2;
+      continue;
+    }
     float cma = -INFINITY, cmb = -INFINITY;
 #pragma unroll
     for (int q = 0; q < kT / 8; ++q) {
@@ -134,20 +170,30 @@ ce_fwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     sa += xa;
     sb += xb;
   }
-  // the four threads of a quad hold the same rows: merge their (max, sum) pairs
+  if constexpr (BCE) {
+    sa = quad_sum(sa);
+    sb = quad_sum(sb);
+    float* zrow = reinterpret_cast<float*>(part);
+    if (fc == 0) {
+      if (ta < n_valid) zrow[(size_t)ta * n_splits + split] = sa;
+      if (tb < n_valid) zrow[(size_t)tb * n_splits + split] = sb;
+    }
+  } else {
+    // the four threads of a quad hold the same rows: merge their (max, sum) pairs
 #pragma unroll
-  for (int o = 1; o <= 2; o <<= 1) {
-    const float oma = __shfl_xor_sync(0xffffffffu, ma, o), osa = __shfl_xor_sync(0xffffffffu, sa, o);
-    const float omb = __shfl_xor_sync(0xffffffffu, mb, o), osb = __shfl_xor_sync(0xffffffffu, sb, o);
-    const float na = fmaxf(ma, oma), nb = fmaxf(mb, omb);
-    sa = sa * ex2f(ma - na) + osa * ex2f(oma - na);
-    sb = sb * ex2f(mb - nb) + osb * ex2f(omb - nb);
-    ma = na;
-    mb = nb;
-  }
-  if (fc == 0) {
-    if (ta < n_valid) part[(size_t)ta * n_splits + split] = make_float2(ma, sa);
-    if (tb < n_valid) part[(size_t)tb * n_splits + split] = make_float2(mb, sb);
+    for (int o = 1; o <= 2; o <<= 1) {
+      const float oma = __shfl_xor_sync(0xffffffffu, ma, o), osa = __shfl_xor_sync(0xffffffffu, sa, o);
+      const float omb = __shfl_xor_sync(0xffffffffu, mb, o), osb = __shfl_xor_sync(0xffffffffu, sb, o);
+      const float na = fmaxf(ma, oma), nb = fmaxf(mb, omb);
+      sa = sa * ex2f(ma - na) + osa * ex2f(oma - na);
+      sb = sb * ex2f(mb - nb) + osb * ex2f(omb - nb);
+      ma = na;
+      mb = nb;
+    }
+    if (fc == 0) {
+      if (ta < n_valid) part[(size_t)ta * n_splits + split] = make_float2(ma, sa);
+      if (tb < n_valid) part[(size_t)tb * n_splits + split] = make_float2(mb, sb);
+    }
   }
 }
 
@@ -308,6 +354,11 @@ __global__ void __launch_bounds__(1024) ce_loss_reduce_kernel(const float* __res
 // row-wise epilogue (thread = row, warpgroup = half of the D columns).
 // TN = 128 halves how often the A tile is read from shared memory per column (the S wgmma at N = 64 needs as many bytes per
 // cycle as shared memory delivers); d = 256 keeps TN = 64 because a 128-column S does not fit next to its accumulator.
+// BCE (rp_bce_head_*), G = sigmoid(x) masked to the live columns, no exponent offsets:
+// MODE 3: rows = tokens, the fused pass's split grid: row sums of softplus, dH~ = sum_i G E_i; without column splits
+//         d_hc = (dH~ - E[y]) / T_v and the row losses are final (direct.d_hc / direct.row_loss); else partials, zpart
+// MODE 4: rows = items (COLCONST), columns = the valid tokens: dE = G . Hc / T_v, d_bias = row sums of G / T_v, the bias of
+//         the item row inside the sigmoid
 template <int KCH, int NSTAGE, int TN, int MODE, bool HAS_BIAS>
 __global__ void __launch_bounds__(kThreads, 1)
 ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -317,8 +368,9 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
               const int32_t* __restrict__ n_valid_ptr, int n_items, const float* __restrict__ bias,
               float* __restrict__ d_bias, void* __restrict__ out, const int32_t* __restrict__ safe_flag, int run_if_safe,
               int n_splits, int capacity, float* __restrict__ zpart, const CeDirect direct) {
-  constexpr bool COLCONST = (MODE == 1);
-  constexpr bool FUSED = (MODE == 2);
+  constexpr bool BCE = (MODE >= 3);
+  constexpr bool COLCONST = (MODE == 1 || MODE == 4);
+  constexpr bool FUSED = (MODE == 2 || MODE == 3);
   constexpr int D = KCH * 64;
   constexpr int kChunkB = TN * 128;       // bytes of one [TN rows x 64 bf16] swizzled chunk of a column tile
   constexpr int kStage = KCH * kChunkB;   // one column tile in shared memory
@@ -378,11 +430,16 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     crow_a = (r0 + rla < n_valid) ? cvec[r0 + rla] : -INFINITY;
     crow_b = (r0 + rlb < n_valid) ? cvec[r0 + rlb] : -INFINITY;
   }
-  if (FUSED) {
+  if (FUSED && !BCE) {
     crow_a = (r0 + rla < n_valid) ? (direct.use_lse_off ? -direct.lse[r0 + rla] * kLog2e : 0.f) : -INFINITY;
     crow_b = (r0 + rlb < n_valid) ? (direct.use_lse_off ? -direct.lse[r0 + rlb] * kLog2e : 0.f) : -INFINITY;
   }
-  float za = 0.f, zb = 0.f;   // FUSED: row sums of G~; COLCONST with bias: row sums of G (bias gradient)
+  float brow_a = 0.f, brow_b = 0.f;   // MODE 4: bias of this thread's item rows
+  if (BCE && COLCONST && HAS_BIAS) {
+    brow_a = r0 + rla < n_items ? __ldg(bias + r0 + rla) : 0.f;
+    brow_b = r0 + rlb < n_items ? __ldg(bias + r0 + rlb) : 0.f;
+  }
+  float za = 0.f, zb = 0.f;   // FUSED: row sums of G~ (BCE: of softplus); COLCONST with bias: row sums of G (bias gradient)
   float acc[D / 2];
   acc_zero(acc);
   mbar_wait(&bar_a, 0);
@@ -405,34 +462,75 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     // G = exp2(S log2e + offset) -> bf16 A fragments
     const int col0 = c_begin + jl * TN + fc;
     uint32_t pk[TN / 4];
+    if constexpr (BCE) {
+      // G = sigmoid(S + b) on the live columns (items before the split end / valid tokens), 0 elsewhere
+      float pa = 1.f, pb = 1.f;   // MODE 3: products of (1 + e) over this tile's live columns
 #pragma unroll
-    for (int q = 0; q < TN / 8; ++q) {
-      float g[4];
+      for (int q = 0; q < TN / 8; ++q) {
+        float g[4];
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int col = col0 + 8 * q + e;
-        float va = sacc[4 * q + e], vb = sacc[4 * q + 2 + e];
-        if (COLCONST) {
-          const float cc = __ldg(cvec + col);   // -inf beyond the valid tokens (the buffer is padded to 128 rows)
-          g[e] = ex2f(fmaf(va, kLog2e, cc));
-          g[2 + e] = ex2f(fmaf(vb, kLog2e, cc));
-        } else {
+        for (int e = 0; e < 2; ++e) {
+          const int col = col0 + 8 * q + e;
           const bool in = col < c_end;
-          if (HAS_BIAS && in) {
-            const float bb = __ldg(bias + col);
-            va += bb;
+          float va = sacc[4 * q + e], vb = sacc[4 * q + 2 + e];
+          if (HAS_BIAS) {
+            const float ba = COLCONST ? brow_a : (in ? __ldg(bias + col) : 0.f);
+            const float bb = COLCONST ? brow_b : ba;
+            va += ba;
             vb += bb;
           }
-          g[e] = in ? ex2f(fmaf(va, kLog2e, crow_a)) : 0.f;
-          g[2 + e] = in ? ex2f(fmaf(vb, kLog2e, crow_b)) : 0.f;
+          float oa, ob;
+          const float sa = bce_sigmoid(va, oa), sb = bce_sigmoid(vb, ob);
+          g[e] = in ? sa : 0.f;
+          g[2 + e] = in ? sb : 0.f;
+          if (FUSED) {
+            za += in ? fmaxf(va, 0.f) : 0.f;
+            zb += in ? fmaxf(vb, 0.f) : 0.f;
+            pa *= in ? oa : 1.f;
+            pb *= in ? ob : 1.f;
+          }
         }
+        if (COLCONST && HAS_BIAS) {
+          za += g[0] + g[1];
+          zb += g[2] + g[3];
+        }
+        pk[2 * q] = pack_bf16(g[0], g[1]);
+        pk[2 * q + 1] = pack_bf16(g[2], g[3]);
       }
-      if (FUSED || (COLCONST && HAS_BIAS)) {
-        za += g[0] + g[1];
-        zb += g[2] + g[3];
+      if (FUSED) {
+        za += __log2f(pa) * kLn2;
+        zb += __log2f(pb) * kLn2;
       }
-      pk[2 * q] = pack_bf16(g[0], g[1]);
-      pk[2 * q + 1] = pack_bf16(g[2], g[3]);
+    } else {
+#pragma unroll
+      for (int q = 0; q < TN / 8; ++q) {
+        float g[4];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = col0 + 8 * q + e;
+          float va = sacc[4 * q + e], vb = sacc[4 * q + 2 + e];
+          if (COLCONST) {
+            const float cc = __ldg(cvec + col);   // -inf beyond the valid tokens (the buffer is padded to 128 rows)
+            g[e] = ex2f(fmaf(va, kLog2e, cc));
+            g[2 + e] = ex2f(fmaf(vb, kLog2e, cc));
+          } else {
+            const bool in = col < c_end;
+            if (HAS_BIAS && in) {
+              const float bb = __ldg(bias + col);
+              va += bb;
+              vb += bb;
+            }
+            g[e] = in ? ex2f(fmaf(va, kLog2e, crow_a)) : 0.f;
+            g[2 + e] = in ? ex2f(fmaf(vb, kLog2e, crow_b)) : 0.f;
+          }
+        }
+        if (FUSED || (COLCONST && HAS_BIAS)) {
+          za += g[0] + g[1];
+          zb += g[2] + g[3];
+        }
+        pk[2 * q] = pack_bf16(g[0], g[1]);
+        pk[2 * q + 1] = pack_bf16(g[2], g[3]);
+      }
     }
     wg_fence();
 #pragma unroll
@@ -465,7 +563,62 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   const int row = t, slot = wg;
   const int r = r0 + row;
   const float* arow = stage + row * PITCH + slot * DW;
-  if (COLCONST) {
+  if constexpr (BCE) {
+    const float inv_n = n_valid > 0 ? 1.f / (float)n_valid : 0.f;
+    if (COLCONST) {
+      // dE = G^T-part / T_v and d_bias = sum_t sigmoid / T_v; the one-hot part follows in ce_label_scatter_kernel
+      if (r < n_items) {
+        if (HAS_BIAS && slot == 0) d_bias[r] = s_row[row] * inv_n;
+        float4* dst = reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + (size_t)r * D + slot * DW);
+#pragma unroll 4
+        for (int c = 0; c < DW; c += 4) {
+          const float4 v = *reinterpret_cast<const float4*>(arow + c);
+          dst[c >> 2] = make_float4(v.x * inv_n, v.y * inv_n, v.z * inv_n, v.w * inv_n);
+        }
+      }
+    } else if (direct.d_hc != nullptr) {
+      // no column splits: dH = (sum_i sigmoid_i E_i - E[y]) / T_v, row loss = sum_i softplus - x_y
+      const bool live = r < n_valid;
+      const int y = live ? labels[r] : 0;
+      float dot = 0.f;
+      if (live) {
+        const uint4* ey = reinterpret_cast<const uint4*>(table + (size_t)y * D + slot * DW);
+        const uint4* hr = reinterpret_cast<const uint4*>(a_rows + (size_t)r * D + slot * DW);
+        uint4* dst = reinterpret_cast<uint4*>(direct.d_hc + (size_t)r * D + slot * DW);
+#pragma unroll 4
+        for (int q = 0; q < DW / 8; ++q) {
+          const uint4 e = __ldg(ey + q), hh = __ldg(hr + q);
+          const __nv_bfloat162* e2 = reinterpret_cast<const __nv_bfloat162*>(&e);
+          const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&hh);
+          uint4 w;
+          uint32_t* w32 = reinterpret_cast<uint32_t*>(&w);
+#pragma unroll
+          for (int pp = 0; pp < 4; ++pp) {
+            const float2 ef = __bfloat1622float2(e2[pp]), hf = __bfloat1622float2(h2[pp]);
+            dot = fmaf(hf.x, ef.x, fmaf(hf.y, ef.y, dot));
+            w32[pp] = pack_bf16((arow[8 * q + 2 * pp] - ef.x) * inv_n, (arow[8 * q + 2 * pp + 1] - ef.y) * inv_n);
+          }
+          dst[q] = w;
+        }
+      }
+      s_dot[slot][row] = dot;
+      named_bar_sync(1, 256);
+      if (slot == 0 && live) {
+        float zy = s_dot[0][row] + s_dot[1][row];
+        if (HAS_BIAS) zy += bias[y];
+        direct.row_loss[r] = s_row[row] - zy;
+      }
+    } else {
+      // partial (this column split) sums; bce_finalize_kernel reduces the splits in a fixed order
+      float* o = reinterpret_cast<float*>(out) + (size_t)split * capacity * D;
+      if (r < n_valid) {
+        if (slot == 0) zpart[(size_t)split * capacity + r] = s_row[row];
+        float4* dst = reinterpret_cast<float4*>(o + (size_t)r * D + slot * DW);
+#pragma unroll 4
+        for (int c = 0; c < DW; c += 4) dst[c >> 2] = *reinterpret_cast<const float4*>(arow + c);
+      }
+    }
+  } else if (COLCONST) {
     float* o = reinterpret_cast<float*>(out);
     // biased head: G carries a per-item factor e^{b_i}; it was left out of the loop and is applied to the row here
     const float rs = (HAS_BIAS && r < n_items) ? __expf(bias[r]) : 1.f;
@@ -785,6 +938,88 @@ __global__ void ce_dh_reduce_kernel(const float* __restrict__ part, int n_splits
   }
 }
 
+// BCE: reduce the column splits.  zrow: softplus row sums, element (t, p) at zrow[p * zsp + t * zst]; loss_out (if given)
+// = {mean_t (sum_p zrow - x_t,y), 1 / T_v}, deterministic (fixed partition, the last block adds the block sums in order).
+// part_dh (if given): the fused pass's split partials of sum_i sigmoid_ti E_i -> d_hc[t] = (sum_p part_dh[p][t] - E[y]) / T_v.
+__global__ void bce_finalize_kernel(const float* __restrict__ zrow, long long zsp, int zst, const float* __restrict__ part_dh,
+                                    int n_splits, const __nv_bfloat16* __restrict__ hc, const __nv_bfloat16* __restrict__ table,
+                                    const int32_t* __restrict__ labels, const float* __restrict__ bias,
+                                    const int32_t* __restrict__ n_valid_ptr, int capacity, int d,
+                                    __nv_bfloat16* __restrict__ d_hc, float* __restrict__ block_sums,
+                                    unsigned int* __restrict__ ticket, float* __restrict__ loss_out) {
+  const int n_valid = *n_valid_ptr;
+  const float inv_n = n_valid > 0 ? 1.f / (float)n_valid : 0.f;
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  float local = 0.f;
+  for (int t = blockIdx.x * wpb + (threadIdx.x >> 5); t < n_valid; t += gridDim.x * wpb) {
+    const int y = labels[t];
+    const __nv_bfloat16* er = table + (size_t)y * d;
+    if (loss_out) {
+      float z = 0.f;
+      for (int p = lane; p < n_splits; p += 32) z += zrow[(size_t)p * zsp + (size_t)t * zst];
+      const __nv_bfloat16* hr = hc + (size_t)t * d;
+      float dot = 0.f;
+      for (int c = lane * 2; c < d; c += 64) {
+        const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(hr + c));
+        const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(er + c));
+        dot = fmaf(a.x, b.x, fmaf(a.y, b.y, dot));
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        z += __shfl_xor_sync(0xffffffffu, z, o);
+        dot += __shfl_xor_sync(0xffffffffu, dot, o);
+      }
+      if (bias) dot += bias[y];
+      if (lane == 0) local += z - dot;
+    }
+    if (d_hc) {
+      for (int c = lane * 4; c < d; c += 128) {
+        const uint2 eraw = *reinterpret_cast<const uint2*>(er + c);
+        const float2 e0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&eraw.x));
+        const float2 e1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&eraw.y));
+        float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 8
+        for (int p = 0; p < n_splits; ++p) {
+          const float4 v = __ldg(reinterpret_cast<const float4*>(part_dh + ((size_t)p * capacity + t) * d + c));
+          a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w;
+        }
+        uint2 o;
+        o.x = pack_bf16((a.x - e0.x) * inv_n, (a.y - e0.y) * inv_n);
+        o.y = pack_bf16((a.z - e1.x) * inv_n, (a.w - e1.y) * inv_n);
+        *reinterpret_cast<uint2*>(d_hc + (size_t)t * d + c) = o;
+      }
+    }
+  }
+  if (!loss_out) return;
+  __shared__ float red[32];
+  __shared__ bool last;
+  if (lane == 0) red[threadIdx.x >> 5] = local;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int i = 0; i < wpb; ++i) s += red[i];
+    block_sums[blockIdx.x] = s;
+    __threadfence();
+    last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
+  }
+  __syncthreads();
+  if (last && threadIdx.x == 0) {
+    __threadfence();
+    float s = 0.f;
+    for (int i = 0; i < (int)gridDim.x; ++i) s += reinterpret_cast<volatile float*>(block_sums)[i];
+    loss_out[0] = s * inv_n;
+    loss_out[1] = inv_n;
+  }
+}
+
+// BCE at d = 512: per-row exponent offsets of rp_gemm's sigmoid epilogue (act 4): log2(1 / T_v) on the valid rows, -inf past
+// them, so G = sigmoid / T_v there and exactly 0 on stale rows
+__global__ void bce_row_offset_kernel(const int32_t* __restrict__ n_valid_ptr, int capacity, float* __restrict__ off) {
+  const int n_valid = *n_valid_ptr;
+  const float l = n_valid > 0 ? -log2f((float)n_valid) : 0.f;
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < capacity; t += gridDim.x * blockDim.x) off[t] = t < n_valid ? l : -INFINITY;
+}
+
 // d = 512: the [128 x 512] fp32 gradient accumulator does not fit the registers of the two warpgroups, so the backward
 // materialises the softmax numerators G (bf16) for a chunk of tokens at a time and runs three plain GEMMs per chunk.
 // Chunk rows: as many as fit the G budget (RP_CE_WIDE_G_BYTES, default 8 GiB), multiple of 128.
@@ -865,12 +1100,12 @@ RP_API size_t rp_ce_head_workspace(int capacity_tokens, int n_items, int d) {
   return ce_ws_bytes(capacity_tokens, n_items, d);
 }
 
-template <int KCH, int NSTAGE>
+template <int KCH, int NSTAGE, bool BCE = false>
 static int launch_ce_fwd(const CUtensorMap& tmA, const CUtensorMap& tmB, const int32_t* n_valid, int n_items,
                          int n_splits, int n_tok_tiles, const float* bias, float2* part, const int32_t* skip,
                          cudaStream_t stream) {
   const int smem = (KCH + NSTAGE) * kChunk + 1024;
-  auto kern = ce_fwd_kernel<KCH, NSTAGE>;
+  auto kern = ce_fwd_kernel<KCH, NSTAGE, BCE>;
   RP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   kern<<<n_tok_tiles * n_splits, kThreads, smem, stream>>>(tmA, tmB, n_valid, n_items, n_splits, bias, part, skip);
   RP_LAUNCH_CHECK();
@@ -917,6 +1152,26 @@ static int dispatch_ce_bwd(int d, const CUtensorMap& tmA, const void* b_mat, int
     case 256:
       return launch_ce_bwd<4, 4, 64, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
                                        safe_flag, run_if_safe, n_splits, capacity, zpart, stream, direct);
+    default:
+      return RP_ESHAPE;
+  }
+}
+
+// The BCE token pass (MODE 3) keeps softplus's product and max terms beside the sigmoid: with 128-column tiles at d = 128 it
+// spills, so there it walks 64-column tiles with a ring twice as deep.  The dE pass (MODE 4) uses dispatch_ce_bwd's table.
+static int dispatch_bce_rows(int d, const CUtensorMap& tmA, const void* table, int n_items, const void* hc, const int32_t* labels,
+                             const int32_t* n_valid, const float* bias, float* part_dh, int grid, int n_splits, int capacity,
+                             float* zpart, cudaStream_t stream, const CeDirect& direct) {
+  switch (d) {
+    case 64:
+      return launch_ce_bwd<1, 8, 128, 3>(tmA, table, n_items, hc, nullptr, labels, table, nullptr, n_valid, n_items, bias, nullptr,
+                                         part_dh, grid, nullptr, 0, n_splits, capacity, zpart, stream, direct);
+    case 128:
+      return launch_ce_bwd<2, 8, 64, 3>(tmA, table, n_items, hc, nullptr, labels, table, nullptr, n_valid, n_items, bias, nullptr,
+                                        part_dh, grid, nullptr, 0, n_splits, capacity, zpart, stream, direct);
+    case 256:
+      return launch_ce_bwd<4, 4, 64, 3>(tmA, table, n_items, hc, nullptr, labels, table, nullptr, n_valid, n_items, bias, nullptr,
+                                        part_dh, grid, nullptr, 0, n_splits, capacity, zpart, stream, direct);
     default:
       return RP_ESHAPE;
   }
@@ -1136,6 +1391,167 @@ RP_API int rp_ce_head_bwd(const void* hc, const void* table, const float* bias, 
   if (rc != RP_OK) return rc;
   ce_label_scatter_kernel<<<sm_count() * 4, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(hc), labels, loss_inv,
                                                                n_valid, d, d_table, d_bias, roww);
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- BCE head
+static int check_bce_args(const void* hc, const void* table, const float* bias, const int32_t* labels, const int32_t* n_valid,
+                          int capacity, int n_items, int d, const float* loss_out, void* workspace, size_t workspace_bytes) {
+  if (!hc || !table || !labels || !n_valid || !loss_out || !workspace) return RP_EINVAL;
+  if (capacity <= 0 || n_items <= 0) return RP_ESHAPE;
+  if (d != 64 && d != 128 && d != 256 && d != 512) return RP_ESHAPE;
+  if (d == 512 && bias) return RP_ESHAPE;   // the biased head at d = 512 is not built
+  if (workspace_bytes < ce_ws_bytes(capacity, n_items, d)) return RP_EWORKSPACE;
+  return RP_OK;
+}
+
+// the token-major BCE pass (MODE 3) over the catalog: d_hc, and the row losses when `loss_out` is given.  Without column
+// splits both come out of the pass itself; otherwise bce_finalize_kernel reduces the split partials.
+static int bce_rows_pass(const void* hc, const void* table, const float* bias, const int32_t* labels, const int32_t* n_valid,
+                         int capacity, int n_items, int d, float* loss_out, void* d_hc, int n_valid_hint, const CeWs& ws,
+                         cudaStream_t stream) {
+  const int n_tok_tiles = (capacity + kT - 1) / kT, n_item_tiles = (n_items + kT - 1) / kT;
+  const int hint_tiles = (n_valid_hint > 0 && n_valid_hint <= capacity) ? (n_valid_hint + kT - 1) / kT : n_tok_tiles;
+  CUtensorMap tmA;
+  int rc;
+  if ((rc = make_tmap_bf16(&tmA, hc, capacity, d, d, 128)) != RP_OK) return rc;
+  const int P = pick_splits(hint_tiles, n_item_tiles);
+  CeDirect direct{nullptr, nullptr, nullptr, nullptr, CeRowOpts{nullptr, nullptr, 0, 0.f, 0.f}, 0};
+  if (P == 1) {
+    direct.d_hc = reinterpret_cast<__nv_bfloat16*>(d_hc);
+    direct.row_loss = ws.zpart;
+  }
+  rc = dispatch_bce_rows(d, tmA, table, n_items, hc, labels, n_valid, bias, ws.part_dh, n_tok_tiles * P, P, capacity, ws.zpart,
+                         stream, direct);
+  if (rc != RP_OK) return rc;
+  if (P == 1) {
+    if (loss_out) {
+      ce_loss_reduce_kernel<<<1, 1024, 0, stream>>>(ws.zpart, n_valid, nullptr, loss_out, 0);
+      RP_LAUNCH_CHECK();
+    }
+    return RP_OK;
+  }
+  int blocks = (capacity + 7) / 8;
+  if (blocks > 1024) blocks = 1024;
+  bce_finalize_kernel<<<blocks, 256, 0, stream>>>(ws.zpart, capacity, 1, ws.part_dh, P, reinterpret_cast<const __nv_bfloat16*>(hc),
+                                                  reinterpret_cast<const __nv_bfloat16*>(table), labels, bias, n_valid, capacity, d,
+                                                  reinterpret_cast<__nv_bfloat16*>(d_hc), ws.block_sums, ws.ticket, loss_out);
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+// Forward of the full-catalog BCE head: loss_out fp32 [2] = {sum_t [sum_i softplus(x_ti) - x_t,y_t] / T_v, 1 / T_v}.  Buffers
+// as rp_ce_head_fwd (workspace: rp_ce_head_workspace).  d_hc != NULL (d <= 256): one fused pass also writes the final d_hc.
+RP_API int rp_bce_head_fwd(const void* hc, const void* table, const float* bias, const int32_t* labels, const int32_t* n_valid,
+                           int capacity, int n_items, int d, float* loss_out, void* d_hc, int n_valid_hint, void* workspace,
+                           size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  int rc = check_bce_args(hc, table, bias, labels, n_valid, capacity, n_items, d, loss_out, workspace, workspace_bytes);
+  if (rc != RP_OK) return rc;
+  CeWs ws = ce_ws(workspace, capacity, d);
+  RP_CUDA_CHECK(cudaMemsetAsync(ws.ticket, 0, 4, stream));
+  if (d_hc != nullptr && d <= 256) return bce_rows_pass(hc, table, bias, labels, n_valid, capacity, n_items, d, loss_out, d_hc,
+                                                        n_valid_hint, ws, stream);
+  // un-fused: softplus row sums per (row, split), then the loss
+  const int n_tok_tiles = (capacity + kT - 1) / kT, n_item_tiles = (n_items + kT - 1) / kT;
+  const int hint_tiles = (n_valid_hint > 0 && n_valid_hint <= capacity) ? (n_valid_hint + kT - 1) / kT : n_tok_tiles;
+  const int P = pick_splits(hint_tiles, n_item_tiles);   // <= kMaxSplits: the partials live in ws.zpart
+  CUtensorMap tmA, tmB;
+  if ((rc = make_tmap_bf16(&tmA, hc, capacity, d, d, 128)) != RP_OK) return rc;
+  if ((rc = make_tmap_bf16(&tmB, table, n_items, d, d, 128)) != RP_OK) return rc;
+  float2* zrow = reinterpret_cast<float2*>(ws.zpart);
+  switch (d) {
+    case 64: rc = launch_ce_fwd<1, 8, true>(tmA, tmB, n_valid, n_items, P, n_tok_tiles, bias, zrow, nullptr, stream); break;
+    case 128: rc = launch_ce_fwd<2, 8, true>(tmA, tmB, n_valid, n_items, P, n_tok_tiles, bias, zrow, nullptr, stream); break;
+    case 256: rc = launch_ce_fwd<4, 8, true>(tmA, tmB, n_valid, n_items, P, n_tok_tiles, bias, zrow, nullptr, stream); break;
+    default: rc = launch_ce_fwd<8, 5, true>(tmA, tmB, n_valid, n_items, P, n_tok_tiles, bias, zrow, nullptr, stream); break;
+  }
+  if (rc != RP_OK) return rc;
+  int blocks = (capacity + 7) / 8;
+  if (blocks > 1024) blocks = 1024;
+  bce_finalize_kernel<<<blocks, 256, 0, stream>>>(ws.zpart, 1, P, nullptr, P, reinterpret_cast<const __nv_bfloat16*>(hc),
+                                                  reinterpret_cast<const __nv_bfloat16*>(table), labels, bias, n_valid, capacity, d,
+                                                  nullptr, ws.block_sums, ws.ticket, loss_out);
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+// Backward of rp_bce_head_fwd for d(loss) = 1 (same workspace): d_hc bf16 [capacity, d] (rows < *n_valid; already final when
+// the forward ran fused, `fused` != 0), d_table fp32 [n_items, d] and d_bias fp32 [n_items] (iff bias) OVERWRITTEN with
+// (sigmoid - onehot)^T . hc / T_v and its column sums.  d = 512 (no bias): sigmoid / T_v of a token chunk is materialised in
+// bf16 (rp_gemm act 4) and three GEMMs per chunk produce dH and dE, as rp_ce_head_bwd does.
+RP_API int rp_bce_head_bwd(const void* hc, const void* table, const float* bias, const int32_t* labels, const int32_t* n_valid,
+                           int capacity, int n_items, int d, const float* loss_out, void* d_hc, float* d_table, float* d_bias,
+                           int fused, int n_valid_hint, void* workspace, size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  int rc = check_bce_args(hc, table, bias, labels, n_valid, capacity, n_items, d, loss_out, workspace, workspace_bytes);
+  if (rc != RP_OK) return rc;
+  if (!d_hc || !d_table || (bias == nullptr) != (d_bias == nullptr)) return RP_EINVAL;
+  CeWs ws = ce_ws(workspace, capacity, d);
+  const float* loss_inv = loss_out + 1;
+  if (d == 512) {
+    const long long ldg = wide_ldg(n_items);
+    const int chunk = wide_chunk_rows(capacity, n_items);
+    uint8_t* G = reinterpret_cast<uint8_t*>(workspace) + (ce_ws_base_bytes(capacity, d) + 1023) / 1024 * 1024;
+    float* part = reinterpret_cast<float*>(G + (size_t)chunk * ldg * 2);
+    const long long part_stride = (long long)chunk * d;
+    const int hint = (n_valid_hint > 0 && n_valid_hint < capacity) ? n_valid_hint : capacity;
+    float* off = ws.roww;   // per-row exponent offsets of the sigmoid epilogue (the CE row weights are not used here)
+    bce_row_offset_kernel<<<(capacity + 255) / 256 < 1024 ? (capacity + 255) / 256 : 1024, 256, 0, stream>>>(n_valid, capacity, off);
+    RP_LAUNCH_CHECK();
+    for (int c0 = 0, it = 0; c0 < capacity; c0 += chunk, ++it) {
+      const int rows = (capacity - c0 < chunk) ? capacity - c0 : chunk;
+      rp_gemm_desc g;
+      memset(&g, 0, sizeof(g));
+      g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
+      // G [rows, n_items] = sigmoid(hc[c0:c0+rows] . E^T) / T_v, 0 on rows past T_v
+      g.A = reinterpret_cast<const __nv_bfloat16*>(hc) + (size_t)c0 * d; g.a_rows = rows; g.a_cols = d; g.lda = d; g.a_mn = 0;
+      g.B = table; g.b_rows = n_items; g.b_cols = d; g.ldb = d; g.b_mn = 0;
+      g.M = rows; g.N = n_items; g.K = d;
+      g.C = G; g.ldc = ldg; g.out_mode = 0; g.act = 4; g.row_exp2_offset = off + c0;
+      g.m_limit_dev = n_valid; g.m_limit_base = c0;
+      if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
+      // dH[c0:c0+rows] = G . E - E[y] / T_v   (split-K partials, reduced together with the label term)
+      int live = hint - c0;
+      live = live < 128 ? 128 : (live > rows ? rows : live);
+      int split = (2 * sm_count()) / (((live + 127) / 128) * (d / 128));
+      split = split < 1 ? 1 : (split > kWideSplitK ? kWideSplitK : split);
+      memset(&g, 0, sizeof(g));
+      g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = split;
+      g.A = G; g.a_rows = rows; g.a_cols = n_items; g.lda = ldg; g.a_mn = 0;
+      g.B = table; g.b_rows = n_items; g.b_cols = d; g.ldb = d; g.b_mn = 1;
+      g.M = rows; g.N = d; g.K = n_items;
+      g.C = part; g.ldc = d; g.out_mode = 3; g.c_split_stride = part_stride;
+      g.m_limit_dev = n_valid; g.m_limit_base = c0;
+      if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
+      ce_dh_reduce_kernel<<<sm_count() * 4, 256, 0, stream>>>(part, split, part_stride, rows, c0,
+                                                               reinterpret_cast<__nv_bfloat16*>(d_hc),
+                                                               reinterpret_cast<const __nv_bfloat16*>(table), labels, loss_inv,
+                                                               n_valid, d, nullptr);
+      RP_LAUNCH_CHECK();
+      // dE (+)= G^T . hc[c0:c0+rows]
+      memset(&g, 0, sizeof(g));
+      g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
+      g.A = G; g.a_rows = rows; g.a_cols = n_items; g.lda = ldg; g.a_mn = 1;
+      g.B = reinterpret_cast<const __nv_bfloat16*>(hc) + (size_t)c0 * d; g.b_rows = rows; g.b_cols = d; g.ldb = d; g.b_mn = 1;
+      g.M = n_items; g.N = d; g.K = rows;
+      g.C = d_table; g.ldc = d; g.out_mode = it == 0 ? 2 : 4;
+      g.k_limit_dev = n_valid; g.k_limit_base = c0;
+      if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
+    }
+  } else {
+    if (!fused && (rc = bce_rows_pass(hc, table, bias, labels, n_valid, capacity, n_items, d, nullptr, d_hc, n_valid_hint, ws,
+                                      stream)) != RP_OK)
+      return rc;
+    CUtensorMap tmE;
+    if ((rc = make_tmap_bf16(&tmE, table, n_items, d, d, 128)) != RP_OK) return rc;
+    rc = dispatch_ce_bwd<4>(d, tmE, hc, capacity, table, nullptr, labels, table, loss_inv, n_valid, n_items, bias, d_bias, d_table,
+                            (n_items + kT - 1) / kT, nullptr, 0, 1, capacity, nullptr, stream);
+    if (rc != RP_OK) return rc;
+  }
+  ce_label_scatter_kernel<<<sm_count() * 4, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(hc), labels, loss_inv,
+                                                               n_valid, d, d_table, d_bias, nullptr);
   RP_LAUNCH_CHECK();
   return RP_OK;
 }

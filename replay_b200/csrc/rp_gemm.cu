@@ -42,6 +42,7 @@ struct GemmParams {
   float post_drop_p;           // second dropout applied AFTER the residual add (BERT4Rec block output), 0 = off
   unsigned long long post_drop_offset;
   const float* row_exp2_offset;  // act 3: x = exp2(x * log2(e) + row_exp2_offset[m])   (softmax numerators from stored lse)
+                                 // act 4: x = sigmoid(x) * exp2(row_exp2_offset[m])   (BCE gradient / T_v, 0 past T_v)
   const int32_t* m_limit_dev;    // optional device scalar: rows m with m_limit_base + m >= *m_limit_dev are not computed
   int m_limit_base;
   const int32_t* k_limit_dev;    // optional device scalar: the contraction stops at *k_limit_dev - k_limit_base (whole 64-chunks)
@@ -59,6 +60,9 @@ struct EpiRow {
   unsigned long long seed_eff;
 };
 
+// SIGMOID: the act 4 epilogue (BCE head at d = 512) is compiled only into its own instantiation, so it costs the other
+// GEMMs no registers
+template <bool SIGMOID>
 __device__ __forceinline__ void gemm_epilogue_chunk(const GemmParams& p, const float* __restrict__ s_bias, const EpiRow& er,
                                                     const uint32_t (&raw)[32], int n0, int c) {
   const long long c_base = er.c_base;
@@ -91,6 +95,13 @@ __device__ __forceinline__ void gemm_epilogue_chunk(const GemmParams& p, const f
       } else if (p.act == 3) {
 #pragma unroll
         for (int q = 0; q < 32; ++q) x[q] = ex2f(fmaf(x[q], 1.4426950408889634f, er.exp_off));
+      } else if (SIGMOID && p.act == 4) {  // sigmoid(x) * 2^offset: (1 or e) / (1 + e) with e = exp(-|x|); offset -inf gives exactly 0
+        const float sc = ex2f(er.exp_off);
+#pragma unroll
+        for (int q = 0; q < 32; ++q) {
+          const float e = ex2f(-fabsf(x[q]) * 1.4426950408889634f);
+          x[q] = __fdividef(x[q] >= 0.f ? sc : e * sc, 1.f + e);
+        }
       }
       if (p.drop_p > 0.f) {
         const uint32_t rk = drop_row_key(seed_eff, p.drop_offset, (unsigned long long)er.drop_row);
@@ -197,7 +208,7 @@ __device__ __forceinline__ void gemm_epilogue_chunk(const GemmParams& p, const f
 // the epilogue (thread = output row, warpgroup = column half); warp 8: TMA producer.
 static constexpr int kGemmThreads = 288;
 
-template <int BN, bool A_MN, bool B_MN, int NSTAGE>
+template <int BN, bool A_MN, bool B_MN, int NSTAGE, bool SIGMOID = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   constexpr int A_BYTES = 128 * 128;       // [128 x 64] bf16
@@ -304,7 +315,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   er.c_base = c_base;
   er.drop_row = (long long)bz * p.M + m;
   er.rm = rm;
-  er.exp_off = (p.act == 3 && row_ok) ? p.row_exp2_offset[m] : 0.f;
+  er.exp_off = ((p.act == 3 || (SIGMOID && p.act == 4)) && row_ok) ? p.row_exp2_offset[m] : 0.f;
   er.keep_scale = p.drop_p > 0.f ? 1.f / (1.f - p.drop_p) : 1.f;
   er.drop_thr = p.drop_p > 0.f ? (uint32_t)(p.drop_p * 4294967296.0) : 0u;
   er.seed_eff = p.seed + ((p.drop_p > 0.f && p.seed_ptr) ? *p.seed_ptr : 0ull);
@@ -314,15 +325,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (n0 + c >= p.N) break;
     uint32_t raw[32];
     stage_ld32(stage + row * PITCH + c, raw);
-    gemm_epilogue_chunk(p, s_bias, er, raw, n0, c);
+    gemm_epilogue_chunk<SIGMOID>(p, s_bias, er, raw, n0, c);
   }
 }
 
-template <int BN, bool A_MN, bool B_MN, int NSTAGE>
+template <int BN, bool A_MN, bool B_MN, int NSTAGE, bool SIGMOID = false>
 static int launch_gemm_n(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, int batch, cudaStream_t st) {
   const int ring = NSTAGE * (128 * 128 + BN * 128), stage = 128 * (BN + 4) * 4;
   const int smem = (ring > stage ? ring : stage) + 1024;
-  auto kern = gemm_kernel<BN, A_MN, B_MN, NSTAGE>;
+  auto kern = gemm_kernel<BN, A_MN, B_MN, NSTAGE, SIGMOID>;
   RP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const long long ctas = (long long)((p.N + BN - 1) / BN) * ((p.M + 127) / 128) * p.split_k;
   if (ctas > 0x7fffffffll) return RP_ESHAPE;
@@ -369,14 +380,18 @@ RP_API int rp_gemm(const rp_gemm_desc* g, void* stream_) {
   p.row_exp2_offset = g->row_exp2_offset;
   p.m_limit_dev = g->m_limit_dev; p.m_limit_base = g->m_limit_base;
   p.k_limit_dev = g->k_limit_dev; p.k_limit_base = g->k_limit_base;
-  if (g->act == 3 && !g->row_exp2_offset) return RP_EINVAL;
+  if ((g->act == 3 || g->act == 4) && !g->row_exp2_offset) return RP_EINVAL;
   if (g->out_mode == 4 && g->split_k != 1) return RP_EINVAL;
   CUtensorMap tmA, tmB;
   int rc;
   // K-major operand: box [128 (or BN) rows x 64 cols]; MN-major operand: box [64 k-rows x 64 cols]
-  const int bn = (g->N <= 64) ? 64 : 128;
+  const int bn = (g->N <= 64 && g->act != 4) ? 64 : 128;
   if ((rc = make_tmap_bf16(&tmA, g->A, g->a_rows, g->a_cols, g->lda, g->a_mn ? 64 : 128)) != RP_OK) return rc;
   if ((rc = make_tmap_bf16(&tmB, g->B, g->b_rows, g->b_cols, g->ldb, g->b_mn ? 64 : bn)) != RP_OK) return rc;
+  if (g->act == 4) {   // sigmoid epilogue: one instantiation, K-major operands and 128-column tiles (BCE logit chunks)
+    if (g->a_mn || g->b_mn || g->split_k != 1) return RP_EINVAL;
+    return launch_gemm_n<128, false, false, 4, true>(tmA, tmB, p, g->batch, stream);
+  }
 #define RP_GEMM_CASE(BN_, AMN_, BMN_) return launch_gemm<BN_, AMN_, BMN_>(tmA, tmB, p, g->batch, stream)
   if (bn == 64) {
     if (!g->a_mn && !g->b_mn) RP_GEMM_CASE(64, false, false);

@@ -538,9 +538,10 @@ class SasRecEngine:
         # per-row variants of the full-catalog head (rp_ce_head_fwd_w): "ce_weighted" (LogOutCEWeighted / CEWeighted: sample
         # weights staged with set_row_weights) and "login_ce" (LogInCE); "ce" is the plain head
         self.ce_row = None
-        if kind in ("ce", "ce_weighted", "login_ce"):
+        self.bce = kind == "bce"   # full-catalog BCE (rp_bce_head_*, replay/nn/loss/bce.py:10-95) on the CE head's buffers
+        if kind in ("ce", "ce_weighted", "login_ce", "bce"):
             self.sampled = None
-            if kind != "ce":
+            if kind in ("ce_weighted", "login_ce"):
                 self.ce_row = dict(kind=1 if kind == "login_ce" else 0, log_eps=log_eps, clamp=clamp, weighted=(kind == "ce_weighted"))
                 if not hasattr(self, "in_roww") or self.in_roww.numel() < self.T:
                     self.in_roww = torch.ones(self.T, device=self.dev, dtype=torch.float32)
@@ -759,9 +760,12 @@ class SasRecEngine:
         if self.sampled is not None:
             check(self.lib.rp_sampled_head_fwd(ctypes.byref(self._sampled_desc()), self._stream()), "rp_sampled_head_fwd")
             return self.ce.loss
-        from .ops import ce_head_fwd
+        from .ops import bce_head_fwd, ce_head_fwd
 
         self.lib.count += 2
+        if getattr(self, "bce", False):
+            return bce_head_fwd(self.ce, self.hc, self.params16["item_emb"][: cfg.n_items], self.labels_c, self.n_valid,
+                                d_hc=self.s["dhc"] if self.fused_ce else None, n_valid_hint=self.n_valid_hint)
         row = getattr(self, "ce_row", None)
         roww = None
         if row is not None and row["weighted"]:   # weights of the valid targets in the head's compacted order
@@ -781,9 +785,13 @@ class SasRecEngine:
         drop = cfg.dropout
         ks = 1.0 / (1.0 - drop) if drop > 0 else 1.0
         st = self._stream
-        from .ops import ce_head_bwd
+        from .ops import bce_head_bwd, ce_head_bwd
 
-        if self.sampled is not None:
+        if getattr(self, "bce", False):
+            bce_head_bwd(self.ce, self.hc, p16["item_emb"][: cfg.n_items], self.labels_c, self.n_valid, s["dhc"], G["item_emb"],
+                         n_valid_hint=self.n_valid_hint)
+            self.lib.count += 3
+        elif self.sampled is not None:
             G["item_emb"].zero_()  # the sampled head accumulates sparse rows (the full-CE head overwrites the dense table)
             check(self.lib.rp_sampled_head_bwd(ctypes.byref(self._sampled_desc()), s["dhc"].data_ptr(), G["item_emb"].data_ptr(),
                                                st()), "rp_sampled_head_bwd")

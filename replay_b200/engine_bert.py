@@ -92,7 +92,7 @@ class Bert4RecEngine(SasRecEngine):
         self.params16 = {k: self.p16[o:o + math.prod(s)].view(s) for k, (o, s) in self.layout.items()}
         if with_grad:
             self._alloc_grad_state()
-        self.sampled, self._loss_args = None, None
+        self.sampled, self._loss_args, self.bce = None, None, False
         self.rng_counter = torch.zeros(1, device=self.dev, dtype=torch.int64)
         self.seed = seed & 0xFFFFFFFFFFFF
         self.fused_attn_bwd = (cfg.d // cfg.n_heads) == 64 and seq_len <= 256
@@ -277,8 +277,16 @@ class Bert4RecEngine(SasRecEngine):
         W16 = self.params16["item_emb"] if cfg.tying else self.params16["head_w"]
         return W16, self.params["head_b"]
 
+    def set_loss(self, kind: str = "ce", **kw):
+        """``"ce"`` (bert4rec/lightning.py:332-351) or ``"bce"`` (:273-305), both over the whole catalog through the biased /
+        tied head.  The sampled kinds stage SASRec's buffers and are not built here."""
+        if kind not in ("ce", "bce"):
+            raise NotImplementedError(f"Not supported loss_type {kind!r} for BERT4Rec")
+        self._loss_args = (kind, {})
+        self.sampled, self.bce = None, kind == "bce"
+
     def forward_train(self):
-        from .ops import ce_head_fwd
+        from .ops import bce_head_fwd, ce_head_fwd
 
         self._prepare(True)
         self._body_forward(True)
@@ -286,12 +294,13 @@ class Bert4RecEngine(SasRecEngine):
                                       self.cfg.d, self.hc.data_ptr(), 0, self._stream()), "rp_gather_rows")
         W16, bias = self._head()
         self.lib.count += 2
-        return ce_head_fwd(self.ce, self.hc, W16, self.labels_c, self.n_valid, bias=bias,
-                           d_hc=self.s["dhc"] if self.fused_ce else None, n_valid_hint=self.n_valid_hint)
+        head_fwd = bce_head_fwd if self.bce else ce_head_fwd
+        return head_fwd(self.ce, self.hc, W16, self.labels_c, self.n_valid, bias=bias,
+                        d_hc=self.s["dhc"] if self.fused_ce else None, n_valid_hint=self.n_valid_hint)
 
     # ------------------------------------------------------------------------------------------------ backward
     def backward(self):
-        from .ops import ce_head_bwd
+        from .ops import bce_head_bwd, ce_head_bwd
 
         cfg, T, d, L = self.cfg, self.T, self.cfg.d, self.L
         p16, prm, G, s = self.params16, self.params, self.grads, self.s
@@ -302,7 +311,8 @@ class Bert4RecEngine(SasRecEngine):
         st, rng = self._stream, self.rng_counter.data_ptr()
         W16, bias = self._head()
         dW = G["item_emb"] if cfg.tying else G["head_w"]
-        ce_head_bwd(self.ce, self.hc, W16, self.labels_c, self.n_valid, s["dhc"], dW, bias=bias, d_bias=G["head_b"])
+        head_bwd = bce_head_bwd if self.bce else ce_head_bwd
+        head_bwd(self.ce, self.hc, W16, self.labels_c, self.n_valid, s["dhc"], dW, bias=bias, d_bias=G["head_b"])
         self.lib.count += 3
         dx = s["dxa"]
         dx.zero_()

@@ -97,8 +97,17 @@ class _BertCore(SasRecCore):
                     out[prefix + "_head._item_embedder." + k[len("item_embedder."):]] = v
         return out
 
+    loss_kind = "ce"   # "ce" | "bce": the full-catalog head of every engine this core creates or resizes
+
+    def _apply_loss(self, eng):
+        if getattr(eng, "_loss_applied", None) != self.loss_kind:
+            eng.set_loss(self.loss_kind)
+            eng._loss_applied = self.loss_kind
+            self._drop_graphs()   # captured graphs launch the other head's kernels
+
     def loss(self, ids, pad_mask, token_mask, labels):
         eng = self.ensure_engine(*ids.shape, with_grad=True)
+        self._apply_loss(eng)
         eng.set_batch(ids, pad_mask, token_mask, labels)
         return _EngineLoss.apply(self.flat, self)
 
@@ -107,6 +116,7 @@ class _BertCore(SasRecCore):
         if self._shadow_dirty:
             eng.refresh_shadow(); self._shadow_dirty = False
         self._set_lr(eng, lr)
+        self._apply_loss(eng)
         eng.set_batch(ids, pad_mask, token_mask, labels)
         if isinstance(all_reduce, str):
             return self._graph_trainer(eng).run()[0]
@@ -183,12 +193,17 @@ class Bert4Rec(LightningModuleBase):
                  lr_scheduler_factory=None, fused_optimizer: bool = True, device=None):
         super().__init__()
         self.save_hyperparameters()
-        if loss_type != "CE" or loss_sample_count is not None:
+        # "CE_restricted" is the same CE over the same rows (bert4rec/lightning.py:379-391,475-489); sampled losses are not built
+        kind = {"CE": "ce", "CE_restricted": "ce", "BCE": "bce"}.get(loss_type)
+        if kind is None or loss_sample_count is not None:
             raise NotImplementedError("Not supported loss_type")
+        if kind == "bce" and hidden_size > 256:   # BERT4Rec's head always has a bias; the biased BCE head stops at d = 256
+            raise NotImplementedError("loss_type='BCE' is built for hidden_size <= 256")
         self._model = Bert4RecModel(tensor_schema, max_len=max_seq_len, hidden_size=hidden_size, num_blocks=block_count,
                                     num_heads=head_count, num_passes_over_block=pass_per_transformer_block_count,
                                     dropout=dropout_rate, enable_positional_embedding=enable_positional_embedding,
                                     enable_embedding_tying=enable_embedding_tying, device=device)
+        self._model.core.loss_kind = kind
         self._schema = tensor_schema
         self._optimizer_factory, self._lr_scheduler_factory = optimizer_factory, lr_scheduler_factory
         self._candidates_to_score = None

@@ -119,6 +119,33 @@ def ce_head_bwd(st: CEHeadState, hc, table, labels, n_valid, d_hc, d_table, bias
                                int(n_valid_hint), _ptr(st.ws), st.ws_bytes, _stream()), "rp_ce_head_bwd")
 
 
+def bce_head_fwd(st: CEHeadState, hc, table, labels, n_valid, bias=None, d_hc=None, n_valid_hint: int = 0):
+    """Full-catalog BCE (rp_bce_head_fwd) over the buffers of ``st``: loss = sum over the valid targets of
+    [sum_i softplus(logit_i) - logit_y] / n_valid.  Arguments as ce_head_fwd; with ``d_hc`` (d <= 256) the fused
+    forward + dH pass runs.  Returns st.loss (fp32 [2]: loss, 1/n_valid)."""
+    _need(hc, torch.bfloat16, "hc")
+    _need(table, torch.bfloat16, "table")
+    _need(labels, torch.int32, "labels")
+    _need(n_valid, torch.int32, "n_valid")
+    if d_hc is not None:
+        _need(d_hc, torch.bfloat16, "d_hc")
+    st.fused = d_hc is not None and st.d <= 256
+    check(lib().rp_bce_head_fwd(_ptr(hc), _ptr(table), _ptr(bias), _ptr(labels), _ptr(n_valid), st.capacity, st.n_items, st.d,
+                                _ptr(st.loss), _ptr(d_hc), int(n_valid_hint), _ptr(st.ws), st.ws_bytes, _stream()),
+          "rp_bce_head_fwd")
+    return st.loss
+
+
+def bce_head_bwd(st: CEHeadState, hc, table, labels, n_valid, d_hc, d_table, bias=None, d_bias=None, n_valid_hint: int = 0):
+    """Backward of bce_head_fwd: d_hc bf16 [capacity,d] (computed here unless the forward ran fused), d_table fp32
+    [>=I, d] and d_bias fp32 (iff bias) overwritten."""
+    _need(d_hc, torch.bfloat16, "d_hc")
+    _need(d_table, torch.float32, "d_table")
+    check(lib().rp_bce_head_bwd(_ptr(hc), _ptr(table), _ptr(bias), _ptr(labels), _ptr(n_valid), st.capacity, st.n_items, st.d,
+                                _ptr(st.loss), _ptr(d_hc), _ptr(d_table), _ptr(d_bias), int(getattr(st, "fused", False)),
+                                int(n_valid_hint), _ptr(st.ws), st.ws_bytes, _stream()), "rp_bce_head_bwd")
+
+
 def gemm(A, B, C, M, N, K, *, a_mn=False, b_mn=False, bias=None, act=0, residual=None, rowmask=None, drop_p=0.0,
          drop_offset=0, seed=0, seed_ptr=None, out_mode=0, split_k=1, gate=None, gate_scale=1.0, gate_mode=0, alpha=1.0,
          batch=1, inner=1, a_off=(0, 0, 0, 0, 0, 0), b_off=(0, 0, 0, 0, 0, 0), c_geom=None, rowmask_oo=0, C2=None,
