@@ -88,9 +88,10 @@ int rp_ce_head_fwd(const void* hc, const void* table, const float* bias, const i
  * `fused` != 0 and the bound held, otherwise computed here); d_table fp32 [n_items, d] is OVERWRITTEN (softmax part) and
  * then atomically corrected by the one-hot part; d_bias fp32 [n_items] likewise iff bias.  `fused` must equal
  * (d_hc != NULL) of the matching forward call and then needs the same workspace.  d in {64,128,256}: fused wgmma passes
- * (logits never leave the registers).  d = 512 (bias == NULL only): a [128 x 512] fp32 accumulator does not fit them, so
- * the softmax numerators of a token chunk are materialised in bf16 inside the workspace (chunk sized by RP_CE_WIDE_G_BYTES,
- * default 8 GiB) and three GEMMs per chunk produce dH and dE; the workspace is then always required.
+ * (logits never leave the registers).  d = 512: a [128 x 512] fp32 accumulator does not fit them, so the softmax numerators
+ * of a token chunk are materialised in bf16 inside the workspace (chunk sized by RP_CE_WIDE_G_BYTES, default 8 GiB) and
+ * three GEMMs per chunk produce dH and dE; with a bias, a fixed-order column sum of each chunk gives d_bias (bitwise
+ * reproducible).  The workspace is then always required.
  * n_valid_hint: host estimate of *n_valid (0 = unknown), load-balance only. */
 /* Per-row variants of the full-catalog head, single positive label per position:
  *   row_weight  fp32 [capacity], >= 0, in the compacted order of the valid targets (NULL = 1): loss = mean_t w_t ce_t
@@ -114,7 +115,7 @@ int rp_ce_head_bwd(const void* hc, const void* table, const float* bias, const i
  * The sigmoid is bounded: no log-sum-exp, no bound guard, no second pass.  d_hc (optional, d <= 256) enables the fused
  * forward + dH pass; loss and d_hc are bitwise reproducible.  The backward overwrites d_table (and d_bias iff bias) with
  * (sigmoid - onehot)^T . hc / T_v and its column sums; `fused` must equal (d_hc != NULL && d <= 256) of the forward.
- * d in {64,128,256} with or without bias, 512 without bias (materialised sigmoid chunks, rp_gemm act 4).  The BCE head reads
+ * d in {64,128,256,512} with or without bias (512: materialised sigmoid chunks, rp_gemm act 4).  The BCE head reads
  * bias entries < n_items only, so a bias of exactly n_items entries is enough here. */
 int rp_bce_head_fwd(const void* hc, const void* table, const float* bias, const int32_t* labels, const int32_t* n_valid,
                     int capacity, int n_items, int d, float* loss_out, void* d_hc, int n_valid_hint, void* workspace,

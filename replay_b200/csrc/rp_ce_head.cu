@@ -1020,6 +1020,61 @@ __global__ void bce_row_offset_kernel(const int32_t* __restrict__ n_valid_ptr, i
   for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < capacity; t += gridDim.x * blockDim.x) off[t] = t < n_valid ? l : -INFINITY;
 }
 
+// Biased head at d = 512: d_bias[i] = (first chunk) / += (later chunks) sum_t G[t, i] over the chunk's rows below *n_valid
+// (G already carries 1 / T_v; the one-hot part follows in ce_label_scatter_kernel).  Rows at or past *n_valid are not read:
+// the G GEMM skips whole row tiles there, which keep an earlier chunk's values.  A block owns 256 columns, a lane 8 of them
+// (one 16-byte load per row), the 8 warps take every 8th row and their sums are added in warp order: deterministic, no
+// atomics.  Columns >= n_items are never written (a lane's last vector may load a few; their sums are dropped).
+__global__ void __launch_bounds__(256) ce_bias_colsum_kernel(const __nv_bfloat16* __restrict__ G, long long ldg, int rows, int c0,
+                                                             const int32_t* __restrict__ n_valid_ptr, int n_items,
+                                                             float* __restrict__ d_bias, int accumulate) {
+  __shared__ float part[8][256];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int col0 = blockIdx.x * 256 + lane * 8;
+  int n = *n_valid_ptr - c0;
+  n = n < 0 ? 0 : (n > rows ? rows : n);
+  float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  if (col0 < n_items) {   // col0 + 8 <= round_up(n_items, 8) <= ldg: the load stays inside the row
+    const __nv_bfloat16* g = G + col0;
+    int t = warp;
+    for (; t + 24 < n; t += 32) {   // four rows in flight per lane
+      uint4 v[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) v[u] = __ldg(reinterpret_cast<const uint4*>(g + (size_t)(t + 8 * u) * ldg));
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&v[u]);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float2 f = __bfloat1622float2(h2[q]);
+          acc[2 * q] += f.x;
+          acc[2 * q + 1] += f.y;
+        }
+      }
+    }
+    for (; t < n; t += 8) {
+      const uint4 v = __ldg(reinterpret_cast<const uint4*>(g + (size_t)t * ldg));
+      const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&v);
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const float2 f = __bfloat1622float2(h2[q]);
+        acc[2 * q] += f.x;
+        acc[2 * q + 1] += f.y;
+      }
+    }
+  }
+#pragma unroll
+  for (int q = 0; q < 8; ++q) part[warp][lane * 8 + q] = acc[q];
+  __syncthreads();
+  const int c = blockIdx.x * 256 + threadIdx.x;
+  if (c < n_items) {
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) s += part[w][threadIdx.x];
+    d_bias[c] = accumulate ? d_bias[c] + s : s;
+  }
+}
+
 // d = 512: the [128 x 512] fp32 gradient accumulator does not fit the registers of the two warpgroups, so the backward
 // materialises the softmax numerators G (bf16) for a chunk of tokens at a time and runs three plain GEMMs per chunk.
 // Chunk rows: as many as fit the G budget (RP_CE_WIDE_G_BYTES, default 8 GiB), multiple of 128.
@@ -1303,7 +1358,7 @@ RP_API int rp_ce_head_fwd_w(const void* hc, const void* table, const float* bias
 //          device-side bound held); otherwise computed here from the stored lse.  d = 512: chunked materialised-G path
 //          (three GEMMs per token chunk, see wide_chunk_rows), workspace required
 //   d_table fp32 [n_items, d]  OVERWRITTEN with softmax^T . hc / T_v, then the one-hot part is atomically subtracted
-//   d_bias  fp32 [n_items] (iff bias)  OVERWRITTEN likewise.        d in {64,128,256}; 512 without bias.
+//   d_bias  fp32 [n_items] (iff bias)  OVERWRITTEN likewise.        d in {64,128,256,512}.
 RP_API int rp_ce_head_bwd(const void* hc, const void* table, const float* bias, const int32_t* labels,
                           const int32_t* n_valid, int capacity, int n_items, int d, const float* loss_out /* from fwd */,
                           const float* cvec /* from fwd */, void* d_hc, float* d_table, float* d_bias, int fused,
@@ -1317,8 +1372,7 @@ RP_API int rp_ce_head_bwd(const void* hc, const void* table, const float* bias, 
   // gradient weight per row, written by the forward (all ones for the plain CE head); without a workspace: plain head
   const float* roww = (workspace && workspace_bytes >= ce_ws_bytes(capacity, n_items, d)) ? ce_ws(workspace, capacity, d).roww : nullptr;
   if (d == 512) {
-    // ---- wide-hidden path: per token chunk  G = exp2((hc.E^T + b) log2e + c_t)  ->  dH = G.E,  dE += G^T.hc
-    if (bias) return RP_ESHAPE;  // biased (BERT4Rec) head at d = 512 is not built
+    // ---- wide-hidden path: per token chunk  G = exp2((hc.E^T + b) log2e + c_t)  ->  dH = G.E,  dE += G^T.hc,  db += colsum G
     const long long ldg = wide_ldg(n_items);
     const int chunk = wide_chunk_rows(capacity, n_items);
     uint8_t* G = reinterpret_cast<uint8_t*>(workspace) + (ce_ws_base_bytes(capacity, d) + 1023) / 1024 * 1024;
@@ -1331,13 +1385,18 @@ RP_API int rp_ce_head_bwd(const void* hc, const void* table, const float* bias, 
       rp_gemm_desc g;
       memset(&g, 0, sizeof(g));
       g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
-      // G [rows, n_items] = exp2((hc[c0:c0+rows] . E^T) log2e + cvec)
+      // G [rows, n_items] = exp2((hc[c0:c0+rows] . E^T + b) log2e + cvec)   (the epilogue adds the bias before the act)
       g.A = reinterpret_cast<const __nv_bfloat16*>(hc) + (size_t)c0 * d; g.a_rows = rows; g.a_cols = d; g.lda = d; g.a_mn = 0;
       g.B = table; g.b_rows = n_items; g.b_cols = d; g.ldb = d; g.b_mn = 0;
       g.M = rows; g.N = n_items; g.K = d;
-      g.C = G; g.ldc = ldg; g.out_mode = 0; g.act = 3; g.row_exp2_offset = cvec + c0;
+      g.C = G; g.ldc = ldg; g.out_mode = 0; g.act = 3; g.row_exp2_offset = cvec + c0; g.bias = bias;
       g.m_limit_dev = n_valid; g.m_limit_base = c0;
       if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
+      if (bias) {
+        ce_bias_colsum_kernel<<<(n_items + 255) / 256, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(G), ldg, rows, c0,
+                                                                         n_valid, n_items, d_bias, it != 0);
+        RP_LAUNCH_CHECK();
+      }
       // dH[c0:c0+rows] = G . E - onehot   (A = G K-major over the items, B = E read MN-major).  Few row tiles against a
       // contraction over the whole catalog: split-K partials (fp32, deterministic), reduced together with the label term
       int live = hint - c0;
@@ -1401,7 +1460,6 @@ static int check_bce_args(const void* hc, const void* table, const float* bias, 
   if (!hc || !table || !labels || !n_valid || !loss_out || !workspace) return RP_EINVAL;
   if (capacity <= 0 || n_items <= 0) return RP_ESHAPE;
   if (d != 64 && d != 128 && d != 256 && d != 512) return RP_ESHAPE;
-  if (d == 512 && bias) return RP_ESHAPE;   // the biased head at d = 512 is not built
   if (workspace_bytes < ce_ws_bytes(capacity, n_items, d)) return RP_EWORKSPACE;
   return RP_OK;
 }
@@ -1479,8 +1537,9 @@ RP_API int rp_bce_head_fwd(const void* hc, const void* table, const float* bias,
 
 // Backward of rp_bce_head_fwd for d(loss) = 1 (same workspace): d_hc bf16 [capacity, d] (rows < *n_valid; already final when
 // the forward ran fused, `fused` != 0), d_table fp32 [n_items, d] and d_bias fp32 [n_items] (iff bias) OVERWRITTEN with
-// (sigmoid - onehot)^T . hc / T_v and its column sums.  d = 512 (no bias): sigmoid / T_v of a token chunk is materialised in
-// bf16 (rp_gemm act 4) and three GEMMs per chunk produce dH and dE, as rp_ce_head_bwd does.
+// (sigmoid - onehot)^T . hc / T_v and its column sums.  d = 512: sigmoid / T_v of a token chunk is materialised in bf16
+// (rp_gemm act 4, the bias inside the sigmoid) and three GEMMs per chunk produce dH and dE, as rp_ce_head_bwd does; with a
+// bias, ce_bias_colsum_kernel sums the chunk's columns into d_bias.
 RP_API int rp_bce_head_bwd(const void* hc, const void* table, const float* bias, const int32_t* labels, const int32_t* n_valid,
                            int capacity, int n_items, int d, const float* loss_out, void* d_hc, float* d_table, float* d_bias,
                            int fused, int n_valid_hint, void* workspace, size_t workspace_bytes, void* stream_) {
@@ -1505,13 +1564,18 @@ RP_API int rp_bce_head_bwd(const void* hc, const void* table, const float* bias,
       rp_gemm_desc g;
       memset(&g, 0, sizeof(g));
       g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
-      // G [rows, n_items] = sigmoid(hc[c0:c0+rows] . E^T) / T_v, 0 on rows past T_v
+      // G [rows, n_items] = sigmoid(hc[c0:c0+rows] . E^T + b) / T_v, 0 on rows past T_v
       g.A = reinterpret_cast<const __nv_bfloat16*>(hc) + (size_t)c0 * d; g.a_rows = rows; g.a_cols = d; g.lda = d; g.a_mn = 0;
       g.B = table; g.b_rows = n_items; g.b_cols = d; g.ldb = d; g.b_mn = 0;
       g.M = rows; g.N = n_items; g.K = d;
-      g.C = G; g.ldc = ldg; g.out_mode = 0; g.act = 4; g.row_exp2_offset = off + c0;
+      g.C = G; g.ldc = ldg; g.out_mode = 0; g.act = 4; g.row_exp2_offset = off + c0; g.bias = bias;
       g.m_limit_dev = n_valid; g.m_limit_base = c0;
       if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
+      if (bias) {
+        ce_bias_colsum_kernel<<<(n_items + 255) / 256, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(G), ldg, rows, c0,
+                                                                         n_valid, n_items, d_bias, it != 0);
+        RP_LAUNCH_CHECK();
+      }
       // dH[c0:c0+rows] = G . E - E[y] / T_v   (split-K partials, reduced together with the label term)
       int live = hint - c0;
       live = live < 128 ? 128 : (live > rows ? rows : live);

@@ -70,7 +70,7 @@ class _BertCore(SasRecCore):
         return Bert4RecEngine(self.cfg, batch, seq_len, self._device, seed=self._seed, with_grad=with_grad)
 
     def _to_ref(self, k, v):
-        return v[: self.cfg.n_items] if k == "head_b" else v
+        return v   # export_named already gives the reference shapes (true d, 4d inner width, n_items bias entries)
 
     def _import(self, state):
         inv = {v: k for k, v in self._keymap.items()}
@@ -79,11 +79,7 @@ class _BertCore(SasRecCore):
                 k = inv.get(rk)
                 if k is None:
                     continue
-                val = val.to(self.engine.dev, torch.float32)
-                if k == "head_b":
-                    self.engine.params[k][: val.numel()].copy_(val)
-                else:
-                    self.engine.params[k].copy_(val)
+                self.engine.import_named(k, val)
         self._shadow_dirty = True
 
     def state_dict(self, *a, destination=None, prefix="", keep_vars=False):
@@ -123,7 +119,8 @@ class _BertCore(SasRecCore):
         return eng.train_step(all_reduce, betas=self.adam_betas)[0]
 
     @torch.no_grad()
-    def query_embeddings(self, ids, pad_mask, token_mask):
+    def _query_padded(self, ids, pad_mask, token_mask):
+        """last-position hidden states at the padded width bf16 [B, dp] (pairs with the padded head)"""
         eng = self.ensure_engine(*ids.shape, with_grad=self.engine.with_grad if self.engine is not None else False)
         if self._shadow_dirty:
             eng.refresh_shadow(); self._shadow_dirty = False
@@ -131,21 +128,26 @@ class _BertCore(SasRecCore):
         return eng.forward_last_hidden()[: ids.shape[0]]
 
     @torch.no_grad()
+    def query_embeddings(self, ids, pad_mask, token_mask):
+        """bf16 [B, d] at the model's true hidden size"""
+        return self.engine.unpad_features(self._query_padded(ids, pad_mask, token_mask))
+
+    @torch.no_grad()
     def logits(self, ids, pad_mask, token_mask, candidates=None):
-        hq = self.query_embeddings(ids, pad_mask, token_mask)
+        hq = self._query_padded(ids, pad_mask, token_mask)
         W, b = self.engine.head_for_scoring()
         b = b[: self.cfg.n_items]
         if candidates is not None:
             W, b = W[candidates].contiguous(), b[candidates].contiguous()
         out = torch.empty(hq.shape[0], W.shape[0], device=hq.device, dtype=torch.float32)
-        self.engine._gemm(hq, W, out, hq.shape[0], W.shape[0], self.cfg.d, out_mode=2, bias=b)
+        self.engine._gemm(hq, W, out, hq.shape[0], W.shape[0], self.cfg.dp, out_mode=2, bias=b)
         return out
 
     @torch.no_grad()
     def predict_topk(self, ids, pad_mask, token_mask, k, seen_ids=None, candidates=None):
         from .... import ops
 
-        hq = self.query_embeddings(ids, pad_mask, token_mask).contiguous()
+        hq = self._query_padded(ids, pad_mask, token_mask).contiguous()
         W, b = self.engine.head_for_scoring()
         n_items, inv = self.cfg.n_items, None
         if candidates is not None:
@@ -197,8 +199,6 @@ class Bert4Rec(LightningModuleBase):
         kind = {"CE": "ce", "CE_restricted": "ce", "BCE": "bce"}.get(loss_type)
         if kind is None or loss_sample_count is not None:
             raise NotImplementedError("Not supported loss_type")
-        if kind == "bce" and hidden_size > 256:   # BERT4Rec's head always has a bias; the biased BCE head stops at d = 256
-            raise NotImplementedError("loss_type='BCE' is built for hidden_size <= 256")
         self._model = Bert4RecModel(tensor_schema, max_len=max_seq_len, hidden_size=hidden_size, num_blocks=block_count,
                                     num_heads=head_count, num_passes_over_block=pass_per_transformer_block_count,
                                     dropout=dropout_rate, enable_positional_embedding=enable_positional_embedding,
