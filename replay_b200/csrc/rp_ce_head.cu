@@ -38,8 +38,8 @@ static constexpr int kT = 128;                  // tile edge (rows per CTA, colu
 static constexpr int kChunk = 128 * 128;        // bytes of one [128 rows x 64 bf16] swizzled chunk
 static constexpr float kLog2e = 1.4426950408889634f;
 static constexpr float kLn2 = 0.6931471805599453f;
-// CTA layout of the head kernels: warpgroups 0 / 1 own rows [0, 64) / [64, 128) of the row tile; thread 0 also feeds the TMA
-// ring (a separate producer warp would cap the registers of the accumulating threads)
+// CTA layout of the head kernels: warpgroups 0 / 1 own rows [0, 64) / [64, 128) of the row tile; the same threads also feed
+// the TMA ring (a separate producer warp would cap the registers of the accumulating threads)
 static constexpr int kThreads = 256;
 static constexpr int kTN = 64;                  // grid of the column splits of the fused pass (ce_bwd_kernel tiles: TN)
 
@@ -383,7 +383,8 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   uint8_t* sB = smem + KCH * kChunk;
   __shared__ float s_row[kT];             // per-row sum of G (FUSED) / of G before the item factor (COLCONST with bias)
   __shared__ float s_dot[kSlots][kT];
-  __shared__ uint64_t bar_a, bar_full[NSTAGE], bar_empty[NSTAGE];
+  __shared__ uint64_t bar_a, bar_full[NSTAGE];
+  __shared__ uint32_t s_released[NSTAGE];   // warps that have released the stage, over all its tiles
 
   const int lane = threadIdx.x & 31;
   const int n_valid = *n_valid_ptr;
@@ -404,16 +405,17 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     mbar_init(&bar_a, 1);
     for (int i = 0; i < NSTAGE; ++i) {
       mbar_init(&bar_full[i], 1);
-      mbar_init(&bar_empty[i], 8);
+      s_released[i] = 0;
     }
     fence_barrier_init();
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
   }
   __syncthreads();
-  auto issue = [&](int jl) {   // thread 0: column tile jl -> stage jl % NSTAGE
+  // column tile jl -> stage jl % NSTAGE.  Thread 0 fills the ring; after that, the last of the 8 warps to release a stage
+  // refills it, so no warp ever waits for the other warpgroup and the two can run out of phase.
+  auto issue = [&](int jl) {
     const uint32_t s = jl % NSTAGE;
-    mbar_wait(&bar_empty[s], ((jl / NSTAGE) & 1) ^ 1);
     mbar_arrive_expect_tx(&bar_full[s], kStage);
     for (int kc = 0; kc < KCH; ++kc) tma_load_2d(sB + s * kStage + kc * kChunkB, &tmB, &bar_full[s], kc * 64, c_begin + jl * TN);
   };
@@ -442,13 +444,12 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   float za = 0.f, zb = 0.f;   // FUSED: row sums of G~ (BCE: of softplus); COLCONST with bias: row sums of G (bias gradient)
   float acc[D / 2];
   acc_zero(acc);
+  float sacc[TN / 2];
   mbar_wait(&bar_a, 0);
   const uint32_t a_base = smem_u32(sA) + wg * 8192;
-  for (int jl = 0; jl < n_ct; ++jl) {
-    const uint32_t s = jl % NSTAGE, ph = (jl / NSTAGE) & 1;
-    mbar_wait(&bar_full[s], ph);
-    const uint32_t b0 = smem_u32(sB + s * kStage);
-    float sacc[TN / 2];
+  auto issue_s = [&](int jl) {   // S = A_tile . B_tile^T of column tile jl into sacc, one commit group
+    mbar_wait(&bar_full[jl % NSTAGE], (jl / NSTAGE) & 1);
+    const uint32_t b0 = smem_u32(sB + (jl % NSTAGE) * kStage);
     wg_fence();
 #pragma unroll
     for (int kc = 0; kc < KCH; ++kc)
@@ -457,8 +458,22 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         WgmmaSS<TN>::template run<0, 0>(sacc, desc_k(a_base + kc * kChunk + ks * 32), desc_k(b0 + kc * kChunkB + ks * 32),
                                         (kc | ks) != 0);
     wg_commit();
+  };
+  // S of the next tile goes out behind dH (below), which keeps all of sacc live beside pk and acc; the BCE token pass, which
+  // also carries softplus's terms, would spill at d = 64 and d = 256, so it issues S after dH retires.
+  constexpr bool kSAhead = MODE != 3;
+  if (n_ct > 0) {
+    issue_s(0);
     wg_wait<0>();
     wg_fence_acc(sacc);
+  }
+  // With S ahead, the warpgroups take turns issuing {dH(j), S(j+1)} (named barriers 2 / 3, warpgroup 0 first), so that one
+  // warpgroup's exponentials run while the other's MMAs hold the tensor pipe.  The counts match: warpgroup 1 arrives once up
+  // front and skips its arrival after the last tile.
+  if (kSAhead && wg == 1 && n_ct > 0) named_bar_arrive(2, 256);
+  for (int jl = 0; jl < n_ct; ++jl) {
+    const uint32_t s = jl % NSTAGE;
+    const uint32_t b0 = smem_u32(sB + s * kStage);
     // G = exp2(S log2e + offset) -> bf16 A fragments
     const int col0 = c_begin + jl * TN + fc;
     uint32_t pk[TN / 4];
@@ -532,6 +547,7 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         pk[2 * q + 1] = pack_bf16(g[2], g[3]);
       }
     }
+    if (kSAhead) named_bar_sync(2 + wg, 256);   // this warpgroup's turn
     wg_fence();
 #pragma unroll
     for (int kk = 0; kk < TN / 16; ++kk) {
@@ -539,11 +555,30 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       WgmmaRS<D>::template run<1>(acc, af, desc_mn(b0 + kk * 2048, kChunkB), 1);
     }
     wg_commit();
-    wg_wait<0>();
+    // S of the next tile in its own commit group: wait<1> retires dH (the stage and pk are free again), wait<0> then S, whose
+    // exponentials start the next iteration.  The waits are unconditional (the last tile commits an empty group instead of
+    // S): ptxas follows both sides of a branch and would otherwise find S pending at the loop head and serialize every wgmma
+    // of the kernel.
+    const bool more = jl + 1 < n_ct;
+    if constexpr (kSAhead) {
+      if (more) issue_s(jl + 1);
+      else wg_commit();
+      if (wg == 0) named_bar_arrive(3, 256);   // the other warpgroup's turn
+      else if (more) named_bar_arrive(2, 256);
+      wg_wait<1>();
+    } else {
+      wg_wait<0>();
+    }
     wg_fence_acc(acc);
     __syncwarp();
-    if (lane == 0) mbar_arrive(&bar_empty[s]);
-    if (threadIdx.x == 0 && jl + NSTAGE < n_ct) issue(jl + NSTAGE);
+    // the counter's acq_rel orders every warp's completed wgmma reads of the stage before the TMA write that refills it
+    if (lane == 0 && jl + NSTAGE < n_ct && smem_count_acq_rel(&s_released[s]) % 8 == 7) {
+      fence_proxy_async();
+      issue(jl + NSTAGE);
+    }
+    if (!kSAhead && more) issue_s(jl + 1);
+    wg_wait<0>();
+    wg_fence_acc(sacc);
   }
   // ---- row sums (the quad's threads share rows) and the accumulator stage
 #pragma unroll

@@ -58,6 +58,12 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
 }
+// shared-memory counter += 1 with acquire-release ordering (CTA scope); returns the previous value
+__device__ __forceinline__ uint32_t smem_count_acq_rel(uint32_t* ctr) {
+  uint32_t old;
+  asm volatile("atom.acq_rel.cta.shared::cta.add.u32 %0, [%1], 1;" : "=r"(old) : "r"(smem_u32(ctr)) : "memory");
+  return old;
+}
 // ------------------------------------------------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor) - 2D tiled loads into shared memory, completion on an mbarrier
 // ------------------------------------------------------------------------------------------------------------------
@@ -80,6 +86,9 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
 }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------------------------

@@ -1,0 +1,95 @@
+"""Dump every output of the full-catalog CE and BCE heads on fixed seeds, or compare two dumps bit for bit.
+
+    python tools/ce_head_dump.py --out A.pt          # (RP_B200_LIB=<other build> selects the library to dump)
+    python tools/ce_head_dump.py --compare A.pt B.pt # "identical", or the first differing tensor
+
+Labels are unique (a permutation of the catalog), so the dE pass's one-hot scatter has no order-dependent fp32 atomics and
+two builds that run the same floating-point operations in the same order must agree exactly.  Cases: d = 64 / 128 / 256,
+with and without bias; the fused pass with one column split ("P1": as many row tiles as SMs) and with several ("Pn": one
+row tile); the two-pass path (no d_hc in the forward); the fused pass behind the two-pass forward (large logits fail the
+bound); and the BCE head's fused token pass and dE pass (P1 and Pn).
+"""
+import argparse
+import os
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import torch
+
+
+def _inputs(T, n_valid, I, d, bias, scale_h, scale_e, seed):
+    g = torch.Generator().manual_seed(seed)
+    hc = (torch.randn(T, d, generator=g) * scale_h).to(torch.bfloat16)
+    hc[n_valid:] = 0
+    table = (torch.randn(I, d, generator=g) * scale_e).to(torch.bfloat16)
+    b = (torch.randn(I, generator=g) * 0.5).float().cuda() if bias else None
+    labels = torch.randperm(I, generator=g)[:T].int()
+    nv = torch.tensor([n_valid], dtype=torch.int32, device="cuda")
+    return hc.cuda(), table.cuda(), b, labels.cuda(), nv
+
+
+def _run(ops, loss_kind, path, T, n_valid, I, d, bias, seed):
+    scale_h, scale_e = (2.0, 1.0) if path == "behind" else (0.5, 0.3)
+    hc, table, b, labels, nv = _inputs(T, n_valid, I, d, bias, scale_h, scale_e, seed)
+    st = ops.CEHeadState(T, I, d, "cuda")
+    d_hc = torch.zeros(T, d, device="cuda", dtype=torch.bfloat16)
+    d_tab = torch.zeros(I + 1, d, device="cuda")
+    d_b = torch.zeros(I + 1, device="cuda") if bias else None
+    fwd, bwd = (ops.ce_head_fwd, ops.ce_head_bwd) if loss_kind == "ce" else (ops.bce_head_fwd, ops.bce_head_bwd)
+    loss = fwd(st, hc, table, labels, nv, bias=b, d_hc=None if path == "twopass" else d_hc, n_valid_hint=T).clone()
+    if loss_kind == "ce" and path != "twopass":
+        assert ops.ce_head_fused_taken(st) == (path != "behind"), path
+    bwd(st, hc, table, labels, nv, d_hc, d_tab, bias=b, d_bias=d_b)
+    torch.cuda.synchronize()
+    out = dict(loss=loss, d_hc=d_hc, d_table=d_tab)
+    if loss_kind == "ce":
+        out.update(lse=st.lse, cvec=st.cvec)
+    if bias:
+        out["d_bias"] = d_b
+    return {k: v.cpu() for k, v in out.items()}
+
+
+def dump(path):
+    from replay_b200 import ops
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    res = {}
+    for d in (64, 128, 256):
+        for bias in (False, True):
+            shapes = {"P1": (sms * 128, sms * 128 - 37, sms * 128 + 3011), "Pn": (1024, 999, 20011)}
+            runs = [("ce", p, shapes[p]) for p in ("P1", "Pn")] + [("ce", "twopass", shapes["Pn"]), ("ce", "behind", shapes["Pn"])]
+            runs += [("bce", p, shapes[p]) for p in ("P1", "Pn")]
+            for i, (kind, p, (T, nv, I)) in enumerate(runs):
+                case = f"{kind}_{p}_d{d}_{'bias' if bias else 'nobias'}"
+                for k, v in _run(ops, kind, p, T, nv, I, d, bias, seed=1000 * d + 10 * i + bias).items():
+                    res[f"{case}/{k}"] = v
+    torch.save(res, path)
+    print(f"{len(res)} tensors -> {path}")
+
+
+def _bits(t):
+    return t.contiguous().view(torch.uint8)
+
+
+def compare(a_path, b_path):
+    a, b = torch.load(a_path), torch.load(b_path)
+    if sorted(a) != sorted(b):
+        print("different tensor sets:", sorted(set(a) ^ set(b)))
+        return 1
+    for k in a:
+        if a[k].shape != b[k].shape or not torch.equal(_bits(a[k]), _bits(b[k])):
+            diff = (a[k].double() - b[k].double()).abs()
+            n = int((_bits(a[k]) != _bits(b[k])).sum()) if a[k].shape == b[k].shape else -1
+            print(f"first differing tensor: {k} ({n} bytes differ, max |diff| {diff.nan_to_num(0).max().item():.3e})")
+            return 1
+    print(f"identical ({len(a)} tensors)")
+    return 0
+
+
+if __name__ == "__main__":
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out")
+    ap.add_argument("--compare", nargs=2)
+    args = ap.parse_args()
+    if args.compare:
+        sys.exit(compare(*args.compare))
+    dump(args.out)
