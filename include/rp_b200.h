@@ -48,13 +48,20 @@ const char* rp_version(void);
 int rp_seen_prepare(const int64_t* seen_ids, int n_users, int S, int item_count, const int32_t* inv_map,
                     int32_t* out_sorted, void* stream);
 
+/* Workspace of rp_score_topk.  K <= 32: per (user, item split, 32-column part) sorted partial lists of K (score, column)
+ * pairs.  32 < K <= 1024: per (user, item split) a buffer of C = max(2K, K + 64) rounded up to a power of two keys
+ * (8 bytes each) and its count; the item splits are capped so that one user's buffers hold at most 65 536 keys, and the
+ * size never decreases as n_users or K grows.  Both: one shared admission threshold per user. */
 size_t rp_score_topk_workspace(int n_users, int n_items, int d, int K);
 
 /* hq bf16 [n_users, d]; table bf16 [n_items, d] (the rows that are scored: all items, or the gathered candidates);
  * bias fp32 [round_up(n_items,128)] or NULL (BERT4Rec head); seen_sorted from rp_seen_prepare or NULL (no filter); candidates int64 [n_items] or NULL
  * (maps a scored column back to an item id, predictions_callback.py:91-92).
- * out_ids int64 [n_users, K], out_scores fp32 [n_users, K], sorted by (score desc, column asc).
- * d in {64,128,256,512}; 1 <= K <= 32. */
+ * out_ids int64 [n_users, K], out_scores fp32 [n_users, K], sorted by (score desc, column asc), exact and bit-identical
+ * from run to run.  When fewer than K columns are unmasked, the remaining slots hold the user's masked columns in
+ * ascending order (then -1) with score -inf.
+ * d in {64,128,256,512}; 1 <= K <= min(1024, n_items), else RP_ESHAPE.  K <= 32 keeps a sorted list per thread in
+ * registers; larger K admits candidates into workspace buffers that are compacted to K entries by a radix select. */
 int rp_score_topk(const void* hq, const void* table, const float* bias, const int32_t* seen_sorted, int S, int n_users,
                   int n_items, int d, int K, const int64_t* candidates, int64_t* out_ids, float* out_scores,
                   void* workspace, size_t workspace_bytes, void* stream);

@@ -6,9 +6,14 @@ from ....compat import CallbackBase
 from .postprocessors import RemoveSeenItems
 
 
+def _batch_device(batch):
+    """SasRec batches carry ``padding_mask``, Bert4Rec batches ``pad_mask``."""
+    return (batch["padding_mask"] if "padding_mask" in batch else batch["pad_mask"]).device
+
+
 class BasePredictionCallback(CallbackBase):
     """replay/models/nn/sequential/callbacks/prediction_callbacks.py:30-120.  With a ``replay_b200`` module and only
-    ``RemoveSeenItems`` postprocessors the scores / filter / top-K run fused on the device."""
+    ``RemoveSeenItems`` postprocessors and ``top_k <= ops.MAX_FUSED_K`` the scores / filter / top-K run fused on the device."""
 
     def __init__(self, top_k: int, query_column: str, item_column: str, rating_column: str = "rating", postprocessors=None):
         self.query_column, self.item_column, self.rating_column = query_column, item_column, rating_column
@@ -22,11 +27,13 @@ class BasePredictionCallback(CallbackBase):
             p.candidates = pl_module.candidates_to_score
 
     def on_predict_batch_end(self, trainer, pl_module, outputs, batch, batch_idx, dataloader_idx=0):
+        from ....ops import MAX_FUSED_K
+
         query_ids = batch["query_id"]
-        fusable = hasattr(pl_module, "predict_topk") and all(isinstance(p, RemoveSeenItems) for p in self._postprocessors)
+        fusable = (hasattr(pl_module, "predict_topk") and self._top_k <= MAX_FUSED_K
+                   and all(isinstance(p, RemoveSeenItems) for p in self._postprocessors))
         if fusable:
-            dev = batch["padding_mask"].device
-            seen = self._postprocessors[0].seen_tensor(query_ids, dev) if self._postprocessors else None
+            seen = self._postprocessors[0].seen_tensor(query_ids, _batch_device(batch)) if self._postprocessors else None
             ids, scores = pl_module.predict_topk(batch, self._top_k, seen, pl_module.candidates_to_score)
         else:
             scores_full = outputs
@@ -161,7 +168,7 @@ class ValidationMetricsCallback(CallbackBase):
         query_ids, gt = batch["query_id"], batch["ground_truth"]
         if (hasattr(pl_module, "predict_topk") and b.max_k <= MAX_FUSED_K
                 and all(isinstance(p, RemoveSeenItems) for p in self._postprocessors)):
-            seen = self._postprocessors[0].seen_tensor(query_ids, batch["padding_mask"].device) if self._postprocessors else None
+            seen = self._postprocessors[0].seen_tensor(query_ids, _batch_device(batch)) if self._postprocessors else None
             ids, _ = pl_module.predict_topk(batch, b.max_k, seen)
         else:
             scores = outputs

@@ -41,7 +41,9 @@ def seen_prepare(seen_ids: torch.Tensor, item_count: int, inv_map: torch.Tensor 
     return out
 
 
-MAX_FUSED_K = 32  # rp_score_topk keeps per-thread sorted lists of K entries (include/rp_b200.h); larger K: logits + torch.topk
+# rp_score_topk: K <= 32 in per-thread register lists, 32 < K <= 1024 in per-(user, item split) candidate buffers in its
+# workspace (include/rp_b200.h); larger K: logits + torch.topk
+MAX_FUSED_K = 1024
 
 
 def score_topk(hq: torch.Tensor, table: torch.Tensor, k: int, seen_sorted: torch.Tensor | None = None,
