@@ -20,9 +20,9 @@ import os
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 from dropout_stream import drop_keep, keep_draws
+from fp64_checks import WorstErrors, block_err, feat_mask, ln_bwd_ref, ln_ref, seq_block_err, ulp_err
 from replay_b200._lib import check, lib
 
 SENT = -3.25                       # sentinel for memory a kernel must not write (exact in bf16)
@@ -41,31 +41,20 @@ TOL_LOSS = 2e-4          # BERT4Rec step: relative loss error; worst seen 6.1e-5
 TOL_HID = 1.6e-2         # BERT4Rec step: hidden states, per (sequence, 64-row block); worst seen 5.3e-3
 TOL_GRAD = 5e-2          # BERT4Rec step: parameter gradients, per 64-row block; worst seen 1.6e-2 (in_b)
 TOL_LAST = 1.6e-2        # forward_last_hidden: per-row norm-relative; worst seen 5.2e-3
-BLOCK_FLOOR = 0.05       # a block whose reference norm is below this fraction of the typical block is measured against it
 
 
 def _ru(x, m):
     return (x + m - 1) // m * m
 
 
-_WORST = {}
-
-
-def _note(family, value):
-    """Record the worst error of a family (and the case it came from) for the report printed at the end."""
-    value = float(value)
-    if value >= _WORST.get(family, (0.0, ""))[0]:
-        _WORST[family] = (value, os.environ.get("PYTEST_CURRENT_TEST", "").split("::")[-1].split(" ")[0])
-    return value
+_worst = WorstErrors()
+_note = _worst.note
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _report_worst():
     yield
-    if _WORST:
-        print("\nworst observed error per family:")
-        for k, (v, case) in sorted(_WORST.items()):
-            print(f"  {k:28s} {v:.3g}  {case}")
+    _worst.report()
 
 
 @pytest.fixture(scope="module")
@@ -92,36 +81,7 @@ def _ks(p):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# error measures
-# ----------------------------------------------------------------------------------------------------------------------
-def ulp_err(got, ref, atol):
-    """max |got - ref| / (half a bf16 ulp of ref + atol), element-wise.  ``ref`` float64, ``atol`` >= 0 (tensor or scalar)."""
-    r = ref.abs()
-    half_ulp = torch.exp2(torch.floor(torch.log2(r.clamp_min(1e-300))) - 8)
-    return float(((got.double() - ref).abs() / (half_ulp + atol)).max())
-
-
-def block_err(got, ref, blk=64):
-    """Largest norm-relative error over blocks of ``blk`` leading-axis entries of [R, ...] arrays.  A block whose reference
-    norm is below BLOCK_FLOOR x the RMS block norm is measured against that floor."""
-    got, ref = got.double().reshape(ref.shape[0], -1), ref.double().reshape(ref.shape[0], -1)
-    R = ref.shape[0]
-    nb = -(-R // blk)
-    pad = (0, 0, 0, nb * blk - R)
-    diff = F.pad(got - ref, pad).reshape(nb, -1).norm(dim=-1)
-    den = F.pad(ref, pad).reshape(nb, -1).norm(dim=-1)
-    floor = BLOCK_FLOOR * float(den.square().mean().sqrt()) + 1e-300
-    return float((diff / den.clamp_min(floor)).max())
-
-
-def seq_block_err(got, ref, real):
-    """[B, L, d] hidden states: largest norm-relative error over (sequence, 64-row block)s of the real rows."""
-    m = real[..., None].to(ref.dtype)
-    return max(block_err(got[b] * m[b], ref[b] * m[b]) for b in range(ref.shape[0]))
-
-
-# ----------------------------------------------------------------------------------------------------------------------
-# float64 references: GELU, LayerNorm
+# float64 references: GELU
 # ----------------------------------------------------------------------------------------------------------------------
 _C_TANH = math.sqrt(2.0 / math.pi)
 
@@ -155,34 +115,6 @@ class _GeluTanhGrad(torch.autograd.Function):
     def backward(ctx, g):
         (x,) = ctx.saved_tensors
         return g * gelu_tanh_grad(x)
-
-
-def feat_mask(d, hd_valid):
-    """bool [d]: the real features of a padded layout (hd_valid 0 = all real)."""
-    if hd_valid == 0:
-        return torch.ones(d, dtype=torch.bool)
-    slot = 64 if hd_valid <= 64 else 128
-    return (torch.arange(d) % slot) < hd_valid
-
-
-def ln_ref(x, w, b, eps, valid):
-    """LayerNorm over the real features only -> (y, mean, rstd); padded outputs 0 (their w, b are 0)."""
-    v = valid.to(x.device, x.dtype)
-    n = float(v.sum())
-    mean = (x * v).sum(-1, keepdim=True) / n
-    var = (((x - mean) * v) ** 2).sum(-1, keepdim=True) / n
-    rstd = 1.0 / torch.sqrt(var + eps)
-    return ((x - mean) * rstd * w + b) * v, mean[..., 0], rstd[..., 0]
-
-
-def ln_bwd_ref(dy, x, w, mean, rstd, valid):
-    """dx (padded inputs get 0), sum_r dy * xhat, sum_r dy for one LayerNorm over the real features."""
-    v = valid.to(x.device, x.dtype)
-    n = float(v.sum())
-    xh = (x - mean[:, None]) * rstd[:, None] * v
-    g = dy * w * v
-    dx = rstd[:, None] * (g - g.sum(-1, keepdim=True) / n - xh * (g * xh).sum(-1, keepdim=True) / n) * v
-    return dx, (dy * xh).sum(0), dy.sum(0)
 
 
 # ----------------------------------------------------------------------------------------------------------------------

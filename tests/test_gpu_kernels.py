@@ -337,63 +337,6 @@ def test_ce_head_wide_hidden_gemms_with_more_tiles_than_sms(ops):
     assert eh < 1e-2 and ee < 1e-2, (eh, ee)
 
 
-@pytest.mark.parametrize("T,d,mask", [(3000, 128, False), (20000, 128, True), (777, 64, True), (40000, 64, False)])
-def test_fused_ffn_matches_reference_formula(ops, T, d, mask):
-    """rp_ffn_fused (inference): relu(y W1^T + b1) W2^T + b2 + y in one pass, ragged last tile, optional row mask."""
-    from replay_b200._lib import check, lib
-    g = torch.Generator().manual_seed(T + d)
-    y = torch.randn(T, d, generator=g).to(torch.bfloat16)
-    w1 = (torch.randn(d, d, generator=g) * 0.15).to(torch.bfloat16)
-    w2 = (torch.randn(d, d, generator=g) * 0.15).to(torch.bfloat16)
-    b1, b2 = torch.randn(d, generator=g) * 0.3, torch.randn(d, generator=g) * 0.3
-    rm = (torch.rand(T, generator=g) > 0.3) if mask else None
-    u = torch.relu(y.double() @ w1.double().T + b1.double()).to(torch.bfloat16).double()   # the hidden activation is bf16
-    ref = u @ w2.double().T + b2.double() + y.double()
-    if mask:
-        ref = ref * rm[:, None].double()
-    out = torch.full((T + 5, d), 3.0, device="cuda", dtype=torch.bfloat16)
-    yc, w1c, w2c, b1c, b2c = y.cuda(), w1.cuda(), w2.cuda(), b1.cuda(), b2.cuda()
-    rmc = rm.to(torch.uint8).cuda() if mask else None
-    check(lib().rp_ffn_fused(yc.data_ptr(), w1c.data_ptr(), b1c.data_ptr(), w2c.data_ptr(), b2c.data_ptr(),
-                             None if rmc is None else rmc.data_ptr(), T, d, out.data_ptr(), torch.cuda.current_stream().cuda_stream),
-          "rp_ffn_fused")
-    torch.cuda.synchronize()
-    err = (out[:T].cpu().double() - ref).abs().max().item()
-    assert err < 0.06, err            # bf16 output rounding of O(5) values
-    assert (out[T:] == 3.0).all()     # nothing written beyond T
-
-
-@pytest.mark.parametrize("T,d,mask", [(3000, 128, False), (20000, 128, True), (777, 64, True), (33000, 64, False)])
-def test_fused_post_attention_block_matches_reference_formula(ops, T, d, mask):
-    """rp_post_attn_fused (inference): h = o Wo^T + bo + q ; y = LN(h) ; out = relu(y W1^T + b1) W2^T + b2 + y."""
-    from replay_b200._lib import check, lib
-    g = torch.Generator().manual_seed(T * 3 + d)
-    o = torch.randn(T, d, generator=g).to(torch.bfloat16)
-    qin = torch.randn(T, d, generator=g).to(torch.bfloat16)
-    wo, w1, w2 = ((torch.randn(d, d, generator=g) * 0.15).to(torch.bfloat16) for _ in range(3))
-    bo, b1, b2, lb = (torch.randn(d, generator=g) * 0.3 for _ in range(4))
-    lw = 1 + torch.randn(d, generator=g) * 0.1
-    rm = (torch.rand(T, generator=g) > 0.3) if mask else None
-    h = o.double() @ wo.double().T + bo.double() + qin.double()
-    y = torch.nn.functional.layer_norm(h, (d,), lw.double(), lb.double(), 1e-8)
-    yb = y.to(torch.bfloat16).double()                          # y feeds the FFN (and its residual) as bf16
-    u = torch.relu(yb @ w1.double().T + b1.double()).to(torch.bfloat16).double()
-    ref = u @ w2.double().T + b2.double() + yb
-    if mask:
-        ref = ref * rm[:, None].double()
-    out = torch.full((T + 3, d), 3.0, device="cuda", dtype=torch.bfloat16)
-    t = [x.cuda() for x in (o, qin, wo, bo, lw, lb, w1, b1, w2, b2)]
-    rmc = rm.to(torch.uint8).cuda() if mask else None
-    check(lib().rp_post_attn_fused(t[0].data_ptr(), t[1].data_ptr(), t[2].data_ptr(), t[3].data_ptr(), t[4].data_ptr(), t[5].data_ptr(),
-                                   1e-8, t[6].data_ptr(), t[7].data_ptr(), t[8].data_ptr(), t[9].data_ptr(),
-                                   None if rmc is None else rmc.data_ptr(), T, d, out.data_ptr(), 0, torch.cuda.current_stream().cuda_stream),
-          "rp_post_attn_fused")
-    torch.cuda.synchronize()
-    err = (out[:T].cpu().double() - ref).abs().max().item()
-    assert err < 0.08, err
-    assert (out[T:] == 3.0).all()
-
-
 @pytest.mark.parametrize("T,shapes", [(1000, [(128, 128), (128, 128), (256, 128)]), (4096 + 37, [(64, 64), (128, 64)]),
                                       (700, [(1024, 256), (256, 1024), (768, 256)])])
 def test_wgrad_group_matches_matmul(ops, T, shapes):
@@ -442,129 +385,6 @@ def test_wgrad_group_matches_matmul(ops, T, shapes):
     torch.cuda.synchronize()
     for (_, _, dW, db), (w2, b2) in zip(pairs, again):
         assert torch.equal(dW, w2) and torch.equal(db, b2)
-
-
-@pytest.mark.parametrize("T,d", [(1000, 128), (517, 64), (128 * 150 + 5, 128)])
-def test_ln_qkv_fused_matches_formula(ops, T, d):
-    """rp_ln_qkv_fused: q_in = LN(x), Q = q_in Wq^T + bq, [K|V] = x Wkv^T + bkv in one pass, vs fp64 on the same bf16 inputs
-    (transformer.py:99-106: the query is the NORMALISED x, keys / values the un-normalised one)."""
-    from replay_b200._lib import check, lib
-
-    g = torch.Generator().manual_seed(T + d)
-    x = (torch.randn(T, d, generator=g) * 1.3 + 0.2).to(torch.bfloat16)
-    w_in = (torch.randn(3 * d, d, generator=g) / d ** 0.5).to(torch.bfloat16)
-    b_in = torch.randn(3 * d, generator=g) * 0.1
-    ln_w, ln_b = 1 + 0.1 * torch.randn(d, generator=g), 0.1 * torch.randn(d, generator=g)
-    xd = x.double()
-    mean, var = xd.mean(-1, keepdim=True), xd.var(-1, unbiased=False, keepdim=True)
-    q_ref = (xd - mean) / torch.sqrt(var + 1e-8) * ln_w.double() + ln_b.double()
-    dev = dict(device="cuda")
-    q_in, Q = torch.zeros(T, d, dtype=torch.bfloat16, **dev), torch.zeros(T, d, dtype=torch.bfloat16, **dev)
-    KV = torch.zeros(T, 2 * d, dtype=torch.bfloat16, **dev)
-    mo, ro = torch.zeros(T, **dev), torch.zeros(T, **dev)
-    xc, wc, bc, lw, lb = x.cuda(), w_in.cuda(), b_in.cuda(), ln_w.cuda(), ln_b.cuda()
-    check(lib().rp_ln_qkv_fused(xc.data_ptr(), lw.data_ptr(), lb.data_ptr(), 1e-8, wc.data_ptr(), bc.data_ptr(), T, d,
-                                q_in.data_ptr(), Q.data_ptr(), KV.data_ptr(), mo.data_ptr(), ro.data_ptr(), 0,
-                                torch.cuda.current_stream().cuda_stream), "rp_ln_qkv_fused")
-    torch.cuda.synchronize()
-    assert (q_in.cpu().double() - q_ref).abs().max() < 3e-2
-    torch.testing.assert_close(mo.cpu().double(), mean[:, 0], rtol=1e-4, atol=1e-4)
-    torch.testing.assert_close(ro.cpu().double(), 1 / torch.sqrt(var[:, 0] + 1e-8), rtol=1e-3, atol=1e-4)
-    q16 = q_in.cpu().double()  # the Q GEMM consumes the bf16 q_in the kernel itself produced
-    Q_ref = q16 @ w_in[:d].double().T + b_in[:d].double()
-    KV_ref = xd @ w_in[d:].double().T + b_in[d:].double()
-    assert (Q.cpu().double() - Q_ref).abs().max() < 3e-2 * max(1.0, Q_ref.abs().max().item())
-    assert (KV.cpu().double() - KV_ref).abs().max() < 3e-2 * max(1.0, KV_ref.abs().max().item())
-    assert (Q.cpu().double() - Q_ref).norm() / Q_ref.norm() < 5e-3 and (KV.cpu().double() - KV_ref).norm() / KV_ref.norm() < 5e-3
-
-
-@pytest.mark.parametrize("T,d", [(1000, 128), (517, 64), (128 * 150 + 5, 128)])
-def test_pre_attn_bwd_matches_formula(ops, T, d):
-    """rp_pre_attn_bwd: dq_in = dQ Wq + dh ; LayerNorm backward ; dx = dKV Wkv + t ; dln_w, dln_b - vs fp64 autograd-free formulas."""
-    from replay_b200._lib import check, lib
-
-    g = torch.Generator().manual_seed(T * 3 + d)
-    bf = lambda *s, sc=1.0: (torch.randn(*s, generator=g) * sc).to(torch.bfloat16)  # noqa: E731
-    dQ, dKV, dh, x = bf(T, d, sc=0.3), bf(T, 2 * d, sc=0.3), bf(T, d, sc=0.3), bf(T, d, sc=1.2)
-    w_in = bf(3 * d, d, sc=1 / d ** 0.5)
-    ln_w = 1 + 0.1 * torch.randn(d, generator=g)
-    xd = x.double()
-    mean, var = xd.mean(-1), xd.var(-1, unbiased=False)
-    rstd = 1 / torch.sqrt(var + 1e-8)
-    xhat = (xd - mean[:, None]) * rstd[:, None]
-    dq = dQ.double() @ w_in[:d].double() + dh.double()
-    gg = dq * ln_w.double()
-    t = rstd[:, None] * (gg - gg.mean(-1, keepdim=True) - xhat * (gg * xhat).mean(-1, keepdim=True))
-    dx_ref = dKV.double() @ w_in[d:].double() + t
-    dw_ref, db_ref = (dq * xhat).sum(0), dq.sum(0)
-    dx = torch.zeros(T, d, dtype=torch.bfloat16, device="cuda")
-    dw, db = torch.full((d,), 2.0, device="cuda"), torch.full((d,), -3.0, device="cuda")
-    args = [t_.cuda() for t_ in (dQ, dKV, dh, x, mean.float(), rstd.float(), ln_w, w_in)]
-    check(lib().rp_pre_attn_bwd(*[a.data_ptr() for a in args], T, d, dx.data_ptr(), dw.data_ptr(), db.data_ptr(), 0,
-                                torch.cuda.current_stream().cuda_stream), "rp_pre_attn_bwd")
-    torch.cuda.synchronize()
-    assert (dx.cpu().double() - dx_ref).norm() / dx_ref.norm() < 6e-3
-    assert (dx.cpu().double() - dx_ref).abs().max() < 3e-2 * max(1.0, dx_ref.abs().max().item())
-    assert ((dw.cpu().double() - 2.0) - dw_ref).norm() / dw_ref.norm() < 5e-3   # accumulated on top of the preset values
-    assert ((db.cpu().double() + 3.0) - db_ref).norm() / db_ref.norm() < 5e-3
-
-
-@pytest.mark.parametrize("T,d,drop,masked", [(1000, 128, 0.0, False), (900, 128, 0.25, True), (517, 64, 0.1, False),
-                                             (128 * 150 + 5, 128, 0.2, False)])
-def test_post_attn_bwd_matches_formula(ops, T, d, drop, masked):
-    """rp_post_attn_bwd (dropout' -> FFN backward -> LayerNorm2 backward -> out-projection backward in one pass) vs fp64
-    formulas; the site-2 dropout mask is taken from rp_dropout_bwd (the same stream), site 1 is encoded in the zeros of u."""
-    from replay_b200._lib import check, lib
-
-    L = lib()
-    g = torch.Generator().manual_seed(T * 7 + d)
-    bf = lambda *s, sc=1.0: (torch.randn(*s, generator=g) * sc).to(torch.bfloat16)  # noqa: E731
-    dz, h = bf(T, d, sc=0.5), bf(T, d, sc=1.5)
-    u = torch.relu(bf(T, d))  # ~half zeros, like relu + dropout output
-    w2, w1, wo = bf(d, d, sc=1 / d ** 0.5), bf(d, d, sc=1 / d ** 0.5), bf(d, d, sc=1 / d ** 0.5)
-    ln_w = 1 + 0.1 * torch.randn(d, generator=g)
-    rowmask = (torch.rand(T, generator=g) > 0.3).to(torch.uint8) if masked else None
-    seed, off2 = 1234567, 5 << 40
-    st = torch.cuda.current_stream().cuda_stream
-    ctr = torch.tensor([99], dtype=torch.int64, device="cuda")
-    # reference mask of site 2: d_t_ref = dropout_bwd(dz * rowmask)
-    dzc = dz.cuda()
-    ones = torch.ones(T, d, dtype=torch.bfloat16, device="cuda")
-    keep = torch.empty_like(ones)
-    check(L.rp_dropout_bwd(ones.data_ptr(), keep.data_ptr(), T, d, None, drop, seed, off2, ctr.data_ptr(), st), "rp_dropout_bwd")
-    keep = keep.cpu().double()  # 0 or 1/(1-p) (bf16-rounded scale: divide it out)
-    keep = (keep > 0).double() / (1.0 - drop)
-    rm = rowmask.double()[:, None] if masked else 1.0
-    dzm = dz.double() * rm
-    d_t = dzm * keep
-    hd = h.double()
-    mean, var = hd.mean(-1), hd.var(-1, unbiased=False)
-    rstd = 1 / torch.sqrt(var + 1e-8)
-    xhat = (hd - mean[:, None]) * rstd[:, None]
-    d_t16 = d_t.to(torch.bfloat16).double()
-    du = (d_t16 @ w2.double()) * (u.double() != 0) / (1.0 - drop)
-    du16 = du.to(torch.bfloat16).double()
-    dy = du16 @ w1.double() + dzm
-    gg = dy * ln_w.double()
-    dh = rstd[:, None] * (gg - gg.mean(-1, keepdim=True) - xhat * (gg * xhat).mean(-1, keepdim=True))
-    d_o = dh.to(torch.bfloat16).double() @ wo.double()
-    o = {k: torch.zeros(T, d, dtype=torch.bfloat16, device="cuda") for k in ("d_t", "du", "dh", "d_o")}
-    dw, db = torch.full((d,), 1.0, device="cuda"), torch.full((d,), -1.0, device="cuda")
-    need_dt = masked or drop > 0
-    args = [dzc, u.cuda(), h.cuda(), mean.float().cuda(), rstd.float().cuda(), ln_w.cuda(), w2.cuda(), w1.cuda(), wo.cuda()]
-    rmc = rowmask.cuda() if masked else None
-    check(L.rp_post_attn_bwd(*[a.data_ptr() for a in args], None if rmc is None else rmc.data_ptr(), T, d, drop, seed, off2,
-                             ctr.data_ptr(), o["d_t"].data_ptr() if need_dt else None, o["du"].data_ptr(), o["dh"].data_ptr(),
-                             o["d_o"].data_ptr(), dw.data_ptr(), db.data_ptr(), 0, st), "rp_post_attn_bwd")
-    torch.cuda.synchronize()
-    rel = lambda a, b: float((a.cpu().double() - b).norm() / b.norm())  # noqa: E731
-    if need_dt:
-        assert rel(o["d_t"], d_t) < 5e-3
-    assert rel(o["du"], du) < 8e-3, rel(o["du"], du)
-    assert rel(o["dh"], dh) < 1e-2, rel(o["dh"], dh)
-    assert rel(o["d_o"], d_o) < 1.2e-2, rel(o["d_o"], d_o)
-    assert float(((dw.cpu().double() - 1.0) - (dy * xhat).sum(0)).norm() / (dy * xhat).sum(0).norm()) < 1e-2
-    assert float(((db.cpu().double() + 1.0) - dy.sum(0)).norm() / dy.sum(0).norm()) < 1e-2
 
 
 def test_gemm_tall_kv_projection_beyond_65535_row_tiles(ops):
