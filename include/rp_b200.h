@@ -405,6 +405,41 @@ int rp_sampled_head_fwd(const rp_sampled_desc* s, void* stream);
 int rp_sampled_head_bwd(const rp_sampled_desc* s, void* d_hc, float* d_table, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
+ * Scalable cross-entropy head of the legacy SASRec (loss_type="SCE", arXiv 2409.18721):
+ *   replaces  ScalableCrossEntropyLoss.__call__          replay/models/nn/loss/sce.py:43-124
+ *             SasRec._compute_loss_scalable_ce           replay/models/nn/sequential/sasrec/lightning.py:383-392
+ * hc bf16 [capacity, d]: final hidden state of EVERY position (row b * seq_len + l, pad rows included); table bf16
+ * [n_items, d]; labels int64 [capacity]; pad_mask [capacity] (1 = real input position); n_rows int32 [1] in device memory =
+ * B * seq_len of the batch (<= capacity).  d in {64,128,256,512} is the padded width, d_true the model's hidden size,
+ * hd_valid the feature-slot layout (0 = unpadded).  1 <= bucket_size_x <= min(1024, capacity), 1 <= bucket_size_y <=
+ * min(1024, n_items) (the fused top-K), else RP_ESHAPE.
+ * Caller-owned outputs: draw fp32 = the standard normals, [n_buckets, d_true] (or [capacity, n_buckets] with mix_x; rows
+ * < *n_rows used), drawn from Philox keyed by seed + *rng_counter unless draw_given (then read as given); top_x int64 and
+ * score_x fp32 [n_buckets, bucket_size_x] (slots with score -inf hold no row); top_y int64 [n_buckets, bucket_size_y].
+ * A row carries loss when it is a real position with a label in [0, n_items).  fwd: loss_out fp32 [2] = { mean over the
+ * rows with a non-zero per-row max of the bucket CEs (NaN when there is none), 1 / that count (0 when none) }.
+ * stages: RP_SCE_DRAW | RP_SCE_SELECT_X | RP_SCE_SELECT_Y | RP_SCE_BUCKET_CE run in this order (RP_SCE_ALL = one forward;
+ * the parts exist for timing).  bwd: d_hc bf16 [capacity, d] OVERWRITTEN for every row (zero where no gradient); no table
+ * gradient (the reference scores a detached copy of the table).  Deterministic and CUDA-graph capturable. */
+#define RP_SCE_DRAW 1
+#define RP_SCE_SELECT_X 2
+#define RP_SCE_SELECT_Y 4
+#define RP_SCE_BUCKET_CE 8
+#define RP_SCE_ALL 15
+typedef struct rp_sce_desc {
+  const void* hc; const void* table; const int64_t* labels; const uint8_t* pad_mask; const int32_t* n_rows;
+  int capacity, n_items, d, d_true, hd_valid;
+  int n_buckets, bucket_size_x, bucket_size_y, mix_x;
+  unsigned long long seed; const unsigned long long* rng_counter; int draw_given;
+  float* draw; int64_t* top_x; float* score_x; int64_t* top_y;
+  float* loss_out;
+  void* workspace; size_t workspace_bytes;
+} rp_sce_desc;
+size_t rp_sce_head_workspace(int capacity, int n_items, int d, int n_buckets, int bucket_size_x, int bucket_size_y, int mix_x);
+int rp_sce_head_fwd(const rp_sce_desc* s, int stages, void* stream);
+int rp_sce_head_bwd(const rp_sce_desc* s, void* d_hc, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
  * Device-side batch construction (SURVEY.md §8 f.1).  All histories are resident in HBM as CSR: offsets [n_seq+1] int64,
  * items [offsets[n_seq]] int32.  One call builds B rows of a [B, L] batch: row b is the window of history seq_index[b]
  * starting at seq_offset[b] (NULL: the LAST L(+1) items), left-padded with pad_value.  Replaces the per-sample host path

@@ -83,6 +83,9 @@ def lib():
     _sig(L.rp_sampled_head_workspace, c_size_t, [c_int, c_int, c_int, c_int])
     _sig(L.rp_sampled_head_fwd, c_int, [P, P])
     _sig(L.rp_sampled_head_bwd, c_int, [P, P, P, P])
+    _sig(L.rp_sce_head_workspace, c_size_t, [c_int, c_int, c_int, c_int, c_int, c_int, c_int])
+    _sig(L.rp_sce_head_fwd, c_int, [ctypes.POINTER(SceDesc), c_int, P])
+    _sig(L.rp_sce_head_bwd, c_int, [ctypes.POINTER(SceDesc), P, P])
     _sig(L.rp_selftest_mma_probe, c_int, [c_int, c_int, c_int, P, P])
     _sig(L.rp_selftest_tma_probe, c_int, [P, LL, c_int, c_int, c_int, c_int, c_int, P])
     _sig(L.rp_colsum_multi, c_int, [c_int, P, P, P, P, c_int, P])
@@ -150,6 +153,23 @@ class SampledDesc(ctypes.Structure):
     ]
 
 
+class SceDesc(ctypes.Structure):
+    """Mirror of ``struct rp_sce_desc`` (include/rp_b200.h)."""
+
+    _fields_ = [
+        ("hc", c_void_p), ("table", c_void_p), ("labels", c_void_p), ("pad_mask", c_void_p), ("n_rows", c_void_p),
+        ("capacity", c_int), ("n_items", c_int), ("d", c_int), ("d_true", c_int), ("hd_valid", c_int),
+        ("n_buckets", c_int), ("bucket_size_x", c_int), ("bucket_size_y", c_int), ("mix_x", c_int),
+        ("seed", ctypes.c_ulonglong), ("rng_counter", c_void_p), ("draw_given", c_int),
+        ("draw", c_void_p), ("top_x", c_void_p), ("score_x", c_void_p), ("top_y", c_void_p),
+        ("loss_out", c_void_p),
+        ("workspace", c_void_p), ("workspace_bytes", c_size_t),
+    ]
+
+
+SCE_DRAW, SCE_SELECT_X, SCE_SELECT_Y, SCE_BUCKET_CE, SCE_ALL = 1, 2, 4, 8, 15   # rp_sce_head_fwd stages
+
+
 class AttnDesc(ctypes.Structure):
     """Mirror of ``struct rp_attn_desc`` (include/rp_b200.h)."""
 
@@ -191,4 +211,4 @@ class AttnBwdDesc(ctypes.Structure):
 
 _EXTRA_SIGS: list = []
 
-__all__ = ["GemmDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]
+__all__ = ["GemmDesc", "SceDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]

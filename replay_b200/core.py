@@ -201,7 +201,7 @@ class SasRecCore(torch.nn.Module):
             if kind in self._FULL_CATALOG:
                 self.engine.set_loss(kind, **kw)
 
-    _FULL_CATALOG = ("ce", "ce_weighted", "login_ce", "bce")   # heads over the whole catalog (no negatives)
+    _FULL_CATALOG = ("ce", "ce_weighted", "login_ce", "bce", "sce")   # heads that take no negatives
 
     def _stage(self, eng, ids, pad_mask, labels, target_mask, negatives, row_weights=None):
         spec = getattr(self, "_loss_spec", ("ce", {}))

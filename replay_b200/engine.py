@@ -19,7 +19,7 @@ from dataclasses import dataclass
 
 import torch
 
-from ._lib import SampledDesc, AttnBwdDesc, AttnDesc, GemmDesc, WgradPair, check, lib
+from ._lib import SCE_ALL, SampledDesc, SceDesc, AttnBwdDesc, AttnDesc, GemmDesc, WgradPair, check, lib
 
 
 @dataclass
@@ -154,6 +154,7 @@ class SasRecEngine:
         # fused attention backward: head_dim 64, L <= 256; otherwise saved probabilities + batched GEMMs
         self.fused_attn_bwd = cfg.head_slot == 64 and seq_len <= 256
         self.sampled = None       # full-catalog CE unless set_loss() selects a sampled head
+        self.sce = None           # buffers of the scalable CE head (set_loss("sce", ...))
         self._loss_args = None
         self.fused_ffn_eval = True  # eval / predict: one-pass FFN kernel for d <= 128
         self.fused_post_attn_eval = True  # eval / predict: out-projection + LayerNorm + FFN in one kernel for d <= 128
@@ -525,16 +526,28 @@ class SasRecEngine:
         if n < self.T:
             self.in_pad[n:].zero_()
             self.in_tmask[n:].zero_()
+        if self.sce is not None:
+            self.sce["n_rows"].fill_(n)
 
     # ------------------------------------------------------------------------------------------------ sampled heads
     SAMPLED_KINDS = {"ce_sampled": 0, "bce_sampled": 1, "legacy_ce_sampled": 2, "legacy_bce_sampled": 3}
 
     def set_loss(self, kind: str = "ce", n_neg: int = 0, neg_shape: str = "shared", ignore_index: int = -100,
-                 log_eps: float = 1e-6, clamp: float = 100.0):
+                 log_eps: float = 1e-6, clamp: float = 100.0, n_buckets: int = 0, bucket_size_x: int = 0,
+                 bucket_size_y: int = 0, mix_x: bool = False):
         """``"ce"`` = full-catalog CE (default).  Sampled heads (SURVEY §8 a9): ``ce_sampled`` / ``bce_sampled`` (new path,
         replay/nn/loss/ce.py:146, bce.py:98) and ``legacy_ce_sampled`` / ``legacy_bce_sampled`` (sasrec/lightning.py:310-376)
-        with ``n_neg`` negatives per target, ``neg_shape`` in shared [N] / perseq [B, N] / perpos [B, L, N]."""
-        self._loss_args = (kind, dict(n_neg=n_neg, neg_shape=neg_shape, ignore_index=ignore_index, log_eps=log_eps, clamp=clamp))
+        with ``n_neg`` negatives per target, ``neg_shape`` in shared [N] / perseq [B, N] / perpos [B, L, N].
+        ``"sce"``: the legacy module's scalable cross-entropy (replay/models/nn/loss/sce.py) with ``n_buckets`` buckets of
+        ``bucket_size_x`` rows and ``bucket_size_y`` items (both <= 1024, the fused top-K), ``mix_x`` as the reference."""
+        self._loss_args = (kind, dict(n_neg=n_neg, neg_shape=neg_shape, ignore_index=ignore_index, log_eps=log_eps, clamp=clamp,
+                                      n_buckets=n_buckets, bucket_size_x=bucket_size_x, bucket_size_y=bucket_size_y,
+                                      mix_x=mix_x))
+        self.sce = None
+        if kind == "sce":
+            self.sampled, self.ce_row, self.bce = None, None, False
+            self._set_sce(n_buckets, bucket_size_x, bucket_size_y, bool(mix_x))
+            return
         # per-row variants of the full-catalog head (rp_ce_head_fwd_w): "ce_weighted" (LogOutCEWeighted / CEWeighted: sample
         # weights staged with set_row_weights) and "login_ce" (LogInCE); "ce" is the plain head
         self.ce_row = None
@@ -555,6 +568,51 @@ class SasRecEngine:
         self.sampled = dict(kind=self.SAMPLED_KINDS[kind], n_neg=n_neg, mode=mode, ignore_index=ignore_index, log_eps=log_eps,
                             clamp=clamp, neg=torch.zeros(rows, n_neg, device=self.dev, dtype=torch.int64),
                             ws=torch.zeros(ws_bytes, device=self.dev, dtype=torch.uint8), ws_bytes=ws_bytes)
+
+    def _set_sce(self, n_b: int, bsx: int, bsy: int, mix: bool):
+        cfg, dev, T = self.cfg, self.dev, self.T
+        if not self.with_grad:   # an inference engine has no loss buffers; resize(with_grad=True) applies the loss again
+            return
+        if n_b < 1 or not 1 <= bsx <= min(1024, T) or not 1 <= bsy <= min(1024, cfg.n_items):
+            raise ValueError(f"SCE needs n_buckets >= 1, 1 <= bucket_size_x <= min(1024, B * L = {T}) and 1 <= bucket_size_y "
+                             f"<= min(1024, n_items = {cfg.n_items}) (the fused top-K); got {n_b}, {bsx}, {bsy}")
+        ws_bytes = self.lib.rp_sce_head_workspace(T, cfg.n_items, cfg.dp, n_b, bsx, bsy, int(mix))
+        if ws_bytes == 0:
+            raise ValueError("rp_sce_head: unsupported shape")
+        i64 = dict(device=dev, dtype=torch.int64)
+        sc = dict(n_buckets=n_b, bucket_size_x=bsx, bucket_size_y=bsy, mix_x=mix, draw_given=False,
+                  draw=torch.zeros((T, n_b) if mix else (n_b, cfg.d), device=dev, dtype=torch.float32),
+                  top_x=torch.zeros(n_b, bsx, **i64), score_x=torch.zeros(n_b, bsx, device=dev, dtype=torch.float32),
+                  top_y=torch.zeros(n_b, bsy, **i64), n_rows=torch.full((1,), T, device=dev, dtype=torch.int32),
+                  ws=torch.zeros(ws_bytes, device=dev, dtype=torch.uint8))
+        desc = SceDesc()
+        desc.hc, desc.table = self.hc.data_ptr(), self.params16["item_emb"].data_ptr()
+        desc.labels, desc.pad_mask, desc.n_rows = self.in_labels.data_ptr(), self.in_pad.data_ptr(), sc["n_rows"].data_ptr()
+        desc.capacity, desc.n_items, desc.d, desc.d_true, desc.hd_valid = T, cfg.n_items, cfg.dp, cfg.d, cfg.hd_valid
+        desc.n_buckets, desc.bucket_size_x, desc.bucket_size_y, desc.mix_x = n_b, bsx, bsy, int(mix)
+        desc.seed, desc.rng_counter, desc.draw_given = self.seed, self.rng_counter.data_ptr(), 0
+        desc.draw, desc.top_x, desc.score_x, desc.top_y = (sc[k].data_ptr() for k in ("draw", "top_x", "score_x", "top_y"))
+        desc.loss_out = self.ce.loss.data_ptr()
+        desc.workspace, desc.workspace_bytes = sc["ws"].data_ptr(), ws_bytes
+        sc["desc"] = desc
+        self.sce = sc
+
+    def set_sce_draw(self, draw: torch.Tensor | None):
+        """Tests only: replace the Philox bucket draw by a fixed standard-normal draw - [n_buckets, d] (the model's true
+        hidden size), or with mix_x [B * L, n_buckets] for the staged batch - so that a reference run's captured
+        ``torch.randn`` can be replayed.  ``None`` returns to the Philox draw."""
+        sc = self.sce
+        if sc is None:
+            raise RuntimeError('set_loss("sce", ...) first')
+        if draw is None:
+            sc["desc"].draw_given = 0
+            return
+        if draw.dim() != 2 or draw.shape[1] != sc["draw"].shape[1] or draw.shape[0] > sc["draw"].shape[0] or (
+                not sc["mix_x"] and draw.shape[0] != sc["draw"].shape[0]):
+            raise ValueError(f"draw {tuple(draw.shape)} does not fit {tuple(sc['draw'].shape)}")
+        sc["draw"].zero_()
+        sc["draw"][: draw.shape[0]].copy_(draw)
+        sc["desc"].draw_given = 1
 
     def set_row_weights(self, weights):
         """Stage the sample weights of the current batch ([B, L] float, one per position; only valid targets are read)."""
@@ -753,6 +811,13 @@ class SasRecEngine:
     def forward_train(self):
         """Loss of the staged batch (device fp32 [2] view: mean CE over the valid targets, 1/n_valid)."""
         cfg, T = self.cfg, self.T
+        if self.sce is not None:
+            # SCE reads the final hidden state of every position, pad rows included (the mix_x buckets sum over them)
+            self._prepare(False)
+            self._body_forward(True)
+            self._ln_fwd(self.x[-1], self.params["lnf_w"], self.params["lnf_b"], cfg.lnf_eps, self.hc, self.meanf, self.rstdf, T)
+            check(self.lib.rp_sce_head_fwd(ctypes.byref(self.sce["desc"]), SCE_ALL, self._stream()), "rp_sce_head_fwd")
+            return self.ce.loss
         self._prepare(True)
         self._body_forward(True)
         self._ln_fwd(self.x[-1], self.params["lnf_w"], self.params["lnf_b"], cfg.lnf_eps, self.hc, self.meanf, self.rstdf, T,
@@ -791,6 +856,9 @@ class SasRecEngine:
             bce_head_bwd(self.ce, self.hc, p16["item_emb"][: cfg.n_items], self.labels_c, self.n_valid, s["dhc"], G["item_emb"],
                          n_valid_hint=self.n_valid_hint)
             self.lib.count += 3
+        elif self.sce is not None:
+            G["item_emb"].zero_()  # the reference's SCE scores a detached copy of the table: only the input gather reaches it
+            check(self.lib.rp_sce_head_bwd(ctypes.byref(self.sce["desc"]), s["dhc"].data_ptr(), st()), "rp_sce_head_bwd")
         elif self.sampled is not None:
             G["item_emb"].zero_()  # the sampled head accumulates sparse rows (the full-CE head overwrites the dense table)
             check(self.lib.rp_sampled_head_bwd(ctypes.byref(self._sampled_desc()), s["dhc"].data_ptr(), G["item_emb"].data_ptr(),
@@ -801,8 +869,11 @@ class SasRecEngine:
             self.lib.count += 3
         dx = s["dxa"]
         dx.zero_()
-        self._ln_bwd(s["dhc"], self.x[-1], prm["lnf_w"], self.meanf, self.rstdf, dx, G["lnf_w"], G["lnf_b"], T,
-                     gather=self.valid_idx, n_rows_dev=self.n_valid)
+        if self.sce is not None:
+            self._ln_bwd(s["dhc"], self.x[-1], prm["lnf_w"], self.meanf, self.rstdf, dx, G["lnf_w"], G["lnf_b"], T)
+        else:
+            self._ln_bwd(s["dhc"], self.x[-1], prm["lnf_w"], self.meanf, self.rstdf, dx, G["lnf_w"], G["lnf_b"], T,
+                         gather=self.valid_idx, n_rows_dev=self.n_valid)
         other = s["dxb"]
         for i in reversed(range(cfg.n_blocks)):
             a, x = self.act[i], self.x[i]

@@ -9,6 +9,7 @@ import torch
 from ....compat import LightningModuleBase
 from ....core import SasRecCore
 from ....engine import EncoderConfig
+from ..loss import check_sce_params
 from ....schema import item_feature_of
 
 
@@ -102,8 +103,11 @@ class SasRec(LightningModuleBase):
                  fused_optimizer: bool = True, device=None):
         super().__init__()
         self.save_hyperparameters()
-        if loss_type not in ("CE", "BCE") or (loss_type == "BCE" and loss_sample_count is None):
-            raise NotImplementedError("Not supported loss_type")  # lightning.py:485 ; full-catalog BCE / SCE: no fused head
+        if loss_type == "SCE":
+            assert sce_params is not None, "You should define ``sce_params`` when using SCE loss function."  # lightning.py:105-106
+            check_sce_params(sce_params)
+        elif loss_type not in ("CE", "BCE") or (loss_type == "BCE" and loss_sample_count is None):
+            raise NotImplementedError("Not supported loss_type")  # lightning.py:485 ; full-catalog BCE: no fused head
         if negative_sampling_strategy not in {"global_uniform", "inbatch"}:
             raise AssertionError("negative_sampling_strategy must be 'global_uniform' or 'inbatch'")
         if loss_sample_count is not None and negative_sampling_strategy != "global_uniform":
@@ -115,7 +119,15 @@ class SasRec(LightningModuleBase):
         self._loss_type, self._loss_sample_count = loss_type, loss_sample_count
         self._negative_sampling_strategy, self._negatives_sharing = negative_sampling_strategy, negatives_sharing
         self._vocab_size = self._model.item_count
-        if loss_sample_count is not None:
+        self._sce_params = sce_params if loss_type == "SCE" else None
+        if self._sce_params is not None:
+            p = self._sce_params
+            if p.bucket_size_y > min(1024, self._vocab_size):
+                raise ValueError(f"bucket_size_y = {p.bucket_size_y} exceeds min(1024, item count = {self._vocab_size}): "
+                                 "the fused top-K of the SCE head selects at most 1024 items per bucket")
+            self._model.core.set_loss("sce", n_buckets=p.n_buckets, bucket_size_x=p.bucket_size_x,
+                                      bucket_size_y=p.bucket_size_y, mix_x=bool(p.mix_x))
+        elif loss_sample_count is not None:
             self._model.core.set_loss("legacy_ce_sampled" if loss_type == "CE" else "legacy_bce_sampled")
         self._optimizer_factory = optimizer_factory
         self._lr_scheduler_factory = lr_scheduler_factory
@@ -144,7 +156,10 @@ class SasRec(LightningModuleBase):
         ids = batch["feature_tensor"][self._model.item_feature_name]
         args = (ids, batch["padding_mask"], batch["positive_labels"], batch["target_padding_mask"])
         core = self._model.core
-        neg = self._sample_negatives(ids) if self._loss_sample_count is not None else None
+        if self._sce_params is not None and self._sce_params.bucket_size_x > min(1024, ids.numel()):
+            raise ValueError(f"bucket_size_x = {self._sce_params.bucket_size_x} exceeds min(1024, B * L = {ids.numel()}): "
+                             "the fused top-K of the SCE head selects at most 1024 rows per bucket")
+        neg = (self._sample_negatives(ids) if self._loss_sample_count is not None and self._sce_params is None else None)
         if self.fused_optimizer:
             loss = core.fused_step(*args, lr=self._fused_lr(), negatives=neg)  # all_reduce="auto": DDP exchange inside
         else:
