@@ -288,15 +288,10 @@ int rp_bert_embed_bwd(const void* dx, const int32_t* ids, const uint8_t* pad_mas
 int rp_gather_rows(const void* src, const int32_t* idx, int n_max, const int32_t* n_dev, int d, void* dst, int scatter,
                    void* stream);
 
-/* Inference / predict(): the whole point-wise FFN in one pass  out = relu(y W1^T + b1) W2^T + b2 + y  (weights resident in shared
- * memory, hidden activation kept in registers, residual read from the staged y tile): y is read once and out written once.
- *   replaces (eval)  SasRecPointWiseFeedForward.forward  replay/models/nn/sequential/sasrec/model.py:496-506 ; replay/nn/ffn.py:43-57
- * y, out bf16 [T, d] (no aliasing), w1 / w2 bf16 [d, d], b1 / b2 fp32 [d], rowmask optional uint8 [T] (0 -> zero row), d in {64,128}. */
-int rp_ffn_fused(const void* y, const void* w1, const float* b1, const void* w2, const float* b2, const uint8_t* rowmask, int T,
-                 int d, void* out, void* stream);
-
 /* Inference: out-projection + residual + LayerNorm + FFN of one SASRec block in one pass  (h = o Wo^T + bo + q_in ;
- * y = LN(h) ; out = relu(y W1^T + b1) W2^T + b2 + y); h and y never reach HBM.  Shapes as rp_ffn_fused; out may not alias o / q_in.
+ * y = LN(h) ; out = relu(y W1^T + b1) W2^T + b2 + y); h and y never reach HBM.
+ * o, q_in, out bf16 [T, d] (out may not alias o / q_in); wo / w1 / w2 bf16 [d, d]; bo, ln_w, ln_b, b1, b2 fp32 [d]; rowmask
+ * optional uint8 [T] (0 -> zero row); d in {64,128}.
  *   replaces (eval)  replay/nn/sequential/sasrec/transformer.py:99-110 ; replay/models/nn/sequential/sasrec/model.py:435-441 */
 int rp_post_attn_fused(const void* o, const void* q_in, const void* wo, const float* bo, const float* ln_w, const float* ln_b,
                        float eps, const void* w1, const float* b1, const void* w2, const float* b2, const uint8_t* rowmask, int T,

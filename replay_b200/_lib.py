@@ -90,7 +90,6 @@ def lib():
     _sig(L.rp_selftest_tma_probe, c_int, [P, LL, c_int, c_int, c_int, c_int, c_int, P])
     _sig(L.rp_colsum_multi, c_int, [c_int, P, P, P, P, c_int, P])
     _sig(L.rp_post_attn_fused, c_int, [P, P, P, P, P, P, c_float, P, P, P, P, P, c_int, c_int, P, c_int, P])
-    _sig(L.rp_ffn_fused, c_int, [P, P, P, P, P, P, c_int, c_int, P, P])
     _sig(L.rp_build_batch, c_int, [P, P, LL, P, P, c_int, c_int, c_int, c_int, c_float, P, U64, U64, P, P, P, P, P, P, P])
     _sig(L.rp_post_attn_train, c_int, [P, P, P, P, P, P, c_float, P, P, P, P, P, c_int, c_int, c_float, U64, U64, U64, P,
                                        P, P, P, P, P, P, c_int, P])

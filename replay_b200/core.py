@@ -90,8 +90,11 @@ class SasRecCore(torch.nn.Module):
         self._pending_state = None
         self._shadow_dirty = True
         self.adam_betas = (0.9, 0.98)  # optimizer_factory.py:56-63 / nn/lightning/optimizer.py:44-60
-        self._keymap = reference_key_map(cfg.variant, cfg.n_blocks, item_feature)
+        self._keymap = self._key_map()
         self._materialise()
+
+    def _key_map(self) -> dict:
+        return reference_key_map(self.cfg.variant, self.cfg.n_blocks, self.item_feature)
 
     def _materialise(self):
         """Parameters exist from construction on (their layout depends on the configuration only), so ``parameters()``,
@@ -154,17 +157,16 @@ class SasRecCore(torch.nn.Module):
     def _to_ref(self, k, v):
         return v.unsqueeze(-1) if k.endswith((".w1", ".w2")) else v  # Conv1d weight [d, d, 1]
 
+    def _from_ref(self, k, v):
+        return v[:, :, 0] if k.endswith((".w1", ".w2")) and v.dim() == 3 else v
+
     def _import(self, state: dict):
         inv = {v: k for k, v in self._keymap.items()}
         with torch.no_grad():
             for rk, val in state.items():
                 k = inv.get(rk)
-                if k is None:
-                    continue
-                val = val.to(self.engine.dev, torch.float32)
-                if k.endswith((".w1", ".w2")) and val.dim() == 3:
-                    val = val[:, :, 0]
-                self.engine.import_named(k, val)
+                if k is not None:
+                    self.engine.import_named(k, self._from_ref(k, val))
         self._shadow_dirty = True
 
     # ---- reference-compatible checkpoints

@@ -378,104 +378,14 @@ RP_API int rp_pre_attn_bwd(const void* dQ, const void* dKV, const void* dh, cons
 
 
 // ==================================================================================================================
-// Point-wise feed-forward for inference / predict():  out = relu(y W1^T + b1) W2^T + b2 + y  in ONE pass.
-//   replaces  SasRecPointWiseFeedForward.forward (eval)   replay/models/nn/sequential/sasrec/model.py:496-506
-//             PointWiseFeedForward.forward (eval)          replay/nn/ffn.py:43-57
-// predict() is HBM-bound on [T, d] activation passes (T = users x L tokens); two GEMM launches read y, write u, read u, read y
-// again (residual) and write the result.  Here both d x d weights stay resident in shared memory, a persistent CTA walks
-// 128-token tiles of y (TMA), the hidden activation u never leaves the registers (bf16, the A operand of the second wgmma)
-// and the residual is read from the y tile that is already in shared memory: y is read once, the result written once.
-// d in {64, 128}.
+// Post-attention block (out-projection + LayerNorm + point-wise feed-forward) for inference and training.
 
 namespace rp {
-
-struct FfnParams {
-  const float* b1;
-  const float* b2;
-  const uint8_t* rowmask;   // optional [T]: rows with 0 are written as zeros (legacy SASRec pad rows)
-  __nv_bfloat16* out;       // [T, d]
-  int T;
-};
-
-template <int KCH /* d / 64 */>
-__global__ void __launch_bounds__(kBlockThreads, 1)
-ffn_fused_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmW1,
-                 const __grid_constant__ CUtensorMap tmW2, const FfnParams p) {
-  constexpr int D = KCH * 64, R = D / 2;
-  constexpr int W_BYTES = KCH * D * 128;      // [D x D] bf16 as KCH chunks of [D rows x 64]
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sW1 = smem;
-  uint8_t* sW2 = smem + W_BYTES;
-  uint8_t* sY = smem + 2 * W_BYTES;           // [128 x D]
-  __shared__ uint64_t bar_w, bar_y;
-  __shared__ __align__(16) float s_b1[D], s_b2[D];
-
-  const int n_tiles = (p.T + 127) / 128;
-  const int my_tiles = n_tiles > (int)blockIdx.x ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-  auto load_y = [&](int it) {
-    const int t = (int)blockIdx.x + it * (int)gridDim.x;
-    mbar_arrive_expect_tx(&bar_y, KCH * 16384);
-    for (int kc = 0; kc < KCH; ++kc) tma_load_2d(sY + kc * 16384, &tmY, &bar_y, kc * 64, t * 128);
-  };
-  if (threadIdx.x == 0) {
-    mbar_init(&bar_w, 1);
-    mbar_init(&bar_y, 1);
-    fence_barrier_init();
-    mbar_arrive_expect_tx(&bar_w, 2 * W_BYTES);
-    for (int kc = 0; kc < KCH; ++kc) {
-      tma_load_2d(sW1 + kc * (D * 128), &tmW1, &bar_w, kc * 64, 0);
-      tma_load_2d(sW2 + kc * (D * 128), &tmW2, &bar_w, kc * 64, 0);
-    }
-    if (my_tiles > 0) load_y(0);
-  }
-  for (int i = threadIdx.x; i < D; i += kBlockThreads) {
-    s_b1[i] = p.b1[i];
-    s_b2[i] = p.b2[i];
-  }
-  __syncthreads();
-  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127;
-  const int fr = frag_row(t), fc = frag_col(t);
-  mbar_wait(&bar_w, 0);
-  for (int it = 0; it < my_tiles; ++it) {
-    const int tile = (int)blockIdx.x + it * (int)gridDim.x;
-    const int ra = tile * 128 + 64 * wg + fr;
-    mbar_wait(&bar_y, it & 1);
-    float acc[R], yv[R];
-    wg_gemm_ss_wt<D, KCH>(acc, smem_u32(sY) + wg * 8192, smem_u32(sW1));   // y . W1^T
-    frag_load_tile(sY, 64 * wg + fr, yv);
-    named_bar_sync(1, kBlockThreads);   // the y tile has been read
-    if (threadIdx.x == 0 && it + 1 < my_tiles) load_y(it + 1);
-    uint32_t pu[R / 2];
-#pragma unroll
-    for (int j = 0; j < R / 4; ++j) {
-      const float b0 = s_b1[8 * j + fc], b1 = s_b1[8 * j + fc + 1];
-      pu[2 * j] = pack_bf16(fmaxf(acc[4 * j] + b0, 0.f), fmaxf(acc[4 * j + 1] + b1, 0.f));
-      pu[2 * j + 1] = pack_bf16(fmaxf(acc[4 * j + 2] + b0, 0.f), fmaxf(acc[4 * j + 3] + b1, 0.f));
-    }
-    wg_gemm_rs_wt<D, KCH>(acc, pu, smem_u32(sW2));   // u . W2^T
-    float keep[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int r = ra + 8 * h;
-      keep[h] = (p.rowmask == nullptr || (r < p.T && p.rowmask[r])) ? 1.f : 0.f;
-    }
-    uint32_t po[R / 2];
-#pragma unroll
-    for (int j = 0; j < R / 4; ++j)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int i = 4 * j + 2 * h, c = 8 * j + fc;
-        po[2 * j + h] = pack_bf16((acc[i] + s_b2[c] + yv[i]) * keep[h], (acc[i + 1] + s_b2[c + 1] + yv[i + 1]) * keep[h]);
-      }
-    frag_store_bf16(po, p.out, D, ra, p.T);
-  }
-}
 
 // ------------------------------------------------------------------------------------------------------------------
 // Everything after the attention of one SASRec block in ONE pass over the tokens:
 //   h = O Wo^T + bo + q_in ;  y = LayerNorm(h) ;  out = relu(y W1^T + b1) W2^T + b2 + y
-// (replaces out-projection GEMM + LayerNorm + the FFN above: h and y never reach HBM in inference).  Per 128-token tile three
+// (replaces out-projection GEMM + LayerNorm + two FFN GEMMs: h and y never reach HBM in inference).  Per 128-token tile three
 // chained wgmma GEMMs; y and u stay in registers as the bf16 A operands of the next one, the LayerNorm statistics of a row
 // come from the four threads of a quad.
 // ------------------------------------------------------------------------------------------------------------------
@@ -662,41 +572,9 @@ static int launch_post_attn(const CUtensorMap& tmO, const CUtensorMap& tmWo, con
   return RP_OK;
 }
 
-template <int KCH>
-static int launch_ffn(const CUtensorMap& tmY, const CUtensorMap& tmW1, const CUtensorMap& tmW2, const FfnParams& p,
-                      cudaStream_t st) {
-  constexpr int D = KCH * 64;
-  const int smem = 2 * KCH * D * 128 + KCH * 128 * 128 + 1024;
-  auto kern = ffn_fused_kernel<KCH>;
-  RP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  const int n_tiles = (p.T + 127) / 128;
-  const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
-  kern<<<grid, kBlockThreads, smem, st>>>(tmY, tmW1, tmW2, p);
-  RP_LAUNCH_CHECK();
-  return RP_OK;
-}
-
 }  // namespace rp
 
 using namespace rp;
-
-// y, out bf16 [T, d] (out may not alias y); w1, w2 bf16 [d, d] (row = output feature, as torch Linear / Conv1d(k=1) weights);
-// b1, b2 fp32 [d]; rowmask optional uint8 [T].  d in {64, 128}.
-RP_API int rp_ffn_fused(const void* y, const void* w1, const float* b1, const void* w2, const float* b2,
-                        const uint8_t* rowmask, int T, int d, void* out, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!y || !w1 || !b1 || !w2 || !b2 || !out || T <= 0) return RP_EINVAL;
-  if (d != 64 && d != 128) return RP_ESHAPE;
-  if (y == out) return RP_EINVAL;
-  CUtensorMap tmY, tmW1, tmW2;
-  int rc;
-  if ((rc = make_tmap_bf16(&tmY, y, T, d, d, 128)) != RP_OK) return rc;
-  if ((rc = make_tmap_bf16(&tmW1, w1, d, d, d, d)) != RP_OK) return rc;
-  if ((rc = make_tmap_bf16(&tmW2, w2, d, d, d, d)) != RP_OK) return rc;
-  FfnParams p;
-  p.b1 = b1; p.b2 = b2; p.rowmask = rowmask; p.out = reinterpret_cast<__nv_bfloat16*>(out); p.T = T;
-  return d == 64 ? launch_ffn<1>(tmY, tmW1, tmW2, p, stream) : launch_ffn<2>(tmY, tmW1, tmW2, p, stream);
-}
 
 // Inference: out-projection + residual + LayerNorm + FFN of one SASRec block in one pass (see post_attn_fused_kernel).
 //   o, q_in, out bf16 [T, d] (out may not alias o / q_in); wo, w1, w2 bf16 [d, d]; bo, ln_w, ln_b, b1, b2 fp32 [d]; d in {64,128}.

@@ -22,20 +22,25 @@ import torch
 from ._lib import SCE_ALL, SampledDesc, SceDesc, AttnBwdDesc, AttnDesc, GemmDesc, WgradPair, check, lib
 
 
+_BLOCK_PARAMS = ("ln1_w", "ln1_b", "in_w", "in_b", "out_w", "out_b", "ln2_w", "ln2_b", "w1", "b1", "w2", "b2")
+
+
+def _ru(x, m):
+    return (x + m - 1) // m * m
+
+
 @dataclass
-class EncoderConfig:
+class BaseConfig:
+    """What SASRec (EncoderConfig) and BERT4Rec (BertConfig) share: the transformer's sizes, the feature-slot geometry
+    the kernels see, and the padded parameter layout with its pad kinds."""
     n_items: int
     d: int
     n_heads: int
     n_blocks: int
     max_len: int
     dropout: float = 0.0
-    variant: str = "new"  # "new": replay.nn.sequential.SasRec ; "legacy": replay.models.nn.sequential.SasRecModel
-    lnf_eps: float | None = None
 
     def __post_init__(self):
-        if self.variant not in ("new", "legacy"):
-            raise ValueError(f"unknown variant {self.variant}")
         if self.d % self.n_heads:
             raise ValueError("d must be divisible by n_heads")
         if self.d // self.n_heads > 128:
@@ -43,13 +48,6 @@ class EncoderConfig:
         if self.dp not in (64, 128, 256, 512):
             raise ValueError(f"hidden size {self.d} with {self.n_heads} heads needs {self.dp} padded columns; the kernels "
                              "support 64/128/256/512 (= n_heads x 64-wide slots, or 128-wide for head_dim > 64)")
-        if self.lnf_eps is None:
-            # new: torch.nn.LayerNorm default (nn/sequential/sasrec/model.py:248); legacy: 1e-8 (sasrec/model.py:463)
-            self.lnf_eps = 1e-5 if self.variant == "new" else 1e-8
-
-    @property
-    def pad_id(self) -> int:
-        return self.n_items
 
     # ---- feature slots: every head occupies one 64-wide (head_dim <= 64) or 128-wide tensor-core slot.  The reference's own
     # defaults (embedding_dim 192 / 4 heads -> head_dim 48; legacy hidden_size 50; examples d 64 / 2 heads -> 32) leave padded
@@ -78,12 +76,52 @@ class EncoderConfig:
         j = torch.arange(self.head_dim, device=device).repeat(self.n_heads)
         return h * self.head_slot + j
 
+    # ---- padded parameter layout: (name, padded shape, (row kind, column kind)) in flat-buffer order.  Pad kinds: 'f' = a
+    # feature axis (true features scattered into the head slots), 'f3' = three stacked feature axes (packed in-projection),
+    # None = not padded; BertConfig adds the FFN's inner axis and the head bias, whose true entries lead.
+    def param_layout(self) -> list:
+        raise NotImplementedError
 
-_BLOCK_PARAMS = ("ln1_w", "ln1_b", "in_w", "in_b", "out_w", "out_b", "ln2_w", "ln2_b", "w1", "b1", "w2", "b2")
+    def axis_sizes(self) -> dict:
+        """true size of every pad kind"""
+        return {"f": self.d, "f3": 3 * self.d}
+
+    def true_shapes(self) -> dict:
+        """name -> shape of the parameter in the reference model"""
+        size = self.axis_sizes()
+        return {name: tuple(n if k is None else size[k] for n, k in zip(shp, kinds)) for name, shp, kinds in self.param_layout()}
+
+    def _block_layout(self, i: int, ffn: int, ffn_kind: str) -> list:
+        """block ``i``'s parameters (_BLOCK_PARAMS order) with an FFN inner axis of ``ffn`` columns of kind ``ffn_kind``"""
+        d, vec, mat = self.dp, ("f", None), ("f", "f")
+        shapes = ((d,), (d,), (3 * d, d), (3 * d,), (d, d), (d,), (d,), (d,), (ffn, d), (ffn,), (d, ffn), (d,))
+        kinds = (vec, vec, ("f3", "f"), ("f3", None), mat, vec, vec, vec, (ffn_kind, "f"), (ffn_kind, None), ("f", ffn_kind), vec)
+        return [(f"b{i}.{k}", s, pk) for k, s, pk in zip(_BLOCK_PARAMS, shapes, kinds)]
 
 
-def _ru(x, m):
-    return (x + m - 1) // m * m
+@dataclass
+class EncoderConfig(BaseConfig):
+    variant: str = "new"  # "new": replay.nn.sequential.SasRec ; "legacy": replay.models.nn.sequential.SasRecModel
+    lnf_eps: float | None = None
+
+    def __post_init__(self):
+        if self.variant not in ("new", "legacy"):
+            raise ValueError(f"unknown variant {self.variant}")
+        super().__post_init__()
+        if self.lnf_eps is None:
+            # new: torch.nn.LayerNorm default (nn/sequential/sasrec/model.py:248); legacy: 1e-8 (sasrec/model.py:463)
+            self.lnf_eps = 1e-5 if self.variant == "new" else 1e-8
+
+    @property
+    def pad_id(self) -> int:
+        return self.n_items
+
+    def param_layout(self) -> list:
+        d, emb, vec = self.dp, (None, "f"), ("f", None)
+        out = [("item_emb", (self.n_items + 1, d), emb), ("pos_emb", (self.max_len, d), emb)]
+        for i in range(self.n_blocks):
+            out += self._block_layout(i, d, "f")
+        return out + [("lnf_w", (d,), vec), ("lnf_b", (d,), vec)]
 
 
 class _CountingLib:
@@ -92,7 +130,7 @@ class _CountingLib:
     KERNELS = {"rp_gemm": 1, "rp_attn_fwd": 1, "rp_attn_bwd": 1, "rp_attn_last": 1, "rp_attn_softmax_bwd": 1, "rp_prepare_batch": 2, "rp_embed_fwd": 1,
                "rp_embed_bwd": 2, "rp_layernorm_fwd": 1, "rp_layernorm_bwd": 1, "rp_dropout_bwd": 1, "rp_colsum": 1, "rp_colsum_multi": 1,
                "rp_adam_step": 2, "rp_cast_bf16": 1, "rp_counter_add": 1, "rp_reduce_splits": 1, "rp_ce_head_fwd": 2, "rp_ce_head_bwd": 3,
-               "rp_score_topk": 2, "rp_seen_prepare": 1, "rp_sampled_head_fwd": 4, "rp_sampled_head_bwd": 4, "rp_ffn_fused": 1, "rp_post_attn_fused": 1,
+               "rp_score_topk": 2, "rp_seen_prepare": 1, "rp_sampled_head_fwd": 4, "rp_sampled_head_bwd": 4, "rp_post_attn_fused": 1,
                "rp_post_attn_train": 1, "rp_wgrad_group": 2, "rp_ln_qkv_fused": 1, "rp_pre_attn_bwd": 1,
                "rp_post_attn_bwd": 1}
 
@@ -125,21 +163,14 @@ class SasRecEngine:
         self.Lp = _ru(seq_len, 64)
         self.with_grad = with_grad
         self.lib = _CountingLib(lib())
-        d, I = cfg.dp, cfg.n_items   # padded width: what buffers and kernels use; cfg.d is the model's true hidden size
+        d = cfg.dp   # padded width: what buffers and kernels use; cfg.d is the model's true hidden size
         self._feat = cfg.feat_index(self.dev)
         # ---------------------------------------------------------------- flat parameter layout
-        shapes = [("item_emb", (I + 1, d)), ("pos_emb", (cfg.max_len, d))]
-        for i in range(cfg.n_blocks):
-            shapes += [(f"b{i}.ln1_w", (d,)), (f"b{i}.ln1_b", (d,)), (f"b{i}.in_w", (3 * d, d)), (f"b{i}.in_b", (3 * d,)),
-                       (f"b{i}.out_w", (d, d)), (f"b{i}.out_b", (d,)), (f"b{i}.ln2_w", (d,)), (f"b{i}.ln2_b", (d,)),
-                       (f"b{i}.w1", (d, d)), (f"b{i}.b1", (d,)), (f"b{i}.w2", (d, d)), (f"b{i}.b2", (d,))]
-        shapes += [("lnf_w", (d,)), ("lnf_b", (d,))]
-        self.layout = {}
-        off = 0
-        for name, shp in shapes:
-            n = math.prod(shp)
-            self.layout[name] = (off, shp)
-            off = _ru(off + n, 64)
+        self.layout, self._kinds, off = {}, {}, 0
+        for name, shp, kinds in cfg.param_layout():
+            self.layout[name], self._kinds[name] = (off, shp), kinds
+            off = _ru(off + math.prod(shp), 64)
+        self._true = cfg.true_shapes()
         self.n_flat = off
         f32 = dict(device=self.dev, dtype=torch.float32)
         self.p32 = torch.zeros(off, **f32)
@@ -155,9 +186,8 @@ class SasRecEngine:
         self.fused_attn_bwd = cfg.head_slot == 64 and seq_len <= 256
         self.sampled = None       # full-catalog CE unless set_loss() selects a sampled head
         self.sce = None           # buffers of the scalable CE head (set_loss("sce", ...))
+        self.bce, self.ce_row = False, None   # full-catalog BCE / per-row CE variants (set_loss)
         self._loss_args = None
-        self.fused_ffn_eval = True  # eval / predict: one-pass FFN kernel for d <= 128
-        self.fused_post_attn_eval = True  # eval / predict: out-projection + LayerNorm + FFN in one kernel for d <= 128
         # training: out-projection + LayerNorm + FFN (+ dropouts, saved activations) in one pass for d <= 128; all weight / bias
         # gradients of a block in one grouped launch (RP_FUSED_BODY=0 restores round 1's launch-per-GEMM body for A/B runs)
         fused_body = os.environ.get("RP_FUSED_BODY", "1") != "0"
@@ -209,75 +239,62 @@ class SasRecEngine:
         self.T = max_batch * seq_len
         self.Lp = _ru(seq_len, 64)
         self.fused_attn_bwd = self.cfg.head_slot == 64 and seq_len <= 256
-        self._realloc_workspace()
+        self._alloc_workspace()
         if self._loss_args is not None and self._loss_args[0] != "ce":  # sampled-head buffers are sized by (B, T)
             self.sampled = None
             if self.with_grad:
                 self.set_loss(*self._loss_args[:1], **self._loss_args[1])
         return self
 
-    def _realloc_workspace(self):
-        self._alloc_workspace()
-
     # ------------------------------------------------------------------------------------------------ parameters
     def _pad_kind(self, name: str):
-        """(row kind, column kind) of a parameter in the padded layout: 'f' = feature axis (scattered into the head slots),
-        'f3' = three stacked feature axes (packed in-projection), None = not a feature axis."""
-        leaf = name.split(".")[-1]
-        if leaf in ("item_emb", "pos_emb"):
-            return (None, "f")
-        if leaf == "in_w":
-            return ("f3", "f")
-        if leaf == "in_b":
-            return ("f3", None)
-        if leaf in ("out_w", "w1", "w2"):
-            return ("f", "f")
-        return ("f", None)  # LayerNorm weights / biases, linear biases
+        """(row kind, column kind) of a parameter in the padded layout (BaseConfig.param_layout)."""
+        return self._kinds[name]
 
     def _axis_index(self, kind):
+        """padded position of every true entry of an axis of pad kind ``kind``"""
         if kind == "f":
             return self._feat
-        dp = self.cfg.dp
-        return torch.cat([self._feat + k * dp for k in range(3)])
+        if kind == "f3":
+            return torch.cat([self._feat + k * self.cfg.dp for k in range(3)])
+        return torch.arange(self.cfg.axis_sizes()[kind], device=self.dev)   # true entries first, zero tail
+
+    def _true_index(self, name: str, shape):
+        """(rows, cols | None): where the true entries of parameter ``name`` sit in its padded tensor"""
+        idx = [self._axis_index(k) if k else torch.arange(n, device=self.dev) for n, k in zip(shape, self._kinds[name])]
+        return idx[0], (idx[1] if len(idx) == 2 else None)
 
     def import_named(self, name: str, value: torch.Tensor, dst=None):
         """Write a TRUE-shape tensor (reference layout) into the padded parameter ``name`` (padded entries become zero)."""
         tgt = (self.params if dst is None else dst)[name]
         v = value.to(self.dev, torch.float32)
-        if self._hdv() == 0:
+        if self._true[name] == tgt.shape:
             tgt.copy_(v.reshape(tgt.shape))
             return
-        rk, ck = self._pad_kind(name)
+        rows, cols = self._true_index(name, tgt.shape)
         tgt.zero_()
-        if tgt.dim() == 1:
-            tgt[self._axis_index(rk)] = v
+        if cols is None:
+            tgt[rows] = v.reshape(-1)
         else:
-            rows = self._axis_index(rk) if rk else torch.arange(tgt.shape[0], device=self.dev)
-            cols = self._axis_index(ck) if ck else torch.arange(tgt.shape[1], device=self.dev)
-            tgt[rows[:, None], cols[None, :]] = v
+            tgt[rows[:, None], cols[None, :]] = v.reshape(len(rows), len(cols))
 
     def export_named(self, name: str, source=None) -> torch.Tensor:
-        """The TRUE-shape view (a copy) of the padded parameter / gradient ``name``."""
+        """The TRUE-shape view (a copy) of the padded parameter / gradient / moment ``name``."""
         t = (self.params if source is None else source)[name].detach()
-        if self._hdv() == 0:
+        if self._true[name] == t.shape:
             return t.clone()
-        rk, ck = self._pad_kind(name)
-        if t.dim() == 1:
-            return t[self._axis_index(rk)].clone()
-        rows = self._axis_index(rk) if rk else torch.arange(t.shape[0], device=t.device)
-        cols = self._axis_index(ck) if ck else torch.arange(t.shape[1], device=t.device)
-        return t[rows[:, None], cols[None, :]].clone()
+        rows, cols = self._true_index(name, t.shape)
+        return (t[rows] if cols is None else t[rows[:, None], cols[None, :]]).clone()
 
     def true_shape(self, name: str):
-        d, dp = self.cfg.d, self.cfg.dp
-        return tuple({dp: d, 3 * dp: 3 * d, 2 * dp: 2 * d}.get(x, x) for x in self.layout[name][1]) if self._hdv() else self.layout[name][1]
+        return self._true[name]
 
     def init_parameters(self, seed: int = 0):
-        """Reference-style init: xavier_normal_ on >=2-D tensors, LN (1, 0), biases zero / U(+-1/sqrt(fan_in)) for the
-        conv layers, pad row zero (new path, nn/embedding.py:198-200) - drawn in the model's TRUE shapes, then laid out in the
-        head slots.  Weights are normally loaded from a reference state_dict instead (``load_canonical``)."""
+        """Reference-style init: xavier_normal_ on >=2-D tensors, LN (1, 0), FFN biases U(+-1/sqrt(fan_in)), other biases
+        zero, pad row zero (SASRec new path, nn/embedding.py:198-200; BERT4Rec: bert4rec/model.py:167-170) - drawn in the
+        model's TRUE shapes, then laid out in the head slots.  Weights are normally loaded from a reference state_dict instead
+        (``load_canonical``)."""
         g = torch.Generator(device="cpu").manual_seed(seed)
-        d = self.cfg.d
         with torch.no_grad():
             for name in self.layout:
                 shp = self.true_shape(name)
@@ -289,7 +306,8 @@ class SasRecEngine:
                 elif name.endswith(("ln1_w", "ln2_w", "lnf_w")):
                     v = torch.ones(shp)
                 elif name.endswith((".b1", ".b2")):
-                    v = (torch.rand(shp, generator=g) * 2 - 1) / math.sqrt(d)
+                    fan_in = self.true_shape(name[:-2] + "w" + name[-1])[1]
+                    v = (torch.rand(shp, generator=g) * 2 - 1) / math.sqrt(fan_in)
                 else:
                     v = torch.zeros(shp)
                 self.import_named(name, v)
@@ -299,30 +317,34 @@ class SasRecEngine:
         check(self.lib.rp_cast_bf16(self.p32.data_ptr(), self.p16.data_ptr(), self.n_flat, self._stream()), "rp_cast_bf16")
 
     def load_canonical(self, P: dict):
-        """Copy weights from the canonical dict used by oracle/ (keys item_emb, pos_emb, blocks[i][...], lnf_w, lnf_b)."""
+        """Copy weights from the canonical dict used by oracle/ (true shapes; block parameters under blocks[i][...], every
+        other parameter under its own name)."""
         with torch.no_grad():
-            self.import_named("item_emb", P["item_emb"])
-            self.import_named("pos_emb", P["pos_emb"])
-            for i, blk in enumerate(P["blocks"]):
-                for k in _BLOCK_PARAMS:
-                    self.import_named(f"b{i}.{k}", blk[k])
-            self.import_named("lnf_w", P["lnf_w"])
-            self.import_named("lnf_b", P["lnf_b"])
+            for name in self.layout:
+                blk, _, leaf = name.partition(".")
+                self.import_named(name, P["blocks"][int(blk[1:])][leaf] if leaf else P[name])
         self.refresh_shadow()
 
     def export_canonical(self, source=None) -> dict:
-        ex = lambda k: self.export_named(k, source).cpu()  # noqa: E731
-        P = {"item_emb": ex("item_emb"), "pos_emb": ex("pos_emb"), "blocks": [], "lnf_w": ex("lnf_w"), "lnf_b": ex("lnf_b")}
-        for i in range(self.cfg.n_blocks):
-            P["blocks"].append({k: ex(f"b{i}.{k}") for k in _BLOCK_PARAMS})
+        P = {}
+        for name in self.layout:
+            v = self.export_named(name, source).cpu()
+            blk, _, leaf = name.partition(".")
+            if not leaf:
+                P[name] = v
+                continue
+            blocks = P.setdefault("blocks", [])
+            if int(blk[1:]) == len(blocks):
+                blocks.append({})
+            blocks[-1][leaf] = v
         return P
 
     def unpad_features(self, t: torch.Tensor) -> torch.Tensor:
         """[..., dp] activations -> [..., d] (the reference's hidden size)"""
-        return t if self._hdv() == 0 else t[..., self._feat].contiguous()
+        return t if self.cfg.hd_valid == 0 else t[..., self._feat].contiguous()
 
     def pad_features(self, t: torch.Tensor) -> torch.Tensor:
-        if self._hdv() == 0:
+        if self.cfg.hd_valid == 0:
             return t
         out = torch.zeros(*t.shape[:-1], self.cfg.dp, device=t.device, dtype=t.dtype)
         out[..., self._feat] = t
@@ -330,6 +352,8 @@ class SasRecEngine:
 
     # ------------------------------------------------------------------------------------------------ workspace
     def _alloc_workspace(self):
+        """Activation workspace of the current batch geometry: batch staging, hidden states, the attention core's saves,
+        LayerNorm statistics and the CE head's state here; the block program's own buffers in ``_alloc_body``."""
         cfg, T, d, dev = self.cfg, self.T, self.cfg.dp, self.dev
         self._alloc_B, self._alloc_T, self._sub_last_idx = self.B, self.T, {}
         bf = dict(device=dev, dtype=torch.bfloat16)
@@ -337,7 +361,6 @@ class SasRecEngine:
         i32 = dict(device=dev, dtype=torch.int32)
         BH = self.B * cfg.n_heads
         self.ids32 = torch.zeros(T, **i32)
-        self.pad_u8 = torch.zeros(T, device=dev, dtype=torch.uint8)
         self.in_ids = torch.zeros(T, device=dev, dtype=torch.int64)
         self.in_pad = torch.zeros(T, device=dev, dtype=torch.bool)
         self.in_labels = torch.zeros(T, device=dev, dtype=torch.int64)
@@ -346,14 +369,11 @@ class SasRecEngine:
         self.labels_c = torch.zeros(T, **i32)
         self.n_valid = torch.zeros(1, **i32)
         self.prep_scratch = torch.zeros((T + 1023) // 1024 + 1, **i32)
-        nb = cfg.n_blocks
-        self.x = [torch.zeros(T, d, **bf) for _ in range(nb + 1)]
+        self.x = [torch.zeros(T, d, **bf) for _ in range(cfg.n_blocks + 1)]
         self.act = []
-        for _ in range(nb):
-            a = {k: torch.zeros(T, d, **bf) for k in ("q_in", "Q", "O", "h", "y", "u")}
-            a["KV"] = torch.zeros(T, 2 * d, **bf)
-            for k in ("mean1", "rstd1", "mean2", "rstd2"):
-                a[k] = torch.zeros(T, **f32)
+        for _ in range(cfg.n_blocks):
+            a = {k: torch.zeros(T, **f32) for k in ("mean1", "rstd1", "mean2", "rstd2")}
+            a["O"] = torch.zeros(T, d, **bf)
             if self.with_grad:
                 if not self.fused_attn_bwd:
                     a["P"] = torch.zeros(BH, self.Lp, self.Lp, **bf)
@@ -361,22 +381,34 @@ class SasRecEngine:
                 a["m2"] = torch.zeros(BH, self.Lp, **f32)
             self.act.append(a)
         self.hc = torch.zeros(T, d, **bf)
-        self.meanf = torch.zeros(T, **f32)
-        self.rstdf = torch.zeros(T, **f32)
         self.hq = torch.zeros(self.B, d, **bf)
         self.last_idx = (torch.arange(self.B, device=dev, dtype=torch.int32) * self.L + (self.L - 1)).contiguous()
-        self.last_buf = {k: torch.zeros(self.B, d, **bf) for k in ("q_in", "Q", "O", "h", "y", "u")}
-        self.last_rows = torch.zeros(self.B, d, **bf)
-        self.last_pad = torch.zeros(self.B, device=dev, dtype=torch.bool)
         if self.with_grad:
             from .ops import CEHeadState
 
             self.ce = CEHeadState(T, cfg.n_items, d, dev)
-            self.s = {k: torch.zeros(T, d, **bf) for k in ("dhc", "dxa", "dxb", "d_t", "du", "dy", "dh", "d_o", "dQ", "dq_in", "tmp")}
-            self.s["dKV"] = torch.zeros(T, 2 * d, **bf)
+            self.s = {k: torch.zeros(T, d, **bf) for k in ("dhc", "dxa", "dxb", "d_o")}
             if not self.fused_attn_bwd:
                 self.s["dpd"] = torch.zeros(BH, self.Lp, self.Lp, **bf)
             self.wg_ws = torch.zeros(self.n_sm * 4 * d * d, **f32)  # split-K partials of the weight-gradient GEMMs
+        self._alloc_body()
+
+    def _alloc_body(self):
+        """SASRec's block buffers: LN1 output, Q and packed [K | V], the FFN's saved activations, the predict path's last-row
+        buffers and the backward's scratch."""
+        T, d, dev = self.T, self.cfg.dp, self.dev
+        bf = dict(device=dev, dtype=torch.bfloat16)
+        for a in self.act:
+            a.update({k: torch.zeros(T, d, **bf) for k in ("q_in", "Q", "h", "y", "u")})
+            a["KV"] = torch.zeros(T, 2 * d, **bf)
+        self.meanf = torch.zeros(T, device=dev, dtype=torch.float32)
+        self.rstdf = torch.zeros(T, device=dev, dtype=torch.float32)
+        self.last_buf = {k: torch.zeros(self.B, d, **bf) for k in ("q_in", "Q", "O", "h", "y", "u")}
+        self.last_rows = torch.zeros(self.B, d, **bf)
+        self.last_pad = torch.zeros(self.B, device=dev, dtype=torch.bool)
+        if self.with_grad:
+            self.s.update({k: torch.zeros(T, d, **bf) for k in ("d_t", "du", "dy", "dh", "dQ", "dq_in", "tmp")})
+            self.s["dKV"] = torch.zeros(T, 2 * d, **bf)
             self._wgrad_ws = None  # workspace of rp_wgrad_group, sized on first use
 
     def _stream(self):
@@ -450,8 +482,7 @@ class SasRecEngine:
         tiles = ((n_out + 127) // 128) * ((n_in + 127) // 128 if n_in > 64 else 1)
         chunks = (self.T + 63) // 64
         n = n_out * n_in
-        per = int(os.environ.get("RP_WGRAD_CHUNKS", "8"))
-        split = max(1, min(chunks // per, (self.n_sm + tiles - 1) // tiles, self.wg_ws.numel() // n))
+        split = max(1, min(chunks // 8, (self.n_sm + tiles - 1) // tiles, self.wg_ws.numel() // n))
         self._gemm(dY, X, self.wg_ws, n_out, n_in, self.T, a_mn=True, b_mn=True, out_mode=3, split_k=split,
                    c_geom=(n_in, 0, 0, 0), c_split_stride=n)
         check(self.lib.rp_reduce_splits(self.wg_ws.data_ptr(), split, n, n, dW.data_ptr(), 1, self._stream()), "rp_reduce_splits")
@@ -489,23 +520,17 @@ class SasRecEngine:
         check(self.lib.rp_colsum_multi(n, dy, cols, ld, db, pairs[0][0].shape[0], self._stream()), "rp_colsum_multi")
 
     def _ln_fwd(self, x, w, b, eps, y, mean, rstd, n_rows, gather=None, n_rows_dev=None):
-        check(self.lib.rp_layernorm_fwd(x.data_ptr(), w.data_ptr(), b.data_ptr(), eps, n_rows, self._dp(),
+        check(self.lib.rp_layernorm_fwd(x.data_ptr(), w.data_ptr(), b.data_ptr(), eps, n_rows, self.cfg.dp,
                                         None if n_rows_dev is None else n_rows_dev.data_ptr(),
                                         None if gather is None else gather.data_ptr(), y.data_ptr(), mean.data_ptr(),
-                                        rstd.data_ptr(), self._hdv(), self._stream()), "rp_layernorm_fwd")
+                                        rstd.data_ptr(), self.cfg.hd_valid, self._stream()), "rp_layernorm_fwd")
 
     def _ln_bwd(self, dy, x, w, mean, rstd, dx, dw, db, n_rows, gather=None, n_rows_dev=None, add_to=None):
         check(self.lib.rp_layernorm_bwd(dy.data_ptr(), x.data_ptr(), w.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
-                                        n_rows, self._dp(), None if n_rows_dev is None else n_rows_dev.data_ptr(),
+                                        n_rows, self.cfg.dp, None if n_rows_dev is None else n_rows_dev.data_ptr(),
                                         None if gather is None else gather.data_ptr(),
                                         None if add_to is None else add_to.data_ptr(), dx.data_ptr(), dw.data_ptr(),
-                                        db.data_ptr(), self._hdv(), self._stream()), "rp_layernorm_bwd")
-
-    def _dp(self) -> int:
-        return getattr(self.cfg, "dp", self.cfg.d)   # BertConfig has no padded layout
-
-    def _hdv(self) -> int:
-        return getattr(self.cfg, "hd_valid", 0)
+                                        db.data_ptr(), self.cfg.hd_valid, self._stream()), "rp_layernorm_bwd")
 
     def _site(self, blk, k):
         return 1 + blk * 8 + k
@@ -564,7 +589,7 @@ class SasRecEngine:
             raise NotImplementedError(f"Not supported loss_type {kind!r}")
         mode = {"shared": 0, "perpos": 1, "perseq": 2}[neg_shape]
         rows = {0: 1, 1: self.T, 2: self.B}[mode]
-        ws_bytes = self.lib.rp_sampled_head_workspace(self.T, self._dp(), n_neg, mode)
+        ws_bytes = self.lib.rp_sampled_head_workspace(self.T, self.cfg.dp, n_neg, mode)
         self.sampled = dict(kind=self.SAMPLED_KINDS[kind], n_neg=n_neg, mode=mode, ignore_index=ignore_index, log_eps=log_eps,
                             clamp=clamp, neg=torch.zeros(rows, n_neg, device=self.dev, dtype=torch.int64),
                             ws=torch.zeros(ws_bytes, device=self.dev, dtype=torch.uint8), ws_bytes=ws_bytes)
@@ -635,7 +660,7 @@ class SasRecEngine:
         sd.hc, sd.table = self.hc.data_ptr(), self.params16["item_emb"].data_ptr()
         sd.labels, sd.valid_idx, sd.negatives = self.labels_c.data_ptr(), self.valid_idx.data_ptr(), sp["neg"].data_ptr()
         sd.n_valid = self.n_valid.data_ptr()
-        sd.capacity, sd.n_items, sd.d, sd.n_neg, sd.neg_mode, sd.seq_len = self.T, cfg.n_items, self._dp(), sp["n_neg"], sp["mode"], self.L
+        sd.capacity, sd.n_items, sd.d, sd.n_neg, sd.neg_mode, sd.seq_len = self.T, cfg.n_items, cfg.dp, sp["n_neg"], sp["mode"], self.L
         sd.kind, sd.ignore_index, sd.vocab_size = sp["kind"], sp["ignore_index"], cfg.n_items
         sd.log_eps, sd.clamp = sp["log_eps"], sp["clamp"]
         sd.loss_out = self.ce.loss.data_ptr()
@@ -684,7 +709,7 @@ class SasRecEngine:
                 check(self.lib.rp_attn_last(lb["Q"].data_ptr(), a["KV"].data_ptr(), a["KV"].data_ptr(), 2 * d, 2 * d, 0, d,
                                             pad.data_ptr(), Bq, H, L, hd, int(not legacy), lb["O"].data_ptr(), att_scale,
                                             self._stream()), "rp_attn_last")
-                if d <= 128 and self.fused_post_attn_eval:
+                if d <= 128:
                     # out-projection + residual + LayerNorm + FFN of the B last rows in the same fused pass the full blocks
                     # use (one launch instead of GEMM, LayerNorm, GEMM, GEMM: ~10 us each on [4096, d] rows)
                     check(self.lib.rp_post_attn_fused(lb["O"].data_ptr(), lb["q_in"].data_ptr(), w("out_w").data_ptr(),
@@ -709,8 +734,8 @@ class SasRecEngine:
                 self._ln_fwd(x, f("ln1_w"), f("ln1_b"), 1e-8, a["q_in"], a["mean1"], a["rstd1"], T)
                 self._gemm(a["q_in"], in_w[:d], a["Q"], T, d, d, bias=in_b[:d])
                 self._gemm(x, in_w[d:], a["KV"], T, 2 * d, d, bias=in_b[d:])
-            self._attention_forward(i, training)
-            if not training and d <= 128 and self.fused_post_attn_eval:
+            self._attention_forward(i, training, (a["Q"], 0), (a["KV"], 0), (a["KV"], d), causal=True, mask_pad_keys=not legacy)
+            if not training and d <= 128:
                 # inference: out-projection + residual + LayerNorm + FFN in one pass over the tokens (csrc/rp_block_fused.cu)
                 check(self.lib.rp_post_attn_fused(a["O"].data_ptr(), a["q_in"].data_ptr(), w("out_w").data_ptr(),
                                                   f("out_b").data_ptr(), f("ln2_w").data_ptr(), f("ln2_b").data_ptr(), 1e-8,
@@ -731,82 +756,73 @@ class SasRecEngine:
                 continue
             self._gemm(a["O"], w("out_w"), a["h"], T, d, d, bias=f("out_b"), residual=a["q_in"])
             self._ln_fwd(a["h"], f("ln2_w"), f("ln2_b"), 1e-8, a["y"], a["mean2"], a["rstd2"], T)
-            if not training and d <= 128 and self.fused_ffn_eval:
-                # inference: both FFN GEMMs in one pass, the hidden activation never leaves the SM (csrc/rp_block_fused.cu)
-                check(self.lib.rp_ffn_fused(a["y"].data_ptr(), w("w1").data_ptr(), f("b1").data_ptr(), w("w2").data_ptr(),
-                                            f("b2").data_ptr(), pad.data_ptr() if legacy else None, T, d,
-                                            self.x[i + 1].data_ptr(), self._stream()), "rp_ffn_fused")
-                continue
             self._gemm(a["y"], w("w1"), a["u"], T, d, d, bias=f("b1"), act=1, drop_p=drop, drop_site=self._site(i, 1))
             self._gemm(a["u"], w("w2"), self.x[i + 1], T, d, d, bias=f("b2"), drop_p=drop, drop_site=self._site(i, 2),
                        residual=a["y"], rowmask=pad if legacy else None)
 
-    def _attention_forward(self, i: int, training: bool):
-        """Attention core of block ``i``: O = softmax(Q.K^T * scale, causal + pad-key mask) . V over act[i]'s Q and packed
-        [K | V] (one [T, 2d] array), saving the row statistics (and P on the un-fused path) when training with gradients."""
-        cfg, T, d, L = self.cfg, self.T, self.cfg.dp, self.L
-        H, a = cfg.n_heads, self.act[i]
-        ad = AttnDesc()
-        ad.q, ad.q_rows, ad.q_cols, ad.ldq, ad.q_c0 = a["Q"].data_ptr(), T, d, d, 0
-        ad.k, ad.k_rows, ad.k_cols, ad.ldk, ad.k_c0 = a["KV"].data_ptr(), T, 2 * d, 2 * d, 0
-        ad.v, ad.v_rows, ad.v_cols, ad.ldv, ad.v_c0 = a["KV"].data_ptr(), T, 2 * d, 2 * d, d
-        ad.B, ad.H, ad.L, ad.head_dim = self.B, H, L, d // H
-        ad.causal, ad.mask_pad_keys = 1, int(cfg.variant != "legacy")
-        ad.scale = 1.0 / math.sqrt(cfg.head_dim)
-        ad.pad_mask = self.in_pad.data_ptr()
-        ad.out, ad.ldo = a["O"].data_ptr(), d
+    def _attn_desc(self, desc, i, q, k, v, causal, mask_pad_keys, drop_p):
+        """The fields rp_attn_fwd's and rp_attn_bwd's descriptors share, for block ``i`` (output act[i]["O"])."""
+        cfg = self.cfg
+        for nm, (t, c0) in zip("qkv", (q, k, v)):
+            setattr(desc, nm, t.data_ptr())
+            setattr(desc, nm + "_rows", self.T)
+            setattr(desc, nm + "_cols", t.shape[1])
+            setattr(desc, "ld" + nm, t.stride(0))
+            setattr(desc, nm + "_c0", c0)
+        desc.B, desc.H, desc.L, desc.head_dim = self.B, cfg.n_heads, self.L, cfg.head_slot
+        desc.causal, desc.mask_pad_keys = int(causal), int(mask_pad_keys)
+        desc.scale = 1.0 / math.sqrt(cfg.head_dim)
+        desc.pad_mask = self.in_pad.data_ptr()
+        desc.out, desc.ldo = self.act[i]["O"].data_ptr(), cfg.dp
+        desc.drop_p, desc.seed, desc.drop_off, desc.seed_ptr = drop_p, self.seed, self._site(i, 0) << 40, self.rng_counter.data_ptr()
+        return desc
+
+    def _attention_forward(self, i: int, training: bool, q, k, v, causal: bool, mask_pad_keys: bool):
+        """Attention core of block ``i``: act[i]["O"] = softmax(Q.K^T * scale, causal and / or pad-key mask) . V, with Q, K
+        and V given as (tensor, first column) of [T, *] arrays; saves the row statistics (and P on the un-fused path) when
+        training with gradients."""
+        a = self.act[i]
+        ad = self._attn_desc(AttnDesc(), i, q, k, v, causal, mask_pad_keys, self.cfg.dropout if training else 0.0)
         if training and self.with_grad:
             ad.p_save = None if self.fused_attn_bwd else a["P"].data_ptr()
             ad.inv_sum, ad.m_save = a["inv_sum"].data_ptr(), a["m2"].data_ptr()
         else:
             ad.p_save, ad.inv_sum, ad.m_save = None, None, None
-        ad.drop_p = cfg.dropout if training else 0.0
-        ad.seed, ad.drop_off, ad.seed_ptr = self.seed, self._site(i, 0) << 40, self.rng_counter.data_ptr()
         check(self.lib.rp_attn_fwd(ctypes.byref(ad), self._stream()), "rp_attn_fwd")
 
-    def _attention_backward(self, i: int):
-        """dQ (into s["dQ"]) and packed [dK | dV] (into s["dKV"]) of block ``i``'s attention core from s["d_o"] and what
-        ``_attention_forward(i, True)`` saved: the fused kernel for head slot 64 at L <= 256, otherwise dPd = dO.V^T, the
-        row-wise softmax backward over the saved probabilities, and three batched GEMMs."""
+    def _attention_backward(self, i: int, q, k, v, dq, dk, dv, causal: bool, mask_pad_keys: bool):
+        """dQ, dK, dV of block ``i``'s attention core into the (tensor, first column) destinations ``dq``, ``dk``, ``dv`` from
+        s["d_o"] and what ``_attention_forward(i, True, q, k, v, ...)`` saved: the fused kernel for head slot 64 at L <= 256,
+        otherwise dPd = dO.V^T, the row-wise softmax backward over the saved probabilities, and three batched GEMMs."""
         cfg, T, d, L, Lp = self.cfg, self.T, self.cfg.dp, self.L, self.Lp
-        H, a, s, st = cfg.n_heads, self.act[i], self.s, self._stream
-        hd, BH = d // H, self.B * H
-        att_scale, drop = 1.0 / math.sqrt(cfg.head_dim), cfg.dropout
-        KV, Q = a["KV"], a["Q"]
+        a, s, drop = self.act[i], self.s, cfg.dropout
         if self.fused_attn_bwd:
-            bd = AttnBwdDesc()
-            bd.q, bd.q_rows, bd.q_cols, bd.ldq, bd.q_c0 = Q.data_ptr(), T, d, d, 0
-            bd.k, bd.k_rows, bd.k_cols, bd.ldk, bd.k_c0 = KV.data_ptr(), T, 2 * d, 2 * d, 0
-            bd.v, bd.v_rows, bd.v_cols, bd.ldv, bd.v_c0 = KV.data_ptr(), T, 2 * d, 2 * d, d
+            bd = self._attn_desc(AttnBwdDesc(), i, q, k, v, causal, mask_pad_keys, drop)
             bd.d_out, bd.do_rows, bd.do_cols, bd.ld_do = s["d_o"].data_ptr(), T, d, d
-            bd.out, bd.ldo = a["O"].data_ptr(), d
-            bd.B, bd.H, bd.L, bd.head_dim = self.B, H, L, hd
-            bd.causal, bd.mask_pad_keys = 1, int(cfg.variant != "legacy")
-            bd.scale = att_scale
-            bd.pad_mask = self.in_pad.data_ptr()
             bd.m_save, bd.inv_sum = a["m2"].data_ptr(), a["inv_sum"].data_ptr()
-            bd.dq, bd.ld_dq, bd.dq_c0 = s["dQ"].data_ptr(), d, 0
-            bd.dk, bd.ld_dk, bd.dk_c0 = s["dKV"].data_ptr(), 2 * d, 0
-            bd.dv, bd.ld_dv, bd.dv_c0 = s["dKV"].data_ptr(), 2 * d, d
-            bd.drop_p, bd.seed, bd.drop_off, bd.seed_ptr = drop, self.seed, self._site(i, 0) << 40, self.rng_counter.data_ptr()
-            check(self.lib.rp_attn_bwd(ctypes.byref(bd), st()), "rp_attn_bwd")
+            for nm, (t, c0) in zip(("dq", "dk", "dv"), (dq, dk, dv)):
+                setattr(bd, nm, t.data_ptr())
+                setattr(bd, "ld_" + nm, t.stride(0))
+                setattr(bd, nm + "_c0", c0)
+            check(self.lib.rp_attn_bwd(ctypes.byref(bd), self._stream()), "rp_attn_bwd")
             return
+        H, hd = cfg.n_heads, cfg.head_slot
+        BH = self.B * H
         P, dpd = a["P"].view(BH * Lp, Lp), s["dpd"].view(BH * Lp, Lp)
+        heads = dict(batch=BH, inner=H, a_off=(0, H * Lp, Lp, 0, 0, 0))   # A = dS / Pd [BH*Lp, Lp]
+        out = lambda t, c0: (t.stride(0), c0, L * t.stride(0), hd)  # noqa: E731  per-head [L, hd] blocks of a [T, *] array
         # dPd = dO . V^T
-        self._gemm(s["d_o"], KV, dpd, L, L, hd, batch=BH, inner=H, a_off=(0, L, 0, 0, 0, hd), b_off=(0, L, 0, d, 0, hd),
+        self._gemm(s["d_o"], v[0], dpd, L, L, hd, batch=BH, inner=H, a_off=(0, L, 0, 0, 0, hd), b_off=(0, L, 0, v[1], 0, hd),
                    c_geom=(Lp, 0, H * Lp * Lp, Lp * Lp))
         check(self.lib.rp_attn_softmax_bwd(P.data_ptr(), dpd.data_ptr(), a["inv_sum"].data_ptr(), BH, L,
-                                           att_scale, drop, self.seed, self._site(i, 0) << 40,
-                                           self.rng_counter.data_ptr(), st()), "rp_attn_softmax_bwd")
-        # dQ = dS . K      (A = dS [BH*Lp, Lp] K-major, B = K MN-major)
-        self._gemm(dpd, KV, s["dQ"], L, hd, L, b_mn=True, batch=BH, inner=H, a_off=(0, H * Lp, Lp, 0, 0, 0),
-                   b_off=(0, L, 0, 0, 0, hd), c_geom=(d, 0, L * d, hd))
+                                           1.0 / math.sqrt(cfg.head_dim), drop, self.seed, self._site(i, 0) << 40,
+                                           self.rng_counter.data_ptr(), self._stream()), "rp_attn_softmax_bwd")
+        # dQ = dS . K      (A = dS K-major, B = K MN-major)
+        self._gemm(dpd, k[0], dq[0], L, hd, L, b_mn=True, b_off=(0, L, 0, k[1], 0, hd), c_geom=out(*dq), **heads)
         # dK = dS^T . Q    (A = dS MN-major, B = Q MN-major)
-        self._gemm(dpd, Q, s["dKV"], L, hd, L, a_mn=True, b_mn=True, batch=BH, inner=H, a_off=(0, H * Lp, Lp, 0, 0, 0),
-                   b_off=(0, L, 0, 0, 0, hd), c_geom=(2 * d, 0, L * 2 * d, hd))
+        self._gemm(dpd, q[0], dk[0], L, hd, L, a_mn=True, b_mn=True, b_off=(0, L, 0, q[1], 0, hd), c_geom=out(*dk), **heads)
         # dV = Pd^T . dO
-        self._gemm(P, s["d_o"], s["dKV"], L, hd, L, a_mn=True, b_mn=True, batch=BH, inner=H,
-                   a_off=(0, H * Lp, Lp, 0, 0, 0), b_off=(0, L, 0, 0, 0, hd), c_geom=(2 * d, d, L * 2 * d, hd))
+        self._gemm(P, s["d_o"], dv[0], L, hd, L, a_mn=True, b_mn=True, b_off=(0, L, 0, 0, 0, hd), c_geom=out(*dv), **heads)
 
     def forward_train(self):
         """Loss of the staged batch (device fp32 [2] view: mean CE over the valid targets, 1/n_valid)."""
@@ -828,10 +844,10 @@ class SasRecEngine:
         from .ops import bce_head_fwd, ce_head_fwd
 
         self.lib.count += 2
-        if getattr(self, "bce", False):
+        if self.bce:
             return bce_head_fwd(self.ce, self.hc, self.params16["item_emb"][: cfg.n_items], self.labels_c, self.n_valid,
                                 d_hc=self.s["dhc"] if self.fused_ce else None, n_valid_hint=self.n_valid_hint)
-        row = getattr(self, "ce_row", None)
+        row = self.ce_row
         roww = None
         if row is not None and row["weighted"]:   # weights of the valid targets in the head's compacted order
             torch.index_select(self.in_roww, 0, self.valid_idx, out=self.roww_c)
@@ -852,7 +868,7 @@ class SasRecEngine:
         st = self._stream
         from .ops import bce_head_bwd, ce_head_bwd
 
-        if getattr(self, "bce", False):
+        if self.bce:
             bce_head_bwd(self.ce, self.hc, p16["item_emb"][: cfg.n_items], self.labels_c, self.n_valid, s["dhc"], G["item_emb"],
                          n_valid_hint=self.n_valid_hint)
             self.lib.count += 3
@@ -882,7 +898,7 @@ class SasRecEngine:
             g = lambda k: G[f"b{i}.{k}"]  # noqa: E731
             dz = dx
             if self.fused_post_attn_bwd:
-                # one pass: d_t, du, dh (operands of the grouped weight gradients), d_o (into the attention backward), dLN2
+                # one pass: d_t, du, dh (operands of the weight gradients), d_o (into the attention backward), dLN2
                 masked = legacy or drop > 0
                 check(self.lib.rp_post_attn_bwd(dz.data_ptr(), a["u"].data_ptr(), a["h"].data_ptr(), a["mean2"].data_ptr(),
                                                 a["rstd2"].data_ptr(), f("ln2_w").data_ptr(), w("w2").data_ptr(),
@@ -893,17 +909,10 @@ class SasRecEngine:
                                                 s["d_o"].data_ptr(), g("ln2_w").data_ptr(), g("ln2_b").data_ptr(), hdv, st()),
                       "rp_post_attn_bwd")
                 d_t = s["d_t"] if masked else dz
-                fw = self.fused_wgrad
-                wpairs = [(d_t, a["u"], g("w2"), g("b2")), (s["du"], a["y"], g("w1"), g("b1")), (s["dh"], a["O"], g("out_w"), g("out_b"))]
-                bias_grads = [(d_t, g("b2")), (s["du"], g("b1")), (s["dh"], g("out_b"))]
-                if not fw:
-                    self._wgrad(d_t, a["u"], g("w2"), d, d)
-                    self._wgrad(s["du"], a["y"], g("w1"), d, d)
-                    self._wgrad(s["dh"], a["O"], g("out_w"), d, d)
-            if not self.fused_post_attn_bwd and legacy:  # x_next = (...) * pad   (sasrec/model.py:441)
-                check(self.lib.rp_dropout_bwd(dz.data_ptr(), dz.data_ptr(), T, d, self.in_pad.data_ptr(), 0.0, 0, 0, None, st()),
-                      "rp_dropout_bwd")
-            if not self.fused_post_attn_bwd:
+            else:
+                if legacy:  # x_next = (...) * pad   (sasrec/model.py:441)
+                    check(self.lib.rp_dropout_bwd(dz.data_ptr(), dz.data_ptr(), T, d, self.in_pad.data_ptr(), 0.0, 0, 0, None,
+                                                  st()), "rp_dropout_bwd")
                 if drop > 0:
                     check(self.lib.rp_dropout_bwd(dz.data_ptr(), s["d_t"].data_ptr(), T, d, None, drop, self.seed,
                                                   self._site(i, 2) << 40, self.rng_counter.data_ptr(), st()), "rp_dropout_bwd")
@@ -911,25 +920,13 @@ class SasRecEngine:
                 else:
                     d_t = dz
                 # ---- FFN backward
-                fw = self.fused_wgrad
-                wpairs = [(d_t, a["u"], g("w2"), g("b2"))]  # (dY, X, dW, db): weight + bias gradients, one grouped launch per block
-                if not fw:
-                    self._wgrad(d_t, a["u"], g("w2"), d, d)
-                bias_grads = [(d_t, g("b2"))]  # column sums of this block, one launch at the end of its backward
                 self._gemm(d_t, w("w2"), s["du"], T, d, d, b_mn=True, gate=a["u"], gate_scale=ks)
-                wpairs.append((s["du"], a["y"], g("w1"), g("b1")))
-                if not fw:
-                    self._wgrad(s["du"], a["y"], g("w1"), d, d)
-                bias_grads.append((s["du"], g("b1")))
                 self._gemm(s["du"], w("w1"), s["dy"], T, d, d, b_mn=True, residual=dz)
                 self._ln_bwd(s["dy"], a["h"], f("ln2_w"), a["mean2"], a["rstd2"], s["dh"], g("ln2_w"), g("ln2_b"), T)
                 # ---- out projection
                 self._gemm(s["dh"], w("out_w"), s["d_o"], T, d, d, b_mn=True)
-                wpairs.append((s["dh"], a["O"], g("out_w"), g("out_b")))
-                if not fw:
-                    self._wgrad(s["dh"], a["O"], g("out_w"), d, d)
-                bias_grads.append((s["dh"], g("out_b")))
-            self._attention_backward(i)
+            self._attention_backward(i, (a["Q"], 0), (a["KV"], 0), (a["KV"], d), (s["dQ"], 0), (s["dKV"], 0), (s["dKV"], d),
+                                     causal=True, mask_pad_keys=not legacy)
             # ---- projections
             in_w = w("in_w")
             if self.fused_pre_attn:
@@ -941,17 +938,15 @@ class SasRecEngine:
                 self._gemm(s["dQ"], in_w[:d], s["dq_in"], T, d, d, b_mn=True, residual=s["dh"])
                 self._ln_bwd(s["dq_in"], x, f("ln1_w"), a["mean1"], a["rstd1"], s["tmp"], g("ln1_w"), g("ln1_b"), T)
                 self._gemm(s["dKV"], in_w[d:], other, T, d, 2 * d, b_mn=True, residual=s["tmp"])
-            wpairs.append((s["dQ"], a["q_in"], g("in_w")[:d], g("in_b")[:d]))
-            if not fw:
-                self._wgrad(s["dQ"], a["q_in"], g("in_w")[:d], d, d)
-            bias_grads.append((s["dQ"], g("in_b")[:d]))
-            wpairs.append((s["dKV"], x, g("in_w")[d:], g("in_b")[d:]))
-            if fw:
-                self._wgrad_group(wpairs)
+            # ---- the block's weight and bias gradients (dY, X, dW, db) in one dispatch: no operand is overwritten within the block
+            pairs = [(d_t, a["u"], g("w2"), g("b2")), (s["du"], a["y"], g("w1"), g("b1")), (s["dh"], a["O"], g("out_w"), g("out_b")),
+                     (s["dQ"], a["q_in"], g("in_w")[:d], g("in_b")[:d]), (s["dKV"], x, g("in_w")[d:], g("in_b")[d:])]
+            if self.fused_wgrad:
+                self._wgrad_group(pairs)
             else:
-                self._wgrad(s["dKV"], x, g("in_w")[d:], 2 * d, d)
-                bias_grads.append((s["dKV"], g("in_b")[d:]))
-                self._colsum_multi(bias_grads)
+                for dY, X, dW, _ in pairs:
+                    self._wgrad(dY, X, dW, *dW.shape)
+                self._colsum_multi([(dY, db) for dY, _, _, db in pairs])
             dx, other = other, dx
         pos0 = 0 if legacy else cfg.max_len - L
         check(self.lib.rp_embed_bwd(dx.data_ptr(), self.ids32.data_ptr(), self.in_pad.data_ptr(), self.B, L, d, cfg.pad_id,

@@ -7,7 +7,8 @@ import torch
 
 from ....compat import LightningModuleBase
 from ....core import SasRecCore, _EngineLoss, dist_grad_all_reduce
-from ....engine_bert import _BERT_BLOCK, Bert4RecEngine, BertConfig
+from ....engine import _BLOCK_PARAMS
+from ....engine_bert import Bert4RecEngine, BertConfig
 from ....schema import item_feature_of
 
 _BLEAF = {"ln1_w": "attention_norm.weight", "ln1_b": "attention_norm.bias", "in_w": "attention.in_proj_weight",
@@ -21,7 +22,7 @@ def bert_key_map(n_blocks: int, tying: bool, item_feature: str = "item_id") -> d
     m = {"item_emb": f"item_embedder.cat_embeddings.{item_feature}.weight", "mask_emb": "item_embedder.mask_embedding.weight",
          "pos_emb": "item_embedder.position.pe.weight"}
     for i in range(n_blocks):
-        for k in _BERT_BLOCK:
+        for k in _BLOCK_PARAMS:
             m[f"b{i}.{k}"] = f"transformer_blocks.{i}." + _BLEAF[k]
     if tying:
         m["head_b"] = "_head.out_bias"
@@ -54,14 +55,8 @@ def shift_features(ids, pad_mask, token_mask, pad_value: int = 0):
 
 
 class _BertCore(SasRecCore):
-    def __init__(self, cfg: BertConfig, item_feature="item_id", device=None, seed=0):
-        torch.nn.Module.__init__(self)
-        self.cfg, self.item_feature = cfg, item_feature
-        self._device = torch.device(device) if device is not None else torch.device("cuda")
-        self._seed, self.engine, self.flat, self._pending_state, self._shadow_dirty = seed, None, None, None, True
-        self.adam_betas = (0.9, 0.98)
-        self._keymap = bert_key_map(cfg.n_blocks, cfg.tying, item_feature)
-        self._materialise()
+    def _key_map(self):
+        return bert_key_map(self.cfg.n_blocks, self.cfg.tying, self.item_feature)
 
     def _initial_seq_len(self):
         return self.cfg.max_len
@@ -72,15 +67,8 @@ class _BertCore(SasRecCore):
     def _to_ref(self, k, v):
         return v   # export_named already gives the reference shapes (true d, 4d inner width, n_items bias entries)
 
-    def _import(self, state):
-        inv = {v: k for k, v in self._keymap.items()}
-        with torch.no_grad():
-            for rk, val in state.items():
-                k = inv.get(rk)
-                if k is None:
-                    continue
-                self.engine.import_named(k, val)
-        self._shadow_dirty = True
+    def _from_ref(self, k, v):
+        return v
 
     def state_dict(self, *a, destination=None, prefix="", keep_vars=False):
         src = self._export() if self.engine is not None else (self._pending_state or {})

@@ -270,7 +270,6 @@ def test_c_abi_argument_errors_without_a_gpu():
     assert L.rp_score_topk(None, None, None, None, 0, 1, 1, 128, 10, None, None, None, None, 0, None) != 0
     assert L.rp_ce_head_fwd(None, None, None, None, None, 1, 1, 128, None, None, None, None, 0, None, 0, None) == EINVAL
     assert L.rp_ce_head_bwd(None, None, None, None, None, 1, 1, 128, None, None, None, None, None, 0, 0, None, 0, None) == EINVAL
-    assert L.rp_ffn_fused(None, None, None, None, None, None, 1, 128, None, None) == EINVAL
     assert L.rp_post_attn_fused(None, None, None, None, None, None, 1e-8, None, None, None, None, None, 1, 128, None, 0, None) == EINVAL
     assert L.rp_post_attn_train(None, None, None, None, None, None, 1e-8, None, None, None, None, None, 1, 128, 0.0, 0, 0, 0, None,
                                 None, None, None, None, None, None, 0, None) == EINVAL
@@ -288,7 +287,6 @@ def test_c_abi_argument_errors_without_a_gpu():
     # shape errors with non-NULL dummies (no memory is touched before the shape check)
     buf = ctypes.create_string_buffer(64)
     p = ctypes.cast(buf, ctypes.c_void_p)
-    assert L.rp_ffn_fused(p, p, p, p, p, None, 10, 96, ctypes.cast(ctypes.create_string_buffer(8), ctypes.c_void_p), None) == ESHAPE
     assert L.rp_ce_head_fwd(p, p, None, p, p, 128, 100, 96, p, p, p, None, 0, p, 1 << 40, None) == ESHAPE
 
 

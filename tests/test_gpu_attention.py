@@ -603,9 +603,10 @@ def test_attn_softmax_bwd_matches_formula(cuda, hd, L, drop):
                                                 (256, 2, 256, "legacy", 0.0), (256, 2, 65, "legacy", P_DROP),
                                                 (128, 2, 300, "new", P_DROP), (128, 2, 512, "new", 0.0),
                                                 (128, 2, 512, "legacy", P_DROP)])
-def test_unfused_attention_backward_matches_autograd(cuda, d, H, L, variant, drop):
+def test_attention_drivers_unfused_backward_matches_autograd(cuda, d, H, L, variant, drop):
     """The engine's un-fused attention backward (dPd = dO.V^T, rp_attn_softmax_bwd over the saved probabilities, three
-    batched GEMMs) run through SasRecEngine._attention_forward / _attention_backward on planted Q, K, V and dO: O, dQ, dK,
+    batched GEMMs) run through the shared attention drivers SasRecEngine._attention_forward / _attention_backward, with
+    SASRec's Q and packed [K | V] as sources and dQ / packed [dK | dV] as destinations, on planted Q, K, V and dO: O, dQ, dK,
     dV against fp64 autograd per 64-row block, at head_dim 128 and at head_dim 64 with L > 256."""
     from replay_b200.engine import EncoderConfig, SasRecEngine
 
@@ -619,10 +620,11 @@ def test_unfused_attention_backward_matches_autograd(cuda, d, H, L, variant, dro
     a["Q"].copy_(c.qd)
     a["KV"].copy_(c.kvd)
     eng.rng_counter.fill_(CTR)
-    eng._attention_forward(0, True)
+    qkv = (a["Q"], 0), (a["KV"], 0), (a["KV"], d)
+    eng._attention_forward(0, True, *qkv, causal=True, mask_pad_keys=bool(mpk))
     d_o = _d_out(c, seed=L)
     eng.s["d_o"].copy_(d_o.to(cuda))
-    eng._attention_backward(0)
+    eng._attention_backward(0, *qkv, (eng.s["dQ"], 0), (eng.s["dKV"], 0), (eng.s["dKV"], d), causal=True, mask_pad_keys=bool(mpk))
     torch.cuda.synchronize()
     B, hd, T = c.B, c.hd, c.T
     keep = drop_keep(eng.seed + CTR, eng._site(0, 0) << 40, drop, B, H, L, c.Lp) if drop > 0 else None

@@ -120,15 +120,15 @@ class _GeluTanhGrad(torch.autograd.Function):
 # ----------------------------------------------------------------------------------------------------------------------
 # float64 reference of the BERT4Rec training loss with every dropout site
 # ----------------------------------------------------------------------------------------------------------------------
-def _bsite(blk, k):
-    """Bert4RecEngine._bsite: dropout site k of block blk (offset = site << 40; the embedding is site 0)."""
+def _site(blk, k):
+    """SasRecEngine._site (both engines): dropout site k of block blk (offset = site << 40; the embedding is site 0)."""
     return 1 + blk * 8 + k
 
 
 def engine_keeps(seed_eff, p, B, L, d, H, n_blocks, site_shift=0, dev=None):
     """Keep masks (0 or 1/(1-p), float64) of every dropout site of Bert4RecEngine's training body: the embedding at
     offset 0; per block k = 0 attention probabilities (row key bz*Lp + i), 1 out-projection, 2 GELU output, 3 FFN output,
-    4 block output, at offset _bsite(i, k) << 40.  ``site_shift`` moves every block site number (a plausible mistake)."""
+    4 block output, at offset _site(i, k) << 40.  ``site_shift`` moves every block site number (a plausible mistake)."""
     T, Lp, ks = B * L, _ru(L, 64), _ks(p)
     rows = np.arange(T)
 
@@ -137,7 +137,7 @@ def engine_keeps(seed_eff, p, B, L, d, H, n_blocks, site_shift=0, dev=None):
 
     out = {"emb": tok(0, d), "blocks": []}
     for i in range(n_blocks):
-        s = lambda k: (_bsite(i, k) + site_shift) << 40  # noqa: E731
+        s = lambda k: (_site(i, k) + site_shift) << 40  # noqa: E731
         out["blocks"].append({"attn": drop_keep(seed_eff, s(0), p, B, H, L, Lp).to(dev), "out": tok(s(1), d),
                               "gelu": tok(s(2), 4 * d), "ffn": tok(s(3), d), "blk": tok(s(4), d)})
     return out
@@ -438,7 +438,7 @@ def test_gemm_tolerance_discriminates_gelu_mistakes(mistake):
     """At the FFN-in GEMM test's inputs (M = 600) and element-wise tolerance, the tanh GELU in the forward or in gelu',
     and dropout applied before the GELU, move the output by >= 10x TOL_ULP."""
     M = 600
-    keep = keep_draws(SEED + CTR, _bsite(0, 2) << 40, P_DROP, np.arange(M), 1024).double()
+    keep = keep_draws(SEED + CTR, _site(0, 2) << 40, P_DROP, np.arange(M), 1024).double()
     ks = _ks(P_DROP)
     if mistake == "gelu_tanh_bwd":
         _, _, pre, acc, S = _ffn_in_bwd_case(M, 5)
@@ -559,7 +559,7 @@ def test_gemm_ffn_in_forward_gelu_dropout_c2(cuda, M):
     rows end in a ragged tile, 51 200 is config 3's token count): the zero pattern is the ported keep mask bit for bit,
     the values are one rounding from fp64, C2 is the rounded pre-activation everywhere, nothing is written outside."""
     N, K = 1024, 256
-    off = _bsite(1, 2) << 40
+    off = _site(1, 2) << 40
     A, W, bias, pre, S = _ffn_in_case(M, 3 if M == 600 else 4, dev=cuda)
     ctr = torch.tensor([CTR], dtype=torch.int64, device=cuda)
     C, C2 = _sent_buf(M, N, cuda), _sent_buf(M, N, cuda)
@@ -582,7 +582,7 @@ def test_gemm_ffn_in_backward_gelu_grad_dropout(cuda, M):
     """du = (d_t W2) * keep/(1-p) * gelu'(pre) (b_mn, gate_mode 1), and SASRec's un-fused ReLU backward
     du = (d_t W2) * (gate != 0 ? 1/(1-p) : 0) (gate_mode 0, gate = the dropped ReLU output)."""
     d = 256
-    off = _bsite(0, 2) << 40
+    off = _site(0, 2) << 40
     dT, W2, pre, acc, S = _ffn_in_bwd_case(M, 5 if M == 600 else 6, dev=cuda)
     ctr = torch.tensor([CTR], dtype=torch.int64, device=cuda)
     ks = _ks(P_DROP)
@@ -629,7 +629,7 @@ def test_gemm_block_output_two_dropout_sites(cuda, M):
     with a zero residual it is site 3's AND site 4's, so both sites draw their own masks and both add the counter;
     values against fp64; a row mask applied after everything zeroes its rows exactly and leaves the others bit-identical."""
     d, K = 256, 1024
-    off3, off4 = _bsite(1, 3) << 40, _bsite(1, 4) << 40
+    off3, off4 = _site(1, 3) << 40, _site(1, 4) << 40
     U, W2, b2, y, t, S = _block_out_case(M, 7 if M == 600 else 8, cuda)
     ctr = torch.tensor([CTR], dtype=torch.int64, device=cuda)
     ks = _ks(P_DROP)
@@ -985,7 +985,7 @@ def test_gather_rows(cuda, d, scatter, n_dev):
 def test_dropout_bwd_with_row_mask(cuda, cols):
     """rp_dropout_bwd: out = in * keep / (1-p) (fp32 product rounded to bf16: exact), rows with mask 0 exactly zero;
     the in-place row-mask-only form the legacy backward uses."""
-    rows, off = 1400, _bsite(1, 4) << 40
+    rows, off = 1400, _site(1, 4) << 40
     g = _gen(cols)
     x = _bf(torch.randn(rows, cols, generator=g)).to(cuda)
     rm = (torch.rand(rows, generator=g) > 0.3).to(torch.uint8).to(cuda)

@@ -1,5 +1,5 @@
 """SASRec's fused block kernels (csrc/rp_block_fused.cu: rp_ln_qkv_fused, rp_post_attn_train, rp_post_attn_fused,
-rp_ffn_fused, rp_post_attn_bwd, rp_pre_attn_bwd; csrc/rp_wgrad.cu: rp_wgrad_group) and SasRecEngine's training step, each
+rp_post_attn_bwd, rp_pre_attn_bwd; csrc/rp_wgrad.cu: rp_wgrad_group) and SasRecEngine's training step, each
 against a float64 reference computed from the same bf16 inputs, at the config-2 shape (L = 200, d = 128, H = 2, two blocks,
 dropout 0.2, T = 102 400 tokens) and at the edges where these kernels change behaviour.
 
@@ -696,7 +696,7 @@ def test_post_attn_train_and_bwd(cuda, T, d, hdv, drop, masked):
 
 
 # ======================================================================================================================
-# GPU 3: the eval kernels rp_post_attn_fused and rp_ffn_fused
+# GPU 3: the eval kernel rp_post_attn_fused
 # ======================================================================================================================
 _EVAL_CASES = [(1, 128, 0, True), (129, 64, 0, False), (1400, 128, 0, True), (1400, 64, 50, True), (1400, 128, 32, False),
                (1400, 128, 48, True), (102400, 128, 0, False), (102363, 64, 0, True), (102363, 128, 48, False)]
@@ -713,11 +713,10 @@ def _eval_atol(y, u, W1, W2, S2):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("T,d,hdv,masked", _EVAL_CASES)
-def test_post_attn_fused_and_ffn_fused(cuda, T, d, hdv, masked):
+def test_post_attn_fused(cuda, T, d, hdv, masked):
     """rp_post_attn_fused (predict: h = O Wo^T + bo + q_in in fp32, y = LN2(h) over the real features, out = (y +
-    relu(y W1^T + b1) W2^T + b2) * rowmask) and rp_ffn_fused (out = (y + relu(y W1^T + b1) W2^T + b2) * rowmask from a
-    bf16 y) element-wise against fp64 with the internal bf16 roundings of y and u allowed one flip; rows with row mask 0
-    exactly 0; nothing written past T."""
+    relu(y W1^T + b1) W2^T + b2) * rowmask) element-wise against fp64 with the internal bf16 roundings of y and u allowed
+    one flip; rows with row mask 0 exactly 0; nothing written past T."""
     O, q_in, Wo, bo, lw, lb, W1, b1, W2, b2, v = _post_attn_inputs(T, d, hdv, T + d + hdv + 17, cuda)
     rm = _rowmask(T, masked, T + 2, cuda)
     on = (rm if rm is not None else torch.ones(T, dtype=torch.uint8, device=cuda)).bool()
@@ -739,17 +738,6 @@ def test_post_attn_fused_and_ffn_fused(cuda, T, d, hdv, masked):
     assert (out[:T][~on] == 0).all(), "rows with row mask 0 must be exactly 0"
     assert (out[:T][:, ~v] == 0).all(), "padded features must be 0"
     assert _note("post_attn_fused out ulp", ulp_err(out[:T], ref, _eval_atol(y, u, W1, W2, S2))) < TOL_ULP_EVAL
-    # rp_ffn_fused on the same y rows (bf16 input)
-    yin = _bf(y).contiguous()
-    out2 = _sent(T, d, cuda)
-    check(lib().rp_ffn_fused(yin.data_ptr(), W1.data_ptr(), b1.data_ptr(), W2.data_ptr(), b2.data_ptr(), ptr(rm), T, d,
-                             out2.data_ptr(), _stream()), "rp_ffn_fused")
-    torch.cuda.synchronize()
-    _untouched(out2, T, "ffn out")
-    assert (out2[:T][~on] == 0).all(), "rows with row mask 0 must be exactly 0"
-    atol = HALF_ULP_SLACK * S2 + torch.exp2(torch.floor(torch.log2(u.abs().clamp_min(1e-300))) - 7).amax(-1, keepdim=True) \
-        * Dd(W2).abs().amax(-1)[None, :] + 1e-30
-    assert _note("ffn_fused out ulp", ulp_err(out2[:T], ref, atol)) < TOL_ULP_EVAL
 
 
 # ======================================================================================================================
