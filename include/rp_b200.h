@@ -379,9 +379,12 @@ int rp_counter_add(unsigned long long* counter, unsigned long long inc, void* st
  * batch (tensor-core path), 1 = [B*seq_len, n_neg] per position, 2 = [B, n_neg] per sequence (1, 2: rows addressed through
  * valid_idx[t] = flat b*seq_len + l of compacted row t; gather-dot kernels).  kind: RP_LOSS_CE_SAMPLED (negatives equal to the
  * positive or to ignore_index get logit -1e9), RP_LOSS_BCE_SAMPLED (same masking, log_eps / clamp as the reference),
- * RP_LOSS_LEGACY_CE_SAMPLED (log(vocab_size-1) - 1e6*reject - log(n_neg - #reject) correction), RP_LOSS_LEGACY_BCE_SAMPLED (no
- * masking).  One positive per position.  fwd: loss_out[0] = mean loss, loss_out[1] = 1/T_v, d(loss)/d(logits) stays in the
- * workspace; bwd: d_hc bf16 [capacity, d] rows < *n_valid, d_table fp32 ACCUMULATED (zero it first; dense rows untouched).
+ * RP_LOSS_LEGACY_CE_SAMPLED (log(vocab_size-1) - 1e6*reject - log(min(n_neg, vocab_size) - #reject) correction),
+ * RP_LOSS_LEGACY_BCE_SAMPLED (no masking).  One positive per position.  fwd: loss_out[0] = mean loss, loss_out[1] = 1/T_v,
+ * d(loss)/d(logits) stays in the workspace (which need not be zeroed); bwd: d_hc bf16 [capacity, d] rows < *n_valid, d_table
+ * fp32 ACCUMULATED (+=: zero it first; rows that no positive and no unmasked negative points at are left as they were).
+ * d_hc rows >= *n_valid: untouched with per-row negatives; with shared negatives rows [*n_valid, min(round_up(*n_valid, 128),
+ * capacity)) are written with 0 and the rest are untouched.  *n_valid == 0: loss_out = {0, 0}, d_table unchanged.
  * ------------------------------------------------------------------------------------------------------------- */
 #define RP_LOSS_CE_SAMPLED 0
 #define RP_LOSS_BCE_SAMPLED 1

@@ -102,9 +102,13 @@ __global__ void sampled_logits_kernel(const SampledArgs a) {
 // one warp per token: masks, loss, d(loss)/d(logits) in place; deterministic mean (block partials, last block adds)
 __global__ void sampled_loss_kernel(const SampledArgs a) {
   const int n_valid = *a.n_valid;
-  const float inv_n = n_valid > 0 ? 1.f / (float)n_valid : 0.f;
+  const float inv_n = n_valid > 0 ? __frcp_rn((float)n_valid) : 0.f;   // loss_out[1] = 1/T_v rounded once (fast-math safe)
   const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
-  const int t_end = a.neg_mode == 0 ? min(((n_valid + 127) / 128) * 128, a.capacity) : n_valid;  // GEMM tail rows -> 0
+  // shared negatives: the GEMMs read dz16 in whole 128-row M tiles (dH) and 64-row K chunks (dE_neg), past the capacity when
+  // it is not a multiple of 64 - zero every row they can reach (dz16 has round_up(capacity, 128) rows), so that a stale
+  // workspace cannot reach dE_neg as 0 x NaN
+  const int t_end = a.neg_mode == 0 ? ((n_valid + 127) / 128) * 128 : n_valid;
+  const int n_neg_drawn = min(a.N, a.vocab_size);   // legacy CE: the reference corrects by min(N, vocab_size) - #reject
   const bool ce = a.kind == kCESampled || a.kind == kLegacyCE;
   const bool masked = a.kind == kCESampled || a.kind == kBCESampled;
   float local = 0.f;
@@ -131,7 +135,7 @@ __global__ void sampled_loss_kernel(const SampledArgs a) {
       const int64_t nj = nr[j];
       float z = zr[j];
       if (masked && (nj == (int64_t)y || (a.ignore_index >= 0 && nj == (int64_t)a.ignore_index))) z = -1e9f;
-      if (a.kind == kLegacyCE) z = z + logf((float)(a.vocab_size - 1)) - (nj == (int64_t)y ? 1e6f : 0.f) - logf((float)(a.N - n_reject));
+      if (a.kind == kLegacyCE) z = z + logf((float)(a.vocab_size - 1)) - (nj == (int64_t)y ? 1e6f : 0.f) - logf((float)(n_neg_drawn - n_reject));
       zr[j] = z;
       mx = fmaxf(mx, z);
     }
