@@ -409,13 +409,18 @@ int rp_sampled_head_bwd(const rp_sampled_desc* s, void* d_hc, float* d_table, vo
  * hc bf16 [capacity, d]: final hidden state of EVERY position (row b * seq_len + l, pad rows included); table bf16
  * [n_items, d]; labels int64 [capacity]; pad_mask [capacity] (1 = real input position); n_rows int32 [1] in device memory =
  * B * seq_len of the batch (<= capacity).  d in {64,128,256,512} is the padded width, d_true the model's hidden size,
- * hd_valid the feature-slot layout (0 = unpadded).  1 <= bucket_size_x <= min(1024, capacity), 1 <= bucket_size_y <=
- * min(1024, n_items) (the fused top-K), else RP_ESHAPE.
+ * hd_valid the feature-slot layout (0 = unpadded; else <= 128 with d a multiple of its slot, and d_true must equal the
+ * real features of that layout: d / slot * hd_valid, or d when unpadded).  1 <= bucket_size_x <= min(1024, capacity),
+ * 1 <= bucket_size_y <= min(1024, n_items) (the fused top-K), else RP_ESHAPE.  The S = X_b . Y_b^T scores and dX run in
+ * chunks of buckets whose fp32 share of the workspace stays within RP_SCE_CHUNK_BYTES (environment, read at every call,
+ * default 256 MiB; at least one bucket per chunk).
  * Caller-owned outputs: draw fp32 = the standard normals, [n_buckets, d_true] (or [capacity, n_buckets] with mix_x; rows
  * < *n_rows used), drawn from Philox keyed by seed + *rng_counter unless draw_given (then read as given); top_x int64 and
  * score_x fp32 [n_buckets, bucket_size_x] (slots with score -inf hold no row); top_y int64 [n_buckets, bucket_size_y].
- * A row carries loss when it is a real position with a label in [0, n_items).  fwd: loss_out fp32 [2] = { mean over the
- * rows with a non-zero per-row max of the bucket CEs (NaN when there is none), 1 / that count (0 when none) }.
+ * A row carries loss when it is a real position < *n_rows with a label in [0, n_items); every other row (pad, t >=
+ * *n_rows, label outside the catalog) is also left out of the row selection: it scores -inf in top_x.
+ * fwd: loss_out fp32 [2] = { mean over the rows with a non-zero per-row max of the bucket CEs (NaN when there is none),
+ * 1 / that count rounded once (0 when none) }.
  * stages: RP_SCE_DRAW | RP_SCE_SELECT_X | RP_SCE_SELECT_Y | RP_SCE_BUCKET_CE run in this order (RP_SCE_ALL = one forward;
  * the parts exist for timing).  bwd: d_hc bf16 [capacity, d] OVERWRITTEN for every row (zero where no gradient); no table
  * gradient (the reference scores a detached copy of the table).  Deterministic and CUDA-graph capturable. */

@@ -17,6 +17,7 @@
 // G = softmax * weight in bf16 in place of S, dX_b = G . Y_b (batched rp_gemm), then every row gathers its winners' dX rows
 // plus (p_c - 1) * weight * table[y_t] in bucket order: no float atomics, bitwise reproducible.
 #include <algorithm>
+#include <cstdlib>
 
 #include "rp_host.h"
 #include "rp_gemm_desc.h"
@@ -38,7 +39,7 @@ extern "C" int rp_score_topk(const void* hq, const void* table, const float* bia
 namespace rp {
 
 constexpr unsigned long long kSceSite = 0x5CEull << 40;   // Philox counter offset of the bucket draw
-constexpr size_t kSceChunkBytes = 256ull << 20;            // fp32 S + dX of one chunk of buckets
+constexpr size_t kSceChunkBytes = 256ull << 20;            // fp32 S + dX of one chunk of buckets (RP_SCE_CHUNK_BYTES overrides)
 
 struct SceArgs {
   const __nv_bfloat16* hc;
@@ -292,7 +293,7 @@ __global__ void sce_loss_kernel(const SceArgs a) {
       s3 += reinterpret_cast<volatile float*>(a.block_sums)[i];
       n3 += reinterpret_cast<volatile int*>(a.block_sums)[512 + i];
     }
-    const float inv = n3 > 0 ? 1.f / (float)n3 : 0.f;
+    const float inv = n3 > 0 ? __frcp_rn((float)n3) : 0.f;   // 1 / count rounded once (fast-math 1.f / x is approximate)
     a.loss_out[0] = n3 > 0 ? s3 * inv : __int_as_float(0x7fc00000);   // mean of nothing: NaN, as torch.mean
     a.loss_out[1] = inv;
     a.inv_n[0] = inv;
@@ -422,7 +423,9 @@ static size_t sce_layout(const rp_sce_desc* s, SceArgs* a) {
   const size_t bsx = (size_t)s->bucket_size_x, bsy = (size_t)s->bucket_size_y;
   const size_t bsxp = ru(bsx, 64), bsyp = ru(bsy, 64), nbp = ru(nb, 64);
   const size_t per_bucket = bsxp * bsyp * 4 + bsxp * d * 4;
-  size_t chunk = kSceChunkBytes / per_bucket;
+  const char* env = getenv("RP_SCE_CHUNK_BYTES");   // read per call: the workspace query and the launches must agree
+  const size_t budget = env ? (size_t)atoll(env) : kSceChunkBytes;
+  size_t chunk = budget / per_bucket;
   chunk = chunk < 1 ? 1 : (chunk > nb ? nb : chunk);
   const size_t topk_ws = std::max(rp_score_topk_workspace((int)nb, (int)cap, (int)d, (int)bsx),
                                   rp_score_topk_workspace((int)nb, s->n_items, (int)d, (int)bsy));
@@ -473,7 +476,8 @@ static size_t sce_layout(const rp_sce_desc* s, SceArgs* a) {
 static bool sce_shape_ok(const rp_sce_desc* s) {
   if (s->capacity <= 0 || s->n_items <= 0 || s->n_buckets <= 0) return false;
   if (s->d != 64 && s->d != 128 && s->d != 256 && s->d != 512) return false;
-  if (s->d_true <= 0 || s->d_true > s->d || s->hd_valid < 0) return false;
+  if (s->hd_valid < 0 || s->hd_valid > 128 || (s->hd_valid > 0 && s->d % (s->hd_valid <= 64 ? 64 : 128))) return false;
+  if (s->d_true != feat_count(s->d, s->hd_valid)) return false;   // pad_col scatters exactly d_true columns into the slots
   if (s->bucket_size_x < 1 || s->bucket_size_x > 1024 || s->bucket_size_x > s->capacity) return false;
   if (s->bucket_size_y < 1 || s->bucket_size_y > 1024 || s->bucket_size_y > s->n_items) return false;
   return true;
