@@ -44,7 +44,9 @@ const char* rp_version(void);
 /* seen_ids int64 [n_users, S] (any order, duplicates allowed, ids outside [0,item_count) are padding)
  *   -> out_sorted int32 [n_users, S], ascending, padding = INT32_MAX.
  * inv_map (optional, int32 [item_count]): position of each item in candidates_to_score, -1 if absent; when given the
- * output holds candidate positions instead of item ids (seen_items.py:68-71,80-81). */
+ * output holds candidate positions instead of item ids (seen_items.py:68-71,80-81).
+ * 1 <= S <= 4096 (one block sorts a user's list in shared memory), else RP_ESHAPE.  rp_score_topk takes any S: the
+ * Python wrapper (ops.seen_prepare) prepares longer lists with a device-side sort to the same contract. */
 int rp_seen_prepare(const int64_t* seen_ids, int n_users, int S, int item_count, const int32_t* inv_map,
                     int32_t* out_sorted, void* stream);
 

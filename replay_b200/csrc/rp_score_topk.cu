@@ -13,6 +13,8 @@
 //               into the user's sorted seen list, running top-K (sorted, registers), partial top-K per (user, split, part)
 // Kernel 2 (topk_merge_kernel): one warp per user merges the per-split partial lists (score desc, column asc).
 // This register path serves K <= 32; 32 < K <= 1024 runs score_topk_wide_kernel + topk_wide_merge_kernel (see "wide K").
+#include <cfloat>
+
 #include "rp_host.h"
 #include "rp_sm90.cuh"
 
@@ -193,6 +195,10 @@ score_topk_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   for (int t = t_begin, j = 0; t < t_end; ++t, ++j) {
     if ((j & 3) == 0) {  // refresh every 4th tile: the shared threshold moves slowly once the lists are full
       gthr = gk != 0u ? key2f(gk - 1u) : -INFINITY;  // largest value strictly below the shared K-th best
+      // ... except around zero: below a published +0 lies -0, and below -0 or a denormal lies a denormal, which
+      // --use_fast_math compares as 0, so "0 > gthr" would reject the zeros that win an exact-zero tie at the K-th place on
+      // their smaller column.  -FLT_MIN (normal, never flushed) admits them; a lower threshold only admits more, never wrong.
+      if (fabsf(gthr) < FLT_MIN) gthr = -FLT_MIN;
       if (live) gk = *reinterpret_cast<volatile uint32_t*>(row_thr + u);  // lands long before its use 4 tiles later
     }
     float acc[kTileN / 2];

@@ -30,13 +30,28 @@ def selftest_mma(mode: int, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     return d
 
 
+# the longest seen list rp_seen_prepare sorts in one block's shared memory
+SEEN_PREPARE_MAX_S = 4096
+
+
 def seen_prepare(seen_ids: torch.Tensor, item_count: int, inv_map: torch.Tensor | None = None) -> torch.Tensor:
-    """int64 [B,S] seen ids -> int32 [B,S] sorted ascending, padding = INT32_MAX (include/rp_b200.h rp_seen_prepare)."""
+    """int64 [B,S] seen ids -> int32 [B,S] sorted ascending, padding = INT32_MAX (include/rp_b200.h rp_seen_prepare).
+
+    Lists longer than SEEN_PREPARE_MAX_S (a batch padded to one heavy user's whole history) are prepared to the same
+    contract by a device-side torch sort instead; rp_score_topk itself takes any S.  Both paths are CUDA-graph capturable."""
     _need(seen_ids, torch.int64, "seen_ids")
     B, S = seen_ids.shape
-    out = torch.empty(B, S, device=seen_ids.device, dtype=torch.int32)
     if inv_map is not None:
         _need(inv_map, torch.int32, "inv_map")
+    if S > SEEN_PREPARE_MAX_S:
+        ok = (seen_ids >= 0) & (seen_ids < item_count)
+        col = torch.where(ok, seen_ids, 0)
+        if inv_map is not None:
+            col = inv_map[col]
+            ok &= col >= 0
+        out = torch.where(ok, col, torch.iinfo(torch.int32).max).to(torch.int32)
+        return torch.sort(out, dim=1).values
+    out = torch.empty(B, S, device=seen_ids.device, dtype=torch.int32)
     check(lib().rp_seen_prepare(_ptr(seen_ids), B, S, item_count, _ptr(inv_map), _ptr(out), _stream()), "rp_seen_prepare")
     return out
 

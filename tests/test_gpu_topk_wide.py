@@ -4,6 +4,8 @@ predict shape, and through the modules and callbacks that pick it up via ops.MAX
 import pytest
 import torch
 
+import topk_reference as tr
+
 pytestmark = pytest.mark.gpu
 
 
@@ -16,65 +18,8 @@ def ops():
     return _ops
 
 
-def _oracle(hq, table, seen, K, bias=None, candidates=None):
-    """oracle.sasrec.score_topk in fp64; a bias enters as one more feature column (hq . 1 + bias)."""
-    from oracle import sasrec as osr
-
-    hq, table = hq.double(), table.double()
-    if bias is not None:
-        hq = torch.cat([hq, torch.ones(hq.shape[0], 1, dtype=torch.float64)], 1)
-        table = torch.cat([table, bias[:table.shape[0], None].double()], 1)
-    return osr.score_topk(hq, table, seen, K, candidates=candidates, acc_dtype=torch.float64), hq, table
-
-
-def _check(ids, sc, ref, hq64, tb64, columns=True):
-    """_topk_case's adjudication: scores within fp32 noise; an index swap only between scores closer than fp32 accumulation
-    noise and never inside an exact tie.  ids are item ids, i.e. rows of tb64 (the full, bias-augmented table)."""
-    (ids_ref, sc_ref) = ref
-    ids, sc = ids.cpu(), sc.cpu()
-    torch.testing.assert_close(sc.double(), sc_ref, rtol=1e-4, atol=1e-4)
-    assert ((sc[:, :-1] > sc[:, 1:]) | (sc[:, :-1] == sc[:, 1:])).all()
-    mism = ids != ids_ref
-    if mism.any():
-        full = hq64 @ tb64.T
-        gap = (torch.gather(full, 1, ids.clamp_min(0)) - torch.gather(full, 1, ids_ref.clamp_min(0))).abs()
-        assert (gap[mism] < 1e-5).all(), f"{int(mism.sum())} index mismatches"
-        assert mism.float().mean() < 1e-3
-        # two rows can tie exactly in fp64 yet round to different fp32 sums; the kernel orders by its own scores, and
-        # bit-equal kernel scores by ascending column (bit-equal table rows are checked exactly in the tie test)
-        if columns:
-            same = sc[:, :-1] == sc[:, 1:]
-            assert (ids[:, :-1][same] < ids[:, 1:][same]).all()
-
-
 def _case(ops, B, I, d, K, S, seed, bias=False, cands=False):
-    g = torch.Generator().manual_seed(seed)
-    hq = (torch.randn(B, d, generator=g) * 0.5).to(torch.bfloat16)
-    table = (torch.randn(I, d, generator=g) * 0.5).to(torch.bfloat16)
-    b = torch.randn(I, generator=g) * 2.0 if bias else None
-    seen = None
-    if S:
-        seen = torch.randint(-3, I + 5, (B, S), generator=g)  # ids outside [0, I) are padding
-        seen[0, :] = I                                       # a user with nothing seen
-        if B > 1:
-            seen[1, : S // 2] = seen[1, 0]                   # duplicates
-    c = torch.randperm(I, generator=g)[: max(K, I * 3 // 4)] if cands else None
-    ref, hq64, tb64 = _oracle(hq, table, seen, K, b, c)
-    # the kernel scores the gathered rows; its bias is per scored column, padded to a multiple of 128
-    tb_k = table if c is None else table[c]
-    b_k = None
-    if b is not None:
-        b_k = torch.zeros((tb_k.shape[0] + 127) // 128 * 128)
-        b_k[:tb_k.shape[0]] = b if c is None else b[c]
-    inv = None
-    if c is not None:
-        inv = torch.full((I,), -1, dtype=torch.int32)
-        inv[c] = torch.arange(c.numel(), dtype=torch.int32)
-    seen_sorted = ops.seen_prepare(seen.cuda(), I, None if inv is None else inv.cuda()) if seen is not None else None
-    ids, sc = ops.score_topk(hq.cuda(), tb_k.contiguous().cuda(), K, seen_sorted, None if c is None else c.cuda(),
-                             bias=None if b_k is None else b_k.cuda())
-    _check(ids, sc, ref, hq64, tb64, columns=c is None)
-    return ids, sc
+    return tr.run_case(ops, B, I, d, K, S, seed, bias=bias, cands=cands)
 
 
 @pytest.mark.parametrize("B,I,d,K,S,bias,cands", [
@@ -97,14 +42,7 @@ def test_wide_topk_matches_oracle(ops, B, I, d, K, S, bias, cands):
 
 
 def _wide_splits(B, I, K):
-    """item-split boundaries of the wide kernel (rp_score_topk.cu wide_splits)"""
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
-    C = 128
-    while C < 2 * K or C < K + 64:
-        C *= 2
-    n_tiles, ut = (I + 127) // 128, (B + 127) // 128
-    p = min(max(1, sms // ut), n_tiles, 64, 65536 // C)
-    return [(n_tiles * s // p) * 128 for s in range(1, p)]
+    return tr.wide_cuts(B, I, K, tr.sm_count())
 
 
 @pytest.mark.parametrize("K", [100, 1000])
@@ -131,13 +69,13 @@ def test_wide_topk_ties_at_every_boundary(ops, K):
     seen[5, :4] = torch.tensor([ga[0], ga[-1], gb[0], gb[3]])  # user 5: tie rows seen
     ids, sc = ops.score_topk(hq.cuda(), table.cuda(), K, ops.seen_prepare(seen.cuda(), I))
     ids, sc = ids.cpu(), sc.cpu()
-    (ids_ref, sc_ref), hq64, tb64 = _oracle(hq, table, seen, K)
+    (ids_ref, sc_ref), hq64, tb64 = tr.oracle(hq, table, seen, K)
     for user in (0, 1, 5, 127, 128, 129):
         assert torch.equal(ids[user], ids_ref[user]), user
     want0 = ga + gb[: K - n_a]
     assert ids[0].tolist() == want0
     assert (sc[0, :n_a] == sc[0, 0]).all() and (sc[0, n_a:] == sc[0, n_a]).all() and sc[0, 0] > sc[0, n_a]
-    _check(ids, sc, (ids_ref, sc_ref), hq64, tb64)
+    tr.check(ids, sc, (ids_ref, sc_ref), hq64, tb64)
 
 
 @pytest.mark.parametrize("K,d", [(100, 128), (1000, 512)])
@@ -151,21 +89,11 @@ def test_wide_topk_fewer_than_k_unseen(ops, K, d):
     seen = torch.cat([seen, seen[:, :5], torch.full((B, 3), I + 7)], 1)  # duplicates and padding
     ids, sc = ops.score_topk(hq.cuda(), table.cuda(), K, ops.seen_prepare(seen.cuda(), I))
     ids, sc = ids.cpu(), sc.cpu()
-    (ids_ref, sc_ref), _, _ = _oracle(hq, table, seen, K)
+    (ids_ref, sc_ref), _, _ = tr.oracle(hq, table, seen, K)
     assert torch.equal(ids, ids_ref)
     assert torch.isinf(sc[:, K - 15:]).all() and torch.isfinite(sc[:, : K - 15]).all()
     for b in range(B):
         assert ids[b, K - 15:].tolist() == sorted(set(seen[b].tolist()) - {I + 7})[:15]
-
-
-def _ordered_table(I, d, descending):
-    """hq = (1, 2^-8, 2^-16, 0, ...) and rows = base-256 digits of the column: every score is exact in bf16 x fp32 and
-    strictly increasing (or decreasing) with the column."""
-    j = torch.arange(I)
-    v = (I - j) if descending else (j + 1)
-    table = torch.zeros(I, d)
-    table[:, 0], table[:, 1], table[:, 2] = (v // 65536).float(), ((v // 256) % 256).float(), (v % 256).float()
-    return table.to(torch.bfloat16)
 
 
 @pytest.mark.parametrize("descending", [False, True])
@@ -176,13 +104,13 @@ def test_wide_topk_adversarial_item_orders(ops, K, descending):
     hq = torch.zeros(B, d)
     hq[:, 0], hq[:, 1], hq[:, 2] = 1.0, 2.0 ** -8, 2.0 ** -16
     hq = hq.to(torch.bfloat16)
-    table = _ordered_table(I, d, descending)
+    table = tr.ordered_table(I, d, descending)
     g = torch.Generator().manual_seed(1)
     seen = torch.randint(0, I + 10, (B, 200), generator=g)
     hi = torch.arange(I - 2 * K, I) if not descending else torch.arange(0, 2 * K)
     seen[:, :50] = hi[torch.randint(0, hi.numel(), (B, 50), generator=g)]  # seen items among the winners
     ids, sc = ops.score_topk(hq.cuda(), table.cuda(), K, ops.seen_prepare(seen.cuda(), I))
-    (ids_ref, sc_ref), _, _ = _oracle(hq, table, seen, K)
+    (ids_ref, sc_ref), _, _ = tr.oracle(hq, table, seen, K)
     assert torch.equal(ids.cpu(), ids_ref)
     assert torch.equal(sc.cpu().double(), sc_ref)
 
