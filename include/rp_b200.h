@@ -177,8 +177,9 @@ int rp_gemm(const rp_gemm_desc* g, void* stream);
 /* dst[i] (+)= sum_s src[s * stride + i], i < n (n, stride multiples of 4) */
 int rp_reduce_splits(const float* src, int n_splits, long long stride, long long n, float* dst, int accumulate, void* stream);
 
-/* Fused multi-head attention forward for L <= 256, head_dim in {64,128}: S = Q.K^T, causal / key-padding mask derived
- * from pad_mask (no [B*H,L,L] mask tensor), softmax, dropout, O = P.V.
+/* Fused multi-head attention forward for L <= 512, head_dim in {64,128}: S = Q.K^T, causal / key-padding mask derived
+ * from pad_mask (no [B*H,L,L] mask tensor), softmax, dropout, O = P.V.  Q, K and V of a 128-query tile stay in shared
+ * memory, except at head_dim 128 with L > 256, where V streams through a ring of 64-key stages (same outputs and saves).
  *   replaces  torch.nn.MultiheadAttention's SDPA core + replay/nn/mask.py:18-51 (new path: causal & pad keys masked)
  *             models/nn/sequential/sasrec/model.py:229-231,435 (legacy: causal only) ; bert4rec/model.py:494 (pad keys only)
  * q/k/v: 2-D bf16 arrays whose rows are tokens; head h reads columns x_c0 + h*head_dim.  out: bf16 [B*L, ldo].

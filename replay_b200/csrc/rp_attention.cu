@@ -1,4 +1,4 @@
-// rp_attention.cu - padded-sequence multi-head attention for L <= 512 (L > 256: head_dim 64 only) (SASRec causal + key-padding, BERT4Rec key-padding):
+// rp_attention.cu - padded-sequence multi-head attention for L <= 512, head_dim 64 or 128 (SASRec causal + key-padding, BERT4Rec key-padding):
 // fused forward on wgmma (S = Q.K^T in registers -> masked softmax in registers -> P bf16 as the register A operand of O = P.V),
 // the row-wise softmax backward that sits between the batched backward GEMMs (rp_gemm), and the fused backward (below).
 //
@@ -32,12 +32,19 @@ struct AttnParams {
 static constexpr float kLog2eA = 1.4426950408889634f;
 
 static constexpr int kAfThreads = 256;  // two warpgroups: query rows [0, 64) and [64, 128) of the tile
+static constexpr int kAfVStages = 3;    // V ring of attn_fwd_kernel<128, 2>: 64-key stages of 16 KB
 
 // KB = number of 256-key blocks the CTA keeps resident (1: L <= 256, 2: L <= 512).  Q, K and V of the tile stay in shared
 // memory; each warpgroup walks the visible keys in 64-key chunks twice: pass 1 takes the row max of S = Q.K^T, pass 2
 // recomputes the chunk, forms P = exp(S - max) in registers (saved un-dropped to p_save if asked, then dropped) and
 // accumulates O += P.V with P as the register A operand.  Chunks entirely above the causal diagonal of a warpgroup's rows
 // are skipped (their P is zero).
+//
+// <128, 2> (STREAM_V): 512 keys of K and V at 128 head dims do not both fit in shared memory.  Q and K stay resident, so
+// pass 1 is the same; V streams through a ring of kAfVStages 64-key stages (TMA box [64 rows x 64 columns], tmV built with a
+// 64-row box), loaded by thread 0 ahead of pass 2.  Both warpgroups walk every loaded chunk of the tile - a warpgroup whose
+// rows see none of the chunk's keys skips the MMA - and every thread releases a stage once its wgmma on it has completed,
+// so the "empty" barrier always counts kAfThreads arrivals and thread 0 refills the stage after both warpgroups let it go.
 template <int HD, int KB>
 __global__ void __launch_bounds__(kAfThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -46,11 +53,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   constexpr int Q_BYTES = HC * 128 * 128;     // [128 x HD]
   constexpr int KV_CHUNK = KB * 256 * 128;    // one 64-wide head-dim chunk of all resident keys
   constexpr int KV_BYTES = HC * KV_CHUNK;     // [256*KB x HD]
+  constexpr bool STREAM_V = HD == 128 && KB == 2;
+  constexpr int V_STAGE = HC * 64 * 128;      // one 64-key chunk of V: HC boxes of [64 x 64], 8 KB apart
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + Q_BYTES;
-  uint8_t* sV = sK + KV_BYTES;
+  uint8_t* sV = sK + KV_BYTES;                // STREAM_V: the ring, then its full / empty barriers
+  uint64_t* v_full = reinterpret_cast<uint64_t*>(sV + kAfVStages * V_STAGE);
+  uint64_t* v_empty = v_full + kAfVStages;
   __shared__ __align__(16) uint32_t s_colkey[256 * KB];   // dropout key of every key position
   __shared__ uint8_t s_keyok[256 * KB];                    // key position is real (j < L, and not padding if masked)
   __shared__ uint64_t bar_load;
@@ -81,18 +92,33 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int n_boxes = (nk32 + 127) / 128;
   const int n64 = (nk32 + 63) / 64;
 
+  // STREAM_V: 64-key chunk ch of V into stage ch % kAfVStages
+  auto v_load = [&](int ch) {
+    uint64_t* full = v_full + ch % kAfVStages;
+    mbar_arrive_expect_tx(full, V_STAGE);
+    for (int c = 0; c < HC; ++c)
+      tma_load_2d(sV + (ch % kAfVStages) * V_STAGE + c * 8192, &tmV, full, p.v_c0 + h * HD + c * 64, b * L + ch * 64);
+  };
   if (threadIdx.x == 0) {
     mbar_init(&bar_load, 1);
+    if constexpr (STREAM_V)
+      for (int s = 0; s < kAfVStages; ++s) {
+        mbar_init(v_full + s, 1);
+        mbar_init(v_empty + s, kAfThreads);
+      }
     fence_barrier_init();
     const int row0 = b * L;
-    mbar_arrive_expect_tx(&bar_load, HC * 128 * 128 + 2 * HC * n_boxes * 128 * 128);
+    mbar_arrive_expect_tx(&bar_load, HC * 128 * 128 + (STREAM_V ? 1 : 2) * HC * n_boxes * 128 * 128);
     for (int c = 0; c < HC; ++c) {
       tma_load_2d(sQ + c * 16384, &tmQ, &bar_load, p.q_c0 + h * HD + c * 64, row0 + q0);
       for (int bx = 0; bx < n_boxes; ++bx) {
         tma_load_2d(sK + c * KV_CHUNK + bx * 16384, &tmK, &bar_load, p.k_c0 + h * HD + c * 64, row0 + bx * 128);
-        tma_load_2d(sV + c * KV_CHUNK + bx * 16384, &tmV, &bar_load, p.v_c0 + h * HD + c * 64, row0 + bx * 128);
+        if constexpr (!STREAM_V)
+          tma_load_2d(sV + c * KV_CHUNK + bx * 16384, &tmV, &bar_load, p.v_c0 + h * HD + c * 64, row0 + bx * 128);
       }
     }
+    if constexpr (STREAM_V)
+      for (int ch = 0; ch < min(kAfVStages, n64); ++ch) v_load(ch);
   }
   for (int j = threadIdx.x; j < 256 * KB; j += kAfThreads) {
     s_colkey[j] = p.drop_p > 0.f ? drop_col_key((uint32_t)j) : 0u;
@@ -155,7 +181,25 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   float oacc[HD / 2];
   acc_zero(oacc);
   float suma = 0.f, sumb = 0.f;
-  for (int ch = 0; ch < n_live; ++ch) {
+  // STREAM_V: hand stage ch back once this thread's wgmma on it has completed; thread 0 refills it with chunk ch + kAfVStages
+  // after all kAfThreads threads have
+  auto v_release = [&](int ch) {
+    mbar_arrive(v_empty + ch % kAfVStages);
+    if (threadIdx.x == 0 && ch + kAfVStages < n64) {
+      mbar_wait(v_empty + ch % kAfVStages, (ch / kAfVStages) & 1);
+      v_load(ch + kAfVStages);
+    }
+    __syncwarp();
+  };
+  const int n_walk = STREAM_V ? n64 : n_live;
+  for (int ch = 0; ch < n_walk; ++ch) {
+    if constexpr (STREAM_V) {
+      mbar_wait(v_full + ch % kAfVStages, (ch / kAfVStages) & 1);
+      if (ch >= n_live) {
+        v_release(ch);
+        continue;
+      }
+    }
     float sacc[32];
     qk_chunk(sacc, ch * 64);
     uint32_t pk[16];
@@ -189,11 +233,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {  // 16 keys per step: A fragment = P columns [16 kk, 16 kk + 16) of the chunk
       const uint32_t a[4] = {pk[4 * kk], pk[4 * kk + 1], pk[4 * kk + 2], pk[4 * kk + 3]};
-      WgmmaRS<HD>::template run<1>(oacc, a, desc_mn(smem_u32(sV) + (ch * 4 + kk) * 2048, KV_CHUNK), 1);
+      if constexpr (STREAM_V)
+        WgmmaRS<HD>::template run<1>(oacc, a, desc_mn(smem_u32(sV) + (ch % kAfVStages) * V_STAGE + kk * 2048, 8192), 1);
+      else
+        WgmmaRS<HD>::template run<1>(oacc, a, desc_mn(smem_u32(sV) + (ch * 4 + kk) * 2048, KV_CHUNK), 1);
     }
     wg_commit();
     wg_wait<0>();
     wg_fence_acc(oacc);
+    if constexpr (STREAM_V) v_release(ch);
   }
   // probability rows of the chunks above the diagonal of this warpgroup are zero
   for (int ch = n_live; ch < n64; ++ch)
@@ -457,7 +505,6 @@ RP_API int rp_attn_fwd(const rp_attn_desc* a, void* stream_) {
   if (!a || !a->q || !a->k || !a->v || !a->out || !a->pad_mask) return RP_EINVAL;
   if (a->L <= 0 || a->L > 512 || a->B <= 0 || a->H <= 0) return RP_ESHAPE;
   if (a->head_dim != 64 && a->head_dim != 128) return RP_ESHAPE;
-  if (a->L > 256 && a->head_dim != 64) return RP_ESHAPE;  // 512 resident keys x 128 head dims do not fit shared memory
   if (a->ldo % 8 != 0) return RP_EALIGN;
   AttnParams p;
   p.B = a->B; p.H = a->H; p.L = a->L; p.Lp = (a->L + 63) & ~63;
@@ -472,9 +519,14 @@ RP_API int rp_attn_fwd(const rp_attn_desc* a, void* stream_) {
   int rc;
   if ((rc = make_tmap_bf16(&tmQ, a->q, a->q_rows, a->q_cols, a->ldq, 128)) != RP_OK) return rc;
   if ((rc = make_tmap_bf16(&tmK, a->k, a->k_rows, a->k_cols, a->ldk, 128)) != RP_OK) return rc;
-  if ((rc = make_tmap_bf16(&tmV, a->v, a->v_rows, a->v_cols, a->ldv, 128)) != RP_OK) return rc;
+  const bool stream_v = a->L > 256 && a->head_dim == 128;   // V through the 64-key ring of attn_fwd_kernel<128, 2>
+  if ((rc = make_tmap_bf16(&tmV, a->v, a->v_rows, a->v_cols, a->ldv, stream_v ? 64 : 128)) != RP_OK) return rc;
   dim3 grid((a->L + 127) / 128, a->H, a->B);
-  if (a->L > 256) {
+  if (stream_v) {
+    const int smem = 2 * (16384 + 65536) + kAfVStages * (16384 + 2 * 8) + 1024;
+    RP_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel<128, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attn_fwd_kernel<128, 2><<<grid, kAfThreads, smem, stream>>>(tmQ, tmK, tmV, p);
+  } else if (a->L > 256) {
     const int smem = 16384 + 2 * 65536 + 1024;
     RP_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel<64, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attn_fwd_kernel<64, 2><<<grid, kAfThreads, smem, stream>>>(tmQ, tmK, tmV, p);

@@ -182,7 +182,8 @@ class SasRecEngine:
         self.rng_counter = torch.zeros(1, device=self.dev, dtype=torch.int64)
         self.seed = seed & 0xFFFFFFFFFFFF
         self.training = with_grad
-        # fused attention backward: head_dim 64, L <= 256; otherwise saved probabilities + batched GEMMs
+        # fused attention backward: head_dim 64, L <= 256; otherwise (head_dim 128, or L in (256, 512]) saved probabilities +
+        # batched GEMMs
         self.fused_attn_bwd = cfg.head_slot == 64 and seq_len <= 256
         self.sampled = None       # full-catalog CE unless set_loss() selects a sampled head
         self.sce = None           # buffers of the scalable CE head (set_loss("sce", ...))
@@ -223,8 +224,8 @@ class SasRecEngine:
             raise ValueError(f"sequence length {seq_len} exceeds max_len {cfg.max_len}")
         if cfg.variant == "legacy" and seq_len != cfg.max_len:
             raise ValueError("legacy SASRec needs seq_len == max_len (sasrec/model.py:528-529)")
-        if seq_len > 512 or (seq_len > 256 and cfg.head_slot != 64):
-            raise ValueError("attention kernels support seq_len <= 256 (head_dim 128) / <= 512 (head_dim 64)")
+        if seq_len > 512:
+            raise ValueError("attention kernels support seq_len <= 512")
 
     def resize(self, max_batch: int, seq_len: int, with_grad: bool | None = None):
         """New batch geometry (a larger validation / predict batch, another sequence length): ONLY the activation workspace is
@@ -793,7 +794,8 @@ class SasRecEngine:
     def _attention_backward(self, i: int, q, k, v, dq, dk, dv, causal: bool, mask_pad_keys: bool):
         """dQ, dK, dV of block ``i``'s attention core into the (tensor, first column) destinations ``dq``, ``dk``, ``dv`` from
         s["d_o"] and what ``_attention_forward(i, True, q, k, v, ...)`` saved: the fused kernel for head slot 64 at L <= 256,
-        otherwise dPd = dO.V^T, the row-wise softmax backward over the saved probabilities, and three batched GEMMs."""
+        otherwise (head slot 128 at any L <= 512, head slot 64 at L > 256) dPd = dO.V^T, the row-wise softmax backward over
+        the saved probabilities, and three batched GEMMs."""
         cfg, T, d, L, Lp = self.cfg, self.T, self.cfg.dp, self.L, self.Lp
         a, s, drop = self.act[i], self.s, cfg.dropout
         if self.fused_attn_bwd:
