@@ -1110,9 +1110,8 @@ __global__ void __launch_bounds__(256) ce_bias_colsum_kernel(const __nv_bfloat16
   }
 }
 
-// d = 512: the [128 x 512] fp32 gradient accumulator does not fit the registers of the two warpgroups, so the backward
-// materialises the softmax numerators G (bf16) for a chunk of tokens at a time and runs three plain GEMMs per chunk.
-// Chunk rows: as many as fit the G budget (RP_CE_WIDE_G_BYTES, default 8 GiB), multiple of 128.
+// d = 512 backward (wide_bwd): the materialised G is bf16 [chunk rows, wide_ldg]; chunk rows: as many as fit the G budget
+// (RP_CE_WIDE_G_BYTES, default 8 GiB), multiple of 128.
 static long long wide_ldg(int n_items) { return ((long long)n_items + 63) / 64 * 64; }
 static int wide_chunk_rows(int cap, int n_items) {
   const char* env = getenv("RP_CE_WIDE_G_BYTES");  // read per call: the workspace query and the launch must agree
@@ -1143,8 +1142,15 @@ static int pick_splits(int n_row_tiles, int n_col_tiles, int max_splits = 8) {
 
 using namespace rp;
 
-// workspace layout: [part float2 cap*8*2][block_sums 1024 f][ticket, bound[3], flag, pad -> 64 B][zpart 16*cap f]
-//                   [part_dh 8*cap*d f]
+// Workspace of the CE and BCE heads (cap = capacity; ops.ce_head_fused_taken reads `flag` at this layout):
+//   part        float2 [cap * kMaxSplitsFwd * 2]   (max, sum) per row and column split of the two-pass forward
+//   block_sums  float [1024]                        per-block sums of the deterministic loss reductions
+//   ticket, bound[3], flag, pad -> 64 B            zeroed by every CE forward
+//   zpart       float [kMaxSplits * cap]            row sums / row losses per column split (BCE's un-fused forward: its
+//                                                   softplus row sums)
+//   roww        float [round_up(cap, 4)]            gradient weight per row (BCE at d = 512: the sigmoid's exponent offsets)
+//   part_dh     float [kMaxSplits * cap * d]        partial dH per column split, d <= 256 only
+// then 256 B of slack; at d = 512, from the next 1 KiB boundary, the G chunk and the split-K partials of dH (ce_ws_bytes).
 struct CeWs {
   float2* part; float* block_sums; unsigned int* ticket; unsigned int* bound; int32_t* flag; float* zpart; float* roww; float* part_dh;
 };
@@ -1165,7 +1171,7 @@ static size_t ce_ws_bytes(int cap, int n_items, int d) {
   }
   return b;
 }
-static CeWs ce_ws(void* workspace, int cap, int d) {
+static CeWs ce_ws(void* workspace, int cap) {
   uint8_t* w = reinterpret_cast<uint8_t*>(workspace);
   CeWs r;
   r.part = reinterpret_cast<float2*>(w);
@@ -1181,7 +1187,6 @@ static CeWs ce_ws(void* workspace, int cap, int d) {
   r.roww = reinterpret_cast<float*>(w);   // gradient weight per row (CeRowOpts), written by every forward finalisation
   w += (size_t)(cap + 3) / 4 * 16;
   r.part_dh = reinterpret_cast<float*>(w);
-  (void)d;
   return r;
 }
 
@@ -1190,7 +1195,32 @@ RP_API size_t rp_ce_head_workspace(int capacity_tokens, int n_items, int d) {
   return ce_ws_bytes(capacity_tokens, n_items, d);
 }
 
-template <int KCH, int NSTAGE, bool BCE = false>
+// Argument checks of the five head entry points, in the order their error codes take precedence.  `args_ok`: the entry
+// point's own required arguments are valid (an entry point that always reads the workspace counts it here, so a null one is
+// RP_EINVAL there); `needs_ws`: this call reads the workspace, which must then be present and large enough.
+static int check_head_args(const void* hc, const void* table, const int32_t* labels, const int32_t* n_valid,
+                           const float* loss_out, bool args_ok, int capacity, int n_items, int d, bool needs_ws,
+                           const void* workspace, size_t workspace_bytes) {
+  if (!hc || !table || !labels || !n_valid || !loss_out || !args_ok) return RP_EINVAL;
+  if (capacity <= 0 || n_items <= 0) return RP_ESHAPE;
+  if (d != 64 && d != 128 && d != 256 && d != 512) return RP_ESHAPE;
+  if (needs_ws && (!workspace || workspace_bytes < ce_ws_bytes(capacity, n_items, d))) return RP_EWORKSPACE;
+  return RP_OK;
+}
+
+// row tiles the column splits are balanced over: those the host expects to hold valid targets, else all of them
+static int hint_row_tiles(int n_valid_hint, int capacity) {
+  const int rows = (n_valid_hint > 0 && n_valid_hint <= capacity) ? n_valid_hint : capacity;
+  return (rows + kT - 1) / kT;
+}
+
+// grid of the finalisation kernels (one warp per row, 8 per CTA)
+static int finalize_blocks(int capacity) {
+  const int blocks = (capacity + 7) / 8;
+  return blocks > 1024 ? 1024 : blocks;
+}
+
+template <int KCH, int NSTAGE, bool BCE>
 static int launch_ce_fwd(const CUtensorMap& tmA, const CUtensorMap& tmB, const int32_t* n_valid, int n_items,
                          int n_splits, int n_tok_tiles, const float* bias, float2* part, const int32_t* skip,
                          cudaStream_t stream) {
@@ -1202,12 +1232,25 @@ static int launch_ce_fwd(const CUtensorMap& tmA, const CUtensorMap& tmB, const i
   return RP_OK;
 }
 
+// CE's two-pass forward and BCE's un-fused forward: (max, sum) or softplus row sums per (row, column split)
+template <bool BCE>
+static int dispatch_ce_fwd(int d, const CUtensorMap& tmA, const CUtensorMap& tmB, const int32_t* n_valid, int n_items,
+                           int n_splits, int n_tok_tiles, const float* bias, float2* part, const int32_t* skip,
+                           cudaStream_t stream) {
+  switch (d) {
+    case 64: return launch_ce_fwd<1, 8, BCE>(tmA, tmB, n_valid, n_items, n_splits, n_tok_tiles, bias, part, skip, stream);
+    case 128: return launch_ce_fwd<2, 8, BCE>(tmA, tmB, n_valid, n_items, n_splits, n_tok_tiles, bias, part, skip, stream);
+    case 256: return launch_ce_fwd<4, 8, BCE>(tmA, tmB, n_valid, n_items, n_splits, n_tok_tiles, bias, part, skip, stream);
+    default: return launch_ce_fwd<8, 5, BCE>(tmA, tmB, n_valid, n_items, n_splits, n_tok_tiles, bias, part, skip, stream);
+  }
+}
+
 template <int KCH, int NSTAGE, int TN, int MODE>
 static int launch_ce_bwd(const CUtensorMap& tmA, const void* b_mat, int b_rows, const void* a_rows, const float* cvec,
                          const int32_t* labels,
                          const void* table, const float* loss_inv, const int32_t* n_valid, int n_items, const float* bias,
                          float* d_bias, void* out, int grid, const int32_t* safe_flag, int run_if_safe, int n_splits,
-                         int capacity, float* zpart, cudaStream_t stream, const CeDirect& direct = CeDirect{nullptr, nullptr, nullptr, nullptr, CeRowOpts{nullptr, nullptr, 0, 0.f, 0.f}, 0}) {
+                         int capacity, float* zpart, cudaStream_t stream, const CeDirect& direct) {
   // row tile + a ring of NSTAGE column tiles; the fp32 accumulator stage reuses the ring at the end
   const int ring = NSTAGE * KCH * TN * 128, stage = 128 * (KCH * 64 + 4) * 4;
   const int smem = KCH * kChunk + (ring > stage ? ring : stage) + 1024;
@@ -1231,7 +1274,7 @@ static int dispatch_ce_bwd(int d, const CUtensorMap& tmA, const void* b_mat, int
                            const int32_t* labels,
                            const void* table, const float* loss_inv, const int32_t* n_valid, int n_items, const float* bias,
                            float* d_bias, void* out, int grid, const int32_t* safe_flag, int run_if_safe, int n_splits,
-                           int capacity, float* zpart, cudaStream_t stream, const CeDirect& direct = CeDirect{nullptr, nullptr, nullptr, nullptr, CeRowOpts{nullptr, nullptr, 0, 0.f, 0.f}, 0}) {
+                           int capacity, float* zpart, cudaStream_t stream, const CeDirect& direct = CeDirect{}) {
   switch (d) {
     case 64:
       return launch_ce_bwd<1, 8, 128, MODE>(tmA, b_mat, b_rows, a_rows, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, out, grid,
@@ -1267,6 +1310,101 @@ static int dispatch_bce_rows(int d, const CUtensorMap& tmA, const void* table, i
   }
 }
 
+// The fused CE pass (MODE 2: row sums of exp(s) and the un-normalised dH in one sweep) and its completion.  With one column
+// split every CTA sees the whole catalog: lse / cvec / dH / row losses come straight out of the pass and
+// ce_loss_reduce_kernel sums the losses.  With several, ce_fused_finalize_kernel reduces the split partials.
+// behind == false: runs when the device-side bound held, exponent offset 0.  behind == true: the pass behind the two-pass
+// forward, runs when the bound failed, exponent offset -lse[t] (G = softmax, z ~ 1, whatever |logit| is).
+static int ce_fused_pass(bool behind, const CUtensorMap& tmA, const void* hc, const void* table, const float* bias,
+                         const int32_t* labels, const int32_t* n_valid, int capacity, int n_items, int d, float* loss_out,
+                         float* lse, float* cvec, void* d_hc, int n_valid_hint, const CeRowOpts& row, const CeWs& ws,
+                         cudaStream_t stream) {
+  const int run_if_safe = behind ? 0 : 1, use_lse_off = behind ? 1 : 0;
+  const int hint_tiles = hint_row_tiles(n_valid_hint, capacity), n_item_tiles = (n_items + kT - 1) / kT;
+  const int P = pick_splits(hint_tiles, n_item_tiles);
+  CeDirect direct{nullptr, lse, nullptr, nullptr, row, use_lse_off};
+  if (P == 1) {
+    direct.d_hc = reinterpret_cast<__nv_bfloat16*>(d_hc);
+    direct.cvec = cvec;
+    direct.row_loss = ws.zpart;  // the row-sum partials are not needed in this mode: reuse their buffer
+  }
+  const int rc = dispatch_ce_bwd<2>(d, tmA, table, n_items, hc, cvec, labels, table, loss_out + 1, n_valid, n_items, bias, nullptr,
+                                    ws.part_dh, (capacity + kT - 1) / kT * P, ws.flag, run_if_safe, P, capacity, ws.zpart, stream,
+                                    direct);
+  if (rc != RP_OK) return rc;
+  if (P == 1)
+    ce_loss_reduce_kernel<<<1, 1024, 0, stream>>>(ws.zpart, n_valid, ws.flag, loss_out, run_if_safe);
+  else
+    ce_fused_finalize_kernel<<<finalize_blocks(capacity), 256, 0, stream>>>(
+        ws.part_dh, ws.zpart, reinterpret_cast<const __nv_bfloat16*>(hc), reinterpret_cast<const __nv_bfloat16*>(table), labels,
+        bias, n_valid, ws.flag, P, 1, capacity, d, lse, cvec, reinterpret_cast<__nv_bfloat16*>(d_hc), ws.block_sums, ws.ticket,
+        loss_out, row, use_lse_off, run_if_safe);
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+// d = 512 backward of both heads.  The [128 x 512] fp32 gradient accumulator does not fit the registers of the two
+// warpgroups, so per token chunk (wide_chunk_rows) three plain GEMMs run on the materialised G (bf16):
+//   G = act(hc . E^T + b) with per-row exponent offsets `off`:  act 3 (CE): exp2(x log2e + cvec[t]), the weighted softmax
+//       / T_v;  act 4 (BCE): sigmoid / T_v, 0 on rows past T_v (bce_row_offset_kernel)
+//   d_bias (+)= colsum G (iff bias);  dH = G . E - roww[t] E[y_t] / T_v (roww null = 1);  dE (+)= G^T . hc
+// The one-hot part of dE and d_bias is the caller's ce_label_scatter_kernel.
+static int wide_bwd(int act, const float* off, const float* roww, const void* hc, const void* table, const float* bias,
+                    const int32_t* labels, const int32_t* n_valid, int capacity, int n_items, int d, const float* loss_inv,
+                    void* d_hc, float* d_table, float* d_bias, int n_valid_hint, void* workspace, cudaStream_t stream) {
+  const long long ldg = wide_ldg(n_items);
+  const int chunk = wide_chunk_rows(capacity, n_items);
+  uint8_t* G = reinterpret_cast<uint8_t*>(workspace) + (ce_ws_base_bytes(capacity, d) + 1023) / 1024 * 1024;
+  float* part = reinterpret_cast<float*>(G + (size_t)chunk * ldg * 2);
+  const long long part_stride = (long long)chunk * d;
+  const int hint = (n_valid_hint > 0 && n_valid_hint < capacity) ? n_valid_hint : capacity;
+  int rc;
+  for (int c0 = 0, it = 0; c0 < capacity; c0 += chunk, ++it) {
+    const int rows = (capacity - c0 < chunk) ? capacity - c0 : chunk;
+    // G [rows, n_items] = act((hc[c0:c0+rows] . E^T + b), off[c0:c0+rows])   (the epilogue adds the bias before the act)
+    rp_gemm_desc g = rp_gemm_default();
+    g.A = reinterpret_cast<const __nv_bfloat16*>(hc) + (size_t)c0 * d; g.a_rows = rows; g.a_cols = d; g.lda = d; g.a_mn = 0;
+    g.B = table; g.b_rows = n_items; g.b_cols = d; g.ldb = d; g.b_mn = 0;
+    g.M = rows; g.N = n_items; g.K = d;
+    g.C = G; g.ldc = ldg; g.out_mode = 0; g.act = act; g.row_exp2_offset = off + c0; g.bias = bias;
+    g.m_limit_dev = n_valid; g.m_limit_base = c0;
+    if ((rc = rp_gemm(&g, stream)) != RP_OK) return rc;
+    if (bias) {
+      ce_bias_colsum_kernel<<<(n_items + 255) / 256, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(G), ldg, rows, c0,
+                                                                       n_valid, n_items, d_bias, it != 0);
+      RP_LAUNCH_CHECK();
+    }
+    // dH[c0:c0+rows] = G . E - label term   (A = G K-major over the items, B = E read MN-major).  Few row tiles against a
+    // contraction over the whole catalog: split-K partials (fp32, deterministic), reduced together with the label term
+    int live = hint - c0;
+    live = live < 128 ? 128 : (live > rows ? rows : live);
+    int split = (2 * sm_count()) / (((live + 127) / 128) * (d / 128));
+    split = split < 1 ? 1 : (split > kWideSplitK ? kWideSplitK : split);
+    g = rp_gemm_default();
+    g.split_k = split;
+    g.A = G; g.a_rows = rows; g.a_cols = n_items; g.lda = ldg; g.a_mn = 0;
+    g.B = table; g.b_rows = n_items; g.b_cols = d; g.ldb = d; g.b_mn = 1;
+    g.M = rows; g.N = d; g.K = n_items;
+    g.C = part; g.ldc = d; g.out_mode = 3; g.c_split_stride = part_stride;
+    g.m_limit_dev = n_valid; g.m_limit_base = c0;
+    if ((rc = rp_gemm(&g, stream)) != RP_OK) return rc;
+    ce_dh_reduce_kernel<<<sm_count() * 4, 256, 0, stream>>>(part, split, part_stride, rows, c0,
+                                                             reinterpret_cast<__nv_bfloat16*>(d_hc),
+                                                             reinterpret_cast<const __nv_bfloat16*>(table), labels, loss_inv,
+                                                             n_valid, d, roww);
+    RP_LAUNCH_CHECK();
+    // dE (+)= G^T . hc[c0:c0+rows]      (A = G read MN-major, contraction over the chunk's valid tokens)
+    g = rp_gemm_default();
+    g.A = G; g.a_rows = rows; g.a_cols = n_items; g.lda = ldg; g.a_mn = 1;
+    g.B = reinterpret_cast<const __nv_bfloat16*>(hc) + (size_t)c0 * d; g.b_rows = rows; g.b_cols = d; g.ldb = d; g.b_mn = 1;
+    g.M = n_items; g.N = d; g.K = rows;
+    g.C = d_table; g.ldc = d; g.out_mode = it == 0 ? 2 : 4;
+    g.k_limit_dev = n_valid; g.k_limit_base = c0;
+    if ((rc = rp_gemm(&g, stream)) != RP_OK) return rc;
+  }
+  return RP_OK;
+}
+
 // Forward of the CE head.  hc bf16 [capacity, d] (rows >= *n_valid ignored), table bf16 [n_items, d], labels int32
 // [capacity], n_valid int32 [1] (device).  Outputs: loss_out fp32 [2] = {mean CE, 1/T_v}; lse fp32 [capacity]; cvec fp32
 // (exponent offsets consumed by rp_ce_head_bwd).
@@ -1294,23 +1432,17 @@ RP_API int rp_ce_head_fwd_w(const void* hc, const void* table, const float* bias
                             void* d_hc, int n_valid_hint, const float* row_weight, int loss_kind, float log_eps, float clamp,
                             void* workspace, size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (loss_kind != 0 && loss_kind != 1) return RP_EINVAL;
-  if (!hc || !table || !labels || !n_valid || !loss_out || !lse || !cvec || !workspace) return RP_EINVAL;
-  if (capacity <= 0 || n_items <= 0) return RP_ESHAPE;
-  if (d != 64 && d != 128 && d != 256 && d != 512) return RP_ESHAPE;
-  if (workspace_bytes < ce_ws_bytes(capacity, n_items, d)) return RP_EWORKSPACE;
+  int rc = check_head_args(hc, table, labels, n_valid, loss_out, (loss_kind == 0 || loss_kind == 1) && lse && cvec && workspace,
+                           capacity, n_items, d, true, workspace, workspace_bytes);
+  if (rc != RP_OK) return rc;
   const bool fused = d_hc != nullptr && d <= 256;
   const int n_tok_tiles = (capacity + kT - 1) / kT, n_item_tiles = (n_items + kT - 1) / kT;
-  const int hint_tiles = (n_valid_hint > 0 && n_valid_hint <= capacity) ? (n_valid_hint + kT - 1) / kT : n_tok_tiles;
-  CeWs ws = ce_ws(workspace, capacity, d);
+  const CeWs ws = ce_ws(workspace, capacity);
+  const CeRowOpts row{row_weight, ws.roww, loss_kind, log_eps, clamp};
   CUtensorMap tmA, tmB;
-  int rc;
   if ((rc = make_tmap_bf16(&tmA, hc, capacity, d, d, 128)) != RP_OK) return rc;
   if ((rc = make_tmap_bf16(&tmB, table, n_items, d, d, 128)) != RP_OK) return rc;
   RP_CUDA_CHECK(cudaMemsetAsync(ws.ticket, 0, 64, stream));  // ticket, bound[3], flag
-  const int32_t* skip = nullptr;
-  int blocks = (capacity + 7) / 8;
-  if (blocks > 1024) blocks = 1024;
   if (fused) {
     ce_bound_kernel<<<sm_count() * 8, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(hc),
                                                         reinterpret_cast<const __nv_bfloat16*>(table), bias, n_valid, n_items, d,
@@ -1318,72 +1450,32 @@ RP_API int rp_ce_head_fwd_w(const void* hc, const void* table, const float* bias
     RP_LAUNCH_CHECK();
     ce_flag_kernel<<<1, 1, 0, stream>>>(ws.bound, ws.flag);
     RP_LAUNCH_CHECK();
-    const int P = pick_splits(hint_tiles, n_item_tiles);
-    CeDirect direct{nullptr, lse, nullptr, nullptr, CeRowOpts{row_weight, ws.roww, loss_kind, log_eps, clamp}, 0};
-    if (P == 1) {  // every CTA sees the whole catalog: lse / dH / loss terms come straight out of the fused kernel
-      direct.d_hc = reinterpret_cast<__nv_bfloat16*>(d_hc);
-      direct.cvec = cvec;
-      direct.row_loss = ws.zpart;  // the row-sum partials are not needed in this mode: reuse their buffer
-    }
-    rc = dispatch_ce_bwd<2>(d, tmA, table, n_items, hc, cvec, labels, table, loss_out + 1, n_valid, n_items, bias, nullptr, ws.part_dh,
-                            n_tok_tiles * P, ws.flag, 1, P, capacity, ws.zpart, stream, direct);
-    if (rc != RP_OK) return rc;
-    if (P == 1) {
-      ce_loss_reduce_kernel<<<1, 1024, 0, stream>>>(ws.zpart, n_valid, ws.flag, loss_out, 1);
-      RP_LAUNCH_CHECK();
-    } else
-    ce_fused_finalize_kernel<<<blocks, 256, 0, stream>>>(ws.part_dh, ws.zpart, reinterpret_cast<const __nv_bfloat16*>(hc),
-                                                         reinterpret_cast<const __nv_bfloat16*>(table), labels, bias, n_valid,
-                                                         ws.flag, P, 1, capacity, d, lse, cvec,
-                                                         reinterpret_cast<__nv_bfloat16*>(d_hc), ws.block_sums, ws.ticket, loss_out,
-                                                         CeRowOpts{row_weight, ws.roww, loss_kind, log_eps, clamp}, 0, 1);
-    RP_LAUNCH_CHECK();
-    skip = ws.flag;
+    if ((rc = ce_fused_pass(false, tmA, hc, table, bias, labels, n_valid, capacity, n_items, d, loss_out, lse, cvec, d_hc,
+                            n_valid_hint, row, ws, stream)) != RP_OK)
+      return rc;
   }
-  int P2 = pick_splits(hint_tiles, n_item_tiles, kMaxSplitsFwd);
+  int P2 = pick_splits(hint_row_tiles(n_valid_hint, capacity), n_item_tiles, kMaxSplitsFwd);
   if (fused) {  // two-pass fallback behind the fused pass: it only runs when the bound failed; launching (and retiring) tens of
                 // thousands of CTAs that exit at once is not free, so keep it at about two waves
     const int cap = (2 * sm_count() + n_tok_tiles - 1) / n_tok_tiles;
     if (P2 > cap) P2 = cap;
   }
-  switch (d) {
-    case 64: rc = launch_ce_fwd<1, 8>(tmA, tmB, n_valid, n_items, P2, n_tok_tiles, bias, ws.part, skip, stream); break;
-    case 128: rc = launch_ce_fwd<2, 8>(tmA, tmB, n_valid, n_items, P2, n_tok_tiles, bias, ws.part, skip, stream); break;
-    case 256: rc = launch_ce_fwd<4, 8>(tmA, tmB, n_valid, n_items, P2, n_tok_tiles, bias, ws.part, skip, stream); break;
-    default: rc = launch_ce_fwd<8, 5>(tmA, tmB, n_valid, n_items, P2, n_tok_tiles, bias, ws.part, skip, stream); break;
-  }
-  if (rc != RP_OK) return rc;
-  ce_finalize_kernel<<<blocks, 256, 0, stream>>>(ws.part, reinterpret_cast<const __nv_bfloat16*>(hc),
-                                                 reinterpret_cast<const __nv_bfloat16*>(table), labels, bias, n_valid, P2,
-                                                 capacity, d, lse, cvec, ws.block_sums, ws.ticket, loss_out, skip,
-                                                 CeRowOpts{row_weight, ws.roww, loss_kind, log_eps, clamp});
+  const int32_t* skip = fused ? ws.flag : nullptr;
+  if ((rc = dispatch_ce_fwd<false>(d, tmA, tmB, n_valid, n_items, P2, n_tok_tiles, bias, ws.part, skip, stream)) != RP_OK) return rc;
+  ce_finalize_kernel<<<finalize_blocks(capacity), 256, 0, stream>>>(ws.part, reinterpret_cast<const __nv_bfloat16*>(hc),
+                                                                    reinterpret_cast<const __nv_bfloat16*>(table), labels, bias,
+                                                                    n_valid, P2, capacity, d, lse, cvec, ws.block_sums,
+                                                                    ws.ticket, loss_out, skip, row);
   RP_LAUNCH_CHECK();
   if (fused) {
     // The bound failed (these launches exit at once otherwise): the two-pass forward above has produced lse; the gradient
     // dH comes from the SAME fused kernel, now with the exponent offset -lse[t] per row (G = softmax, z ~ 1) - with its column
     // splits and all SMs busy, where the row-tile-per-CTA MODE 0 pass ran 32 CTAs at BERT4Rec's ~4000 masked positions
     // (2.2 ms of a 4.3 ms step at config 3, whose un-normalised outputs outgrow the bound within a few hundred steps).
-    const int P = pick_splits(hint_tiles, n_item_tiles);
-    CeDirect direct{nullptr, lse, nullptr, nullptr, CeRowOpts{row_weight, ws.roww, loss_kind, log_eps, clamp}, 1};
-    if (P == 1) {
-      direct.d_hc = reinterpret_cast<__nv_bfloat16*>(d_hc);
-      direct.cvec = cvec;
-      direct.row_loss = ws.zpart;
-    }
     RP_CUDA_CHECK(cudaMemsetAsync(ws.ticket, 0, 4, stream));   // the deterministic loss reduction's ticket was used above
-    rc = dispatch_ce_bwd<2>(d, tmA, table, n_items, hc, cvec, labels, table, loss_out + 1, n_valid, n_items, bias, nullptr, ws.part_dh,
-                            n_tok_tiles * P, ws.flag, 0, P, capacity, ws.zpart, stream, direct);
-    if (rc != RP_OK) return rc;
-    if (P == 1) {
-      ce_loss_reduce_kernel<<<1, 1024, 0, stream>>>(ws.zpart, n_valid, ws.flag, loss_out, 0);
-    } else {
-      ce_fused_finalize_kernel<<<blocks, 256, 0, stream>>>(ws.part_dh, ws.zpart, reinterpret_cast<const __nv_bfloat16*>(hc),
-                                                           reinterpret_cast<const __nv_bfloat16*>(table), labels, bias, n_valid,
-                                                           ws.flag, P, 1, capacity, d, lse, cvec,
-                                                           reinterpret_cast<__nv_bfloat16*>(d_hc), ws.block_sums, ws.ticket, loss_out,
-                                                           CeRowOpts{row_weight, ws.roww, loss_kind, log_eps, clamp}, 1, 0);
-    }
-    RP_LAUNCH_CHECK();
+    if ((rc = ce_fused_pass(true, tmA, hc, table, bias, labels, n_valid, capacity, n_items, d, loss_out, lse, cvec, d_hc,
+                            n_valid_hint, row, ws, stream)) != RP_OK)
+      return rc;
   }
   return RP_OK;
 }
@@ -1391,7 +1483,7 @@ RP_API int rp_ce_head_fwd_w(const void* hc, const void* table, const float* bias
 // Backward of rp_ce_head_fwd for d(loss) = 1:
 //   d_hc   bf16 [capacity, d]  (rows < *n_valid) - already written by the forward when it ran fused (`fused` != 0 and the
 //          device-side bound held); otherwise computed here from the stored lse.  d = 512: chunked materialised-G path
-//          (three GEMMs per token chunk, see wide_chunk_rows), workspace required
+//          (three GEMMs per token chunk, see wide_bwd), workspace required
 //   d_table fp32 [n_items, d]  OVERWRITTEN with softmax^T . hc / T_v, then the one-hot part is atomically subtracted
 //   d_bias  fp32 [n_items] (iff bias)  OVERWRITTEN likewise.        d in {64,128,256,512}.
 RP_API int rp_ce_head_bwd(const void* hc, const void* table, const float* bias, const int32_t* labels,
@@ -1399,90 +1491,32 @@ RP_API int rp_ce_head_bwd(const void* hc, const void* table, const float* bias, 
                           const float* cvec /* from fwd */, void* d_hc, float* d_table, float* d_bias, int fused,
                           int n_valid_hint, void* workspace, size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!hc || !table || !labels || !n_valid || !loss_out || !cvec || !d_hc || !d_table) return RP_EINVAL;
-  if ((bias == nullptr) != (d_bias == nullptr)) return RP_EINVAL;
-  if (capacity <= 0 || n_items <= 0) return RP_ESHAPE;
-  if (d != 64 && d != 128 && d != 256 && d != 512) return RP_ESHAPE;
-  if ((fused || d == 512) && (!workspace || workspace_bytes < ce_ws_bytes(capacity, n_items, d))) return RP_EWORKSPACE;
+  int rc = check_head_args(hc, table, labels, n_valid, loss_out, cvec && d_hc && d_table && (bias == nullptr) == (d_bias == nullptr),
+                           capacity, n_items, d, fused || d == 512, workspace, workspace_bytes);
+  if (rc != RP_OK) return rc;
   // gradient weight per row, written by the forward (all ones for the plain CE head); without a workspace: plain head
-  const float* roww = (workspace && workspace_bytes >= ce_ws_bytes(capacity, n_items, d)) ? ce_ws(workspace, capacity, d).roww : nullptr;
-  if (d == 512) {
-    // ---- wide-hidden path: per token chunk  G = exp2((hc.E^T + b) log2e + c_t)  ->  dH = G.E,  dE += G^T.hc,  db += colsum G
-    const long long ldg = wide_ldg(n_items);
-    const int chunk = wide_chunk_rows(capacity, n_items);
-    uint8_t* G = reinterpret_cast<uint8_t*>(workspace) + (ce_ws_base_bytes(capacity, d) + 1023) / 1024 * 1024;
-    float* part = reinterpret_cast<float*>(G + (size_t)chunk * ldg * 2);
-    const long long part_stride = (long long)chunk * d;
-    const int hint = (n_valid_hint > 0 && n_valid_hint < capacity) ? n_valid_hint : capacity;
-    int rc;
-    for (int c0 = 0, it = 0; c0 < capacity; c0 += chunk, ++it) {
-      const int rows = (capacity - c0 < chunk) ? capacity - c0 : chunk;
-      rp_gemm_desc g;
-      memset(&g, 0, sizeof(g));
-      g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
-      // G [rows, n_items] = exp2((hc[c0:c0+rows] . E^T + b) log2e + cvec)   (the epilogue adds the bias before the act)
-      g.A = reinterpret_cast<const __nv_bfloat16*>(hc) + (size_t)c0 * d; g.a_rows = rows; g.a_cols = d; g.lda = d; g.a_mn = 0;
-      g.B = table; g.b_rows = n_items; g.b_cols = d; g.ldb = d; g.b_mn = 0;
-      g.M = rows; g.N = n_items; g.K = d;
-      g.C = G; g.ldc = ldg; g.out_mode = 0; g.act = 3; g.row_exp2_offset = cvec + c0; g.bias = bias;
-      g.m_limit_dev = n_valid; g.m_limit_base = c0;
-      if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
-      if (bias) {
-        ce_bias_colsum_kernel<<<(n_items + 255) / 256, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(G), ldg, rows, c0,
-                                                                         n_valid, n_items, d_bias, it != 0);
-        RP_LAUNCH_CHECK();
-      }
-      // dH[c0:c0+rows] = G . E - onehot   (A = G K-major over the items, B = E read MN-major).  Few row tiles against a
-      // contraction over the whole catalog: split-K partials (fp32, deterministic), reduced together with the label term
-      int live = hint - c0;
-      live = live < 128 ? 128 : (live > rows ? rows : live);
-      int split = (2 * sm_count()) / (((live + 127) / 128) * (d / 128));
-      split = split < 1 ? 1 : (split > kWideSplitK ? kWideSplitK : split);
-      memset(&g, 0, sizeof(g));
-      g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = split;
-      g.A = G; g.a_rows = rows; g.a_cols = n_items; g.lda = ldg; g.a_mn = 0;
-      g.B = table; g.b_rows = n_items; g.b_cols = d; g.ldb = d; g.b_mn = 1;
-      g.M = rows; g.N = d; g.K = n_items;
-      g.C = part; g.ldc = d; g.out_mode = 3; g.c_split_stride = part_stride;
-      g.m_limit_dev = n_valid; g.m_limit_base = c0;
-      if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
-      ce_dh_reduce_kernel<<<sm_count() * 4, 256, 0, stream>>>(part, split, part_stride, rows, c0,
-                                                               reinterpret_cast<__nv_bfloat16*>(d_hc),
-                                                               reinterpret_cast<const __nv_bfloat16*>(table), labels,
-                                                               loss_out + 1, n_valid, d, roww);
-      RP_LAUNCH_CHECK();
-      // dE (+)= G^T . hc[c0:c0+rows]      (A = G read MN-major, contraction over the chunk's valid tokens)
-      memset(&g, 0, sizeof(g));
-      g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
-      g.A = G; g.a_rows = rows; g.a_cols = n_items; g.lda = ldg; g.a_mn = 1;
-      g.B = reinterpret_cast<const __nv_bfloat16*>(hc) + (size_t)c0 * d; g.b_rows = rows; g.b_cols = d; g.ldb = d; g.b_mn = 1;
-      g.M = n_items; g.N = d; g.K = rows;
-      g.C = d_table; g.ldc = d; g.out_mode = it == 0 ? 2 : 4;
-      g.k_limit_dev = n_valid; g.k_limit_base = c0;
-      if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
-    }
-    ce_label_scatter_kernel<<<sm_count() * 4, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(hc), labels, loss_out + 1,
-                                                                 n_valid, d, d_table, d_bias, roww);
-    RP_LAUNCH_CHECK();
-    return RP_OK;
-  }
-  CUtensorMap tmH, tmE;
-  int rc;
-  if ((rc = make_tmap_bf16(&tmH, hc, capacity, d, d, 128)) != RP_OK) return rc;
-  if ((rc = make_tmap_bf16(&tmE, table, n_items, d, d, 128)) != RP_OK) return rc;
-  const int n_tok_tiles = (capacity + kT - 1) / kT, n_item_tiles = (n_items + kT - 1) / kT;
+  const float* roww = (workspace && workspace_bytes >= ce_ws_bytes(capacity, n_items, d)) ? ce_ws(workspace, capacity).roww : nullptr;
   const float* loss_inv = loss_out + 1;
-  const int32_t* flag = fused ? ce_ws(workspace, capacity, d).flag : nullptr;
-  // token-major pass: only when the forward did not already produce d_hc (a fused forward always does: from the fused pass
-  // itself, or - bound failed - from its second launch behind the two-pass forward)
-  if (!fused)
-  rc = dispatch_ce_bwd<0>(d, tmH, table, n_items, hc, cvec, labels, table, loss_inv, n_valid, n_items, bias, nullptr, d_hc, n_tok_tiles, flag, 0,
-                          1, capacity, nullptr, stream,
-                          CeDirect{nullptr, nullptr, nullptr, nullptr, CeRowOpts{nullptr, const_cast<float*>(roww), 0, 0.f, 0.f}});
-  if (rc != RP_OK) return rc;
-  rc = dispatch_ce_bwd<1>(d, tmE, hc, capacity, table, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, d_table, n_item_tiles,
-                          nullptr, 0, 1, capacity, nullptr, stream);
-  if (rc != RP_OK) return rc;
+  if (d == 512) {
+    if ((rc = wide_bwd(3, cvec, roww, hc, table, bias, labels, n_valid, capacity, n_items, d, loss_inv, d_hc, d_table, d_bias,
+                       n_valid_hint, workspace, stream)) != RP_OK)
+      return rc;
+  } else {
+    CUtensorMap tmH, tmE;
+    if ((rc = make_tmap_bf16(&tmH, hc, capacity, d, d, 128)) != RP_OK) return rc;
+    if ((rc = make_tmap_bf16(&tmE, table, n_items, d, d, 128)) != RP_OK) return rc;
+    const int n_tok_tiles = (capacity + kT - 1) / kT, n_item_tiles = (n_items + kT - 1) / kT;
+    // token-major pass: only when the forward did not already produce d_hc (a fused forward always does: from the fused pass
+    // itself, or - bound failed - from its second launch behind the two-pass forward)
+    if (!fused && (rc = dispatch_ce_bwd<0>(d, tmH, table, n_items, hc, cvec, labels, table, loss_inv, n_valid, n_items, bias, nullptr,
+                                           d_hc, n_tok_tiles, nullptr, 0, 1, capacity, nullptr, stream,
+                                           CeDirect{nullptr, nullptr, nullptr, nullptr,
+                                                    CeRowOpts{nullptr, const_cast<float*>(roww), 0, 0.f, 0.f}})) != RP_OK)
+      return rc;
+    rc = dispatch_ce_bwd<1>(d, tmE, hc, capacity, table, cvec, labels, table, loss_inv, n_valid, n_items, bias, d_bias, d_table,
+                            n_item_tiles, nullptr, 0, 1, capacity, nullptr, stream);
+    if (rc != RP_OK) return rc;
+  }
   ce_label_scatter_kernel<<<sm_count() * 4, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(hc), labels, loss_inv,
                                                                n_valid, d, d_table, d_bias, roww);
   RP_LAUNCH_CHECK();
@@ -1490,27 +1524,17 @@ RP_API int rp_ce_head_bwd(const void* hc, const void* table, const float* bias, 
 }
 
 // ---------------------------------------------------------------------------------------------------------------- BCE head
-static int check_bce_args(const void* hc, const void* table, const float* bias, const int32_t* labels, const int32_t* n_valid,
-                          int capacity, int n_items, int d, const float* loss_out, void* workspace, size_t workspace_bytes) {
-  if (!hc || !table || !labels || !n_valid || !loss_out || !workspace) return RP_EINVAL;
-  if (capacity <= 0 || n_items <= 0) return RP_ESHAPE;
-  if (d != 64 && d != 128 && d != 256 && d != 512) return RP_ESHAPE;
-  if (workspace_bytes < ce_ws_bytes(capacity, n_items, d)) return RP_EWORKSPACE;
-  return RP_OK;
-}
-
 // the token-major BCE pass (MODE 3) over the catalog: d_hc, and the row losses when `loss_out` is given.  Without column
 // splits both come out of the pass itself; otherwise bce_finalize_kernel reduces the split partials.
 static int bce_rows_pass(const void* hc, const void* table, const float* bias, const int32_t* labels, const int32_t* n_valid,
                          int capacity, int n_items, int d, float* loss_out, void* d_hc, int n_valid_hint, const CeWs& ws,
                          cudaStream_t stream) {
   const int n_tok_tiles = (capacity + kT - 1) / kT, n_item_tiles = (n_items + kT - 1) / kT;
-  const int hint_tiles = (n_valid_hint > 0 && n_valid_hint <= capacity) ? (n_valid_hint + kT - 1) / kT : n_tok_tiles;
   CUtensorMap tmA;
   int rc;
   if ((rc = make_tmap_bf16(&tmA, hc, capacity, d, d, 128)) != RP_OK) return rc;
-  const int P = pick_splits(hint_tiles, n_item_tiles);
-  CeDirect direct{nullptr, nullptr, nullptr, nullptr, CeRowOpts{nullptr, nullptr, 0, 0.f, 0.f}, 0};
+  const int P = pick_splits(hint_row_tiles(n_valid_hint, capacity), n_item_tiles);
+  CeDirect direct{};
   if (P == 1) {
     direct.d_hc = reinterpret_cast<__nv_bfloat16*>(d_hc);
     direct.row_loss = ws.zpart;
@@ -1525,11 +1549,11 @@ static int bce_rows_pass(const void* hc, const void* table, const float* bias, c
     }
     return RP_OK;
   }
-  int blocks = (capacity + 7) / 8;
-  if (blocks > 1024) blocks = 1024;
-  bce_finalize_kernel<<<blocks, 256, 0, stream>>>(ws.zpart, capacity, 1, ws.part_dh, P, reinterpret_cast<const __nv_bfloat16*>(hc),
-                                                  reinterpret_cast<const __nv_bfloat16*>(table), labels, bias, n_valid, capacity, d,
-                                                  reinterpret_cast<__nv_bfloat16*>(d_hc), ws.block_sums, ws.ticket, loss_out);
+  bce_finalize_kernel<<<finalize_blocks(capacity), 256, 0, stream>>>(ws.zpart, capacity, 1, ws.part_dh, P,
+                                                                     reinterpret_cast<const __nv_bfloat16*>(hc),
+                                                                     reinterpret_cast<const __nv_bfloat16*>(table), labels, bias,
+                                                                     n_valid, capacity, d, reinterpret_cast<__nv_bfloat16*>(d_hc),
+                                                                     ws.block_sums, ws.ticket, loss_out);
   RP_LAUNCH_CHECK();
   return RP_OK;
 }
@@ -1540,32 +1564,26 @@ RP_API int rp_bce_head_fwd(const void* hc, const void* table, const float* bias,
                            int capacity, int n_items, int d, float* loss_out, void* d_hc, int n_valid_hint, void* workspace,
                            size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  int rc = check_bce_args(hc, table, bias, labels, n_valid, capacity, n_items, d, loss_out, workspace, workspace_bytes);
+  int rc = check_head_args(hc, table, labels, n_valid, loss_out, workspace != nullptr, capacity, n_items, d, true, workspace,
+                           workspace_bytes);
   if (rc != RP_OK) return rc;
-  CeWs ws = ce_ws(workspace, capacity, d);
+  const CeWs ws = ce_ws(workspace, capacity);
   RP_CUDA_CHECK(cudaMemsetAsync(ws.ticket, 0, 4, stream));
   if (d_hc != nullptr && d <= 256) return bce_rows_pass(hc, table, bias, labels, n_valid, capacity, n_items, d, loss_out, d_hc,
                                                         n_valid_hint, ws, stream);
   // un-fused: softplus row sums per (row, split), then the loss
   const int n_tok_tiles = (capacity + kT - 1) / kT, n_item_tiles = (n_items + kT - 1) / kT;
-  const int hint_tiles = (n_valid_hint > 0 && n_valid_hint <= capacity) ? (n_valid_hint + kT - 1) / kT : n_tok_tiles;
-  const int P = pick_splits(hint_tiles, n_item_tiles);   // <= kMaxSplits: the partials live in ws.zpart
+  const int P = pick_splits(hint_row_tiles(n_valid_hint, capacity), n_item_tiles);   // <= kMaxSplits: the partials live in ws.zpart
   CUtensorMap tmA, tmB;
   if ((rc = make_tmap_bf16(&tmA, hc, capacity, d, d, 128)) != RP_OK) return rc;
   if ((rc = make_tmap_bf16(&tmB, table, n_items, d, d, 128)) != RP_OK) return rc;
-  float2* zrow = reinterpret_cast<float2*>(ws.zpart);
-  switch (d) {
-    case 64: rc = launch_ce_fwd<1, 8, true>(tmA, tmB, n_valid, n_items, P, n_tok_tiles, bias, zrow, nullptr, stream); break;
-    case 128: rc = launch_ce_fwd<2, 8, true>(tmA, tmB, n_valid, n_items, P, n_tok_tiles, bias, zrow, nullptr, stream); break;
-    case 256: rc = launch_ce_fwd<4, 8, true>(tmA, tmB, n_valid, n_items, P, n_tok_tiles, bias, zrow, nullptr, stream); break;
-    default: rc = launch_ce_fwd<8, 5, true>(tmA, tmB, n_valid, n_items, P, n_tok_tiles, bias, zrow, nullptr, stream); break;
-  }
+  rc = dispatch_ce_fwd<true>(d, tmA, tmB, n_valid, n_items, P, n_tok_tiles, bias, reinterpret_cast<float2*>(ws.zpart), nullptr, stream);
   if (rc != RP_OK) return rc;
-  int blocks = (capacity + 7) / 8;
-  if (blocks > 1024) blocks = 1024;
-  bce_finalize_kernel<<<blocks, 256, 0, stream>>>(ws.zpart, 1, P, nullptr, P, reinterpret_cast<const __nv_bfloat16*>(hc),
-                                                  reinterpret_cast<const __nv_bfloat16*>(table), labels, bias, n_valid, capacity, d,
-                                                  nullptr, ws.block_sums, ws.ticket, loss_out);
+  bce_finalize_kernel<<<finalize_blocks(capacity), 256, 0, stream>>>(ws.zpart, 1, P, nullptr, P,
+                                                                     reinterpret_cast<const __nv_bfloat16*>(hc),
+                                                                     reinterpret_cast<const __nv_bfloat16*>(table), labels, bias,
+                                                                     n_valid, capacity, d, nullptr, ws.block_sums, ws.ticket,
+                                                                     loss_out);
   RP_LAUNCH_CHECK();
   return RP_OK;
 }
@@ -1579,66 +1597,19 @@ RP_API int rp_bce_head_bwd(const void* hc, const void* table, const float* bias,
                            int capacity, int n_items, int d, const float* loss_out, void* d_hc, float* d_table, float* d_bias,
                            int fused, int n_valid_hint, void* workspace, size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  int rc = check_bce_args(hc, table, bias, labels, n_valid, capacity, n_items, d, loss_out, workspace, workspace_bytes);
+  int rc = check_head_args(hc, table, labels, n_valid, loss_out, workspace != nullptr, capacity, n_items, d, true, workspace,
+                           workspace_bytes);
   if (rc != RP_OK) return rc;
   if (!d_hc || !d_table || (bias == nullptr) != (d_bias == nullptr)) return RP_EINVAL;
-  CeWs ws = ce_ws(workspace, capacity, d);
+  const CeWs ws = ce_ws(workspace, capacity);
   const float* loss_inv = loss_out + 1;
   if (d == 512) {
-    const long long ldg = wide_ldg(n_items);
-    const int chunk = wide_chunk_rows(capacity, n_items);
-    uint8_t* G = reinterpret_cast<uint8_t*>(workspace) + (ce_ws_base_bytes(capacity, d) + 1023) / 1024 * 1024;
-    float* part = reinterpret_cast<float*>(G + (size_t)chunk * ldg * 2);
-    const long long part_stride = (long long)chunk * d;
-    const int hint = (n_valid_hint > 0 && n_valid_hint < capacity) ? n_valid_hint : capacity;
     float* off = ws.roww;   // per-row exponent offsets of the sigmoid epilogue (the CE row weights are not used here)
     bce_row_offset_kernel<<<(capacity + 255) / 256 < 1024 ? (capacity + 255) / 256 : 1024, 256, 0, stream>>>(n_valid, capacity, off);
     RP_LAUNCH_CHECK();
-    for (int c0 = 0, it = 0; c0 < capacity; c0 += chunk, ++it) {
-      const int rows = (capacity - c0 < chunk) ? capacity - c0 : chunk;
-      rp_gemm_desc g;
-      memset(&g, 0, sizeof(g));
-      g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
-      // G [rows, n_items] = sigmoid(hc[c0:c0+rows] . E^T + b) / T_v, 0 on rows past T_v
-      g.A = reinterpret_cast<const __nv_bfloat16*>(hc) + (size_t)c0 * d; g.a_rows = rows; g.a_cols = d; g.lda = d; g.a_mn = 0;
-      g.B = table; g.b_rows = n_items; g.b_cols = d; g.ldb = d; g.b_mn = 0;
-      g.M = rows; g.N = n_items; g.K = d;
-      g.C = G; g.ldc = ldg; g.out_mode = 0; g.act = 4; g.row_exp2_offset = off + c0; g.bias = bias;
-      g.m_limit_dev = n_valid; g.m_limit_base = c0;
-      if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
-      if (bias) {
-        ce_bias_colsum_kernel<<<(n_items + 255) / 256, 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(G), ldg, rows, c0,
-                                                                         n_valid, n_items, d_bias, it != 0);
-        RP_LAUNCH_CHECK();
-      }
-      // dH[c0:c0+rows] = G . E - E[y] / T_v   (split-K partials, reduced together with the label term)
-      int live = hint - c0;
-      live = live < 128 ? 128 : (live > rows ? rows : live);
-      int split = (2 * sm_count()) / (((live + 127) / 128) * (d / 128));
-      split = split < 1 ? 1 : (split > kWideSplitK ? kWideSplitK : split);
-      memset(&g, 0, sizeof(g));
-      g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = split;
-      g.A = G; g.a_rows = rows; g.a_cols = n_items; g.lda = ldg; g.a_mn = 0;
-      g.B = table; g.b_rows = n_items; g.b_cols = d; g.ldb = d; g.b_mn = 1;
-      g.M = rows; g.N = d; g.K = n_items;
-      g.C = part; g.ldc = d; g.out_mode = 3; g.c_split_stride = part_stride;
-      g.m_limit_dev = n_valid; g.m_limit_base = c0;
-      if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
-      ce_dh_reduce_kernel<<<sm_count() * 4, 256, 0, stream>>>(part, split, part_stride, rows, c0,
-                                                               reinterpret_cast<__nv_bfloat16*>(d_hc),
-                                                               reinterpret_cast<const __nv_bfloat16*>(table), labels, loss_inv,
-                                                               n_valid, d, nullptr);
-      RP_LAUNCH_CHECK();
-      // dE (+)= G^T . hc[c0:c0+rows]
-      memset(&g, 0, sizeof(g));
-      g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
-      g.A = G; g.a_rows = rows; g.a_cols = n_items; g.lda = ldg; g.a_mn = 1;
-      g.B = reinterpret_cast<const __nv_bfloat16*>(hc) + (size_t)c0 * d; g.b_rows = rows; g.b_cols = d; g.ldb = d; g.b_mn = 1;
-      g.M = n_items; g.N = d; g.K = rows;
-      g.C = d_table; g.ldc = d; g.out_mode = it == 0 ? 2 : 4;
-      g.k_limit_dev = n_valid; g.k_limit_base = c0;
-      if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
-    }
+    if ((rc = wide_bwd(4, off, nullptr, hc, table, bias, labels, n_valid, capacity, n_items, d, loss_inv, d_hc, d_table, d_bias,
+                       n_valid_hint, workspace, stream)) != RP_OK)
+      return rc;
   } else {
     if (!fused && (rc = bce_rows_pass(hc, table, bias, labels, n_valid, capacity, n_items, d, nullptr, d_hc, n_valid_hint, ws,
                                       stream)) != RP_OK)

@@ -1,8 +1,9 @@
 // rp_gemm_desc.h - flat C view of the GEMM parameter block shared by the C-ABI entry point (rp_gemm.cu) and the kernels
-// host code that sequences GEMMs internally (rp_ce_head.cu).  Field-for-field the public `rp_gemm_desc` of
+// host code that sequences GEMMs internally (the CE, sampled and SCE heads).  Field-for-field the public `rp_gemm_desc` of
 // include/rp_b200.h (tests/test_api_cpu.py checks the ctypes mirror against the header).
 #pragma once
 #include <stdint.h>
+#include <string.h>
 
 struct rp_gemm_desc {
   const void* A; long long a_rows, a_cols, lda; int a_mn;
@@ -22,5 +23,13 @@ struct rp_gemm_desc {
   const int32_t* m_limit_dev; int m_limit_base;
   const int32_t* k_limit_dev; int k_limit_base;
 };
+
+// a plain single GEMM: every field zero except batch = inner = 1, alpha = 1, split_k = 1
+inline rp_gemm_desc rp_gemm_default() {
+  rp_gemm_desc g;
+  memset(&g, 0, sizeof(g));
+  g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
+  return g;
+}
 
 extern "C" int rp_gemm(const rp_gemm_desc* g, void* stream);

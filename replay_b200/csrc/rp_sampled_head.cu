@@ -350,9 +350,7 @@ RP_API int rp_sampled_head_fwd(const rp_sampled_desc* s, void* stream_) {
   if (a.neg_mode == 0) {
     sampled_gather_neg_kernel<<<(a.N + 7) / 8, 256, 0, stream>>>(a);
     RP_LAUNCH_CHECK();
-    rp_gemm_desc g;
-    memset(&g, 0, sizeof(g));
-    g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
+    rp_gemm_desc g = rp_gemm_default();
     g.A = a.hc; g.a_rows = a.capacity; g.a_cols = a.d; g.lda = a.d;
     g.B = a.e_neg; g.b_rows = a.N; g.b_cols = a.d; g.ldb = a.d;
     g.M = a.capacity; g.N = a.N; g.K = a.d;
@@ -376,10 +374,8 @@ RP_API int rp_sampled_head_bwd(const rp_sampled_desc* s, void* d_hc, float* d_ta
   if (!d_hc || !d_table) return RP_EINVAL;
   const int blocks = sm_count() * 4;
   if (a.neg_mode == 0) {
-    rp_gemm_desc g;
     // dH = dz . E_neg
-    memset(&g, 0, sizeof(g));
-    g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
+    rp_gemm_desc g = rp_gemm_default();
     g.A = a.dz16; g.a_rows = (a.capacity + 127) / 128 * 128; g.a_cols = a.N; g.lda = a.ldn;
     g.B = a.e_neg; g.b_rows = a.N; g.b_cols = a.d; g.ldb = a.d; g.b_mn = 1;
     g.M = a.capacity; g.N = a.d; g.K = a.N;
@@ -387,8 +383,7 @@ RP_API int rp_sampled_head_bwd(const rp_sampled_desc* s, void* d_hc, float* d_ta
     g.m_limit_dev = a.n_valid;
     if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
     // dE_neg = dz^T . hc
-    memset(&g, 0, sizeof(g));
-    g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
+    g = rp_gemm_default();
     g.A = a.dz16; g.a_rows = (a.capacity + 127) / 128 * 128; g.a_cols = a.N; g.lda = a.ldn; g.a_mn = 1;
     g.B = a.hc; g.b_rows = a.capacity; g.b_cols = a.d; g.ldb = a.d; g.b_mn = 1;
     g.M = a.N; g.N = a.d; g.K = a.capacity;

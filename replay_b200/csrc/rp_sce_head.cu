@@ -508,16 +508,9 @@ static int sce_args(const rp_sce_desc* s, SceArgs* a) {
     default: { constexpr int D = 512; CALL; } break;   \
   }
 
-static rp_gemm_desc gemm_base() {
-  rp_gemm_desc g;
-  memset(&g, 0, sizeof(g));
-  g.batch = 1; g.inner = 1; g.alpha = 1.f; g.split_k = 1;
-  return g;
-}
-
 // S[b] = X_b . Y_b^T for the buckets [b0, b0 + nc) of a chunk (fp32, pitch bsyp)
 static int sce_scores(const SceArgs& a, int b0, int nc, void* stream) {
-  rp_gemm_desc g = gemm_base();
+  rp_gemm_desc g = rp_gemm_default();
   g.A = a.xb; g.a_rows = (long long)a.nb * a.bsxp; g.a_cols = a.d; g.lda = a.d;
   g.B = a.yb; g.b_rows = (long long)a.nb * a.bsyp; g.b_cols = a.d; g.ldb = a.d;
   g.M = a.bsx; g.N = a.bsy; g.K = a.d; g.batch = nc;
@@ -556,7 +549,7 @@ RP_API int rp_sce_head_fwd(const rp_sce_desc* s, int stages, void* stream_) {
     sce_bucket_kernel<<<a.mix ? blocks : 1, 256, 0, stream>>>(a, scale);
     RP_LAUNCH_CHECK();
     if (a.mix) {   // buckets = omega^T . hc over the rows of the batch (k_limit: *n_rows, omega is zero beyond)
-      rp_gemm_desc g = gemm_base();
+      rp_gemm_desc g = rp_gemm_default();
       g.A = a.omega; g.a_rows = (a.cap + 63) / 64 * 64; g.a_cols = a.nbp; g.lda = a.nbp; g.a_mn = 1;
       g.B = a.hc; g.b_rows = a.cap; g.b_cols = a.d; g.ldb = a.d; g.b_mn = 1;
       g.M = a.nb; g.N = a.d; g.K = a.cap;
@@ -612,7 +605,7 @@ RP_API int rp_sce_head_bwd(const rp_sce_desc* s, void* d_hc, void* stream_) {
     sce_row_bwd_kernel<<<blocks, 256, 0, stream>>>(a, b0, nc);
     RP_LAUNCH_CHECK();
     // dX_b = G_b . Y_b  (G bf16 in place of S: pitch 2 * bsyp elements; Y_b read MN-major)
-    rp_gemm_desc g = gemm_base();
+    rp_gemm_desc g = rp_gemm_default();
     g.A = a.S; g.a_rows = (long long)a.chunk * a.bsxp; g.a_cols = a.bsyp; g.lda = 2ll * a.bsyp;
     g.B = a.yb; g.b_rows = (long long)a.nb * a.bsyp; g.b_cols = a.d; g.ldb = a.d; g.b_mn = 1;
     g.M = a.bsx; g.N = a.d; g.K = a.bsyp; g.batch = nc;

@@ -843,21 +843,35 @@ class SasRecEngine:
         if self.sampled is not None:
             check(self.lib.rp_sampled_head_fwd(ctypes.byref(self._sampled_desc()), self._stream()), "rp_sampled_head_fwd")
             return self.ce.loss
+        return self._catalog_head_fwd(self.params16["item_emb"][: cfg.n_items])
+
+    def _catalog_head_fwd(self, table, bias=None):
+        """Full-catalog CE (or its per-row variants) / BCE head over the gathered rows self.hc -> loss (device fp32 [2])."""
         from .ops import bce_head_fwd, ce_head_fwd
 
         self.lib.count += 2
+        d_hc = self.s["dhc"] if self.fused_ce else None
         if self.bce:
-            return bce_head_fwd(self.ce, self.hc, self.params16["item_emb"][: cfg.n_items], self.labels_c, self.n_valid,
-                                d_hc=self.s["dhc"] if self.fused_ce else None, n_valid_hint=self.n_valid_hint)
+            return bce_head_fwd(self.ce, self.hc, table, self.labels_c, self.n_valid, bias=bias, d_hc=d_hc,
+                                n_valid_hint=self.n_valid_hint)
         row = self.ce_row
         roww = None
         if row is not None and row["weighted"]:   # weights of the valid targets in the head's compacted order
             torch.index_select(self.in_roww, 0, self.valid_idx, out=self.roww_c)
             roww = self.roww_c
-        return ce_head_fwd(self.ce, self.hc, self.params16["item_emb"][: cfg.n_items], self.labels_c, self.n_valid,
-                           d_hc=self.s["dhc"] if self.fused_ce else None, n_valid_hint=self.n_valid_hint, row_weight=roww,
-                           loss_kind=row["kind"] if row else 0, log_eps=row["log_eps"] if row else 1e-6,
-                           clamp=row["clamp"] if row else 100.0)
+        return ce_head_fwd(self.ce, self.hc, table, self.labels_c, self.n_valid, bias=bias, d_hc=d_hc,
+                           n_valid_hint=self.n_valid_hint, row_weight=roww, loss_kind=row["kind"] if row else 0,
+                           log_eps=row["log_eps"] if row else 1e-6, clamp=row["clamp"] if row else 100.0)
+
+    def _catalog_head_bwd(self, table, d_table, bias=None, d_bias=None, n_valid_hint=None):
+        """Backward of _catalog_head_fwd: d_hc into self.s["dhc"] (unless the forward already wrote it), d_table and d_bias
+        (iff bias) overwritten.  ``n_valid_hint`` None: self.n_valid_hint."""
+        from .ops import bce_head_bwd, ce_head_bwd
+
+        head_bwd = bce_head_bwd if self.bce else ce_head_bwd
+        head_bwd(self.ce, self.hc, table, self.labels_c, self.n_valid, self.s["dhc"], d_table, bias=bias, d_bias=d_bias,
+                 n_valid_hint=self.n_valid_hint if n_valid_hint is None else n_valid_hint)
+        self.lib.count += 3
 
     # ------------------------------------------------------------------------------------------------ backward
     def backward(self):
@@ -868,13 +882,7 @@ class SasRecEngine:
         drop = cfg.dropout
         ks = 1.0 / (1.0 - drop) if drop > 0 else 1.0
         st = self._stream
-        from .ops import bce_head_bwd, ce_head_bwd
-
-        if self.bce:
-            bce_head_bwd(self.ce, self.hc, p16["item_emb"][: cfg.n_items], self.labels_c, self.n_valid, s["dhc"], G["item_emb"],
-                         n_valid_hint=self.n_valid_hint)
-            self.lib.count += 3
-        elif self.sce is not None:
+        if self.sce is not None:
             G["item_emb"].zero_()  # the reference's SCE scores a detached copy of the table: only the input gather reaches it
             check(self.lib.rp_sce_head_bwd(ctypes.byref(self.sce["desc"]), s["dhc"].data_ptr(), st()), "rp_sce_head_bwd")
         elif self.sampled is not None:
@@ -882,9 +890,7 @@ class SasRecEngine:
             check(self.lib.rp_sampled_head_bwd(ctypes.byref(self._sampled_desc()), s["dhc"].data_ptr(), G["item_emb"].data_ptr(),
                                                st()), "rp_sampled_head_bwd")
         else:
-            ce_head_bwd(self.ce, self.hc, p16["item_emb"][: cfg.n_items], self.labels_c, self.n_valid, s["dhc"], G["item_emb"],
-                        n_valid_hint=self.n_valid_hint)
-            self.lib.count += 3
+            self._catalog_head_bwd(p16["item_emb"][: cfg.n_items], G["item_emb"])
         dx = s["dxa"]
         dx.zero_()
         if self.sce is not None:

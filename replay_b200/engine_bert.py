@@ -139,31 +139,24 @@ class Bert4RecEngine(SasRecEngine):
         self.sampled, self.bce = None, kind == "bce"
 
     def forward_train(self):
-        from .ops import bce_head_fwd, ce_head_fwd
-
         self._prepare(True)
         self._body_forward(True)
         check(self.lib.rp_gather_rows(self.x[-1].data_ptr(), self.valid_idx.data_ptr(), self.T, self.n_valid.data_ptr(),
                                       self.cfg.dp, self.hc.data_ptr(), 0, self._stream()), "rp_gather_rows")
         W16, bias = self._head()
-        self.lib.count += 2
-        head_fwd = bce_head_fwd if self.bce else ce_head_fwd
-        return head_fwd(self.ce, self.hc, W16, self.labels_c, self.n_valid, bias=bias,
-                        d_hc=self.s["dhc"] if self.fused_ce else None, n_valid_hint=self.n_valid_hint)
+        return self._catalog_head_fwd(W16, bias)
 
     # ------------------------------------------------------------------------------------------------ backward
     def backward(self):
-        from .ops import bce_head_bwd, ce_head_bwd
-
         cfg, T, d, F, L = self.cfg, self.T, self.cfg.dp, self.cfg.ffn_p, self.L
         p16, prm, G, s = self.params16, self.params, self.grads, self.s
         drop = cfg.dropout
         st, rng = self._stream, self.rng_counter.data_ptr()
         W16, bias = self._head()
         dW = G["item_emb"] if cfg.tying else G["head_w"]
-        head_bwd = bce_head_bwd if self.bce else ce_head_bwd
-        head_bwd(self.ce, self.hc, W16, self.labels_c, self.n_valid, s["dhc"], dW, bias=bias, d_bias=G["head_b"])
-        self.lib.count += 3
+        # balanced over the whole capacity: the hint picks the split counts, and so the fp32 summation order, of the d = 512
+        # and un-fused BCE gradient passes
+        self._catalog_head_bwd(W16, dW, bias, G["head_b"], n_valid_hint=0)
         dx = s["dxa"]
         dx.zero_()
         check(self.lib.rp_gather_rows(s["dhc"].data_ptr(), self.valid_idx.data_ptr(), T, self.n_valid.data_ptr(), d,

@@ -96,6 +96,18 @@ class CEHeadState:
         self.lse = torch.zeros(capacity, device=device, dtype=torch.float32)
         cap128 = (capacity + 127) // 128 * 128
         self.cvec = torch.full((cap128,), float("-inf"), device=device, dtype=torch.float32)
+        self.fused = False   # did the last forward run the fused forward + dH pass (the backward must be told)
+
+
+def _need_head(hc, table, labels, n_valid, *optional):
+    """Input checks shared by the full-catalog CE / BCE wrappers; ``optional``: (tensor or None, dtype, name), checked when given."""
+    _need(hc, torch.bfloat16, "hc")
+    _need(table, torch.bfloat16, "table")
+    _need(labels, torch.int32, "labels")
+    _need(n_valid, torch.int32, "n_valid")
+    for t, dtype, name in optional:
+        if t is not None:
+            _need(t, dtype, name)
 
 
 def ce_head_fwd(st: CEHeadState, hc, table, labels, n_valid, bias=None, d_hc=None, n_valid_hint: int = 0, row_weight=None,
@@ -104,15 +116,8 @@ def ce_head_fwd(st: CEHeadState, hc, table, labels, n_valid, bias=None, d_hc=Non
     With ``d_hc`` (bf16 [capacity,d]) the fused forward+dH pass runs and d_hc is final after this call.
     ``row_weight`` fp32 [capacity] (compacted order) / ``loss_kind`` 1 = LogInCE: the per-row variants (rp_ce_head_fwd_w).
     Returns st.loss (fp32 [2]: mean loss, 1/n_valid) - a view that the next call overwrites."""
-    _need(hc, torch.bfloat16, "hc")
-    _need(table, torch.bfloat16, "table")
-    _need(labels, torch.int32, "labels")
-    _need(n_valid, torch.int32, "n_valid")
-    if d_hc is not None:
-        _need(d_hc, torch.bfloat16, "d_hc")
+    _need_head(hc, table, labels, n_valid, (d_hc, torch.bfloat16, "d_hc"), (row_weight, torch.float32, "row_weight"))
     st.fused = d_hc is not None and st.d <= 256
-    if row_weight is not None:
-        _need(row_weight, torch.float32, "row_weight")
     check(lib().rp_ce_head_fwd_w(_ptr(hc), _ptr(table), _ptr(bias), _ptr(labels), _ptr(n_valid), st.capacity, st.n_items, st.d,
                                  _ptr(st.loss), _ptr(st.lse), _ptr(st.cvec), _ptr(d_hc), int(n_valid_hint), _ptr(row_weight),
                                  int(loss_kind), float(log_eps), float(clamp), _ptr(st.ws), st.ws_bytes, _stream()),
@@ -129,10 +134,9 @@ def ce_head_fused_taken(st: CEHeadState) -> bool:
 
 def ce_head_bwd(st: CEHeadState, hc, table, labels, n_valid, d_hc, d_table, bias=None, d_bias=None, n_valid_hint: int = 0):
     """d_hc bf16 [capacity,d] (computed here unless the forward ran fused), d_table fp32 [>=I, d] (rows < I overwritten)."""
-    _need(d_hc, torch.bfloat16, "d_hc")
-    _need(d_table, torch.float32, "d_table")
+    _need_head(hc, table, labels, n_valid, (d_hc, torch.bfloat16, "d_hc"), (d_table, torch.float32, "d_table"))
     check(lib().rp_ce_head_bwd(_ptr(hc), _ptr(table), _ptr(bias), _ptr(labels), _ptr(n_valid), st.capacity, st.n_items, st.d,
-                               _ptr(st.loss), _ptr(st.cvec), _ptr(d_hc), _ptr(d_table), _ptr(d_bias), int(getattr(st, "fused", False)),
+                               _ptr(st.loss), _ptr(st.cvec), _ptr(d_hc), _ptr(d_table), _ptr(d_bias), int(st.fused),
                                int(n_valid_hint), _ptr(st.ws), st.ws_bytes, _stream()), "rp_ce_head_bwd")
 
 
@@ -140,12 +144,7 @@ def bce_head_fwd(st: CEHeadState, hc, table, labels, n_valid, bias=None, d_hc=No
     """Full-catalog BCE (rp_bce_head_fwd) over the buffers of ``st``: loss = sum over the valid targets of
     [sum_i softplus(logit_i) - logit_y] / n_valid.  Arguments as ce_head_fwd; with ``d_hc`` (d <= 256) the fused
     forward + dH pass runs.  Returns st.loss (fp32 [2]: loss, 1/n_valid)."""
-    _need(hc, torch.bfloat16, "hc")
-    _need(table, torch.bfloat16, "table")
-    _need(labels, torch.int32, "labels")
-    _need(n_valid, torch.int32, "n_valid")
-    if d_hc is not None:
-        _need(d_hc, torch.bfloat16, "d_hc")
+    _need_head(hc, table, labels, n_valid, (d_hc, torch.bfloat16, "d_hc"))
     st.fused = d_hc is not None and st.d <= 256
     check(lib().rp_bce_head_fwd(_ptr(hc), _ptr(table), _ptr(bias), _ptr(labels), _ptr(n_valid), st.capacity, st.n_items, st.d,
                                 _ptr(st.loss), _ptr(d_hc), int(n_valid_hint), _ptr(st.ws), st.ws_bytes, _stream()),
@@ -156,10 +155,9 @@ def bce_head_fwd(st: CEHeadState, hc, table, labels, n_valid, bias=None, d_hc=No
 def bce_head_bwd(st: CEHeadState, hc, table, labels, n_valid, d_hc, d_table, bias=None, d_bias=None, n_valid_hint: int = 0):
     """Backward of bce_head_fwd: d_hc bf16 [capacity,d] (computed here unless the forward ran fused), d_table fp32
     [>=I, d] and d_bias fp32 (iff bias) overwritten."""
-    _need(d_hc, torch.bfloat16, "d_hc")
-    _need(d_table, torch.float32, "d_table")
+    _need_head(hc, table, labels, n_valid, (d_hc, torch.bfloat16, "d_hc"), (d_table, torch.float32, "d_table"))
     check(lib().rp_bce_head_bwd(_ptr(hc), _ptr(table), _ptr(bias), _ptr(labels), _ptr(n_valid), st.capacity, st.n_items, st.d,
-                                _ptr(st.loss), _ptr(d_hc), _ptr(d_table), _ptr(d_bias), int(getattr(st, "fused", False)),
+                                _ptr(st.loss), _ptr(d_hc), _ptr(d_table), _ptr(d_bias), int(st.fused),
                                 int(n_valid_hint), _ptr(st.ws), st.ws_bytes, _stream()), "rp_bce_head_bwd")
 
 

@@ -4,10 +4,13 @@
     python tools/ce_head_dump.py --compare A.pt B.pt # "identical", or the first differing tensor
 
 Labels are unique (a permutation of the catalog), so the dE pass's one-hot scatter has no order-dependent fp32 atomics and
-two builds that run the same floating-point operations in the same order must agree exactly.  Cases: d = 64 / 128 / 256,
-with and without bias; the fused pass with one column split ("P1": as many row tiles as SMs) and with several ("Pn": one
-row tile); the two-pass path (no d_hc in the forward); the fused pass behind the two-pass forward (large logits fail the
-bound); and the BCE head's fused token pass and dE pass (P1 and Pn).
+two builds that run the same floating-point operations in the same order must agree exactly.  Cases, each with and
+without bias:
+- d = 64 / 128 / 256: the fused pass with one column split ("P1": as many row tiles as SMs) and with several ("Pn": one
+  row tile); the two-pass path (no d_hc in the forward); the fused pass behind the two-pass forward (large logits fail the
+  bound) at both shapes; the BCE head's fused token pass (P1 and Pn) and its un-fused forward; and the per-row CE
+  variants (row_weight, and loss_kind 1 = LogInCE) on the fused, two-pass and behind paths.
+- d = 512: the materialised-G backward of CE, its per-row variants and BCE, in one G chunk and in 128-row chunks.
 """
 import argparse
 import os
@@ -25,24 +28,27 @@ def _inputs(T, n_valid, I, d, bias, scale_h, scale_e, seed):
     b = (torch.randn(I, generator=g) * 0.5).float().cuda() if bias else None
     labels = torch.randperm(I, generator=g)[:T].int()
     nv = torch.tensor([n_valid], dtype=torch.int32, device="cuda")
-    return hc.cuda(), table.cuda(), b, labels.cuda(), nv
+    row_weight = (torch.rand(T, generator=g) * 2).cuda()
+    return hc.cuda(), table.cuda(), b, labels.cuda(), nv, row_weight
 
 
-def _run(ops, loss_kind, path, T, n_valid, I, d, bias, seed):
+def _run(ops, kind, path, T, n_valid, I, d, bias, seed):
+    """kind: "ce", "ce_w" (row_weight), "login" (LogInCE) or "bce"; path: "fused", "twopass" (no d_hc) or "behind"."""
     scale_h, scale_e = (2.0, 1.0) if path == "behind" else (0.5, 0.3)
-    hc, table, b, labels, nv = _inputs(T, n_valid, I, d, bias, scale_h, scale_e, seed)
+    hc, table, b, labels, nv, roww = _inputs(T, n_valid, I, d, bias, scale_h, scale_e, seed)
     st = ops.CEHeadState(T, I, d, "cuda")
     d_hc = torch.zeros(T, d, device="cuda", dtype=torch.bfloat16)
     d_tab = torch.zeros(I + 1, d, device="cuda")
     d_b = torch.zeros(I + 1, device="cuda") if bias else None
-    fwd, bwd = (ops.ce_head_fwd, ops.ce_head_bwd) if loss_kind == "ce" else (ops.bce_head_fwd, ops.bce_head_bwd)
-    loss = fwd(st, hc, table, labels, nv, bias=b, d_hc=None if path == "twopass" else d_hc, n_valid_hint=T).clone()
-    if loss_kind == "ce" and path != "twopass":
+    fwd, bwd = (ops.bce_head_fwd, ops.bce_head_bwd) if kind == "bce" else (ops.ce_head_fwd, ops.ce_head_bwd)
+    row = {"ce_w": dict(row_weight=roww), "login": dict(loss_kind=1, log_eps=1e-6, clamp=10.0)}.get(kind, {})
+    loss = fwd(st, hc, table, labels, nv, bias=b, d_hc=None if path == "twopass" else d_hc, n_valid_hint=T, **row).clone()
+    if kind != "bce" and path != "twopass" and d <= 256:
         assert ops.ce_head_fused_taken(st) == (path != "behind"), path
     bwd(st, hc, table, labels, nv, d_hc, d_tab, bias=b, d_bias=d_b)
     torch.cuda.synchronize()
     out = dict(loss=loss, d_hc=d_hc, d_table=d_tab)
-    if loss_kind == "ce":
+    if kind != "bce":
         out.update(lse=st.lse, cvec=st.cvec)
     if bias:
         out["d_bias"] = d_b
@@ -52,16 +58,24 @@ def _run(ops, loss_kind, path, T, n_valid, I, d, bias, seed):
 def dump(path):
     from replay_b200 import ops
     sms = torch.cuda.get_device_properties(0).multi_processor_count
+    shapes = {"P1": (sms * 128, sms * 128 - 37, sms * 128 + 3011), "Pn": (1024, 999, 20011)}
+    narrow = [("ce", "fused", "P1"), ("ce", "fused", "Pn"), ("ce", "twopass", "Pn"), ("ce", "behind", "Pn"), ("ce", "behind", "P1"),
+              ("bce", "fused", "P1"), ("bce", "fused", "Pn"), ("bce", "twopass", "Pn")]
+    narrow += [(k, p, s) for k in ("ce_w", "login") for p, s in (("fused", "P1"), ("fused", "Pn"), ("twopass", "Pn"),
+                                                                 ("behind", "P1"), ("behind", "Pn"))]
+    wide = [(k, "twopass", "Pn") for k in ("ce", "ce_w", "login", "bce")]
     res = {}
-    for d in (64, 128, 256):
-        for bias in (False, True):
-            shapes = {"P1": (sms * 128, sms * 128 - 37, sms * 128 + 3011), "Pn": (1024, 999, 20011)}
-            runs = [("ce", p, shapes[p]) for p in ("P1", "Pn")] + [("ce", "twopass", shapes["Pn"]), ("ce", "behind", shapes["Pn"])]
-            runs += [("bce", p, shapes[p]) for p in ("P1", "Pn")]
-            for i, (kind, p, (T, nv, I)) in enumerate(runs):
-                case = f"{kind}_{p}_d{d}_{'bias' if bias else 'nobias'}"
-                for k, v in _run(ops, kind, p, T, nv, I, d, bias, seed=1000 * d + 10 * i + bias).items():
-                    res[f"{case}/{k}"] = v
+    for d in (64, 128, 256, 512):
+        for chunks in (("one",) if d <= 256 else ("one", "several")):
+            if chunks == "several":
+                os.environ["RP_CE_WIDE_G_BYTES"] = "1"   # the smallest budget: 128-row G chunks (read on every call)
+            for bias in (False, True):
+                for i, (kind, p, s) in enumerate(narrow if d <= 256 else wide):
+                    T, nv, I = shapes[s]
+                    case = f"{kind}_{p}_{s}_d{d}_{'bias' if bias else 'nobias'}" + (f"_{chunks}" if d > 256 else "")
+                    for k, v in _run(ops, kind, p, T, nv, I, d, bias, seed=1000 * d + 10 * i + bias).items():
+                        res[f"{case}/{k}"] = v
+            os.environ.pop("RP_CE_WIDE_G_BYTES", None)
     torch.save(res, path)
     print(f"{len(res)} tensors -> {path}")
 
