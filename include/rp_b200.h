@@ -485,6 +485,67 @@ int rp_selftest_mma_probe(int mode, int iters, int grid, long long* cycles_out, 
 int rp_selftest_tma_probe(const void* table, long long rows, int d, int box_rows, int tiles, int same_tile, int grid,
                           void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * DiffTransformer encoder (replay/nn/sequential/sasrec/diff_transformer.py, replay/nn/attention.py:67-157,
+ * replay/nn/ffn.py:60-99; arXiv 2410.05258).  Per head h of true width head_dim <= 64:
+ *   lambda_h = exp(sum_j lq1[h,j] lk1[h,j]) - exp(sum_j lq2[h,j] lk2[h,j]) + lambda_init   (fp32, read on the device)
+ *   A = softmax(Q1 K1^T s + M) - lambda_h softmax(Q2 K2^T s + M),  O = A V,  out = O / sqrt(mean(O^2) + eps) * rms_scale
+ *       * (1 - lambda_init)
+ * with M: key j visible to query i iff j <= i and (pad_mask[j] or j == i) - pad rows attend to themselves
+ * (replay/nn/mask.py:29-51; the encoder ignores padding_mask).  Column layout of one token row: the q / k array holds per
+ * head [q1 (64-wide slot) | q2 (64-wide slot)] at x_c0 + h*128; v / out / o_pre hold per head a v_slot-wide slot (64 for
+ * head_dim <= 32, 128 for head_dim <= 64) whose first 2*head_dim columns are real.  L <= 256.
+ * ------------------------------------------------------------------------------------------------------------- */
+typedef struct rp_diff_lambda {
+  const float* q1; const float* k1; const float* q2; const float* k2;   /* fp32 [H, head_dim] each */
+  int head_dim; float lambda_init;
+} rp_diff_lambda;
+typedef struct rp_diff_attn_desc {
+  const void* qk; long long ld_qk; int q_c0, k_c0;   /* Q and K columns may live in one array (packed projection) */
+  const void* v; long long ldv; int v_c0;
+  const uint8_t* pad_mask;                          /* [B*L], 1 = real item */
+  int B, H, L, head_dim, v_slot;
+  float scale;                                      /* 1/sqrt(head_dim) */
+  float eps;                                        /* per-head RMSNorm eps (1e-5) */
+  rp_diff_lambda lam;
+  const float* rms_scale;                           /* fp32 [v_slot], zero beyond 2*head_dim */
+  void* out; long long ldo;                         /* bf16 normalised output */
+  /* training saves (all NULL in eval): o_pre = O before the per-head RMSNorm (geometry of out); e1 / e2 bf16
+   * [B*H, Lp, Lp] = exp(s - rowmax) of either map (zero where masked; Lp = round_up(L, 64); rows >= L are not written,
+   * so the buffers are zero-initialised once); inv1 / inv2 fp32 [B*H, Lp] the reciprocal row sums */
+  void* o_pre; void* e1_save; void* e2_save; float* inv1; float* inv2;
+  float* o32_save; float* o2_save;                  /* fp32, geometry of out: O_pre and A2 . V (inputs of the lambda gradient) */
+} rp_diff_attn_desc;
+int rp_diff_attn_fwd(const rp_diff_attn_desc* a, void* stream);
+/* Row-wise backward between the batched rp_gemm calls, from the forward's saves and dA = dO_pre . V^T (bf16 [B*H, Lp, Lp]):
+ * dS1 = A1 (dA - sum A1 dA) s, dS2 = -lambda A2 (dA - r2) s, A = A1 - lambda A2 (the A operand of dV = A^T dO_pre; A may
+ * alias dA), dlam_part fp32 [B*H, Lp] = -r2 per row, with r2 = sum_j A2 dA = dO_pre . (A2 V), dO_pre recomputed in fp32
+ * from d_on (bf16, gradient of the normalised output), the forward's o32_save / o2_save and rms_scale (eps of the per-head
+ * norm); all of pitch ld_o with v_slot columns per head.  Columns >= L are not written. */
+int rp_diff_attn_softmax_bwd(const void* e1, const void* e2, const float* inv1, const float* inv2, const void* dA, void* dS1,
+                             void* dS2, void* A, float* dlam_part, int BH, int H, int L, float scale, const rp_diff_lambda* lam,
+                             const void* d_on, const float* o32, const float* o2, const float* rms_scale, float eps,
+                             long long ld_o, int v_slot, void* stream);
+/* dlambda_h = sum over sequences and rows of dlam_part (fixed order) chained into the lambda_* gradients (+=). */
+int rp_diff_lambda_bwd(const float* dlam_part, int B, int H, int L, const rp_diff_lambda* lam, float* gq1, float* gk1, float* gq2,
+                       float* gk2, void* stream);
+/* RMSNorm over groups of `group` columns (64 / 128 / 256; d a multiple of it, d <= 512): y = x * rstd * w[c % group] * alpha,
+ * rstd = 1/sqrt(sum_group x^2 / n_true + eps) - torch.nn.RMSNorm (group = d) and the per-head norm of the differential
+ * attention (group = v_slot, n_true = 2*head_dim, alpha = 1 - lambda_init).  Padded columns must be zero in x and w.
+ * With `gather` output row r reads input row gather[r] and only min(n_rows, *n_rows_dev) rows exist; the backward then
+ * writes dx to those input rows.  dw (fp32 [group]) += the weight gradient, reduced in a fixed order through the workspace
+ * (rp_rmsnorm_bwd_workspace bytes). */
+int rp_rmsnorm_fwd(const void* x, const float* w, float eps, float alpha, int n_rows, int d, int group, int n_true,
+                   const int32_t* n_rows_dev, const int32_t* gather, void* y, void* stream);
+size_t rp_rmsnorm_bwd_workspace(int group);
+int rp_rmsnorm_bwd(const void* dy, const void* x, const float* w, float eps, float alpha, int n_rows, int d, int group, int n_true,
+                   const int32_t* n_rows_dev, const int32_t* gather, void* dx, float* dw, void* workspace, size_t workspace_bytes,
+                   void* stream);
+/* SwiGLU gate: gl bf16 [n_rows, 2F] = [g | l] (pre-activations, biases applied) -> u = silu(g) * l bf16 [n_rows, F];
+ * backward dgl = [du * l * silu'(g) | du * silu(g)]. */
+int rp_swiglu_fwd(const void* gl, long long n_rows, int F, void* u, void* stream);
+int rp_swiglu_bwd(const void* du, const void* gl, long long n_rows, int F, void* dgl, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

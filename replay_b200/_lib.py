@@ -208,6 +208,41 @@ class AttnBwdDesc(ctypes.Structure):
     ]
 
 
-_EXTRA_SIGS: list = []
+class DiffLambda(ctypes.Structure):
+    """Mirror of ``struct rp_diff_lambda`` (include/rp_b200.h)."""
 
-__all__ = ["GemmDesc", "SceDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]
+    _fields_ = [("q1", c_void_p), ("k1", c_void_p), ("q2", c_void_p), ("k2", c_void_p), ("head_dim", c_int),
+                ("lambda_init", c_float)]
+
+
+class DiffAttnDesc(ctypes.Structure):
+    """Mirror of ``struct rp_diff_attn_desc`` (include/rp_b200.h)."""
+
+    _fields_ = [
+        ("qk", c_void_p), ("ld_qk", ctypes.c_longlong), ("q_c0", c_int), ("k_c0", c_int),
+        ("v", c_void_p), ("ldv", ctypes.c_longlong), ("v_c0", c_int),
+        ("pad_mask", c_void_p),
+        ("B", c_int), ("H", c_int), ("L", c_int), ("head_dim", c_int), ("v_slot", c_int),
+        ("scale", c_float), ("eps", c_float),
+        ("lam", DiffLambda),
+        ("rms_scale", c_void_p),
+        ("out", c_void_p), ("ldo", ctypes.c_longlong),
+        ("o_pre", c_void_p), ("e1_save", c_void_p), ("e2_save", c_void_p), ("inv1", c_void_p), ("inv2", c_void_p),
+        ("o32_save", c_void_p), ("o2_save", c_void_p),
+    ]
+
+
+_P, _LL = c_void_p, ctypes.c_longlong
+_EXTRA_SIGS: list = [
+    ("rp_diff_attn_fwd", c_int, [ctypes.POINTER(DiffAttnDesc), _P]),
+    ("rp_diff_attn_softmax_bwd", c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_float,
+                                         ctypes.POINTER(DiffLambda), _P, _P, _P, _P, c_float, _LL, c_int, _P]),
+    ("rp_diff_lambda_bwd", c_int, [_P, c_int, c_int, c_int, ctypes.POINTER(DiffLambda), _P, _P, _P, _P, _P]),
+    ("rp_rmsnorm_fwd", c_int, [_P, _P, c_float, c_float, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
+    ("rp_rmsnorm_bwd_workspace", c_size_t, [c_int]),
+    ("rp_rmsnorm_bwd", c_int, [_P, _P, _P, c_float, c_float, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_size_t, _P]),
+    ("rp_swiglu_fwd", c_int, [_P, _LL, c_int, _P, _P]),
+    ("rp_swiglu_bwd", c_int, [_P, _P, _LL, c_int, _P, _P]),
+]
+
+__all__ = ["GemmDesc", "DiffAttnDesc", "DiffLambda", "SceDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]

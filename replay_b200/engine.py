@@ -833,17 +833,27 @@ class SasRecEngine:
             # SCE reads the final hidden state of every position, pad rows included (the mix_x buckets sum over them)
             self._prepare(False)
             self._body_forward(True)
-            self._ln_fwd(self.x[-1], self.params["lnf_w"], self.params["lnf_b"], cfg.lnf_eps, self.hc, self.meanf, self.rstdf, T)
+            self._final_norm_fwd(self.x[-1], self.hc, T)
             check(self.lib.rp_sce_head_fwd(ctypes.byref(self.sce["desc"]), SCE_ALL, self._stream()), "rp_sce_head_fwd")
             return self.ce.loss
         self._prepare(True)
         self._body_forward(True)
-        self._ln_fwd(self.x[-1], self.params["lnf_w"], self.params["lnf_b"], cfg.lnf_eps, self.hc, self.meanf, self.rstdf, T,
-                     gather=self.valid_idx, n_rows_dev=self.n_valid)
+        self._final_norm_fwd(self.x[-1], self.hc, T, gather=self.valid_idx, n_rows_dev=self.n_valid)
         if self.sampled is not None:
             check(self.lib.rp_sampled_head_fwd(ctypes.byref(self._sampled_desc()), self._stream()), "rp_sampled_head_fwd")
             return self.ce.loss
         return self._catalog_head_fwd(self.params16["item_emb"][: cfg.n_items])
+
+    def _final_norm_fwd(self, x, out, n_rows, gather=None, n_rows_dev=None):
+        """The body's output normalization (LayerNorm lnf_w / lnf_b) of ``n_rows`` rows of ``x`` (or of the rows ``gather``
+        lists) into ``out``; its statistics land in meanf / rstdf for ``_final_norm_bwd``."""
+        self._ln_fwd(x, self.params["lnf_w"], self.params["lnf_b"], self.cfg.lnf_eps, out, self.meanf, self.rstdf, n_rows,
+                     gather=gather, n_rows_dev=n_rows_dev)
+
+    def _final_norm_bwd(self, dy, x, dx, n_rows, gather=None, n_rows_dev=None):
+        G = self.grads
+        self._ln_bwd(dy, x, self.params["lnf_w"], self.meanf, self.rstdf, dx, G["lnf_w"], G["lnf_b"], n_rows, gather=gather,
+                     n_rows_dev=n_rows_dev)
 
     def _catalog_head_fwd(self, table, bias=None):
         """Full-catalog CE (or its per-row variants) / BCE head over the gathered rows self.hc -> loss (device fp32 [2])."""
@@ -874,14 +884,9 @@ class SasRecEngine:
         self.lib.count += 3
 
     # ------------------------------------------------------------------------------------------------ backward
-    def backward(self):
-        cfg, T, d, L = self.cfg, self.T, self.cfg.dp, self.L
-        hdv = cfg.hd_valid
-        p16, prm, G, s = self.params16, self.params, self.grads, self.s
-        legacy = cfg.variant == "legacy"
-        drop = cfg.dropout
-        ks = 1.0 / (1.0 - drop) if drop > 0 else 1.0
-        st = self._stream
+    def _head_backward(self):
+        """Backward of the loss head and the output normalization: returns d(last block's output), bf16 [T, dp]."""
+        cfg, T, p16, G, s, st = self.cfg, self.T, self.params16, self.grads, self.s, self._stream
         if self.sce is not None:
             G["item_emb"].zero_()  # the reference's SCE scores a detached copy of the table: only the input gather reaches it
             check(self.lib.rp_sce_head_bwd(ctypes.byref(self.sce["desc"]), s["dhc"].data_ptr(), st()), "rp_sce_head_bwd")
@@ -894,10 +899,20 @@ class SasRecEngine:
         dx = s["dxa"]
         dx.zero_()
         if self.sce is not None:
-            self._ln_bwd(s["dhc"], self.x[-1], prm["lnf_w"], self.meanf, self.rstdf, dx, G["lnf_w"], G["lnf_b"], T)
+            self._final_norm_bwd(s["dhc"], self.x[-1], dx, T)
         else:
-            self._ln_bwd(s["dhc"], self.x[-1], prm["lnf_w"], self.meanf, self.rstdf, dx, G["lnf_w"], G["lnf_b"], T,
-                         gather=self.valid_idx, n_rows_dev=self.n_valid)
+            self._final_norm_bwd(s["dhc"], self.x[-1], dx, T, gather=self.valid_idx, n_rows_dev=self.n_valid)
+        return dx
+
+    def backward(self):
+        cfg, T, d, L = self.cfg, self.T, self.cfg.dp, self.L
+        hdv = cfg.hd_valid
+        p16, prm, G, s = self.params16, self.params, self.grads, self.s
+        legacy = cfg.variant == "legacy"
+        drop = cfg.dropout
+        ks = 1.0 / (1.0 - drop) if drop > 0 else 1.0
+        st = self._stream
+        dx = self._head_backward()
         other = s["dxb"]
         for i in reversed(range(cfg.n_blocks)):
             a, x = self.act[i], self.x[i]

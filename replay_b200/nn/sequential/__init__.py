@@ -1,1 +1,1 @@
-from .sasrec import SasRec  # noqa: F401
+from .sasrec import DiffTransformerLayer, PositionAwareAggregator, SasRec, SasRecBody, SasRecTransformerLayer  # noqa: F401

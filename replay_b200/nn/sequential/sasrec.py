@@ -4,6 +4,7 @@ Same construction (``from_params``), same ``forward`` signature and train / infe
 ``state_dict`` key names (SURVEY.md Appendix B); the computation is the fused CUDA path (``replay_b200.core``)."""
 from __future__ import annotations
 
+import math
 import warnings
 
 import torch
@@ -11,7 +12,142 @@ import torch
 from ...core import SasRecCore
 from ..loss import CE
 from ...engine import EncoderConfig
+from ...engine_diff import DiffConfig, DiffEngine
 from ...schema import item_feature_of
+from ..agg import SumAggregator
+from ..embedding import SequenceEmbedding
+from ..mask import DefaultAttentionMask
+
+_DIFF_LEAF = {"wq": "attn.W_q.weight", "wk": "attn.W_k.weight", "wv": "attn.W_v.weight", "wo": "attn.W_o.weight",
+              "lambda_q1": "attn.lambda_q1", "lambda_k1": "attn.lambda_k1", "lambda_q2": "attn.lambda_q2",
+              "lambda_k2": "attn.lambda_k2", "rms_scale": "attn.rms_scale", "attn_norm": "attn_norm.weight",
+              "ff_norm": "ff_norm.weight", "ff_wg": "ff.WG.weight", "ff_w1": "ff.W1.weight", "ff_bg": "ff.WG.bias",
+              "ff_b1": "ff.W1.bias", "ff_w2": "ff.W2.weight", "ff_b2": "ff.W2.bias"}
+
+
+def diff_key_map(cfg: DiffConfig, item_feature: str = "item_id") -> dict:
+    """engine parameter name -> key of the reference's ``SasRec(body=SasRecBody(..., encoder=DiffTransformerLayer(...)))``"""
+    m = {"item_emb": f"body.embedder.feature_embedders.{item_feature}.emb.weight",
+         "pos_emb": "body.embedding_aggregator.pe.weight", "lnf_w": "body.output_normalization.weight"}
+    if cfg.out_norm == "layernorm":
+        m["lnf_b"] = "body.output_normalization.bias"
+    for i in range(cfg.n_blocks):
+        m.update({f"b{i}.{k}": f"body.encoder.layers.{i}.{v}" for k, v in _DIFF_LEAF.items()})
+    return m
+
+
+class _DiffCore(SasRecCore):
+    """SasRecCore on the DiffTransformer engine.  ``state_dict`` also carries each block's ``attn.scaling`` buffer
+    (1/sqrt(head_dim)), which ``load_state_dict`` checks."""
+
+    def _key_map(self):
+        return diff_key_map(self.cfg, self.item_feature)
+
+    def _make_engine(self, batch, seq_len, with_grad):
+        return DiffEngine(self.cfg, batch, seq_len, self._device, seed=self._seed, with_grad=with_grad)
+
+    def _scaling(self) -> dict:
+        v = torch.tensor(1.0 / math.sqrt(self.cfg.head_dim), dtype=torch.float32)
+        return {f"body.encoder.layers.{i}.attn.scaling": v.clone() for i in range(self.cfg.n_blocks)}
+
+    def state_dict(self, *args, destination=None, prefix="", keep_vars=False):  # noqa: D102
+        out = super().state_dict(*args, destination=destination, prefix=prefix, keep_vars=keep_vars)
+        for k, v in self._scaling().items():
+            out[prefix + k] = v
+        return out
+
+    def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):  # noqa: D102
+        for k, v in self._scaling().items():
+            if k in state_dict and not torch.allclose(torch.as_tensor(state_dict[k]).float().cpu(), v):
+                raise ValueError(f"{k} = {float(state_dict[k])} does not match this model's 1/sqrt(head_dim) = {float(v)}")
+            if strict and k not in state_dict:
+                raise RuntimeError(f"missing keys in state_dict: [{k!r}] ...")
+        return super().load_state_dict(state_dict, strict=strict, assign=assign)
+
+
+class PositionAwareAggregator:
+    """replay/nn/sequential/sasrec/agg.py: item embedding * sqrt(d) + the last-L positional embedding, then dropout."""
+
+    def __init__(self, embedding_aggregator, max_sequence_length: int, dropout: float) -> None:
+        self.embedding_aggregator = embedding_aggregator
+        self.max_sequence_length = max_sequence_length
+        self.dropout = dropout
+
+
+class SasRecTransformerLayer:
+    """replay/nn/sequential/sasrec/transformer.py (config only): pre-LN blocks with a ReLU FFN."""
+
+    def __init__(self, embedding_dim: int, num_heads: int, num_blocks: int, dropout: float, activation: str = "gelu") -> None:
+        self.embedding_dim, self.num_heads, self.num_blocks = embedding_dim, num_heads, num_blocks
+        self.dropout, self.activation = dropout, activation
+
+
+class DiffTransformerLayer:
+    """replay/nn/sequential/sasrec/diff_transformer.py (config only): post-norm blocks of multi-head differential
+    attention and a SwiGLU FFN of width 2 * embedding_dim.  Head width <= 64, at most 256 padded columns (heads x 64)."""
+
+    def __init__(self, embedding_dim: int, num_heads: int, num_blocks: int) -> None:
+        self.embedding_dim, self.num_heads, self.num_blocks = embedding_dim, num_heads, num_blocks
+
+
+class SasRecBody:
+    """replay/nn/sequential/sasrec/model.py ``SasRecBody`` (config only): the parts are read when ``SasRec(body, loss)``
+    builds the engine.  ``output_normalization`` is a ``torch.nn.LayerNorm`` or ``torch.nn.RMSNorm`` of the model width."""
+
+    def __init__(self, embedder, embedding_aggregator, attn_mask_builder, encoder, output_normalization) -> None:
+        self.embedder = embedder
+        self.embedding_aggregator = embedding_aggregator
+        self.attn_mask_builder = attn_mask_builder
+        self.encoder = encoder
+        self.output_normalization = output_normalization
+
+    def build_core(self, device=None, seed: int = 0) -> SasRecCore:
+        """The engine configuration this body describes; ValueError for anything the CUDA path does not implement."""
+        emb, agg, mask, enc, norm = (self.embedder, self.embedding_aggregator, self.attn_mask_builder, self.encoder,
+                                     self.output_normalization)
+        if not isinstance(emb, SequenceEmbedding):
+            raise ValueError(f"embedder must be SequenceEmbedding, got {type(emb).__name__}")
+        schema = emb.schema
+        name, card, pad, feat_dim = item_feature_of(schema)
+        if pad != card:
+            raise ValueError("the item feature's padding_value must equal its cardinality (replay/data/nn/schema.py:89-90)")
+        skip = set(emb.excluded_features) | {schema.query_id_feature_name, schema.timestamp_feature_name}
+        others = [f for f, _ in schema.items() if f not in skip and f != name]
+        if others:
+            raise ValueError(f"side features {others} are not supported; exclude them from the SequenceEmbedding")
+        if not isinstance(agg, PositionAwareAggregator) or not isinstance(agg.embedding_aggregator, SumAggregator):
+            raise ValueError("embedding_aggregator must be PositionAwareAggregator(SumAggregator(...), ...)")
+        if not isinstance(mask, DefaultAttentionMask) or mask.reference_feature_name != name:
+            raise ValueError(f"attn_mask_builder must be DefaultAttentionMask on the item feature {name!r}")
+        if not isinstance(enc, (SasRecTransformerLayer, DiffTransformerLayer)):
+            raise ValueError(f"encoder must be SasRecTransformerLayer or DiffTransformerLayer, got {type(enc).__name__}")
+        d = enc.embedding_dim
+        if agg.embedding_aggregator.embedding_dim != d or (feat_dim is not None and feat_dim != d):
+            raise ValueError("the embedder, the aggregator and the encoder must share one embedding_dim")
+        if mask.num_heads != enc.num_heads:
+            raise ValueError("attn_mask_builder.num_heads must equal the encoder's num_heads")
+        if isinstance(norm, torch.nn.LayerNorm) and norm.elementwise_affine and norm.bias is not None:
+            out_norm = "layernorm"
+        elif isinstance(norm, torch.nn.RMSNorm) and norm.elementwise_affine:
+            out_norm = "rmsnorm"
+        else:
+            raise ValueError("output_normalization must be torch.nn.LayerNorm or torch.nn.RMSNorm with affine weights")
+        if tuple(norm.normalized_shape) != (d,):
+            raise ValueError(f"output_normalization must normalise {d} features")
+        eps = norm.eps
+        if isinstance(enc, SasRecTransformerLayer):
+            if enc.activation != "relu":
+                raise ValueError(f"SasRecTransformerLayer supports activation='relu' only, got {enc.activation!r}")
+            if out_norm != "layernorm":
+                raise ValueError("SasRecTransformerLayer supports a LayerNorm output normalization only")
+            if enc.dropout != agg.dropout:
+                raise ValueError("the aggregator and SasRecTransformerLayer must share one dropout")
+            cfg = EncoderConfig(n_items=card, d=d, n_heads=enc.num_heads, n_blocks=enc.num_blocks,
+                                max_len=agg.max_sequence_length, dropout=agg.dropout, variant="new", lnf_eps=eps)
+            return SasRecCore(cfg, item_feature=name, device=device, seed=seed)
+        cfg = DiffConfig(n_items=card, d=d, n_heads=enc.num_heads, n_blocks=enc.num_blocks, max_len=agg.max_sequence_length,
+                         dropout=agg.dropout, out_norm=out_norm, lnf_eps=eps)
+        return _DiffCore(cfg, item_feature=name, device=device, seed=seed)
 
 
 class _InferenceOutput(dict):
@@ -31,8 +167,10 @@ class _InferenceOutput(dict):
 
 
 class SasRec(torch.nn.Module):
-    def __init__(self, core: SasRecCore, loss=None):
+    def __init__(self, body, loss=None, device=None, seed: int = 0):
+        """``body``: a ``SasRecBody`` (the reference's constructor) or an already built ``SasRecCore``."""
         super().__init__()
+        core = body.build_core(device=device, seed=seed) if isinstance(body, SasRecBody) else body
         self.core = core
         self.loss = loss if loss is not None else CE(ignore_index=core.cfg.n_items)
 
