@@ -198,6 +198,10 @@ typedef struct rp_attn_desc {
   float* m_save;  /* optional fp32 [B*H, Lp]: row max in exp2 units, input of rp_attn_bwd */
   float scale;    /* softmax scale; 0 -> 1/sqrt(head_dim).  Padded head slots (true head_dim 32 / 48 / 50 inside a 64-wide
                      slot) pass 1/sqrt(true head_dim) */
+  /* Packed rows (causal, head_dim 64, L <= 256; both or neither, NULL = padded rows b*L + position): sequence b holds its
+   * positions seq_first[b] .. L-1 in rows seq_off[b] ... of q / k / v / out (rp_row_plan).  Masks and dropout stay keyed
+   * by position; inv_sum / m_save row i is position (seq_first[b] & ~63) + i. */
+  const int32_t* seq_first; const int32_t* seq_off;
 } rp_attn_desc;
 int rp_attn_fwd(const rp_attn_desc* a, void* stream);
 
@@ -222,6 +226,7 @@ typedef struct rp_attn_bwd_desc {
   void* dv; int ld_dv, dv_c0;
   float drop_p; unsigned long long seed, drop_off; const unsigned long long* seed_ptr;
   float scale;    /* as in rp_attn_desc */
+  const int32_t* seq_first; const int32_t* seq_off;   /* packed rows as in rp_attn_desc; dq / dk / dv rows likewise */
 } rp_attn_bwd_desc;
 int rp_attn_bwd(const rp_attn_bwd_desc* a, void* stream);
 
@@ -245,6 +250,14 @@ int rp_prepare_batch(const int64_t* ids, const uint8_t* pad_mask, const int64_t*
                      int pad_id, int n_items, int32_t* ids32, int32_t* valid_idx, int32_t* labels_c, int32_t* n_valid,
                      int32_t* scratch /* >= ceil(T/1024) ints, needed with targets */, void* stream);
 
+/* Row plan of a causal training batch (packed body): seq_first[b] = first position of sequence b whose pad_mask is set or
+ * that holds a valid target (L if none); the positions seq_first[b] .. L-1 of all sequences are packed back to back:
+ * seq_off[b] = first packed row, *n_rows = packed row count, row_tok[r] = token b*L + position of packed row r,
+ * valid_rows[k] = packed row of valid_idx[k] (k < *n_valid; valid_idx may be NULL).  All on the device. */
+int rp_row_plan(const uint8_t* pad_mask, const int64_t* labels, const uint8_t* target_mask, int B, int L, int n_items,
+                const int32_t* valid_idx, const int32_t* n_valid, int32_t* seq_first, int32_t* seq_off, int32_t* n_rows,
+                int32_t* row_tok, int32_t* valid_rows, void* stream);
+
 /* x[t] = table[ids[t]] * scale + pos[pos0 + t % L] -> dropout -> (zero pad rows)      nn/sequential/sasrec/agg.py:37-53,
  * models/nn/sequential/sasrec/model.py:346-357 ; and its backward (fp32 atomics into d_table, pad row frozen). */
 int rp_embed_fwd(const void* table, const float* pos, const int32_t* ids, const uint8_t* pad_mask, int T, int L, int d,
@@ -253,6 +266,16 @@ int rp_embed_fwd(const void* table, const float* pos, const int32_t* ids, const 
 int rp_embed_bwd(const void* dx, const int32_t* ids, const uint8_t* pad_mask, int B, int L, int d, int pad_id, int pos0,
                  float scale, int zero_pad_rows, float drop_p, unsigned long long seed, unsigned long long drop_off,
                  const unsigned long long* seed_ptr, float* d_table, float* d_pos, void* stream);
+/* The same on packed rows (rp_row_plan): row r < *n_rows_dev is token row_tok[r]; dropout keyed by the token.  T = capacity. */
+int rp_embed_fwd_rows(const void* table, const float* pos, const int32_t* ids, const uint8_t* pad_mask, const int32_t* row_tok,
+                      const int32_t* n_rows_dev, int T, int L, int d, int pos0, float scale, int zero_pad_rows, float drop_p,
+                      unsigned long long seed, unsigned long long drop_off, const unsigned long long* seed_ptr, void* out,
+                      void* stream);
+int rp_embed_bwd_rows(const void* dx, const int32_t* ids, const uint8_t* pad_mask, const int32_t* row_tok,
+                      const int32_t* n_rows_dev, const int32_t* seq_first, const int32_t* seq_off, int B, int L, int d,
+                      int pad_id, int pos0, float scale, int zero_pad_rows, float drop_p, unsigned long long seed,
+                      unsigned long long drop_off, const unsigned long long* seed_ptr, float* d_table, float* d_pos,
+                      void* stream);
 
 /* torch.nn.LayerNorm forward / backward (transformer.py:47-49,60-62 eps 1e-8; model.py:248 eps 1e-5).  With `gather`
  * output row r reads input row gather[r] and only *n_rows_dev rows exist (valid-target compaction); the backward then
@@ -313,6 +336,14 @@ int rp_post_attn_train(const void* o, const void* q_in, const void* wo, const fl
                        int d, float drop_p, unsigned long long seed, unsigned long long drop_off1, unsigned long long drop_off2,
                        const unsigned long long* seed_ptr, void* h_save, void* y_save, void* u_save, float* mean_out,
                        float* rstd_out, void* out, int hd_valid, void* stream);
+/* Packed rows: only the first *n_rows_dev of the T rows (T, the capacity, sizes the grid and the tensor maps); row r draws its
+ * dropout with the key of token row_tok[r] (rp_row_plan).  No row mask. */
+int rp_post_attn_train_rows(const void* o, const void* q_in, const void* wo, const float* bo, const float* ln_w, const float* ln_b,
+                            float eps, const void* w1, const float* b1, const void* w2, const float* b2, int T, int d, float drop_p,
+                            unsigned long long seed, unsigned long long drop_off1, unsigned long long drop_off2,
+                            const unsigned long long* seed_ptr, void* h_save, void* y_save, void* u_save, float* mean_out,
+                            float* rstd_out, void* out, int hd_valid, const int32_t* n_rows_dev, const int32_t* row_tok,
+                            void* stream);
 
 /* Backward of rp_post_attn_train in one pass over the tokens.  Given dz = d loss / d out:
  *   dzm = dz [* rowmask] ;  d_t = dropout2'(dzm) ;  du = (d_t W2) * [u != 0] / keep ;  dy = du W1 + dzm ;
@@ -325,6 +356,11 @@ int rp_post_attn_bwd(const void* dz, const void* u, const void* h, const float* 
                      const void* w2, const void* w1, const void* wo, const uint8_t* rowmask, int T, int d, float drop_p,
                      unsigned long long seed, unsigned long long drop_off2, const unsigned long long* seed_ptr, void* d_t, void* du,
                      void* dh, void* d_o, float* dln_w, float* dln_b, int hd_valid, void* stream);
+int rp_post_attn_bwd_rows(const void* dz, const void* u, const void* h, const float* mean, const float* rstd, const float* ln_w,
+                          const void* w2, const void* w1, const void* wo, int T, int d, float drop_p, unsigned long long seed,
+                          unsigned long long drop_off2, const unsigned long long* seed_ptr, void* d_t, void* du, void* dh,
+                          void* d_o, float* dln_w, float* dln_b, int hd_valid, const int32_t* n_rows_dev,
+                          const int32_t* row_tok, void* stream);
 
 /* Everything BEFORE the attention of one SASRec block in one pass over the tokens (training and inference):
  *   q_in = LayerNorm(x) ;  Q = q_in Wq^T + bq ;  [K | V] = x [Wk | Wv]^T + [bk | bv]      (K, V from the un-normalised x)
@@ -335,11 +371,17 @@ int rp_post_attn_bwd(const void* dz, const void* u, const void* h, const float* 
  *   replaces  replay/nn/sequential/sasrec/transformer.py:99-106 ; replay/models/nn/sequential/sasrec/model.py:434-435 */
 int rp_ln_qkv_fused(const void* x, const float* ln_w, const float* ln_b, float eps, const void* w_in, const float* b_in, int T,
                     int d, void* q_in, void* Q, void* KV, float* mean_out, float* rstd_out, int hd_valid, void* stream);
+int rp_ln_qkv_fused_rows(const void* x, const float* ln_w, const float* ln_b, float eps, const void* w_in, const float* b_in,
+                         int T, int d, void* q_in, void* Q, void* KV, float* mean_out, float* rstd_out, int hd_valid,
+                         const int32_t* n_rows_dev, void* stream);
 /* Its backward in one pass:  dq_in = dQ Wq + dh ;  t = LayerNorm-backward(dq_in; x, mean, rstd, ln_w) ;  dx = [dK | dV] Wkv + t.
  * dln_w / dln_b fp32 [d] are ACCUMULATED (one fp32 atomic per column and CTA).  dx may not alias an input; d in {64,128}. */
 int rp_pre_attn_bwd(const void* dQ, const void* dKV, const void* dh, const void* x, const float* mean, const float* rstd,
                     const float* ln_w, const void* w_in, int T, int d, void* dx, float* dln_w, float* dln_b, int hd_valid,
                     void* stream);
+int rp_pre_attn_bwd_rows(const void* dQ, const void* dKV, const void* dh, const void* x, const float* mean, const float* rstd,
+                         const float* ln_w, const void* w_in, int T, int d, void* dx, float* dln_w, float* dln_b, int hd_valid,
+                         const int32_t* n_rows_dev, void* stream);
 
 /* ALL weight and bias gradients of one transformer block in one launch (+ one deterministic reduction launch):
  *   dW_i[n_out_i, n_in_i] (+)= dY_i[T, n_out_i]^T . X_i[T, n_in_i] ;  db_i[n_out_i] (+)= column sums of dY_i      i < n_pairs <= 8
@@ -356,6 +398,9 @@ typedef struct rp_wgrad_pair {
 size_t rp_wgrad_group_workspace(const rp_wgrad_pair* pairs, int n_pairs);
 int rp_wgrad_group(const rp_wgrad_pair* pairs, int n_pairs, int T, int accumulate, void* workspace, size_t workspace_bytes,
                    void* stream);
+/* Packed rows: the contraction covers the first *n_rows_dev of the T rows (rows past it are never read as nonzero). */
+int rp_wgrad_group_rows(const rp_wgrad_pair* pairs, int n_pairs, int T, int accumulate, const int32_t* n_rows_dev,
+                        void* workspace, size_t workspace_bytes, void* stream);
 
 int rp_adam_step(float* p, float* g, float* m, float* v, void* shadow_bf16, long long n, const float* lr_dev,
                  int32_t* step_dev, float beta1, float beta2, float eps, float grad_scale, const uint8_t* frozen,

@@ -184,6 +184,7 @@ class AttnDesc(ctypes.Structure):
         ("drop_p", c_float), ("seed", ctypes.c_ulonglong), ("drop_off", ctypes.c_ulonglong), ("seed_ptr", c_void_p),
         ("m_save", c_void_p),
         ("scale", c_float),
+        ("seq_first", c_void_p), ("seq_off", c_void_p),   # packed rows (rp_row_plan); None = padded rows b * L + position
     ]
 
 
@@ -205,6 +206,7 @@ class AttnBwdDesc(ctypes.Structure):
         ("dv", c_void_p), ("ld_dv", c_int), ("dv_c0", c_int),
         ("drop_p", c_float), ("seed", ctypes.c_ulonglong), ("drop_off", ctypes.c_ulonglong), ("seed_ptr", c_void_p),
         ("scale", c_float),
+        ("seq_first", c_void_p), ("seq_off", c_void_p),   # as in AttnDesc
     ]
 
 
@@ -232,7 +234,7 @@ class DiffAttnDesc(ctypes.Structure):
     ]
 
 
-_P, _LL = c_void_p, ctypes.c_longlong
+_P, _LL, _U64 = c_void_p, ctypes.c_longlong, ctypes.c_ulonglong
 _EXTRA_SIGS: list = [
     ("rp_diff_attn_fwd", c_int, [ctypes.POINTER(DiffAttnDesc), _P]),
     ("rp_diff_attn_softmax_bwd", c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_float,
@@ -243,6 +245,18 @@ _EXTRA_SIGS: list = [
     ("rp_rmsnorm_bwd", c_int, [_P, _P, _P, c_float, c_float, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_size_t, _P]),
     ("rp_swiglu_fwd", c_int, [_P, _LL, c_int, _P, _P]),
     ("rp_swiglu_bwd", c_int, [_P, _P, _LL, c_int, _P, _P]),
+    ("rp_row_plan", c_int, [_P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P]),
+    ("rp_embed_fwd_rows", c_int, [_P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, c_int, c_float, _U64, _U64, _P,
+                                  _P, _P]),
+    ("rp_embed_bwd_rows", c_int, [_P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_float, _U64,
+                                  _U64, _P, _P, _P, _P]),
+    ("rp_ln_qkv_fused_rows", c_int, [_P, _P, _P, c_float, _P, _P, c_int, c_int, _P, _P, _P, _P, _P, c_int, _P, _P]),
+    ("rp_post_attn_train_rows", c_int, [_P, _P, _P, _P, _P, _P, c_float, _P, _P, _P, _P, c_int, c_int, c_float, _U64, _U64, _U64,
+                                        _P, _P, _P, _P, _P, _P, _P, c_int, _P, _P, _P]),
+    ("rp_post_attn_bwd_rows", c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_float, _U64, _U64, _P, _P, _P, _P, _P,
+                                      _P, _P, c_int, _P, _P, _P]),
+    ("rp_pre_attn_bwd_rows", c_int, [_P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P, c_int, _P, _P]),
+    ("rp_wgrad_group_rows", c_int, [ctypes.POINTER(WgradPair), c_int, c_int, c_int, _P, _P, c_size_t, _P]),
 ]
 
 __all__ = ["GemmDesc", "DiffAttnDesc", "DiffLambda", "SceDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]

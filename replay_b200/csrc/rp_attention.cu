@@ -27,6 +27,10 @@ struct AttnParams {
   float drop_p;
   unsigned long long seed, drop_off;
   const unsigned long long* seed_ptr;
+  // packed rows (training, head_dim 64, L <= 256): sequence b owns rows [seq_off[b], seq_off[b] + L - seq_first[b]) of q / k / v
+  // / out, its positions seq_first[b] .. L - 1; null = padded rows b * L + position
+  const int32_t* seq_first;
+  const int32_t* seq_off;
 };
 
 static constexpr float kLog2eA = 1.4426950408889634f;
@@ -69,6 +73,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int q0 = blockIdx.x * 128, h = blockIdx.y, b = blockIdx.z;
   const int bz = b * p.H + h;
   const int L = p.L;
+  // packed rows: the sequence's rows hold positions first .. L - 1 from row seq_off[b] on.  The CTA's window starts `lead`
+  // rows earlier, at the 64-aligned position `shift`, so that its 64-key chunks cover the same positions as in the padded
+  // layout (every row sums the same products in the same order); the lead rows belong to the sequence before and are
+  // masked as keys and never stored.  Local index = position - shift; masks and dropout keys use the position.
+  const bool packed = p.seq_first != nullptr;
+  const int first = packed ? p.seq_first[b] : 0;
+  const int lead = first & 63, shift = first - lead;
+  const int n = L - shift;
+  const int row0 = packed ? p.seq_off[b] - lead : b * L;
+  if (packed && q0 >= n) return;   // no live query in this tile: nothing reads its rows
   // Inference: a query tile whose rows are ALL padding (left-padded windows: the first tile of every user with at most L - 128
   // items) produces nothing anybody reads - the new path masks pad positions as keys and never queries them, the legacy
   // path zeroes pad rows after the block.  Such a CTA writes zeros and leaves before any load or MMA.  (Training keeps the
@@ -87,7 +101,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       return;
     }
   }
-  const int nk = p.causal ? min(L, q0 + 128) : L;  // keys that can be visible to this query tile
+  const int nk = p.causal ? min(n, q0 + 128) : n;  // keys that can be visible to this query tile
   const int nk32 = (nk + 31) & ~31;                // extent of the saved probability rows
   const int n_boxes = (nk32 + 127) / 128;
   const int n64 = (nk32 + 63) / 64;
@@ -97,7 +111,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     uint64_t* full = v_full + ch % kAfVStages;
     mbar_arrive_expect_tx(full, V_STAGE);
     for (int c = 0; c < HC; ++c)
-      tma_load_2d(sV + (ch % kAfVStages) * V_STAGE + c * 8192, &tmV, full, p.v_c0 + h * HD + c * 64, b * L + ch * 64);
+      tma_load_2d(sV + (ch % kAfVStages) * V_STAGE + c * 8192, &tmV, full, p.v_c0 + h * HD + c * 64, row0 + ch * 64);
   };
   if (threadIdx.x == 0) {
     mbar_init(&bar_load, 1);
@@ -107,7 +121,6 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         mbar_init(v_empty + s, kAfThreads);
       }
     fence_barrier_init();
-    const int row0 = b * L;
     mbar_arrive_expect_tx(&bar_load, HC * 128 * 128 + (STREAM_V ? 1 : 2) * HC * n_boxes * 128 * 128);
     for (int c = 0; c < HC; ++c) {
       tma_load_2d(sQ + c * 16384, &tmQ, &bar_load, p.q_c0 + h * HD + c * 64, row0 + q0);
@@ -121,8 +134,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       for (int ch = 0; ch < min(kAfVStages, n64); ++ch) v_load(ch);
   }
   for (int j = threadIdx.x; j < 256 * KB; j += kAfThreads) {
-    s_colkey[j] = p.drop_p > 0.f ? drop_col_key((uint32_t)j) : 0u;
-    s_keyok[j] = (j < L) && (!p.mask_pad_keys || p.pad_mask[(size_t)b * L + j] != 0);
+    s_colkey[j] = p.drop_p > 0.f ? drop_col_key((uint32_t)(shift + j)) : 0u;
+    s_keyok[j] = (j >= lead && j < n) && (!p.mask_pad_keys || p.pad_mask[(size_t)b * L + shift + j] != 0);
   }
   __syncthreads();
 
@@ -136,8 +149,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const uint32_t thr = drop ? (uint32_t)(p.drop_p * 4294967296.0) : 0u;
   const float ks_drop = drop ? 1.f / (1.f - p.drop_p) : 1.f;
   const unsigned long long seed_eff = p.seed + ((drop && p.seed_ptr) ? *p.seed_ptr : 0ull);
-  const uint32_t rk_a = drop ? drop_row_key(seed_eff, p.drop_off, (unsigned long long)bz * p.Lp + (unsigned long long)ia) : 0u;
-  const uint32_t rk_b = drop ? drop_row_key(seed_eff, p.drop_off, (unsigned long long)bz * p.Lp + (unsigned long long)ib) : 0u;
+  const uint32_t rk_a = drop ? drop_row_key(seed_eff, p.drop_off, (unsigned long long)bz * p.Lp + (unsigned long long)(shift + ia)) : 0u;
+  const uint32_t rk_b = drop ? drop_row_key(seed_eff, p.drop_off, (unsigned long long)bz * p.Lp + (unsigned long long)(shift + ib)) : 0u;
   auto visible = [&](int key, int i) -> bool { return s_keyok[key] && (!p.causal || key <= i); };
   const uint32_t q_base = smem_u32(sQ) + wg * 8192;
   auto qk_chunk = [&](float (&sacc)[32], int j0) {
@@ -153,6 +166,20 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     wg_fence_acc(sacc);
   };
   mbar_wait(&bar_load, 0);
+  if constexpr (!STREAM_V) {
+    if (packed) {
+      // rows [n, n_boxes * 128) of the loaded boxes belong to the next sequence or to no sequence (stale rows past the packed
+      // count, possibly not finite): their probabilities are zero, but 0 * Inf / NaN in O += P.V is not, so the value rows are
+      // cleared (the lead rows are rows of the sequence before: finite)
+      const int n_pad = n_boxes * 128 - n;
+      for (int i = threadIdx.x; i < HC * max(n_pad, 0) * 8; i += kAfThreads) {
+        const int c = i / (max(n_pad, 1) * 8), r = n + (i / 8) % max(n_pad, 1);
+        *reinterpret_cast<uint4*>(sV + c * KV_CHUNK + r * 128 + (i % 8) * 16) = make_uint4(0u, 0u, 0u, 0u);
+      }
+      fence_proxy_async();
+      __syncthreads();
+    }
+  }
 
   // ---- pass 1: row max over the visible keys
   float mxa = -INFINITY, mxb = -INFINITY;
@@ -176,8 +203,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const float moa = (mxa == -INFINITY) ? 0.f : mxa * sl2, mob = (mxb == -INFINITY) ? 0.f : mxb * sl2;
 
   // ---- pass 2: P = exp2(S * scale * log2e - max), row sums, optional copy of the un-dropped P, O += P.V
-  __nv_bfloat16* pa = (p.p_save && ia < L) ? p.p_save + ((size_t)bz * p.Lp + ia) * p.Lp : nullptr;
-  __nv_bfloat16* pb = (p.p_save && ib < L) ? p.p_save + ((size_t)bz * p.Lp + ib) * p.Lp : nullptr;
+  const bool own_a = ia >= lead && ia < n, own_b = ib >= lead && ib < n;   // rows of this sequence
+  __nv_bfloat16* pa = (p.p_save && own_a) ? p.p_save + ((size_t)bz * p.Lp + ia) * p.Lp : nullptr;
+  __nv_bfloat16* pb = (p.p_save && own_b) ? p.p_save + ((size_t)bz * p.Lp + ib) * p.Lp : nullptr;
   float oacc[HD / 2];
   acc_zero(oacc);
   float suma = 0.f, sumb = 0.f;
@@ -260,11 +288,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
   const float inva = suma > 0.f ? 1.f / suma : 0.f, invb = sumb > 0.f ? 1.f / sumb : 0.f;
   if (fc == 0) {
-    if (ia < L) {
+    if (own_a) {
       if (p.inv_sum) p.inv_sum[(size_t)bz * p.Lp + ia] = inva;
       if (p.m_save) p.m_save[(size_t)bz * p.Lp + ia] = moa;
     }
-    if (ib < L) {
+    if (own_b) {
       if (p.inv_sum) p.inv_sum[(size_t)bz * p.Lp + ib] = invb;
       if (p.m_save) p.m_save[(size_t)bz * p.Lp + ib] = mob;
     }
@@ -273,8 +301,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
   for (int j = 0; j < HD / 8; ++j) {
     const int c = h * HD + 8 * j + fc;
-    if (ia < L) *reinterpret_cast<uint32_t*>(p.out + ((size_t)b * L + ia) * p.ldo + c) = pack_bf16(oacc[4 * j] * inva, oacc[4 * j + 1] * inva);
-    if (ib < L) *reinterpret_cast<uint32_t*>(p.out + ((size_t)b * L + ib) * p.ldo + c) = pack_bf16(oacc[4 * j + 2] * invb, oacc[4 * j + 3] * invb);
+    if (own_a) *reinterpret_cast<uint32_t*>(p.out + ((size_t)row0 + ia) * p.ldo + c) = pack_bf16(oacc[4 * j] * inva, oacc[4 * j + 1] * inva);
+    if (own_b) *reinterpret_cast<uint32_t*>(p.out + ((size_t)row0 + ib) * p.ldo + c) = pack_bf16(oacc[4 * j + 2] * invb, oacc[4 * j + 3] * invb);
   }
 }
 
@@ -498,6 +526,7 @@ struct rp_attn_desc {
   float drop_p; unsigned long long seed, drop_off; const unsigned long long* seed_ptr;
   float* m_save;
   float scale;
+  const int32_t* seq_first; const int32_t* seq_off;
 };
 
 RP_API int rp_attn_fwd(const rp_attn_desc* a, void* stream_) {
@@ -515,6 +544,10 @@ RP_API int rp_attn_fwd(const rp_attn_desc* a, void* stream_) {
   p.p_save = reinterpret_cast<__nv_bfloat16*>(a->p_save); p.inv_sum = a->inv_sum; p.m_save = a->m_save;
   p.q_c0 = a->q_c0; p.k_c0 = a->k_c0; p.v_c0 = a->v_c0;
   p.drop_p = a->drop_p; p.seed = a->seed; p.drop_off = a->drop_off; p.seed_ptr = a->seed_ptr;
+  p.seq_first = a->seq_first; p.seq_off = a->seq_off;
+  if ((a->seq_first == nullptr) != (a->seq_off == nullptr)) return RP_EINVAL;
+  if (a->seq_first && (a->head_dim != 64 || a->L > 256)) return RP_ESHAPE;
+  if (a->seq_first && !a->causal) return RP_EINVAL;   // a lead row is never a visible key only under the causal mask
   CUtensorMap tmQ, tmK, tmV;
   int rc;
   if ((rc = make_tmap_bf16(&tmQ, a->q, a->q_rows, a->q_cols, a->ldq, 128)) != RP_OK) return rc;
@@ -597,6 +630,8 @@ struct AttnBwdParams {
   float drop_p;
   unsigned long long seed, drop_off;
   const unsigned long long* seed_ptr;
+  const int32_t* seq_first;    // packed rows as in AttnParams (then the five maps are 2-D over the rows), or null
+  const int32_t* seq_off;
 };
 
 static constexpr int kAbThreads = 256;   // two warpgroups
@@ -661,7 +696,14 @@ attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
 
   const int h = blockIdx.x % p.H, b = blockIdx.x / p.H;
   const int bz = b * p.H + h;
-  const int L = p.L;
+  // packed rows: the window of attn_fwd_kernel (lead rows of the sequence before, then positions first .. p.L - 1); L is
+  // its length, local index = position - shift.  Causal only: a query before `lead` sees no key, a key before it is masked.
+  const bool packed = p.seq_first != nullptr;
+  const int first = packed ? p.seq_first[b] : 0;
+  const int lead = first & 63, shift = first - lead;
+  const int L = p.L - shift;
+  const int row0 = packed ? p.seq_off[b] - lead : b * p.L;
+  if (packed && first == p.L) return;
   const int n_t = (L + 127) / 128;  // 128-row tiles
   const int n_blk = (L + 63) / 64;  // 64-row blocks
   const bool drop = p.drop_p > 0.f;
@@ -671,6 +713,14 @@ attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
     fence_barrier_init();
     mbar_arrive_expect_tx(&bar_load, 5 * n_t * TILE);
     for (int t = 0; t < n_t; ++t) {
+      if (packed) {
+        tma_load_2d(sK + t * TILE, &tm.k, &bar_load, p.k_c0 + h * HD, row0 + t * 128);
+        tma_load_2d(sQ + t * TILE, &tm.q, &bar_load, p.q_c0 + h * HD, row0 + t * 128);
+        tma_load_2d(sV + t * TILE, &tm.v, &bar_load, p.v_c0 + h * HD, row0 + t * 128);
+        tma_load_2d(sdO + t * TILE, &tm.d_o, &bar_load, h * HD, row0 + t * 128);
+        tma_load_2d(sO + t * TILE, &tm.o, &bar_load, h * HD, row0 + t * 128);
+        continue;
+      }
       tma_load_3d(sK + t * TILE, &tm.k, &bar_load, p.k_c0 + h * HD, t * 128, b);
       tma_load_3d(sQ + t * TILE, &tm.q, &bar_load, p.q_c0 + h * HD, t * 128, b);
       tma_load_3d(sV + t * TILE, &tm.v, &bar_load, p.v_c0 + h * HD, t * 128, b);
@@ -684,13 +734,13 @@ attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
     const int i = threadIdx.x, ti = i >> 7, r = i & 127;
     const unsigned long long seed_eff = p.seed + ((drop && p.seed_ptr) ? *p.seed_ptr : 0ull);
     float m = 0.f, inv = 0.f, dl = 0.f;
-    if (i < L) {
+    if (i >= lead && i < L) {
       m = p.m_save[(size_t)bz * p.Lp + i];
       inv = p.inv_sum[(size_t)bz * p.Lp + i];
     }
-    const uint32_t rk = drop_row_key(seed_eff, p.drop_off, (unsigned long long)bz * p.Lp + (unsigned long long)i);
-    s_keyok[i] = i < L && (!p.mask_pad_keys || p.pad_mask[(size_t)b * L + i] != 0);
-    s_colkey[i] = drop_col_key((uint32_t)i);
+    const uint32_t rk = drop_row_key(seed_eff, p.drop_off, (unsigned long long)bz * p.Lp + (unsigned long long)(shift + i));
+    s_keyok[i] = i >= lead && i < L && (!p.mask_pad_keys || p.pad_mask[(size_t)b * p.L + shift + i] != 0);
+    s_colkey[i] = drop_col_key((uint32_t)(shift + i));
     mbar_wait(&bar_load, 0);
     if (ti < n_t) {
 #pragma unroll
@@ -707,6 +757,18 @@ attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
       }
     }
     s_stat[i] = make_float4(m, inv, dl * p.scale, __uint_as_float(rk));
+  }
+  if (packed) {
+    // rows [L, n_t * 128) of the tiles belong to the next sequence or to no sequence (stale rows past the packed count): every
+    // probability that touches them is zero, but 0 * Inf / NaN in the MMAs is not, so the operand rows are cleared
+    __syncthreads();   // the statistics above have read sO / sdO
+    const int n_pad = n_t * 128 - L;
+    for (int i = threadIdx.x; i < 4 * n_pad * 8; i += kAbThreads) {
+      const int a = i / (n_pad * 8), r = L + (i / 8) % n_pad;
+      uint8_t* base = a == 0 ? sQ : a == 1 ? sK : a == 2 ? sV : sdO;
+      *reinterpret_cast<uint4*>(base + r * 128 + (i % 8) * 16) = make_uint4(0u, 0u, 0u, 0u);
+    }
+    fence_proxy_async();
   }
   __syncthreads();
 
@@ -726,8 +788,8 @@ attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int c = c0 + h * HD + 8 * j + fc;
-      if (ra < L) *reinterpret_cast<uint32_t*>(base + ((size_t)b * L + ra) * ld + c) = pack_bf16(acc[4 * j], acc[4 * j + 1]);
-      if (rb < L) *reinterpret_cast<uint32_t*>(base + ((size_t)b * L + rb) * ld + c) = pack_bf16(acc[4 * j + 2], acc[4 * j + 3]);
+      if (ra >= lead && ra < L) *reinterpret_cast<uint32_t*>(base + ((size_t)row0 + ra) * ld + c) = pack_bf16(acc[4 * j], acc[4 * j + 1]);
+      if (rb >= lead && rb < L) *reinterpret_cast<uint32_t*>(base + ((size_t)row0 + rb) * ld + c) = pack_bf16(acc[4 * j + 2], acc[4 * j + 3]);
     }
   };
   // blocks of this warpgroup: wg and 3 - wg (balances the causal triangle)
@@ -822,6 +884,7 @@ struct rp_attn_bwd_desc {
   void* dv; int ld_dv, dv_c0;
   float drop_p; unsigned long long seed, drop_off; const unsigned long long* seed_ptr;
   float scale;
+  const int32_t* seq_first; const int32_t* seq_off;
 };
 
 RP_API int rp_attn_bwd(const rp_attn_bwd_desc* a, void* stream_) {
@@ -844,16 +907,29 @@ RP_API int rp_attn_bwd(const rp_attn_bwd_desc* a, void* stream_) {
   p.dV = reinterpret_cast<__nv_bfloat16*>(a->dv); p.ld_dv = a->ld_dv; p.dv_c0 = a->dv_c0;
   p.q_c0 = a->q_c0; p.k_c0 = a->k_c0; p.v_c0 = a->v_c0;
   p.drop_p = a->drop_p; p.seed = a->seed; p.drop_off = a->drop_off; p.seed_ptr = a->seed_ptr;
+  p.seq_first = a->seq_first; p.seq_off = a->seq_off;
+  if ((a->seq_first == nullptr) != (a->seq_off == nullptr)) return RP_EINVAL;
+  if (a->seq_first && !a->causal) return RP_EINVAL;
   AttnBwdMaps tm;
   int rc;
   const uint64_t B = (uint64_t)a->B, L = (uint64_t)a->L;
   if ((uint64_t)a->q_rows < B * L || (uint64_t)a->k_rows < B * L || (uint64_t)a->v_rows < B * L || (uint64_t)a->do_rows < B * L)
     return RP_ESHAPE;
-  if ((rc = make_tmap_bf16_seq(&tm.q, a->q, B, L, a->q_cols, a->ldq, 128)) != RP_OK) return rc;
-  if ((rc = make_tmap_bf16_seq(&tm.k, a->k, B, L, a->k_cols, a->ldk, 128)) != RP_OK) return rc;
-  if ((rc = make_tmap_bf16_seq(&tm.v, a->v, B, L, a->v_cols, a->ldv, 128)) != RP_OK) return rc;
-  if ((rc = make_tmap_bf16_seq(&tm.d_o, a->d_out, B, L, a->do_cols, a->ld_do, 128)) != RP_OK) return rc;
-  if ((rc = make_tmap_bf16_seq(&tm.o, a->out, B, L, (uint64_t)a->H * 64, a->ldo, 128)) != RP_OK) return rc;
+  if (a->seq_first) {
+    // packed rows: 2-D maps over the row arrays (a window starts inside the sequence before - at a negative row for the first
+    // sequence: zero-filled - and may run into the next sequence's rows, which the kernel clears)
+    if ((rc = make_tmap_bf16(&tm.q, a->q, a->q_rows, a->q_cols, a->ldq, 128)) != RP_OK) return rc;
+    if ((rc = make_tmap_bf16(&tm.k, a->k, a->k_rows, a->k_cols, a->ldk, 128)) != RP_OK) return rc;
+    if ((rc = make_tmap_bf16(&tm.v, a->v, a->v_rows, a->v_cols, a->ldv, 128)) != RP_OK) return rc;
+    if ((rc = make_tmap_bf16(&tm.d_o, a->d_out, a->do_rows, a->do_cols, a->ld_do, 128)) != RP_OK) return rc;
+    if ((rc = make_tmap_bf16(&tm.o, a->out, a->do_rows, (uint64_t)a->H * 64, a->ldo, 128)) != RP_OK) return rc;
+  } else {
+    if ((rc = make_tmap_bf16_seq(&tm.q, a->q, B, L, a->q_cols, a->ldq, 128)) != RP_OK) return rc;
+    if ((rc = make_tmap_bf16_seq(&tm.k, a->k, B, L, a->k_cols, a->ldk, 128)) != RP_OK) return rc;
+    if ((rc = make_tmap_bf16_seq(&tm.v, a->v, B, L, a->v_cols, a->ldv, 128)) != RP_OK) return rc;
+    if ((rc = make_tmap_bf16_seq(&tm.d_o, a->d_out, B, L, a->do_cols, a->ld_do, 128)) != RP_OK) return rc;
+    if ((rc = make_tmap_bf16_seq(&tm.o, a->out, B, L, (uint64_t)a->H * 64, a->ldo, 128)) != RP_OK) return rc;
+  }
   const int smem = 10 * 128 * 128 + 1024;
   RP_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   attn_bwd_kernel<<<a->B * a->H, kAbThreads, smem, stream>>>(tm, p);

@@ -22,6 +22,11 @@ namespace rp {
 
 static constexpr int kBlockThreads = 256;   // two warpgroups: rows [0, 64) / [64, 128) of the token tile
 
+// dropout row key of row r: its token (packed rows) or the row itself
+__device__ __forceinline__ unsigned long long row_token(const int32_t* row_tok, int r, int n_rows) {
+  return (unsigned long long)(row_tok && r < n_rows ? row_tok[r] : r);
+}
+
 struct LnQkvParams {
   const float* ln_w;
   const float* ln_b;
@@ -35,6 +40,7 @@ struct LnQkvParams {
   float* mean_out;            // [T] or null
   float* rstd_out;
   int kv_only;                // predict, final block: only [K | V] = x Wkv^T + bkv (no LayerNorm, no Q: those run on the B last rows)
+  const int32_t* n_rows_dev;  // packed rows: the row count lives on the device (<= T, which sizes the grid and the maps), or null
 };
 
 // acc + bias (columns c0 + fragment column) -> packed bf16
@@ -64,7 +70,8 @@ ln_qkv_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
   __shared__ uint64_t bar_w, bar_x;
   __shared__ __align__(16) float s_lnw[D], s_lnb[D], s_bias[3 * D];
 
-  const int n_tiles = (p.T + 127) / 128;
+  const int T = p.n_rows_dev ? *p.n_rows_dev : p.T;   // rows [T, p.T) of a packed batch are stale: never stored nor summed
+  const int n_tiles = (T + 127) / 128;
   const int my_tiles = n_tiles > (int)blockIdx.x ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   auto load_x = [&](int it) {
     const int t = (int)blockIdx.x + it * (int)gridDim.x;
@@ -106,7 +113,7 @@ ln_qkv_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
       uint32_t pk[R / 2];
       wg_gemm_ss_wt<D, KCH>(acc, aX, smem_u32(sWkv) + hv * D * 128, 2 * D * 128);
       frag_bias_pack(acc, s_bias + D + hv * D, pk);
-      frag_store_bf16(pk, p.KV + hv * D, 2 * D, ra, p.T);
+      frag_store_bf16(pk, p.KV + hv * D, 2 * D, ra, T);
     }
     float xv[R];
     if (!p.kv_only) frag_load_tile(sX, 64 * wg + fr, xv);
@@ -141,11 +148,11 @@ ln_qkv_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
         pq[2 * j + h] = pack_bf16((xv[4 * j + 2 * h] - mean[h]) * rstd[h] * s_lnw[c] + s_lnb[c],
                                   (xv[4 * j + 2 * h + 1] - mean[h]) * rstd[h] * s_lnw[c + 1] + s_lnb[c + 1]);
       }
-    frag_store_bf16(pq, p.q_in, D, ra, p.T);
+    frag_store_bf16(pq, p.q_in, D, ra, T);
     if (fc == 0 && p.mean_out) {
 #pragma unroll
       for (int h = 0; h < 2; ++h)
-        if (ra + 8 * h < p.T) {
+        if (ra + 8 * h < T) {
           p.mean_out[ra + 8 * h] = mean[h];
           p.rstd_out[ra + 8 * h] = rstd[h];
         }
@@ -155,7 +162,7 @@ ln_qkv_fused_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_consta
     uint32_t pk[R / 2];
     wg_gemm_rs_wt<D, KCH>(acc, pq, smem_u32(sWq));
     frag_bias_pack(acc, s_bias, pk);
-    frag_store_bf16(pk, p.Q, D, ra, p.T);
+    frag_store_bf16(pk, p.Q, D, ra, T);
   }
 }
 
@@ -180,9 +187,9 @@ using namespace rp;
 // x bf16 [T, d]; w_in bf16 [3d, d] (packed in_proj_weight: rows [0,d) = Wq, [d,3d) = Wk | Wv), b_in fp32 [3d]; ln_w / ln_b fp32 [d].
 // Outputs: q_in bf16 [T, d] = LayerNorm(x), Q bf16 [T, d] = q_in Wq^T + bq, KV bf16 [T, 2d] = x [Wk | Wv]^T + [bk | bv],
 // mean / rstd fp32 [T] (optional, both or none).  No output may alias x.  d in {64, 128}.
-RP_API int rp_ln_qkv_fused(const void* x, const float* ln_w, const float* ln_b, float eps, const void* w_in, const float* b_in,
-                           int T, int d, void* q_in, void* Q, void* KV, float* mean_out, float* rstd_out, int hd_valid,
-                           void* stream_) {
+static int ln_qkv(const void* x, const float* ln_w, const float* ln_b, float eps, const void* w_in, const float* b_in, int T,
+                  int d, void* q_in, void* Q, void* KV, float* mean_out, float* rstd_out, int hd_valid, const int32_t* n_rows_dev,
+                  void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   const bool kv_only = q_in == nullptr && Q == nullptr;   // [K | V] projection alone (LayerNorm parameters not read)
   if (!x || !w_in || !b_in || !KV || T <= 0) return RP_EINVAL;
@@ -203,7 +210,22 @@ RP_API int rp_ln_qkv_fused(const void* x, const float* ln_w, const float* ln_b, 
   p.q_in = reinterpret_cast<__nv_bfloat16*>(q_in); p.Q = reinterpret_cast<__nv_bfloat16*>(Q);
   p.KV = reinterpret_cast<__nv_bfloat16*>(KV); p.mean_out = mean_out; p.rstd_out = rstd_out;
   p.kv_only = kv_only ? 1 : 0;
+  p.n_rows_dev = n_rows_dev;
   return d == 64 ? launch_ln_qkv<1>(tmX, tmWq, tmWkv, p, stream) : launch_ln_qkv<2>(tmX, tmWq, tmWkv, p, stream);
+}
+
+RP_API int rp_ln_qkv_fused(const void* x, const float* ln_w, const float* ln_b, float eps, const void* w_in, const float* b_in,
+                           int T, int d, void* q_in, void* Q, void* KV, float* mean_out, float* rstd_out, int hd_valid,
+                           void* stream_) {
+  return ln_qkv(x, ln_w, ln_b, eps, w_in, b_in, T, d, q_in, Q, KV, mean_out, rstd_out, hd_valid, nullptr, stream_);
+}
+
+// Packed rows: the same over the first *n_rows_dev rows of the [T, *] arrays (T, the capacity, sizes the grid and the maps).
+RP_API int rp_ln_qkv_fused_rows(const void* x, const float* ln_w, const float* ln_b, float eps, const void* w_in,
+                                const float* b_in, int T, int d, void* q_in, void* Q, void* KV, float* mean_out, float* rstd_out,
+                                int hd_valid, const int32_t* n_rows_dev, void* stream_) {
+  if (!n_rows_dev) return RP_EINVAL;
+  return ln_qkv(x, ln_w, ln_b, eps, w_in, b_in, T, d, q_in, Q, KV, mean_out, rstd_out, hd_valid, n_rows_dev, stream_);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -228,6 +250,7 @@ struct PreAttnBwdParams {
   float* dln_b;               // [d] +=
   int T;
   int hd_valid;               // > 0: padded feature slots - statistics over the real features, no gradient into padded inputs
+  const int32_t* n_rows_dev;  // as in LnQkvParams
 };
 
 template <int KCH>
@@ -247,7 +270,8 @@ pre_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmDQ, const __grid_const
   __shared__ __align__(16) float s_lnw[D];
   __shared__ float s_red[2 * 8 * D];
 
-  const int n_tiles = (p.T + 127) / 128;
+  const int T = p.n_rows_dev ? *p.n_rows_dev : p.T;   // rows [T, p.T) of a packed batch are stale: never stored nor summed
+  const int n_tiles = (T + 127) / 128;
   const int my_tiles = n_tiles > (int)blockIdx.x ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   auto load_a = [&](int it) {
     const int t = (int)blockIdx.x + it * (int)gridDim.x;
@@ -286,18 +310,18 @@ pre_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmDQ, const __grid_const
     wg_gemm_ss_w<D, KCH>(dq, aA, smem_u32(sWq));   // dQ . Wq
     {
       float hv[R];
-      frag_load_bf16(p.dh, D, ra, p.T, hv);
+      frag_load_bf16(p.dh, D, ra, T, hv);
 #pragma unroll
       for (int i = 0; i < R; ++i) dq[i] += hv[i];
     }
     {
       // LayerNorm backward, in place: dq -> t (the LayerNorm input gradient)
       float xv[R];
-      frag_load_bf16(p.x, D, ra, p.T, xv);
+      frag_load_bf16(p.x, D, ra, T, xv);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = ra + 8 * h;
-        const bool ok = r < p.T;
+        const bool ok = r < T;
         const float rs = ok ? p.rstd[r] : 0.f, nmr = ok ? -p.mean[r] * rs : 0.f;   // xhat = x * rstd - mean * rstd (0 beyond T)
         float s1 = 0.f, s2 = 0.f;
 #pragma unroll
@@ -308,8 +332,10 @@ pre_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmDQ, const __grid_const
             const float g = dq[i] * s_lnw[8 * j + fc + e], xh = fmaf(xv[i], rs, nmr);
             s1 += g;
             s2 = fmaf(g, xh, s2);
-            cw[2 * j + e] = fmaf(dq[i], xh, cw[2 * j + e]);
-            cb[2 * j + e] += dq[i];
+            if (ok) {
+              cw[2 * j + e] = fmaf(dq[i], xh, cw[2 * j + e]);
+              cb[2 * j + e] += dq[i];
+            }
           }
         const float m1 = quad_sum(s1) * inv_d, m2 = quad_sum(s2) * inv_d;
 #pragma unroll
@@ -330,7 +356,7 @@ pre_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmDQ, const __grid_const
     for (int i = 0; i < R; ++i) acc2[i] += dq[i];
     uint32_t pk[R / 2];
     frag_pack(acc2, pk);
-    frag_store_bf16(pk, p.dx, D, ra, p.T);
+    frag_store_bf16(pk, p.dx, D, ra, T);
   }
   frag_colsum_commit<R>(cw, cb, s_red, p.dln_w, p.dln_b, kBlockThreads);
 }
@@ -353,9 +379,9 @@ static int launch_pre_attn_bwd(const CUtensorMap& tmDQ, const CUtensorMap& tmDKV
 // dQ bf16 [T, d]; dKV bf16 [T, 2d]; dh, x bf16 [T, d]; mean, rstd fp32 [T] (LayerNorm1 statistics of x); ln_w fp32 [d];
 // w_in bf16 [3d, d] (packed in_proj_weight).  Outputs: dx bf16 [T, d] (no aliasing with the inputs); dln_w / dln_b fp32 [d] are
 // ACCUMULATED (+=, fp32 atomics: one per column and CTA).  d in {64, 128}.
-RP_API int rp_pre_attn_bwd(const void* dQ, const void* dKV, const void* dh, const void* x, const float* mean, const float* rstd,
-                           const float* ln_w, const void* w_in, int T, int d, void* dx, float* dln_w, float* dln_b,
-                           int hd_valid, void* stream_) {
+static int pre_attn_bwd(const void* dQ, const void* dKV, const void* dh, const void* x, const float* mean, const float* rstd,
+                        const float* ln_w, const void* w_in, int T, int d, void* dx, float* dln_w, float* dln_b, int hd_valid,
+                        const int32_t* n_rows_dev, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!dQ || !dKV || !dh || !x || !mean || !rstd || !ln_w || !w_in || !dx || !dln_w || !dln_b || T <= 0) return RP_EINVAL;
   if (d != 64 && d != 128) return RP_ESHAPE;
@@ -371,9 +397,23 @@ RP_API int rp_pre_attn_bwd(const void* dQ, const void* dKV, const void* dh, cons
   PreAttnBwdParams p;
   p.dh = reinterpret_cast<const __nv_bfloat16*>(dh); p.x = reinterpret_cast<const __nv_bfloat16*>(x);
   p.mean = mean; p.rstd = rstd; p.ln_w = ln_w; p.dx = reinterpret_cast<__nv_bfloat16*>(dx);
-  p.dln_w = dln_w; p.dln_b = dln_b; p.T = T; p.hd_valid = hd_valid;
+  p.dln_w = dln_w; p.dln_b = dln_b; p.T = T; p.hd_valid = hd_valid; p.n_rows_dev = n_rows_dev;
   return d == 64 ? launch_pre_attn_bwd<1>(tmDQ, tmDKV, tmWq, tmWkv, p, stream)
                  : launch_pre_attn_bwd<2>(tmDQ, tmDKV, tmWq, tmWkv, p, stream);
+}
+
+RP_API int rp_pre_attn_bwd(const void* dQ, const void* dKV, const void* dh, const void* x, const float* mean, const float* rstd,
+                           const float* ln_w, const void* w_in, int T, int d, void* dx, float* dln_w, float* dln_b,
+                           int hd_valid, void* stream_) {
+  return pre_attn_bwd(dQ, dKV, dh, x, mean, rstd, ln_w, w_in, T, d, dx, dln_w, dln_b, hd_valid, nullptr, stream_);
+}
+
+// Packed rows: the first *n_rows_dev rows only (the LayerNorm parameter gradients sum exactly those rows).
+RP_API int rp_pre_attn_bwd_rows(const void* dQ, const void* dKV, const void* dh, const void* x, const float* mean,
+                                const float* rstd, const float* ln_w, const void* w_in, int T, int d, void* dx, float* dln_w,
+                                float* dln_b, int hd_valid, const int32_t* n_rows_dev, void* stream_) {
+  if (!n_rows_dev) return RP_EINVAL;
+  return pre_attn_bwd(dQ, dKV, dh, x, mean, rstd, ln_w, w_in, T, d, dx, dln_w, dln_b, hd_valid, n_rows_dev, stream_);
 }
 
 
@@ -411,6 +451,8 @@ struct PostAttnParams {
   unsigned long long seed, off1, off2;
   const unsigned long long* seed_ptr;
   int hd_valid;                // > 0: padded feature slots (rp_sm90.cuh): LayerNorm statistics over the real features only
+  const int32_t* n_rows_dev;   // packed rows (as in LnQkvParams), or null
+  const int32_t* row_tok;      // packed rows: token of every row, the dropout row key (null: the row itself)
 };
 
 template <int KCH, bool TRAIN>
@@ -429,7 +471,8 @@ post_attn_fused_kernel(const __grid_constant__ CUtensorMap tmO, const __grid_con
   __shared__ __align__(16) float s_vec[5][D];     // bo, ln_w, ln_b, b1, b2
   __shared__ __align__(16) uint32_t s_ck[D];      // dropout column keys
 
-  const int n_tiles = (p.T + 127) / 128;
+  const int T = p.n_rows_dev ? *p.n_rows_dev : p.T;   // rows [T, p.T) of a packed batch are stale: never stored nor summed
+  const int n_tiles = (T + 127) / 128;
   const int my_tiles = n_tiles > (int)blockIdx.x ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   auto load_o = [&](int it) {
     const int t = (int)blockIdx.x + it * (int)gridDim.x;
@@ -476,7 +519,7 @@ post_attn_fused_kernel(const __grid_constant__ CUtensorMap tmO, const __grid_con
     if (threadIdx.x == 0 && it + 1 < my_tiles) load_o(it + 1);
     {
       float qv[R];
-      frag_load_bf16(p.q_in, D, ra, p.T, qv);
+      frag_load_bf16(p.q_in, D, ra, T, qv);
 #pragma unroll
       for (int i = 0; i < R; ++i) {
         hv[i] += s_vec[0][8 * (i >> 2) + fc + (i & 1)] + qv[i];
@@ -486,7 +529,7 @@ post_attn_fused_kernel(const __grid_constant__ CUtensorMap tmO, const __grid_con
     if (TRAIN) {
       uint32_t ph[R / 2];
       frag_pack(hv, ph);
-      frag_store_bf16(ph, p.h_save, D, ra, p.T);
+      frag_store_bf16(ph, p.h_save, D, ra, T);
     }
     // ---- y = LayerNorm(h) (bf16: the A operand of the next GEMM and the residual of the block)
     uint32_t py[R / 2];
@@ -504,7 +547,7 @@ post_attn_fused_kernel(const __grid_constant__ CUtensorMap tmO, const __grid_con
       const float mean = quad_sum(sum) * inv_d;
       const float var = fmaxf(quad_sum(sq) * inv_d - mean * mean, 0.f);
       const float rstd = rsqrtf(var + p.eps);
-      if (TRAIN && fc == 0 && ra + 8 * h < p.T) {
+      if (TRAIN && fc == 0 && ra + 8 * h < T) {
         p.mean_out[ra + 8 * h] = mean;
         p.rstd_out[ra + 8 * h] = rstd;
       }
@@ -514,14 +557,14 @@ post_attn_fused_kernel(const __grid_constant__ CUtensorMap tmO, const __grid_con
         py[2 * j + h] = pack_bf16((hv[i] - mean) * rstd * s_vec[1][c] + s_vec[2][c], (hv[i + 1] - mean) * rstd * s_vec[1][c + 1] + s_vec[2][c + 1]);
       }
     }
-    if (TRAIN) frag_store_bf16(py, p.y_save, D, ra, p.T);
+    if (TRAIN) frag_store_bf16(py, p.y_save, D, ra, T);
     // ---- u = dropout1(relu(y W1^T + b1))
     float acc[R];
     wg_gemm_rs_wt<D, KCH>(acc, py, smem_u32(sW1));
     uint32_t pu[R / 2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const uint32_t rk1 = drop ? drop_row_key(seed_eff, p.off1, (unsigned long long)(ra + 8 * h)) : 0u;
+      const uint32_t rk1 = drop ? drop_row_key(seed_eff, p.off1, row_token(p.row_tok, ra + 8 * h, T)) : 0u;
 #pragma unroll
       for (int j = 0; j < R / 4; ++j) {
         const int i = 4 * j + 2 * h, c = 8 * j + fc;
@@ -533,15 +576,15 @@ post_attn_fused_kernel(const __grid_constant__ CUtensorMap tmO, const __grid_con
         pu[2 * j + h] = pack_bf16(a0, a1);
       }
     }
-    if (TRAIN) frag_store_bf16(pu, p.u_save, D, ra, p.T);
+    if (TRAIN) frag_store_bf16(pu, p.u_save, D, ra, T);
     // ---- out = (y + dropout2(u W2^T + b2)) [* rowmask]
     wg_gemm_rs_wt<D, KCH>(acc, pu, smem_u32(sW2));
     uint32_t po[R / 2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = ra + 8 * h;
-      const float keep = (p.rowmask == nullptr || (r < p.T && p.rowmask[r])) ? 1.f : 0.f;
-      const uint32_t rk2 = drop ? drop_row_key(seed_eff, p.off2, (unsigned long long)r) : 0u;
+      const float keep = (p.rowmask == nullptr || (r < T && p.rowmask[r])) ? 1.f : 0.f;
+      const uint32_t rk2 = drop ? drop_row_key(seed_eff, p.off2, row_token(p.row_tok, r, T)) : 0u;
 #pragma unroll
       for (int j = 0; j < R / 4; ++j) {
         const int i = 4 * j + 2 * h, c = 8 * j + fc;
@@ -554,7 +597,7 @@ post_attn_fused_kernel(const __grid_constant__ CUtensorMap tmO, const __grid_con
         po[2 * j + h] = pack_bf16((f0 + yf.x) * keep, (f1 + yf.y) * keep);
       }
     }
-    frag_store_bf16(po, p.out, D, ra, p.T);
+    frag_store_bf16(po, p.out, D, ra, T);
   }
 }
 
@@ -600,6 +643,7 @@ RP_API int rp_post_attn_fused(const void* o, const void* q_in, const void* wo, c
   p.out = reinterpret_cast<__nv_bfloat16*>(out); p.eps = eps; p.T = T;
   p.h_save = p.y_save = p.u_save = nullptr; p.mean_out = p.rstd_out = nullptr;
   p.drop_p = 0.f; p.seed = p.off1 = p.off2 = 0ull; p.seed_ptr = nullptr; p.hd_valid = hd_valid;
+  p.n_rows_dev = nullptr; p.row_tok = nullptr;
   return d == 64 ? launch_post_attn<1, false>(tmO, tmWo, tmW1, tmW2, p, stream)
                  : launch_post_attn<2, false>(tmO, tmWo, tmW1, tmW2, p, stream);
 }
@@ -612,12 +656,12 @@ RP_API int rp_post_attn_fused(const void* o, const void* q_in, const void* wo, c
 // drop_mix(drop_row_key(seed + *seed_ptr, off_s, row), drop_col_key(column)): the same stream rp_gemm's epilogue and rp_dropout_bwd use.
 //   replaces (train)  replay/nn/sequential/sasrec/transformer.py:99-110 ; replay/nn/ffn.py:43-57 ;
 //                     replay/models/nn/sequential/sasrec/model.py:435-441,496-506
-RP_API int rp_post_attn_train(const void* o, const void* q_in, const void* wo, const float* bo, const float* ln_w,
-                              const float* ln_b, float eps, const void* w1, const float* b1, const void* w2, const float* b2,
-                              const uint8_t* rowmask, int T, int d, float drop_p, unsigned long long seed,
-                              unsigned long long drop_off1, unsigned long long drop_off2, const unsigned long long* seed_ptr,
-                              void* h_save, void* y_save, void* u_save, float* mean_out, float* rstd_out, void* out,
-                              int hd_valid, void* stream_) {
+static int post_attn_train(const void* o, const void* q_in, const void* wo, const float* bo, const float* ln_w,
+                           const float* ln_b, float eps, const void* w1, const float* b1, const void* w2, const float* b2,
+                           const uint8_t* rowmask, int T, int d, float drop_p, unsigned long long seed,
+                           unsigned long long drop_off1, unsigned long long drop_off2, const unsigned long long* seed_ptr,
+                           void* h_save, void* y_save, void* u_save, float* mean_out, float* rstd_out, void* out, int hd_valid,
+                           const int32_t* n_rows_dev, const int32_t* row_tok, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!o || !q_in || !wo || !bo || !ln_w || !ln_b || !w1 || !b1 || !w2 || !b2 || !out || T <= 0) return RP_EINVAL;
   if (!h_save || !y_save || !u_save || !mean_out || !rstd_out) return RP_EINVAL;
@@ -638,8 +682,32 @@ RP_API int rp_post_attn_train(const void* o, const void* q_in, const void* wo, c
   p.h_save = reinterpret_cast<__nv_bfloat16*>(h_save); p.y_save = reinterpret_cast<__nv_bfloat16*>(y_save);
   p.u_save = reinterpret_cast<__nv_bfloat16*>(u_save); p.mean_out = mean_out; p.rstd_out = rstd_out;
   p.drop_p = drop_p; p.seed = seed; p.off1 = drop_off1; p.off2 = drop_off2; p.seed_ptr = seed_ptr; p.hd_valid = hd_valid;
+  p.n_rows_dev = n_rows_dev; p.row_tok = row_tok;
   return d == 64 ? launch_post_attn<1, true>(tmO, tmWo, tmW1, tmW2, p, stream)
                  : launch_post_attn<2, true>(tmO, tmWo, tmW1, tmW2, p, stream);
+}
+
+RP_API int rp_post_attn_train(const void* o, const void* q_in, const void* wo, const float* bo, const float* ln_w,
+                              const float* ln_b, float eps, const void* w1, const float* b1, const void* w2, const float* b2,
+                              const uint8_t* rowmask, int T, int d, float drop_p, unsigned long long seed,
+                              unsigned long long drop_off1, unsigned long long drop_off2, const unsigned long long* seed_ptr,
+                              void* h_save, void* y_save, void* u_save, float* mean_out, float* rstd_out, void* out,
+                              int hd_valid, void* stream_) {
+  return post_attn_train(o, q_in, wo, bo, ln_w, ln_b, eps, w1, b1, w2, b2, rowmask, T, d, drop_p, seed, drop_off1, drop_off2,
+                         seed_ptr, h_save, y_save, u_save, mean_out, rstd_out, out, hd_valid, nullptr, nullptr, stream_);
+}
+
+// Packed rows: the first *n_rows_dev rows only; row r draws its dropout with the key of token row_tok[r], so the kept
+// elements are those of the padded run.
+RP_API int rp_post_attn_train_rows(const void* o, const void* q_in, const void* wo, const float* bo, const float* ln_w,
+                                   const float* ln_b, float eps, const void* w1, const float* b1, const void* w2, const float* b2,
+                                   int T, int d, float drop_p, unsigned long long seed, unsigned long long drop_off1,
+                                   unsigned long long drop_off2, const unsigned long long* seed_ptr, void* h_save, void* y_save,
+                                   void* u_save, float* mean_out, float* rstd_out, void* out, int hd_valid,
+                                   const int32_t* n_rows_dev, const int32_t* row_tok, void* stream_) {
+  if (!n_rows_dev || !row_tok) return RP_EINVAL;
+  return post_attn_train(o, q_in, wo, bo, ln_w, ln_b, eps, w1, b1, w2, b2, nullptr, T, d, drop_p, seed, drop_off1, drop_off2,
+                         seed_ptr, h_save, y_save, u_save, mean_out, rstd_out, out, hd_valid, n_rows_dev, row_tok, stream_);
 }
 
 
@@ -677,6 +745,8 @@ struct PostAttnBwdParams {
   const unsigned long long* seed_ptr;
   int T;
   int hd_valid;                // > 0: padded feature slots - LN statistics over the real features, no gradient into padded inputs
+  const int32_t* n_rows_dev;   // as in PostAttnParams
+  const int32_t* row_tok;
 };
 
 template <int KCH>
@@ -696,7 +766,8 @@ post_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmDZ, const __grid_cons
   __shared__ __align__(16) uint32_t s_ck[D];      // dropout column keys (rp_philox.cuh)
   __shared__ float s_red[2 * 8 * D];
 
-  const int n_tiles = (p.T + 127) / 128;
+  const int T = p.n_rows_dev ? *p.n_rows_dev : p.T;   // rows [T, p.T) of a packed batch are stale: never stored nor summed
+  const int n_tiles = (T + 127) / 128;
   const int my_tiles = n_tiles > (int)blockIdx.x ? (n_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   auto load_z = [&](int it) {
     const int t = (int)blockIdx.x + it * (int)gridDim.x;
@@ -736,7 +807,7 @@ post_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmDZ, const __grid_cons
     const int ra = tile * 128 + 64 * wg + fr;
     float rm[2];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) rm[h] = (p.rowmask == nullptr || (ra + 8 * h < p.T && p.rowmask[ra + 8 * h])) ? 1.f : 0.f;
+    for (int h = 0; h < 2; ++h) rm[h] = (p.rowmask == nullptr || (ra + 8 * h < T && p.rowmask[ra + 8 * h])) ? 1.f : 0.f;
     // ---- dzm = dz * pad (kept for the residual branch), d_t = dropout2'(dzm)
     float dzm[R];
     mbar_wait(&bar_z, it & 1);
@@ -746,7 +817,7 @@ post_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmDZ, const __grid_cons
     uint32_t pk[R / 2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const uint32_t rk2 = p.drop_p > 0.f ? drop_row_key(seed_eff, p.off2, (unsigned long long)(ra + 8 * h)) : 0u;
+      const uint32_t rk2 = p.drop_p > 0.f ? drop_row_key(seed_eff, p.off2, row_token(p.row_tok, ra + 8 * h, T)) : 0u;
 #pragma unroll
       for (int j = 0; j < R / 4; ++j) {
         const int i = 4 * j + 2 * h, c = 8 * j + fc;
@@ -760,7 +831,7 @@ post_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmDZ, const __grid_cons
         pk[2 * j + h] = pack_bf16(v0, v1);
       }
     }
-    if (p.d_t != nullptr) frag_store_bf16(pk, p.d_t, D, ra, p.T);
+    if (p.d_t != nullptr) frag_store_bf16(pk, p.d_t, D, ra, T);
     // ---- du = (d_t W2) * [u != 0] / keep
     float acc[R];
     wg_gemm_rs_w<D, KCH>(acc, pk, smem_u32(sW2));
@@ -769,28 +840,28 @@ post_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmDZ, const __grid_cons
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = ra + 8 * h;
-        const __nv_bfloat16* urow = p.u + (size_t)(r < p.T ? r : 0) * D + fcol;
+        const __nv_bfloat16* urow = p.u + (size_t)(r < T ? r : 0) * D + fcol;
 #pragma unroll
         for (int j = 0; j < R / 4; ++j) {
-          const uint32_t w = r < p.T ? *reinterpret_cast<const uint32_t*>(urow + 8 * j) : 0u;
+          const uint32_t w = r < T ? *reinterpret_cast<const uint32_t*>(urow + 8 * j) : 0u;
           const int i = 4 * j + 2 * h;
           // bf16 zero test on the raw halves (-0 cannot occur after ReLU)
           pk[2 * j + h] = pack_bf16((w & 0x7fffu) ? acc[i] * ks_ : 0.f, (w & 0x7fff0000u) ? acc[i + 1] * ks_ : 0.f);
         }
       }
     }
-    frag_store_bf16(pk, p.du, D, ra, p.T);
+    frag_store_bf16(pk, p.du, D, ra, T);
     // ---- dy = du W1 + dzm ; dh = LayerNorm2-backward(dy) ; LN parameter gradients
     wg_gemm_rs_w<D, KCH>(acc, pk, smem_u32(sW1));
 #pragma unroll
     for (int i = 0; i < R; ++i) acc[i] += dzm[i];   // acc = dy
     {
       float hv[R];
-      frag_load_bf16(p.h, D, ra, p.T, hv);
+      frag_load_bf16(p.h, D, ra, T, hv);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int r = ra + 8 * h;
-        const bool ok = r < p.T;
+        const bool ok = r < T;
         const float rs = ok ? p.rstd[r] : 0.f, nmr = ok ? -p.mean[r] * rs : 0.f;
         float s1 = 0.f, s2 = 0.f;
 #pragma unroll
@@ -801,8 +872,10 @@ post_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmDZ, const __grid_cons
             const float g = acc[i] * s_lnw[8 * j + fc + e], hh = fmaf(hv[i], rs, nmr);
             s1 += g;
             s2 = fmaf(g, hh, s2);
-            cw[2 * j + e] = fmaf(acc[i], hh, cw[2 * j + e]);
-            cb[2 * j + e] += acc[i];
+            if (ok) {
+              cw[2 * j + e] = fmaf(acc[i], hh, cw[2 * j + e]);
+              cb[2 * j + e] += acc[i];
+            }
           }
         const float m1 = quad_sum(s1) * inv_d, m2 = quad_sum(s2) * inv_d;
 #pragma unroll
@@ -818,11 +891,11 @@ post_attn_bwd_kernel(const __grid_constant__ CUtensorMap tmDZ, const __grid_cons
         }
       }
     }
-    frag_store_bf16(pk, p.dh, D, ra, p.T);
+    frag_store_bf16(pk, p.dh, D, ra, T);
     // ---- d_o = dh Wo
     wg_gemm_rs_w<D, KCH>(acc, pk, smem_u32(sWo));
     frag_pack(acc, pk);
-    frag_store_bf16(pk, p.d_o, D, ra, p.T);
+    frag_store_bf16(pk, p.d_o, D, ra, T);
   }
   frag_colsum_commit<R>(cw, cb, s_red, p.dln_w, p.dln_b, kBlockThreads);
 }
@@ -849,10 +922,11 @@ using namespace rp;
 // element index) exactly as rp_post_attn_train / rp_gemm drew it; site 1 is encoded in the zeros of u.
 // Outputs bf16 [T, d]: d_t (may be NULL when drop_p == 0 and rowmask == NULL: then d_t == dz), du, dh, d_o (none may alias an
 // input); dln_w / dln_b fp32 [d] are ACCUMULATED (one atomic per column and CTA).  d in {64, 128}.
-RP_API int rp_post_attn_bwd(const void* dz, const void* u, const void* h, const float* mean, const float* rstd, const float* ln_w,
-                            const void* w2, const void* w1, const void* wo, const uint8_t* rowmask, int T, int d, float drop_p,
-                            unsigned long long seed, unsigned long long drop_off2, const unsigned long long* seed_ptr, void* d_t,
-                            void* du, void* dh, void* d_o, float* dln_w, float* dln_b, int hd_valid, void* stream_) {
+static int post_attn_bwd(const void* dz, const void* u, const void* h, const float* mean, const float* rstd, const float* ln_w,
+                         const void* w2, const void* w1, const void* wo, const uint8_t* rowmask, int T, int d, float drop_p,
+                         unsigned long long seed, unsigned long long drop_off2, const unsigned long long* seed_ptr, void* d_t,
+                         void* du, void* dh, void* d_o, float* dln_w, float* dln_b, int hd_valid, const int32_t* n_rows_dev,
+                         const int32_t* row_tok, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!dz || !u || !h || !mean || !rstd || !ln_w || !w2 || !w1 || !wo || !du || !dh || !d_o || !dln_w || !dln_b || T <= 0)
     return RP_EINVAL;
@@ -873,7 +947,26 @@ RP_API int rp_post_attn_bwd(const void* dz, const void* u, const void* h, const 
   p.d_t = reinterpret_cast<__nv_bfloat16*>(d_t); p.du = reinterpret_cast<__nv_bfloat16*>(du);
   p.dh = reinterpret_cast<__nv_bfloat16*>(dh); p.d_o = reinterpret_cast<__nv_bfloat16*>(d_o);
   p.dln_w = dln_w; p.dln_b = dln_b; p.drop_p = drop_p; p.seed = seed; p.off2 = drop_off2; p.seed_ptr = seed_ptr; p.T = T;
-  p.hd_valid = hd_valid;
+  p.hd_valid = hd_valid; p.n_rows_dev = n_rows_dev; p.row_tok = row_tok;
   return d == 64 ? launch_post_attn_bwd<1>(tmDZ, tmW2, tmW1, tmWo, p, stream)
                  : launch_post_attn_bwd<2>(tmDZ, tmW2, tmW1, tmWo, p, stream);
+}
+
+RP_API int rp_post_attn_bwd(const void* dz, const void* u, const void* h, const float* mean, const float* rstd, const float* ln_w,
+                            const void* w2, const void* w1, const void* wo, const uint8_t* rowmask, int T, int d, float drop_p,
+                            unsigned long long seed, unsigned long long drop_off2, const unsigned long long* seed_ptr, void* d_t,
+                            void* du, void* dh, void* d_o, float* dln_w, float* dln_b, int hd_valid, void* stream_) {
+  return post_attn_bwd(dz, u, h, mean, rstd, ln_w, w2, w1, wo, rowmask, T, d, drop_p, seed, drop_off2, seed_ptr, d_t, du, dh, d_o,
+                       dln_w, dln_b, hd_valid, nullptr, nullptr, stream_);
+}
+
+// Packed rows: the first *n_rows_dev rows only, dropout keyed by row_tok as in rp_post_attn_train_rows.
+RP_API int rp_post_attn_bwd_rows(const void* dz, const void* u, const void* h, const float* mean, const float* rstd,
+                                 const float* ln_w, const void* w2, const void* w1, const void* wo, int T, int d, float drop_p,
+                                 unsigned long long seed, unsigned long long drop_off2, const unsigned long long* seed_ptr,
+                                 void* d_t, void* du, void* dh, void* d_o, float* dln_w, float* dln_b, int hd_valid,
+                                 const int32_t* n_rows_dev, const int32_t* row_tok, void* stream_) {
+  if (!n_rows_dev || !row_tok) return RP_EINVAL;
+  return post_attn_bwd(dz, u, h, mean, rstd, ln_w, w2, w1, wo, nullptr, T, d, drop_p, seed, drop_off2, seed_ptr, d_t, du, dh, d_o,
+                       dln_w, dln_b, hd_valid, n_rows_dev, row_tok, stream_);
 }

@@ -178,7 +178,10 @@ __global__ void embed_bwd_table_kernel(const __nv_bfloat16* __restrict__ dx, con
                                        int zero_pad_rows, float drop_p, unsigned long long seed,
                                        unsigned long long drop_off, const unsigned long long* __restrict__ seed_ptr,
                                        const uint8_t* __restrict__ tok_mask, float* __restrict__ d_mask_emb,
-                                       float* __restrict__ dE) {
+                                       float* __restrict__ dE, const int32_t* __restrict__ row_tok = nullptr,
+                                       const int32_t* __restrict__ n_rows_dev = nullptr) {
+  // row_tok != null: dx holds packed rows, row r being token row_tok[r]; *n_rows_dev of them
+  if (n_rows_dev) T = *n_rows_dev;
   if (drop_p > 0.f && seed_ptr) seed += *seed_ptr;
   constexpr int D = VEC * 32;
   const int lane = threadIdx.x & 31;
@@ -195,7 +198,7 @@ __global__ void embed_bwd_table_kernel(const __nv_bfloat16* __restrict__ dx, con
     __nv_bfloat162 gv[TOK][VEC / 2];
 #pragma unroll
     for (int k = 0; k < TOK; ++k) {
-      const int t = min(tb + k, T - 1);
+      const int t = row_tok ? row_tok[min(tb + k, T - 1)] : min(tb + k, T - 1);
       id[k] = ids[t];
       on[k] = tb + k < T && id[k] != pad_id && !((zero_pad_rows || tok_mask) && !pad_mask[t]);  // pads receive no gradient
     }
@@ -208,7 +211,7 @@ __global__ void embed_bwd_table_kernel(const __nv_bfloat16* __restrict__ dx, con
 #pragma unroll
     for (int k = 0; k < TOK; ++k) {
       if (!on[k]) continue;
-      const int t = tb + k;
+      const int t = row_tok ? row_tok[tb + k] : tb + k;
       float* dst = (tok_mask && !tok_mask[t]) ? d_mask_emb + lane * VEC : dE + (size_t)id[k] * D + lane * VEC;
       float v[VEC];
 #pragma unroll
@@ -239,7 +242,9 @@ __global__ void embed_bwd_table_kernel(const __nv_bfloat16* __restrict__ dx, con
 __global__ void embed_bwd_pos_kernel(const __nv_bfloat16* __restrict__ dx, const uint8_t* __restrict__ pad_mask, int B,
                                      int L, int D, int pos0, int zero_pad_rows, float drop_p, unsigned long long seed,
                                      unsigned long long drop_off, const unsigned long long* __restrict__ seed_ptr,
-                                     float* __restrict__ dP) {
+                                     float* __restrict__ dP, const int32_t* __restrict__ seq_first = nullptr,
+                                     const int32_t* __restrict__ seq_off = nullptr) {
+  // seq_first != null: dx holds packed rows - position l of sequence b is row seq_off[b] + l - seq_first[b], if l >= seq_first[b]
   if (drop_p > 0.f && seed_ptr) seed += *seed_ptr;
   extern __shared__ float red4[];  // [rows_per_iter][D]
   const int l = blockIdx.x;
@@ -257,7 +262,13 @@ __global__ void embed_bwd_pos_kernel(const __nv_bfloat16* __restrict__ dx, const
   for (int b = b0 + rl; b < b1; b += rlanes) {
     const int t = b * L + l;
     if (zero_pad_rows && !pad_mask[t]) continue;
-    const uint2 raw = *reinterpret_cast<const uint2*>(dx + (size_t)t * D + cg * 4);
+    int row = t;
+    if (seq_first) {
+      const int f = seq_first[b];
+      if (l < f) continue;
+      row = seq_off[b] + l - f;
+    }
+    const uint2 raw = *reinterpret_cast<const uint2*>(dx + (size_t)row * D + cg * 4);
     const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&raw);
     const float2 a = __bfloat1622float2(h[0]), c = __bfloat1622float2(h[1]);
     float v[4] = {a.x, a.y, c.x, c.y};
@@ -276,6 +287,140 @@ __global__ void embed_bwd_pos_kernel(const __nv_bfloat16* __restrict__ dx, const
     float sum = 0.f;
     for (int r = 0; r < rlanes; ++r) sum += red4[r * D + c];
     atomicAdd(dP + (size_t)(pos0 + l) * D + c, sum);
+  }
+}
+
+// packed rows: x[r] = E[ids[t]] * scale + P[pos0 + t % L] -> dropout -> (* pad) with t = row_tok[r], r < *n_rows_dev; the
+// dropout key is the token index t, so the kept elements are those of the padded embedding.  TOK rows per warp and iteration.
+template <int VEC>
+__global__ void embed_fwd_rows_kernel(const __nv_bfloat16* __restrict__ table, const float* __restrict__ pos,
+                                      const int32_t* __restrict__ ids, const uint8_t* __restrict__ pad_mask,
+                                      const int32_t* __restrict__ row_tok, const int32_t* __restrict__ n_rows_dev, int L,
+                                      int pos0, float scale, int zero_pad_rows, float drop_p, unsigned long long seed,
+                                      unsigned long long drop_off, const unsigned long long* __restrict__ seed_ptr,
+                                      __nv_bfloat16* __restrict__ out) {
+  if (drop_p > 0.f && seed_ptr) seed += *seed_ptr;
+  constexpr int D = VEC * 32;
+  constexpr int TOK = 4;
+  const int n_rows = *n_rows_dev;
+  const int lane = threadIdx.x & 31;
+  const int wpb = blockDim.x >> 5;
+  const uint32_t thr = drop_p > 0.f ? (uint32_t)(drop_p * 4294967296.0) : 0u;
+  const float ks = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
+  uint32_t ck[VEC];
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) ck[i] = drop_col_key((uint32_t)(lane * VEC + i));
+  for (int rb = (blockIdx.x * wpb + (threadIdx.x >> 5)) * TOK; rb < n_rows; rb += gridDim.x * wpb * TOK) {
+    int t[TOK];
+    __nv_bfloat162 ev[TOK][VEC / 2];
+#pragma unroll
+    for (int k = 0; k < TOK; ++k) t[k] = row_tok[min(rb + k, n_rows - 1)];
+#pragma unroll
+    for (int k = 0; k < TOK; ++k) {
+      const __nv_bfloat16* e = table + (size_t)ids[t[k]] * D + lane * VEC;
+#pragma unroll
+      for (int i = 0; i < VEC; i += 2) ev[k][i >> 1] = *reinterpret_cast<const __nv_bfloat162*>(e + i);
+    }
+#pragma unroll
+    for (int k = 0; k < TOK; ++k) {
+      if (rb + k >= n_rows) break;
+      const float* pp = pos + (size_t)(pos0 + t[k] % L) * D + lane * VEC;
+      float v[VEC];
+#pragma unroll
+      for (int i = 0; i < VEC; i += 2) {
+        const float2 f = __bfloat1622float2(ev[k][i >> 1]);
+        v[i] = f.x * scale + pp[i];
+        v[i + 1] = f.y * scale + pp[i + 1];
+      }
+      if (drop_p > 0.f) {
+        const uint32_t rk = drop_row_key(seed, drop_off, (unsigned long long)t[k]);
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) v[i] = drop_mix(rk, ck[i]) >= thr ? v[i] * ks : 0.f;
+      }
+      if (zero_pad_rows && !pad_mask[t[k]]) {
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) v[i] = 0.f;
+      }
+      __nv_bfloat16* o = out + (size_t)(rb + k) * D + lane * VEC;
+#pragma unroll
+      for (int i = 0; i < VEC; i += 2) *reinterpret_cast<uint32_t*>(o + i) = pack_bf16(v[i], v[i + 1]);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Row plan of a causal batch: sequence b keeps the suffix of positions [first_b, L) that starts at its first real token or
+// valid target (first_b = L: no row), and the kept rows of all sequences are packed in sequence order.
+// ------------------------------------------------------------------------------------------------------------------
+// one warp per sequence: first_b and the kept row count L - first_b
+__global__ void row_plan_first_kernel(const uint8_t* __restrict__ pad_mask, const int64_t* __restrict__ labels,
+                                      const uint8_t* __restrict__ target_mask, int B, int L, int n_items,
+                                      int32_t* __restrict__ seq_first) {
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (b >= B) return;
+  int first = L;
+  for (int l0 = 0; l0 < L; l0 += 32) {
+    const int l = l0 + lane;
+    bool keep = false;
+    if (l < L) {
+      const size_t t = (size_t)b * L + l;
+      keep = pad_mask[t] != 0;
+      if (target_mask && target_mask[t]) {
+        const int64_t y = labels[t];
+        keep |= y >= 0 && y < n_items;
+      }
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, keep);
+    if (bal) {
+      first = l0 + __ffs(bal) - 1;
+      break;
+    }
+  }
+  if (lane == 0) seq_first[b] = first;
+}
+
+// one CTA: exclusive prefix sum of the kept row counts over the sequences -> seq_off, and the packed row count
+__global__ void __launch_bounds__(1024) row_plan_scan_kernel(const int32_t* __restrict__ seq_first, int B, int L,
+                                                              int32_t* __restrict__ seq_off, int32_t* __restrict__ n_rows) {
+  __shared__ int warp_tot[32];
+  __shared__ int carry_s;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (threadIdx.x == 0) carry_s = 0;
+  __syncthreads();
+  for (int b0 = 0; b0 < B; b0 += 1024) {
+    const int b = b0 + threadIdx.x;
+    const int cnt = b < B ? L - seq_first[b] : 0;
+    int inc = cnt;   // inclusive scan inside the warp
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += v;
+    }
+    if (lane == 31) warp_tot[warp] = inc;
+    __syncthreads();
+    int wbase = 0;
+    for (int w = 0; w < warp; ++w) wbase += warp_tot[w];
+    const int carry = carry_s;
+    if (b < B) seq_off[b] = carry + wbase + inc - cnt;
+    __syncthreads();
+    if (threadIdx.x == 1023) carry_s = carry + wbase + inc;
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *n_rows = carry_s;
+}
+
+// grid over the tokens: row_tok of every kept row; valid_rows[k] = packed row of the k-th valid target (k < *n_valid)
+__global__ void row_plan_fill_kernel(const int32_t* __restrict__ seq_first, const int32_t* __restrict__ seq_off, int T, int L,
+                                     const int32_t* __restrict__ valid_idx, const int32_t* __restrict__ n_valid,
+                                     int32_t* __restrict__ row_tok, int32_t* __restrict__ valid_rows) {
+  const int nv = valid_idx ? *n_valid : 0;
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < T; t += gridDim.x * blockDim.x) {
+    const int b = t / L, l = t % L, f = seq_first[b];
+    if (l >= f) row_tok[seq_off[b] + l - f] = t;
+    if (t < nv) {
+      const int u = valid_idx[t], ub = u / L, uf = seq_first[ub];
+      valid_rows[t] = seq_off[ub] + u % L - uf;   // a valid target is never before first_b
+    }
   }
 }
 
@@ -702,6 +847,66 @@ RP_API int rp_embed_bwd(const void* dx, const int32_t* ids, const uint8_t* pad_m
     embed_bwd_pos_kernel<<<dim3(L, G), 256, (size_t)rlanes * d * sizeof(float), stream>>>(
         reinterpret_cast<const __nv_bfloat16*>(dx), pad_mask, B, L, d, pos0, zero_pad_rows, drop_p, seed, drop_off, seed_ptr,
         d_pos);
+  }
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+RP_API int rp_row_plan(const uint8_t* pad_mask, const int64_t* labels, const uint8_t* target_mask, int B, int L, int n_items,
+                       const int32_t* valid_idx, const int32_t* n_valid, int32_t* seq_first, int32_t* seq_off,
+                       int32_t* n_rows, int32_t* row_tok, int32_t* valid_rows, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!pad_mask || !seq_first || !seq_off || !n_rows || !row_tok || B <= 0 || L <= 0) return RP_EINVAL;
+  if (target_mask && !labels) return RP_EINVAL;
+  if (valid_idx && (!n_valid || !valid_rows)) return RP_EINVAL;
+  row_plan_first_kernel<<<(B + 7) / 8, 256, 0, stream>>>(pad_mask, labels, target_mask, B, L, n_items, seq_first);
+  RP_LAUNCH_CHECK();
+  row_plan_scan_kernel<<<1, 1024, 0, stream>>>(seq_first, B, L, seq_off, n_rows);
+  RP_LAUNCH_CHECK();
+  const int T = B * L;
+  row_plan_fill_kernel<<<grid_for(T, 8), 256, 0, stream>>>(seq_first, seq_off, T, L, valid_idx, n_valid, row_tok, valid_rows);
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+RP_API int rp_embed_fwd_rows(const void* table, const float* pos, const int32_t* ids, const uint8_t* pad_mask,
+                             const int32_t* row_tok, const int32_t* n_rows_dev, int T, int L, int d, int pos0, float scale,
+                             int zero_pad_rows, float drop_p, unsigned long long seed, unsigned long long drop_off,
+                             const unsigned long long* seed_ptr, void* out, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!table || !pos || !ids || !row_tok || !n_rows_dev || !out || T <= 0 || L <= 0) return RP_EINVAL;
+  if (zero_pad_rows && !pad_mask) return RP_EINVAL;
+  const int grid = grid_for(T, 8);
+  RP_DISPATCH_D(d, (embed_fwd_rows_kernel<VEC><<<grid, 256, 0, stream>>>(
+                       reinterpret_cast<const __nv_bfloat16*>(table), pos, ids, pad_mask, row_tok, n_rows_dev, L, pos0, scale,
+                       zero_pad_rows, drop_p, seed, drop_off, seed_ptr, reinterpret_cast<__nv_bfloat16*>(out))));
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+RP_API int rp_embed_bwd_rows(const void* dx, const int32_t* ids, const uint8_t* pad_mask, const int32_t* row_tok,
+                             const int32_t* n_rows_dev, const int32_t* seq_first, const int32_t* seq_off, int B, int L, int d,
+                             int pad_id, int pos0, float scale, int zero_pad_rows, float drop_p, unsigned long long seed,
+                             unsigned long long drop_off, const unsigned long long* seed_ptr, float* d_table, float* d_pos,
+                             void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!dx || !ids || !row_tok || !n_rows_dev || !seq_first || !seq_off || !d_table || !d_pos || B <= 0 || L <= 0)
+    return RP_EINVAL;
+  if (zero_pad_rows && !pad_mask) return RP_EINVAL;
+  const int T = B * L;
+  const int grid = grid_for(T, 8);
+  RP_DISPATCH_D(d, (embed_bwd_table_kernel<VEC><<<grid, 256, 0, stream>>>(
+                       reinterpret_cast<const __nv_bfloat16*>(dx), ids, pad_mask, T, pad_id, scale, zero_pad_rows, drop_p,
+                       seed, drop_off, seed_ptr, nullptr, nullptr, d_table, row_tok, n_rows_dev)));
+  RP_LAUNCH_CHECK();
+  {
+    const int rlanes = 256 / (d / 4);
+    int G = (B + 31) / 32;
+    if (G < 1) G = 1;
+    if (G > 16) G = 16;
+    embed_bwd_pos_kernel<<<dim3(L, G), 256, (size_t)rlanes * d * sizeof(float), stream>>>(
+        reinterpret_cast<const __nv_bfloat16*>(dx), pad_mask, B, L, d, pos0, zero_pad_rows, drop_p, seed, drop_off, seed_ptr,
+        d_pos, seq_first, seq_off);
   }
   RP_LAUNCH_CHECK();
   return RP_OK;

@@ -30,6 +30,7 @@ struct WgradParams {
   CUtensorMap tmB[kWgMaxPairs];   // X_i : [T rows, n_in_i cols],  box [64 tokens x 64 features]
   int unit_pair[kWgMaxUnits], unit_m0[kWgMaxUnits], unit_n0[kWgMaxUnits];
   int n_units, splits, T;
+  const int32_t* n_rows_dev;   // packed rows: the token count lives on the device (<= T, which sizes the maps), or null
   float* part;     // [n_units][splits][128 * BN]
   float* part_b;   // [n_units][splits][128]
 };
@@ -49,7 +50,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_group_kernel(const __grid
   const int unit = blockIdx.x / p.splits, split = blockIdx.x % p.splits;
   const int pair = p.unit_pair[unit], m0 = p.unit_m0[unit], n0 = p.unit_n0[unit];
   const bool do_bias = (n0 == 0);              // exactly one column tile per dY row block carries the bias gradient
-  const int chunks = (p.T + 63) / 64;
+  const int T = p.n_rows_dev ? *p.n_rows_dev : p.T;
+  const int chunks = (T + 63) / 64;
   const int c_begin = (int)(((long long)chunks * split) / p.splits);
   const int c_end = (int)(((long long)chunks * (split + 1)) / p.splits);
   const CUtensorMap* tmA = &p.tmA[pair];
@@ -91,6 +93,16 @@ __global__ void __launch_bounds__(kWgThreads, 1) wgrad_group_kernel(const __grid
   for (int it = 0; it < n_it; ++it) {
     const uint32_t s = it % kWgStages, ph = (it / kWgStages) & 1;
     mbar_wait(&bar_full[s], ph);
+    if (p.n_rows_dev && (c_begin + it) * 64 + 64 > T) {
+      // the last chunk of a packed batch: its rows [T, ...) are stale (not zero-filled by TMA, possibly not even finite), so
+      // they are cleared in every box of the stage before the MMAs read it
+      const int r0 = T - (c_begin + it) * 64, per = (64 - r0) * 8;
+      uint8_t* st = sRing + s * STAGE;
+      for (int i = threadIdx.x; i < (STAGE / 8192) * per; i += kWgThreads)
+        *reinterpret_cast<uint4*>(st + (i / per) * 8192 + (r0 + (i % per) / 8) * 128 + (i % 8) * 16) = make_uint4(0u, 0u, 0u, 0u);
+      fence_proxy_async();
+      __syncthreads();
+    }
     const uint32_t a0 = smem_u32(sRing + s * STAGE) + wg * 8192, b0 = smem_u32(sRing + s * STAGE + A_BYTES);
     wg_fence();
 #pragma unroll
@@ -222,9 +234,8 @@ RP_API size_t rp_wgrad_group_workspace(const rp_wgrad_pair* pairs, int n_pairs) 
   return (size_t)nu * sp * (128 * bn + 128) * sizeof(float);
 }
 
-// All pairs share the token count T.  accumulate != 0: dW / db += result, else they are overwritten.
-RP_API int rp_wgrad_group(const rp_wgrad_pair* pairs, int n_pairs, int T, int accumulate, void* workspace,
-                          size_t workspace_bytes, void* stream_) {
+static int wgrad_group(const rp_wgrad_pair* pairs, int n_pairs, int T, int accumulate, const int32_t* n_rows_dev,
+                       void* workspace, size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (T <= 0 || !workspace) return RP_EINVAL;
   WgradParams p;
@@ -242,7 +253,7 @@ RP_API int rp_wgrad_group(const rp_wgrad_pair* pairs, int n_pairs, int T, int ac
     r.dW[i] = pairs[i].dW; r.db[i] = pairs[i].db; r.ld_dw[i] = pairs[i].dw_ld;
     r.n_out[i] = pairs[i].n_out; r.n_in[i] = pairs[i].n_in;
   }
-  p.n_units = nu; p.splits = sp; p.T = T;
+  p.n_units = nu; p.splits = sp; p.T = T; p.n_rows_dev = n_rows_dev;
   p.part = reinterpret_cast<float*>(workspace);
   p.part_b = p.part + (size_t)nu * sp * 128 * bn;
   memcpy(r.unit_pair, p.unit_pair, sizeof(p.unit_pair));
@@ -265,4 +276,17 @@ RP_API int rp_wgrad_group(const rp_wgrad_pair* pairs, int n_pairs, int T, int ac
   wgrad_reduce_kernel<<<dim3(nu, by), 256, 0, stream>>>(r);
   RP_LAUNCH_CHECK();
   return RP_OK;
+}
+
+// All pairs share the token count T.  accumulate != 0: dW / db += result, else they are overwritten.
+RP_API int rp_wgrad_group(const rp_wgrad_pair* pairs, int n_pairs, int T, int accumulate, void* workspace,
+                          size_t workspace_bytes, void* stream_) {
+  return wgrad_group(pairs, n_pairs, T, accumulate, nullptr, workspace, workspace_bytes, stream_);
+}
+
+// Packed rows: the contraction covers the first *n_rows_dev of the T rows (T, the capacity, sizes the maps).
+RP_API int rp_wgrad_group_rows(const rp_wgrad_pair* pairs, int n_pairs, int T, int accumulate, const int32_t* n_rows_dev,
+                               void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!n_rows_dev) return RP_EINVAL;
+  return wgrad_group(pairs, n_pairs, T, accumulate, n_rows_dev, workspace, workspace_bytes, stream_);
 }

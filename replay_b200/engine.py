@@ -132,7 +132,8 @@ class _CountingLib:
                "rp_adam_step": 2, "rp_cast_bf16": 1, "rp_counter_add": 1, "rp_reduce_splits": 1, "rp_ce_head_fwd": 2, "rp_ce_head_bwd": 3,
                "rp_score_topk": 2, "rp_seen_prepare": 1, "rp_sampled_head_fwd": 4, "rp_sampled_head_bwd": 4, "rp_post_attn_fused": 1,
                "rp_post_attn_train": 1, "rp_wgrad_group": 2, "rp_ln_qkv_fused": 1, "rp_pre_attn_bwd": 1,
-               "rp_post_attn_bwd": 1}
+               "rp_post_attn_bwd": 1, "rp_row_plan": 3, "rp_embed_fwd_rows": 1, "rp_embed_bwd_rows": 2, "rp_ln_qkv_fused_rows": 1,
+               "rp_post_attn_train_rows": 1, "rp_post_attn_bwd_rows": 1, "rp_pre_attn_bwd_rows": 1, "rp_wgrad_group_rows": 2}
 
     def __init__(self, L):
         self._L = L
@@ -196,6 +197,10 @@ class SasRecEngine:
         self.fused_wgrad = fused_body and d <= 256          # rp_wgrad_group: at most 48 output tiles per block
         self.fused_pre_attn = fused_body and d <= 128       # LN1 + Q / KV projections in one pass (forward and backward)
         self.fused_post_attn_bwd = fused_body and d <= 128  # dropout' + FFN + LN2 + out-projection backward in one pass
+        # new-path training with the fused body on each sequence's live suffix only, packed (packed_eligible).  The training
+        # driver (trainer.Trainer) turns it on; direct callers keep the padded rows, whose activation buffers they may read
+        self.packed_body = False
+        self._packed = False      # the staged training batch runs packed (set by _prepare)
         self.fused_ce = True      # single-pass CE forward + dH (guarded on the device by a bound on |logit|)
         self.n_valid_hint = 0     # host estimate of the number of valid targets per step (load balance of the CE head only)
         self._alloc_workspace()
@@ -370,6 +375,13 @@ class SasRecEngine:
         self.labels_c = torch.zeros(T, **i32)
         self.n_valid = torch.zeros(1, **i32)
         self.prep_scratch = torch.zeros((T + 1023) // 1024 + 1, **i32)
+        # row plan of a packed batch (rp_row_plan): first kept position and first packed row of every sequence, the packed row
+        # count, the token of every packed row and the packed row of every valid target
+        self.seq_first = torch.zeros(self.B, **i32)
+        self.seq_off = torch.zeros(self.B, **i32)
+        self.n_rows = torch.zeros(1, **i32)
+        self.row_tok = torch.zeros(T, **i32)
+        self.valid_rows = torch.zeros(T, **i32)
         self.x = [torch.zeros(T, d, **bf) for _ in range(cfg.n_blocks + 1)]
         self.act = []
         for _ in range(cfg.n_blocks):
@@ -488,7 +500,7 @@ class SasRecEngine:
                    c_geom=(n_in, 0, 0, 0), c_split_stride=n)
         check(self.lib.rp_reduce_splits(self.wg_ws.data_ptr(), split, n, n, dW.data_ptr(), 1, self._stream()), "rp_reduce_splits")
 
-    def _wgrad_group(self, pairs):
+    def _wgrad_group(self, pairs, n_rows_dev=None):
         """[(dY bf16 [T, n_out], X bf16 [T, n_in], dW fp32 [n_out, n_in], db fp32 [n_out] | None), ...]: every weight and bias
         gradient of a block in one wgmma launch + one deterministic reduction launch (csrc/rp_wgrad.cu).  Gradients are
         accumulated (+=) like the un-fused path does."""
@@ -504,6 +516,10 @@ class SasRecEngine:
             raise ValueError("rp_wgrad_group: unsupported gradient shapes")
         if self._wgrad_ws is None or self._wgrad_ws.numel() < need:
             self._wgrad_ws = torch.zeros(need, device=self.dev, dtype=torch.uint8)
+        if n_rows_dev is not None:
+            check(self.lib.rp_wgrad_group_rows(arr, n, self.T, 1, n_rows_dev.data_ptr(), self._wgrad_ws.data_ptr(),
+                                               self._wgrad_ws.numel(), self._stream()), "rp_wgrad_group_rows")
+            return
         check(self.lib.rp_wgrad_group(arr, n, self.T, 1, self._wgrad_ws.data_ptr(), self._wgrad_ws.numel(), self._stream()),
               "rp_wgrad_group")
 
@@ -675,6 +691,28 @@ class SasRecEngine:
                                         self.in_tmask.data_ptr() if with_targets else None, self.T, cfg.pad_id, cfg.n_items,
                                         self.ids32.data_ptr(), self.valid_idx.data_ptr(), self.labels_c.data_ptr(),
                                         self.n_valid.data_ptr(), self.prep_scratch.data_ptr(), self._stream()), "rp_prepare_batch")
+        self._packed = with_targets and self.packed_eligible()
+        if self._packed:
+            check(self.lib.rp_row_plan(self.in_pad.data_ptr(), self.in_labels.data_ptr(), self.in_tmask.data_ptr(), self.B,
+                                       self.L, cfg.n_items, self.valid_idx.data_ptr(), self.n_valid.data_ptr(),
+                                       self.seq_first.data_ptr(), self.seq_off.data_ptr(), self.n_rows.data_ptr(),
+                                       self.row_tok.data_ptr(), self.valid_rows.data_ptr(), self._stream()), "rp_row_plan")
+
+    def packed_eligible(self) -> bool:
+        """Whether a training step runs the body on packed rows: sequence b keeps only its positions [first_b, L), from its
+        first real token or valid target on (the row before the first real token is a target whose input is padding), and
+        the kept rows of all sequences are stored back to back.  Exact for the new-path SASRec: pad keys are masked, a pad
+        query sees nothing live, and no loss reads a row before first_b, so those rows contribute exactly zero to every
+        gradient.  Not for the legacy model (its attention sees pad keys), SCE (it reads every row's hidden state), other
+        encoders, or shapes outside the fused body (d <= 128, head slot 64, L <= 256)."""
+        cfg = self.cfg
+        return (self.packed_body and isinstance(cfg, EncoderConfig) and cfg.variant == "new" and self.with_grad
+                and self.sce is None and cfg.dp <= 128 and cfg.head_slot == 64 and self.L <= 256 and self.fused_attn_bwd
+                and self.fused_pre_attn and self.fused_post_attn_train and self.fused_post_attn_bwd and self.fused_wgrad)
+
+    def _target_rows(self):
+        """Rows of the body's output that hold the valid targets, in the CE head's order."""
+        return self.valid_rows if self._packed else self.valid_idx
 
     def _body_forward(self, training: bool, last_only: bool = False):
         """``last_only`` (predict): the final block is evaluated for the LAST position of every sequence only - LN1, the Q
@@ -687,9 +725,16 @@ class SasRecEngine:
         drop = cfg.dropout if training else 0.0
         pad = self.in_pad
         pos0 = 0 if legacy else cfg.max_len - L
-        check(self.lib.rp_embed_fwd(p16["item_emb"].data_ptr(), prm["pos_emb"].data_ptr(), self.ids32.data_ptr(),
-                                    pad.data_ptr(), T, L, d, pos0, math.sqrt(cfg.d), int(legacy), drop, self.seed, 0,
-                                    self.rng_counter.data_ptr(), self.x[0].data_ptr(), self._stream()), "rp_embed_fwd")
+        packed = self._packed
+        if packed:
+            check(self.lib.rp_embed_fwd_rows(p16["item_emb"].data_ptr(), prm["pos_emb"].data_ptr(), self.ids32.data_ptr(),
+                                             pad.data_ptr(), self.row_tok.data_ptr(), self.n_rows.data_ptr(), T, L, d, pos0,
+                                             math.sqrt(cfg.d), 0, drop, self.seed, 0, self.rng_counter.data_ptr(),
+                                             self.x[0].data_ptr(), self._stream()), "rp_embed_fwd_rows")
+        else:
+            check(self.lib.rp_embed_fwd(p16["item_emb"].data_ptr(), prm["pos_emb"].data_ptr(), self.ids32.data_ptr(),
+                                        pad.data_ptr(), T, L, d, pos0, math.sqrt(cfg.d), int(legacy), drop, self.seed, 0,
+                                        self.rng_counter.data_ptr(), self.x[0].data_ptr(), self._stream()), "rp_embed_fwd")
         H, hd = cfg.n_heads, d // cfg.n_heads
         for i in range(cfg.n_blocks):
             a, x = self.act[i], self.x[i]
@@ -726,7 +771,12 @@ class SasRecEngine:
                            rowmask=self.last_pad if legacy else None)
                 return
             in_w, in_b = w("in_w"), f("in_b")
-            if self.fused_pre_attn:
+            if packed:
+                check(self.lib.rp_ln_qkv_fused_rows(x.data_ptr(), f("ln1_w").data_ptr(), f("ln1_b").data_ptr(), 1e-8,
+                                                    in_w.data_ptr(), in_b.data_ptr(), T, d, a["q_in"].data_ptr(), a["Q"].data_ptr(),
+                                                    a["KV"].data_ptr(), a["mean1"].data_ptr(), a["rstd1"].data_ptr(), hdv,
+                                                    self.n_rows.data_ptr(), self._stream()), "rp_ln_qkv_fused_rows")
+            elif self.fused_pre_attn:
                 check(self.lib.rp_ln_qkv_fused(x.data_ptr(), f("ln1_w").data_ptr(), f("ln1_b").data_ptr(), 1e-8,
                                                in_w.data_ptr(), in_b.data_ptr(), T, d, a["q_in"].data_ptr(), a["Q"].data_ptr(),
                                                a["KV"].data_ptr(), a["mean1"].data_ptr(), a["rstd1"].data_ptr(), hdv,
@@ -743,6 +793,17 @@ class SasRecEngine:
                                                   w("w1").data_ptr(), f("b1").data_ptr(), w("w2").data_ptr(), f("b2").data_ptr(),
                                                   pad.data_ptr() if legacy else None, T, d, self.x[i + 1].data_ptr(), hdv,
                                                   self._stream()), "rp_post_attn_fused")
+                continue
+            if packed:
+                check(self.lib.rp_post_attn_train_rows(a["O"].data_ptr(), a["q_in"].data_ptr(), w("out_w").data_ptr(),
+                                                       f("out_b").data_ptr(), f("ln2_w").data_ptr(), f("ln2_b").data_ptr(), 1e-8,
+                                                       w("w1").data_ptr(), f("b1").data_ptr(), w("w2").data_ptr(),
+                                                       f("b2").data_ptr(), T, d, drop, self.seed, self._site(i, 1) << 40,
+                                                       self._site(i, 2) << 40, self.rng_counter.data_ptr(), a["h"].data_ptr(),
+                                                       a["y"].data_ptr(), a["u"].data_ptr(), a["mean2"].data_ptr(),
+                                                       a["rstd2"].data_ptr(), self.x[i + 1].data_ptr(), hdv,
+                                                       self.n_rows.data_ptr(), self.row_tok.data_ptr(), self._stream()),
+                      "rp_post_attn_train_rows")
                 continue
             if training and d <= 128 and self.fused_post_attn_train:
                 # training: the same chain in one pass, saving h / y / u and the LayerNorm statistics for the backward
@@ -776,6 +837,8 @@ class SasRecEngine:
         desc.pad_mask = self.in_pad.data_ptr()
         desc.out, desc.ldo = self.act[i]["O"].data_ptr(), cfg.dp
         desc.drop_p, desc.seed, desc.drop_off, desc.seed_ptr = drop_p, self.seed, self._site(i, 0) << 40, self.rng_counter.data_ptr()
+        if self._packed:   # a packed training batch (set by _prepare; predict is never packed)
+            desc.seq_first, desc.seq_off = self.seq_first.data_ptr(), self.seq_off.data_ptr()
         return desc
 
     def _attention_forward(self, i: int, training: bool, q, k, v, causal: bool, mask_pad_keys: bool):
@@ -838,7 +901,7 @@ class SasRecEngine:
             return self.ce.loss
         self._prepare(True)
         self._body_forward(True)
-        self._final_norm_fwd(self.x[-1], self.hc, T, gather=self.valid_idx, n_rows_dev=self.n_valid)
+        self._final_norm_fwd(self.x[-1], self.hc, T, gather=self._target_rows(), n_rows_dev=self.n_valid)
         if self.sampled is not None:
             check(self.lib.rp_sampled_head_fwd(ctypes.byref(self._sampled_desc()), self._stream()), "rp_sampled_head_fwd")
             return self.ce.loss
@@ -901,7 +964,7 @@ class SasRecEngine:
         if self.sce is not None:
             self._final_norm_bwd(s["dhc"], self.x[-1], dx, T)
         else:
-            self._final_norm_bwd(s["dhc"], self.x[-1], dx, T, gather=self.valid_idx, n_rows_dev=self.n_valid)
+            self._final_norm_bwd(s["dhc"], self.x[-1], dx, T, gather=self._target_rows(), n_rows_dev=self.n_valid)
         return dx
 
     def backward(self):
@@ -912,6 +975,8 @@ class SasRecEngine:
         drop = cfg.dropout
         ks = 1.0 / (1.0 - drop) if drop > 0 else 1.0
         st = self._stream
+        packed = self._packed
+        rows = self.n_rows.data_ptr() if packed else None
         dx = self._head_backward()
         other = s["dxb"]
         for i in reversed(range(cfg.n_blocks)):
@@ -920,7 +985,17 @@ class SasRecEngine:
             f = lambda k: prm[f"b{i}.{k}"]  # noqa: E731
             g = lambda k: G[f"b{i}.{k}"]  # noqa: E731
             dz = dx
-            if self.fused_post_attn_bwd:
+            if packed:
+                check(self.lib.rp_post_attn_bwd_rows(dz.data_ptr(), a["u"].data_ptr(), a["h"].data_ptr(), a["mean2"].data_ptr(),
+                                                     a["rstd2"].data_ptr(), f("ln2_w").data_ptr(), w("w2").data_ptr(),
+                                                     w("w1").data_ptr(), w("out_w").data_ptr(), T, d, drop, self.seed,
+                                                     self._site(i, 2) << 40, self.rng_counter.data_ptr(),
+                                                     s["d_t"].data_ptr() if drop > 0 else None, s["du"].data_ptr(),
+                                                     s["dh"].data_ptr(), s["d_o"].data_ptr(), g("ln2_w").data_ptr(),
+                                                     g("ln2_b").data_ptr(), hdv, rows, self.row_tok.data_ptr(), st()),
+                      "rp_post_attn_bwd_rows")
+                d_t = s["d_t"] if drop > 0 else dz
+            elif self.fused_post_attn_bwd:
                 # one pass: d_t, du, dh (operands of the weight gradients), d_o (into the attention backward), dLN2
                 masked = legacy or drop > 0
                 check(self.lib.rp_post_attn_bwd(dz.data_ptr(), a["u"].data_ptr(), a["h"].data_ptr(), a["mean2"].data_ptr(),
@@ -952,7 +1027,12 @@ class SasRecEngine:
                                      causal=True, mask_pad_keys=not legacy)
             # ---- projections
             in_w = w("in_w")
-            if self.fused_pre_attn:
+            if packed:
+                check(self.lib.rp_pre_attn_bwd_rows(s["dQ"].data_ptr(), s["dKV"].data_ptr(), s["dh"].data_ptr(), x.data_ptr(),
+                                                    a["mean1"].data_ptr(), a["rstd1"].data_ptr(), f("ln1_w").data_ptr(),
+                                                    in_w.data_ptr(), T, d, other.data_ptr(), g("ln1_w").data_ptr(),
+                                                    g("ln1_b").data_ptr(), hdv, rows, st()), "rp_pre_attn_bwd_rows")
+            elif self.fused_pre_attn:
                 check(self.lib.rp_pre_attn_bwd(s["dQ"].data_ptr(), s["dKV"].data_ptr(), s["dh"].data_ptr(), x.data_ptr(),
                                                a["mean1"].data_ptr(), a["rstd1"].data_ptr(), f("ln1_w").data_ptr(),
                                                in_w.data_ptr(), T, d, other.data_ptr(), g("ln1_w").data_ptr(),
@@ -965,13 +1045,19 @@ class SasRecEngine:
             pairs = [(d_t, a["u"], g("w2"), g("b2")), (s["du"], a["y"], g("w1"), g("b1")), (s["dh"], a["O"], g("out_w"), g("out_b")),
                      (s["dQ"], a["q_in"], g("in_w")[:d], g("in_b")[:d]), (s["dKV"], x, g("in_w")[d:], g("in_b")[d:])]
             if self.fused_wgrad:
-                self._wgrad_group(pairs)
+                self._wgrad_group(pairs, self.n_rows if packed else None)
             else:
                 for dY, X, dW, _ in pairs:
                     self._wgrad(dY, X, dW, *dW.shape)
                 self._colsum_multi([(dY, db) for dY, _, _, db in pairs])
             dx, other = other, dx
         pos0 = 0 if legacy else cfg.max_len - L
+        if packed:
+            check(self.lib.rp_embed_bwd_rows(dx.data_ptr(), self.ids32.data_ptr(), self.in_pad.data_ptr(), self.row_tok.data_ptr(),
+                                             rows, self.seq_first.data_ptr(), self.seq_off.data_ptr(), self.B, L, d, cfg.pad_id,
+                                             pos0, math.sqrt(cfg.d), 0, drop, self.seed, 0, self.rng_counter.data_ptr(),
+                                             G["item_emb"].data_ptr(), G["pos_emb"].data_ptr(), st()), "rp_embed_bwd_rows")
+            return
         check(self.lib.rp_embed_bwd(dx.data_ptr(), self.ids32.data_ptr(), self.in_pad.data_ptr(), self.B, L, d, cfg.pad_id,
                                     pos0, math.sqrt(cfg.d), int(legacy), drop, self.seed, 0, self.rng_counter.data_ptr(),
                                     G["item_emb"].data_ptr(), G["pos_emb"].data_ptr(), st()), "rp_embed_bwd")

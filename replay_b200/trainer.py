@@ -27,6 +27,9 @@ class Trainer:
         # the engine's gradient sits in a symmetric allocation: the exchange is rp_peer_allreduce, a kernel of the step graph
         self.peer = getattr(engine, "peer", None) if self.world > 1 else None
         self.betas = tuple(betas)
+        # the step reads only the loss and the gradients, so the body runs on packed rows where that is exact
+        # (SasRecEngine.packed_eligible); RP_PACKED_BODY=0 keeps the padded rows for A/B runs
+        engine.packed_body = os.environ.get("RP_PACKED_BODY", "1") != "0"
         self.launches_per_step = None
         self.invalidate()
 
