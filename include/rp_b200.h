@@ -304,7 +304,9 @@ int rp_colsum_multi(int n, const void* const* dy, const int* cols, const long lo
 /* torch.optim.Adam (models/nn/optimizer_utils/optimizer_factory.py:71-87; no weight decay) on flat fp32 buffers; refreshes
  * the bf16 shadow, optionally zeroes the gradient; lr and the step counter live in device memory. */
 /* BERT4Rec embedding: where(token_mask, table[ids], mask_emb) + pos[t % L] (bert4rec/model.py:239-296) and its backward;
- * row gather / scatter with a device-side row count (dst[r] = src[idx[r]] or dst[idx[r]] = src[r]). */
+ * row gather / scatter with a device-side row count (dst[r] = src[idx[r]] or dst[idx[r]] = src[r]).
+ * pos == NULL (forward) / d_pos == NULL (backward): the model has no positional embedding (enable_positional_embedding
+ * = False); the forward adds no positional term and the backward skips the positional column sums. */
 int rp_bert_embed_fwd(const void* table, const void* mask_emb, const float* pos, const int32_t* ids, const uint8_t* tok_mask,
                       int T, int L, int d, float drop_p, unsigned long long seed, unsigned long long drop_off,
                       const unsigned long long* seed_ptr, void* out, void* stream);

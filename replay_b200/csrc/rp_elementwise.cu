@@ -139,10 +139,13 @@ __global__ void embed_fwd_kernel(const __nv_bfloat16* __restrict__ table, const 
       for (int i = 0; i < VEC; i += 2) ev[k][i >> 1] = *reinterpret_cast<const __nv_bfloat162*>(e + i);
     }
     float pv[VEC];
-    {
+    if (pos) {
       const float* p = pos + (size_t)(pos0 + pidx) * D + lane * VEC;
 #pragma unroll
       for (int i = 0; i < VEC; ++i) pv[i] = p[i];
+    } else {  // BERT4Rec without positional embedding (bert4rec/model.py:289-291): x = where(token_mask, E[ids], mask_emb)
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) pv[i] = 0.f;
     }
 #pragma unroll
     for (int k = 0; k < TOK; ++k) {
@@ -1033,7 +1036,8 @@ RP_API int rp_bert_embed_fwd(const void* table, const void* mask_emb, const floa
                              const uint8_t* tok_mask, int T, int L, int d, float drop_p, unsigned long long seed,
                              unsigned long long drop_off, const unsigned long long* seed_ptr, void* out, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!table || !mask_emb || !pos || !ids || !tok_mask || !out || T <= 0 || L <= 0) return RP_EINVAL;
+  // pos == null: no positional term (enable_positional_embedding=False)
+  if (!table || !mask_emb || !ids || !tok_mask || !out || T <= 0 || L <= 0) return RP_EINVAL;
   if (T % L != 0) return RP_ESHAPE;
   const int grid = grid_for(T, 8);
   RP_DISPATCH_D(d, (embed_fwd_kernel<VEC><<<grid, 256, 0, stream>>>(
@@ -1048,14 +1052,15 @@ RP_API int rp_bert_embed_bwd(const void* dx, const int32_t* ids, const uint8_t* 
                              const unsigned long long* seed_ptr, float* d_table, float* d_mask_emb, float* d_pos,
                              void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!dx || !ids || !pad_mask || !tok_mask || !d_table || !d_mask_emb || !d_pos || B <= 0 || L <= 0) return RP_EINVAL;
+  // d_pos == null: the model has no positional table, and its column-sum pass is skipped
+  if (!dx || !ids || !pad_mask || !tok_mask || !d_table || !d_mask_emb || B <= 0 || L <= 0) return RP_EINVAL;
   const int T = B * L;
   const int grid = grid_for(T, 8);
   RP_DISPATCH_D(d, (embed_bwd_table_kernel<VEC><<<grid, 256, 0, stream>>>(
                        reinterpret_cast<const __nv_bfloat16*>(dx), ids, pad_mask, T, -1, 1.f, 0, drop_p, seed, drop_off, seed_ptr,
                        tok_mask, d_mask_emb, d_table)));
   RP_LAUNCH_CHECK();
-  {
+  if (d_pos) {
     const int rlanes = 256 / (d / 4);
     int G = (B + 31) / 32;
     if (G < 1) G = 1;

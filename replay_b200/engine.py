@@ -66,6 +66,11 @@ class BaseConfig:
         return self.n_heads * self.head_slot
 
     @property
+    def n_apps(self) -> int:
+        """block applications of one body pass: each has its own activations and dropout sites (BertConfig repeats blocks)"""
+        return self.n_blocks
+
+    @property
     def hd_valid(self) -> int:
         """the kernels' `hd_valid` argument: real features per slot, 0 when nothing is padded"""
         return 0 if self.head_dim == self.head_slot else self.head_dim
@@ -382,9 +387,10 @@ class SasRecEngine:
         self.n_rows = torch.zeros(1, **i32)
         self.row_tok = torch.zeros(T, **i32)
         self.valid_rows = torch.zeros(T, **i32)
-        self.x = [torch.zeros(T, d, **bf) for _ in range(cfg.n_blocks + 1)]
+        # hidden states and saved activations per block APPLICATION (cfg.n_apps; the same as n_blocks unless blocks repeat)
+        self.x = [torch.zeros(T, d, **bf) for _ in range(cfg.n_apps + 1)]
         self.act = []
-        for _ in range(cfg.n_blocks):
+        for _ in range(cfg.n_apps):
             a = {k: torch.zeros(T, **f32) for k in ("mean1", "rstd1", "mean2", "rstd2")}
             a["O"] = torch.zeros(T, d, **bf)
             if self.with_grad:
@@ -549,8 +555,9 @@ class SasRecEngine:
                                         None if add_to is None else add_to.data_ptr(), dx.data_ptr(), dw.data_ptr(),
                                         db.data_ptr(), self.cfg.hd_valid, self._stream()), "rp_layernorm_bwd")
 
-    def _site(self, blk, k):
-        return 1 + blk * 8 + k
+    def _site(self, app, k):
+        """dropout site k of block application ``app`` (offset ``site << 40``; the embedding is site 0)"""
+        return 1 + app * 8 + k
 
     # ------------------------------------------------------------------------------------------------ forward
     def set_batch(self, ids, pad_mask, labels=None, target_mask=None):

@@ -19,6 +19,25 @@ class BertConfig(BaseConfig):
     pad_id: int = 0  # TensorFeatureInfo.padding_value: a VALID row for BERT4Rec (the table has |I| rows, no pad row)
     variant: str = "bert4rec"
     lnf_eps: float = 1e-5
+    # num_passes_over_block: block i runs `passes` times in a row with its own weights (bert4rec/model.py:139-141); 0 applies
+    # no block at all, as the reference's range(0) does
+    passes: int = 1
+    positional: bool = True   # enable_positional_embedding: the learned position table pos_emb [max_len, d]
+
+    def __post_init__(self):
+        if int(self.passes) != self.passes or self.passes < 0:
+            raise ValueError(f"num_passes_over_block must be a non-negative integer, got {self.passes}")
+        super().__post_init__()
+        if 1 + 8 * self.n_apps >= 1 << 24:   # a dropout site's offset is site << 40 in a 64-bit counter
+            raise ValueError(f"{self.n_blocks} blocks x {self.passes} passes exceed the dropout sites' numbering")
+
+    @property
+    def n_apps(self) -> int:
+        """block applications of one body pass: application a runs block a // passes"""
+        return self.n_blocks * self.passes
+
+    def block_of(self, app: int) -> int:
+        return app // self.passes
 
     # ---- the feature slots of BaseConfig; the FFN's inner axis (4d) has no head structure: its true units take the leading
     # columns and the width is rounded up to whole 128-column tiles.  The reference tutorial's hidden 300 / 4 heads
@@ -40,7 +59,9 @@ class BertConfig(BaseConfig):
 
     def param_layout(self) -> list:
         d, I, emb = self.dp, self.n_items, (None, "f")
-        out = [("item_emb", (I, d), emb), ("mask_emb", (1, d), emb), ("pos_emb", (self.max_len, d), emb)]
+        out = [("item_emb", (I, d), emb), ("mask_emb", (1, d), emb)]
+        if self.positional:
+            out.append(("pos_emb", (self.max_len, d), emb))
         for i in range(self.n_blocks):
             out += self._block_layout(i, self.ffn_p, "i")
         if not self.tying:
@@ -99,13 +120,16 @@ class Bert4RecEngine(SasRecEngine):
         p16, prm = self.params16, self.params
         drop = cfg.dropout if training else 0.0
         rng = self.rng_counter.data_ptr()
-        check(self.lib.rp_bert_embed_fwd(p16["item_emb"].data_ptr(), p16["mask_emb"].data_ptr(), prm["pos_emb"].data_ptr(),
+        pos = prm["pos_emb"].data_ptr() if cfg.positional else None
+        check(self.lib.rp_bert_embed_fwd(p16["item_emb"].data_ptr(), p16["mask_emb"].data_ptr(), pos,
                                          self.ids32.data_ptr(), self.in_tok.data_ptr(), T, L, d, drop, self.seed, 0, rng,
                                          self.x[0].data_ptr(), self._stream()), "rp_bert_embed_fwd")
-        for i in range(cfg.n_blocks):
-            a, x = self.act[i], self.x[i]
-            w = lambda k: p16[f"b{i}.{k}"]  # noqa: E731
-            f = lambda k: prm[f"b{i}.{k}"]  # noqa: E731
+        # application i runs block cfg.block_of(i): activations, saved statistics and dropout sites are per application,
+        # weights per block
+        for i in range(cfg.n_apps):
+            a, x, blk = self.act[i], self.x[i], cfg.block_of(i)
+            w = lambda k: p16[f"b{blk}.{k}"]  # noqa: E731
+            f = lambda k: prm[f"b{blk}.{k}"]  # noqa: E731
             self._ln_fwd(x, f("ln1_w"), f("ln1_b"), 1e-5, a["xn"], a["mean1"], a["rstd1"], T)
             self._gemm(a["xn"], w("in_w"), a["QKV"], T, 3 * d, d, bias=f("in_b"))
             QKV = a["QKV"]
@@ -170,11 +194,14 @@ class Bert4RecEngine(SasRecEngine):
                 return dst
             return src
 
-        for i in reversed(range(cfg.n_blocks)):
-            a, x = self.act[i], self.x[i]
-            w = lambda k: p16[f"b{i}.{k}"]  # noqa: E731
-            f = lambda k: prm[f"b{i}.{k}"]  # noqa: E731
-            g = lambda k: G[f"b{i}.{k}"]  # noqa: E731
+        # applications in reverse; each one ADDS its weight, bias and LayerNorm gradients into its block's (_wgrad reduces
+        # into dW with +=, rp_colsum and rp_layernorm_bwd accumulate into db / dw), so a repeated block gets the sum over
+        # its passes
+        for i in reversed(range(cfg.n_apps)):
+            a, x, blk = self.act[i], self.x[i], cfg.block_of(i)
+            w = lambda k: p16[f"b{blk}.{k}"]  # noqa: E731
+            f = lambda k: prm[f"b{blk}.{k}"]  # noqa: E731
+            g = lambda k: G[f"b{blk}.{k}"]  # noqa: E731
             dz = dbwd(dx, s["dz"], self._site(i, 4))          # x_next = drop(z)
             d_t = dbwd(dz, s["d_t"], self._site(i, 3))        # z = y + drop(u W2^T + b2)
             self._wgrad(d_t, a["u"], g("w2"), d, F)
@@ -203,7 +230,8 @@ class Bert4RecEngine(SasRecEngine):
             dx, other = other, dx
         check(self.lib.rp_bert_embed_bwd(dx.data_ptr(), self.ids32.data_ptr(), self.in_pad.data_ptr(), self.in_tok.data_ptr(),
                                          self.B, L, d, drop, self.seed, 0, rng, G["item_emb"].data_ptr(),
-                                         G["mask_emb"].data_ptr(), G["pos_emb"].data_ptr(), st()), "rp_bert_embed_bwd")
+                                         G["mask_emb"].data_ptr(), G["pos_emb"].data_ptr() if cfg.positional else None, st()),
+              "rp_bert_embed_bwd")
 
     # ------------------------------------------------------------------------------------------------ inference
     def forward_last_hidden(self):

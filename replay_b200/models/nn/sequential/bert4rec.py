@@ -17,10 +17,12 @@ _BLEAF = {"ln1_w": "attention_norm.weight", "ln1_b": "attention_norm.bias", "in_
           "w2": "pff.w_2.weight", "b2": "pff.w_2.bias"}
 
 
-def bert_key_map(n_blocks: int, tying: bool, item_feature: str = "item_id") -> dict:
-    """engine parameter name -> reference state_dict key (SURVEY.md Appendix B)."""
-    m = {"item_emb": f"item_embedder.cat_embeddings.{item_feature}.weight", "mask_emb": "item_embedder.mask_embedding.weight",
-         "pos_emb": "item_embedder.position.pe.weight"}
+def bert_key_map(n_blocks: int, tying: bool, item_feature: str = "item_id", positional: bool = True) -> dict:
+    """engine parameter name -> reference state_dict key (SURVEY.md Appendix B).  Without the positional embedding the
+    reference registers no ``item_embedder.position`` module (bert4rec/model.py:236-237), so there is no pos_emb key."""
+    m = {"item_emb": f"item_embedder.cat_embeddings.{item_feature}.weight", "mask_emb": "item_embedder.mask_embedding.weight"}
+    if positional:
+        m["pos_emb"] = "item_embedder.position.pe.weight"
     for i in range(n_blocks):
         for k in _BLOCK_PARAMS:
             m[f"b{i}.{k}"] = f"transformer_blocks.{i}." + _BLEAF[k]
@@ -56,7 +58,7 @@ def shift_features(ids, pad_mask, token_mask, pad_value: int = 0):
 
 class _BertCore(SasRecCore):
     def _key_map(self):
-        return bert_key_map(self.cfg.n_blocks, self.cfg.tying, self.item_feature)
+        return bert_key_map(self.cfg.n_blocks, self.cfg.tying, self.item_feature, self.cfg.positional)
 
     def _initial_seq_len(self):
         return self.cfg.max_len
@@ -116,6 +118,31 @@ class _BertCore(SasRecCore):
         return eng.forward_last_hidden()[: ids.shape[0]]
 
     @torch.no_grad()
+    def hidden_states(self, ids, pad_mask, token_mask):
+        """eval-mode hidden states of every position at the model's true hidden size, bf16 [B, L, d]"""
+        B, L = ids.shape
+        eng = self.ensure_engine(B, L, with_grad=self.engine.with_grad if self.engine is not None else False)
+        if self._shadow_dirty:
+            eng.refresh_shadow(); self._shadow_dirty = False
+        eng.set_batch(ids, pad_mask, token_mask)
+        return eng.unpad_features(eng.forward_hidden_all().view(eng.B, L, -1)[:B])
+
+    @torch.no_grad()
+    def head_logits(self, h, item_ids=None):
+        """Biased head scores fp32 [N, |I|] (or [N, |item_ids|]) of hidden rows ``h`` [N, d] at the true hidden size."""
+        eng = self.engine
+        if self._shadow_dirty:
+            eng.refresh_shadow(); self._shadow_dirty = False
+        hp = eng.pad_features(h.to(torch.bfloat16)).contiguous()
+        W, b = eng.head_for_scoring()
+        b = b[: self.cfg.n_items]
+        if item_ids is not None:
+            W, b = W[item_ids].contiguous(), b[item_ids].contiguous()
+        out = torch.empty(hp.shape[0], W.shape[0], device=hp.device, dtype=torch.float32)
+        eng._gemm(hp, W, out, hp.shape[0], W.shape[0], self.cfg.dp, out_mode=2, bias=b)
+        return out
+
+    @torch.no_grad()
     def query_embeddings(self, ids, pad_mask, token_mask):
         """bf16 [B, d] at the model's true hidden size"""
         return self.engine.unpad_features(self._query_padded(ids, pad_mask, token_mask))
@@ -154,12 +181,14 @@ class Bert4RecModel(torch.nn.Module):
                  num_passes_over_block: int = 1, dropout: float = 0.1, enable_positional_embedding: bool = True,
                  enable_embedding_tying: bool = False, device=None, seed: int = 0):
         super().__init__()
-        if num_passes_over_block != 1 or not enable_positional_embedding:
-            raise NotImplementedError("only the reference defaults (one pass per block, positional embedding) are built")
         name, card, pad, _ = item_feature_of(schema)
         self.schema, self.item_feature_name, self.item_count, self.max_len = schema, name, card, max_len
+        self.hidden_size, self.num_blocks, self.num_heads, self.dropout = hidden_size, num_blocks, num_heads, dropout
+        self.num_passes_over_block = num_passes_over_block
+        self.enable_positional_embedding, self.enable_embedding_tying = enable_positional_embedding, enable_embedding_tying
         cfg = BertConfig(n_items=card, d=hidden_size, n_heads=num_heads, n_blocks=num_blocks, max_len=max_len, dropout=dropout,
-                         tying=enable_embedding_tying, pad_id=pad if 0 <= pad < card else 0)
+                         tying=enable_embedding_tying, pad_id=pad if 0 <= pad < card else 0, passes=num_passes_over_block,
+                         positional=bool(enable_positional_embedding))
         self.core = _BertCore(cfg, item_feature=name, device=device, seed=seed)
 
     def state_dict(self, *a, **k):
@@ -170,6 +199,65 @@ class Bert4RecModel(torch.nn.Module):
 
     def get_query_embeddings(self, inputs, pad_mask, token_mask):
         return self.core.query_embeddings(inputs[self.item_feature_name], pad_mask, token_mask).float()
+
+    # ---- inference-only restatements of the reference's forward / forward_step / get_logits (bert4rec/model.py:86-157)
+    def forward_step(self, inputs, pad_mask, token_mask):
+        """Hidden states of every position, fp32 [B, L, d] (eval mode: no dropout)."""
+        return self.core.hidden_states(inputs[self.item_feature_name], pad_mask, token_mask).float()
+
+    def get_logits(self, out_embeddings, item_ids=None):
+        """Biased head scores of hidden states [..., d]: [..., |I|], or [..., |item_ids|]."""
+        h = out_embeddings.reshape(-1, out_embeddings.shape[-1])
+        out = self.core.head_logits(h, item_ids)
+        return out.view(*out_embeddings.shape[:-1], out.shape[-1])
+
+    def forward(self, inputs, pad_mask, token_mask):
+        """All-position scores [B, L, |I|] - materialised; use only for small problems."""
+        return self.get_logits(self.forward_step(inputs, pad_mask, token_mask))
+
+    # ---- catalog growth
+    def _weights(self) -> dict:
+        """reference-keyed copies of every weight (materialises the seeded initial ones on first use)"""
+        if self.core.engine is None and not self.core._pending_state:
+            self.core.ensure_engine(1, self.max_len, with_grad=False)
+        return {k: v.detach().clone() for k, v in self.core.state_dict().items()}
+
+    def get_all_embeddings(self) -> dict:
+        """Copies of the item table [I, d] and, when it is on, the position table [max_len, d] (model.py:298-312)."""
+        sd = self._weights()
+        out = {"item_embedding": sd[f"item_embedder.cat_embeddings.{self.item_feature_name}.weight"]}
+        if self.enable_positional_embedding:
+            out["positional_embedding"] = sd["item_embedder.position.pe.weight"]
+        return out
+
+    def resize_items(self, table: torch.Tensor):
+        """Rebuild for the catalog of ``table`` [I', d] (I' >= I), keeping every other weight (lightning.py:612-627): the
+        head keeps its first I rows and bias entries and takes fresh ones for the new items - ``Linear(hidden, I')``'s
+        default initialisation untied, N(0, 0.01) bias entries tied.  The new core starts with fresh Adam moments, as the
+        reference's newly created parameters do, and without captured graphs; the loss, the Adam betas, the passes and the
+        positional setting carry over."""
+        import dataclasses
+
+        old, n_new = self.core, int(table.shape[0])
+        sd = {k: v.float().cpu() for k, v in self._weights().items()}
+        n_old, d = self.item_count, self.hidden_size
+        sd[f"item_embedder.cat_embeddings.{self.item_feature_name}.weight"] = table.detach().float().cpu()
+        if self.enable_embedding_tying:
+            bias = torch.empty(n_new).normal_(0, 0.01)
+            bias[:n_old] = sd["_head.out_bias"]
+            sd["_head.out_bias"] = bias
+        else:
+            lin = torch.nn.Linear(d, n_new)
+            w, b = lin.weight.detach().clone(), lin.bias.detach().clone()
+            w[:n_old], b[:n_old] = sd["_head.linear.weight"], sd["_head.linear.bias"]
+            sd["_head.linear.weight"], sd["_head.linear.bias"] = w, b
+        old._drop_graphs()
+        core = _BertCore(dataclasses.replace(old.cfg, n_items=n_new), item_feature=self.item_feature_name, device=old._device,
+                         seed=old._seed)
+        core.loss_kind, core.adam_betas = old.loss_kind, tuple(old.adam_betas)
+        core.load_state_dict(sd)
+        self.core = core
+        self.item_count = n_new
 
     def predict(self, inputs, pad_mask, token_mask, candidates_to_score=None):
         return self.core.logits(inputs[self.item_feature_name], pad_mask, token_mask, candidates_to_score)
@@ -193,6 +281,7 @@ class Bert4Rec(LightningModuleBase):
                                     enable_embedding_tying=enable_embedding_tying, device=device)
         self._model.core.loss_kind = kind
         self._schema = tensor_schema
+        self._vocab_size = self._model.item_count
         self._optimizer_factory, self._lr_scheduler_factory = optimizer_factory, lr_scheduler_factory
         self._candidates_to_score = None
         self.fused_optimizer = fused_optimizer
@@ -280,6 +369,61 @@ class Bert4Rec(LightningModuleBase):
         opt = self._optimizer_factory.create(params) if self._optimizer_factory is not None else torch.optim.Adam(
             params, lr=1e-3, betas=(0.9, 0.98))
         return opt if self._lr_scheduler_factory is None else ([opt], [self._lr_scheduler_factory.create(opt)])
+
+    # ---- catalog growth for fine-tuning on new items (bert4rec/lightning.py:501-628)
+    def get_all_embeddings(self) -> dict:
+        return self._model.get_all_embeddings()
+
+    def _embedding_dim(self) -> int:
+        dim = item_feature_of(self._model.schema)[3]
+        return self._model.hidden_size if dim is None else int(dim)
+
+    def _set_new_item_table(self, table: torch.Tensor):
+        self._model.resize_items(table)
+        self._vocab_size = self._model.item_count
+        feats = self._schema.item_id_features
+        feat = feats.item() if hasattr(feats, "item") else feats[self._schema.item_id_feature_name]
+        feat._set_cardinality(self._vocab_size)
+
+    def set_item_embeddings_by_size(self, new_vocab_size: int):
+        """Keep the fitted item embeddings and add xavier-normal rows (drawn over the whole new table) for the new items."""
+        if new_vocab_size <= self._vocab_size:
+            raise ValueError("New vocabulary size must be greater then already fitted")
+        new = torch.empty(new_vocab_size, self._embedding_dim())
+        torch.nn.init.xavier_normal_(new)
+        new[: self._vocab_size] = self.get_all_embeddings()["item_embedding"]
+        self._set_new_item_table(new)
+
+    def set_item_embeddings_by_tensor(self, all_item_embeddings: torch.Tensor):
+        """Replace the whole item table, possibly with more items."""
+        if all_item_embeddings.dim() != 2:
+            raise ValueError("Input tensor must have (number of all items, model hidden size) shape")
+        if all_item_embeddings.shape[0] < self._vocab_size:
+            raise ValueError("New vocabulary size can't be less then already fitted")
+        if all_item_embeddings.shape[1] != self._embedding_dim():
+            raise ValueError("Input tensor second dimension doesn't match embedding dim")
+        self._set_new_item_table(all_item_embeddings.detach().float().cpu())
+
+    def append_item_embeddings(self, item_embeddings: torch.Tensor):
+        """Append rows for new items only."""
+        if item_embeddings.dim() != 2:
+            raise ValueError("Input tensor must have (number of all items, model hidden size) shape")
+        if item_embeddings.shape[1] != self._embedding_dim():
+            raise ValueError("Input tensor second dimension doesn't match embedding dim")
+        new = torch.cat([self.get_all_embeddings()["item_embedding"].cpu(), item_embeddings.detach().float().cpu()])
+        self._set_new_item_table(new)
+
+    @property
+    def optimizer_factory(self):
+        return self._optimizer_factory
+
+    @optimizer_factory.setter
+    def optimizer_factory(self, optimizer_factory):
+        if not hasattr(optimizer_factory, "create"):  # lightning.py:614-626 (isinstance check against OptimizerFactory)
+            raise ValueError(f"Expected optimizer_factory of type OptimizerFactory, got {type(optimizer_factory)}")
+        self._optimizer_factory = optimizer_factory
+        self._lr = getattr(optimizer_factory, "learning_rate", 1e-3)
+        self._model.core.adam_betas = tuple(getattr(optimizer_factory, "betas", (0.9, 0.98)))
 
     @property
     def candidates_to_score(self):
