@@ -425,12 +425,17 @@ int rp_counter_add(unsigned long long* counter, unsigned long long inc, void* st
  *   replaces  SampledLossBase.get_sampled_logits + mask_negative_logits   replay/nn/loss/base.py:40-154,157-196
  *             CESampled.forward / BCESampled.forward                      replay/nn/loss/ce.py:199-249 ; bce.py:154-218
  *             legacy _compute_loss_ce_sampled / _compute_loss_bce_sampled  replay/models/nn/sequential/sasrec/lightning.py:310-376
+ *             LogInCESampled.forward / CESampledWeighted.forward           replay/nn/loss/login_ce.py:240-375 ; ce.py:252-330
  * hc / labels / n_valid as for rp_ce_head_fwd (compacted valid targets).  negatives int64: neg_mode 0 = [n_neg] shared by the
  * batch (tensor-core path), 1 = [B*seq_len, n_neg] per position, 2 = [B, n_neg] per sequence (1, 2: rows addressed through
  * valid_idx[t] = flat b*seq_len + l of compacted row t; gather-dot kernels).  kind: RP_LOSS_CE_SAMPLED (negatives equal to the
  * positive or to ignore_index get logit -1e9), RP_LOSS_BCE_SAMPLED (same masking, log_eps / clamp as the reference),
  * RP_LOSS_LEGACY_CE_SAMPLED (log(vocab_size-1) - 1e6*reject - log(min(n_neg, vocab_size) - #reject) correction),
- * RP_LOSS_LEGACY_BCE_SAMPLED (no masking).  One positive per position.  fwd: loss_out[0] = mean loss, loss_out[1] = 1/T_v,
+ * RP_LOSS_LEGACY_BCE_SAMPLED (no masking), RP_LOSS_LOGIN_CE_SAMPLED (CE_SAMPLED's masking and softmax over [positive |
+ * negatives]; -clamp(log(p + log_eps), -clamp, clamp) of the positive's share p, gradient 0 where the clamp is active),
+ * RP_LOSS_CE_SAMPLED_WEIGHTED (CE_SAMPLED's row loss times row_weight[t]; mean over the valid targets, not divided by the
+ * weights' sum).  row_weight: fp32 [capacity] in the compacted row order, required (RP_EINVAL) by RP_LOSS_CE_SAMPLED_WEIGHTED
+ * and ignored by every other kind.  One positive per position.  fwd: loss_out[0] = mean loss, loss_out[1] = 1/T_v,
  * d(loss)/d(logits) stays in the workspace (which need not be zeroed); bwd: d_hc bf16 [capacity, d] rows < *n_valid, d_table
  * fp32 ACCUMULATED (+=: zero it first; rows that no positive and no unmasked negative points at are left as they were).
  * d_hc rows >= *n_valid: untouched with per-row negatives; with shared negatives rows [*n_valid, min(round_up(*n_valid, 128),
@@ -440,6 +445,8 @@ int rp_counter_add(unsigned long long* counter, unsigned long long inc, void* st
 #define RP_LOSS_BCE_SAMPLED 1
 #define RP_LOSS_LEGACY_CE_SAMPLED 2
 #define RP_LOSS_LEGACY_BCE_SAMPLED 3
+#define RP_LOSS_LOGIN_CE_SAMPLED 4
+#define RP_LOSS_CE_SAMPLED_WEIGHTED 5
 typedef struct rp_sampled_desc {
   const void* hc; const void* table; const int32_t* labels; const int32_t* valid_idx; const int64_t* negatives;
   const int32_t* n_valid;
@@ -447,6 +454,7 @@ typedef struct rp_sampled_desc {
   float log_eps, clamp;
   float* loss_out;
   void* workspace; size_t workspace_bytes;
+  const float* row_weight;
 } rp_sampled_desc;
 size_t rp_sampled_head_workspace(int capacity, int d, int n_neg, int neg_mode);
 int rp_sampled_head_fwd(const rp_sampled_desc* s, void* stream);

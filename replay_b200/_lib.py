@@ -149,6 +149,7 @@ class SampledDesc(ctypes.Structure):
         ("log_eps", c_float), ("clamp", c_float),
         ("loss_out", c_void_p),
         ("workspace", c_void_p), ("workspace_bytes", c_size_t),
+        ("row_weight", c_void_p),
     ]
 
 

@@ -204,6 +204,7 @@ class SasRecCore(torch.nn.Module):
                 self.engine.set_loss(kind, **kw)
 
     _FULL_CATALOG = ("ce", "ce_weighted", "login_ce", "bce", "sce")   # heads that take no negatives
+    _WEIGHTED = ("ce_weighted", "ce_sampled_weighted")                # heads that read per-row sample weights
 
     def _stage(self, eng, ids, pad_mask, labels, target_mask, negatives, row_weights=None):
         spec = getattr(self, "_loss_spec", ("ce", {}))
@@ -212,7 +213,7 @@ class SasRecCore(torch.nn.Module):
                 eng.set_loss(spec[0], **spec[1])
                 eng._loss_applied = (spec[0], tuple(sorted(spec[1].items())))
             eng.set_batch(ids, pad_mask, labels, target_mask)
-            if spec[0] == "ce_weighted":
+            if spec[0] in self._WEIGHTED:
                 if row_weights is None:
                     raise ValueError("this loss needs the sample weights of the batch")
                 eng.set_row_weights(row_weights)
@@ -230,6 +231,10 @@ class SasRecCore(torch.nn.Module):
             if negatives is None:
                 raise ValueError("this loss needs negative_labels")
             eng.set_negatives(negatives)
+        if spec[0] in self._WEIGHTED:
+            if row_weights is None:
+                raise ValueError("this loss needs the sample weights of the batch")
+            eng.set_row_weights(row_weights)
 
     # ---- training / inference on [B, L] batches
     def loss(self, ids, pad_mask, labels, target_mask, negatives=None, row_weights=None) -> torch.Tensor:

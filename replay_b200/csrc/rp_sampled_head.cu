@@ -3,6 +3,8 @@
 //   SampledLossBase.get_sampled_logits + mask_negative_logits      replay/nn/loss/base.py:40-154,157-196
 //   CESampled.forward                                             replay/nn/loss/ce.py:199-249
 //   BCESampled.forward                                            replay/nn/loss/bce.py:154-218
+//   LogInCESampled.forward                                        replay/nn/loss/login_ce.py:240-375
+//   CESampledWeighted.forward                                     replay/nn/loss/ce.py:252-330
 //   legacy _compute_loss_ce_sampled / _compute_loss_bce_sampled    replay/models/nn/sequential/sasrec/lightning.py:310-376
 // (single positive per position; the negatives are an INPUT, as in the reference's new path).
 //
@@ -18,7 +20,7 @@
 
 namespace rp {
 
-enum { kCESampled = 0, kBCESampled = 1, kLegacyCE = 2, kLegacyBCE = 3 };
+enum { kCESampled = 0, kBCESampled = 1, kLegacyCE = 2, kLegacyBCE = 3, kLogInCESampled = 4, kCESampledWeighted = 5 };
 
 struct SampledArgs {
   const __nv_bfloat16* hc;
@@ -27,6 +29,7 @@ struct SampledArgs {
   const int32_t* valid_idx;
   const int64_t* negatives;
   const int32_t* n_valid;
+  const float* row_weight;  // [capacity] sample weight of each compacted row (kCESampledWeighted only)
   int capacity, n_items, d, N, neg_mode, L, kind, ignore_index, vocab_size;
   float log_eps, clamp;
   float* loss_out;
@@ -109,8 +112,8 @@ __global__ void sampled_loss_kernel(const SampledArgs a) {
   // workspace cannot reach dE_neg as 0 x NaN
   const int t_end = a.neg_mode == 0 ? ((n_valid + 127) / 128) * 128 : n_valid;
   const int n_neg_drawn = min(a.N, a.vocab_size);   // legacy CE: the reference corrects by min(N, vocab_size) - #reject
-  const bool ce = a.kind == kCESampled || a.kind == kLegacyCE;
-  const bool masked = a.kind == kCESampled || a.kind == kBCESampled;
+  const bool ce = a.kind == kCESampled || a.kind == kLegacyCE || a.kind == kLogInCESampled || a.kind == kCESampledWeighted;
+  const bool masked = a.kind == kCESampled || a.kind == kBCESampled || a.kind == kLogInCESampled || a.kind == kCESampledWeighted;
   float local = 0.f;
   for (int t = blockIdx.x * wpb + (threadIdx.x >> 5); t < t_end; t += gridDim.x * wpb) {
     float* zr = a.zneg + (size_t)t * a.ldz;
@@ -147,17 +150,34 @@ __global__ void sampled_loss_kernel(const SampledArgs a) {
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
       const float ep = __expf(zp - mx);
+      const float s_neg = s;
       s += ep;
       const float lse = mx + logf(s);
       const float inv_s = 1.f / s;
+      // every CE kind's gradient is wg * (softmax - onehot) / T_v with a per-row factor wg (1 for CE / legacy CE)
+      float row_loss = lse - zp, wg = 1.f, dpos = ep * inv_s - 1.f;
+      if (a.kind == kCESampledWeighted) {
+        // (row CE * w_t).mean() over the valid targets (replay/nn/loss/ce.py:252-330)
+        wg = a.row_weight[t];
+        row_loss *= wg;
+      } else if (a.kind == kLogInCESampled) {
+        // -clamp(log(p + eps), -c, c) of the positive's softmax share p: d/dz = p / (p + eps) x the CE gradient inside the
+        // clamp, 0 outside (same edge rule as the catalog LogInCE); 1 - p from the negatives' sum, not from p
+        const float p = ep * inv_s;
+        const float lg = logf(p + a.log_eps);
+        row_loss = -fminf(fmaxf(lg, -a.clamp), a.clamp);
+        wg = (lg > -a.clamp && lg < a.clamp) ? p / (p + a.log_eps) : 0.f;
+        dpos = -s_neg * inv_s;
+      }
+      const float gs = wg * inv_n;
       for (int j = lane; j < a.N; j += 32) {
-        const float g = __expf(zr[j] - mx) * inv_s * inv_n;
+        const float g = __expf(zr[j] - mx) * inv_s * gs;
         zr[j] = g;
         if (gr) gr[j] = __float2bfloat16(g);
       }
       if (lane == 0) {
-        a.zpos[t] = (ep * inv_s - 1.f) * inv_n;
-        local += lse - zp;
+        a.zpos[t] = dpos * gs;
+        local += row_loss;
       }
     } else {
       // BCE: -( clamp(log(sigmoid(z_pos) + eps)) + sum_j clamp(log(1 - sigmoid(z_j) + eps)) ), fp32 as the reference
@@ -276,6 +296,7 @@ struct rp_sampled_desc {
   float log_eps, clamp;
   float* loss_out;
   void* workspace; size_t workspace_bytes;
+  const float* row_weight;
 };
 
 static size_t ru(size_t x, size_t m) { return (x + m - 1) / m * m; }
@@ -309,13 +330,15 @@ static int sampled_args(const rp_sampled_desc* s, SampledArgs* a) {
   if (!s || !s->hc || !s->table || !s->labels || !s->negatives || !s->n_valid || !s->loss_out || !s->workspace) return RP_EINVAL;
   if (s->capacity <= 0 || s->n_items <= 0 || s->n_neg <= 0) return RP_ESHAPE;
   if (s->d != 64 && s->d != 128 && s->d != 256 && s->d != 512) return RP_ESHAPE;
-  if (s->neg_mode < 0 || s->neg_mode > 2 || s->kind < 0 || s->kind > 3) return RP_EINVAL;
+  if (s->neg_mode < 0 || s->neg_mode > 2 || s->kind < 0 || s->kind > 5) return RP_EINVAL;
+  if (s->kind == kCESampledWeighted && !s->row_weight) return RP_EINVAL;
   if (s->neg_mode != 0 && (!s->valid_idx || s->seq_len <= 0)) return RP_EINVAL;
   if (s->kind == kLegacyCE && s->vocab_size < 2) return RP_EINVAL;
   if (s->workspace_bytes < sampled_layout(s, nullptr)) return RP_EWORKSPACE;
   a->hc = reinterpret_cast<const __nv_bfloat16*>(s->hc);
   a->table = reinterpret_cast<const __nv_bfloat16*>(s->table);
   a->labels = s->labels; a->valid_idx = s->valid_idx; a->negatives = s->negatives; a->n_valid = s->n_valid;
+  a->row_weight = s->kind == kCESampledWeighted ? s->row_weight : nullptr;
   a->capacity = s->capacity; a->n_items = s->n_items; a->d = s->d; a->N = s->n_neg; a->neg_mode = s->neg_mode;
   a->L = s->seq_len; a->kind = s->kind; a->ignore_index = s->ignore_index; a->vocab_size = s->vocab_size;
   a->log_eps = s->log_eps; a->clamp = s->clamp; a->loss_out = s->loss_out;

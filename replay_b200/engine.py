@@ -579,13 +579,16 @@ class SasRecEngine:
             self.sce["n_rows"].fill_(n)
 
     # ------------------------------------------------------------------------------------------------ sampled heads
-    SAMPLED_KINDS = {"ce_sampled": 0, "bce_sampled": 1, "legacy_ce_sampled": 2, "legacy_bce_sampled": 3}
+    SAMPLED_KINDS = {"ce_sampled": 0, "bce_sampled": 1, "legacy_ce_sampled": 2, "legacy_bce_sampled": 3, "login_ce_sampled": 4,
+                     "ce_sampled_weighted": 5}
 
     def set_loss(self, kind: str = "ce", n_neg: int = 0, neg_shape: str = "shared", ignore_index: int = -100,
                  log_eps: float = 1e-6, clamp: float = 100.0, n_buckets: int = 0, bucket_size_x: int = 0,
                  bucket_size_y: int = 0, mix_x: bool = False):
         """``"ce"`` = full-catalog CE (default).  Sampled heads (SURVEY §8 a9): ``ce_sampled`` / ``bce_sampled`` (new path,
-        replay/nn/loss/ce.py:146, bce.py:98) and ``legacy_ce_sampled`` / ``legacy_bce_sampled`` (sasrec/lightning.py:310-376)
+        replay/nn/loss/ce.py:146, bce.py:98), ``login_ce_sampled`` (LogInCESampled, login_ce.py:240, with ``log_eps`` /
+        ``clamp``), ``ce_sampled_weighted`` (CESampledWeighted, ce.py:252: sample weights staged with set_row_weights) and
+        ``legacy_ce_sampled`` / ``legacy_bce_sampled`` (sasrec/lightning.py:310-376)
         with ``n_neg`` negatives per target, ``neg_shape`` in shared [N] / perseq [B, N] / perpos [B, L, N].
         ``"sce"``: the legacy module's scalable cross-entropy (replay/models/nn/loss/sce.py) with ``n_buckets`` buckets of
         ``bucket_size_x`` rows and ``bucket_size_y`` items (both <= 1024, the fused top-K), ``mix_x`` as the reference."""
@@ -605,15 +608,15 @@ class SasRecEngine:
             self.sampled = None
             if kind in ("ce_weighted", "login_ce"):
                 self.ce_row = dict(kind=1 if kind == "login_ce" else 0, log_eps=log_eps, clamp=clamp, weighted=(kind == "ce_weighted"))
-                if not hasattr(self, "in_roww") or self.in_roww.numel() < self.T:
-                    self.in_roww = torch.ones(self.T, device=self.dev, dtype=torch.float32)
-                    self.roww_c = torch.ones(self.T, device=self.dev, dtype=torch.float32)
+                self._alloc_row_weights()
             return
         if kind not in self.SAMPLED_KINDS:
             raise NotImplementedError(f"Not supported loss_type {kind!r}")
         mode = {"shared": 0, "perpos": 1, "perseq": 2}[neg_shape]
         rows = {0: 1, 1: self.T, 2: self.B}[mode]
         ws_bytes = self.lib.rp_sampled_head_workspace(self.T, self.cfg.dp, n_neg, mode)
+        if kind == "ce_sampled_weighted":
+            self._alloc_row_weights()
         self.sampled = dict(kind=self.SAMPLED_KINDS[kind], n_neg=n_neg, mode=mode, ignore_index=ignore_index, log_eps=log_eps,
                             clamp=clamp, neg=torch.zeros(rows, n_neg, device=self.dev, dtype=torch.int64),
                             ws=torch.zeros(ws_bytes, device=self.dev, dtype=torch.uint8), ws_bytes=ws_bytes)
@@ -663,6 +666,13 @@ class SasRecEngine:
         sc["draw"][: draw.shape[0]].copy_(draw)
         sc["desc"].draw_given = 1
 
+    def _alloc_row_weights(self):
+        """Static staging buffers of the per-row sample weights: in_roww [T] by flat position, roww_c [T] in the heads'
+        compacted order (filled on the stream by each forward, so a captured step reads the weights staged for its batch)."""
+        if not hasattr(self, "in_roww") or self.in_roww.numel() < self.T:
+            self.in_roww = torch.ones(self.T, device=self.dev, dtype=torch.float32)
+            self.roww_c = torch.ones(self.T, device=self.dev, dtype=torch.float32)
+
     def set_row_weights(self, weights):
         """Stage the sample weights of the current batch ([B, L] float, one per position; only valid targets are read)."""
         n = weights.numel()
@@ -689,6 +699,8 @@ class SasRecEngine:
         sd.log_eps, sd.clamp = sp["log_eps"], sp["clamp"]
         sd.loss_out = self.ce.loss.data_ptr()
         sd.workspace, sd.workspace_bytes = sp["ws"].data_ptr(), sp["ws_bytes"]
+        if sp["kind"] == self.SAMPLED_KINDS["ce_sampled_weighted"]:
+            sd.row_weight = self.roww_c.data_ptr()
         return sd
 
     def _prepare(self, with_targets: bool):
@@ -910,6 +922,8 @@ class SasRecEngine:
         self._body_forward(True)
         self._final_norm_fwd(self.x[-1], self.hc, T, gather=self._target_rows(), n_rows_dev=self.n_valid)
         if self.sampled is not None:
+            if self.sampled["kind"] == self.SAMPLED_KINDS["ce_sampled_weighted"]:   # weights in the head's compacted order
+                torch.index_select(self.in_roww, 0, self.valid_idx, out=self.roww_c)
             check(self.lib.rp_sampled_head_fwd(ctypes.byref(self._sampled_desc()), self._stream()), "rp_sampled_head_fwd")
             return self.ce.loss
         return self._catalog_head_fwd(self.params16["item_emb"][: cfg.n_items])

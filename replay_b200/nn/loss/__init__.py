@@ -1,10 +1,27 @@
-"""Loss selectors with the reference's names and constructor arguments (replay/nn/loss/{ce,bce}.py).  They carry no
-computation: assigning one to ``SasRec.loss`` selects the fused CUDA head that implements it (full-catalog CE:
-rp_ce_head_*; full-catalog BCE: rp_bce_head_*; sampled heads: rp_sampled_head_*).  Single positive label per position (multi-positive: NotImplementedError,
-as in the reference's CE)."""
+"""Loss selectors with the reference's names and constructor arguments (replay/nn/loss/{ce,bce,login_ce,logout_ce}.py):
+every name of the reference's ``replay.nn.loss``.  They carry no computation: assigning one to ``SasRec.loss`` selects the
+fused CUDA head that implements it (full-catalog CE and its per-row variants: rp_ce_head_*; full-catalog BCE:
+rp_bce_head_*; sampled heads - CESampled, CESampledWeighted, BCESampled, LogInCESampled: rp_sampled_head_*).  Single
+positive label per position (multi-positive: NotImplementedError, as in the reference's CE)."""
 from __future__ import annotations
 
+from typing import Callable, Optional, Protocol
+
 import torch
+
+
+class LossProto(Protocol):
+    """replay/nn/loss/base.py: the interface every loss of the reference implements (a ``typing.Protocol``)."""
+
+    @property
+    def logits_callback(self) -> Callable[[torch.Tensor, Optional[torch.Tensor]], torch.Tensor]: ...
+
+    @logits_callback.setter
+    def logits_callback(self, func: Optional[Callable]) -> None: ...
+
+    def forward(self, model_embeddings: torch.Tensor, feature_tensors: dict, positive_labels: torch.LongTensor,
+                negative_labels: torch.LongTensor, padding_mask: torch.BoolTensor,
+                target_padding_mask: torch.BoolTensor) -> torch.Tensor: ...
 
 
 class _LossSpec:
@@ -117,6 +134,16 @@ class CEWeighted(_Weighted, CE):
         return (w.mean() * target_mask.to(torch.float32).mean()).expand(target_mask.shape[0], target_mask.shape[1])
 
 
+class CESampledWeighted(_Weighted, CESampled):
+    """replay/nn/loss/ce.py:252-330: ``CESampled``'s row losses times the sample weights of the valid targets, mean over the
+    valid targets (not divided by the weights' sum) -> per-row weights of the sampled head (rp_sampled_head_*)."""
+    kind = "ce_sampled_weighted"
+
+    def __init__(self, feature_name: str, negative_labels_ignore_index: int = -100, **kwargs):
+        CESampled.__init__(self, negative_labels_ignore_index, **kwargs)
+        self.feature_name = feature_name
+
+
 class LogInCE(_LossSpec):
     """replay/nn/loss/login_ce.py:102-239 with the whole catalog as negatives and one positive per position:
     ``-clamp(log(p + log_epsilon), -clamp_border, clamp_border)`` of the positive's softmax probability, mean over the valid
@@ -130,3 +157,22 @@ class LogInCE(_LossSpec):
 
     def engine_kwargs(self):
         return {"log_eps": self.log_epsilon, "clamp": self.clamp_border}
+
+
+class LogInCESampled(_LossSpec):
+    """replay/nn/loss/login_ce.py:240-375 with one positive per position: ``-clamp(log(p + log_epsilon), -clamp_border,
+    clamp_border)`` of the positive's softmax share over [positive | sampled negatives] (negatives masked as in CESampled),
+    mean over the valid targets."""
+    kind = "login_ce_sampled"
+    needs_negatives = True
+
+    def __init__(self, log_epsilon: float = 1e-6, clamp_border: float = 100.0, negative_labels_ignore_index: int = -100):
+        self.log_epsilon, self.clamp_border = log_epsilon, clamp_border
+        self.negative_labels_ignore_index = negative_labels_ignore_index
+
+    def engine_kwargs(self):
+        return {"ignore_index": self.negative_labels_ignore_index, "log_eps": self.log_epsilon, "clamp": self.clamp_border}
+
+
+__all__ = ["BCE", "CE", "BCESampled", "CESampled", "CESampledWeighted", "CEWeighted", "LogInCE", "LogInCESampled", "LogOutCE",
+           "LogOutCESampled", "LogOutCEWeighted", "LossProto"]

@@ -176,15 +176,16 @@ class SasRec(torch.nn.Module):
 
     @property
     def loss(self):
-        """The reference's ``SasRec.loss`` attribute (model.py:181-197): assign ``CE`` / ``BCE`` / ``CESampled`` /
-        ``BCESampled`` from ``replay_b200.nn.loss`` to select the fused head."""
+        """The reference's ``SasRec.loss`` attribute (model.py:181-197): assign a selector from ``replay_b200.nn.loss``
+        (``CE``, ``BCE``, ``CESampled``, ``LogInCESampled``, ...) to select the fused head."""
         return self._loss
 
     @loss.setter
     def loss(self, spec):
         if not hasattr(spec, "kind"):
             raise NotImplementedError(f"loss {type(spec).__name__} has no fused CUDA head (supported: CE, BCE, CEWeighted, "
-                                      "LogOutCE, LogOutCEWeighted, LogInCE, CESampled, BCESampled)")
+                                      "LogOutCE, LogOutCEWeighted, LogInCE, CESampled, CESampledWeighted, BCESampled, "
+                                      "LogInCESampled)")
         self._loss = spec
         self.core.set_loss(spec.kind, **spec.engine_kwargs())
 
