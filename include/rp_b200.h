@@ -584,8 +584,8 @@ int rp_diff_attn_softmax_bwd(const void* e1, const void* e2, const float* inv1, 
 /* dlambda_h = sum over sequences and rows of dlam_part (fixed order) chained into the lambda_* gradients (+=). */
 int rp_diff_lambda_bwd(const float* dlam_part, int B, int H, int L, const rp_diff_lambda* lam, float* gq1, float* gk1, float* gq2,
                        float* gk2, void* stream);
-/* RMSNorm over groups of `group` columns (64 / 128 / 256; d a multiple of it, d <= 512): y = x * rstd * w[c % group] * alpha,
- * rstd = 1/sqrt(sum_group x^2 / n_true + eps) - torch.nn.RMSNorm (group = d) and the per-head norm of the differential
+/* RMSNorm over groups of `group` columns (64 / 128 / 256 / 512; d a multiple of it, d <= 512): y = x * rstd * w[c % group] * alpha,
+ * rstd = 1/sqrt(sum_group x^2 / n_true + eps) - torch.nn.RMSNorm (group = d, the SwiGLU item tower's norms) and the per-head norm of the differential
  * attention (group = v_slot, n_true = 2*head_dim, alpha = 1 - lambda_init).  Padded columns must be zero in x and w.
  * With `gather` output row r reads input row gather[r] and only min(n_rows, *n_rows_dev) rows exist; the backward then
  * writes dx to those input rows.  dw (fp32 [group]) += the weight gradient, reduced in a fixed order through the workspace
@@ -600,6 +600,27 @@ int rp_rmsnorm_bwd(const void* dy, const void* x, const float* w, float eps, flo
  * backward dgl = [du * l * silu'(g) | du * silu(g)]. */
 int rp_swiglu_fwd(const void* gl, long long n_rows, int F, void* u, void* stream);
 int rp_swiglu_bwd(const void* du, const void* gl, long long n_rows, int F, void* dgl, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * Candidate compaction of the TwoTower model's sampled losses (replay/nn/sequential/twotower/model.py get_logits(h,
+ * candidates) -> item_tower(candidates)): the SwiGLU item tower runs on the distinct items one step references only.
+ * Inputs as for rp_sampled_head_fwd: compacted labels [capacity] with *n_valid valid, negatives int64 in neg_mode 0 (shared
+ * [n_neg]), 1 (per position [B*seq_len, n_neg], rows valid_idx[t]) or 2 (per sequence [n_neg_rows = B, n_neg], all rows).
+ * Outputs: *n_slots; item_of_slot int32 [cap] in ascending item id (-1 from *n_slots on); labels_out int32 [capacity] and
+ * negatives_out int64 (the negatives' layout; per-position rows of invalid targets untouched) as slot ids - negatives equal to
+ * ignore_index (>= 0) become `cap` (give the head ignore_index = cap), ids outside [0, n_items) become cap + 1 (the head
+ * reads row 0, item 0, as it does for such ids over the whole catalog, and never matches a positive); rows_out bf16 [cap, d]
+ * = table[item_of_slot[s]], zero rows from *n_slots on.  cap = min(n_items, capacity + negative entries) bounds the slots.
+ * No host synchronisation (graph-capturable).  Workspace: rp_tower_compact_workspace(n_items) bytes, need not be zeroed.
+ * rp_tower_scatter_rows: d_table fp32 [*, d] row item_of_slot[s] += dx bf16 [n_rows, d] row s, s < min(*n_slots, n_rows);
+ * item_of_slot = null: identity over n_rows rows.  Each item has at most one slot: plain stores, deterministic. */
+size_t rp_tower_compact_workspace(int n_items);
+int rp_tower_compact(const int32_t* labels, const int32_t* n_valid, int capacity, const int64_t* negatives, int n_neg,
+                     int neg_mode, int n_neg_rows, const int32_t* valid_idx, int seq_len, int ignore_index, int n_items,
+                     const void* table, int d, int cap, int32_t* n_slots, int32_t* item_of_slot, int32_t* labels_out,
+                     int64_t* negatives_out, void* rows_out, void* workspace, size_t workspace_bytes, void* stream);
+int rp_tower_scatter_rows(const void* dx, const int32_t* item_of_slot, const int32_t* n_slots, int n_rows, int d,
+                          float* d_table, void* stream);
 
 #ifdef __cplusplus
 }

@@ -258,6 +258,10 @@ _EXTRA_SIGS: list = [
                                       _P, _P, c_int, _P, _P, _P]),
     ("rp_pre_attn_bwd_rows", c_int, [_P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, _P, _P, _P, c_int, _P, _P]),
     ("rp_wgrad_group_rows", c_int, [ctypes.POINTER(WgradPair), c_int, c_int, c_int, _P, _P, c_size_t, _P]),
+    ("rp_tower_compact_workspace", c_size_t, [c_int]),
+    ("rp_tower_compact", c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, _P, c_int, c_int, c_int, _P, c_int, c_int, _P, _P, _P,
+                                 _P, _P, _P, c_size_t, _P]),
+    ("rp_tower_scatter_rows", c_int, [_P, _P, _P, c_int, c_int, _P, _P]),
 ]
 
 __all__ = ["GemmDesc", "DiffAttnDesc", "DiffLambda", "SceDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]

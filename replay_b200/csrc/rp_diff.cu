@@ -441,7 +441,7 @@ RP_API int rp_diff_lambda_bwd(const float* dlam_part, int B, int H, int L, const
 }
 
 static bool rms_shape_ok(int group, int d, int n_true, int n_rows) {
-  return (group == 64 || group == 128 || group == 256) && d > 0 && d <= 512 && d % group == 0 && n_true >= 1 &&
+  return (group == 64 || group == 128 || group == 256 || group == 512) && d > 0 && d <= 512 && d % group == 0 && n_true >= 1 &&
          n_true <= group && n_rows >= 0;
 }
 
@@ -456,13 +456,14 @@ RP_API int rp_rmsnorm_fwd(const void* x, const float* w, float eps, float alpha,
   auto yp = reinterpret_cast<__nv_bfloat16*>(y);
   if (group == 64) rmsnorm_fwd_kernel<64><<<grid, 256, 0, stream>>>(xp, w, eps, alpha, n_rows, d, n_true, n_rows_dev, gather, yp);
   else if (group == 128) rmsnorm_fwd_kernel<128><<<grid, 256, 0, stream>>>(xp, w, eps, alpha, n_rows, d, n_true, n_rows_dev, gather, yp);
-  else rmsnorm_fwd_kernel<256><<<grid, 256, 0, stream>>>(xp, w, eps, alpha, n_rows, d, n_true, n_rows_dev, gather, yp);
+  else if (group == 256) rmsnorm_fwd_kernel<256><<<grid, 256, 0, stream>>>(xp, w, eps, alpha, n_rows, d, n_true, n_rows_dev, gather, yp);
+  else rmsnorm_fwd_kernel<512><<<grid, 256, 0, stream>>>(xp, w, eps, alpha, n_rows, d, n_true, n_rows_dev, gather, yp);
   RP_LAUNCH_CHECK();
   return RP_OK;
 }
 
 RP_API size_t rp_rmsnorm_bwd_workspace(int group) {
-  return (group == 64 || group == 128 || group == 256) ? (size_t)kRmsParts * group * sizeof(float) : 0;
+  return (group == 64 || group == 128 || group == 256 || group == 512) ? (size_t)kRmsParts * group * sizeof(float) : 0;
 }
 
 RP_API int rp_rmsnorm_bwd(const void* dy, const void* x, const float* w, float eps, float alpha, int n_rows, int d, int group,
@@ -480,7 +481,8 @@ RP_API int rp_rmsnorm_bwd(const void* dy, const void* x, const float* w, float e
   float* part = reinterpret_cast<float*>(workspace);
   if (group == 64) rmsnorm_bwd_kernel<64><<<grid, 256, 0, stream>>>(dyp, xp, w, eps, alpha, n_rows, d, n_true, n_rows_dev, gather, dxp, part);
   else if (group == 128) rmsnorm_bwd_kernel<128><<<grid, 256, 0, stream>>>(dyp, xp, w, eps, alpha, n_rows, d, n_true, n_rows_dev, gather, dxp, part);
-  else rmsnorm_bwd_kernel<256><<<grid, 256, 0, stream>>>(dyp, xp, w, eps, alpha, n_rows, d, n_true, n_rows_dev, gather, dxp, part);
+  else if (group == 256) rmsnorm_bwd_kernel<256><<<grid, 256, 0, stream>>>(dyp, xp, w, eps, alpha, n_rows, d, n_true, n_rows_dev, gather, dxp, part);
+  else rmsnorm_bwd_kernel<512><<<grid, 256, 0, stream>>>(dyp, xp, w, eps, alpha, n_rows, d, n_true, n_rows_dev, gather, dxp, part);
   RP_LAUNCH_CHECK();
   return rp_reduce_splits(part, kRmsParts, group, group, dw, 1, stream_);
 }

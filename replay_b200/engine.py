@@ -456,7 +456,7 @@ class SasRecEngine:
     def _gemm(self, A, B, C, M, N, K, *, a_mn=False, b_mn=False, bias=None, act=0, residual=None, rowmask=None,
               drop_p=0.0, drop_site=0, out_mode=0, split_k=1, gate=None, gate_scale=1.0, alpha=1.0, batch=1, inner=1,
               a_off=(0, 0, 0, 0, 0, 0), b_off=(0, 0, 0, 0, 0, 0), c_geom=None, rowmask_oo=0, C2=None, gate_mode=0,
-              post_drop_p=0.0, post_drop_site=0, c_split_stride=0):
+              post_drop_p=0.0, post_drop_site=0, c_split_stride=0, m_limit=None):
         g = GemmDesc()
         g.A, g.a_rows, g.a_cols, g.lda, g.a_mn = A.data_ptr(), A.shape[0], A.shape[1], A.stride(0), int(a_mn)
         g.B, g.b_rows, g.b_cols, g.ldb, g.b_mn = B.data_ptr(), B.shape[0], B.shape[1], B.stride(0), int(b_mn)
@@ -487,6 +487,8 @@ class SasRecEngine:
         g.post_drop_p = post_drop_p
         g.post_drop_offset = post_drop_site << 40
         g.c_split_stride = c_split_stride
+        if m_limit is not None:   # device row count: 128-row tiles at or past it are skipped
+            g.m_limit_dev = m_limit.data_ptr()
         check(self.lib.rp_gemm(ctypes.byref(g), self._stream()), "rp_gemm")
 
     @property
@@ -494,15 +496,16 @@ class SasRecEngine:
         """Streaming multiprocessors of the engine's GPU (sizes the split-K waves of the weight gradients)."""
         return torch.cuda.get_device_properties(self.dev).multi_processor_count
 
-    def _wgrad(self, dY, X, dW, n_out, n_in):
-        """dW[n_out, n_in] += dY[T, n_out]^T . X[T, n_in]: both operands read MN-major in place; split-K over about one wave
-        of CTAs, each storing its fp32 partial tile (no atomics: 100+ CTAs hammering the same 16 K addresses serialise in
-        L2), then one reduction pass adds the partials into the gradient buffer (deterministic)."""
+    def _wgrad(self, dY, X, dW, n_out, n_in, rows=None):
+        """dW[n_out, n_in] += dY[rows, n_out]^T . X[rows, n_in] (rows: T by default): both operands read MN-major in place;
+        split-K over about one wave of CTAs, each storing its fp32 partial tile (no atomics: 100+ CTAs hammering the same
+        16 K addresses serialise in L2), then one reduction pass adds the partials into the gradient buffer (deterministic)."""
+        rows = self.T if rows is None else rows
         tiles = ((n_out + 127) // 128) * ((n_in + 127) // 128 if n_in > 64 else 1)
-        chunks = (self.T + 63) // 64
+        chunks = (rows + 63) // 64
         n = n_out * n_in
         split = max(1, min(chunks // 8, (self.n_sm + tiles - 1) // tiles, self.wg_ws.numel() // n))
-        self._gemm(dY, X, self.wg_ws, n_out, n_in, self.T, a_mn=True, b_mn=True, out_mode=3, split_k=split,
+        self._gemm(dY, X, self.wg_ws, n_out, n_in, rows, a_mn=True, b_mn=True, out_mode=3, split_k=split,
                    c_geom=(n_in, 0, 0, 0), c_split_stride=n)
         check(self.lib.rp_reduce_splits(self.wg_ws.data_ptr(), split, n, n, dW.data_ptr(), 1, self._stream()), "rp_reduce_splits")
 

@@ -18,11 +18,11 @@ import torch
 
 from ._lib import DiffAttnDesc, DiffLambda, check
 from .engine import BaseConfig, SasRecEngine, _ru
+from .engine_swiglu import RMS_EPS, SwiGLUOps
 
 _QK_SLOT = 64   # each of q1 / q2 / k1 / k2 occupies a 64-wide slot per head
 _DIFF_BLOCK = ("wq", "wk", "wv", "wo", "lambda_q1", "lambda_k1", "lambda_q2", "lambda_k2", "rms_scale", "attn_norm",
                "ff_norm", "ff_wg", "ff_w1", "ff_bg", "ff_b1", "ff_w2", "ff_b2")
-RMS_EPS = float(torch.finfo(torch.float32).eps)   # torch.nn.RMSNorm(d) with eps=None on fp32 activations
 
 
 def lambda_init(block: int) -> float:
@@ -91,7 +91,7 @@ class DiffConfig(BaseConfig):
         return out
 
 
-class DiffEngine(SasRecEngine):
+class DiffEngine(SwiGLUOps, SasRecEngine):
     def _check_geometry(self, seq_len: int):
         if seq_len > self.cfg.max_len:
             raise ValueError(f"sequence length {seq_len} exceeds max_len {self.cfg.max_len}")
@@ -130,14 +130,6 @@ class DiffEngine(SasRecEngine):
                 self.import_named(name, v)
         self.refresh_shadow()
 
-    def _span(self, bufs: dict, first: str, last: str, rows: int) -> torch.Tensor:
-        """[rows, cols] view over the adjacent parameters ``first`` .. ``last`` of one flat buffer (the packed QKV weight,
-        [WG; W1] and [bg; b1])"""
-        t0, t1 = bufs[first], bufs[last]
-        n = t1.data_ptr() - t0.data_ptr() + t1.numel() * t1.element_size()
-        flat = t0.view(-1).as_strided((n // t0.element_size(),), (1,))
-        return flat.view(rows, -1)
-
     # ------------------------------------------------------------------------------------------------ workspace
     def _alloc_body(self):
         cfg, T, d, dev = self.cfg, self.T, self.cfg.dp, self.dev
@@ -167,18 +159,6 @@ class DiffEngine(SasRecEngine):
             self.rms_ws = torch.zeros(need, device=dev, dtype=torch.uint8)
 
     # ------------------------------------------------------------------------------------------------ kernel helpers
-    def _rms_fwd(self, x, w, eps, y, n_rows, group, n_true, alpha=1.0, gather=None, n_rows_dev=None):
-        check(self.lib.rp_rmsnorm_fwd(x.data_ptr(), w.data_ptr(), eps, alpha, n_rows, x.shape[1], group, n_true,
-                                      None if n_rows_dev is None else n_rows_dev.data_ptr(),
-                                      None if gather is None else gather.data_ptr(), y.data_ptr(), self._stream()),
-              "rp_rmsnorm_fwd")
-
-    def _rms_bwd(self, dy, x, w, eps, dx, dw, n_rows, group, n_true, alpha=1.0, gather=None, n_rows_dev=None):
-        check(self.lib.rp_rmsnorm_bwd(dy.data_ptr(), x.data_ptr(), w.data_ptr(), eps, alpha, n_rows, x.shape[1], group, n_true,
-                                      None if n_rows_dev is None else n_rows_dev.data_ptr(),
-                                      None if gather is None else gather.data_ptr(), dx.data_ptr(), dw.data_ptr(),
-                                      self.rms_ws.data_ptr(), self.rms_ws.numel(), self._stream()), "rp_rmsnorm_bwd")
-
     def _lambda(self, i: int) -> DiffLambda:
         prm = self.params
         lam = DiffLambda()
@@ -234,11 +214,7 @@ class DiffEngine(SasRecEngine):
             self._attention_forward(i, training and self.with_grad)
             self._gemm(a["On"], w("wo"), a["h"], T, d, cfg.n_heads * cfg.v_slot, residual=x)
             self._rms_fwd(a["h"], f("attn_norm"), RMS_EPS, a["y"], T, d, cfg.d)
-            self._gemm(a["y"], self._span(p16, f"b{i}.ff_wg", f"b{i}.ff_w1", 2 * F), a["GL"], T, 2 * F, d,
-                       bias=self._span(prm, f"b{i}.ff_bg", f"b{i}.ff_b1", 1)[0])
-            check(self.lib.rp_swiglu_fwd(a["GL"].data_ptr(), T, F, a["U"].data_ptr(), self._stream()), "rp_swiglu_fwd")
-            self._gemm(a["U"], w("ff_w2"), a["z"], T, d, F, bias=f("ff_b2"), residual=a["y"])
-            self._rms_fwd(a["z"], f("ff_norm"), RMS_EPS, self.x[i + 1], T, d, cfg.d)
+            self._swiglu_block_fwd(f"b{i}.ff_", a["y"], a["GL"], a["U"], a["z"], self.x[i + 1], T, F)
 
     # ------------------------------------------------------------------------------------------------ backward
     def _attention_backward(self, i: int):
@@ -287,12 +263,7 @@ class DiffEngine(SasRecEngine):
             w = lambda k: p16[f"b{i}.{k}"]  # noqa: E731
             f = lambda k: prm[f"b{i}.{k}"]  # noqa: E731
             g = lambda k: G[f"b{i}.{k}"]  # noqa: E731
-            self._rms_bwd(dx, a["z"], f("ff_norm"), RMS_EPS, s["dz"], g("ff_norm"), T, d, cfg.d)
-            self._gemm(s["dz"], w("ff_w2"), s["dU"], T, F, d, b_mn=True)
-            check(self.lib.rp_swiglu_bwd(s["dU"].data_ptr(), a["GL"].data_ptr(), T, F, s["dGL"].data_ptr(), self._stream()),
-                  "rp_swiglu_bwd")
-            self._gemm(s["dGL"], self._span(p16, f"b{i}.ff_wg", f"b{i}.ff_w1", 2 * F), s["dy"], T, d, 2 * F, b_mn=True,
-                       residual=s["dz"])
+            self._swiglu_block_bwd(f"b{i}.ff_", dx, a["y"], a["GL"], a["U"], a["z"], s["dz"], s["dU"], s["dGL"], s["dy"], T, F)
             self._rms_bwd(s["dy"], a["h"], f("attn_norm"), RMS_EPS, s["dh"], g("attn_norm"), T, d, cfg.d)
             self._gemm(s["dh"], w("wo"), s["dOn"], T, H * vs, d, b_mn=True)
             self._rms_bwd(s["dOn"], a["Opre"], f("rms_scale"), 1e-5, s["dOpre"], g("rms_scale"), T, vs, 2 * cfg.head_dim,
@@ -300,11 +271,8 @@ class DiffEngine(SasRecEngine):
             self._attention_backward(i)
             self._gemm(s["dQKV"], self._span(p16, f"b{i}.wq", f"b{i}.wv", cfg.n_qkv), other, T, d, cfg.n_qkv, b_mn=True,
                        residual=s["dh"])
-            self._wgrad(s["dz"], a["U"], g("ff_w2"), d, F)
-            self._wgrad(s["dGL"], a["y"], self._span(G, f"b{i}.ff_wg", f"b{i}.ff_w1", 2 * F), 2 * F, d)
             self._wgrad(s["dh"], a["On"], g("wo"), d, H * vs)
             self._wgrad(s["dQKV"], x, self._span(G, f"b{i}.wq", f"b{i}.wv", cfg.n_qkv), cfg.n_qkv, d)
-            self._colsum_multi([(s["dz"], g("ff_b2")), (s["dGL"], self._span(G, f"b{i}.ff_bg", f"b{i}.ff_b1", 1)[0])])
             dx, other = other, dx
         check(self.lib.rp_embed_bwd(dx.data_ptr(), self.ids32.data_ptr(), self.in_pad.data_ptr(), self.B, L, d, cfg.pad_id,
                                     cfg.max_len - L, math.sqrt(cfg.d), 0, cfg.dropout, self.seed, 0, self.rng_counter.data_ptr(),
