@@ -290,6 +290,12 @@ int rp_embed_bwd_rows(const void* dx, const int32_t* ids, const uint8_t* pad_mas
  * inputs - every entry point that contains a LayerNorm takes `hd_valid`; the attention takes the true softmax scale. */
 int rp_layernorm_fwd(const void* x, const float* w, const float* b, float eps, int n_rows, int d, const int32_t* n_rows_dev,
                      const int32_t* gather, void* y, float* mean, float* rstd, int hd_valid, void* stream);
+/* rp_layernorm_fwd compacting rows for a loss head (gather and n_rows_dev required): the output rows after *n_rows_dev up to
+ * the next multiple of 128 (at most n_rows) are also zeroed.  The heads read their input in whole 128-row tiles, and a stale
+ * non-finite row there would reach every item's gradient through a zero weight in an MMA. */
+int rp_layernorm_fwd_compact(const void* x, const float* w, const float* b, float eps, int n_rows, int d,
+                             const int32_t* n_rows_dev, const int32_t* gather, void* y, float* mean, float* rstd, int hd_valid,
+                             void* stream);
 int rp_layernorm_bwd(const void* dy, const void* x, const float* w, const float* mean, const float* rstd, int n_rows, int d,
                      const int32_t* n_rows_dev, const int32_t* gather, const void* add_to, void* dx, float* dw, float* db,
                      int hd_valid, void* stream);

@@ -68,6 +68,7 @@ def lib():
     _sig(L.rp_embed_fwd, c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_float, c_int, c_float, U64, U64, P, P, P])
     _sig(L.rp_embed_bwd, c_int, [P, P, P, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_float, U64, U64, P, P, P, P])
     _sig(L.rp_layernorm_fwd, c_int, [P, P, P, c_float, c_int, c_int, P, P, P, P, P, c_int, P])
+    _sig(L.rp_layernorm_fwd_compact, c_int, [P, P, P, c_float, c_int, c_int, P, P, P, P, P, c_int, P])
     _sig(L.rp_layernorm_bwd, c_int, [P, P, P, P, P, c_int, c_int, P, P, P, P, P, P, c_int, P])
     _sig(L.rp_dropout_bwd, c_int, [P, P, LL, c_int, P, c_float, U64, U64, P, P])
     _sig(L.rp_colsum, c_int, [P, c_int, c_int, LL, P, P])

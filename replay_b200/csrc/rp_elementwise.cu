@@ -429,14 +429,15 @@ __global__ void row_plan_fill_kernel(const int32_t* __restrict__ seq_first, cons
 
 // ------------------------------------------------------------------------------------------------------------------
 // LayerNorm forward.  One warp per output row.  gather != null: output row r reads input row gather[r] and only
-// r < *n_rows_dev rows are produced (compaction of the valid targets for the CE head).
+// r < *n_rows_dev rows are produced (compaction of the valid targets for the CE head).  zero_tail (with gather and
+// n_rows_dev): the rows after them up to the next multiple of 128 (at most n_rows) are zeroed.
 // ------------------------------------------------------------------------------------------------------------------
 template <int VEC>
 __global__ void layernorm_fwd_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ w,
                                      const float* __restrict__ b, float eps, int n_rows,
                                      const int32_t* __restrict__ n_rows_dev, const int32_t* __restrict__ gather,
                                      __nv_bfloat16* __restrict__ y, float* __restrict__ mean_out,
-                                     float* __restrict__ rstd_out, int hd_valid) {
+                                     float* __restrict__ rstd_out, int hd_valid, int zero_tail) {
   constexpr int D = VEC * 32;
   const float inv_d = 1.f / (float)feat_count(D, hd_valid);
   const int lane = threadIdx.x & 31;
@@ -494,6 +495,16 @@ __global__ void layernorm_fwd_kernel(const __nv_bfloat16* __restrict__ x, const 
         mean_out[r] = mean;
         rstd_out[r] = rstd;
       }
+    }
+  }
+  if (zero_tail) {
+    // the loss heads read the compacted rows in 128-row tiles: the rows past *n_rows_dev up to the tile edge are zeroed, so
+    // that a stale value there (possibly not finite, e.g. from an earlier diverged step) never meets a zero weight in an MMA
+    const int tail = min(n_rows, (rows + 127) & ~127);
+    for (int r = rows + blockIdx.x * wpb + (threadIdx.x >> 5); r < tail; r += gridDim.x * wpb) {
+      __nv_bfloat16* yr = y + (size_t)r * D + lane * VEC;
+#pragma unroll
+      for (int i = 0; i < VEC; i += 2) *reinterpret_cast<uint32_t*>(yr + i) = 0u;
     }
   }
 }
@@ -915,18 +926,30 @@ RP_API int rp_embed_bwd_rows(const void* dx, const int32_t* ids, const uint8_t* 
   return RP_OK;
 }
 
-RP_API int rp_layernorm_fwd(const void* x, const float* w, const float* b, float eps, int n_rows, int d,
-                            const int32_t* n_rows_dev, const int32_t* gather, void* y, float* mean, float* rstd,
-                            int hd_valid, void* stream_) {
+static int layernorm_fwd(const void* x, const float* w, const float* b, float eps, int n_rows, int d, const int32_t* n_rows_dev,
+                         const int32_t* gather, void* y, float* mean, float* rstd, int hd_valid, int zero_tail, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (!x || !w || !b || !y || !mean || !rstd || n_rows <= 0) return RP_EINVAL;
   if (hd_valid < 0 || hd_valid > 128 || (hd_valid > 0 && d % (hd_valid <= 64 ? 64 : 128))) return RP_ESHAPE;
   const int grid = grid_for(n_rows, 8);
   RP_DISPATCH_D(d, (layernorm_fwd_kernel<VEC><<<grid, 256, 0, stream>>>(
                        reinterpret_cast<const __nv_bfloat16*>(x), w, b, eps, n_rows, n_rows_dev, gather,
-                       reinterpret_cast<__nv_bfloat16*>(y), mean, rstd, hd_valid)));
+                       reinterpret_cast<__nv_bfloat16*>(y), mean, rstd, hd_valid, zero_tail)));
   RP_LAUNCH_CHECK();
   return RP_OK;
+}
+
+RP_API int rp_layernorm_fwd(const void* x, const float* w, const float* b, float eps, int n_rows, int d,
+                            const int32_t* n_rows_dev, const int32_t* gather, void* y, float* mean, float* rstd,
+                            int hd_valid, void* stream_) {
+  return layernorm_fwd(x, w, b, eps, n_rows, d, n_rows_dev, gather, y, mean, rstd, hd_valid, 0, stream_);
+}
+
+RP_API int rp_layernorm_fwd_compact(const void* x, const float* w, const float* b, float eps, int n_rows, int d,
+                                    const int32_t* n_rows_dev, const int32_t* gather, void* y, float* mean, float* rstd,
+                                    int hd_valid, void* stream_) {
+  if (!n_rows_dev || !gather) return RP_EINVAL;
+  return layernorm_fwd(x, w, b, eps, n_rows, d, n_rows_dev, gather, y, mean, rstd, hd_valid, 1, stream_);
 }
 
 RP_API int rp_layernorm_bwd(const void* dy, const void* x, const float* w, const float* mean, const float* rstd,

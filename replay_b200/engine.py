@@ -133,7 +133,7 @@ class _CountingLib:
     """Proxy over the ctypes library that counts the sm_90a kernel launches issued through it (bench.py reports them)."""
 
     KERNELS = {"rp_gemm": 1, "rp_attn_fwd": 1, "rp_attn_bwd": 1, "rp_attn_last": 1, "rp_attn_softmax_bwd": 1, "rp_prepare_batch": 2, "rp_embed_fwd": 1,
-               "rp_embed_bwd": 2, "rp_layernorm_fwd": 1, "rp_layernorm_bwd": 1, "rp_dropout_bwd": 1, "rp_colsum": 1, "rp_colsum_multi": 1,
+               "rp_embed_bwd": 2, "rp_layernorm_fwd": 1, "rp_layernorm_fwd_compact": 1, "rp_layernorm_bwd": 1, "rp_dropout_bwd": 1, "rp_colsum": 1, "rp_colsum_multi": 1,
                "rp_adam_step": 2, "rp_cast_bf16": 1, "rp_counter_add": 1, "rp_reduce_splits": 1, "rp_ce_head_fwd": 2, "rp_ce_head_bwd": 3,
                "rp_score_topk": 2, "rp_seen_prepare": 1, "rp_sampled_head_fwd": 4, "rp_sampled_head_bwd": 4, "rp_post_attn_fused": 1,
                "rp_post_attn_train": 1, "rp_wgrad_group": 2, "rp_ln_qkv_fused": 1, "rp_pre_attn_bwd": 1,
@@ -546,10 +546,14 @@ class SasRecEngine:
         check(self.lib.rp_colsum_multi(n, dy, cols, ld, db, pairs[0][0].shape[0], self._stream()), "rp_colsum_multi")
 
     def _ln_fwd(self, x, w, b, eps, y, mean, rstd, n_rows, gather=None, n_rows_dev=None):
-        check(self.lib.rp_layernorm_fwd(x.data_ptr(), w.data_ptr(), b.data_ptr(), eps, n_rows, self.cfg.dp,
-                                        None if n_rows_dev is None else n_rows_dev.data_ptr(),
-                                        None if gather is None else gather.data_ptr(), y.data_ptr(), mean.data_ptr(),
-                                        rstd.data_ptr(), self.cfg.hd_valid, self._stream()), "rp_layernorm_fwd")
+        # the compaction of the valid targets for the loss heads also zeroes the rows after them up to the heads' 128-row tile
+        # edge (a stale non-finite row there would reach every item's gradient)
+        compact = gather is not None and n_rows_dev is not None
+        fn = self.lib.rp_layernorm_fwd_compact if compact else self.lib.rp_layernorm_fwd
+        check(fn(x.data_ptr(), w.data_ptr(), b.data_ptr(), eps, n_rows, self.cfg.dp,
+                 None if n_rows_dev is None else n_rows_dev.data_ptr(), None if gather is None else gather.data_ptr(),
+                 y.data_ptr(), mean.data_ptr(), rstd.data_ptr(), self.cfg.hd_valid, self._stream()),
+              "rp_layernorm_fwd_compact" if compact else "rp_layernorm_fwd")
 
     def _ln_bwd(self, dy, x, w, mean, rstd, dx, dw, db, n_rows, gather=None, n_rows_dev=None, add_to=None):
         check(self.lib.rp_layernorm_bwd(dy.data_ptr(), x.data_ptr(), w.data_ptr(), mean.data_ptr(), rstd.data_ptr(),
