@@ -277,6 +277,49 @@ int rp_embed_bwd_rows(const void* dx, const int32_t* ids, const uint8_t* pad_mas
                       unsigned long long drop_off, const unsigned long long* seed_ptr, float* d_table, float* d_pos,
                       void* stream);
 
+/* SASRec input with side features (nn/embedding.py SequenceEmbedding + nn/agg.py SumAggregator, csrc/rp_features.cu):
+ *   x[r] = dropout((table[ids[t]] + sum_f term_f(t)) * scale + pos[pos0 + t % L]),  t = r or row_tok[r] (packed rows)
+ * with the dropout stream of rp_embed_fwd (row key = token t).  Feature kinds and their term:
+ *   RP_FEAT_CAT       values int32 [T]:    table[v] (bf16 [n_rows, d]); v == padding_value or outside [0, n_rows): zero
+ *   RP_FEAT_BAG_SUM   values int32 [T, K]: sum of table[v_j] over the non-padding entries (torch.nn.EmbeddingBag "sum")
+ *   RP_FEAT_BAG_MEAN  the same divided by their count; an all-padding bag gives zero ("mean")
+ *   RP_FEAT_NUM       values fp32 [T, K]:  v . W^T + b, table = W fp32 [d, K] (padded rows zero), bias fp32 [d]
+ *   RP_FEAT_IDENT     values fp32 [T, K]:  v itself, K = the true hidden size (scattered into the head slots by hd_valid)
+ * Numerical features take consecutive val_col ranges (0, K0, K0 + K1, ...), at most RP_FEAT_MAX_NUM_COLS columns in all.
+ * Backward (the item table and the positions stay with rp_embed_bwd / _rows): dS = scale * dropout'(dx) is added into each
+ * categorical d_table row (fp32 atomics, padding rows untouched, mean bags scaled by 1 / count).  With numerical features
+ * it also writes d_s bf16 [rows, d] = dS and v_rows bf16 [rows, v_ld] (numerical values at their val_col, other columns
+ * zero), the operands of rp_wgrad_group for dW = dS^T . V and db = column sums of dS.  v_ld a multiple of 8.
+ * RP_EINVAL: null pointer, unknown kind, drop_p outside [0, 1); RP_ESHAPE: d, hd_valid, n_feats, widths, val_col, v_ld. */
+#define RP_FEAT_MAX 16
+#define RP_FEAT_MAX_NUM_COLS 64
+#define RP_FEAT_CAT 0
+#define RP_FEAT_BAG_SUM 1
+#define RP_FEAT_BAG_MEAN 2
+#define RP_FEAT_NUM 3
+#define RP_FEAT_IDENT 4
+typedef struct rp_feature {
+  int kind, width, n_rows, padding_value, val_col;
+  const void* values;
+  const void* table;
+  const float* bias;
+  float* d_table;
+} rp_feature;
+int rp_feature_embed_fwd(const void* item_table, const float* pos, const int32_t* ids, const rp_feature* feats, int n_feats,
+                         int T, int L, int d, int hd_valid, int pos0, float scale, float drop_p, unsigned long long seed,
+                         unsigned long long drop_off, const unsigned long long* seed_ptr, void* out, void* stream);
+int rp_feature_embed_fwd_rows(const void* item_table, const float* pos, const int32_t* ids, const rp_feature* feats,
+                              int n_feats, const int32_t* row_tok, const int32_t* n_rows_dev, int T, int L, int d, int hd_valid,
+                              int pos0, float scale, float drop_p, unsigned long long seed, unsigned long long drop_off,
+                              const unsigned long long* seed_ptr, void* out, void* stream);
+int rp_feature_embed_bwd(const void* dx, const rp_feature* feats, int n_feats, int T, int d, int hd_valid, float scale,
+                         float drop_p, unsigned long long seed, unsigned long long drop_off, const unsigned long long* seed_ptr,
+                         void* d_s, void* v_rows, int v_ld, void* stream);
+int rp_feature_embed_bwd_rows(const void* dx, const rp_feature* feats, int n_feats, const int32_t* row_tok,
+                              const int32_t* n_rows_dev, int T, int d, int hd_valid, float scale, float drop_p,
+                              unsigned long long seed, unsigned long long drop_off, const unsigned long long* seed_ptr,
+                              void* d_s, void* v_rows, int v_ld, void* stream);
+
 /* torch.nn.LayerNorm forward / backward (transformer.py:47-49,60-62 eps 1e-8; model.py:248 eps 1e-5).  With `gather`
  * output row r reads input row gather[r] and only *n_rows_dev rows exist (valid-target compaction); the backward then
  * scatters dx to those rows.  add_to (optional, bf16 [*, d]) is added to dx (residual-branch gradient). */

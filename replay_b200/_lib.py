@@ -236,6 +236,19 @@ class DiffAttnDesc(ctypes.Structure):
     ]
 
 
+class RpFeature(ctypes.Structure):
+    """Mirror of ``struct rp_feature`` (include/rp_b200.h): one side feature of the SASRec input stage."""
+
+    _fields_ = [
+        ("kind", c_int), ("width", c_int), ("n_rows", c_int), ("padding_value", c_int), ("val_col", c_int),
+        ("values", c_void_p), ("table", c_void_p), ("bias", c_void_p), ("d_table", c_void_p),
+    ]
+
+
+FEAT_CAT, FEAT_BAG_SUM, FEAT_BAG_MEAN, FEAT_NUM, FEAT_IDENT = range(5)   # rp_feature.kind
+FEAT_MAX, FEAT_MAX_NUM_COLS = 16, 64
+
+
 _P, _LL, _U64 = c_void_p, ctypes.c_longlong, ctypes.c_ulonglong
 _EXTRA_SIGS: list = [
     ("rp_diff_attn_fwd", c_int, [ctypes.POINTER(DiffAttnDesc), _P]),
@@ -263,6 +276,14 @@ _EXTRA_SIGS: list = [
     ("rp_tower_compact", c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, _P, c_int, c_int, c_int, _P, c_int, c_int, _P, _P, _P,
                                  _P, _P, _P, c_size_t, _P]),
     ("rp_tower_scatter_rows", c_int, [_P, _P, _P, c_int, c_int, _P, _P]),
+    ("rp_feature_embed_fwd", c_int, [_P, _P, _P, ctypes.POINTER(RpFeature), c_int, c_int, c_int, c_int, c_int, c_int, c_float,
+                                     c_float, _U64, _U64, _P, _P, _P]),
+    ("rp_feature_embed_fwd_rows", c_int, [_P, _P, _P, ctypes.POINTER(RpFeature), c_int, _P, _P, c_int, c_int, c_int, c_int,
+                                          c_int, c_float, c_float, _U64, _U64, _P, _P, _P]),
+    ("rp_feature_embed_bwd", c_int, [_P, ctypes.POINTER(RpFeature), c_int, c_int, c_int, c_int, c_float, c_float, _U64, _U64, _P,
+                                     _P, _P, c_int, _P]),
+    ("rp_feature_embed_bwd_rows", c_int, [_P, ctypes.POINTER(RpFeature), c_int, _P, _P, c_int, c_int, c_int, c_float, c_float,
+                                          _U64, _U64, _P, _P, _P, c_int, _P]),
 ]
 
-__all__ = ["GemmDesc", "DiffAttnDesc", "DiffLambda", "SceDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]
+__all__ = ["GemmDesc", "DiffAttnDesc", "DiffLambda", "SceDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "RpFeature", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]

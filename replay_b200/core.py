@@ -94,7 +94,19 @@ class SasRecCore(torch.nn.Module):
         self._materialise()
 
     def _key_map(self) -> dict:
-        return reference_key_map(self.cfg.variant, self.cfg.n_blocks, self.item_feature)
+        m = reference_key_map(self.cfg.variant, self.cfg.n_blocks, self.item_feature)
+        for f in getattr(self.cfg, "features", ()):   # nn/embedding.py CategoricalEmbedding.emb / NumericalEmbedding.linear
+            pre = f"body.embedder.feature_embedders.{f.name}."
+            if f.categorical:
+                m[f"feat.{f.name}"] = pre + "emb.weight"
+            elif f.kind == "num":
+                m.update({f"feat.{f.name}.w": pre + "linear.weight", f"feat.{f.name}.b": pre + "linear.bias"})
+        return m
+
+    def _stage_features(self, eng, feats):
+        """Stage the side features of the batch (a model without them ignores ``feats``)."""
+        if getattr(eng, "features", ()) and eng.set_features(feats or {}):
+            self._drop_graphs()   # a categorical list's staging buffer moved
 
     def _materialise(self):
         """Parameters exist from construction on (their layout depends on the configuration only), so ``parameters()``,
@@ -175,6 +187,9 @@ class SasRecCore(torch.nn.Module):
         src = self._export() if self.engine is not None else (self._pending_state or {})
         for k, v in src.items():
             out[prefix + k] = v
+        for f in getattr(self.cfg, "features", ()):   # IdentityEmbedding's buffer (nn/embedding.py): eye(d), no parameter
+            if f.kind == "ident":
+                out[prefix + f"body.embedder.feature_embedders.{f.name}._weight"] = torch.eye(self.cfg.d)
         if self.cfg.variant == "legacy":  # the reference's head registers the embedder again (Appendix B aliases)
             for a, b in (("_head._item_embedder.item_emb.weight", "item_embedder.item_emb.weight"),
                          ("_head._item_embedder.pos_emb.pe.weight", "item_embedder.pos_emb.pe.weight")):
@@ -206,7 +221,8 @@ class SasRecCore(torch.nn.Module):
     _FULL_CATALOG = ("ce", "ce_weighted", "login_ce", "bce", "sce")   # heads that take no negatives
     _WEIGHTED = ("ce_weighted", "ce_sampled_weighted")                # heads that read per-row sample weights
 
-    def _stage(self, eng, ids, pad_mask, labels, target_mask, negatives, row_weights=None):
+    def _stage(self, eng, ids, pad_mask, labels, target_mask, negatives, row_weights=None, feats=None):
+        self._stage_features(eng, feats)
         spec = getattr(self, "_loss_spec", ("ce", {}))
         if spec[0] in self._FULL_CATALOG:
             if eng.sampled is not None or getattr(eng, "_loss_applied", None) != (spec[0], tuple(sorted(spec[1].items()))):
@@ -237,14 +253,14 @@ class SasRecCore(torch.nn.Module):
             eng.set_row_weights(row_weights)
 
     # ---- training / inference on [B, L] batches
-    def loss(self, ids, pad_mask, labels, target_mask, negatives=None, row_weights=None) -> torch.Tensor:
+    def loss(self, ids, pad_mask, labels, target_mask, negatives=None, row_weights=None, feats=None) -> torch.Tensor:
         B, L = ids.shape
         eng = self.ensure_engine(B, L, with_grad=True)
-        self._stage(eng, ids, pad_mask, labels, target_mask, negatives, row_weights)
+        self._stage(eng, ids, pad_mask, labels, target_mask, negatives, row_weights, feats)
         return _EngineLoss.apply(self.flat, self)
 
     def fused_step(self, ids, pad_mask, labels, target_mask, all_reduce="auto", lr: float | None = None,
-                   negatives=None, row_weights=None) -> torch.Tensor:
+                   negatives=None, row_weights=None, feats=None) -> torch.Tensor:
         """forward + backward + Adam entirely inside the engine (no autograd, no torch optimizer).  ``all_reduce="auto"``
         exchanges the gradient over ``torch.distributed`` whenever a process group with more than one rank is initialised
         (Lightning ``strategy="ddp"``): this path has no autograd backward for DDP's hooks to fire on."""
@@ -255,7 +271,7 @@ class SasRecCore(torch.nn.Module):
             self._shadow_dirty = False
         self._set_lr(eng, lr)
         loss_before = getattr(eng, "_loss_applied", None), eng.sampled is None
-        self._stage(eng, ids, pad_mask, labels, target_mask, negatives, row_weights)
+        self._stage(eng, ids, pad_mask, labels, target_mask, negatives, row_weights, feats)
         if (getattr(eng, "_loss_applied", None), eng.sampled is None) != loss_before:
             self._drop_graphs()  # another loss head: different kernels / buffers
         if isinstance(all_reduce, str):  # "auto": torch.distributed when initialised (inside Trainer.run)
@@ -280,10 +296,10 @@ class SasRecCore(torch.nn.Module):
         return eng
 
     @torch.no_grad()
-    def query_embeddings(self, ids, pad_mask) -> torch.Tensor:
+    def query_embeddings(self, ids, pad_mask, feats=None) -> torch.Tensor:
         """Last-position hidden state, bf16 [B, d] (get_query_embeddings / forward_inference's last_hidden_state)."""
         eng = self._eval_engine(ids)
-        return eng.unpad_features(self._last_hidden(eng, ids, pad_mask))
+        return eng.unpad_features(self._last_hidden(eng, ids, pad_mask, feats))
 
     def _last_hidden_padded(self, eng, ids):
         return eng.forward_last_hidden()[: ids.shape[0]]
@@ -300,12 +316,13 @@ class SasRecCore(torch.nn.Module):
     predict_bucket_min_users = 1024    # smaller buckets join the next wider one
     predict_bucket_min_batch = 8192    # calls with fewer users take the single full-window pass
 
-    def _last_hidden(self, eng, ids, pad_mask):
+    def _last_hidden(self, eng, ids, pad_mask, feats=None):
         """Padded-width last hidden states bf16 [B, dp] of a batch; stages the batch (or its buckets) itself."""
         B, L = ids.shape
         widths = [w for w in self.predict_buckets if w < L]
         if self.cfg.variant != "new" or not widths or B < self.predict_bucket_min_batch:
             eng.set_batch(ids, pad_mask)
+            self._stage_features(eng, feats)
             return self._last_hidden_padded(eng, ids)
         n_real = pad_mask.sum(1)
         bucket = sum((n_real > w).to(torch.int64) for w in widths)            # 0 .. len(widths): index of the narrowest fit
@@ -318,6 +335,7 @@ class SasRecCore(torch.nn.Module):
                 counts[b] = 0
         if not ok or counts[-1] == B:
             eng.set_batch(ids, pad_mask)
+            self._stage_features(eng, feats)
             return self._last_hidden_padded(eng, ids)
         order = torch.argsort(bucket, stable=True)
         out = torch.empty(B, self.cfg.dp, device=ids.device, dtype=torch.bfloat16)
@@ -330,13 +348,16 @@ class SasRecCore(torch.nn.Module):
             start += cnt
             with eng.sub_geometry(cnt, w):
                 eng.set_batch(ids[idx, L - w:], pad_mask[idx, L - w:])
+                if eng.features:
+                    self._stage_features(eng, {k: v[idx, L - w:] for k, v in feats.items()})
                 out[idx] = eng.forward_last_hidden()[:cnt]
         return out
 
     @torch.no_grad()
-    def hidden_states(self, ids, pad_mask) -> torch.Tensor:
+    def hidden_states(self, ids, pad_mask, feats=None) -> torch.Tensor:
         eng = self._eval_engine(ids)
         eng.set_batch(ids, pad_mask)
+        self._stage_features(eng, feats)
         B, L = ids.shape
         return eng.unpad_features(eng.forward_hidden_all().view(eng.B, L, -1)[:B])
 
@@ -346,17 +367,17 @@ class SasRecCore(torch.nn.Module):
         return t if candidates is None else t[candidates].contiguous()
 
     @torch.no_grad()
-    def logits(self, ids, pad_mask, candidates=None) -> torch.Tensor:
+    def logits(self, ids, pad_mask, candidates=None, feats=None) -> torch.Tensor:
         """Materialised fp32 scores [B, |I|] or [B, |C|] (API compatibility; the fused top-K path never builds them)."""
         eng = self._eval_engine(ids)
-        hq = self._last_hidden(eng, ids, pad_mask)   # padded width: pairs with the padded table
+        hq = self._last_hidden(eng, ids, pad_mask, feats)   # padded width: pairs with the padded table
         tab = self.item_table(candidates)
         out = torch.empty(hq.shape[0], tab.shape[0], device=hq.device, dtype=torch.float32)
         self.engine._gemm(hq, tab, out, hq.shape[0], tab.shape[0], self.cfg.dp, out_mode=2)
         return out
 
     @torch.no_grad()
-    def predict_topk(self, ids, pad_mask, k: int, seen_ids=None, candidates=None):
+    def predict_topk(self, ids, pad_mask, k: int, seen_ids=None, candidates=None, feats=None):
         """Fused predict: body -> last hidden -> scores -> seen filter -> top-k.  Returns (item ids int64 [B,k], scores)."""
         from . import ops
 
@@ -368,6 +389,7 @@ class SasRecCore(torch.nn.Module):
             # one CUDA-graph replay per call (body kernels + seen-list sort + fused scoring / top-K, ~20 launches): at 512 .. 4096
             # users per call the eager launches, not the GPU, bound the call through the callbacks (bench r2: 4096 users 1.91 ms
             # on the device, 2.08 ms end to end).  Inputs are staged into static buffers, the result is copied out.
+            self._stage_features(eng, feats)   # before the lookup: staging a new list width drops the captured graphs
             key = (B, L, int(k), tuple(seen_ids.shape), eng.B, eng.L)
             graphs = self.__dict__.setdefault("_predict_graphs", {})
             st = graphs.get(key)
@@ -395,7 +417,7 @@ class SasRecCore(torch.nn.Module):
             st["graph"] = g
             g.replay()
             return st["ids"].clone(), st["scores"].clone()
-        hq = self._last_hidden(eng, ids, pad_mask).contiguous()
+        hq = self._last_hidden(eng, ids, pad_mask, feats).contiguous()
         inv = None
         if candidates is not None:
             inv = torch.full((n_items,), -1, device=hq.device, dtype=torch.int32)

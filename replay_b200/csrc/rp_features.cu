@@ -1,0 +1,314 @@
+// rp_features.cu - the new-path SASRec input stage with side features (replay/nn/embedding.py, replay/nn/agg.py:44-53,
+// replay/nn/sequential/sasrec/agg.py:37-53):
+//
+//   s_t = E_item[id_t] + sum_cat E_f[id_f,t] + sum_bag bag_f(E_f, ids_f,t) + sum_num v_f,t . W_f^T + b_f + sum_ident v_f,t
+//   x_t = dropout(s_t * scale + P[pos0 + t % L])
+//
+// One warp per token gathers every row, so the summed input is rounded to bf16 once, as the reference rounds nothing.  The
+// numerical projections run in the same pass: their summed tensor_dim is at most RP_FEAT_MAX_NUM_COLS, so a lane's dot
+// products are a few dozen FMAs per column on a weight slab that stays in L1, while a separate GEMM would need a bf16
+// staging copy of the values and a second read-modify-write pass over [T, d].  The dropout stream is rp_embed_fwd's (row
+// key = the token index, embedding site 0), so an item-only model and a side-feature model drop the same elements.
+//
+// Backward (rp_embed_bwd keeps the item table and the positions): dS = scale * dropout'(dx) is scattered into the side
+// tables with fp32 atomics (padding rows frozen, mean bags scaled by 1 / count), and written as bf16 next to the gathered
+// numerical values, the operands of the weight-gradient GEMM (rp_wgrad_group) that gives dW and db in a fixed order.
+#include "rp_b200.h"
+#include "rp_host.h"
+#include "rp_philox.cuh"
+#include "rp_sm90.cuh"
+
+namespace rp {
+
+struct FeatArgs {
+  rp_feature f[RP_FEAT_MAX];
+  int n;
+};
+
+// true feature index of padded column c (head slots of 64 / 128 columns with hd_valid real features each), -1 for padding
+__device__ __forceinline__ int feat_true_col(int c, int hd_valid) {
+  if (hd_valid == 0) return c;
+  const int slot = hd_valid <= 64 ? 64 : 128, j = c % slot;
+  return j < hd_valid ? (c / slot) * hd_valid + j : -1;
+}
+
+__device__ __forceinline__ bool feat_live(int id, const rp_feature& f) {
+  return id != f.padding_value && id >= 0 && id < f.n_rows;
+}
+
+template <int VEC>
+__device__ __forceinline__ void add_row(float* acc, const __nv_bfloat16* row, float w) {
+#pragma unroll
+  for (int i = 0; i < VEC; i += 2) {
+    const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(row + i));
+    acc[i] += v.x * w;
+    acc[i + 1] += v.y * w;
+  }
+}
+
+// row r of the output is token row_tok[r] (packed rows, *n_rows_dev of them) or token r (row_tok == null, n_tok rows)
+template <int VEC>
+__global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) feature_embed_fwd_kernel(
+    const __nv_bfloat16* __restrict__ item, const float* __restrict__ pos, const int32_t* __restrict__ ids, const __grid_constant__ FeatArgs fa,
+    int n_tok, int L, int hd_valid, int pos0, float scale, float drop_p, unsigned long long seed, unsigned long long drop_off,
+    const unsigned long long* __restrict__ seed_ptr, const int32_t* __restrict__ row_tok, const int32_t* __restrict__ n_rows_dev,
+    __nv_bfloat16* __restrict__ out) {
+  if (drop_p > 0.f && seed_ptr) seed += *seed_ptr;
+  constexpr int D = VEC * 32;
+  const int n = n_rows_dev ? *n_rows_dev : n_tok;
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  const int c0 = lane * VEC;
+  const uint32_t thr = drop_p > 0.f ? (uint32_t)(drop_p * 4294967296.0) : 0u;
+  const float ks = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
+  for (int r = blockIdx.x * wpb + (threadIdx.x >> 5); r < n; r += gridDim.x * wpb) {
+    const int t = row_tok ? row_tok[r] : r;
+    float acc[VEC];
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) acc[i] = 0.f;
+    add_row<VEC>(acc, item + (size_t)ids[t] * D + c0, 1.f);
+    for (int k = 0; k < fa.n; ++k) {
+      const rp_feature& f = fa.f[k];
+      if (f.kind == RP_FEAT_CAT || f.kind == RP_FEAT_BAG_SUM || f.kind == RP_FEAT_BAG_MEAN) {
+        const int32_t* v = reinterpret_cast<const int32_t*>(f.values) + (size_t)t * f.width;
+        const __nv_bfloat16* tab = reinterpret_cast<const __nv_bfloat16*>(f.table);
+        float bag[VEC];
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) bag[i] = 0.f;
+        int cnt = 0;
+        for (int j = 0; j < f.width; ++j) {
+          const int id = v[j];
+          if (!feat_live(id, f)) continue;
+          add_row<VEC>(bag, tab + (size_t)id * D + c0, 1.f);
+          ++cnt;
+        }
+        const float w = (f.kind == RP_FEAT_BAG_MEAN && cnt > 0) ? 1.f / (float)cnt : 1.f;
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) acc[i] += bag[i] * w;
+      } else if (f.kind == RP_FEAT_NUM) {
+        const float* v = reinterpret_cast<const float*>(f.values) + (size_t)t * f.width;
+        const float* W = reinterpret_cast<const float*>(f.table);
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) acc[i] += f.bias[c0 + i];
+        for (int j = 0; j < f.width; ++j) {
+          const float vj = v[j];
+#pragma unroll
+          for (int i = 0; i < VEC; ++i) acc[i] += vj * W[(size_t)(c0 + i) * f.width + j];
+        }
+      } else {  // RP_FEAT_IDENT: the values are the embedding (true features only; padded columns stay zero)
+        const float* v = reinterpret_cast<const float*>(f.values) + (size_t)t * f.width;
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) {
+          const int tc = feat_true_col(c0 + i, hd_valid);
+          if (tc >= 0) acc[i] += v[tc];
+        }
+      }
+    }
+    const float* p = pos + (size_t)(pos0 + t % L) * D + c0;
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) acc[i] = acc[i] * scale + p[i];
+    if (drop_p > 0.f) {
+      const uint32_t rk = drop_row_key(seed, drop_off, (unsigned long long)t);
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) acc[i] = drop_mix(rk, drop_col_key((uint32_t)(c0 + i))) >= thr ? acc[i] * ks : 0.f;
+    }
+    __nv_bfloat16* o = out + (size_t)r * D + c0;
+#pragma unroll
+    for (int i = 0; i < VEC; i += 2) *reinterpret_cast<uint32_t*>(o + i) = pack_bf16(acc[i], acc[i + 1]);
+  }
+}
+
+template <int VEC>
+__device__ __forceinline__ void scatter_row(float* dst, const float* g, float w) {
+  if constexpr (VEC % 4 == 0) {
+#pragma unroll
+    for (int i = 0; i < VEC; i += 4) atomicAdd(reinterpret_cast<float4*>(dst + i), make_float4(g[i] * w, g[i + 1] * w, g[i + 2] * w, g[i + 3] * w));
+  } else {
+#pragma unroll
+    for (int i = 0; i < VEC; i += 2) atomicAdd(reinterpret_cast<float2*>(dst + i), make_float2(g[i] * w, g[i + 1] * w));
+  }
+}
+
+template <int VEC>
+__global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) feature_embed_bwd_kernel(
+    const __nv_bfloat16* __restrict__ dx, const __grid_constant__ FeatArgs fa, int n_tok, float scale, float drop_p, unsigned long long seed,
+    unsigned long long drop_off, const unsigned long long* __restrict__ seed_ptr, const int32_t* __restrict__ row_tok,
+    const int32_t* __restrict__ n_rows_dev, __nv_bfloat16* __restrict__ d_s, __nv_bfloat16* __restrict__ v_rows, int v_ld) {
+  if (drop_p > 0.f && seed_ptr) seed += *seed_ptr;
+  constexpr int D = VEC * 32;
+  const int n = n_rows_dev ? *n_rows_dev : n_tok;
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  const int c0 = lane * VEC;
+  const uint32_t thr = drop_p > 0.f ? (uint32_t)(drop_p * 4294967296.0) : 0u;
+  const float ks = (drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f) * scale;
+  for (int r = blockIdx.x * wpb + (threadIdx.x >> 5); r < n; r += gridDim.x * wpb) {
+    const int t = row_tok ? row_tok[r] : r;
+    float g[VEC];
+    const __nv_bfloat16* gx = dx + (size_t)r * D + c0;
+#pragma unroll
+    for (int i = 0; i < VEC; i += 2) {
+      const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(gx + i));
+      g[i] = v.x * ks;
+      g[i + 1] = v.y * ks;
+    }
+    if (drop_p > 0.f) {
+      const uint32_t rk = drop_row_key(seed, drop_off, (unsigned long long)t);
+#pragma unroll
+      for (int i = 0; i < VEC; ++i)
+        if (drop_mix(rk, drop_col_key((uint32_t)(c0 + i))) < thr) g[i] = 0.f;
+    }
+    if (d_s) {
+      __nv_bfloat16* o = d_s + (size_t)r * D + c0;
+#pragma unroll
+      for (int i = 0; i < VEC; i += 2) *reinterpret_cast<uint32_t*>(o + i) = pack_bf16(g[i], g[i + 1]);
+    }
+    if (v_rows)  // zero the staging row first: its numerical columns are written below, the padding columns stay zero
+      for (int j = lane; j < v_ld; j += 32) v_rows[(size_t)r * v_ld + j] = __float2bfloat16(0.f);
+    __syncwarp();
+    for (int k = 0; k < fa.n; ++k) {
+      const rp_feature& f = fa.f[k];
+      if (f.kind == RP_FEAT_CAT || f.kind == RP_FEAT_BAG_SUM || f.kind == RP_FEAT_BAG_MEAN) {
+        const int32_t* v = reinterpret_cast<const int32_t*>(f.values) + (size_t)t * f.width;
+        float w = 1.f;
+        if (f.kind == RP_FEAT_BAG_MEAN) {
+          int cnt = 0;
+          for (int j = 0; j < f.width; ++j) cnt += feat_live(v[j], f);
+          w = cnt > 0 ? 1.f / (float)cnt : 0.f;
+        }
+        for (int j = 0; j < f.width; ++j) {
+          const int id = v[j];
+          if (feat_live(id, f)) scatter_row<VEC>(f.d_table + (size_t)id * D + c0, g, w);
+        }
+      } else if (f.kind == RP_FEAT_NUM && v_rows) {
+        const float* v = reinterpret_cast<const float*>(f.values) + (size_t)t * f.width;
+        for (int j = lane; j < f.width; j += 32) v_rows[(size_t)r * v_ld + f.val_col + j] = __float2bfloat16(v[j]);
+      }
+    }
+  }
+}
+
+}  // namespace rp
+
+using namespace rp;
+
+#define RP_FEAT_DISPATCH(d, CALL)                      \
+  switch (d) {                                         \
+    case 64: { constexpr int VEC = 2; CALL; } break;   \
+    case 128: { constexpr int VEC = 4; CALL; } break;  \
+    case 256: { constexpr int VEC = 8; CALL; } break;  \
+    case 512: { constexpr int VEC = 16; CALL; } break; \
+    default: return RP_ESHAPE;                         \
+  }
+
+static inline int feat_grid(long long rows) {   // one warp per row, about 8 blocks of 8 warps per SM
+  long long b = (rows + 7) / 8;
+  const long long cap = (long long)sm_count() * 8;
+  return (int)(b > cap ? cap : (b < 1 ? 1 : b));
+}
+
+// shared argument checks: RP_EINVAL for a null pointer or unknown kind, RP_ESHAPE for a size the kernels do not take
+static int feat_args(const rp_feature* feats, int n_feats, int d, int hd_valid, bool bwd, int v_ld, FeatArgs* fa) {
+  if (n_feats < 0 || n_feats > RP_FEAT_MAX || (n_feats > 0 && !feats)) return n_feats < 0 || n_feats > RP_FEAT_MAX ? RP_ESHAPE : RP_EINVAL;
+  if (hd_valid < 0 || hd_valid > 128 || (hd_valid > 0 && d % (hd_valid <= 64 ? 64 : 128))) return RP_ESHAPE;
+  const int d_true = hd_valid ? d / (hd_valid <= 64 ? 64 : 128) * hd_valid : d;
+  int num_cols = 0;
+  fa->n = n_feats;
+  for (int k = 0; k < n_feats; ++k) {
+    const rp_feature& f = feats[k];
+    if (!f.values) return RP_EINVAL;
+    if (f.width <= 0) return RP_ESHAPE;
+    switch (f.kind) {
+      case RP_FEAT_CAT:
+      case RP_FEAT_BAG_SUM:
+      case RP_FEAT_BAG_MEAN:
+        if (!f.table || (bwd && !f.d_table)) return RP_EINVAL;
+        if (f.n_rows <= 0 || (f.kind == RP_FEAT_CAT && f.width != 1)) return RP_ESHAPE;
+        break;
+      case RP_FEAT_NUM:
+        if (!f.table || !f.bias) return RP_EINVAL;
+        if (f.val_col != num_cols) return RP_ESHAPE;   // consecutive columns of the staging rows, in feature order
+        num_cols += f.width;
+        break;
+      case RP_FEAT_IDENT:
+        if (f.width != d_true) return RP_ESHAPE;
+        break;
+      default:
+        return RP_EINVAL;
+    }
+    fa->f[k] = f;
+  }
+  if (num_cols > RP_FEAT_MAX_NUM_COLS) return RP_ESHAPE;
+  if (bwd && num_cols > 0 && (v_ld < num_cols || v_ld % 8)) return RP_ESHAPE;
+  return RP_OK;
+}
+
+static int feature_fwd(const void* item_table, const float* pos, const int32_t* ids, const rp_feature* feats, int n_feats,
+                       const int32_t* row_tok, const int32_t* n_rows_dev, int T, int L, int d, int hd_valid, int pos0,
+                       float scale, float drop_p, unsigned long long seed, unsigned long long drop_off,
+                       const unsigned long long* seed_ptr, void* out, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!item_table || !pos || !ids || !out || T <= 0 || L <= 0 || pos0 < 0) return RP_EINVAL;
+  if (drop_p < 0.f || drop_p >= 1.f) return RP_EINVAL;
+  FeatArgs fa;
+  const int rc = feat_args(feats, n_feats, d, hd_valid, false, 0, &fa);
+  if (rc != RP_OK) return rc;
+  const int grid = feat_grid(T);
+  RP_FEAT_DISPATCH(d, (feature_embed_fwd_kernel<VEC><<<grid, 256, 0, stream>>>(
+                          reinterpret_cast<const __nv_bfloat16*>(item_table), pos, ids, fa, T, L, hd_valid, pos0, scale, drop_p,
+                          seed, drop_off, seed_ptr, row_tok, n_rows_dev, reinterpret_cast<__nv_bfloat16*>(out))));
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+static int feature_bwd(const void* dx, const rp_feature* feats, int n_feats, const int32_t* row_tok, const int32_t* n_rows_dev,
+                       int T, int d, int hd_valid, float scale, float drop_p, unsigned long long seed,
+                       unsigned long long drop_off, const unsigned long long* seed_ptr, void* d_s, void* v_rows, int v_ld,
+                       void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!dx || T <= 0) return RP_EINVAL;
+  if (drop_p < 0.f || drop_p >= 1.f) return RP_EINVAL;
+  FeatArgs fa;
+  const int rc = feat_args(feats, n_feats, d, hd_valid, true, v_ld, &fa);
+  if (rc != RP_OK) return rc;
+  bool has_num = false;
+  for (int k = 0; k < n_feats; ++k) has_num |= feats[k].kind == RP_FEAT_NUM;
+  if (has_num && (!d_s || !v_rows)) return RP_EINVAL;
+  const int grid = feat_grid(T);
+  RP_FEAT_DISPATCH(d, (feature_embed_bwd_kernel<VEC><<<grid, 256, 0, stream>>>(
+                          reinterpret_cast<const __nv_bfloat16*>(dx), fa, T, scale, drop_p, seed, drop_off, seed_ptr, row_tok,
+                          n_rows_dev, reinterpret_cast<__nv_bfloat16*>(d_s), reinterpret_cast<__nv_bfloat16*>(v_rows), v_ld)));
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+RP_API int rp_feature_embed_fwd(const void* item_table, const float* pos, const int32_t* ids, const rp_feature* feats,
+                                int n_feats, int T, int L, int d, int hd_valid, int pos0, float scale, float drop_p,
+                                unsigned long long seed, unsigned long long drop_off, const unsigned long long* seed_ptr,
+                                void* out, void* stream) {
+  return feature_fwd(item_table, pos, ids, feats, n_feats, nullptr, nullptr, T, L, d, hd_valid, pos0, scale, drop_p, seed,
+                     drop_off, seed_ptr, out, stream);
+}
+
+RP_API int rp_feature_embed_fwd_rows(const void* item_table, const float* pos, const int32_t* ids, const rp_feature* feats,
+                                     int n_feats, const int32_t* row_tok, const int32_t* n_rows_dev, int T, int L, int d,
+                                     int hd_valid, int pos0, float scale, float drop_p, unsigned long long seed,
+                                     unsigned long long drop_off, const unsigned long long* seed_ptr, void* out, void* stream) {
+  if (!row_tok || !n_rows_dev) return RP_EINVAL;
+  return feature_fwd(item_table, pos, ids, feats, n_feats, row_tok, n_rows_dev, T, L, d, hd_valid, pos0, scale, drop_p, seed,
+                     drop_off, seed_ptr, out, stream);
+}
+
+RP_API int rp_feature_embed_bwd(const void* dx, const rp_feature* feats, int n_feats, int T, int d, int hd_valid, float scale,
+                                float drop_p, unsigned long long seed, unsigned long long drop_off,
+                                const unsigned long long* seed_ptr, void* d_s, void* v_rows, int v_ld, void* stream) {
+  return feature_bwd(dx, feats, n_feats, nullptr, nullptr, T, d, hd_valid, scale, drop_p, seed, drop_off, seed_ptr, d_s, v_rows,
+                     v_ld, stream);
+}
+
+RP_API int rp_feature_embed_bwd_rows(const void* dx, const rp_feature* feats, int n_feats, const int32_t* row_tok,
+                                     const int32_t* n_rows_dev, int T, int d, int hd_valid, float scale, float drop_p,
+                                     unsigned long long seed, unsigned long long drop_off, const unsigned long long* seed_ptr,
+                                     void* d_s, void* v_rows, int v_ld, void* stream) {
+  if (!row_tok || !n_rows_dev) return RP_EINVAL;
+  return feature_bwd(dx, feats, n_feats, row_tok, n_rows_dev, T, d, hd_valid, scale, drop_p, seed, drop_off, seed_ptr, d_s,
+                     v_rows, v_ld, stream);
+}

@@ -19,7 +19,8 @@ from dataclasses import dataclass
 
 import torch
 
-from ._lib import SCE_ALL, SampledDesc, SceDesc, AttnBwdDesc, AttnDesc, GemmDesc, WgradPair, check, lib
+from ._lib import (FEAT_BAG_MEAN, FEAT_BAG_SUM, FEAT_CAT, FEAT_IDENT, FEAT_MAX, FEAT_MAX_NUM_COLS, FEAT_NUM, RpFeature,
+                   SCE_ALL, SampledDesc, SceDesc, AttnBwdDesc, AttnDesc, GemmDesc, WgradPair, check, lib)
 
 
 _BLOCK_PARAMS = ("ln1_w", "ln1_b", "in_w", "in_b", "out_w", "out_b", "ln2_w", "ln2_b", "w1", "b1", "w2", "b2")
@@ -104,10 +105,33 @@ class BaseConfig:
         return [(f"b{i}.{k}", s, pk) for k, s, pk in zip(_BLOCK_PARAMS, shapes, kinds)]
 
 
+@dataclass(frozen=True)
+class SideFeature:
+    """One side feature of the new-path SASRec input (replay/nn/embedding.py), summed into the item embedding.
+
+    ``kind``: "cat" (Embedding), "bag_sum" / "bag_mean" (EmbeddingBag over a categorical list), "num" (Linear(tensor_dim,
+    d)) or "ident" (tensor_dim == d: the values themselves).  ``cardinality`` / ``padding_value``: categorical kinds (the
+    table has cardinality + 1 rows, the padding row is zero and frozen).  ``width``: tensor_dim of the numerical kinds; a
+    categorical list takes its width from the batch."""
+    name: str
+    kind: str
+    cardinality: int = 0
+    padding_value: int = 0
+    width: int = 1
+
+    @property
+    def categorical(self) -> bool:
+        return self.kind in ("cat", "bag_sum", "bag_mean")
+
+
+_FEAT_KINDS = {"cat": FEAT_CAT, "bag_sum": FEAT_BAG_SUM, "bag_mean": FEAT_BAG_MEAN, "num": FEAT_NUM, "ident": FEAT_IDENT}
+
+
 @dataclass
 class EncoderConfig(BaseConfig):
     variant: str = "new"  # "new": replay.nn.sequential.SasRec ; "legacy": replay.models.nn.sequential.SasRecModel
     lnf_eps: float | None = None
+    features: tuple = ()  # SideFeature, ... (new path only); empty: the item-only input of rp_embed_fwd
 
     def __post_init__(self):
         if self.variant not in ("new", "legacy"):
@@ -116,6 +140,33 @@ class EncoderConfig(BaseConfig):
         if self.lnf_eps is None:
             # new: torch.nn.LayerNorm default (nn/sequential/sasrec/model.py:248); legacy: 1e-8 (sasrec/model.py:463)
             self.lnf_eps = 1e-5 if self.variant == "new" else 1e-8
+        self.features = tuple(self.features)
+        if self.features:
+            self._check_features()
+
+    def _check_features(self):
+        fs = self.features
+        if self.variant != "new":
+            raise ValueError("side features exist on the new-path SASRec only")
+        if len(fs) > FEAT_MAX or len({f.name for f in fs}) != len(fs):
+            raise ValueError(f"at most {FEAT_MAX} side features with distinct names")
+        for f in fs:
+            if f.kind not in _FEAT_KINDS:
+                raise ValueError(f"side feature {f.name!r}: unknown kind {f.kind!r}")
+            if f.categorical and f.cardinality < 1:
+                raise ValueError(f"side feature {f.name!r}: cardinality must be positive")
+            if f.kind == "ident" and f.width != self.d:
+                raise ValueError(f"side feature {f.name!r}: an identity feature needs tensor_dim == {self.d}")
+            if f.kind == "num" and f.width < 1:
+                raise ValueError(f"side feature {f.name!r}: tensor_dim must be positive")
+        if self.num_cols > FEAT_MAX_NUM_COLS:
+            raise ValueError(f"the numerical side features' tensor_dims sum to {self.num_cols}; at most {FEAT_MAX_NUM_COLS} "
+                             "are projected inside the embedding kernel")
+
+    @property
+    def num_cols(self) -> int:
+        """summed tensor_dim of the numerical (Linear) side features"""
+        return sum(f.width for f in self.features if f.kind == "num")
 
     @property
     def pad_id(self) -> int:
@@ -126,7 +177,13 @@ class EncoderConfig(BaseConfig):
         out = [("item_emb", (self.n_items + 1, d), emb), ("pos_emb", (self.max_len, d), emb)]
         for i in range(self.n_blocks):
             out += self._block_layout(i, d, "f")
-        return out + [("lnf_w", (d,), vec), ("lnf_b", (d,), vec)]
+        out += [("lnf_w", (d,), vec), ("lnf_b", (d,), vec)]
+        for f in self.features:   # after every item-only parameter: an item-only model keeps its layout and seeded init
+            if f.categorical:
+                out.append((f"feat.{f.name}", (f.cardinality + 1, d), emb))
+            elif f.kind == "num":
+                out += [(f"feat.{f.name}.w", (d, f.width), ("f", None)), (f"feat.{f.name}.b", (d,), vec)]
+        return out
 
 
 class _CountingLib:
@@ -177,6 +234,8 @@ class SasRecEngine:
             self.layout[name], self._kinds[name] = (off, shp), kinds
             off = _ru(off + math.prod(shp), 64)
         self._true = cfg.true_shapes()
+        self.features = tuple(getattr(cfg, "features", ()))
+        self._side_pad = {f"feat.{f.name}": f.padding_value for f in self.features if f.categorical}
         self.n_flat = off
         f32 = dict(device=self.dev, dtype=torch.float32)
         self.p32 = torch.zeros(off, **f32)
@@ -314,6 +373,11 @@ class SasRecEngine:
                     v = torch.randn(shp, generator=g) * std
                     if name == "item_emb" and self.cfg.variant == "new":
                         v[self.cfg.pad_id].zero_()
+                    elif name in self._side_pad:   # CategoricalEmbedding.reset_parameters (nn/embedding.py)
+                        v[self._side_pad[name]].zero_()
+                elif name.startswith("feat."):     # a numerical feature's Linear bias keeps torch's default init
+                    fan_in = self.true_shape(name[:-1] + "w")[1]
+                    v = (torch.rand(shp, generator=g) * 2 - 1) / math.sqrt(fan_in)
                 elif name.endswith(("ln1_w", "ln2_w", "lnf_w")):
                     v = torch.ones(shp)
                 elif name.endswith((".b1", ".b2")):
@@ -401,6 +465,7 @@ class SasRecEngine:
             self.act.append(a)
         self.hc = torch.zeros(T, d, **bf)
         self.hq = torch.zeros(self.B, d, **bf)
+        self._alloc_features()
         self.last_idx = (torch.arange(self.B, device=dev, dtype=torch.int32) * self.L + (self.L - 1)).contiguous()
         if self.with_grad:
             from .ops import CEHeadState
@@ -411,6 +476,136 @@ class SasRecEngine:
                 self.s["dpd"] = torch.zeros(BH, self.Lp, self.Lp, **bf)
             self.wg_ws = torch.zeros(self.n_sm * 4 * d * d, **f32)  # split-K partials of the weight-gradient GEMMs
         self._alloc_body()
+
+    def _alloc_features(self):
+        """Static staging buffers of the side features (a captured step reads the batch staged into them): int32 [T] / [T, K]
+        ids, fp32 [T, tensor_dim] values; a categorical list's buffer is sized by the first batch (set_features).  With
+        numerical features the backward also keeps dS bf16 [T, dp], the gathered values bf16 [T, 64] and their gradients."""
+        self.feat_in = {}
+        if not self.features:
+            return
+        i32, f32 = dict(device=self.dev, dtype=torch.int32), dict(device=self.dev, dtype=torch.float32)
+        for f in self.features:
+            if f.kind == "cat":
+                self.feat_in[f.name] = torch.full((self.T, 1), f.padding_value, **i32)
+            elif not f.categorical:
+                self.feat_in[f.name] = torch.zeros(self.T, f.width, **f32)
+        if self.with_grad and self.cfg.num_cols:
+            self.feat_ds = torch.zeros(self.T, self.cfg.dp, device=self.dev, dtype=torch.bfloat16)
+            self.feat_v = torch.zeros(self.T, FEAT_MAX_NUM_COLS, device=self.dev, dtype=torch.bfloat16)
+            self.feat_dw = torch.zeros(self.cfg.dp, FEAT_MAX_NUM_COLS, **f32)
+            self.feat_db = torch.zeros(self.cfg.dp, **f32)
+
+    def set_features(self, feats: dict) -> bool:
+        """Stage the side features of the current batch (name -> [B, L] or [B, L, K] tensor, as the reference's
+        ``feature_tensors``) into the static buffers; B * L <= T rows.  Returns True when a categorical list's buffer had to
+        be (re)allocated for a new list width, which moves it: graphs captured before then read the old buffer."""
+        moved = False
+        for f in self.features:
+            if f.name not in feats:
+                raise ValueError(f"feature_tensors lacks the side feature {f.name!r}")
+            v = feats[f.name]
+            n = v.shape[0] * v.shape[1]
+            if f.categorical:
+                k = 1 if f.kind == "cat" else (v.shape[2] if v.dim() == 3 else 1)
+                if f.kind == "cat" and v.dim() != 2 or f.kind != "cat" and v.dim() != 3:
+                    raise ValueError(f"side feature {f.name!r}: expected {'[B, L]' if f.kind == 'cat' else '[B, L, K]'} ids, "
+                                     f"got {tuple(v.shape)}")
+                buf = self.feat_in.get(f.name)
+                if buf is None or buf.shape[1] != k:
+                    buf = self.feat_in[f.name] = torch.full((self._alloc_T, k), f.padding_value, device=self.dev,
+                                                            dtype=torch.int32)
+                    moved = True
+            else:
+                buf = self.feat_in[f.name]
+                want = (v.shape[0], v.shape[1], f.width) if f.width > 1 or v.dim() == 3 else (v.shape[0], v.shape[1])
+                if tuple(v.shape) != want:
+                    raise ValueError(f"side feature {f.name!r}: expected values {want}, got {tuple(v.shape)}")
+            if n > buf.shape[0]:
+                raise ValueError(f"side feature {f.name!r}: {n} rows do not fit the engine's {buf.shape[0]}")
+            buf[:n].copy_(v.reshape(n, -1), non_blocking=True)
+        return moved
+
+    def _feature_descs(self, with_grad: bool):
+        """ctypes array of rp_feature for the staged side features (gradient pointers when ``with_grad``)."""
+        fs = self.features
+        arr = (RpFeature * len(fs))()
+        col = 0
+        for k, f in enumerate(fs):
+            a, buf = arr[k], self.feat_in[f.name]
+            a.kind, a.width, a.values = _FEAT_KINDS[f.kind], buf.shape[1], buf.data_ptr()
+            if f.categorical:
+                a.n_rows, a.padding_value = f.cardinality + 1, f.padding_value
+                a.table = self.params16[f"feat.{f.name}"].data_ptr()
+                a.d_table = self.grads[f"feat.{f.name}"].data_ptr() if with_grad else None
+            elif f.kind == "num":
+                a.table, a.bias = self.params[f"feat.{f.name}.w"].data_ptr(), self.params[f"feat.{f.name}.b"].data_ptr()
+                a.val_col = col
+                col += f.width
+        return arr
+
+    def _embed_fwd(self, drop: float, pos0: int):
+        """x[0] = the block input: rp_embed_fwd(_rows) for an item-only model, rp_feature_embed_fwd(_rows) with side features."""
+        cfg, T, L, d = self.cfg, self.T, self.L, self.cfg.dp
+        p16, prm, pad = self.params16, self.params, self.in_pad
+        legacy = cfg.variant == "legacy"
+        if self.features:
+            fa = self._feature_descs(False)
+            if self._packed:
+                check(self.lib.rp_feature_embed_fwd_rows(p16["item_emb"].data_ptr(), prm["pos_emb"].data_ptr(),
+                                                         self.ids32.data_ptr(), fa, len(fa), self.row_tok.data_ptr(),
+                                                         self.n_rows.data_ptr(), T, L, d, cfg.hd_valid, pos0, math.sqrt(cfg.d),
+                                                         drop, self.seed, 0, self.rng_counter.data_ptr(), self.x[0].data_ptr(),
+                                                         self._stream()), "rp_feature_embed_fwd_rows")
+            else:
+                check(self.lib.rp_feature_embed_fwd(p16["item_emb"].data_ptr(), prm["pos_emb"].data_ptr(), self.ids32.data_ptr(),
+                                                    fa, len(fa), T, L, d, cfg.hd_valid, pos0, math.sqrt(cfg.d), drop, self.seed,
+                                                    0, self.rng_counter.data_ptr(), self.x[0].data_ptr(), self._stream()),
+                      "rp_feature_embed_fwd")
+        elif self._packed:
+            check(self.lib.rp_embed_fwd_rows(p16["item_emb"].data_ptr(), prm["pos_emb"].data_ptr(), self.ids32.data_ptr(),
+                                             pad.data_ptr(), self.row_tok.data_ptr(), self.n_rows.data_ptr(), T, L, d, pos0,
+                                             math.sqrt(cfg.d), 0, drop, self.seed, 0, self.rng_counter.data_ptr(),
+                                             self.x[0].data_ptr(), self._stream()), "rp_embed_fwd_rows")
+        else:
+            check(self.lib.rp_embed_fwd(p16["item_emb"].data_ptr(), prm["pos_emb"].data_ptr(), self.ids32.data_ptr(),
+                                        pad.data_ptr(), T, L, d, pos0, math.sqrt(cfg.d), int(legacy), drop, self.seed, 0,
+                                        self.rng_counter.data_ptr(), self.x[0].data_ptr(), self._stream()), "rp_embed_fwd")
+
+    def _feature_bwd(self, dx, drop: float):
+        """Side-feature gradients from the block input's gradient ``dx``: table rows by rp_feature_embed_bwd(_rows); the
+        numerical Linears' dW = dS^T . V and db = colsum(dS) by one fixed-order rp_wgrad_group(_rows) over its staging."""
+        cfg, G, T, d, st = self.cfg, self.grads, self.T, self.cfg.dp, self._stream
+        fa = self._feature_descs(True)
+        nc = cfg.num_cols
+        ds, vr = (self.feat_ds.data_ptr(), self.feat_v.data_ptr()) if nc else (None, None)
+        args = (cfg.hd_valid, math.sqrt(cfg.d), drop, self.seed, 0, self.rng_counter.data_ptr(), ds, vr, FEAT_MAX_NUM_COLS, st())
+        if self._packed:
+            check(self.lib.rp_feature_embed_bwd_rows(dx.data_ptr(), fa, len(fa), self.row_tok.data_ptr(), self.n_rows.data_ptr(),
+                                                     T, d, *args), "rp_feature_embed_bwd_rows")
+        else:
+            check(self.lib.rp_feature_embed_bwd(dx.data_ptr(), fa, len(fa), T, d, *args), "rp_feature_embed_bwd")
+        if not nc:
+            return
+        pair = (WgradPair * 1)()
+        p = pair[0]
+        p.dY, p.dy_ld, p.n_out = self.feat_ds.data_ptr(), d, d
+        p.X, p.x_ld, p.n_in = self.feat_v.data_ptr(), FEAT_MAX_NUM_COLS, FEAT_MAX_NUM_COLS
+        p.dW, p.dw_ld, p.db = self.feat_dw.data_ptr(), FEAT_MAX_NUM_COLS, self.feat_db.data_ptr()
+        need = self.lib.rp_wgrad_group_workspace(pair, 1)
+        if self._wgrad_ws is None or self._wgrad_ws.numel() < need:
+            self._wgrad_ws = torch.zeros(need, device=self.dev, dtype=torch.uint8)
+        if self._packed:
+            check(self.lib.rp_wgrad_group_rows(pair, 1, T, 0, self.n_rows.data_ptr(), self._wgrad_ws.data_ptr(),
+                                               self._wgrad_ws.numel(), st()), "rp_wgrad_group_rows")
+        else:
+            check(self.lib.rp_wgrad_group(pair, 1, T, 0, self._wgrad_ws.data_ptr(), self._wgrad_ws.numel(), st()), "rp_wgrad_group")
+        col = 0
+        for f in self.features:
+            if f.kind == "num":
+                G[f"feat.{f.name}.w"].add_(self.feat_dw[:, col:col + f.width])
+                G[f"feat.{f.name}.b"].add_(self.feat_db)
+                col += f.width
 
     def _alloc_body(self):
         """SASRec's block buffers: LN1 output, Q and packed [K | V], the FFN's saved activations, the predict path's last-row
@@ -752,15 +947,7 @@ class SasRecEngine:
         pad = self.in_pad
         pos0 = 0 if legacy else cfg.max_len - L
         packed = self._packed
-        if packed:
-            check(self.lib.rp_embed_fwd_rows(p16["item_emb"].data_ptr(), prm["pos_emb"].data_ptr(), self.ids32.data_ptr(),
-                                             pad.data_ptr(), self.row_tok.data_ptr(), self.n_rows.data_ptr(), T, L, d, pos0,
-                                             math.sqrt(cfg.d), 0, drop, self.seed, 0, self.rng_counter.data_ptr(),
-                                             self.x[0].data_ptr(), self._stream()), "rp_embed_fwd_rows")
-        else:
-            check(self.lib.rp_embed_fwd(p16["item_emb"].data_ptr(), prm["pos_emb"].data_ptr(), self.ids32.data_ptr(),
-                                        pad.data_ptr(), T, L, d, pos0, math.sqrt(cfg.d), int(legacy), drop, self.seed, 0,
-                                        self.rng_counter.data_ptr(), self.x[0].data_ptr(), self._stream()), "rp_embed_fwd")
+        self._embed_fwd(drop, pos0)
         H, hd = cfg.n_heads, d // cfg.n_heads
         for i in range(cfg.n_blocks):
             a, x = self.act[i], self.x[i]
@@ -1080,6 +1267,8 @@ class SasRecEngine:
                 self._colsum_multi([(dY, db) for dY, _, _, db in pairs])
             dx, other = other, dx
         pos0 = 0 if legacy else cfg.max_len - L
+        if self.features:
+            self._feature_bwd(dx, drop)
         if packed:
             check(self.lib.rp_embed_bwd_rows(dx.data_ptr(), self.ids32.data_ptr(), self.in_pad.data_ptr(), self.row_tok.data_ptr(),
                                              rows, self.seq_first.data_ptr(), self.seq_off.data_ptr(), self.B, L, d, cfg.pad_id,

@@ -3,8 +3,9 @@ from __future__ import annotations
 
 
 class SequenceEmbedding:
-    """replay/nn/embedding.py: one embedding per schema feature.  The CUDA path embeds the item id feature only; any other
-    feature that is not excluded is rejected when the model is built."""
+    """replay/nn/embedding.py: one embedding per schema feature that is not in ``excluded_features``.  The CUDA path
+    (csrc/rp_features.cu) embeds categorical features, categorical lists ("sum" / "mean") and numerical features of the
+    model's width next to the item id; the new-path SASRec body with SasRecTransformerLayer takes them."""
 
     def __init__(self, schema, excluded_features=None, categorical_list_feature_aggregation_method: str = "sum"):
         self.schema = schema

@@ -138,8 +138,9 @@ class LightningModule(LightningModuleBase):
                 raise ValueError(f"{type(spec).__name__} needs `negative_labels` in the batch")
             lr = self._current_lr()
             rw = spec.row_weights(batch["feature_tensors"], tm) if hasattr(spec, "row_weights") else None
+            side = {"feats": batch["feature_tensors"]} if getattr(core.cfg, "features", ()) else {}
             loss = core.fused_step(batch["feature_tensors"][core.item_feature], batch["padding_mask"], lab, tm,
-                                   lr=lr, negatives=neg, row_weights=rw)  # all_reduce="auto": DDP gradient exchange inside
+                                   lr=lr, negatives=neg, row_weights=rw, **side)  # all_reduce="auto": DDP exchange inside
             self.log("learning_rate", lr, on_step=True, on_epoch=True, prog_bar=True, sync_dist=True)
         else:
             loss = self(batch)["loss"]

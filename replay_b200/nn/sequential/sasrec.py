@@ -13,7 +13,7 @@ from ...core import SasRecCore
 from ..loss import CE
 from ...engine import EncoderConfig
 from ...engine_diff import DiffConfig, DiffEngine
-from ...schema import item_feature_of
+from ...schema import item_feature_of, side_features_of
 from ..agg import SumAggregator
 from ..embedding import SequenceEmbedding
 from ..mask import DefaultAttentionMask
@@ -112,9 +112,7 @@ class SasRecBody:
         if pad != card:
             raise ValueError("the item feature's padding_value must equal its cardinality (replay/data/nn/schema.py:89-90)")
         skip = set(emb.excluded_features) | {schema.query_id_feature_name, schema.timestamp_feature_name}
-        others = [f for f, _ in schema.items() if f not in skip and f != name]
-        if others:
-            raise ValueError(f"side features {others} are not supported; exclude them from the SequenceEmbedding")
+        side = side_features_of(schema, skip, emb.categorical_list_feature_aggregation_method)
         if not isinstance(agg, PositionAwareAggregator) or not isinstance(agg.embedding_aggregator, SumAggregator):
             raise ValueError("embedding_aggregator must be PositionAwareAggregator(SumAggregator(...), ...)")
         if not isinstance(mask, DefaultAttentionMask) or mask.reference_feature_name != name:
@@ -124,6 +122,9 @@ class SasRecBody:
         d = enc.embedding_dim
         if agg.embedding_aggregator.embedding_dim != d or (feat_dim is not None and feat_dim != d):
             raise ValueError("the embedder, the aggregator and the encoder must share one embedding_dim")
+        _check_side(schema, side, d)
+        if side and not isinstance(enc, SasRecTransformerLayer):
+            raise ValueError(f"side features {[f.name for f in side]} need the SasRecTransformerLayer encoder")
         if mask.num_heads != enc.num_heads:
             raise ValueError("attn_mask_builder.num_heads must equal the encoder's num_heads")
         if isinstance(norm, torch.nn.LayerNorm) and norm.elementwise_affine and norm.bias is not None:
@@ -143,11 +144,20 @@ class SasRecBody:
             if enc.dropout != agg.dropout:
                 raise ValueError("the aggregator and SasRecTransformerLayer must share one dropout")
             cfg = EncoderConfig(n_items=card, d=d, n_heads=enc.num_heads, n_blocks=enc.num_blocks,
-                                max_len=agg.max_sequence_length, dropout=agg.dropout, variant="new", lnf_eps=eps)
+                                max_len=agg.max_sequence_length, dropout=agg.dropout, variant="new", lnf_eps=eps,
+                                features=tuple(side))
             return SasRecCore(cfg, item_feature=name, device=device, seed=seed)
         cfg = DiffConfig(n_items=card, d=d, n_heads=enc.num_heads, n_blocks=enc.num_blocks, max_len=agg.max_sequence_length,
                          dropout=agg.dropout, out_norm=out_norm, lnf_eps=eps)
         return _DiffCore(cfg, item_feature=name, device=device, seed=seed)
+
+
+def _check_side(schema, side, d: int) -> None:
+    """Every side feature is summed into the d-wide input (SumAggregator): its embedding_dim must be d."""
+    for f in side:
+        if schema[f.name].embedding_dim != d:
+            raise ValueError(f"side feature {f.name!r} has embedding_dim {schema[f.name].embedding_dim}; SumAggregator needs "
+                             f"every feature at the model's embedding_dim {d}")
 
 
 class _InferenceOutput(dict):
@@ -193,13 +203,17 @@ class SasRec(torch.nn.Module):
     def from_params(cls, schema, embedding_dim: int = 192, num_heads: int = 4, num_blocks: int = 2,
                     max_sequence_length: int = 50, dropout: float = 0.3, excluded_features=None,
                     categorical_list_feature_aggregation_method: str = "sum", device=None, seed: int = 0) -> "SasRec":
-        """replay/nn/sequential/sasrec/model.py:199-253.  Only the item-id feature takes part (SURVEY §2: multi-feature
-        embedders are out of the hot-path scope); ReLU FFN, LayerNorm(eps=1e-5) output normalisation, full CE loss."""
+        """replay/nn/sequential/sasrec/model.py:199-253: every schema feature except the query id, the timestamp and
+        ``excluded_features`` is embedded and summed into the input (side features: csrc/rp_features.cu); ReLU FFN,
+        LayerNorm(eps=1e-5) output normalisation, full CE loss."""
         name, card, pad, _ = item_feature_of(schema)
         if pad != card:
             raise ValueError("the item feature's padding_value must equal its cardinality (replay/data/nn/schema.py:89-90)")
+        skip = {schema.query_id_feature_name, schema.timestamp_feature_name, *(excluded_features or [])}
+        side = side_features_of(schema, skip, categorical_list_feature_aggregation_method)
+        _check_side(schema, side, embedding_dim)
         cfg = EncoderConfig(n_items=card, d=embedding_dim, n_heads=num_heads, n_blocks=num_blocks,
-                            max_len=max_sequence_length, dropout=dropout, variant="new")
+                            max_len=max_sequence_length, dropout=dropout, variant="new", features=tuple(side))
         return cls(SasRecCore(cfg, item_feature=name, device=device, seed=seed))
 
     # ---- reference surface
@@ -243,16 +257,17 @@ class SasRec(torch.nn.Module):
             raise ValueError(f"{type(self._loss).__name__} needs negative_labels")
         rw = self._loss.row_weights(feature_tensors, target_padding_mask) if hasattr(self._loss, "row_weights") else None
         loss = self.core.loss(ids, padding_mask, positive_labels, target_padding_mask,
-                              negatives=negative_labels if self._loss.needs_negatives else None, row_weights=rw)
+                              negatives=negative_labels if self._loss.needs_negatives else None, row_weights=rw,
+                              **self._side(feature_tensors))
         return {"loss": loss, "hidden_states": ()}
 
     def forward_inference(self, feature_tensors, padding_mask, candidates_to_score=None):
         """model.py:292-307: ``logits`` = scores of the LAST position [B, |I|] (or [B, |C|]); ``hidden_states`` = ([B, L, d],).
         The scores come from the last-position shortcut of the engine; the all-position hidden states (a second, full pass over
         the body) are only computed if that key is actually read."""
-        ids = feature_tensors[self.core.item_feature]
-        logits = self.core.logits(ids, padding_mask, candidates_to_score)
-        return _InferenceOutput(logits, lambda: (self.core.hidden_states(ids, padding_mask).float(),))
+        ids, side = feature_tensors[self.core.item_feature], self._side(feature_tensors)
+        logits = self.core.logits(ids, padding_mask, candidates_to_score, **side)
+        return _InferenceOutput(logits, lambda: (self.core.hidden_states(ids, padding_mask, **side).float(),))
 
     def forward(self, feature_tensors, padding_mask, candidates_to_score=None, positive_labels=None, negative_labels=None,
                 target_padding_mask=None):
@@ -265,4 +280,9 @@ class SasRec(torch.nn.Module):
 
     # ---- fused extras
     def predict_topk(self, feature_tensors, padding_mask, k: int, seen_ids=None, candidates_to_score=None):
-        return self.core.predict_topk(feature_tensors[self.core.item_feature], padding_mask, k, seen_ids, candidates_to_score)
+        return self.core.predict_topk(feature_tensors[self.core.item_feature], padding_mask, k, seen_ids, candidates_to_score,
+                                      **self._side(feature_tensors))
+
+    def _side(self, feature_tensors) -> dict:
+        """The core's ``feats`` argument: the batch's feature tensors when the model embeds side features."""
+        return {"feats": feature_tensors} if getattr(self.core.cfg, "features", ()) else {}
