@@ -31,10 +31,11 @@ from test_gpu_attention import BIG, OFF, SENT, TOL_INV_REL, TOL_M_ABS, TOL_M_REL
 from test_gpu_attention import _case, _check_grads, _d_out, _heads, attn_grads_given_o, attn_ref, visibility
 from test_gpu_attention import block_err as head_block_err
 from test_gpu_packed_body import _windows, expected_plan
-from test_gpu_sasrec_body import (CTR, EPS, HALF_ULP_SLACK, P_DROP, SEED, TOL_BWD, TOL_LN_GRAD, TOL_SPLITK, TOL_SUM, TOL_ULP,
-                                  _assert_keep_pattern, _bf, _Case, _check_stats, _check_step, _ks, _leaves, _ln_fwd_atol, _map,
-                                  _post_attn_inputs, _site, _vec, _weights, _x_rows, engine_keeps, post_attn_bwd_ref,
-                                  post_attn_train_ref, ref_loss_and_grads, sasrec_ref, step_batch)
+from sasrec_fp64 import (CTR, EPS, P_DROP, SEED, _bf, _Case, _ks, _leaves, _map, _site, engine_keeps, ref_loss_and_grads,
+                         sasrec_ref, step_batch)
+from test_gpu_sasrec_body import (HALF_ULP_SLACK, TOL_BWD, TOL_LN_GRAD, TOL_SPLITK, TOL_SUM, TOL_ULP, _assert_keep_pattern,
+                                  _check_stats, _check_step, _ln_fwd_atol, _post_attn_inputs, _vec, _weights, _x_rows,
+                                  post_attn_bwd_ref, post_attn_train_ref)
 
 POISON = (float("nan"), float("inf"), float("-inf"))
 

@@ -24,14 +24,13 @@ import numpy as np
 import pytest
 import torch
 
-from dropout_stream import drop_keep, keep_draws
+from dropout_stream import keep_draws
 from fp64_checks import WorstErrors, block_err, feat_mask, ln_bwd_ref, ln_ref, seq_block_err, ulp_err
 from replay_b200._lib import WgradPair, check, lib
+from sasrec_fp64 import (CTR, EPS, P_DROP, SEED, _bf, _Case, _gen, _ks, _leaves, _map, _site, engine_keeps,
+                         ref_loss_and_grads, step_batch, unit_keeps)
 
 SENT = -3.25                           # sentinel for memory a kernel must not write (exact in bf16)
-SEED, CTR = 0x5EED1234ABC, 987654321   # dropout stream of the kernel-level tests (seed_ptr holds CTR)
-P_DROP = 0.2                           # config 2
-EPS = 1e-8                             # LayerNorm 1 / 2 of a SASRec block
 HALF_ULP_SLACK = 2.0 ** -21            # fp32 accumulation slack, times sum_k |a_k b_k|
 
 # Tolerances.  Each bound is about 3x the worst error observed over every case of this file on one H100 80GB HBM3
@@ -68,194 +67,6 @@ def cuda():
 
 def _stream():
     return torch.cuda.current_stream().cuda_stream
-
-
-def _gen(seed):
-    return torch.Generator().manual_seed(seed)
-
-
-def _bf(x):
-    return x.to(torch.bfloat16)
-
-
-def _ks(p):
-    return 1.0 / (1.0 - float(np.float32(p)))
-
-
-def _ru(x, m):
-    return (x + m - 1) // m * m
-
-
-def _site(blk, k):
-    """SasRecEngine._site: dropout site k of block blk (offset = site << 40; the embedding is offset 0)."""
-    return 1 + 8 * blk + k
-
-
-# ----------------------------------------------------------------------------------------------------------------------
-# float64 reference of the SASRec training loss with every dropout site
-# ----------------------------------------------------------------------------------------------------------------------
-def engine_keeps(seed_eff, p, B, L, cfg, site_shift=0, dev=None):
-    """Keep masks (0 or 1/(1-p), float64) of every dropout site of SasRecEngine's training body, in the model's true
-    feature space: the embedding at offset 0; per block attention probabilities at _site(i, 0) << 40 (row key
-    bz * Lp + i), the FFN hidden activation after the ReLU at _site(i, 1) << 40 and the FFN output before the residual at
-    _site(i, 2) << 40.  Token sites are drawn over the padded width dp (the kernels' column keys) and gathered at
-    cfg.feat_index().  ``site_shift`` moves every block site number (a plausible mistake)."""
-    T, Lp, ks = B * L, _ru(L, 64), _ks(p)
-    rows = np.arange(T)
-    feat = cfg.feat_index()
-
-    def tok(off):
-        return (keep_draws(seed_eff, off, p, rows, cfg.dp)[:, feat].double() * ks).view(B, L, cfg.d).to(dev)
-
-    out = {"emb": tok(0), "blocks": []}
-    for i in range(cfg.n_blocks):
-        s = lambda k: (_site(i, k) + site_shift) << 40  # noqa: E731
-        out["blocks"].append({"attn": drop_keep(seed_eff, s(0), p, B, cfg.n_heads, L, Lp).to(dev), "ffn1": tok(s(1)),
-                              "ffn2": tok(s(2))})
-    return out
-
-
-def unit_keeps(B, L, d, H, n_blocks):
-    ones = lambda *s: torch.ones(*s, dtype=torch.float64)  # noqa: E731
-    return {"emb": ones(B, L, d), "blocks": [{"attn": ones(B, H, L, L), "ffn1": ones(B, L, d), "ffn2": ones(B, L, d)}
-                                             for _ in range(n_blocks)]}
-
-
-def _ln64(x, w, b, eps, width=None):
-    """LayerNorm; ``width`` > d takes the statistics over ``width`` features of which the extra ones are zero (the
-    padded-width mistake)."""
-    n = x.shape[-1] if width is None else width
-    mu = x.sum(-1, keepdim=True) / n
-    var = (((x - mu) ** 2).sum(-1, keepdim=True) + (n - x.shape[-1]) * mu ** 2) / n
-    return (x - mu) / torch.sqrt(var + eps) * w + b
-
-
-def sasrec_ref(P, ids, pad, labels, tmask, H, variant, lnf_eps, keeps=None, mistake=None, dp=None):
-    """oracle.sasrec.sasrec_body + the full-catalog CE restated with a keep mask at every dropout site -> (loss, x[-1]
-    [B, L, d] before the final LayerNorm, hidden [B, L, d] after it).  ``mistake`` (a plausible kernel / engine error, for
-    the tolerance checks): 'ffn_drop_after_residual', 'ln_padded_width' (LayerNorm statistics over ``dp`` features),
-    'no_row_mask' (legacy), 'kv_from_normed', 'pos_first_rows' (the new path's positional window from the front)."""
-    B, L = ids.shape
-    item_emb, pos = P["item_emb"], P["pos_emb"]
-    d = item_emb.shape[1]
-    hd = d // H
-    I = item_emb.shape[0] - 1
-    width = dp if mistake == "ln_padded_width" else None
-    legacy = variant == "legacy"
-    real = pad[..., None].to(item_emb.dtype)
-    x = item_emb[ids.masked_fill(~pad, I)] * math.sqrt(d)
-    x = x + (pos[:L] if legacy or mistake == "pos_first_rows" else pos[pos.shape[0] - L:])
-    if keeps is not None:
-        x = x * keeps["emb"]
-    if legacy:
-        x = x * real
-    causal = torch.tril(torch.ones(L, L, dtype=torch.bool, device=ids.device))
-    vis = (causal[None] if legacy else causal[None] & pad[:, None, :])[:, None]
-    for i, blk in enumerate(P["blocks"]):
-        kb = keeps["blocks"][i] if keeps is not None else None
-        q_in = _ln64(x, blk["ln1_w"], blk["ln1_b"], EPS, width)
-        kv_in = q_in if mistake == "kv_from_normed" else x
-        w, b = blk["in_w"], blk["in_b"]
-        q = (q_in @ w[:d].T + b[:d]).view(B, L, H, hd).transpose(1, 2)
-        k = (kv_in @ w[d:2 * d].T + b[d:2 * d]).view(B, L, H, hd).transpose(1, 2)
-        v = (kv_in @ w[2 * d:].T + b[2 * d:]).view(B, L, H, hd).transpose(1, 2)
-        s = ((q @ k.transpose(-1, -2)) / math.sqrt(hd)).masked_fill(~vis, float("-inf"))
-        m = s.detach().amax(-1, keepdim=True)
-        m = torch.where(torch.isinf(m), torch.zeros_like(m), m)
-        e = torch.exp(s - m)
-        den = e.sum(-1, keepdim=True)
-        pr = torch.where(den > 0, e / den.clamp_min(1e-300), torch.zeros_like(e))
-        if kb is not None:
-            pr = pr * kb["attn"]
-        o = (pr @ v).transpose(1, 2).reshape(B, L, d)
-        h = q_in + o @ blk["out_w"].T + blk["out_b"]
-        y = _ln64(h, blk["ln2_w"], blk["ln2_b"], EPS, width)
-        u = torch.relu(y @ blk["w1"].T + blk["b1"])
-        if kb is not None:
-            u = u * kb["ffn1"]
-        t = u @ blk["w2"].T + blk["b2"]
-        if kb is not None and mistake == "ffn_drop_after_residual":
-            x = (y + t) * kb["ffn2"]
-        else:
-            x = y + (t * kb["ffn2"] if kb is not None else t)
-        if legacy and mistake != "no_row_mask":
-            x = x * real
-    hid = _ln64(x, P["lnf_w"], P["lnf_b"], lnf_eps, width)
-    sel = tmask & (labels >= 0) & (labels < I)
-    logits = hid[sel] @ item_emb[:I].T
-    loss = (torch.logsumexp(logits, -1) - logits.gather(1, labels[sel][:, None])[:, 0]).mean()
-    return loss, x, hid
-
-
-_BLOCK_KEYS = ("ln1_w", "ln1_b", "in_w", "in_b", "out_w", "out_b", "ln2_w", "ln2_b", "w1", "b1", "w2", "b2")
-
-
-def _leaves(P):
-    """[(name, tensor)] of a canonical parameter dict in SasRecEngine's naming."""
-    out = [("item_emb", P["item_emb"]), ("pos_emb", P["pos_emb"])]
-    for i, blk in enumerate(P["blocks"]):
-        out += [(f"b{i}.{k}", blk[k]) for k in _BLOCK_KEYS]
-    return out + [("lnf_w", P["lnf_w"]), ("lnf_b", P["lnf_b"])]
-
-
-def _map(P, f):
-    Q = {k: f(k, v) for k, v in P.items() if k != "blocks"}
-    Q["blocks"] = [{k: f(f"b{i}.{k}", v) for k, v in blk.items()} for i, blk in enumerate(P["blocks"])]
-    return Q
-
-
-def ref_loss_and_grads(P, ids, pad, labels, tmask, H, variant, lnf_eps, keeps=None, mistake=None, dp=None):
-    """float64 loss, x[-1], hidden states and autograd gradients {name: tensor} (the pad row of item_emb frozen)."""
-    Q = _map(P, lambda k, v: v.detach().double().clone().requires_grad_(True))
-    loss, x, hid = sasrec_ref(Q, ids, pad, labels, tmask, H, variant, lnf_eps, keeps, mistake, dp)
-    leaves = _leaves(Q)
-    grads = torch.autograd.grad(loss, [t for _, t in leaves], allow_unused=True)
-    G = {k: (g if g is not None else torch.zeros_like(t)) for (k, t), g in zip(leaves, grads)}
-    G["item_emb"][-1] = 0
-    return loss.detach(), x.detach(), hid.detach(), G
-
-
-# the bf16-consumed parameters of SasRecEngine (the kernels read their bf16 shadow): the reference uses them rounded
-_BF16_PARAMS = ("item_emb", "in_w", "out_w", "w1", "w2")
-
-
-def engine_view(P):
-    """The parameters as SasRecEngine computes with them: bf16-consumed ones rounded to bf16, the rest fp32."""
-    return _map(P, lambda k, v: (_bf(v).float() if k.split(".")[-1] in _BF16_PARAMS else v.float()))
-
-
-_LENGTHS = [200, 200, 150, 57, 13, 1, 120]
-
-
-def step_batch(B, L, I, seed):
-    """Left-padded histories of lengths 200, 200, 150, 57, 13, 1, 120 (repeated), next-item labels on ~90 % of the real
-    positions."""
-    g = _gen(seed)
-    pad = torch.zeros(B, L, dtype=torch.bool)
-    for b in range(B):
-        pad[b, L - min(_LENGTHS[b % len(_LENGTHS)], L):] = True
-    items = torch.randint(0, I, (B, L + 1), generator=g)
-    ids = torch.where(pad, items[:, :-1], torch.zeros_like(pad, dtype=torch.int64))
-    labels = items[:, 1:]
-    tmask = pad & (torch.rand(B, L, generator=g) > 0.1)
-    return ids, pad, labels, tmask
-
-
-class _Case:
-    """One configuration of the step test: the engine's EncoderConfig, the reference's view of it, the fused-body flag."""
-
-    def __init__(self, variant, d, H, fused=True, L=200, I=2000):
-        from replay_b200.engine import EncoderConfig
-
-        self.variant, self.d, self.H, self.fused, self.L, self.I = variant, d, H, fused, L, I
-        self.max_len = L if variant == "legacy" else L + 10     # the new path's positional window is offset
-        self.cfg = EncoderConfig(n_items=I, d=d, n_heads=H, n_blocks=2, max_len=self.max_len, variant=variant)
-        self.lnf_eps = self.cfg.lnf_eps
-
-    def params(self, seed):
-        from oracle import sasrec as osr
-
-        return engine_view(osr.random_params(self.I, self.d, self.max_len, 2, seed=seed, bias_scale=0.1))
 
 
 _CASES = {"c2": ("new", 128, 2, True), "c2_unfused": ("new", 128, 2, False), "d64h2": ("new", 64, 2, True),

@@ -8,7 +8,8 @@ import torch
 from dropout_stream import keep_draws
 from test_gpu_packed_body import expected_plan
 from test_gpu_packed_fp64 import T_CAP, _attn_firsts, _tokens, plan_batch
-from test_gpu_sasrec_body import (CTR, P_DROP, SEED, TOL_ULP, _bf, _ks, _post_attn_inputs, _site, post_attn_train_ref)
+from sasrec_fp64 import CTR, P_DROP, SEED, _bf, _ks, _site
+from test_gpu_sasrec_body import TOL_ULP, _post_attn_inputs, post_attn_train_ref
 from fp64_checks import ulp_err
 
 
