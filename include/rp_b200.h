@@ -319,6 +319,21 @@ int rp_feature_embed_bwd_rows(const void* dx, const rp_feature* feats, int n_fea
                               const int32_t* n_rows_dev, int T, int d, int hd_valid, float scale, float drop_p,
                               unsigned long long seed, unsigned long long drop_off, const unsigned long long* seed_ptr,
                               void* d_s, void* v_rows, int v_ld, void* stream);
+/* The BERT form (legacy BERT4Rec's BertEmbedding with side features, bert4rec/model.py:173-296):
+ *   x[t] = dropout(where(tok_mask[t], table[ids[t]] + sum_f term_f(t), mask_emb) + pos[t % L])
+ * with no scale, pos == NULL for no positional term, and the dropout stream of rp_bert_embed_fwd (row key = token t), so
+ * all-zero side tables and values give exactly rp_bert_embed_fwd's output.  Kinds RP_FEAT_CAT and RP_FEAT_IDENT only; any
+ * other kind is RP_EINVAL.  A BERT categorical table has no padding row: pass padding_value = -1, so every id in
+ * [0, n_rows) is a row.  An id outside [0, n_rows) adds zero (the reference raises IndexError there).  T a multiple of L.
+ * Backward (the item table, mask_emb and pos stay with rp_bert_embed_bwd): dS = dropout'(dx) is added into each categorical
+ * d_table row with fp32 atomics, at tokens with pad_mask && tok_mask only; identity features take no gradient. */
+int rp_bert_feature_embed_fwd(const void* item_table, const void* mask_emb, const float* pos, const int32_t* ids,
+                              const uint8_t* tok_mask, const rp_feature* feats, int n_feats, int T, int L, int d, int hd_valid,
+                              float drop_p, unsigned long long seed, unsigned long long drop_off,
+                              const unsigned long long* seed_ptr, void* out, void* stream);
+int rp_bert_feature_embed_bwd(const void* dx, const uint8_t* pad_mask, const uint8_t* tok_mask, const rp_feature* feats,
+                              int n_feats, int T, int d, int hd_valid, float drop_p, unsigned long long seed,
+                              unsigned long long drop_off, const unsigned long long* seed_ptr, void* stream);
 
 /* torch.nn.LayerNorm forward / backward (transformer.py:47-49,60-62 eps 1e-8; model.py:248 eps 1e-5).  With `gather`
  * output row r reads input row gather[r] and only *n_rows_dev rows exist (valid-target compaction); the backward then

@@ -237,7 +237,7 @@ class DiffAttnDesc(ctypes.Structure):
 
 
 class RpFeature(ctypes.Structure):
-    """Mirror of ``struct rp_feature`` (include/rp_b200.h): one side feature of the SASRec input stage."""
+    """Mirror of ``struct rp_feature`` (include/rp_b200.h): one side feature of the SASRec or BERT4Rec input stage."""
 
     _fields_ = [
         ("kind", c_int), ("width", c_int), ("n_rows", c_int), ("padding_value", c_int), ("val_col", c_int),
@@ -284,6 +284,10 @@ _EXTRA_SIGS: list = [
                                      _P, _P, c_int, _P]),
     ("rp_feature_embed_bwd_rows", c_int, [_P, ctypes.POINTER(RpFeature), c_int, _P, _P, c_int, c_int, c_int, c_float, c_float,
                                           _U64, _U64, _P, _P, _P, c_int, _P]),
+    ("rp_bert_feature_embed_fwd", c_int, [_P, _P, _P, _P, _P, ctypes.POINTER(RpFeature), c_int, c_int, c_int, c_int, c_int,
+                                          c_float, _U64, _U64, _P, _P, _P]),
+    ("rp_bert_feature_embed_bwd", c_int, [_P, _P, _P, ctypes.POINTER(RpFeature), c_int, c_int, c_int, c_int, c_float, _U64,
+                                          _U64, _P, _P]),
 ]
 
 __all__ = ["GemmDesc", "DiffAttnDesc", "DiffLambda", "SceDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "RpFeature", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]

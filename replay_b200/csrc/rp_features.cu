@@ -13,6 +13,15 @@
 // Backward (rp_embed_bwd keeps the item table and the positions): dS = scale * dropout'(dx) is scattered into the side
 // tables with fp32 atomics (padding rows frozen, mean bags scaled by 1 / count), and written as bf16 next to the gathered
 // numerical values, the operands of the weight-gradient GEMM (rp_wgrad_group) that gives dW and db in a fixed order.
+//
+// The BERT form (template flag BERT; legacy bert4rec/model.py:173-296, BertEmbedding with sum aggregation):
+//
+//   s_t = E_item[id_t] + sum_cat E_f[id_f,t] + sum_ident v_f,t
+//   x_t = dropout(where(token_mask_t, s_t, mask_emb) + P[t % L])        (no sqrt(d) scale; P optional)
+//
+// Its categorical tables have no padding row (the host passes padding_value = -1), and its dropout is rp_bert_embed_fwd's
+// stream.  Backward: dS = dropout'(dx) goes to the side tables at the real, unmasked tokens only; rp_bert_embed_bwd keeps
+// the item table, mask_emb and the positions.  The SASRec instantiations compile none of this.
 #include "rp_b200.h"
 #include "rp_host.h"
 #include "rp_philox.cuh"
@@ -47,12 +56,13 @@ __device__ __forceinline__ void add_row(float* acc, const __nv_bfloat16* row, fl
 }
 
 // row r of the output is token row_tok[r] (packed rows, *n_rows_dev of them) or token r (row_tok == null, n_tok rows)
-template <int VEC>
+// BERT: tok_mask / mask_emb replace the masked tokens' sum, pos may be null, scale is not applied (only CAT and IDENT kinds)
+template <int VEC, bool BERT>
 __global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) feature_embed_fwd_kernel(
     const __nv_bfloat16* __restrict__ item, const float* __restrict__ pos, const int32_t* __restrict__ ids, const __grid_constant__ FeatArgs fa,
     int n_tok, int L, int hd_valid, int pos0, float scale, float drop_p, unsigned long long seed, unsigned long long drop_off,
     const unsigned long long* __restrict__ seed_ptr, const int32_t* __restrict__ row_tok, const int32_t* __restrict__ n_rows_dev,
-    __nv_bfloat16* __restrict__ out) {
+    const uint8_t* __restrict__ tok_mask, const __nv_bfloat16* __restrict__ mask_emb, __nv_bfloat16* __restrict__ out) {
   if (drop_p > 0.f && seed_ptr) seed += *seed_ptr;
   constexpr int D = VEC * 32;
   const int n = n_rows_dev ? *n_rows_dev : n_tok;
@@ -65,10 +75,12 @@ __global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) feature_embed_fwd_kern
     float acc[VEC];
 #pragma unroll
     for (int i = 0; i < VEC; ++i) acc[i] = 0.f;
-    add_row<VEC>(acc, item + (size_t)ids[t] * D + c0, 1.f);
-    for (int k = 0; k < fa.n; ++k) {
+    // BERT's <MASK> and pad tokens take mask_emb in place of the whole sum, so nothing else is gathered for them
+    const bool masked = BERT && !tok_mask[t];
+    add_row<VEC>(acc, masked ? mask_emb + c0 : item + (size_t)ids[t] * D + c0, 1.f);
+    for (int k = 0; k < (masked ? 0 : fa.n); ++k) {
       const rp_feature& f = fa.f[k];
-      if (f.kind == RP_FEAT_CAT || f.kind == RP_FEAT_BAG_SUM || f.kind == RP_FEAT_BAG_MEAN) {
+      if (f.kind == RP_FEAT_CAT || (!BERT && (f.kind == RP_FEAT_BAG_SUM || f.kind == RP_FEAT_BAG_MEAN))) {
         const int32_t* v = reinterpret_cast<const int32_t*>(f.values) + (size_t)t * f.width;
         const __nv_bfloat16* tab = reinterpret_cast<const __nv_bfloat16*>(f.table);
         float bag[VEC];
@@ -84,7 +96,7 @@ __global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) feature_embed_fwd_kern
         const float w = (f.kind == RP_FEAT_BAG_MEAN && cnt > 0) ? 1.f / (float)cnt : 1.f;
 #pragma unroll
         for (int i = 0; i < VEC; ++i) acc[i] += bag[i] * w;
-      } else if (f.kind == RP_FEAT_NUM) {
+      } else if (!BERT && f.kind == RP_FEAT_NUM) {
         const float* v = reinterpret_cast<const float*>(f.values) + (size_t)t * f.width;
         const float* W = reinterpret_cast<const float*>(f.table);
 #pragma unroll
@@ -103,9 +115,17 @@ __global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) feature_embed_fwd_kern
         }
       }
     }
-    const float* p = pos + (size_t)(pos0 + t % L) * D + c0;
+    if (BERT) {
+      if (pos) {
+        const float* p = pos + (size_t)(t % L) * D + c0;
 #pragma unroll
-    for (int i = 0; i < VEC; ++i) acc[i] = acc[i] * scale + p[i];
+        for (int i = 0; i < VEC; ++i) acc[i] += p[i];
+      }
+    } else {
+      const float* p = pos + (size_t)(pos0 + t % L) * D + c0;
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) acc[i] = acc[i] * scale + p[i];
+    }
     if (drop_p > 0.f) {
       const uint32_t rk = drop_row_key(seed, drop_off, (unsigned long long)t);
 #pragma unroll
@@ -128,11 +148,13 @@ __device__ __forceinline__ void scatter_row(float* dst, const float* g, float w)
   }
 }
 
-template <int VEC>
+// BERT: only tokens with pad_mask && tok_mask reach the tables (a masked token's sum was replaced by mask_emb); CAT only
+template <int VEC, bool BERT>
 __global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) feature_embed_bwd_kernel(
     const __nv_bfloat16* __restrict__ dx, const __grid_constant__ FeatArgs fa, int n_tok, float scale, float drop_p, unsigned long long seed,
     unsigned long long drop_off, const unsigned long long* __restrict__ seed_ptr, const int32_t* __restrict__ row_tok,
-    const int32_t* __restrict__ n_rows_dev, __nv_bfloat16* __restrict__ d_s, __nv_bfloat16* __restrict__ v_rows, int v_ld) {
+    const int32_t* __restrict__ n_rows_dev, __nv_bfloat16* __restrict__ d_s, __nv_bfloat16* __restrict__ v_rows, int v_ld,
+    const uint8_t* __restrict__ pad_mask, const uint8_t* __restrict__ tok_mask) {
   if (drop_p > 0.f && seed_ptr) seed += *seed_ptr;
   constexpr int D = VEC * 32;
   const int n = n_rows_dev ? *n_rows_dev : n_tok;
@@ -142,6 +164,7 @@ __global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) feature_embed_bwd_kern
   const float ks = (drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f) * scale;
   for (int r = blockIdx.x * wpb + (threadIdx.x >> 5); r < n; r += gridDim.x * wpb) {
     const int t = row_tok ? row_tok[r] : r;
+    if (BERT && !(pad_mask[t] && tok_mask[t])) continue;
     float g[VEC];
     const __nv_bfloat16* gx = dx + (size_t)r * D + c0;
 #pragma unroll
@@ -156,20 +179,20 @@ __global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) feature_embed_bwd_kern
       for (int i = 0; i < VEC; ++i)
         if (drop_mix(rk, drop_col_key((uint32_t)(c0 + i))) < thr) g[i] = 0.f;
     }
-    if (d_s) {
+    if (!BERT && d_s) {
       __nv_bfloat16* o = d_s + (size_t)r * D + c0;
 #pragma unroll
       for (int i = 0; i < VEC; i += 2) *reinterpret_cast<uint32_t*>(o + i) = pack_bf16(g[i], g[i + 1]);
     }
-    if (v_rows)  // zero the staging row first: its numerical columns are written below, the padding columns stay zero
+    if (!BERT && v_rows)  // zero the staging row first: its numerical columns are written below, the padding columns stay zero
       for (int j = lane; j < v_ld; j += 32) v_rows[(size_t)r * v_ld + j] = __float2bfloat16(0.f);
     __syncwarp();
     for (int k = 0; k < fa.n; ++k) {
       const rp_feature& f = fa.f[k];
-      if (f.kind == RP_FEAT_CAT || f.kind == RP_FEAT_BAG_SUM || f.kind == RP_FEAT_BAG_MEAN) {
+      if (f.kind == RP_FEAT_CAT || (!BERT && (f.kind == RP_FEAT_BAG_SUM || f.kind == RP_FEAT_BAG_MEAN))) {
         const int32_t* v = reinterpret_cast<const int32_t*>(f.values) + (size_t)t * f.width;
         float w = 1.f;
-        if (f.kind == RP_FEAT_BAG_MEAN) {
+        if (!BERT && f.kind == RP_FEAT_BAG_MEAN) {
           int cnt = 0;
           for (int j = 0; j < f.width; ++j) cnt += feat_live(v[j], f);
           w = cnt > 0 ? 1.f / (float)cnt : 0.f;
@@ -178,7 +201,7 @@ __global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) feature_embed_bwd_kern
           const int id = v[j];
           if (feat_live(id, f)) scatter_row<VEC>(f.d_table + (size_t)id * D + c0, g, w);
         }
-      } else if (f.kind == RP_FEAT_NUM && v_rows) {
+      } else if (!BERT && f.kind == RP_FEAT_NUM && v_rows) {
         const float* v = reinterpret_cast<const float*>(f.values) + (size_t)t * f.width;
         for (int j = lane; j < f.width; j += 32) v_rows[(size_t)r * v_ld + f.val_col + j] = __float2bfloat16(v[j]);
       }
@@ -206,7 +229,9 @@ static inline int feat_grid(long long rows) {   // one warp per row, about 8 blo
 }
 
 // shared argument checks: RP_EINVAL for a null pointer or unknown kind, RP_ESHAPE for a size the kernels do not take
-static int feat_args(const rp_feature* feats, int n_feats, int d, int hd_valid, bool bwd, int v_ld, FeatArgs* fa) {
+// bert: the BERT form, which takes the CAT and IDENT kinds only
+static int feat_args(const rp_feature* feats, int n_feats, int d, int hd_valid, bool bwd, int v_ld, FeatArgs* fa,
+                     bool bert = false) {
   if (n_feats < 0 || n_feats > RP_FEAT_MAX || (n_feats > 0 && !feats)) return n_feats < 0 || n_feats > RP_FEAT_MAX ? RP_ESHAPE : RP_EINVAL;
   if (hd_valid < 0 || hd_valid > 128 || (hd_valid > 0 && d % (hd_valid <= 64 ? 64 : 128))) return RP_ESHAPE;
   const int d_true = hd_valid ? d / (hd_valid <= 64 ? 64 : 128) * hd_valid : d;
@@ -215,6 +240,7 @@ static int feat_args(const rp_feature* feats, int n_feats, int d, int hd_valid, 
   for (int k = 0; k < n_feats; ++k) {
     const rp_feature& f = feats[k];
     if (!f.values) return RP_EINVAL;
+    if (bert && f.kind != RP_FEAT_CAT && f.kind != RP_FEAT_IDENT) return RP_EINVAL;
     if (f.width <= 0) return RP_ESHAPE;
     switch (f.kind) {
       case RP_FEAT_CAT:
@@ -252,9 +278,9 @@ static int feature_fwd(const void* item_table, const float* pos, const int32_t* 
   const int rc = feat_args(feats, n_feats, d, hd_valid, false, 0, &fa);
   if (rc != RP_OK) return rc;
   const int grid = feat_grid(T);
-  RP_FEAT_DISPATCH(d, (feature_embed_fwd_kernel<VEC><<<grid, 256, 0, stream>>>(
+  RP_FEAT_DISPATCH(d, (feature_embed_fwd_kernel<VEC, false><<<grid, 256, 0, stream>>>(
                           reinterpret_cast<const __nv_bfloat16*>(item_table), pos, ids, fa, T, L, hd_valid, pos0, scale, drop_p,
-                          seed, drop_off, seed_ptr, row_tok, n_rows_dev, reinterpret_cast<__nv_bfloat16*>(out))));
+                          seed, drop_off, seed_ptr, row_tok, n_rows_dev, nullptr, nullptr, reinterpret_cast<__nv_bfloat16*>(out))));
   RP_LAUNCH_CHECK();
   return RP_OK;
 }
@@ -273,9 +299,10 @@ static int feature_bwd(const void* dx, const rp_feature* feats, int n_feats, con
   for (int k = 0; k < n_feats; ++k) has_num |= feats[k].kind == RP_FEAT_NUM;
   if (has_num && (!d_s || !v_rows)) return RP_EINVAL;
   const int grid = feat_grid(T);
-  RP_FEAT_DISPATCH(d, (feature_embed_bwd_kernel<VEC><<<grid, 256, 0, stream>>>(
+  RP_FEAT_DISPATCH(d, (feature_embed_bwd_kernel<VEC, false><<<grid, 256, 0, stream>>>(
                           reinterpret_cast<const __nv_bfloat16*>(dx), fa, T, scale, drop_p, seed, drop_off, seed_ptr, row_tok,
-                          n_rows_dev, reinterpret_cast<__nv_bfloat16*>(d_s), reinterpret_cast<__nv_bfloat16*>(v_rows), v_ld)));
+                          n_rows_dev, reinterpret_cast<__nv_bfloat16*>(d_s), reinterpret_cast<__nv_bfloat16*>(v_rows), v_ld,
+                          nullptr, nullptr)));
   RP_LAUNCH_CHECK();
   return RP_OK;
 }
@@ -311,4 +338,43 @@ RP_API int rp_feature_embed_bwd_rows(const void* dx, const rp_feature* feats, in
   if (!row_tok || !n_rows_dev) return RP_EINVAL;
   return feature_bwd(dx, feats, n_feats, row_tok, n_rows_dev, T, d, hd_valid, scale, drop_p, seed, drop_off, seed_ptr, d_s,
                      v_rows, v_ld, stream);
+}
+
+// ---- the BERT form (legacy BERT4Rec's BertEmbedding over side features): see the top of this file and include/rp_b200.h
+RP_API int rp_bert_feature_embed_fwd(const void* item_table, const void* mask_emb, const float* pos, const int32_t* ids,
+                                     const uint8_t* tok_mask, const rp_feature* feats, int n_feats, int T, int L, int d,
+                                     int hd_valid, float drop_p, unsigned long long seed, unsigned long long drop_off,
+                                     const unsigned long long* seed_ptr, void* out, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  // pos == null: no positional term (enable_positional_embedding=False)
+  if (!item_table || !mask_emb || !ids || !tok_mask || !out || T <= 0 || L <= 0) return RP_EINVAL;
+  if (drop_p < 0.f || drop_p >= 1.f) return RP_EINVAL;
+  if (T % L != 0) return RP_ESHAPE;
+  FeatArgs fa;
+  const int rc = feat_args(feats, n_feats, d, hd_valid, false, 0, &fa, true);
+  if (rc != RP_OK) return rc;
+  const int grid = feat_grid(T);
+  RP_FEAT_DISPATCH(d, (feature_embed_fwd_kernel<VEC, true><<<grid, 256, 0, stream>>>(
+                          reinterpret_cast<const __nv_bfloat16*>(item_table), pos, ids, fa, T, L, hd_valid, 0, 1.f, drop_p, seed,
+                          drop_off, seed_ptr, nullptr, nullptr, tok_mask, reinterpret_cast<const __nv_bfloat16*>(mask_emb),
+                          reinterpret_cast<__nv_bfloat16*>(out))));
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+RP_API int rp_bert_feature_embed_bwd(const void* dx, const uint8_t* pad_mask, const uint8_t* tok_mask, const rp_feature* feats,
+                                     int n_feats, int T, int d, int hd_valid, float drop_p, unsigned long long seed,
+                                     unsigned long long drop_off, const unsigned long long* seed_ptr, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!dx || !pad_mask || !tok_mask || T <= 0) return RP_EINVAL;
+  if (drop_p < 0.f || drop_p >= 1.f) return RP_EINVAL;
+  FeatArgs fa;
+  const int rc = feat_args(feats, n_feats, d, hd_valid, true, 0, &fa, true);
+  if (rc != RP_OK) return rc;
+  const int grid = feat_grid(T);
+  RP_FEAT_DISPATCH(d, (feature_embed_bwd_kernel<VEC, true><<<grid, 256, 0, stream>>>(
+                          reinterpret_cast<const __nv_bfloat16*>(dx), fa, T, 1.f, drop_p, seed, drop_off, seed_ptr, nullptr,
+                          nullptr, nullptr, nullptr, 0, pad_mask, tok_mask)));
+  RP_LAUNCH_CHECK();
+  return RP_OK;
 }

@@ -127,11 +127,26 @@ class SideFeature:
 _FEAT_KINDS = {"cat": FEAT_CAT, "bag_sum": FEAT_BAG_SUM, "bag_mean": FEAT_BAG_MEAN, "num": FEAT_NUM, "ident": FEAT_IDENT}
 
 
+def _check_side_features(fs, d: int, kinds):
+    """The checks SASRec's and BERT4Rec's side features share: at most FEAT_MAX of them with distinct names, every kind one
+    of ``kinds``, positive cardinalities, and identity features as wide as the true hidden size ``d``."""
+    if len(fs) > FEAT_MAX or len({f.name for f in fs}) != len(fs):
+        raise ValueError(f"at most {FEAT_MAX} side features with distinct names")
+    for f in fs:
+        if f.kind not in kinds:
+            raise ValueError(f"side feature {f.name!r}: unknown kind {f.kind!r}")
+        if f.categorical and f.cardinality < 1:
+            raise ValueError(f"side feature {f.name!r}: cardinality must be positive")
+        if f.kind == "ident" and f.width != d:
+            raise ValueError(f"side feature {f.name!r}: an identity feature needs tensor_dim == {d}")
+
+
 @dataclass
 class EncoderConfig(BaseConfig):
     variant: str = "new"  # "new": replay.nn.sequential.SasRec ; "legacy": replay.models.nn.sequential.SasRecModel
     lnf_eps: float | None = None
     features: tuple = ()  # SideFeature, ... (new path only); empty: the item-only input of rp_embed_fwd
+    side_pad_rows = True  # a categorical side table has cardinality + 1 rows, its padding row zero and frozen
 
     def __post_init__(self):
         if self.variant not in ("new", "legacy"):
@@ -148,15 +163,8 @@ class EncoderConfig(BaseConfig):
         fs = self.features
         if self.variant != "new":
             raise ValueError("side features exist on the new-path SASRec only")
-        if len(fs) > FEAT_MAX or len({f.name for f in fs}) != len(fs):
-            raise ValueError(f"at most {FEAT_MAX} side features with distinct names")
+        _check_side_features(fs, self.d, _FEAT_KINDS)
         for f in fs:
-            if f.kind not in _FEAT_KINDS:
-                raise ValueError(f"side feature {f.name!r}: unknown kind {f.kind!r}")
-            if f.categorical and f.cardinality < 1:
-                raise ValueError(f"side feature {f.name!r}: cardinality must be positive")
-            if f.kind == "ident" and f.width != self.d:
-                raise ValueError(f"side feature {f.name!r}: an identity feature needs tensor_dim == {self.d}")
             if f.kind == "num" and f.width < 1:
                 raise ValueError(f"side feature {f.name!r}: tensor_dim must be positive")
         if self.num_cols > FEAT_MAX_NUM_COLS:
@@ -195,7 +203,8 @@ class _CountingLib:
                "rp_score_topk": 2, "rp_seen_prepare": 1, "rp_sampled_head_fwd": 4, "rp_sampled_head_bwd": 4, "rp_post_attn_fused": 1,
                "rp_post_attn_train": 1, "rp_wgrad_group": 2, "rp_ln_qkv_fused": 1, "rp_pre_attn_bwd": 1,
                "rp_post_attn_bwd": 1, "rp_row_plan": 3, "rp_embed_fwd_rows": 1, "rp_embed_bwd_rows": 2, "rp_ln_qkv_fused_rows": 1,
-               "rp_post_attn_train_rows": 1, "rp_post_attn_bwd_rows": 1, "rp_pre_attn_bwd_rows": 1, "rp_wgrad_group_rows": 2}
+               "rp_post_attn_train_rows": 1, "rp_post_attn_bwd_rows": 1, "rp_pre_attn_bwd_rows": 1, "rp_wgrad_group_rows": 2,
+               "rp_bert_feature_embed_fwd": 1, "rp_bert_feature_embed_bwd": 1}
 
     def __init__(self, L):
         self._L = L
@@ -235,7 +244,8 @@ class SasRecEngine:
             off = _ru(off + math.prod(shp), 64)
         self._true = cfg.true_shapes()
         self.features = tuple(getattr(cfg, "features", ()))
-        self._side_pad = {f"feat.{f.name}": f.padding_value for f in self.features if f.categorical}
+        self._side_pad = {f"feat.{f.name}": f.padding_value for f in self.features
+                          if f.categorical and cfg.side_pad_rows}
         self.n_flat = off
         f32 = dict(device=self.dev, dtype=torch.float32)
         self.p32 = torch.zeros(off, **f32)
@@ -490,7 +500,7 @@ class SasRecEngine:
                 self.feat_in[f.name] = torch.full((self.T, 1), f.padding_value, **i32)
             elif not f.categorical:
                 self.feat_in[f.name] = torch.zeros(self.T, f.width, **f32)
-        if self.with_grad and self.cfg.num_cols:
+        if self.with_grad and any(f.kind == "num" for f in self.features):
             self.feat_ds = torch.zeros(self.T, self.cfg.dp, device=self.dev, dtype=torch.bfloat16)
             self.feat_v = torch.zeros(self.T, FEAT_MAX_NUM_COLS, device=self.dev, dtype=torch.bfloat16)
             self.feat_dw = torch.zeros(self.cfg.dp, FEAT_MAX_NUM_COLS, **f32)
@@ -535,7 +545,9 @@ class SasRecEngine:
             a, buf = arr[k], self.feat_in[f.name]
             a.kind, a.width, a.values = _FEAT_KINDS[f.kind], buf.shape[1], buf.data_ptr()
             if f.categorical:
-                a.n_rows, a.padding_value = f.cardinality + 1, f.padding_value
+                # without padding rows (BERT4Rec) every id in [0, cardinality) is a row: -1 matches no id
+                a.n_rows, a.padding_value = ((f.cardinality + 1, f.padding_value) if self.cfg.side_pad_rows
+                                             else (f.cardinality, -1))
                 a.table = self.params16[f"feat.{f.name}"].data_ptr()
                 a.d_table = self.grads[f"feat.{f.name}"].data_ptr() if with_grad else None
             elif f.kind == "num":

@@ -10,7 +10,7 @@ from dataclasses import dataclass
 import torch
 
 from ._lib import check
-from .engine import BaseConfig, SasRecEngine, _ru
+from .engine import BaseConfig, SasRecEngine, _check_side_features, _ru
 
 
 @dataclass
@@ -23,6 +23,10 @@ class BertConfig(BaseConfig):
     # no block at all, as the reference's range(0) does
     passes: int = 1
     positional: bool = True   # enable_positional_embedding: the learned position table pos_emb [max_len, d]
+    # side features summed into the item embedding (BertEmbedding, bert4rec/model.py:173-296): kinds "cat" (an Embedding of
+    # cardinality rows, no padding row) and "ident" (tensor_dim == d, the values themselves); empty: item-only
+    features: tuple = ()
+    side_pad_rows = False
 
     def __post_init__(self):
         if int(self.passes) != self.passes or self.passes < 0:
@@ -30,6 +34,8 @@ class BertConfig(BaseConfig):
         super().__post_init__()
         if 1 + 8 * self.n_apps >= 1 << 24:   # a dropout site's offset is site << 40 in a 64-bit counter
             raise ValueError(f"{self.n_blocks} blocks x {self.passes} passes exceed the dropout sites' numbering")
+        self.features = tuple(self.features)
+        _check_side_features(self.features, self.d, ("cat", "ident"))
 
     @property
     def n_apps(self) -> int:
@@ -66,7 +72,9 @@ class BertConfig(BaseConfig):
             out += self._block_layout(i, self.ffn_p, "i")
         if not self.tying:
             out.append(("head_w", (I, d), emb))
-        return out + [("head_b", (_ru(I, 128),), ("b", None))]  # padded: the kernels read the bias in 128-entry tiles
+        out.append(("head_b", (_ru(I, 128),), ("b", None)))  # padded: the kernels read the bias in 128-entry tiles
+        # after every item-only parameter: an item-only model keeps its layout and seeded init
+        return out + [(f"feat.{f.name}", (f.cardinality, d), emb) for f in self.features if f.kind == "cat"]
 
 
 class Bert4RecEngine(SasRecEngine):
@@ -121,9 +129,16 @@ class Bert4RecEngine(SasRecEngine):
         drop = cfg.dropout if training else 0.0
         rng = self.rng_counter.data_ptr()
         pos = prm["pos_emb"].data_ptr() if cfg.positional else None
-        check(self.lib.rp_bert_embed_fwd(p16["item_emb"].data_ptr(), p16["mask_emb"].data_ptr(), pos,
-                                         self.ids32.data_ptr(), self.in_tok.data_ptr(), T, L, d, drop, self.seed, 0, rng,
-                                         self.x[0].data_ptr(), self._stream()), "rp_bert_embed_fwd")
+        if self.features:
+            fa = self._feature_descs(False)
+            check(self.lib.rp_bert_feature_embed_fwd(p16["item_emb"].data_ptr(), p16["mask_emb"].data_ptr(), pos,
+                                                     self.ids32.data_ptr(), self.in_tok.data_ptr(), fa, len(fa), T, L, d,
+                                                     cfg.hd_valid, drop, self.seed, 0, rng, self.x[0].data_ptr(),
+                                                     self._stream()), "rp_bert_feature_embed_fwd")
+        else:
+            check(self.lib.rp_bert_embed_fwd(p16["item_emb"].data_ptr(), p16["mask_emb"].data_ptr(), pos,
+                                             self.ids32.data_ptr(), self.in_tok.data_ptr(), T, L, d, drop, self.seed, 0, rng,
+                                             self.x[0].data_ptr(), self._stream()), "rp_bert_embed_fwd")
         # application i runs block cfg.block_of(i): activations, saved statistics and dropout sites are per application,
         # weights per block
         for i in range(cfg.n_apps):
@@ -232,6 +247,11 @@ class Bert4RecEngine(SasRecEngine):
                                          self.B, L, d, drop, self.seed, 0, rng, G["item_emb"].data_ptr(),
                                          G["mask_emb"].data_ptr(), G["pos_emb"].data_ptr() if cfg.positional else None, st()),
               "rp_bert_embed_bwd")
+        if self.features:
+            fa = self._feature_descs(True)
+            check(self.lib.rp_bert_feature_embed_bwd(dx.data_ptr(), self.in_pad.data_ptr(), self.in_tok.data_ptr(), fa, len(fa),
+                                                     T, d, cfg.hd_valid, drop, self.seed, 0, rng, st()),
+                  "rp_bert_feature_embed_bwd")
 
     # ------------------------------------------------------------------------------------------------ inference
     def forward_last_hidden(self):

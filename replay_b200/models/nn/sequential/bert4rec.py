@@ -7,25 +7,31 @@ import torch
 
 from ....compat import LightningModuleBase
 from ....core import SasRecCore, _EngineLoss, dist_grad_all_reduce
-from ....engine import _BLOCK_PARAMS
 from ....engine_bert import Bert4RecEngine, BertConfig
-from ....schema import item_feature_of
+from ....schema import bert_side_features_of, item_feature_of
 
-_BLEAF = {"ln1_w": "attention_norm.weight", "ln1_b": "attention_norm.bias", "in_w": "attention.in_proj_weight",
-          "in_b": "attention.in_proj_bias", "out_w": "attention.out_proj.weight", "out_b": "attention.out_proj.bias",
-          "ln2_w": "pff_norm.weight", "ln2_b": "pff_norm.bias", "w1": "pff.w_1.weight", "b1": "pff.w_1.bias",
-          "w2": "pff.w_2.weight", "b2": "pff.w_2.bias"}
+# in the order TransformerBlock registers its parameters (bert4rec/model.py:481-500)
+_BLEAF = {"in_w": "attention.in_proj_weight", "in_b": "attention.in_proj_bias", "out_w": "attention.out_proj.weight",
+          "out_b": "attention.out_proj.bias", "ln1_w": "attention_norm.weight", "ln1_b": "attention_norm.bias",
+          "w1": "pff.w_1.weight", "b1": "pff.w_1.bias", "w2": "pff.w_2.weight", "b2": "pff.w_2.bias",
+          "ln2_w": "pff_norm.weight", "ln2_b": "pff_norm.bias"}
 
 
-def bert_key_map(n_blocks: int, tying: bool, item_feature: str = "item_id", positional: bool = True) -> dict:
-    """engine parameter name -> reference state_dict key (SURVEY.md Appendix B).  Without the positional embedding the
-    reference registers no ``item_embedder.position`` module (bert4rec/model.py:236-237), so there is no pos_emb key."""
-    m = {"item_emb": f"item_embedder.cat_embeddings.{item_feature}.weight", "mask_emb": "item_embedder.mask_embedding.weight"}
+def bert_key_map(n_blocks: int, tying: bool, item_feature: str = "item_id", positional: bool = True, features=()) -> dict:
+    """engine parameter name -> reference state_dict key (SURVEY.md Appendix B), in the reference's order.  Without the
+    positional embedding the reference registers no ``item_embedder.position`` module (bert4rec/model.py:236-237), so there
+    is no pos_emb key.  The categorical side ``features`` follow the item table (its ``cat_embeddings``, in schema order for
+    a schema that starts with the item id)."""
+    m = {"item_emb": f"item_embedder.cat_embeddings.{item_feature}.weight"}
+    for f in features:
+        if f.kind == "cat":
+            m[f"feat.{f.name}"] = f"item_embedder.cat_embeddings.{f.name}.weight"
+    m["mask_emb"] = "item_embedder.mask_embedding.weight"
     if positional:
         m["pos_emb"] = "item_embedder.position.pe.weight"
     for i in range(n_blocks):
-        for k in _BLOCK_PARAMS:
-            m[f"b{i}.{k}"] = f"transformer_blocks.{i}." + _BLEAF[k]
+        for k, leaf in _BLEAF.items():
+            m[f"b{i}.{k}"] = f"transformer_blocks.{i}." + leaf
     if tying:
         m["head_b"] = "_head.out_bias"
     else:
@@ -58,7 +64,7 @@ def shift_features(ids, pad_mask, token_mask, pad_value: int = 0):
 
 class _BertCore(SasRecCore):
     def _key_map(self):
-        return bert_key_map(self.cfg.n_blocks, self.cfg.tying, self.item_feature, self.cfg.positional)
+        return bert_key_map(self.cfg.n_blocks, self.cfg.tying, self.item_feature, self.cfg.positional, self.cfg.features)
 
     def _initial_seq_len(self):
         return self.cfg.max_len
@@ -75,8 +81,9 @@ class _BertCore(SasRecCore):
     def state_dict(self, *a, destination=None, prefix="", keep_vars=False):
         src = self._export() if self.engine is not None else (self._pending_state or {})
         out = destination if destination is not None else {}
-        for k, v in src.items():
-            out[prefix + k] = v
+        for k in self._keymap.values():   # the reference's order
+            if k in src:
+                out[prefix + k] = src[k]
         if self.cfg.tying:  # the tied head registers the embedder again (Appendix B)
             for k, v in list(src.items()):
                 if k.startswith("item_embedder."):
@@ -91,39 +98,45 @@ class _BertCore(SasRecCore):
             eng._loss_applied = self.loss_kind
             self._drop_graphs()   # captured graphs launch the other head's kernels
 
-    def loss(self, ids, pad_mask, token_mask, labels):
+    # ``feats``: the batch's feature tensors by name (its "inputs"); a model with side features stages them, an item-only
+    # model ignores them
+    def loss(self, ids, pad_mask, token_mask, labels, feats=None):
         eng = self.ensure_engine(*ids.shape, with_grad=True)
         self._apply_loss(eng)
+        self._stage_features(eng, feats)
         eng.set_batch(ids, pad_mask, token_mask, labels)
         return _EngineLoss.apply(self.flat, self)
 
-    def fused_step(self, ids, pad_mask, token_mask, labels, all_reduce="auto", lr=None):
+    def fused_step(self, ids, pad_mask, token_mask, labels, all_reduce="auto", lr=None, feats=None):
         eng = self.ensure_engine(*ids.shape, with_grad=True)
         if self._shadow_dirty:
             eng.refresh_shadow(); self._shadow_dirty = False
         self._set_lr(eng, lr)
         self._apply_loss(eng)
+        self._stage_features(eng, feats)
         eng.set_batch(ids, pad_mask, token_mask, labels)
         if isinstance(all_reduce, str):
             return self._graph_trainer(eng).run()[0]
         return eng.train_step(all_reduce, betas=self.adam_betas)[0]
 
     @torch.no_grad()
-    def _query_padded(self, ids, pad_mask, token_mask):
+    def _query_padded(self, ids, pad_mask, token_mask, feats=None):
         """last-position hidden states at the padded width bf16 [B, dp] (pairs with the padded head)"""
         eng = self.ensure_engine(*ids.shape, with_grad=self.engine.with_grad if self.engine is not None else False)
         if self._shadow_dirty:
             eng.refresh_shadow(); self._shadow_dirty = False
+        self._stage_features(eng, feats)
         eng.set_batch(ids, pad_mask, token_mask)
         return eng.forward_last_hidden()[: ids.shape[0]]
 
     @torch.no_grad()
-    def hidden_states(self, ids, pad_mask, token_mask):
+    def hidden_states(self, ids, pad_mask, token_mask, feats=None):
         """eval-mode hidden states of every position at the model's true hidden size, bf16 [B, L, d]"""
         B, L = ids.shape
         eng = self.ensure_engine(B, L, with_grad=self.engine.with_grad if self.engine is not None else False)
         if self._shadow_dirty:
             eng.refresh_shadow(); self._shadow_dirty = False
+        self._stage_features(eng, feats)
         eng.set_batch(ids, pad_mask, token_mask)
         return eng.unpad_features(eng.forward_hidden_all().view(eng.B, L, -1)[:B])
 
@@ -143,13 +156,13 @@ class _BertCore(SasRecCore):
         return out
 
     @torch.no_grad()
-    def query_embeddings(self, ids, pad_mask, token_mask):
+    def query_embeddings(self, ids, pad_mask, token_mask, feats=None):
         """bf16 [B, d] at the model's true hidden size"""
-        return self.engine.unpad_features(self._query_padded(ids, pad_mask, token_mask))
+        return self.engine.unpad_features(self._query_padded(ids, pad_mask, token_mask, feats))
 
     @torch.no_grad()
-    def logits(self, ids, pad_mask, token_mask, candidates=None):
-        hq = self._query_padded(ids, pad_mask, token_mask)
+    def logits(self, ids, pad_mask, token_mask, candidates=None, feats=None):
+        hq = self._query_padded(ids, pad_mask, token_mask, feats)
         W, b = self.engine.head_for_scoring()
         b = b[: self.cfg.n_items]
         if candidates is not None:
@@ -159,10 +172,10 @@ class _BertCore(SasRecCore):
         return out
 
     @torch.no_grad()
-    def predict_topk(self, ids, pad_mask, token_mask, k, seen_ids=None, candidates=None):
+    def predict_topk(self, ids, pad_mask, token_mask, k, seen_ids=None, candidates=None, feats=None):
         from .... import ops
 
-        hq = self._query_padded(ids, pad_mask, token_mask).contiguous()
+        hq = self._query_padded(ids, pad_mask, token_mask, feats).contiguous()
         W, b = self.engine.head_for_scoring()
         n_items, inv = self.cfg.n_items, None
         if candidates is not None:
@@ -186,9 +199,10 @@ class Bert4RecModel(torch.nn.Module):
         self.hidden_size, self.num_blocks, self.num_heads, self.dropout = hidden_size, num_blocks, num_heads, dropout
         self.num_passes_over_block = num_passes_over_block
         self.enable_positional_embedding, self.enable_embedding_tying = enable_positional_embedding, enable_embedding_tying
+        # every other categorical and numerical feature of the schema is summed into the item embedding (BertEmbedding)
         cfg = BertConfig(n_items=card, d=hidden_size, n_heads=num_heads, n_blocks=num_blocks, max_len=max_len, dropout=dropout,
                          tying=enable_embedding_tying, pad_id=pad if 0 <= pad < card else 0, passes=num_passes_over_block,
-                         positional=bool(enable_positional_embedding))
+                         positional=bool(enable_positional_embedding), features=tuple(bert_side_features_of(schema)))
         self.core = _BertCore(cfg, item_feature=name, device=device, seed=seed)
 
     def state_dict(self, *a, **k):
@@ -198,12 +212,12 @@ class Bert4RecModel(torch.nn.Module):
         return self.core.load_state_dict(sd, strict=strict)
 
     def get_query_embeddings(self, inputs, pad_mask, token_mask):
-        return self.core.query_embeddings(inputs[self.item_feature_name], pad_mask, token_mask).float()
+        return self.core.query_embeddings(inputs[self.item_feature_name], pad_mask, token_mask, inputs).float()
 
     # ---- inference-only restatements of the reference's forward / forward_step / get_logits (bert4rec/model.py:86-157)
     def forward_step(self, inputs, pad_mask, token_mask):
         """Hidden states of every position, fp32 [B, L, d] (eval mode: no dropout)."""
-        return self.core.hidden_states(inputs[self.item_feature_name], pad_mask, token_mask).float()
+        return self.core.hidden_states(inputs[self.item_feature_name], pad_mask, token_mask, inputs).float()
 
     def get_logits(self, out_embeddings, item_ids=None):
         """Biased head scores of hidden states [..., d]: [..., |I|], or [..., |item_ids|]."""
@@ -222,16 +236,28 @@ class Bert4RecModel(torch.nn.Module):
             self.core.ensure_engine(1, self.max_len, with_grad=False)
         return {k: v.detach().clone() for k, v in self.core.state_dict().items()}
 
+    def item_embeddings(self) -> torch.Tensor:
+        """A copy of the item table [I, d] (BertEmbedding.item_embeddings, model.py:298-303)."""
+        return self._weights()[f"item_embedder.cat_embeddings.{self.item_feature_name}.weight"]
+
     def get_all_embeddings(self) -> dict:
-        """Copies of the item table [I, d] and, when it is on, the position table [max_len, d] (model.py:298-312)."""
+        """Copies of the item table [I, d], every categorical side table under its feature's name and, when it is on, the
+        position table [max_len, d] (model.py:298-312).  A numerical feature has no table: KeyError, as in the reference."""
         sd = self._weights()
         out = {"item_embedding": sd[f"item_embedder.cat_embeddings.{self.item_feature_name}.weight"]}
+        for name, _ in self.schema.items():
+            if name != self.item_feature_name:
+                key = f"item_embedder.cat_embeddings.{name}.weight"
+                if key not in sd:
+                    raise KeyError(name)
+                out[name] = sd[key]
         if self.enable_positional_embedding:
             out["positional_embedding"] = sd["item_embedder.position.pe.weight"]
         return out
 
     def resize_items(self, table: torch.Tensor):
-        """Rebuild for the catalog of ``table`` [I', d] (I' >= I), keeping every other weight (lightning.py:612-627): the
+        """Rebuild for the catalog of ``table`` [I', d] (I' >= I), keeping every other weight, side tables included
+        (lightning.py:612-627): the
         head keeps its first I rows and bias entries and takes fresh ones for the new items - ``Linear(hidden, I')``'s
         default initialisation untied, N(0, 0.01) bias entries tied.  The new core starts with fresh Adam moments, as the
         reference's newly created parameters do, and without captured graphs; the loss, the Adam betas, the passes and the
@@ -260,7 +286,7 @@ class Bert4RecModel(torch.nn.Module):
         self.item_count = n_new
 
     def predict(self, inputs, pad_mask, token_mask, candidates_to_score=None):
-        return self.core.logits(inputs[self.item_feature_name], pad_mask, token_mask, candidates_to_score)
+        return self.core.logits(inputs[self.item_feature_name], pad_mask, token_mask, candidates_to_score, inputs)
 
 
 class Bert4Rec(LightningModuleBase):
@@ -300,48 +326,64 @@ class Bert4Rec(LightningModuleBase):
         """batch keys (bert4rec/dataset.py:167-173): query_id, pad_mask, inputs, token_mask, positive_labels."""
         ids = batch["inputs"][self._model.item_feature_name]
         args = (ids, batch["pad_mask"], batch["token_mask"], batch["positive_labels"])
-        core = self._model.core
-        loss = core.fused_step(*args, lr=self._fused_lr()) if self.fused_optimizer else core.loss(*args)
+        core, feats = self._model.core, batch["inputs"]
+        loss = core.fused_step(*args, lr=self._fused_lr(), feats=feats) if self.fused_optimizer else core.loss(*args, feats)
         self.log("train_loss", loss, on_step=True, on_epoch=True, prog_bar=True, sync_dist=True)
         return loss
 
     def _prepared(self, batch):
         """_prepare_prediction_batch (bert4rec/lightning.py:649-683): a batch of full length is taken AS IS (the prediction
         dataset already shifted it, bert4rec/dataset.py:322-345); a shorter one is left-padded with the padding value and
-        then shifted; a longer one is an error."""
+        then shifted; a longer one is an error.  Every categorical side feature is padded and shifted the same way with its
+        own padding value.  A short batch with a numerical side feature raises: the reference's ``view(B, L)`` of its
+        [B, L, tensor_dim] values fails there.  Returns (ids, pad_mask, token_mask, feature tensors)."""
         ids, pm, tm = batch["inputs"][self._model.item_feature_name], batch["pad_mask"], batch["token_mask"]
         seq_len, max_len = pm.shape[1], self._model.max_len
+        feats = batch["inputs"]
         if seq_len > max_len:
             raise ValueError("The length of the submitted sequence must not exceed the maximum length of the sequence. "
                              f"The length of the sequence is given {seq_len}, while the maximum length is {max_len}")
         if seq_len < max_len:
-            feats = self._schema.item_id_features
-            feat = feats.item() if hasattr(feats, "item") else feats[self._schema.item_id_feature_name]
-            ids = torch.nn.functional.pad(ids, (max_len - seq_len, 0), value=int(feat.padding_value))
-            pm = torch.nn.functional.pad(pm, (max_len - seq_len, 0), value=0)
-            ids, pm, tm = shift_features(ids, pm, pm, int(feat.padding_value))
-        return ids, pm, tm
+            side = self._model.core.cfg.features
+            num = [f.name for f in side if f.kind != "cat"]
+            if num:
+                raise ValueError(f"a batch shorter than max_seq_len cannot carry the numerical features {num}: the reference "
+                                 "cannot left-pad their [B, L, tensor_dim] values")
+            item = self._schema.item_id_features
+            item = item.item() if hasattr(item, "item") else item[self._schema.item_id_feature_name]
+            padded = torch.nn.functional.pad(pm, (max_len - seq_len, 0), value=0)
+            pads = [(self._model.item_feature_name, int(item.padding_value))] + [(f.name, f.padding_value) for f in side]
+            feats = {}
+            for name, pad in pads:
+                v = torch.nn.functional.pad(batch["inputs"][name], (max_len - seq_len, 0), value=pad)
+                feats[name], pm, tm = shift_features(v, padded, padded, pad)
+            ids = feats[self._model.item_feature_name]
+        return ids, pm, tm, feats
 
-    def _model_predict(self, ids, pm, tm, candidates_to_score=None):
+    def _model_predict(self, ids, pm, tm, candidates_to_score=None, feats=None):
         cands = self._candidates_to_score if candidates_to_score is None else candidates_to_score
-        return self._model.core.logits(ids, pm, tm, cands)
+        return self._model.core.logits(ids, pm, tm, cands, feats)
 
     def forward(self, feature_tensors, padding_mask, tokens_mask, candidates_to_score=None):
-        return self._model_predict(feature_tensors[self._model.item_feature_name], padding_mask, tokens_mask, candidates_to_score)
+        return self._model_predict(feature_tensors[self._model.item_feature_name], padding_mask, tokens_mask, candidates_to_score,
+                                   feature_tensors)
 
     def validation_step(self, batch: dict, batch_idx: int = 0, dataloader_idx: int = 0):
-        return self._model_predict(batch["inputs"][self._model.item_feature_name], batch["pad_mask"], batch["token_mask"])
+        return self._model_predict(batch["inputs"][self._model.item_feature_name], batch["pad_mask"], batch["token_mask"],
+                                   feats=batch["inputs"])
 
     def predict_step(self, batch: dict, batch_idx: int = 0, dataloader_idx: int = 0):
-        return self._model_predict(*self._prepared(batch))
+        ids, pm, tm, feats = self._prepared(batch)
+        return self._model_predict(ids, pm, tm, feats=feats)
 
     def predict(self, batch: dict, candidates_to_score=None):
-        return self._model_predict(*self._prepared(batch), candidates_to_score)
+        ids, pm, tm, feats = self._prepared(batch)
+        return self._model_predict(ids, pm, tm, candidates_to_score, feats)
 
     def predict_topk(self, batch: dict, k: int, seen_ids=None, candidates_to_score=None):
-        ids, pm, tm = self._prepared(batch)
+        ids, pm, tm, feats = self._prepared(batch)
         cands = self._candidates_to_score if candidates_to_score is None else candidates_to_score
-        return self._model.core.predict_topk(ids, pm, tm, k, seen_ids, cands)
+        return self._model.core.predict_topk(ids, pm, tm, k, seen_ids, cands, feats)
 
     def _fused_lr(self) -> float:
         try:
@@ -391,7 +433,7 @@ class Bert4Rec(LightningModuleBase):
             raise ValueError("New vocabulary size must be greater then already fitted")
         new = torch.empty(new_vocab_size, self._embedding_dim())
         torch.nn.init.xavier_normal_(new)
-        new[: self._vocab_size] = self.get_all_embeddings()["item_embedding"]
+        new[: self._vocab_size] = self._model.item_embeddings()
         self._set_new_item_table(new)
 
     def set_item_embeddings_by_tensor(self, all_item_embeddings: torch.Tensor):
@@ -410,7 +452,7 @@ class Bert4Rec(LightningModuleBase):
             raise ValueError("Input tensor must have (number of all items, model hidden size) shape")
         if item_embeddings.shape[1] != self._embedding_dim():
             raise ValueError("Input tensor second dimension doesn't match embedding dim")
-        new = torch.cat([self.get_all_embeddings()["item_embedding"].cpu(), item_embeddings.detach().float().cpu()])
+        new = torch.cat([self._model.item_embeddings().cpu(), item_embeddings.detach().float().cpu()])
         self._set_new_item_table(new)
 
     @property

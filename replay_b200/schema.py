@@ -100,3 +100,35 @@ def side_features_of(schema, excluded=(), list_aggregation: str = "sum") -> list
             td = int(f.tensor_dim)
             out.append(SideFeature(name, "ident" if td == f.embedding_dim else "num", 0, 0, td))
     return out
+
+
+def bert_side_features_of(schema) -> list:
+    """The side features the legacy BERT4Rec sums into its item embedding (BertEmbedding, bert4rec/model.py:173-296), as
+    ``engine.SideFeature``s: every categorical feature but the item id (kind "cat", an Embedding of ``cardinality`` rows
+    without a padding row), then every numerical one (kind "ident": its values are added as they are), each in schema order,
+    the order of the reference's sum.  Raises as the reference's constructor does: NotImplementedError for a non-sequential
+    feature, ValueError when a feature's dim (``embedding_dim`` of a categorical, ``tensor_dim`` of a numerical) differs from
+    the first feature's.  A categorical list raises NotImplementedError here; the reference fails later, at forward."""
+    from .engine import SideFeature
+
+    item = schema.item_id_feature_name
+    common, cats, nums = None, [], []
+    for name, f in schema.items():
+        if not f.is_seq:
+            raise NotImplementedError("Non-sequential features is not yet supported")
+        dim = f.embedding_dim if f.is_cat else f.tensor_dim
+        if common is None:
+            common = dim
+        if dim != common:
+            raise ValueError("Dimension of all features must be the same for sum aggregation")
+        if name == item:
+            continue
+        if f.is_cat:
+            cats.append(SideFeature(name, "bag_sum" if getattr(f, "is_list", False) else "cat", int(f.cardinality),
+                                    int(f.padding_value), 1))
+        else:
+            nums.append(SideFeature(name, "ident", 0, 0, int(f.tensor_dim)))
+    for f in cats:   # after the loop: the reference's own construction errors come first
+        if f.kind != "cat":
+            raise NotImplementedError(f"BERT4Rec cannot sum the categorical list feature {f.name!r} into its input")
+    return cats + nums
