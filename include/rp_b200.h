@@ -83,7 +83,8 @@ int rp_score_topk(const void* hq, const void* table, const float* bias, const in
 size_t rp_ce_head_workspace(int capacity_tokens, int n_items, int d);
 
 /* loss_out fp32 [2] = { mean CE over the valid targets, 1 / n_valid }; lse fp32 [capacity];
- * cvec fp32 [round_up(capacity,128)] (per-token exponent offsets for the backward; entries >= capacity must be -inf).
+ * cvec fp32 [round_up(capacity,128)], 16-byte aligned (per-token exponent offsets for the backward; entries >= capacity
+ * must be -inf).
  * d_hc (optional, bf16 [capacity, d], d <= 256): enables the FUSED training path - a single pass accumulates the row sums of
  * exp(s) against a fixed reference maximum together with the un-normalised gradient sum_i exp(s_i) E_i, so the separate
  * log-sum-exp pass disappears and d_hc is final after this call.  A device-side Cauchy-Schwarz bound on |s| guards the

@@ -376,11 +376,16 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   constexpr int kStage = KCH * kChunkB;   // one column tile in shared memory
   constexpr int PITCH = D + 4;            // fp32 accumulator stage (over the ring once the column tiles are done)
   constexpr int kSlots = 2, DW = D / kSlots;
+  // MODE 1: the column tile's TN exponent offsets ride the ring in a slot of their own (launch_ce_bwd sizes them), behind the ring and the
+  // accumulator stage that reuses it; they are in shared memory once the tile is, so the exponentials never wait on a load
+  constexpr bool OFF_RING = COLCONST && !BCE;
+  constexpr int kOffBytes = TN * 4;
   if (safe_flag && (*safe_flag != 0) != (run_if_safe != 0)) return;  // fused path vs two-pass fallback (uniform)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + KCH * kChunk;
+  float* sOff = reinterpret_cast<float*>(sB + (NSTAGE * kStage > kT * PITCH * 4 ? NSTAGE * kStage : kT * PITCH * 4));
   __shared__ float s_row[kT];             // per-row sum of G (FUSED) / of G before the item factor (COLCONST with bias)
   __shared__ float s_dot[kSlots][kT];
   __shared__ uint64_t bar_a, bar_full[NSTAGE];
@@ -416,8 +421,10 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   // refills it, so no warp ever waits for the other warpgroup and the two can run out of phase.
   auto issue = [&](int jl) {
     const uint32_t s = jl % NSTAGE;
-    mbar_arrive_expect_tx(&bar_full[s], kStage);
+    mbar_arrive_expect_tx(&bar_full[s], kStage + (OFF_RING ? kOffBytes : 0));
     for (int kc = 0; kc < KCH; ++kc) tma_load_2d(sB + s * kStage + kc * kChunkB, &tmB, &bar_full[s], kc * 64, c_begin + jl * TN);
+    // cvec holds round_up(capacity, 128) entries, -inf past the valid tokens: the last tile's slot is read in full
+    if (OFF_RING) bulk_load_1d(sOff + s * TN, cvec + c_begin + jl * TN, kOffBytes, &bar_full[s]);
   };
   if (threadIdx.x == 0) {
     mbar_arrive_expect_tx(&bar_a, KCH * kChunk);
@@ -517,15 +524,18 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         zb += __log2f(pb) * kLn2;
       }
     } else {
+      const float* off = sOff + s * TN + fc;   // COLCONST: offsets of this thread's columns, -inf beyond the valid tokens
 #pragma unroll
       for (int q = 0; q < TN / 8; ++q) {
         float g[4];
+        float2 cq;
+        if (COLCONST) cq = *reinterpret_cast<const float2*>(off + 8 * q);
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int col = col0 + 8 * q + e;
           float va = sacc[4 * q + e], vb = sacc[4 * q + 2 + e];
           if (COLCONST) {
-            const float cc = __ldg(cvec + col);   // -inf beyond the valid tokens (the buffer is padded to 128 rows)
+            const float cc = e ? cq.y : cq.x;
             g[e] = ex2f(fmaf(va, kLog2e, cc));
             g[2 + e] = ex2f(fmaf(vb, kLog2e, cc));
           } else {
@@ -1251,9 +1261,12 @@ static int launch_ce_bwd(const CUtensorMap& tmA, const void* b_mat, int b_rows, 
                          const void* table, const float* loss_inv, const int32_t* n_valid, int n_items, const float* bias,
                          float* d_bias, void* out, int grid, const int32_t* safe_flag, int run_if_safe, int n_splits,
                          int capacity, float* zpart, cudaStream_t stream, const CeDirect& direct) {
-  // row tile + a ring of NSTAGE column tiles; the fp32 accumulator stage reuses the ring at the end
+  // row tile + a ring of NSTAGE column tiles; the fp32 accumulator stage reuses the ring at the end.  MODE 1 adds the ring's
+  // slots of exponent offsets, which the bulk copy fills from a 16-byte aligned cvec
   const int ring = NSTAGE * KCH * TN * 128, stage = 128 * (KCH * 64 + 4) * 4;
-  const int smem = KCH * kChunk + (ring > stage ? ring : stage) + 1024;
+  const int offsets = MODE == 1 ? NSTAGE * TN * 4 : 0;
+  if (MODE == 1 && (reinterpret_cast<uintptr_t>(cvec) & 15) != 0) return RP_EALIGN;
+  const int smem = KCH * kChunk + (ring > stage ? ring : stage) + offsets + 1024;
   CUtensorMap tmB;   // column-side matrix, one [TN rows x 64 columns] box per chunk
   {
     const int rc = make_tmap_bf16(&tmB, b_mat, b_rows, KCH * 64, KCH * 64, TN);
