@@ -335,6 +335,43 @@ int rp_bert_feature_embed_fwd(const void* item_table, const void* mask_emb, cons
 int rp_bert_feature_embed_bwd(const void* dx, const uint8_t* pad_mask, const uint8_t* tok_mask, const rp_feature* feats,
                               int n_feats, int T, int d, int hd_valid, float drop_p, unsigned long long seed,
                               unsigned long long drop_off, const unsigned long long* seed_ptr, void* stream);
+/* SASRec input through ConcatAggregator (nn/agg.py:56-109 ; nn/sequential/sasrec/agg.py:37-53), every feature at its own
+ * width w_f:
+ *   X[r] = [segments | 0],  Y = X . W^T + b (rp_gemm, fp32 [rows, d], W bf16 [d, kp]),  x[r] = dropout(Y[r] * scale + pos[pos0 + t % L])
+ * rp_concat_gather(_rows) writes X bf16 [rows, kp]: the item's true hidden features (padded columns skipped by hd_valid) at
+ * columns item_col.., feature k's w_f = seg_dim[k] values at seg_col[k]..; columns past the segments are zero.  Segment
+ * terms, each summed in fp32 and rounded to bf16 once:
+ *   RP_FEAT_CAT / _BAG_SUM / _BAG_MEAN   as in rp_feature_embed_fwd, over table bf16 [n_rows, w_f]
+ *   RP_FEAT_NUM                          v . W_f^T + b_f, table = W_f fp32 [w_f, K], bias fp32 [w_f] (val_col consecutive)
+ *   RP_FEAT_IDENT                        v itself, K == w_f
+ * The segments must tile [0, width) exactly and kp be a multiple of 64 with width <= kp <= RP_CONCAT_MAX_COLS.
+ * rp_concat_embed_fwd is the elementwise pass after the projection; its dropout is rp_embed_fwd's stream (row key = token t),
+ * so a concat model drops the elements its item-only model drops.  rp_gemm's epilogue cannot take it: its bias comes after
+ * alpha, it has no per-position row and its dropout is keyed by the output row, which is not the token on packed rows.
+ * Backward: dY = scale * dropout'(dx) (rp_feature_embed_bwd with no features writes it as d_s), dX = dY . W (rp_gemm),
+ * rp_concat_scatter adds dX's item segment into d_item fp32 [., d] (pad_id frozen) and each categorical segment into its
+ * d_table fp32 [n_rows, w_f] (fp32 atomics, padding rows frozen, mean bags by 1 / count) and stages the numerical values
+ * in v_rows as rp_feature_embed_bwd does; rp_wgrad_group gives dW / db of the projection (dY^T . X) and of the numerical
+ * features (dX^T . v_rows, their block at (seg_col, val_col)); rp_embed_pos_bwd gives the positions.
+ * row_tok / n_rows_dev: both (packed rows, *n_rows_dev of the T rows) or neither.  RP_EINVAL: null pointer, unknown kind,
+ * drop_p outside [0, 1); RP_ESHAPE: d, hd_valid, n_feats, segments, kp, widths, val_col, v_ld. */
+#define RP_CONCAT_MAX_COLS 1024
+int rp_concat_gather(const void* item_table, const int32_t* ids, const rp_feature* feats, const int* seg_col, const int* seg_dim,
+                     int n_feats, int item_col, int T, int d, int hd_valid, int kp, void* x, void* stream);
+int rp_concat_gather_rows(const void* item_table, const int32_t* ids, const rp_feature* feats, const int* seg_col,
+                          const int* seg_dim, int n_feats, int item_col, const int32_t* row_tok, const int32_t* n_rows_dev, int T,
+                          int d, int hd_valid, int kp, void* x, void* stream);
+int rp_concat_embed_fwd(const float* y, const float* pos, const int32_t* row_tok, const int32_t* n_rows_dev, int T, int L, int d,
+                        int pos0, float scale, float drop_p, unsigned long long seed, unsigned long long drop_off,
+                        const unsigned long long* seed_ptr, void* out, void* stream);
+int rp_concat_scatter(const void* dx, const int32_t* ids, float* d_item, int pad_id, const rp_feature* feats, const int* seg_col,
+                      const int* seg_dim, int n_feats, int item_col, const int32_t* row_tok, const int32_t* n_rows_dev, int T,
+                      int d, int hd_valid, int kp, void* v_rows, int v_ld, void* stream);
+/* The positional half of rp_embed_bwd(_rows) alone: d_pos[pos0 + l] += sum over the sequences of dropout'(dx) at position l
+ * (new path: no pad-row mask).  seq_first / seq_off (rp_row_plan): both for packed rows, or neither. */
+int rp_embed_pos_bwd(const void* dx, const int32_t* seq_first, const int32_t* seq_off, int B, int L, int d, int pos0,
+                     float drop_p, unsigned long long seed, unsigned long long drop_off, const unsigned long long* seed_ptr,
+                     float* d_pos, void* stream);
 
 /* torch.nn.LayerNorm forward / backward (transformer.py:47-49,60-62 eps 1e-8; model.py:248 eps 1e-5).  With `gather`
  * output row r reads input row gather[r] and only *n_rows_dev rows exist (valid-target compaction); the backward then

@@ -247,6 +247,7 @@ class RpFeature(ctypes.Structure):
 
 FEAT_CAT, FEAT_BAG_SUM, FEAT_BAG_MEAN, FEAT_NUM, FEAT_IDENT = range(5)   # rp_feature.kind
 FEAT_MAX, FEAT_MAX_NUM_COLS = 16, 64
+CONCAT_MAX_COLS = 1024   # RP_CONCAT_MAX_COLS: widest concatenated input of ConcatAggregator (padded to 64 columns)
 
 
 _P, _LL, _U64 = c_void_p, ctypes.c_longlong, ctypes.c_ulonglong
@@ -288,6 +289,13 @@ _EXTRA_SIGS: list = [
                                           c_float, _U64, _U64, _P, _P, _P]),
     ("rp_bert_feature_embed_bwd", c_int, [_P, _P, _P, ctypes.POINTER(RpFeature), c_int, c_int, c_int, c_int, c_float, _U64,
                                           _U64, _P, _P]),
+    ("rp_concat_gather", c_int, [_P, _P, ctypes.POINTER(RpFeature), _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P]),
+    ("rp_concat_gather_rows", c_int, [_P, _P, ctypes.POINTER(RpFeature), _P, _P, c_int, c_int, _P, _P, c_int, c_int, c_int, c_int,
+                                      _P, _P]),
+    ("rp_concat_embed_fwd", c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, c_float, c_float, _U64, _U64, _P, _P, _P]),
+    ("rp_concat_scatter", c_int, [_P, _P, _P, c_int, ctypes.POINTER(RpFeature), _P, _P, c_int, c_int, _P, _P, c_int, c_int, c_int,
+                                  c_int, _P, c_int, _P]),
+    ("rp_embed_pos_bwd", c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_float, _U64, _U64, _P, _P, _P]),
 ]
 
 __all__ = ["GemmDesc", "DiffAttnDesc", "DiffLambda", "SceDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "RpFeature", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]

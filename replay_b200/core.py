@@ -101,6 +101,9 @@ class SasRecCore(torch.nn.Module):
                 m[f"feat.{f.name}"] = pre + "emb.weight"
             elif f.kind == "num":
                 m.update({f"feat.{f.name}.w": pre + "linear.weight", f"feat.{f.name}.b": pre + "linear.bias"})
+        if getattr(self.cfg, "concat", False):   # nn/agg.py ConcatAggregator.feat_projection inside PositionAwareAggregator
+            pre = "body.embedding_aggregator.embedding_aggregator.feat_projection."
+            m.update({"feat_proj.w": pre + "weight", "feat_proj.b": pre + "bias"})
         return m
 
     def _stage_features(self, eng, feats):
@@ -189,7 +192,7 @@ class SasRecCore(torch.nn.Module):
             out[prefix + k] = v
         for f in getattr(self.cfg, "features", ()):   # IdentityEmbedding's buffer (nn/embedding.py): eye(d), no parameter
             if f.kind == "ident":
-                out[prefix + f"body.embedder.feature_embedders.{f.name}._weight"] = torch.eye(self.cfg.d)
+                out[prefix + f"body.embedder.feature_embedders.{f.name}._weight"] = torch.eye(f.dim or self.cfg.d)
         if self.cfg.variant == "legacy":  # the reference's head registers the embedder again (Appendix B aliases)
             for a, b in (("_head._item_embedder.item_emb.weight", "item_embedder.item_emb.weight"),
                          ("_head._item_embedder.pos_emb.pe.weight", "item_embedder.pos_emb.pe.weight")):

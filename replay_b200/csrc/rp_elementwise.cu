@@ -866,6 +866,22 @@ RP_API int rp_embed_bwd(const void* dx, const int32_t* ids, const uint8_t* pad_m
   return RP_OK;
 }
 
+RP_API int rp_embed_pos_bwd(const void* dx, const int32_t* seq_first, const int32_t* seq_off, int B, int L, int d, int pos0,
+                            float drop_p, unsigned long long seed, unsigned long long drop_off,
+                            const unsigned long long* seed_ptr, float* d_pos, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!dx || !d_pos || B <= 0 || L <= 0 || pos0 < 0 || (!seq_first != !seq_off)) return RP_EINVAL;
+  if (d != 64 && d != 128 && d != 256 && d != 512) return RP_ESHAPE;
+  const int rlanes = 256 / (d / 4);
+  int G = (B + 31) / 32;
+  if (G > 16) G = 16;
+  embed_bwd_pos_kernel<<<dim3(L, G), 256, (size_t)rlanes * d * sizeof(float), stream>>>(
+      reinterpret_cast<const __nv_bfloat16*>(dx), nullptr, B, L, d, pos0, 0, drop_p, seed, drop_off, seed_ptr, d_pos, seq_first,
+      seq_off);
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
 RP_API int rp_row_plan(const uint8_t* pad_mask, const int64_t* labels, const uint8_t* target_mask, int B, int L, int n_items,
                        const int32_t* valid_idx, const int32_t* n_valid, int32_t* seq_first, int32_t* seq_off,
                        int32_t* n_rows, int32_t* row_tok, int32_t* valid_rows, void* stream_) {

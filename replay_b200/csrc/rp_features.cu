@@ -209,6 +209,146 @@ __global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) feature_embed_bwd_kern
   }
 }
 
+// ---- ConcatAggregator (replay/nn/agg.py:56-109): every feature at its own width, concatenated in the order the host gives
+// (the reference sorts by feature name), then Linear(sum of widths, d) on the tensor cores (rp_gemm).  One warp per row and
+// one column per lane and step: segment widths are arbitrary (11, 13, ...), so nothing is vector-loaded and neither the side
+// tables nor the segment offsets need padding.  Each segment value is summed in fp32 and rounded to bf16 once.
+struct ConcatArgs {
+  rp_feature f[RP_FEAT_MAX];
+  int col[RP_FEAT_MAX], dim[RP_FEAT_MAX];   // first column and width of feature k's segment
+  int n, item_col;
+};
+
+// padded column of true feature j (the inverse of feat_true_col)
+__device__ __forceinline__ int feat_pad_col(int j, int hd_valid) {
+  if (hd_valid == 0) return j;
+  return (j / hd_valid) * (hd_valid <= 64 ? 64 : 128) + j % hd_valid;
+}
+
+// x[r, :] = [segments | zeros up to kp] for row r (token row_tok[r] on packed rows, *n_rows_dev of them)
+__global__ void __launch_bounds__(256) concat_gather_kernel(
+    const __nv_bfloat16* __restrict__ item, const int32_t* __restrict__ ids, const __grid_constant__ ConcatArgs ca, int n_tok,
+    int D, int d_true, int hd_valid, int width, int kp, const int32_t* __restrict__ row_tok,
+    const int32_t* __restrict__ n_rows_dev, __nv_bfloat16* __restrict__ x) {
+  const int n = n_rows_dev ? *n_rows_dev : n_tok;
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  for (int r = blockIdx.x * wpb + (threadIdx.x >> 5); r < n; r += gridDim.x * wpb) {
+    const int t = row_tok ? row_tok[r] : r;
+    __nv_bfloat16* o = x + (size_t)r * kp;
+    for (int c = width + lane; c < kp; c += 32) o[c] = __float2bfloat16(0.f);
+    const __nv_bfloat16* it = item + (size_t)ids[t] * D;
+    for (int j = lane; j < d_true; j += 32) o[ca.item_col + j] = it[feat_pad_col(j, hd_valid)];
+    for (int k = 0; k < ca.n; ++k) {
+      const rp_feature& f = ca.f[k];
+      const int w = ca.dim[k];
+      __nv_bfloat16* seg = o + ca.col[k];
+      if (f.kind == RP_FEAT_CAT || f.kind == RP_FEAT_BAG_SUM || f.kind == RP_FEAT_BAG_MEAN) {
+        const int32_t* v = reinterpret_cast<const int32_t*>(f.values) + (size_t)t * f.width;
+        const __nv_bfloat16* tab = reinterpret_cast<const __nv_bfloat16*>(f.table);
+        int cnt = 0;
+        for (int i = 0; i < f.width; ++i) cnt += feat_live(v[i], f);
+        const float s = (f.kind == RP_FEAT_BAG_MEAN && cnt > 0) ? 1.f / (float)cnt : 1.f;
+        for (int j = lane; j < w; j += 32) {
+          float acc = 0.f;
+          for (int i = 0; i < f.width; ++i) {
+            const int id = v[i];
+            if (feat_live(id, f)) acc += __bfloat162float(tab[(size_t)id * w + j]);
+          }
+          seg[j] = __float2bfloat16(acc * s);
+        }
+      } else if (f.kind == RP_FEAT_NUM) {   // v . W^T + b at the feature's own width, W fp32 [w, tensor_dim]
+        const float* v = reinterpret_cast<const float*>(f.values) + (size_t)t * f.width;
+        const float* W = reinterpret_cast<const float*>(f.table);
+        for (int j = lane; j < w; j += 32) {
+          float acc = f.bias[j];
+          for (int i = 0; i < f.width; ++i) acc += v[i] * W[(size_t)j * f.width + i];
+          seg[j] = __float2bfloat16(acc);
+        }
+      } else {   // RP_FEAT_IDENT: the values themselves (width == w)
+        const float* v = reinterpret_cast<const float*>(f.values) + (size_t)t * f.width;
+        for (int j = lane; j < w; j += 32) seg[j] = __float2bfloat16(v[j]);
+      }
+    }
+  }
+}
+
+// out[r] = dropout(y[r] * scale + pos[pos0 + t % L]), y fp32 [rows, D] = the projection (bias included); the dropout stream of
+// rp_embed_fwd (row key = token t, embedding site drop_off), so a concat model drops what the item-only model drops
+template <int VEC>
+__global__ void __launch_bounds__(256) concat_embed_fwd_kernel(
+    const float* __restrict__ y, const float* __restrict__ pos, int n_tok, int L, int pos0, float scale, float drop_p,
+    unsigned long long seed, unsigned long long drop_off, const unsigned long long* __restrict__ seed_ptr,
+    const int32_t* __restrict__ row_tok, const int32_t* __restrict__ n_rows_dev, __nv_bfloat16* __restrict__ out) {
+  if (drop_p > 0.f && seed_ptr) seed += *seed_ptr;
+  constexpr int D = VEC * 32;
+  const int n = n_rows_dev ? *n_rows_dev : n_tok;
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  const int c0 = lane * VEC;
+  const uint32_t thr = drop_p > 0.f ? (uint32_t)(drop_p * 4294967296.0) : 0u;
+  const float ks = drop_p > 0.f ? 1.f / (1.f - drop_p) : 1.f;
+  for (int r = blockIdx.x * wpb + (threadIdx.x >> 5); r < n; r += gridDim.x * wpb) {
+    const int t = row_tok ? row_tok[r] : r;
+    const float* yr = y + (size_t)r * D + c0;
+    const float* p = pos + (size_t)(pos0 + t % L) * D + c0;
+    float acc[VEC];
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) acc[i] = yr[i] * scale + p[i];
+    if (drop_p > 0.f) {
+      const uint32_t rk = drop_row_key(seed, drop_off, (unsigned long long)t);
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) acc[i] = drop_mix(rk, drop_col_key((uint32_t)(c0 + i))) >= thr ? acc[i] * ks : 0.f;
+    }
+    __nv_bfloat16* o = out + (size_t)r * D + c0;
+#pragma unroll
+    for (int i = 0; i < VEC; i += 2) *reinterpret_cast<uint32_t*>(o + i) = pack_bf16(acc[i], acc[i + 1]);
+  }
+}
+
+// dX = dY . W (bf16 [rows, kp]) into the tables: the item segment into d_item (pad_id frozen), categorical segments into their
+// d_table (padding rows frozen, mean bags by 1 / count); numerical values staged into v_rows for their dW / db
+__global__ void __launch_bounds__(256) concat_scatter_kernel(
+    const __nv_bfloat16* __restrict__ dx, const int32_t* __restrict__ ids, float* __restrict__ d_item, int pad_id,
+    const __grid_constant__ ConcatArgs ca, int n_tok, int D, int d_true, int hd_valid, int kp, const int32_t* __restrict__ row_tok,
+    const int32_t* __restrict__ n_rows_dev, __nv_bfloat16* __restrict__ v_rows, int v_ld) {
+  const int n = n_rows_dev ? *n_rows_dev : n_tok;
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  for (int r = blockIdx.x * wpb + (threadIdx.x >> 5); r < n; r += gridDim.x * wpb) {
+    const int t = row_tok ? row_tok[r] : r;
+    const __nv_bfloat16* g = dx + (size_t)r * kp;
+    const int id = ids[t];
+    if (id != pad_id) {
+      float* dst = d_item + (size_t)id * D;
+      for (int j = lane; j < d_true; j += 32) atomicAdd(dst + feat_pad_col(j, hd_valid), __bfloat162float(g[ca.item_col + j]));
+    }
+    if (v_rows)   // zero the staging row first: its numerical columns are written below, the other columns stay zero
+      for (int j = lane; j < v_ld; j += 32) v_rows[(size_t)r * v_ld + j] = __float2bfloat16(0.f);
+    __syncwarp();
+    for (int k = 0; k < ca.n; ++k) {
+      const rp_feature& f = ca.f[k];
+      const int w = ca.dim[k];
+      const __nv_bfloat16* seg = g + ca.col[k];
+      if (f.kind == RP_FEAT_CAT || f.kind == RP_FEAT_BAG_SUM || f.kind == RP_FEAT_BAG_MEAN) {
+        const int32_t* v = reinterpret_cast<const int32_t*>(f.values) + (size_t)t * f.width;
+        float s = 1.f;
+        if (f.kind == RP_FEAT_BAG_MEAN) {
+          int cnt = 0;
+          for (int i = 0; i < f.width; ++i) cnt += feat_live(v[i], f);
+          s = cnt > 0 ? 1.f / (float)cnt : 0.f;
+        }
+        for (int i = 0; i < f.width; ++i) {
+          const int fid = v[i];
+          if (!feat_live(fid, f)) continue;
+          float* dst = f.d_table + (size_t)fid * w;
+          for (int j = lane; j < w; j += 32) atomicAdd(dst + j, __bfloat162float(seg[j]) * s);
+        }
+      } else if (f.kind == RP_FEAT_NUM && v_rows) {
+        const float* v = reinterpret_cast<const float*>(f.values) + (size_t)t * f.width;
+        for (int j = lane; j < f.width; j += 32) v_rows[(size_t)r * v_ld + f.val_col + j] = __float2bfloat16(v[j]);
+      }
+    }
+  }
+}
+
 }  // namespace rp
 
 using namespace rp;
@@ -375,6 +515,134 @@ RP_API int rp_bert_feature_embed_bwd(const void* dx, const uint8_t* pad_mask, co
   RP_FEAT_DISPATCH(d, (feature_embed_bwd_kernel<VEC, true><<<grid, 256, 0, stream>>>(
                           reinterpret_cast<const __nv_bfloat16*>(dx), fa, T, 1.f, drop_p, seed, drop_off, seed_ptr, nullptr,
                           nullptr, nullptr, nullptr, 0, pad_mask, tok_mask)));
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+// ---- ConcatAggregator: see the ConcatArgs comment above and include/rp_b200.h
+// RP_EINVAL for a null pointer or unknown kind; RP_ESHAPE unless the segments (the item's d_true columns at item_col, feature
+// k's seg_dim[k] at seg_col[k]) tile [0, width) exactly, kp is a multiple of 64 in [width, RP_CONCAT_MAX_COLS], identity
+// widths equal their segment and the numerical columns are consecutive (at most RP_FEAT_MAX_NUM_COLS)
+static int concat_args(const rp_feature* feats, const int* seg_col, const int* seg_dim, int n_feats, int item_col, int d,
+                       int hd_valid, int kp, bool bwd, ConcatArgs* ca, int* d_true, int* width) {
+  if (n_feats < 0 || n_feats > RP_FEAT_MAX) return RP_ESHAPE;
+  if (n_feats > 0 && (!feats || !seg_col || !seg_dim)) return RP_EINVAL;
+  if (d != 64 && d != 128 && d != 256 && d != 512) return RP_ESHAPE;
+  if (hd_valid < 0 || hd_valid > 128 || (hd_valid > 0 && d % (hd_valid <= 64 ? 64 : 128))) return RP_ESHAPE;
+  *d_true = hd_valid ? d / (hd_valid <= 64 ? 64 : 128) * hd_valid : d;
+  if (kp <= 0 || kp % 64 || kp > RP_CONCAT_MAX_COLS) return RP_ESHAPE;
+  // the segments tile [0, width): sorted by first column, each starts where the previous one ends
+  int lo[RP_FEAT_MAX + 1], hi[RP_FEAT_MAX + 1];
+  lo[0] = item_col;
+  hi[0] = item_col + *d_true;
+  int num_cols = 0;
+  ca->n = n_feats;
+  ca->item_col = item_col;
+  for (int k = 0; k < n_feats; ++k) {
+    const rp_feature& f = feats[k];
+    const int w = seg_dim[k];
+    if (!f.values) return RP_EINVAL;
+    if (f.width <= 0 || w <= 0 || seg_col[k] < 0) return RP_ESHAPE;
+    switch (f.kind) {
+      case RP_FEAT_CAT:
+      case RP_FEAT_BAG_SUM:
+      case RP_FEAT_BAG_MEAN:
+        if (!f.table || (bwd && !f.d_table)) return RP_EINVAL;
+        if (f.n_rows <= 0 || (f.kind == RP_FEAT_CAT && f.width != 1)) return RP_ESHAPE;
+        break;
+      case RP_FEAT_NUM:
+        if (!f.table || !f.bias) return RP_EINVAL;
+        if (f.val_col != num_cols) return RP_ESHAPE;
+        num_cols += f.width;
+        break;
+      case RP_FEAT_IDENT:
+        if (f.width != w) return RP_ESHAPE;
+        break;
+      default:
+        return RP_EINVAL;
+    }
+    ca->f[k] = f;
+    ca->col[k] = seg_col[k];
+    ca->dim[k] = w;
+    lo[k + 1] = seg_col[k];
+    hi[k + 1] = seg_col[k] + w;
+  }
+  if (num_cols > RP_FEAT_MAX_NUM_COLS) return RP_ESHAPE;
+  int end = 0;
+  for (int done = 0; done <= n_feats; ++done) {   // n <= 17 segments: find the one starting at `end`, n times
+    int next = -1;
+    for (int k = 0; k <= n_feats; ++k)
+      if (lo[k] == end) next = k;
+    if (next < 0) return RP_ESHAPE;
+    end = hi[next];
+  }
+  if (end > kp) return RP_ESHAPE;
+  *width = end;
+  return RP_OK;
+}
+
+static int concat_gather(const void* item_table, const int32_t* ids, const rp_feature* feats, const int* seg_col,
+                         const int* seg_dim, int n_feats, int item_col, const int32_t* row_tok, const int32_t* n_rows_dev,
+                         int T, int d, int hd_valid, int kp, void* x, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!item_table || !ids || !x || T <= 0) return RP_EINVAL;
+  ConcatArgs ca;
+  int d_true, width;
+  const int rc = concat_args(feats, seg_col, seg_dim, n_feats, item_col, d, hd_valid, kp, false, &ca, &d_true, &width);
+  if (rc != RP_OK) return rc;
+  concat_gather_kernel<<<feat_grid(T), 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(item_table), ids, ca, T, d,
+                                                         d_true, hd_valid, width, kp, row_tok, n_rows_dev,
+                                                         reinterpret_cast<__nv_bfloat16*>(x));
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+RP_API int rp_concat_gather(const void* item_table, const int32_t* ids, const rp_feature* feats, const int* seg_col,
+                            const int* seg_dim, int n_feats, int item_col, int T, int d, int hd_valid, int kp, void* x,
+                            void* stream) {
+  return concat_gather(item_table, ids, feats, seg_col, seg_dim, n_feats, item_col, nullptr, nullptr, T, d, hd_valid, kp, x,
+                       stream);
+}
+
+RP_API int rp_concat_gather_rows(const void* item_table, const int32_t* ids, const rp_feature* feats, const int* seg_col,
+                                 const int* seg_dim, int n_feats, int item_col, const int32_t* row_tok,
+                                 const int32_t* n_rows_dev, int T, int d, int hd_valid, int kp, void* x, void* stream) {
+  if (!row_tok || !n_rows_dev) return RP_EINVAL;
+  return concat_gather(item_table, ids, feats, seg_col, seg_dim, n_feats, item_col, row_tok, n_rows_dev, T, d, hd_valid, kp, x,
+                       stream);
+}
+
+RP_API int rp_concat_embed_fwd(const float* y, const float* pos, const int32_t* row_tok, const int32_t* n_rows_dev, int T,
+                               int L, int d, int pos0, float scale, float drop_p, unsigned long long seed,
+                               unsigned long long drop_off, const unsigned long long* seed_ptr, void* out, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!y || !pos || !out || T <= 0 || L <= 0 || pos0 < 0 || (!row_tok != !n_rows_dev)) return RP_EINVAL;
+  if (drop_p < 0.f || drop_p >= 1.f) return RP_EINVAL;
+  const int grid = feat_grid(T);
+  RP_FEAT_DISPATCH(d, (concat_embed_fwd_kernel<VEC><<<grid, 256, 0, stream>>>(y, pos, T, L, pos0, scale, drop_p, seed,
+                                                                              drop_off, seed_ptr, row_tok, n_rows_dev,
+                                                                              reinterpret_cast<__nv_bfloat16*>(out))));
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+RP_API int rp_concat_scatter(const void* dx, const int32_t* ids, float* d_item, int pad_id, const rp_feature* feats,
+                             const int* seg_col, const int* seg_dim, int n_feats, int item_col, const int32_t* row_tok,
+                             const int32_t* n_rows_dev, int T, int d, int hd_valid, int kp, void* v_rows, int v_ld,
+                             void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!dx || !ids || !d_item || T <= 0 || (!row_tok != !n_rows_dev)) return RP_EINVAL;
+  ConcatArgs ca;
+  int d_true, width;
+  const int rc = concat_args(feats, seg_col, seg_dim, n_feats, item_col, d, hd_valid, kp, true, &ca, &d_true, &width);
+  if (rc != RP_OK) return rc;
+  int num_cols = 0;
+  for (int k = 0; k < n_feats; ++k) num_cols += feats[k].kind == RP_FEAT_NUM ? feats[k].width : 0;
+  if (num_cols > 0 && !v_rows) return RP_EINVAL;
+  if (v_rows && (v_ld < num_cols || v_ld % 8)) return RP_ESHAPE;
+  concat_scatter_kernel<<<feat_grid(T), 256, 0, stream>>>(reinterpret_cast<const __nv_bfloat16*>(dx), ids, d_item, pad_id, ca,
+                                                          T, d, d_true, hd_valid, kp, row_tok, n_rows_dev,
+                                                          reinterpret_cast<__nv_bfloat16*>(v_rows), v_ld);
   RP_LAUNCH_CHECK();
   return RP_OK;
 }

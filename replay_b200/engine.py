@@ -19,8 +19,8 @@ from dataclasses import dataclass
 
 import torch
 
-from ._lib import (FEAT_BAG_MEAN, FEAT_BAG_SUM, FEAT_CAT, FEAT_IDENT, FEAT_MAX, FEAT_MAX_NUM_COLS, FEAT_NUM, RpFeature,
-                   SCE_ALL, SampledDesc, SceDesc, AttnBwdDesc, AttnDesc, GemmDesc, WgradPair, check, lib)
+from ._lib import (CONCAT_MAX_COLS, FEAT_BAG_MEAN, FEAT_BAG_SUM, FEAT_CAT, FEAT_IDENT, FEAT_MAX, FEAT_MAX_NUM_COLS, FEAT_NUM,
+                   RpFeature, SCE_ALL, SampledDesc, SceDesc, AttnBwdDesc, AttnDesc, GemmDesc, WgradPair, check, lib)
 
 
 _BLOCK_PARAMS = ("ln1_w", "ln1_b", "in_w", "in_b", "out_w", "out_b", "ln2_w", "ln2_b", "w1", "b1", "w2", "b2")
@@ -112,12 +112,14 @@ class SideFeature:
     ``kind``: "cat" (Embedding), "bag_sum" / "bag_mean" (EmbeddingBag over a categorical list), "num" (Linear(tensor_dim,
     d)) or "ident" (tensor_dim == d: the values themselves).  ``cardinality`` / ``padding_value``: categorical kinds (the
     table has cardinality + 1 rows, the padding row is zero and frozen).  ``width``: tensor_dim of the numerical kinds; a
-    categorical list takes its width from the batch."""
+    categorical list takes its width from the batch.  ``dim``: the feature's own embedding_dim under ConcatAggregator (0:
+    the model's d, as SumAggregator needs)."""
     name: str
     kind: str
     cardinality: int = 0
     padding_value: int = 0
     width: int = 1
+    dim: int = 0
 
     @property
     def categorical(self) -> bool:
@@ -137,8 +139,8 @@ def _check_side_features(fs, d: int, kinds):
             raise ValueError(f"side feature {f.name!r}: unknown kind {f.kind!r}")
         if f.categorical and f.cardinality < 1:
             raise ValueError(f"side feature {f.name!r}: cardinality must be positive")
-        if f.kind == "ident" and f.width != d:
-            raise ValueError(f"side feature {f.name!r}: an identity feature needs tensor_dim == {d}")
+        if f.kind == "ident" and f.width != (f.dim or d):
+            raise ValueError(f"side feature {f.name!r}: an identity feature needs tensor_dim == {f.dim or d}")
 
 
 @dataclass
@@ -146,16 +148,25 @@ class EncoderConfig(BaseConfig):
     variant: str = "new"  # "new": replay.nn.sequential.SasRec ; "legacy": replay.models.nn.sequential.SasRecModel
     lnf_eps: float | None = None
     features: tuple = ()  # SideFeature, ... (new path only); empty: the item-only input of rp_embed_fwd
+    # "sum": SumAggregator, every side feature at width d.  "concat": ConcatAggregator + its Linear(sum of widths, d); the
+    # segments come in ``features`` order with the item's after the first ``concat_item_at`` of them (the reference sorts
+    # them by name)
+    aggregator: str = "sum"
+    concat_item_at: int = 0
     side_pad_rows = True  # a categorical side table has cardinality + 1 rows, its padding row zero and frozen
 
     def __post_init__(self):
         if self.variant not in ("new", "legacy"):
             raise ValueError(f"unknown variant {self.variant}")
+        if self.aggregator not in ("sum", "concat"):
+            raise ValueError(f"unknown aggregator {self.aggregator!r}")
         super().__post_init__()
         if self.lnf_eps is None:
             # new: torch.nn.LayerNorm default (nn/sequential/sasrec/model.py:248); legacy: 1e-8 (sasrec/model.py:463)
             self.lnf_eps = 1e-5 if self.variant == "new" else 1e-8
         self.features = tuple(self.features)
+        if self.aggregator == "concat" and not self.features:
+            raise ValueError("a concatenated input needs side features (the item alone is the item-only model)")
         if self.features:
             self._check_features()
 
@@ -170,6 +181,49 @@ class EncoderConfig(BaseConfig):
         if self.num_cols > FEAT_MAX_NUM_COLS:
             raise ValueError(f"the numerical side features' tensor_dims sum to {self.num_cols}; at most {FEAT_MAX_NUM_COLS} "
                              "are projected inside the embedding kernel")
+        if self.aggregator == "sum":
+            for f in fs:
+                if f.dim not in (0, self.d):
+                    raise ValueError(f"side feature {f.name!r} has embedding_dim {f.dim}; SumAggregator needs the model's {self.d}")
+            return
+        for f in fs:
+            if f.dim < 1:
+                raise ValueError(f"side feature {f.name!r}: ConcatAggregator needs its embedding_dim")
+        if not 0 <= self.concat_item_at <= len(fs):
+            raise ValueError(f"concat_item_at {self.concat_item_at} outside [0, {len(fs)}]")
+        if self.concat_kp > CONCAT_MAX_COLS:
+            raise ValueError(f"the concatenated embeddings are {self.concat_width} wide ({self.concat_kp} padded); the CUDA path "
+                             f"projects at most {CONCAT_MAX_COLS} columns")
+
+    @property
+    def concat(self) -> bool:
+        return self.aggregator == "concat"
+
+    @property
+    def concat_width(self) -> int:
+        """columns of the concatenated input (ConcatAggregator): the item's d plus every side feature's embedding_dim"""
+        return self.d + sum(f.dim for f in self.features)
+
+    @property
+    def concat_kp(self) -> int:
+        """the concatenated input's columns padded for the tensor cores: 64, or a multiple of 128 (the weight-gradient
+        kernel's column tiles, rp_wgrad_group)"""
+        return 64 if self.concat_width <= 64 else _ru(self.concat_width, 128)
+
+    def concat_columns(self):
+        """(first column of the item's segment, first column of every side feature's segment) of the concatenated input"""
+        col, item_col, cols = 0, 0, []
+        for k, f in enumerate(self.features):
+            if k == self.concat_item_at:
+                item_col, col = col, col + self.d
+            cols.append(col)
+            col += f.dim
+        if self.concat_item_at == len(self.features):
+            item_col = col
+        return item_col, cols
+
+    def axis_sizes(self) -> dict:
+        return {**super().axis_sizes(), "k": self.concat_width}   # 'k': the projection's input, true columns first
 
     @property
     def num_cols(self) -> int:
@@ -187,10 +241,13 @@ class EncoderConfig(BaseConfig):
             out += self._block_layout(i, d, "f")
         out += [("lnf_w", (d,), vec), ("lnf_b", (d,), vec)]
         for f in self.features:   # after every item-only parameter: an item-only model keeps its layout and seeded init
+            w, k = (f.dim, None) if self.concat else (d, "f")   # concat: each at its own, unpadded width
             if f.categorical:
-                out.append((f"feat.{f.name}", (f.cardinality + 1, d), emb))
+                out.append((f"feat.{f.name}", (f.cardinality + 1, w), (None, k)))
             elif f.kind == "num":
-                out += [(f"feat.{f.name}.w", (d, f.width), ("f", None)), (f"feat.{f.name}.b", (d,), vec)]
+                out += [(f"feat.{f.name}.w", (w, f.width), (k, None)), (f"feat.{f.name}.b", (w,), (k, None))]
+        if self.concat:   # ConcatAggregator.feat_projection, after every other parameter
+            out += [("feat_proj.w", (d, self.concat_kp), ("f", "k")), ("feat_proj.b", (d,), vec)]
         return out
 
 
@@ -204,7 +261,8 @@ class _CountingLib:
                "rp_post_attn_train": 1, "rp_wgrad_group": 2, "rp_ln_qkv_fused": 1, "rp_pre_attn_bwd": 1,
                "rp_post_attn_bwd": 1, "rp_row_plan": 3, "rp_embed_fwd_rows": 1, "rp_embed_bwd_rows": 2, "rp_ln_qkv_fused_rows": 1,
                "rp_post_attn_train_rows": 1, "rp_post_attn_bwd_rows": 1, "rp_pre_attn_bwd_rows": 1, "rp_wgrad_group_rows": 2,
-               "rp_bert_feature_embed_fwd": 1, "rp_bert_feature_embed_bwd": 1}
+               "rp_bert_feature_embed_fwd": 1, "rp_bert_feature_embed_bwd": 1, "rp_concat_gather": 1, "rp_concat_gather_rows": 1,
+               "rp_concat_embed_fwd": 1, "rp_concat_scatter": 1, "rp_embed_pos_bwd": 1}
 
     def __init__(self, L):
         self._L = L
@@ -244,6 +302,7 @@ class SasRecEngine:
             off = _ru(off + math.prod(shp), 64)
         self._true = cfg.true_shapes()
         self.features = tuple(getattr(cfg, "features", ()))
+        self.concat = getattr(cfg, "concat", False)
         self._side_pad = {f"feat.{f.name}": f.padding_value for f in self.features
                           if f.categorical and cfg.side_pad_rows}
         self.n_flat = off
@@ -385,7 +444,7 @@ class SasRecEngine:
                         v[self.cfg.pad_id].zero_()
                     elif name in self._side_pad:   # CategoricalEmbedding.reset_parameters (nn/embedding.py)
                         v[self._side_pad[name]].zero_()
-                elif name.startswith("feat."):     # a numerical feature's Linear bias keeps torch's default init
+                elif name.startswith(("feat.", "feat_proj.")):   # Linear biases keep torch's default init
                     fan_in = self.true_shape(name[:-1] + "w")[1]
                     v = (torch.rand(shp, generator=g) * 2 - 1) / math.sqrt(fan_in)
                 elif name.endswith(("ln1_w", "ln2_w", "lnf_w")):
@@ -490,21 +549,32 @@ class SasRecEngine:
     def _alloc_features(self):
         """Static staging buffers of the side features (a captured step reads the batch staged into them): int32 [T] / [T, K]
         ids, fp32 [T, tensor_dim] values; a categorical list's buffer is sized by the first batch (set_features).  With
-        numerical features the backward also keeps dS bf16 [T, dp], the gathered values bf16 [T, 64] and their gradients."""
+        numerical features the backward also keeps dS bf16 [T, dp], the gathered values bf16 [T, 64] and their gradients.
+        ConcatAggregator adds the concatenated input X bf16 [T, kp] and its projection fp32 [T, dp]; its backward keeps
+        dY = dS and dX bf16 [T, kp], and the numerical gradients cover all kp rows of dX^T . V."""
         self.feat_in = {}
         if not self.features:
             return
         i32, f32 = dict(device=self.dev, dtype=torch.int32), dict(device=self.dev, dtype=torch.float32)
+        bf = dict(device=self.dev, dtype=torch.bfloat16)
         for f in self.features:
             if f.kind == "cat":
                 self.feat_in[f.name] = torch.full((self.T, 1), f.padding_value, **i32)
             elif not f.categorical:
                 self.feat_in[f.name] = torch.zeros(self.T, f.width, **f32)
-        if self.with_grad and any(f.kind == "num" for f in self.features):
-            self.feat_ds = torch.zeros(self.T, self.cfg.dp, device=self.dev, dtype=torch.bfloat16)
-            self.feat_v = torch.zeros(self.T, FEAT_MAX_NUM_COLS, device=self.dev, dtype=torch.bfloat16)
-            self.feat_dw = torch.zeros(self.cfg.dp, FEAT_MAX_NUM_COLS, **f32)
-            self.feat_db = torch.zeros(self.cfg.dp, **f32)
+        has_num = any(f.kind == "num" for f in self.features)
+        if self.with_grad and (has_num or self.concat):
+            self.feat_ds = torch.zeros(self.T, self.cfg.dp, **bf)
+        if self.with_grad and has_num:
+            rows = self.cfg.concat_kp if self.concat else self.cfg.dp
+            self.feat_v = torch.zeros(self.T, FEAT_MAX_NUM_COLS, **bf)
+            self.feat_dw = torch.zeros(rows, FEAT_MAX_NUM_COLS, **f32)
+            self.feat_db = torch.zeros(rows, **f32)
+        if self.concat:
+            self.cat_x = torch.zeros(self.T, self.cfg.concat_kp, **bf)
+            self.cat_y = torch.zeros(self.T, self.cfg.dp, **f32)
+            if self.with_grad:
+                self.cat_dx = torch.zeros(self.T, self.cfg.concat_kp, **bf)
 
     def set_features(self, feats: dict) -> bool:
         """Stage the side features of the current batch (name -> [B, L] or [B, L, K] tensor, as the reference's
@@ -556,12 +626,81 @@ class SasRecEngine:
                 col += f.width
         return arr
 
+    def _concat_segments(self):
+        """(item_col, seg_col, seg_dim) of rp_concat_*: host int arrays in feature order"""
+        item_col, cols = self.cfg.concat_columns()
+        n = len(self.features)
+        return item_col, (ctypes.c_int * n)(*cols), (ctypes.c_int * n)(*[f.dim for f in self.features])
+
+    def _concat_fwd(self, drop: float, pos0: int):
+        """ConcatAggregator's input stage: gather the segments into X, Y = X . W^T + b on the tensor cores (fp32 out), then
+        x[0] = dropout(Y * sqrt(d) + pos) in one elementwise pass with the item-only dropout stream."""
+        cfg, T, L, d, kp = self.cfg, self.T, self.L, self.cfg.dp, self.cfg.concat_kp
+        fa = self._feature_descs(False)
+        item_col, seg_col, seg_dim = self._concat_segments()
+        item, ids = self.params16["item_emb"].data_ptr(), self.ids32.data_ptr()
+        rt, nr = (self.row_tok, self.n_rows) if self._packed else (None, None)
+        if self._packed:
+            check(self.lib.rp_concat_gather_rows(item, ids, fa, seg_col, seg_dim, len(fa), item_col, rt.data_ptr(), nr.data_ptr(),
+                                                 T, d, cfg.hd_valid, kp, self.cat_x.data_ptr(), self._stream()),
+                  "rp_concat_gather_rows")
+        else:
+            check(self.lib.rp_concat_gather(item, ids, fa, seg_col, seg_dim, len(fa), item_col, T, d, cfg.hd_valid, kp,
+                                            self.cat_x.data_ptr(), self._stream()), "rp_concat_gather")
+        self._gemm(self.cat_x, self.params16["feat_proj.w"], self.cat_y, T, d, kp, bias=self.params["feat_proj.b"], out_mode=2,
+                   m_limit=nr)
+        check(self.lib.rp_concat_embed_fwd(self.cat_y.data_ptr(), self.params["pos_emb"].data_ptr(),
+                                           None if rt is None else rt.data_ptr(), None if nr is None else nr.data_ptr(), T, L, d,
+                                           pos0, math.sqrt(cfg.d), drop, self.seed, 0, self.rng_counter.data_ptr(),
+                                           self.x[0].data_ptr(), self._stream()), "rp_concat_embed_fwd")
+
+    def _concat_bwd(self, dx, drop: float, pos0: int):
+        """Backward of _concat_fwd from the block input's gradient ``dx``: dY = sqrt(d) * dropout'(dx), dX = dY . W, the table
+        rows (item included) from dX, dW / db of the projection and of the numerical features in fixed order, positions."""
+        cfg, G, T, L, d, kp, st = self.cfg, self.grads, self.T, self.L, self.cfg.dp, self.cfg.concat_kp, self._stream
+        packed = self._packed
+        rows = self.n_rows.data_ptr() if packed else None
+        dY, dX = self.feat_ds, self.cat_dx
+        args = (cfg.hd_valid, math.sqrt(cfg.d), drop, self.seed, 0, self.rng_counter.data_ptr(), dY.data_ptr(), None, 0, st())
+        if packed:
+            check(self.lib.rp_feature_embed_bwd_rows(dx.data_ptr(), None, 0, self.row_tok.data_ptr(), rows, T, d, *args),
+                  "rp_feature_embed_bwd_rows")
+        else:
+            check(self.lib.rp_feature_embed_bwd(dx.data_ptr(), None, 0, T, d, *args), "rp_feature_embed_bwd")
+        self._gemm(dY, self.params16["feat_proj.w"], dX, T, kp, d, b_mn=True, m_limit=self.n_rows if packed else None)
+        fa = self._feature_descs(True)
+        item_col, seg_col, seg_dim = self._concat_segments()
+        nc = cfg.num_cols
+        check(self.lib.rp_concat_scatter(dX.data_ptr(), self.ids32.data_ptr(), G["item_emb"].data_ptr(), cfg.pad_id, fa, seg_col,
+                                         seg_dim, len(fa), item_col, self.row_tok.data_ptr() if packed else None, rows, T, d,
+                                         cfg.hd_valid, kp, self.feat_v.data_ptr() if nc else None, FEAT_MAX_NUM_COLS if nc else 0,
+                                         st()), "rp_concat_scatter")
+        # dW = dY^T . X: at most (512 / 128) x (1024 / 128) = 32 output tiles, within one rp_wgrad_group launch
+        n_rows = self.n_rows if packed else None
+        self._wgrad_group([(dY, self.cat_x, G["feat_proj.w"], G["feat_proj.b"])], n_rows)
+        if nc:
+            self.feat_dw.zero_()
+            self.feat_db.zero_()
+            self._wgrad_group([(dX, self.feat_v, self.feat_dw, self.feat_db)], n_rows)
+            col = 0
+            for f, c0 in zip(self.features, seg_col):
+                if f.kind == "num":
+                    G[f"feat.{f.name}.w"].add_(self.feat_dw[c0:c0 + f.dim, col:col + f.width])
+                    G[f"feat.{f.name}.b"].add_(self.feat_db[c0:c0 + f.dim])
+                    col += f.width
+        check(self.lib.rp_embed_pos_bwd(dx.data_ptr(), self.seq_first.data_ptr() if packed else None,
+                                        self.seq_off.data_ptr() if packed else None, self.B, L, d, pos0, drop, self.seed, 0,
+                                        self.rng_counter.data_ptr(), G["pos_emb"].data_ptr(), st()), "rp_embed_pos_bwd")
+
     def _embed_fwd(self, drop: float, pos0: int):
-        """x[0] = the block input: rp_embed_fwd(_rows) for an item-only model, rp_feature_embed_fwd(_rows) with side features."""
+        """x[0] = the block input: rp_embed_fwd(_rows) for an item-only model, rp_feature_embed_fwd(_rows) with side features
+        summed in, _concat_fwd with ConcatAggregator."""
         cfg, T, L, d = self.cfg, self.T, self.L, self.cfg.dp
         p16, prm, pad = self.params16, self.params, self.in_pad
         legacy = cfg.variant == "legacy"
-        if self.features:
+        if self.concat:
+            self._concat_fwd(drop, pos0)
+        elif self.features:
             fa = self._feature_descs(False)
             if self._packed:
                 check(self.lib.rp_feature_embed_fwd_rows(p16["item_emb"].data_ptr(), prm["pos_emb"].data_ptr(),
@@ -1279,6 +1418,9 @@ class SasRecEngine:
                 self._colsum_multi([(dY, db) for dY, _, _, db in pairs])
             dx, other = other, dx
         pos0 = 0 if legacy else cfg.max_len - L
+        if self.concat:
+            self._concat_bwd(dx, drop, pos0)
+            return
         if self.features:
             self._feature_bwd(dx, drop)
         if packed:

@@ -4,6 +4,7 @@ Same construction (``from_params``), same ``forward`` signature and train / infe
 ``state_dict`` key names (SURVEY.md Appendix B); the computation is the fused CUDA path (``replay_b200.core``)."""
 from __future__ import annotations
 
+import dataclasses
 import math
 import warnings
 
@@ -14,7 +15,7 @@ from ..loss import CE
 from ...engine import EncoderConfig
 from ...engine_diff import DiffConfig, DiffEngine
 from ...schema import item_feature_of, side_features_of
-from ..agg import SumAggregator
+from ..agg import ConcatAggregator, SumAggregator
 from ..embedding import SequenceEmbedding
 from ..mask import DefaultAttentionMask
 
@@ -113,16 +114,25 @@ class SasRecBody:
             raise ValueError("the item feature's padding_value must equal its cardinality (replay/data/nn/schema.py:89-90)")
         skip = set(emb.excluded_features) | {schema.query_id_feature_name, schema.timestamp_feature_name}
         side = side_features_of(schema, skip, emb.categorical_list_feature_aggregation_method)
-        if not isinstance(agg, PositionAwareAggregator) or not isinstance(agg.embedding_aggregator, SumAggregator):
-            raise ValueError("embedding_aggregator must be PositionAwareAggregator(SumAggregator(...), ...)")
+        if (not isinstance(agg, PositionAwareAggregator)
+                or not isinstance(agg.embedding_aggregator, (SumAggregator, ConcatAggregator))):
+            raise ValueError("embedding_aggregator must be PositionAwareAggregator(SumAggregator(...) or ConcatAggregator(...), ...)")
+        concat = isinstance(agg.embedding_aggregator, ConcatAggregator)
         if not isinstance(mask, DefaultAttentionMask) or mask.reference_feature_name != name:
             raise ValueError(f"attn_mask_builder must be DefaultAttentionMask on the item feature {name!r}")
         if not isinstance(enc, (SasRecTransformerLayer, DiffTransformerLayer)):
             raise ValueError(f"encoder must be SasRecTransformerLayer or DiffTransformerLayer, got {type(enc).__name__}")
         d = enc.embedding_dim
+        if concat and feat_dim is not None and feat_dim != d:
+            raise ValueError(f"the item feature {name!r} has embedding_dim {feat_dim}; ConcatAggregator's model scores against "
+                             f"its table, so it must be the model's {d}")
         if agg.embedding_aggregator.embedding_dim != d or (feat_dim is not None and feat_dim != d):
             raise ValueError("the embedder, the aggregator and the encoder must share one embedding_dim")
-        _check_side(schema, side, d)
+        agg_kw = {}
+        if concat:
+            side, agg_kw = _concat_side(schema, name, side, agg.embedding_aggregator.input_embedding_dims, d)
+        else:
+            _check_side(schema, side, d)
         if side and not isinstance(enc, SasRecTransformerLayer):
             raise ValueError(f"side features {[f.name for f in side]} need the SasRecTransformerLayer encoder")
         if mask.num_heads != enc.num_heads:
@@ -145,11 +155,26 @@ class SasRecBody:
                 raise ValueError("the aggregator and SasRecTransformerLayer must share one dropout")
             cfg = EncoderConfig(n_items=card, d=d, n_heads=enc.num_heads, n_blocks=enc.num_blocks,
                                 max_len=agg.max_sequence_length, dropout=agg.dropout, variant="new", lnf_eps=eps,
-                                features=tuple(side))
+                                features=tuple(side), **agg_kw)
             return SasRecCore(cfg, item_feature=name, device=device, seed=seed)
         cfg = DiffConfig(n_items=card, d=d, n_heads=enc.num_heads, n_blocks=enc.num_blocks, max_len=agg.max_sequence_length,
                          dropout=agg.dropout, out_norm=out_norm, lnf_eps=eps)
         return _DiffCore(cfg, item_feature=name, device=device, seed=seed)
+
+
+def _concat_side(schema, item: str, side, input_dims, d: int):
+    """ConcatAggregator's side features at their own embedding_dim, in its concatenation order (ascending feature name),
+    and the EncoderConfig arguments that place the item's segment among them.  ValueError when ``input_dims`` are not the
+    embedder's features' widths.  Without side features (the item alone, no projection) it is the item-only model."""
+    widths = {item: d, **{f.name: int(schema[f.name].embedding_dim) for f in side}}
+    if sorted(input_dims) != sorted(widths.values()):
+        raise ValueError(f"ConcatAggregator's input_embedding_dims {sorted(input_dims)} do not match the embedder's features "
+                         f"{widths}")
+    if not side:
+        return side, {}
+    order = sorted(widths)
+    side = sorted((dataclasses.replace(f, dim=widths[f.name]) for f in side), key=lambda f: f.name)
+    return side, {"aggregator": "concat", "concat_item_at": order.index(item)}
 
 
 def _check_side(schema, side, d: int) -> None:
