@@ -49,8 +49,10 @@ static constexpr int kAfVStages = 3;    // V ring of attn_fwd_kernel<128, 2>: 64
 // 64-row box), loaded by thread 0 ahead of pass 2.  Both warpgroups walk every loaded chunk of the tile - a warpgroup whose
 // rows see none of the chunk's keys skips the MMA - and every thread releases a stage once its wgmma on it has completed,
 // so the "empty" barrier always counts kAfThreads arrivals and thread 0 refills the stage after both warpgroups let it go.
+// <64, 1> (81 KB of shared memory) is held to 128 registers so that two CTAs share an SM: one's loads and softmax overlap
+// the other's MMAs.
 template <int HD, int KB>
-__global__ void __launch_bounds__(kAfThreads, 1)
+__global__ void __launch_bounds__(kAfThreads, (HD == 64 && KB == 1) ? 2 : 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
   constexpr int HC = HD / 64;                 // 64-wide head-dim chunks
@@ -204,8 +206,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
   // ---- pass 2: P = exp2(S * scale * log2e - max), row sums, optional copy of the un-dropped P, O += P.V
   const bool own_a = ia >= lead && ia < n, own_b = ib >= lead && ib < n;   // rows of this sequence
-  __nv_bfloat16* pa = (p.p_save && own_a) ? p.p_save + ((size_t)bz * p.Lp + ia) * p.Lp : nullptr;
-  __nv_bfloat16* pb = (p.p_save && own_b) ? p.p_save + ((size_t)bz * p.Lp + ib) * p.Lp : nullptr;
+  // saved probability of query row i, key `key` (formed where it is stored: two row pointers held across pass 2 would
+  // cost the registers that let attn_fwd_kernel<64, 1> run two CTAs per SM)
+  auto p_at = [&](int i, int key) { return reinterpret_cast<uint32_t*>(p.p_save + ((size_t)bz * p.Lp + i) * p.Lp + key); };
   float oacc[HD / 2];
   acc_zero(oacc);
   float suma = 0.f, sumb = 0.f;
@@ -243,8 +246,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         sumb += eb[e];
       }
       if (key < nk32) {
-        if (pa) *reinterpret_cast<uint32_t*>(pa + key) = pack_bf16(ea[0], ea[1]);
-        if (pb) *reinterpret_cast<uint32_t*>(pb + key) = pack_bf16(eb[0], eb[1]);
+        if (p.p_save && own_a) *p_at(ia, key) = pack_bf16(ea[0], ea[1]);
+        if (p.p_save && own_b) *p_at(ib, key) = pack_bf16(eb[0], eb[1]);
       }
       if (drop) {
 #pragma unroll
@@ -277,8 +280,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     for (int j = 0; j < 8; ++j) {
       const int key = ch * 64 + 8 * j + fc;
       if (key < nk32) {
-        if (pa) *reinterpret_cast<uint32_t*>(pa + key) = 0u;
-        if (pb) *reinterpret_cast<uint32_t*>(pb + key) = 0u;
+        if (p.p_save && own_a) *p_at(ia, key) = 0u;
+        if (p.p_save && own_b) *p_at(ib, key) = 0u;
       }
     }
 #pragma unroll
@@ -610,7 +613,10 @@ RP_API int rp_attn_softmax_bwd(void* p_save, void* dpd, const float* inv_sum, in
 //     S^T = K_kb . Q_qs^T, dP^T = V_kb . dO_qs^T       (registers)
 //     P = exp2(s*sl2 - m_i) * inv_i (masked), dS = P * (dP * dropmask/keep - delta_i) * scale, Pd = P * dropmask/keep
 //     dV_kb += Pd^T . dO_qs,  dK_kb += dS^T . Q_qs    (bf16 Pd^T / dS^T as register A operands)
-//   phase 2, rows = queries (block qb): for every 64-key block kb the same S, dP, dS (recomputed), dQ_qb += dS . K_kb
+//   phase 2, rows = queries (block qb): dQ_qb += dS_(qb,kb) . K_kb for every visible 64-key block kb
+//     causal: phase 1 also stores each bf16 dS^T block in shared memory (the causal triangle, at most 10 blocks of 8 KB, in
+//             place of O, which is dead once delta is formed), and phase 2 reads it as an MN-major A operand: MMAs only
+//     non-causal: 16 blocks do not fit beside the operands; phase 2 recomputes S, dP and dS with rows = queries
 // Every gradient element is summed by one warpgroup in a fixed order (deterministic, no atomics); causally empty blocks
 // are skipped.  Row statistics m_i (max in exp2 units) and inv_i (1/rowsum) come from the forward; delta_i = sum_c dO[i,c] O[i,c].
 
@@ -643,8 +649,9 @@ struct AttnBwdMaps {
 
 // dS and Pd of the 64 x 64 block held as an accumulator fragment pair (S, dP).  KEYS_ROWS: fragment rows are keys, columns
 // queries (phase 1); otherwise rows are queries, columns keys (phase 2).  r0 / c0: first row / column position of the block.
+// FULL: every (query, key) pair of the block is visible, so no element is tested.
 // Results packed as bf16 A fragments: pk_s = dS, pk_p = Pd (element order of the accumulator).
-template <bool KEYS_ROWS>
+template <bool KEYS_ROWS, bool FULL>
 __device__ __forceinline__ void attn_bwd_block(const float (&sa)[32], const float (&dpa)[32], uint32_t (&pk_s)[16], uint32_t (&pk_p)[16],
                                                const float4* __restrict__ s_stat, const uint8_t* __restrict__ s_keyok,
                                                const uint32_t* __restrict__ s_colkey, int r0, int c0, int L, bool causal,
@@ -669,7 +676,7 @@ __device__ __forceinline__ void attn_bwd_block(const float (&sa)[32], const floa
           kp = keep ? ks_drop : 0.f;
           kps = keep ? keep_s : 0.f;
         }
-        const bool vis = s_keyok[j] && i < L && (!causal || j <= i);
+        const bool vis = FULL || (s_keyok[j] && i < L && (!causal || j <= i));
         ds2[e] = vis ? pr * fmaf(dpa[4 * q + 2 * h + e], kps, -st.z) : 0.f;
         pd2[e] = vis ? pr * kp : 0.f;
       }
@@ -678,6 +685,7 @@ __device__ __forceinline__ void attn_bwd_block(const float (&sa)[32], const floa
     }
 }
 
+template <bool CAUSAL>
 __global__ void __launch_bounds__(kAbThreads, 1)
 attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
   constexpr int HD = 64;
@@ -689,8 +697,10 @@ attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
   uint8_t* sK = sdO + 2 * TILE;
   uint8_t* sV = sK + 2 * TILE;
   uint8_t* sO = sV + 2 * TILE;
+  uint8_t* sdS = sO;                // causal: dS^T block (kb, qs), kb <= qs, at + ds_blk(kb, qs) * 8192 (O is dead by then)
   __shared__ float4 s_stat[256];    // per query: m, 1/sum, delta * scale, dropout row key
   __shared__ uint8_t s_keyok[256];
+  __shared__ uint8_t s_kok32[8];    // all 32 keys [32 g, 32 g + 32) are real
   __shared__ __align__(16) uint32_t s_colkey[256];
   __shared__ uint64_t bar_load;
 
@@ -739,7 +749,10 @@ attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
       inv = p.inv_sum[(size_t)bz * p.Lp + i];
     }
     const uint32_t rk = drop_row_key(seed_eff, p.drop_off, (unsigned long long)bz * p.Lp + (unsigned long long)(shift + i));
-    s_keyok[i] = i >= lead && i < L && (!p.mask_pad_keys || p.pad_mask[(size_t)b * p.L + shift + i] != 0);
+    const bool key_ok = i >= lead && i < L && (!p.mask_pad_keys || p.pad_mask[(size_t)b * p.L + shift + i] != 0);
+    s_keyok[i] = key_ok;
+    const bool all_ok = __all_sync(0xffffffffu, key_ok);
+    if ((i & 31) == 0) s_kok32[i >> 5] = all_ok;
     s_colkey[i] = drop_col_key((uint32_t)(shift + i));
     mbar_wait(&bar_load, 0);
     if (ti < n_t) {
@@ -792,6 +805,12 @@ attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
       if (rb >= lead && rb < L) *reinterpret_cast<uint32_t*>(base + ((size_t)row0 + rb) * ld + c) = pack_bf16(acc[4 * j + 2], acc[4 * j + 3]);
     }
   };
+  // every (query, key) pair of block (query block qb, key block kb) is visible: all its keys are real, all its queries are
+  // rows < L, and under the causal mask it lies below the diagonal
+  auto block_full = [&](int qb, int kb) -> bool {
+    return s_kok32[2 * kb] && s_kok32[2 * kb + 1] && (qb + 1) * 64 <= L && (!CAUSAL || kb < qb);
+  };
+  auto ds_blk = [](int kb, int qs) { return (uint32_t)(qs * (qs + 1) / 2 + kb) * 8192u; };
   // blocks of this warpgroup: wg and 3 - wg (balances the causal triangle)
 #pragma unroll 1
   for (int u = 0; u < 2; ++u) {
@@ -802,7 +821,7 @@ attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
     acc_zero(dk);
     acc_zero(dv);
 #pragma unroll 1
-    for (int qs = p.causal ? kb : 0; qs < n_blk; ++qs) {
+    for (int qs = CAUSAL ? kb : 0; qs < n_blk; ++qs) {
       float sa[32], dpa[32];
       wg_fence();
       qk(sa, aK + kb * 8192, aQ + qs * 8192);
@@ -812,8 +831,21 @@ attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
       wg_fence_acc(sa);
       wg_fence_acc(dpa);
       uint32_t pk_s[16], pk_p[16];
-      attn_bwd_block<true>(sa, dpa, pk_s, pk_p, s_stat, s_keyok, s_colkey, kb * 64, qs * 64, L, p.causal, sl2, p.scale, drop, thr,
-                           ks_drop);
+      if (block_full(qs, kb))
+        attn_bwd_block<true, true>(sa, dpa, pk_s, pk_p, s_stat, s_keyok, s_colkey, kb * 64, qs * 64, L, CAUSAL, sl2, p.scale, drop,
+                                   thr, ks_drop);
+      else
+        attn_bwd_block<true, false>(sa, dpa, pk_s, pk_p, s_stat, s_keyok, s_colkey, kb * 64, qs * 64, L, CAUSAL, sl2, p.scale, drop,
+                                    thr, ks_drop);
+      if constexpr (CAUSAL) {
+        // dS^T as a swizzled [64 keys x 64 queries] tile: row fr (+ 8), 16-byte chunk q, bf16 pair at fc
+        uint8_t* blk = sdS + ds_blk(kb, qs);
+#pragma unroll
+        for (int q = 0; q < 8; ++q)
+#pragma unroll
+          for (int hr = 0; hr < 2; ++hr)
+            *reinterpret_cast<uint32_t*>(blk + sw128_off((uint32_t)(fr + 8 * hr), (uint32_t)q) + fc * 2) = pk_s[2 * q + hr];
+      }
       wg_fence();
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {   // contraction over the 64 queries of the step
@@ -830,6 +862,12 @@ attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
     store_rows(dk, p.dK, p.ld_dk, p.dk_c0, kb * 64);
     store_rows(dv, p.dV, p.ld_dv, p.dv_c0, kb * 64);
   }
+  if constexpr (CAUSAL) {
+    // phase 2 reads the dS^T blocks through the async proxy, some of them written by the other warpgroup
+    fence_proxy_async();
+    __syncthreads();
+  }
+  const uint32_t adS = smem_u32(sdS);
 #pragma unroll 1
   for (int u = 0; u < 2; ++u) {
     const int qb = u == 0 ? wg : 3 - wg;
@@ -837,29 +875,48 @@ attn_bwd_kernel(const __grid_constant__ AttnBwdMaps tm, const AttnBwdParams p) {
     // ---- phase 2: rows = queries of block qb
     float dq[32];
     acc_zero(dq);
-    const int kb_end = p.causal ? qb + 1 : n_blk;
+    if constexpr (CAUSAL) {
+      // one commit group per key block, one wait for all of them (a single group spanning the loop makes ptxas serialise
+      // the wgmmas)
 #pragma unroll 1
-    for (int kb = 0; kb < kb_end; ++kb) {
-      float sa[32], dpa[32];
-      wg_fence();
-      qk(sa, aQ + qb * 8192, aK + kb * 8192);
-      qk(dpa, adO + qb * 8192, aV + kb * 8192);
-      wg_commit();
-      wg_wait<0>();
-      wg_fence_acc(sa);
-      wg_fence_acc(dpa);
-      uint32_t pk_s[16], pk_p[16];
-      attn_bwd_block<false>(sa, dpa, pk_s, pk_p, s_stat, s_keyok, s_colkey, qb * 64, kb * 64, L, p.causal, sl2, p.scale, drop, thr,
-                            ks_drop);
-      wg_fence();
+      for (int kb = 0; kb <= qb; ++kb) {
+        wg_fence();
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {   // contraction over the 64 keys of the block
-        const uint32_t as[4] = {pk_s[4 * kk], pk_s[4 * kk + 1], pk_s[4 * kk + 2], pk_s[4 * kk + 3]};
-        WgmmaRS<64>::template run<1>(dq, as, desc_mn(aK + kb * 8192 + kk * 2048, 8192), 1);
+        for (int kk = 0; kk < 4; ++kk)   // contraction over the 64 keys of the block
+          WgmmaSS<64>::template run<1, 1>(dq, desc_mn(adS + ds_blk(kb, qb) + kk * 2048, 8192),
+                                          desc_mn(aK + kb * 8192 + kk * 2048, 8192), 1);
+        wg_commit();
       }
-      wg_commit();
       wg_wait<0>();
       wg_fence_acc(dq);
+    } else {
+#pragma unroll 1
+      for (int kb = 0; kb < n_blk; ++kb) {
+        float sa[32], dpa[32];
+        wg_fence();
+        qk(sa, aQ + qb * 8192, aK + kb * 8192);
+        qk(dpa, adO + qb * 8192, aV + kb * 8192);
+        wg_commit();
+        wg_wait<0>();
+        wg_fence_acc(sa);
+        wg_fence_acc(dpa);
+        uint32_t pk_s[16], pk_p[16];
+        if (block_full(qb, kb))
+          attn_bwd_block<false, true>(sa, dpa, pk_s, pk_p, s_stat, s_keyok, s_colkey, qb * 64, kb * 64, L, false, sl2, p.scale, drop,
+                                      thr, ks_drop);
+        else
+          attn_bwd_block<false, false>(sa, dpa, pk_s, pk_p, s_stat, s_keyok, s_colkey, qb * 64, kb * 64, L, false, sl2, p.scale, drop,
+                                       thr, ks_drop);
+        wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {   // contraction over the 64 keys of the block
+          const uint32_t as[4] = {pk_s[4 * kk], pk_s[4 * kk + 1], pk_s[4 * kk + 2], pk_s[4 * kk + 3]};
+          WgmmaRS<64>::template run<1>(dq, as, desc_mn(aK + kb * 8192 + kk * 2048, 8192), 1);
+        }
+        wg_commit();
+        wg_wait<0>();
+        wg_fence_acc(dq);
+      }
     }
     store_rows(dq, p.dQ, p.ld_dq, p.dq_c0, qb * 64);
   }
@@ -930,9 +987,15 @@ RP_API int rp_attn_bwd(const rp_attn_bwd_desc* a, void* stream_) {
     if ((rc = make_tmap_bf16_seq(&tm.d_o, a->d_out, B, L, a->do_cols, a->ld_do, 128)) != RP_OK) return rc;
     if ((rc = make_tmap_bf16_seq(&tm.o, a->out, B, L, (uint64_t)a->H * 64, a->ldo, 128)) != RP_OK) return rc;
   }
-  const int smem = 10 * 128 * 128 + 1024;
-  RP_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  attn_bwd_kernel<<<a->B * a->H, kAbThreads, smem, stream>>>(tm, p);
+  // Q, dO, K, V (2 tiles each), then O (2 tiles) or, causal, the dS^T triangle of up to 10 64 x 64 blocks in its place
+  const int smem = 8 * 128 * 128 + (a->causal ? 10 * 8192 : 2 * 128 * 128) + 1024;
+  if (a->causal) {
+    RP_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attn_bwd_kernel<true><<<a->B * a->H, kAbThreads, smem, stream>>>(tm, p);
+  } else {
+    RP_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attn_bwd_kernel<false><<<a->B * a->H, kAbThreads, smem, stream>>>(tm, p);
+  }
   RP_LAUNCH_CHECK();
   return RP_OK;
 }
