@@ -133,6 +133,20 @@ int rp_bce_head_fwd(const void* hc, const void* table, const float* bias, const 
 int rp_bce_head_bwd(const void* hc, const void* table, const float* bias, const int32_t* labels, const int32_t* n_valid,
                     int capacity, int n_items, int d, const float* loss_out, void* d_hc, float* d_table, float* d_bias,
                     int fused, int n_valid_hint, void* workspace, size_t workspace_bytes, void* stream);
+/* Positive SETS for the full-catalog BCE head (replay/nn/loss/bce.py:51-95 with num_positives > 1, no bias): the target of
+ * row t is 1 at every distinct id in [0, n_items) among labels_p [capacity, num_positives] (rp_prepare_batch_multi; the
+ * slot mask is not read), labels[t] being one of them.  rp_bce_head_fwd / _bwd on labels score labels[t]; then
+ *   rp_bce_head_multi_fwd  loss_out[0] -= loss_out[1] x sum of the other ids' logits (row_sum fp32 [capacity] scratch;
+ *                          rows summed in a fixed order)
+ *   rp_bce_head_multi_bwd  d_hc[t] -= loss_out[1] x sum of their table rows (bf16, read-modify-write),
+ *                          d_table[y] -= loss_out[1] x hc[t] (fp32 atomics)
+ * Ids outside [0, n_items) are skipped (the reference's scatter_ fails on them). */
+int rp_bce_head_multi_fwd(const void* hc, const void* table, const int32_t* labels, const int32_t* labels_p,
+                          const int32_t* n_valid, int capacity, int num_positives, int n_items, int d, float* loss_out,
+                          float* row_sum, void* stream);
+int rp_bce_head_multi_bwd(const void* hc, const void* table, const int32_t* labels, const int32_t* labels_p,
+                          const int32_t* n_valid, int capacity, int num_positives, int n_items, int d, const float* loss_out,
+                          void* d_hc, float* d_table, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Transformer body.  All activations are token-major bf16 [T = B*L, d]; weights are the bf16 shadow of the fp32 masters.
@@ -250,6 +264,18 @@ int rp_attn_last(const void* q, const void* k, const void* v, long long ldk, lon
 int rp_prepare_batch(const int64_t* ids, const uint8_t* pad_mask, const int64_t* labels, const uint8_t* target_mask, int T,
                      int pad_id, int n_items, int32_t* ids32, int32_t* valid_idx, int32_t* labels_c, int32_t* n_valid,
                      int32_t* scratch /* >= ceil(T/1024) ints, needed with targets */, void* stream);
+
+/* Multi-positive targets (replay/nn/loss/base.py:49-154): labels int64 / target_mask bool [T, num_positives], 1 <=
+ * num_positives <= RP_MAX_POSITIVES.  A position is live when one of its slots has the mask set and an id in [0, n_items);
+ * live_mask [T] and live_label [T] (its first such id) are written and then compacted by rp_prepare_batch into valid_idx /
+ * labels_c / n_valid (pass live_label / live_mask to rp_row_plan).  For compacted row t < *n_valid, labels_p[t*P + k] is
+ * slot k's raw id saturated to int32 and slot_mask[t*P + k] = mask set and id in [0, n_items); *n_pairs = number of set
+ * slot_mask entries.  All on the device. */
+#define RP_MAX_POSITIVES 32
+int rp_prepare_batch_multi(const int64_t* ids, const uint8_t* pad_mask, const int64_t* labels, const uint8_t* target_mask,
+                           int T, int num_positives, int pad_id, int n_items, int32_t* ids32, int64_t* live_label,
+                           uint8_t* live_mask, int32_t* valid_idx, int32_t* labels_c, int32_t* labels_p, uint8_t* slot_mask,
+                           int32_t* n_valid, int32_t* n_pairs, int32_t* scratch, void* stream);
 
 /* Row plan of a causal training batch (packed body): seq_first[b] = first position of sequence b whose pad_mask is set or
  * that holds a valid target (L if none); the positions seq_first[b] .. L-1 of all sequences are packed back to back:
@@ -537,7 +563,11 @@ int rp_counter_add(unsigned long long* counter, unsigned long long inc, void* st
  * negatives]; -clamp(log(p + log_eps), -clamp, clamp) of the positive's share p, gradient 0 where the clamp is active),
  * RP_LOSS_CE_SAMPLED_WEIGHTED (CE_SAMPLED's row loss times row_weight[t]; mean over the valid targets, not divided by the
  * weights' sum).  row_weight: fp32 [capacity] in the compacted row order, required (RP_EINVAL) by RP_LOSS_CE_SAMPLED_WEIGHTED
- * and ignored by every other kind.  One positive per position.  fwd: loss_out[0] = mean loss, loss_out[1] = 1/T_v,
+ * and ignored by every other kind.  num_positives (0 or 1: one positive per position) up to RP_MAX_POSITIVES, with kinds
+ * CE_SAMPLED, BCE_SAMPLED and CE_SAMPLED_WEIGHTED only: labels, row_weight and slot_mask are [capacity, num_positives]
+ * (rp_prepare_batch_multi), every set slot is a pair - its own positive against the row's negatives, which are masked
+ * against all num_positives labels of the row - and the mean runs over the *n_pairs pairs (loss_out[1] = 1 / *n_pairs).
+ * fwd: loss_out[0] = mean loss, loss_out[1] = 1/T_v,
  * d(loss)/d(logits) stays in the workspace (which need not be zeroed); bwd: d_hc bf16 [capacity, d] rows < *n_valid, d_table
  * fp32 ACCUMULATED (+=: zero it first; rows that no positive and no unmasked negative points at are left as they were).
  * d_hc rows >= *n_valid: untouched with per-row negatives; with shared negatives rows [*n_valid, min(round_up(*n_valid, 128),
@@ -557,8 +587,10 @@ typedef struct rp_sampled_desc {
   float* loss_out;
   void* workspace; size_t workspace_bytes;
   const float* row_weight;
+  int num_positives; const uint8_t* slot_mask; const int32_t* n_pairs;
 } rp_sampled_desc;
 size_t rp_sampled_head_workspace(int capacity, int d, int n_neg, int neg_mode);
+size_t rp_sampled_head_workspace_multi(int capacity, int d, int n_neg, int neg_mode, int num_positives);
 int rp_sampled_head_fwd(const rp_sampled_desc* s, void* stream);
 int rp_sampled_head_bwd(const rp_sampled_desc* s, void* d_hc, float* d_table, void* stream);
 

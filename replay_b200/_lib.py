@@ -151,6 +151,7 @@ class SampledDesc(ctypes.Structure):
         ("loss_out", c_void_p),
         ("workspace", c_void_p), ("workspace_bytes", c_size_t),
         ("row_weight", c_void_p),
+        ("num_positives", c_int), ("slot_mask", c_void_p), ("n_pairs", c_void_p),
     ]
 
 
@@ -247,6 +248,7 @@ class RpFeature(ctypes.Structure):
 
 FEAT_CAT, FEAT_BAG_SUM, FEAT_BAG_MEAN, FEAT_NUM, FEAT_IDENT = range(5)   # rp_feature.kind
 FEAT_MAX, FEAT_MAX_NUM_COLS = 16, 64
+MAX_POSITIVES = 32       # RP_MAX_POSITIVES: most positive slots per position of a multi-positive batch
 CONCAT_MAX_COLS = 1024   # RP_CONCAT_MAX_COLS: widest concatenated input of ConcatAggregator (padded to 64 columns)
 
 
@@ -296,6 +298,10 @@ _EXTRA_SIGS: list = [
     ("rp_concat_scatter", c_int, [_P, _P, _P, c_int, ctypes.POINTER(RpFeature), _P, _P, c_int, c_int, _P, _P, c_int, c_int, c_int,
                                   c_int, _P, c_int, _P]),
     ("rp_embed_pos_bwd", c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_float, _U64, _U64, _P, _P, _P]),
+    ("rp_prepare_batch_multi", c_int, [_P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    ("rp_sampled_head_workspace_multi", c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    ("rp_bce_head_multi_fwd", c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, _P]),
+    ("rp_bce_head_multi_bwd", c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
 ]
 
 __all__ = ["GemmDesc", "DiffAttnDesc", "DiffLambda", "SceDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "RpFeature", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]

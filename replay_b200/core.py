@@ -273,10 +273,13 @@ class SasRecCore(torch.nn.Module):
             eng.refresh_shadow()
             self._shadow_dirty = False
         self._set_lr(eng, lr)
-        loss_before = getattr(eng, "_loss_applied", None), eng.sampled is None
+        def head_key():   # loss head, positives per position and their buffers: what a captured step depends on
+            return getattr(eng, "_loss_applied", None), eng.sampled is None, eng.n_pos, eng.mp_gen
+
+        loss_before = head_key()
         self._stage(eng, ids, pad_mask, labels, target_mask, negatives, row_weights, feats)
-        if (getattr(eng, "_loss_applied", None), eng.sampled is None) != loss_before:
-            self._drop_graphs()  # another loss head: different kernels / buffers
+        if head_key() != loss_before:
+            self._drop_graphs()  # another loss head or positive count: different kernels / buffers
         if isinstance(all_reduce, str):  # "auto": torch.distributed when initialised (inside Trainer.run)
             return self._graph_trainer(eng).run()[0]
         return eng.train_step(all_reduce, betas=self.adam_betas)[0]

@@ -789,6 +789,48 @@ __global__ void cast_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* _
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// multi-positive targets, labels / target_mask [T, P]: a position is live when a slot has its mask set and an id in
+// [0, n_items); its first such id stands for it in the single-label compaction (prepare_*_kernel) and the row plan.
+// ------------------------------------------------------------------------------------------------------------------
+__global__ void multi_live_kernel(const int64_t* __restrict__ labels, const uint8_t* __restrict__ target_mask, int T, int P,
+                                  int n_items, int64_t* __restrict__ live_label, uint8_t* __restrict__ live_mask) {
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < T; t += gridDim.x * blockDim.x) {
+    int64_t y0 = labels[(size_t)t * P];
+    bool live = false;
+    for (int k = 0; k < P && !live; ++k) {
+      const int64_t y = labels[(size_t)t * P + k];
+      if (target_mask[(size_t)t * P + k] && y >= 0 && y < n_items) {
+        y0 = y;
+        live = true;
+      }
+    }
+    live_label[t] = y0;
+    live_mask[t] = live;
+  }
+}
+
+// the P slots of every compacted live row: raw ids (saturated to int32), slot mask (mask set and id in range), pair count
+__global__ void multi_gather_kernel(const int64_t* __restrict__ labels, const uint8_t* __restrict__ target_mask, int P,
+                                    int n_items, const int32_t* __restrict__ valid_idx, const int32_t* __restrict__ n_valid,
+                                    int32_t* __restrict__ labels_p, uint8_t* __restrict__ slot_mask, int32_t* n_pairs) {
+  const long long n = (long long)*n_valid * P;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long n_round = (n + 31) / 32 * 32;   // whole warps through the loop for the ballot
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n_round; i += stride) {
+    bool m = false;
+    if (i < n) {
+      const size_t src = (size_t)valid_idx[i / P] * P + (size_t)(i % P);
+      const int64_t y = labels[src];
+      m = target_mask[src] != 0 && y >= 0 && y < n_items;
+      labels_p[i] = (int32_t)(y < INT32_MIN ? INT32_MIN : y > INT32_MAX ? INT32_MAX : y);
+      slot_mask[i] = m;
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, m);
+    if ((threadIdx.x & 31) == 0 && bal) atomicAdd(n_pairs, __popc(bal));
+  }
+}
+
 static inline int grid_for(long long work_items, int per_block) {
   long long b = (work_items + per_block - 1) / per_block;
   const long long cap = (long long)sm_count() * 8;
@@ -815,6 +857,26 @@ RP_API int rp_prepare_batch(const int64_t* ids, const uint8_t* pad_mask, const i
     prepare_write_kernel<<<n_blocks, 1024, 0, stream>>>(labels, target_mask, T, n_items, scratch, valid_idx, labels_c, n_valid);
     RP_LAUNCH_CHECK();
   }
+  return RP_OK;
+}
+
+RP_API int rp_prepare_batch_multi(const int64_t* ids, const uint8_t* pad_mask, const int64_t* labels,
+                                  const uint8_t* target_mask, int T, int num_positives, int pad_id, int n_items, int32_t* ids32,
+                                  int64_t* live_label, uint8_t* live_mask, int32_t* valid_idx, int32_t* labels_c,
+                                  int32_t* labels_p, uint8_t* slot_mask, int32_t* n_valid, int32_t* n_pairs, int32_t* scratch,
+                                  void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!labels || !target_mask || !live_label || !live_mask || !labels_p || !slot_mask || !n_pairs) return RP_EINVAL;
+  if (T <= 0 || num_positives < 1 || num_positives > RP_MAX_POSITIVES) return RP_ESHAPE;
+  multi_live_kernel<<<grid_for(T, 256), 256, 0, stream>>>(labels, target_mask, T, num_positives, n_items, live_label, live_mask);
+  RP_LAUNCH_CHECK();
+  const int rc = rp_prepare_batch(ids, pad_mask, live_label, live_mask, T, pad_id, n_items, ids32, valid_idx, labels_c, n_valid,
+                                  scratch, stream_);
+  if (rc != RP_OK) return rc;
+  RP_CUDA_CHECK(cudaMemsetAsync(n_pairs, 0, sizeof(int32_t), stream));
+  multi_gather_kernel<<<grid_for((long long)T * num_positives, 256), 256, 0, stream>>>(
+      labels, target_mask, num_positives, n_items, valid_idx, n_valid, labels_p, slot_mask, n_pairs);
+  RP_LAUNCH_CHECK();
   return RP_OK;
 }
 

@@ -15,6 +15,8 @@
 #define RP_EDRIVER (-4)
 #define RP_EWORKSPACE (-5)
 
+#define RP_MAX_POSITIVES 32   // include/rp_b200.h: most positive slots per position of a multi-positive batch
+
 #define RP_CUDA_CHECK(expr)                  \
   do {                                       \
     cudaError_t _e = (expr);                 \

@@ -6,7 +6,9 @@
 //   LogInCESampled.forward                                        replay/nn/loss/login_ce.py:240-375
 //   CESampledWeighted.forward                                     replay/nn/loss/ce.py:252-330
 //   legacy _compute_loss_ce_sampled / _compute_loss_bce_sampled    replay/models/nn/sequential/sasrec/lightning.py:310-376
-// (single positive per position; the negatives are an INPUT, as in the reference's new path).
+// (the negatives are an INPUT, as in the reference's new path).  Multi-positive rows (num_positives P > 1, new-path CE / BCE /
+// weighted CE only): row t carries P raw labels [t*P, t*P+P) and a slot mask; every masked-in slot is a (position, positive)
+// pair scored against the row's negatives, and the mean runs over the pairs.
 //
 // Layout: hc bf16 [capacity, d] = hidden rows of the valid targets (compacted, rows >= *n_valid ignored); labels int32
 // [capacity]; negatives int64 in one of three shapes: 0 = [N] shared by the whole batch, 1 = [B*L, N] per position,
@@ -44,6 +46,14 @@ struct SampledArgs {
   int ldz, ldn;
 };
 
+// multi-positive rows (P > 1): labels / row_weight are [capacity, P], slot_mask [capacity, P], *n_pairs = masked-in slots.
+// A kernel parameter of its own, after SampledArgs, so that the single-positive kernels keep their parameter layout.
+struct MultiPos {
+  int P;
+  const uint8_t* slot_mask;
+  const int32_t* n_pairs;
+};
+
 __device__ __forceinline__ long long neg_row(const SampledArgs& a, int t) {
   if (a.neg_mode == 0) return 0;
   const int flat = a.valid_idx[t];
@@ -77,9 +87,9 @@ __device__ __forceinline__ float warp_dot(const float (&h)[D / 32], const __nv_b
   return acc;
 }
 
-// one warp per valid token: z_pos = h . E[y]; (modes 1, 2) z_neg[j] = h . E[neg(t, j)]
-template <int D>
-__global__ void sampled_logits_kernel(const SampledArgs a) {
+// one warp per valid token: z_pos = h . E[y] (MP: one per masked-in slot); (modes 1, 2) z_neg[j] = h . E[neg(t, j)]
+template <int D, bool MP>
+__global__ void sampled_logits_kernel(const SampledArgs a, const MultiPos mp) {
   const int n_valid = *a.n_valid;
   const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
   for (int t = blockIdx.x * wpb + (threadIdx.x >> 5); t < n_valid; t += gridDim.x * wpb) {
@@ -90,8 +100,16 @@ __global__ void sampled_logits_kernel(const SampledArgs a) {
       h[2 * k] = v.x;
       h[2 * k + 1] = v.y;
     }
-    const float zp = warp_dot<D>(h, a.table + (size_t)a.labels[t] * D, lane);
-    if (lane == 0) a.zpos[t] = zp;
+    if constexpr (MP) {
+      for (int k = 0; k < mp.P; ++k) {
+        const size_t s = (size_t)t * mp.P + k;
+        const float zp = mp.slot_mask[s] ? warp_dot<D>(h, a.table + (size_t)a.labels[s] * D, lane) : 0.f;
+        if (lane == 0) a.zpos[s] = zp;
+      }
+    } else {
+      const float zp = warp_dot<D>(h, a.table + (size_t)a.labels[t] * D, lane);
+      if (lane == 0) a.zpos[t] = zp;
+    }
     if (a.neg_mode != 0) {
       const int64_t* nr = a.negatives + neg_row(a, t) * a.N;
       for (int j = 0; j < a.N; ++j) {
@@ -99,6 +117,31 @@ __global__ void sampled_logits_kernel(const SampledArgs a) {
         if (lane == 0) a.zneg[(size_t)t * a.ldz + j] = z;
       }
     }
+  }
+}
+
+// loss_out = {sum of the warps' `local` * inv_n, inv_n}: deterministic (block partials in a fixed order, the last block adds)
+__device__ __forceinline__ void sampled_mean(const SampledArgs& a, float local, float inv_n) {
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  __shared__ float red[32];
+  __shared__ bool last;
+  if (lane == 0) red[threadIdx.x >> 5] = local;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int i = 0; i < wpb; ++i) s += red[i];
+    a.block_sums[blockIdx.x] = s;
+    __threadfence();
+    last = (atomicAdd(a.ticket, 1u) == gridDim.x - 1);
+  }
+  __syncthreads();
+  if (last && threadIdx.x == 0) {
+    __threadfence();
+    float s = 0.f;
+    for (int i = 0; i < (int)gridDim.x; ++i) s += reinterpret_cast<volatile float*>(a.block_sums)[i];
+    a.loss_out[0] = s * inv_n;
+    a.loss_out[1] = inv_n;
+    *a.ticket = 0u;
   }
 }
 
@@ -207,33 +250,118 @@ __global__ void sampled_loss_kernel(const SampledArgs a) {
     if (gr)
       for (int j = a.N + lane; j < a.ldn; j += 32) gr[j] = __float2bfloat16(0.f);
   }
-  __shared__ float red[32];
-  __shared__ bool last;
-  if (lane == 0) red[threadIdx.x >> 5] = local;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float s = 0.f;
-    for (int i = 0; i < wpb; ++i) s += red[i];
-    a.block_sums[blockIdx.x] = s;
-    __threadfence();
-    last = (atomicAdd(a.ticket, 1u) == gridDim.x - 1);
+  sampled_mean(a, local, inv_n);
+}
+
+// multi-positive rows (kCESampled / kBCESampled / kCESampledWeighted), one warp per row, lane k < P owns slot k.  A negative
+// is masked when it equals any of the row's P raw labels (masked-out slots included: replay/nn/loss/base.py:139-154 hands
+// every pair the whole label row) or ignore_index, so the masked row is shared by the row's pairs.  CE pair k:
+// lse([z_k, z_neg]) - z_k; BCE pair k: its positive term plus the whole negative row.  Both times w_k (weighted CE), mean
+// over the *n_pairs pairs.  d(loss)/d(z_neg[j]) sums the pairs: exp(z_j - m) sum_k w_k exp(m - m_k) / S_k (CE, m = max of
+// the negatives, m_k = max(m, z_k)), n_pairs(row) x the BCE term.
+__global__ void sampled_loss_multi_kernel(const SampledArgs a, const MultiPos mp) {
+  const int n_valid = *a.n_valid, n_pairs = *mp.n_pairs;
+  const float inv_n = n_pairs > 0 ? __frcp_rn((float)n_pairs) : 0.f;
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  const int t_end = a.neg_mode == 0 ? ((n_valid + 127) / 128) * 128 : n_valid;   // see sampled_loss_kernel
+  const bool ce = a.kind != kBCESampled;
+  float local = 0.f;
+  for (int t = blockIdx.x * wpb + (threadIdx.x >> 5); t < t_end; t += gridDim.x * wpb) {
+    float* zr = a.zneg + (size_t)t * a.ldz;
+    __nv_bfloat16* gr = a.dz16 ? a.dz16 + (size_t)t * a.ldn : nullptr;
+    if (t >= n_valid) {
+      if (gr)
+        for (int j = lane; j < a.ldn; j += 32) gr[j] = __float2bfloat16(0.f);
+      continue;
+    }
+    const int64_t* nr = a.negatives + neg_row(a, t) * a.N;
+    const int32_t* yr = a.labels + (size_t)t * mp.P;
+    const size_t sk = (size_t)t * mp.P + lane;
+    const bool live = lane < mp.P && mp.slot_mask[sk] != 0;
+    const float zk = live ? a.zpos[sk] : 0.f;
+    const float wk = live ? (a.row_weight ? a.row_weight[sk] : 1.f) : 0.f;
+    const int n_row = __popc(__ballot_sync(0xffffffffu, live));
+    float mx = -3.0e38f;   // max of the masked negatives (each CE pair adds its own positive below)
+    for (int j = lane; j < a.N; j += 32) {
+      const int64_t nj = nr[j];
+      bool hit = a.ignore_index >= 0 && nj == (int64_t)a.ignore_index;
+      for (int k = 0; k < mp.P; ++k) hit |= nj == (int64_t)yr[k];
+      const float z = hit ? -1e9f : zr[j];
+      zr[j] = z;
+      mx = fmaxf(mx, z);
+    }
+    if (ce) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+      float s = 0.f;
+      for (int j = lane; j < a.N; j += 32) s += __expf(zr[j] - mx);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+      // pair k: its own log-sum-exp over [z_k | negatives] with m_k = max(mx, z_k), so that another positive of the row far
+      // above z_k cannot flush the sum to 0; S_k >= 1
+      float c = 0.f, row_loss = 0.f;
+      if (live) {
+        const float mk = fmaxf(mx, zk);
+        const float en = __expf(mx - mk), ep = __expf(zk - mk);
+        const float S = s * en + ep;
+        const float inv_s = 1.f / S;
+        row_loss = wk * (mk + logf(S) - zk);
+        c = wk * en * inv_s;
+        a.zpos[sk] = wk * (ep * inv_s - 1.f) * inv_n;
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        c += __shfl_xor_sync(0xffffffffu, c, o);
+        row_loss += __shfl_xor_sync(0xffffffffu, row_loss, o);
+      }
+      const float gs = c * inv_n;
+      for (int j = lane; j < a.N; j += 32) {
+        const float g = __expf(zr[j] - mx) * gs;
+        zr[j] = g;
+        if (gr) gr[j] = __float2bfloat16(g);
+      }
+      if (lane == 0) local += row_loss;
+    } else {
+      float acc = 0.f;
+      const float gs = (float)n_row * inv_n;
+      for (int j = lane; j < a.N; j += 32) {
+        const float z = zr[j];
+        const float sg = 1.f / (1.f + __expf(-z));
+        const float arg = (1.f - sg) + a.log_eps;
+        const float lg = logf(arg);
+        const bool in = lg > -a.clamp && lg < a.clamp;
+        acc += fminf(fmaxf(lg, -a.clamp), a.clamp);
+        const float g = in ? (sg * (1.f - sg) / arg) * gs : 0.f;
+        zr[j] = g;
+        if (gr) gr[j] = __float2bfloat16(g);
+      }
+      float pos = 0.f;
+      if (live) {
+        const float sg = 1.f / (1.f + __expf(-zk));
+        const float arg = sg + a.log_eps;
+        const float lg = logf(arg);
+        const bool in = lg > -a.clamp && lg < a.clamp;
+        a.zpos[sk] = in ? -(sg * (1.f - sg) / arg) * inv_n : 0.f;
+        pos = fminf(fmaxf(lg, -a.clamp), a.clamp);
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        acc += __shfl_xor_sync(0xffffffffu, acc, o);
+        pos += __shfl_xor_sync(0xffffffffu, pos, o);
+      }
+      if (lane == 0) local += -(pos + (float)n_row * acc);
+    }
+    if (gr)
+      for (int j = a.N + lane; j < a.ldn; j += 32) gr[j] = __float2bfloat16(0.f);
   }
-  __syncthreads();
-  if (last && threadIdx.x == 0) {
-    __threadfence();
-    float s = 0.f;
-    for (int i = 0; i < (int)gridDim.x; ++i) s += reinterpret_cast<volatile float*>(a.block_sums)[i];
-    a.loss_out[0] = s * inv_n;
-    a.loss_out[1] = inv_n;
-    *a.ticket = 0u;
-  }
+  sampled_mean(a, local, inv_n);
 }
 
 // backward, one warp per token: dH[t] (+)= dz_pos E[y] (+ sum_j dz_j E[neg_j] for per-token negatives);
-// dE[y] += dz_pos h;  dE[neg_j] += dz_j h  (fp32 atomics)
-template <int D>
+// dE[y] += dz_pos h;  dE[neg_j] += dz_j h  (fp32 atomics).  MP: every masked-in slot's positive, summed in slot order
+template <int D, bool MP>
 __global__ void sampled_bwd_kernel(const SampledArgs a, __nv_bfloat16* __restrict__ d_hc, float* __restrict__ d_table,
-                                   int add_to_dhc) {
+                                   int add_to_dhc, const MultiPos mp) {
   const int n_valid = *a.n_valid;
   const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
   for (int t = blockIdx.x * wpb + (threadIdx.x >> 5); t < n_valid; t += gridDim.x * wpb) {
@@ -260,7 +388,14 @@ __global__ void sampled_bwd_kernel(const SampledArgs a, __nv_bfloat16* __restric
         atomicAdd(dr + k * 64 + lane * 2 + 1, g * h[2 * k + 1]);
       }
     };
-    one(a.labels[t], a.zpos[t]);
+    if constexpr (MP) {
+      for (int k = 0; k < mp.P; ++k) {
+        const size_t s = (size_t)t * mp.P + k;
+        if (mp.slot_mask[s]) one(a.labels[s], a.zpos[s]);
+      }
+    } else {
+      one(a.labels[t], a.zpos[t]);
+    }
     if (a.neg_mode != 0) {
       const int64_t* nr = a.negatives + neg_row(a, t) * a.N;
       const float* gz = a.zneg + (size_t)t * a.ldz;
@@ -285,6 +420,107 @@ __global__ void sampled_scatter_neg_kernel(const SampledArgs a, float* __restric
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// Full-catalog BCE over a positive SET per row (replay/nn/loss/bce.py:51-95, num_positives P > 1): the target of live row t
+// is 1 at every distinct id in [0, n_items) among its P raw slots (scatter_(value=1); the slot mask is not read inside a
+// live row).  rp_bce_head_* score labels[t] as the row's positive; the other ids of the set ("extra" positives) add
+// -x_t,y / T_v to the loss and -1/T_v x E[y] to dH[t], -1/T_v x h_t to dE[y].
+// ------------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool bce_extra(const int32_t* __restrict__ yr, int k, int y0, int n_items) {
+  const int y = yr[k];
+  if (y < 0 || y >= n_items || y == y0) return false;
+  for (int j = 0; j < k; ++j)
+    if (yr[j] == y) return false;
+  return true;
+}
+
+// one warp per live row: row_sum[t] = sum of the extra positives' logits
+template <int D>
+__global__ void bce_extra_fwd_kernel(const __nv_bfloat16* __restrict__ hc, const __nv_bfloat16* __restrict__ table,
+                                     const int32_t* __restrict__ labels, const int32_t* __restrict__ labels_p,
+                                     const int32_t* __restrict__ n_valid_dev, int P, int n_items, float* __restrict__ row_sum) {
+  const int n_valid = *n_valid_dev;
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  for (int t = blockIdx.x * wpb + (threadIdx.x >> 5); t < n_valid; t += gridDim.x * wpb) {
+    float h[D / 32];
+#pragma unroll
+    for (int k = 0; k < D / 64; ++k) {
+      const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(hc + (size_t)t * D + k * 64 + lane * 2));
+      h[2 * k] = v.x;
+      h[2 * k + 1] = v.y;
+    }
+    const int32_t* yr = labels_p + (size_t)t * P;
+    float s = 0.f;
+    for (int k = 0; k < P; ++k)
+      if (bce_extra(yr, k, labels[t], n_items)) s += warp_dot<D>(h, table + (size_t)yr[k] * D, lane);
+    if (lane == 0) row_sum[t] = s;
+  }
+}
+
+// one block: loss_out[0] -= (sum_t row_sum[t]) x loss_out[1], the rows summed in a fixed order
+__global__ void __launch_bounds__(1024) bce_extra_loss_kernel(const float* __restrict__ row_sum,
+                                                              const int32_t* __restrict__ n_valid_dev, float* loss_out) {
+  __shared__ float red[32];
+  const int n_valid = *n_valid_dev;
+  float s = 0.f;
+  for (int t = threadIdx.x; t < n_valid; t += blockDim.x) s += row_sum[t];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float tot = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += red[w];
+    if (n_valid > 0) loss_out[0] -= tot * loss_out[1];
+  }
+}
+
+// one warp per live row: dH[t] -= inv_n sum_extra E[y] (in registers, slot order), dE[y] -= inv_n h_t (fp32 atomics)
+template <int D>
+__global__ void bce_extra_bwd_kernel(const __nv_bfloat16* __restrict__ hc, const __nv_bfloat16* __restrict__ table,
+                                     const int32_t* __restrict__ labels, const int32_t* __restrict__ labels_p,
+                                     const int32_t* __restrict__ n_valid_dev, int P, int n_items,
+                                     const float* __restrict__ loss_out, __nv_bfloat16* __restrict__ d_hc,
+                                     float* __restrict__ d_table) {
+  const int n_valid = *n_valid_dev;
+  const float g = -loss_out[1];
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  for (int t = blockIdx.x * wpb + (threadIdx.x >> 5); t < n_valid; t += gridDim.x * wpb) {
+    const int32_t* yr = labels_p + (size_t)t * P;
+    float h[D / 32], acc[D / 32];
+#pragma unroll
+    for (int k = 0; k < D / 64; ++k) {
+      const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(hc + (size_t)t * D + k * 64 + lane * 2));
+      h[2 * k] = v.x;
+      h[2 * k + 1] = v.y;
+      acc[2 * k] = 0.f;
+      acc[2 * k + 1] = 0.f;
+    }
+    bool any = false;
+    for (int kk = 0; kk < P; ++kk) {
+      if (!bce_extra(yr, kk, labels[t], n_items)) continue;
+      any = true;
+      const __nv_bfloat16* er = table + (size_t)yr[kk] * D;
+      float* dr = d_table + (size_t)yr[kk] * D;
+#pragma unroll
+      for (int k = 0; k < D / 64; ++k) {
+        const float2 e = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(er + k * 64 + lane * 2));
+        acc[2 * k] = fmaf(g, e.x, acc[2 * k]);
+        acc[2 * k + 1] = fmaf(g, e.y, acc[2 * k + 1]);
+        atomicAdd(dr + k * 64 + lane * 2, g * h[2 * k]);
+        atomicAdd(dr + k * 64 + lane * 2 + 1, g * h[2 * k + 1]);
+      }
+    }
+    if (!any) continue;
+#pragma unroll
+    for (int k = 0; k < D / 64; ++k) {
+      uint32_t* p = reinterpret_cast<uint32_t*>(d_hc + (size_t)t * D + k * 64 + lane * 2);
+      const float2 o = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p));
+      *p = pack_bf16(o.x + acc[2 * k], o.y + acc[2 * k + 1]);
+    }
+  }
+}
+
 }  // namespace rp
 
 using namespace rp;
@@ -297,6 +533,7 @@ struct rp_sampled_desc {
   float* loss_out;
   void* workspace; size_t workspace_bytes;
   const float* row_weight;
+  int num_positives; const uint8_t* slot_mask; const int32_t* n_pairs;
 };
 
 static size_t ru(size_t x, size_t m) { return (x + m - 1) / m * m; }
@@ -306,7 +543,8 @@ static size_t sampled_layout(const rp_sampled_desc* s, SampledArgs* a) {
   const int ldz = (int)ru((size_t)s->n_neg, 4), ldn = (int)ru((size_t)s->n_neg, 8);
   size_t off = 0;
   auto take = [&](size_t bytes) { const size_t o = off; off = ru(off + bytes, 256); return o; };
-  const size_t o_zpos = take(cap128 * 4), o_zneg = take(cap128 * ldz * 4);
+  const size_t P = s->num_positives > 1 ? (size_t)s->num_positives : 1;
+  const size_t o_zpos = take(cap128 * P * 4), o_zneg = take(cap128 * ldz * 4);
   const size_t o_dz16 = s->neg_mode == 0 ? take(cap128 * ldn * 2) : 0;
   const size_t o_eneg = s->neg_mode == 0 ? take((size_t)s->n_neg * s->d * 2) : 0;
   const size_t o_deneg = s->neg_mode == 0 ? take((size_t)s->n_neg * s->d * 4) : 0;
@@ -326,7 +564,7 @@ static size_t sampled_layout(const rp_sampled_desc* s, SampledArgs* a) {
   return off;
 }
 
-static int sampled_args(const rp_sampled_desc* s, SampledArgs* a) {
+static int sampled_args(const rp_sampled_desc* s, SampledArgs* a, MultiPos* mp) {
   if (!s || !s->hc || !s->table || !s->labels || !s->negatives || !s->n_valid || !s->loss_out || !s->workspace) return RP_EINVAL;
   if (s->capacity <= 0 || s->n_items <= 0 || s->n_neg <= 0) return RP_ESHAPE;
   if (s->d != 64 && s->d != 128 && s->d != 256 && s->d != 512) return RP_ESHAPE;
@@ -334,6 +572,10 @@ static int sampled_args(const rp_sampled_desc* s, SampledArgs* a) {
   if (s->kind == kCESampledWeighted && !s->row_weight) return RP_EINVAL;
   if (s->neg_mode != 0 && (!s->valid_idx || s->seq_len <= 0)) return RP_EINVAL;
   if (s->kind == kLegacyCE && s->vocab_size < 2) return RP_EINVAL;
+  if (s->num_positives < 0 || s->num_positives > RP_MAX_POSITIVES) return RP_ESHAPE;
+  if (s->num_positives > 1 && (!s->slot_mask || !s->n_pairs ||
+                               (s->kind != kCESampled && s->kind != kBCESampled && s->kind != kCESampledWeighted)))
+    return RP_EINVAL;
   if (s->workspace_bytes < sampled_layout(s, nullptr)) return RP_EWORKSPACE;
   a->hc = reinterpret_cast<const __nv_bfloat16*>(s->hc);
   a->table = reinterpret_cast<const __nv_bfloat16*>(s->table);
@@ -342,6 +584,9 @@ static int sampled_args(const rp_sampled_desc* s, SampledArgs* a) {
   a->capacity = s->capacity; a->n_items = s->n_items; a->d = s->d; a->N = s->n_neg; a->neg_mode = s->neg_mode;
   a->L = s->seq_len; a->kind = s->kind; a->ignore_index = s->ignore_index; a->vocab_size = s->vocab_size;
   a->log_eps = s->log_eps; a->clamp = s->clamp; a->loss_out = s->loss_out;
+  mp->P = s->num_positives > 1 ? s->num_positives : 1;
+  mp->slot_mask = mp->P > 1 ? s->slot_mask : nullptr;
+  mp->n_pairs = mp->P > 1 ? s->n_pairs : nullptr;
   sampled_layout(s, a);
   return RP_OK;
 }
@@ -354,19 +599,24 @@ static int sampled_args(const rp_sampled_desc* s, SampledArgs* a) {
     default: { constexpr int D = 512; CALL; } break;   \
   }
 
-RP_API size_t rp_sampled_head_workspace(int capacity, int d, int n_neg, int neg_mode) {
+RP_API size_t rp_sampled_head_workspace_multi(int capacity, int d, int n_neg, int neg_mode, int num_positives) {
   rp_sampled_desc s;
   memset(&s, 0, sizeof(s));
-  s.capacity = capacity; s.d = d; s.n_neg = n_neg; s.neg_mode = neg_mode;
-  if (capacity <= 0 || d <= 0 || n_neg <= 0) return 0;
+  s.capacity = capacity; s.d = d; s.n_neg = n_neg; s.neg_mode = neg_mode; s.num_positives = num_positives;
+  if (capacity <= 0 || d <= 0 || n_neg <= 0 || num_positives < 0 || num_positives > RP_MAX_POSITIVES) return 0;
   return sampled_layout(&s, nullptr);
 }
 
-// loss_out[0] = mean loss over the valid targets, loss_out[1] = 1/T_v; the workspace keeps d(loss)/d(logits) for the backward
+RP_API size_t rp_sampled_head_workspace(int capacity, int d, int n_neg, int neg_mode) {
+  return rp_sampled_head_workspace_multi(capacity, d, n_neg, neg_mode, 1);
+}
+
+// loss_out[0] = mean loss over the valid targets (the pairs with P > 1), loss_out[1] = 1 / their count; the workspace keeps d(loss)/d(logits) for the backward
 RP_API int rp_sampled_head_fwd(const rp_sampled_desc* s, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   SampledArgs a;
-  int rc = sampled_args(s, &a);
+  MultiPos mp;
+  int rc = sampled_args(s, &a, &mp);
   if (rc != RP_OK) return rc;
   const int blocks = sm_count() * 4;
   RP_CUDA_CHECK(cudaMemsetAsync(a.ticket, 0, 64, stream));
@@ -381,9 +631,15 @@ RP_API int rp_sampled_head_fwd(const rp_sampled_desc* s, void* stream_) {
     g.m_limit_dev = a.n_valid;
     if ((rc = rp_gemm(&g, stream_)) != RP_OK) return rc;
   }
-  RP_DISPATCH_SD(a.d, (sampled_logits_kernel<D><<<blocks, 256, 0, stream>>>(a)));
-  RP_LAUNCH_CHECK();
-  sampled_loss_kernel<<<blocks < 1024 ? blocks : 1024, 256, 0, stream>>>(a);
+  if (mp.P > 1) {
+    RP_DISPATCH_SD(a.d, (sampled_logits_kernel<D, true><<<blocks, 256, 0, stream>>>(a, mp)));
+    RP_LAUNCH_CHECK();
+    sampled_loss_multi_kernel<<<blocks < 1024 ? blocks : 1024, 256, 0, stream>>>(a, mp);
+  } else {
+    RP_DISPATCH_SD(a.d, (sampled_logits_kernel<D, false><<<blocks, 256, 0, stream>>>(a, mp)));
+    RP_LAUNCH_CHECK();
+    sampled_loss_kernel<<<blocks < 1024 ? blocks : 1024, 256, 0, stream>>>(a);
+  }
   RP_LAUNCH_CHECK();
   return RP_OK;
 }
@@ -392,7 +648,8 @@ RP_API int rp_sampled_head_fwd(const rp_sampled_desc* s, void* stream_) {
 RP_API int rp_sampled_head_bwd(const rp_sampled_desc* s, void* d_hc, float* d_table, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   SampledArgs a;
-  int rc = sampled_args(s, &a);
+  MultiPos mp;
+  int rc = sampled_args(s, &a, &mp);
   if (rc != RP_OK) return rc;
   if (!d_hc || !d_table) return RP_EINVAL;
   const int blocks = sm_count() * 4;
@@ -416,8 +673,54 @@ RP_API int rp_sampled_head_bwd(const rp_sampled_desc* s, void* d_hc, float* d_ta
     sampled_scatter_neg_kernel<<<(a.N + 7) / 8, 256, 0, stream>>>(a, d_table);
     RP_LAUNCH_CHECK();
   }
-  RP_DISPATCH_SD(a.d, (sampled_bwd_kernel<D><<<blocks, 256, 0, stream>>>(a, reinterpret_cast<__nv_bfloat16*>(d_hc), d_table,
-                                                                        a.neg_mode == 0 ? 1 : 0)));
+  __nv_bfloat16* dh = reinterpret_cast<__nv_bfloat16*>(d_hc);
+  const int add = a.neg_mode == 0 ? 1 : 0;
+  if (mp.P > 1) {
+    RP_DISPATCH_SD(a.d, (sampled_bwd_kernel<D, true><<<blocks, 256, 0, stream>>>(a, dh, d_table, add, mp)));
+  } else {
+    RP_DISPATCH_SD(a.d, (sampled_bwd_kernel<D, false><<<blocks, 256, 0, stream>>>(a, dh, d_table, add, mp)));
+  }
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+static int bce_multi_check(const void* hc, const void* table, const int32_t* labels, const int32_t* labels_p,
+                           const int32_t* n_valid, int capacity, int num_positives, int n_items, int d) {
+  if (!hc || !table || !labels || !labels_p || !n_valid) return RP_EINVAL;
+  if (capacity <= 0 || n_items <= 0 || num_positives < 1 || num_positives > RP_MAX_POSITIVES) return RP_ESHAPE;
+  if (d != 64 && d != 128 && d != 256 && d != 512) return RP_ESHAPE;
+  return RP_OK;
+}
+
+RP_API int rp_bce_head_multi_fwd(const void* hc, const void* table, const int32_t* labels, const int32_t* labels_p,
+                                 const int32_t* n_valid, int capacity, int num_positives, int n_items, int d, float* loss_out,
+                                 float* row_sum, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  int rc = bce_multi_check(hc, table, labels, labels_p, n_valid, capacity, num_positives, n_items, d);
+  if (rc != RP_OK) return rc;
+  if (!loss_out || !row_sum) return RP_EINVAL;
+  const __nv_bfloat16* h = reinterpret_cast<const __nv_bfloat16*>(hc);
+  const __nv_bfloat16* e = reinterpret_cast<const __nv_bfloat16*>(table);
+  RP_DISPATCH_SD(d, (bce_extra_fwd_kernel<D><<<sm_count() * 4, 256, 0, stream>>>(h, e, labels, labels_p, n_valid,
+                                                                                 num_positives, n_items, row_sum)));
+  RP_LAUNCH_CHECK();
+  bce_extra_loss_kernel<<<1, 1024, 0, stream>>>(row_sum, n_valid, loss_out);
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+RP_API int rp_bce_head_multi_bwd(const void* hc, const void* table, const int32_t* labels, const int32_t* labels_p,
+                                 const int32_t* n_valid, int capacity, int num_positives, int n_items, int d,
+                                 const float* loss_out, void* d_hc, float* d_table, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  int rc = bce_multi_check(hc, table, labels, labels_p, n_valid, capacity, num_positives, n_items, d);
+  if (rc != RP_OK) return rc;
+  if (!loss_out || !d_hc || !d_table) return RP_EINVAL;
+  const __nv_bfloat16* h = reinterpret_cast<const __nv_bfloat16*>(hc);
+  const __nv_bfloat16* e = reinterpret_cast<const __nv_bfloat16*>(table);
+  RP_DISPATCH_SD(d, (bce_extra_bwd_kernel<D><<<sm_count() * 4, 256, 0, stream>>>(
+                        h, e, labels, labels_p, n_valid, num_positives, n_items, loss_out,
+                        reinterpret_cast<__nv_bfloat16*>(d_hc), d_table)));
   RP_LAUNCH_CHECK();
   return RP_OK;
 }

@@ -20,7 +20,7 @@ from dataclasses import dataclass
 import torch
 
 from ._lib import (CONCAT_MAX_COLS, FEAT_BAG_MEAN, FEAT_BAG_SUM, FEAT_CAT, FEAT_IDENT, FEAT_MAX, FEAT_MAX_NUM_COLS, FEAT_NUM,
-                   RpFeature, SCE_ALL, SampledDesc, SceDesc, AttnBwdDesc, AttnDesc, GemmDesc, WgradPair, check, lib)
+                   MAX_POSITIVES, RpFeature, SCE_ALL, SampledDesc, SceDesc, AttnBwdDesc, AttnDesc, GemmDesc, WgradPair, check, lib)
 
 
 _BLOCK_PARAMS = ("ln1_w", "ln1_b", "in_w", "in_b", "out_w", "out_b", "ln2_w", "ln2_b", "w1", "b1", "w2", "b2")
@@ -262,7 +262,8 @@ class _CountingLib:
                "rp_post_attn_bwd": 1, "rp_row_plan": 3, "rp_embed_fwd_rows": 1, "rp_embed_bwd_rows": 2, "rp_ln_qkv_fused_rows": 1,
                "rp_post_attn_train_rows": 1, "rp_post_attn_bwd_rows": 1, "rp_pre_attn_bwd_rows": 1, "rp_wgrad_group_rows": 2,
                "rp_bert_feature_embed_fwd": 1, "rp_bert_feature_embed_bwd": 1, "rp_concat_gather": 1, "rp_concat_gather_rows": 1,
-               "rp_concat_embed_fwd": 1, "rp_concat_scatter": 1, "rp_embed_pos_bwd": 1}
+               "rp_concat_embed_fwd": 1, "rp_concat_scatter": 1, "rp_embed_pos_bwd": 1, "rp_prepare_batch_multi": 4,
+               "rp_bce_head_multi_fwd": 2, "rp_bce_head_multi_bwd": 1}
 
     def __init__(self, L):
         self._L = L
@@ -336,6 +337,7 @@ class SasRecEngine:
         self._packed = False      # the staged training batch runs packed (set by _prepare)
         self.fused_ce = True      # single-pass CE forward + dH (guarded on the device by a bound on |logit|)
         self.n_valid_hint = 0     # host estimate of the number of valid targets per step (load balance of the CE head only)
+        self.mp_gen = 0           # bumped whenever the multi-positive buffers move (_ensure_multi)
         self._alloc_workspace()
         self.init_parameters(seed)
 
@@ -520,6 +522,8 @@ class SasRecEngine:
         self.n_rows = torch.zeros(1, **i32)
         self.row_tok = torch.zeros(T, **i32)
         self.valid_rows = torch.zeros(T, **i32)
+        # multi-positive targets of the staged batch (n_pos > 1): buffers sized by (T, n_pos), allocated by _ensure_multi
+        self.n_pos, self.mp = 1, None
         # hidden states and saved activations per block APPLICATION (cfg.n_apps; the same as n_blocks unless blocks repeat)
         self.x = [torch.zeros(T, d, **bf) for _ in range(cfg.n_apps + 1)]
         self.act = []
@@ -913,23 +917,76 @@ class SasRecEngine:
         return 1 + app * 8 + k
 
     # ------------------------------------------------------------------------------------------------ forward
+    # heads that take several positives per position (replay/nn/loss/base.py:49-154, bce.py:51-95)
+    MULTI_POSITIVE_KINDS = ("bce", "ce_sampled", "bce_sampled", "ce_sampled_weighted")
+
     def set_batch(self, ids, pad_mask, labels=None, target_mask=None):
-        """Stage one batch ([B, L] int64 ids, bool masks) into the engine's static input buffers (device copies)."""
+        """Stage one batch ([B, L] int64 ids, bool masks) into the engine's static input buffers (device copies).  Targets
+        are [B, L] or [B, L, P] (P positives per position; P = 1 is the [B, L] batch)."""
         B, L = ids.shape
         if L != self.L or B > self.B:
             raise ValueError(f"batch shape {tuple(ids.shape)} does not fit engine ({self.B}, {self.L})")
+        P = 1
+        if labels is not None:
+            labels, target_mask, P = self._split_positives(labels, target_mask)
         self.cur_B = B
         n = B * L
         self.in_ids[:n].copy_(ids.reshape(-1), non_blocking=True)
         self.in_pad[:n].copy_(pad_mask.reshape(-1), non_blocking=True)
-        if labels is not None:
+        if P > 1:
+            mp = self._ensure_multi(P)
+            mp["labels"][:n].copy_(labels.reshape(n, P), non_blocking=True)
+            mp["tmask"][:n].copy_(target_mask.reshape(n, P), non_blocking=True)
+            mp["tmask"][n:].zero_()
+        elif labels is not None:
             self.in_labels[:n].copy_(labels.reshape(-1), non_blocking=True)
             self.in_tmask[:n].copy_(target_mask.reshape(-1), non_blocking=True)
+        self.n_pos = P
         if n < self.T:
             self.in_pad[n:].zero_()
             self.in_tmask[n:].zero_()
         if self.sce is not None:
             self.sce["n_rows"].fill_(n)
+
+    def _split_positives(self, labels, target_mask):
+        """(labels, target_mask, P) of a [B, L] or [B, L, P] target batch; [B, L, 1] is the [B, L] batch."""
+        if labels.dim() != 3 or labels.shape[-1] == 1:
+            if labels.dim() == 3:
+                labels = labels[..., 0]
+            if target_mask is not None and target_mask.dim() == 3:
+                target_mask = target_mask[..., 0]
+            return labels, target_mask, 1
+        P = labels.shape[-1]
+        if target_mask is None or target_mask.shape != labels.shape:
+            raise ValueError(f"target_padding_mask must have the labels' shape {tuple(labels.shape)}")
+        if P > MAX_POSITIVES:
+            raise ValueError(f"at most {MAX_POSITIVES} positives per position are supported, got {P}")
+        kind = self._loss_args[0] if self._loss_args is not None else "ce"
+        if kind not in self.MULTI_POSITIVE_KINDS:
+            raise NotImplementedError(f"multi-positive labels are not supported by the {kind!r} head")
+        return labels, target_mask, P
+
+    def _ensure_multi(self, P: int) -> dict:
+        """Staging and compaction buffers of a batch with P positives per position (rp_prepare_batch_multi), and a sampled
+        head's workspace large enough for P.  Reallocating bumps ``mp_gen`` (captured steps hold the old buffers)."""
+        T, dev = self.T, self.dev
+        if self.mp is None or self.mp["P"] != P:
+            self.mp = dict(P=P, labels=torch.zeros(T, P, device=dev, dtype=torch.int64),
+                           tmask=torch.zeros(T, P, device=dev, dtype=torch.bool),
+                           labels_p=torch.zeros(T, P, device=dev, dtype=torch.int32),
+                           slot=torch.zeros(T, P, device=dev, dtype=torch.uint8),
+                           n_pairs=torch.zeros(1, device=dev, dtype=torch.int32),
+                           row_sum=torch.zeros(T, device=dev, dtype=torch.float32),
+                           roww=torch.ones(T, P, device=dev, dtype=torch.float32),
+                           roww_c=torch.ones(T, P, device=dev, dtype=torch.float32))
+            self.mp_gen += 1
+        sp = self.sampled
+        if sp is not None:
+            need = self.lib.rp_sampled_head_workspace_multi(T, self.cfg.dp, sp["n_neg"], sp["mode"], P)
+            if sp["ws_bytes"] < need:
+                sp["ws"], sp["ws_bytes"] = torch.zeros(need, device=dev, dtype=torch.uint8), need
+                self.mp_gen += 1
+        return self.mp
 
     # ------------------------------------------------------------------------------------------------ sampled heads
     SAMPLED_KINDS = {"ce_sampled": 0, "bce_sampled": 1, "legacy_ce_sampled": 2, "legacy_bce_sampled": 3, "login_ce_sampled": 4,
@@ -1027,7 +1084,15 @@ class SasRecEngine:
             self.roww_c = torch.ones(self.T, device=self.dev, dtype=torch.float32)
 
     def set_row_weights(self, weights):
-        """Stage the sample weights of the current batch ([B, L] float, one per position; only valid targets are read)."""
+        """Stage the sample weights of the current batch ([B, L] float, one per position; only valid targets are read).
+        A batch with P > 1 positives per position takes [B, L, P] weights, one per (position, positive) pair."""
+        if getattr(self, "n_pos", 1) > 1:
+            n = self.cur_B * self.L
+            if weights.numel() != n * self.n_pos:
+                raise ValueError(f"sample weights {tuple(weights.shape)} must have the labels' shape ({self.cur_B}, {self.L}, "
+                                 f"{self.n_pos})")
+            self.mp["roww"][:n].copy_(weights.reshape(n, self.n_pos).to(torch.float32), non_blocking=True)
+            return
         n = weights.numel()
         self.in_roww[:n].copy_(weights.reshape(-1).to(torch.float32), non_blocking=True)
 
@@ -1054,15 +1119,33 @@ class SasRecEngine:
         sd.workspace, sd.workspace_bytes = sp["ws"].data_ptr(), sp["ws_bytes"]
         if sp["kind"] == self.SAMPLED_KINDS["ce_sampled_weighted"]:
             sd.row_weight = self.roww_c.data_ptr()
+        if getattr(self, "n_pos", 1) > 1:   # [B, L, P] targets staged (set_batch)
+            mp = self.mp
+            sd.labels, sd.num_positives = mp["labels_p"].data_ptr(), self.n_pos
+            sd.slot_mask, sd.n_pairs = mp["slot"].data_ptr(), mp["n_pairs"].data_ptr()
+            if sp["kind"] == self.SAMPLED_KINDS["ce_sampled_weighted"]:
+                sd.row_weight = mp["roww_c"].data_ptr()
         return sd
 
     def _prepare(self, with_targets: bool):
         cfg = self.cfg
-        check(self.lib.rp_prepare_batch(self.in_ids.data_ptr(), self.in_pad.data_ptr(),
-                                        self.in_labels.data_ptr() if with_targets else None,
-                                        self.in_tmask.data_ptr() if with_targets else None, self.T, cfg.pad_id, cfg.n_items,
-                                        self.ids32.data_ptr(), self.valid_idx.data_ptr(), self.labels_c.data_ptr(),
-                                        self.n_valid.data_ptr(), self.prep_scratch.data_ptr(), self._stream()), "rp_prepare_batch")
+        if with_targets and self.n_pos > 1:
+            # the live positions (a set slot with an id in the catalog) go through the single-label compaction and the row
+            # plan as in_labels / in_tmask; the slots of every compacted row land in labels_p / slot
+            mp = self.mp
+            check(self.lib.rp_prepare_batch_multi(
+                self.in_ids.data_ptr(), self.in_pad.data_ptr(), mp["labels"].data_ptr(), mp["tmask"].data_ptr(), self.T,
+                self.n_pos, cfg.pad_id, cfg.n_items, self.ids32.data_ptr(), self.in_labels.data_ptr(), self.in_tmask.data_ptr(),
+                self.valid_idx.data_ptr(), self.labels_c.data_ptr(), mp["labels_p"].data_ptr(), mp["slot"].data_ptr(),
+                self.n_valid.data_ptr(), mp["n_pairs"].data_ptr(), self.prep_scratch.data_ptr(), self._stream()),
+                "rp_prepare_batch_multi")
+        else:
+            check(self.lib.rp_prepare_batch(self.in_ids.data_ptr(), self.in_pad.data_ptr(),
+                                            self.in_labels.data_ptr() if with_targets else None,
+                                            self.in_tmask.data_ptr() if with_targets else None, self.T, cfg.pad_id,
+                                            cfg.n_items, self.ids32.data_ptr(), self.valid_idx.data_ptr(),
+                                            self.labels_c.data_ptr(), self.n_valid.data_ptr(), self.prep_scratch.data_ptr(),
+                                            self._stream()), "rp_prepare_batch")
         self._packed = with_targets and self.packed_eligible()
         if self._packed:
             check(self.lib.rp_row_plan(self.in_pad.data_ptr(), self.in_labels.data_ptr(), self.in_tmask.data_ptr(), self.B,
@@ -1268,7 +1351,10 @@ class SasRecEngine:
         self._final_norm_fwd(self.x[-1], self.hc, T, gather=self._target_rows(), n_rows_dev=self.n_valid)
         if self.sampled is not None:
             if self.sampled["kind"] == self.SAMPLED_KINDS["ce_sampled_weighted"]:   # weights in the head's compacted order
-                torch.index_select(self.in_roww, 0, self.valid_idx, out=self.roww_c)
+                if self.n_pos > 1:
+                    torch.index_select(self.mp["roww"], 0, self.valid_idx, out=self.mp["roww_c"])
+                else:
+                    torch.index_select(self.in_roww, 0, self.valid_idx, out=self.roww_c)
             check(self.lib.rp_sampled_head_fwd(ctypes.byref(self._sampled_desc()), self._stream()), "rp_sampled_head_fwd")
             return self.ce.loss
         return self._catalog_head_fwd(self.params16["item_emb"][: cfg.n_items])
@@ -1291,8 +1377,15 @@ class SasRecEngine:
         self.lib.count += 2
         d_hc = self.s["dhc"] if self.fused_ce else None
         if self.bce:
-            return bce_head_fwd(self.ce, self.hc, table, self.labels_c, self.n_valid, bias=bias, d_hc=d_hc,
+            loss = bce_head_fwd(self.ce, self.hc, table, self.labels_c, self.n_valid, bias=bias, d_hc=d_hc,
                                 n_valid_hint=self.n_valid_hint)
+            if self.n_pos > 1:   # the rest of each row's positive set
+                mp = self.mp
+                check(self.lib.rp_bce_head_multi_fwd(self.hc.data_ptr(), table.data_ptr(), self.labels_c.data_ptr(),
+                                                     mp["labels_p"].data_ptr(), self.n_valid.data_ptr(), self.T, self.n_pos,
+                                                     self.cfg.n_items, self.cfg.dp, loss.data_ptr(), mp["row_sum"].data_ptr(),
+                                                     self._stream()), "rp_bce_head_multi_fwd")
+            return loss
         row = self.ce_row
         roww = None
         if row is not None and row["weighted"]:   # weights of the valid targets in the head's compacted order
@@ -1310,6 +1403,12 @@ class SasRecEngine:
         head_bwd = bce_head_bwd if self.bce else ce_head_bwd
         head_bwd(self.ce, self.hc, table, self.labels_c, self.n_valid, self.s["dhc"], d_table, bias=bias, d_bias=d_bias,
                  n_valid_hint=self.n_valid_hint if n_valid_hint is None else n_valid_hint)
+        if self.bce and self.n_pos > 1:
+            mp = self.mp
+            check(self.lib.rp_bce_head_multi_bwd(self.hc.data_ptr(), table.data_ptr(), self.labels_c.data_ptr(),
+                                                 mp["labels_p"].data_ptr(), self.n_valid.data_ptr(), self.T, self.n_pos,
+                                                 self.cfg.n_items, self.cfg.dp, self.ce.loss.data_ptr(), self.s["dhc"].data_ptr(),
+                                                 d_table.data_ptr(), self._stream()), "rp_bce_head_multi_bwd")
         self.lib.count += 3
 
     # ------------------------------------------------------------------------------------------------ backward

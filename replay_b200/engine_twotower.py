@@ -50,6 +50,7 @@ class TwoTowerConfig(EncoderConfig):
 
 
 class TwoTowerEngine(SwiGLUOps, SasRecEngine):
+    MULTI_POSITIVE_KINDS = ()   # the candidate compaction (rp_tower_compact) takes one label per position
     _KINDS = ("ce", "ce_weighted", "login_ce", "bce", "ce_sampled", "bce_sampled", "login_ce_sampled", "ce_sampled_weighted")
 
     def __init__(self, cfg: TwoTowerConfig, *args, **kwargs):

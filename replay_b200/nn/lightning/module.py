@@ -130,8 +130,12 @@ class LightningModule(LightningModuleBase):
         if self.fused_optimizer and hasattr(self.model, "core"):
             core = self.model.core
             lab, tm = batch["positive_labels"], batch["target_padding_mask"]
-            lab = lab[..., 0] if lab.dim() == 3 else lab
-            tm = tm[..., 0] if tm.dim() == 3 else tm
+            if hasattr(self.model, "check_positives"):   # [B, L, P] targets reach the heads that train on them
+                lab, tm = self.model.check_positives(lab, tm)
+            elif lab.dim() == 3:
+                if lab.size(-1) != 1:
+                    raise NotImplementedError(f"The case of multi-positive labels is not supported in {type(self.model).__name__}")
+                lab, tm = lab[..., 0], (tm[..., 0] if tm.dim() == 3 else tm)
             spec = getattr(self.model, "loss", None)
             neg = batch.get("negative_labels") if getattr(spec, "needs_negatives", False) else None
             if getattr(spec, "needs_negatives", False) and neg is None:

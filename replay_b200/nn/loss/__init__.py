@@ -1,13 +1,16 @@
 """Loss selectors with the reference's names and constructor arguments (replay/nn/loss/{ce,bce,login_ce,logout_ce}.py):
 every name of the reference's ``replay.nn.loss``.  They carry no computation: assigning one to ``SasRec.loss`` selects the
 fused CUDA head that implements it (full-catalog CE and its per-row variants: rp_ce_head_*; full-catalog BCE:
-rp_bce_head_*; sampled heads - CESampled, CESampledWeighted, BCESampled, LogInCESampled: rp_sampled_head_*).  Single
-positive label per position (multi-positive: NotImplementedError, as in the reference's CE)."""
+rp_bce_head_*; sampled heads - CESampled, CESampledWeighted, BCESampled, LogInCESampled: rp_sampled_head_*).  BCE,
+CESampled, BCESampled and CESampledWeighted also take several positives per position ([B, L, P] labels, P <= 32); every other
+loss raises NotImplementedError for them (``check_multi_positive``)."""
 from __future__ import annotations
 
 from typing import Callable, Optional, Protocol
 
 import torch
+
+from ..._lib import MAX_POSITIVES
 
 
 class LossProto(Protocol):
@@ -101,12 +104,15 @@ LogOutCESampled = CE   # replay/nn/loss/__init__.py:6
 
 
 class _Weighted:
-    """Sample weights ride in ``feature_tensors[feature_name]`` ([B, L, 1] or [B, L])."""
+    """Sample weights ride in ``feature_tensors[feature_name]`` ([B, L, 1] or [B, L]; [B, L, P] with P positives per
+    position, one weight per (position, positive) pair)."""
     kind = "ce_weighted"
     feature_name: str
 
     def row_weights(self, feature_tensors, target_mask):
         w = feature_tensors[self.feature_name]
+        if target_mask.dim() == 3 and target_mask.shape[-1] > 1:
+            return w
         return w[..., 0] if w.dim() == 3 else w
 
 
@@ -172,6 +178,20 @@ class LogInCESampled(_LossSpec):
 
     def engine_kwargs(self):
         return {"ignore_index": self.negative_labels_ignore_index, "log_eps": self.log_epsilon, "clamp": self.clamp_border}
+
+
+def check_multi_positive(loss, num_positives: int) -> None:
+    """Raise unless ``loss`` trains on ``num_positives`` positives per position: NotImplementedError for the losses that
+    take one (CE and CEWeighted with the reference's message, replay/nn/loss/ce.py:67-69; LogInCE, LogInCESampled, LogOutCE
+    and LogOutCEWeighted couple a row's positives into one term and have no fused multi-positive head), ValueError above
+    MAX_POSITIVES (32) positives."""
+    if num_positives <= 1:
+        return
+    if not isinstance(loss, (BCE, CESampled, BCESampled)):
+        name = "CE" if type(loss) in (CE, CEWeighted) else type(loss).__name__
+        raise NotImplementedError(f"The case of multi-positive labels is not supported in the {name} loss")
+    if num_positives > MAX_POSITIVES:
+        raise ValueError(f"at most {MAX_POSITIVES} positives per position are supported, got {num_positives}")
 
 
 __all__ = ["BCE", "CE", "BCESampled", "CESampled", "CESampledWeighted", "CEWeighted", "LogInCE", "LogInCESampled", "LogOutCE",

@@ -11,7 +11,7 @@ import warnings
 import torch
 
 from ...core import SasRecCore
-from ..loss import CE
+from ..loss import CE, check_multi_positive
 from ...engine import EncoderConfig
 from ...engine_diff import DiffConfig, DiffEngine
 from ...schema import item_feature_of, side_features_of
@@ -270,13 +270,25 @@ class SasRec(torch.nn.Module):
         self.core.engine._gemm(h, tab, out, h.shape[0], tab.shape[0], self.core.cfg.dp, out_mode=2)
         return out.view(*model_embeddings.shape[:-1], tab.shape[0])
 
-    def forward_train(self, feature_tensors, padding_mask, positive_labels, negative_labels=None, target_padding_mask=None):
+    multi_positive = True   # the heads take [B, L, P] targets (TwoTower's tower compaction takes one label per position)
+
+    def check_positives(self, positive_labels, target_padding_mask):
+        """(labels, mask) of a training batch for the core: [B, L], or [B, L, P] when P > 1 positives per position reach
+        a loss that trains on them (NotImplementedError / ValueError otherwise, see ``check_multi_positive``)."""
+        n_pos = positive_labels.size(-1) if positive_labels.dim() == 3 else 1
+        if n_pos > 1:
+            if not self.multi_positive:
+                raise NotImplementedError(f"The case of multi-positive labels is not supported in {type(self).__name__}")
+            check_multi_positive(self._loss, n_pos)
+            return positive_labels, target_padding_mask
         if positive_labels.dim() == 3:
-            if positive_labels.size(-1) != 1:
-                raise NotImplementedError("The case of multi-positive labels is not supported in the CE loss")
             positive_labels = positive_labels[..., 0]
         if target_padding_mask is not None and target_padding_mask.dim() == 3:
             target_padding_mask = target_padding_mask[..., 0]
+        return positive_labels, target_padding_mask
+
+    def forward_train(self, feature_tensors, padding_mask, positive_labels, negative_labels=None, target_padding_mask=None):
+        positive_labels, target_padding_mask = self.check_positives(positive_labels, target_padding_mask)
         ids = feature_tensors[self.core.item_feature]
         if self._loss.needs_negatives and negative_labels is None:
             raise ValueError(f"{type(self._loss).__name__} needs negative_labels")

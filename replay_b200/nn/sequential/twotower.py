@@ -304,6 +304,8 @@ class TwoTower(SasRec):
     by a dot product.  The losses of ``replay_b200.nn.loss`` select the fused heads (full-catalog and sampled); the sampled
     losses run the item tower on the step's distinct candidates only."""
 
+    multi_positive = False   # the sampled losses' candidate compaction takes one label per position
+
     def __init__(self, body, loss=None, context_merger=None, device=None, seed: int = 0):
         if context_merger is not None:
             raise ValueError("context_merger is not supported (only None)")
