@@ -666,6 +666,9 @@ int rp_build_batch(const int64_t* offsets, const int32_t* items, long long n_seq
  * bit2: A given as At[K,M].  D = A . B^T in every mode.
  * ------------------------------------------------------------------------------------------------------------- */
 int rp_selftest_mma(int mode, const void* A, const void* B, float* D, void* stream);
+/* exp2 helpers of the CE head's exponential loops: y_poly[i] = ex2_poly(x[i]) (polynomial on the FMA pipe), y_mufu[i] =
+ * ex2.approx.ftz(x[i]) (special-function unit), for i < n.  fp32 device arrays. */
+int rp_selftest_exp2(const float* x, float* y_poly, float* y_mufu, long long n, void* stream);
 /* TMA feed-rate probe (tools/probe_tma.py): every CTA streams `tiles` [box_rows x d] row tiles of a K-major bf16 table through
  * an 8-stage ring with no consumer. */
 /* wgmma issue-rate probe (tools/probe_mma.py): mode bit0 B MN-major, bit1 A from registers, bit2 A MN-major, bits 3-4 N = 128 /

@@ -49,6 +49,7 @@ def lib():
     P = c_void_p
     _sig(L.rp_version, c_char_p, [])
     _sig(L.rp_selftest_mma, c_int, [c_int, P, P, P, P])
+    _sig(L.rp_selftest_exp2, c_int, [P, P, P, ctypes.c_longlong, P])
     _sig(L.rp_seen_prepare, c_int, [P, c_int, c_int, c_int, P, P, P])
     _sig(L.rp_score_topk_workspace, c_size_t, [c_int, c_int, c_int, c_int])
     _sig(L.rp_score_topk, c_int, [P, P, P, P, c_int, c_int, c_int, c_int, c_int, P, P, P, P, c_size_t, P])

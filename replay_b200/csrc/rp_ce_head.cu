@@ -359,6 +359,14 @@ __global__ void __launch_bounds__(1024) ce_loss_reduce_kernel(const float* __res
 //         d_hc = (dH~ - E[y]) / T_v and the row losses are final (direct.d_hc / direct.row_loss); else partials, zpart
 // MODE 4: rows = items (COLCONST), columns = the valid tokens: dE = G . Hc / T_v, d_bias = row sums of G / T_v, the bias of
 //         the item row inside the sigmoid
+// Eighths of the CE passes' exponentials (MODE 1 and MODE 2) that ex2_poly computes on the FMA pipe instead of MUFU.EX2:
+// the fragment columns 8 q + {0, 1} with q % 8 < k, the same columns in every tile.  Per logit the S and dH / dE MMAs cost
+// 4 d FLOP and the exponential one MUFU op, so the special-function unit's share grows as d shrinks; the polynomial costs
+// ten FMA / integer instructions instead.  Measured on an H100 SXM 80GB at 700 W for k = 1..4 at d = 64, 128 and 256, with and
+// without bias (README, "Headroom left"): every k > 0 slowed both passes at d = 128 (config 2, k = 1: fused pass +13 %, dE
+// pass +5 %); at d = 64 and 256 only the biased dE pass gained (about 3 % at k = 1) while the unbiased one lost.  So every
+// instantiation keeps MUFU.EX2, and k = 0 compiles to the same code as the loop without the split.
+__host__ __device__ constexpr int ce_poly_eighths(int /*kch*/, int /*tn*/, int /*mode*/) { return 0; }
 template <int KCH, int NSTAGE, int TN, int MODE, bool HAS_BIAS>
 __global__ void __launch_bounds__(kThreads, 1)
 ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -380,6 +388,7 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   // accumulator stage that reuses it; they are in shared memory once the tile is, so the exponentials never wait on a load
   constexpr bool OFF_RING = COLCONST && !BCE;
   constexpr int kOffBytes = TN * 4;
+  constexpr int kPolyEighths = ce_poly_eighths(KCH, TN, MODE);
   if (safe_flag && (*safe_flag != 0) != (run_if_safe != 0)) return;  // fused path vs two-pass fallback (uniform)
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -525,39 +534,67 @@ ce_bwd_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       }
     } else {
       const float* off = sOff + s * TN + fc;   // COLCONST: offsets of this thread's columns, -inf beyond the valid tokens
+      // Token rows: only a split's last column tile reaches past c_end, so every other tile runs without the per-column
+      // compare and select (about one instruction per logit, on the path the other warpgroup's MMAs wait for)
+      auto exps = [&](auto masked) {
+        constexpr bool MASKED = decltype(masked)::value;
 #pragma unroll
-      for (int q = 0; q < TN / 8; ++q) {
-        float g[4];
-        float2 cq;
-        if (COLCONST) cq = *reinterpret_cast<const float2*>(off + 8 * q);
+        for (int q = 0; q < TN / 8; ++q) {
+          float g[4];
+          float2 cq;
+          // ld.shared: the aligned smem base goes through an integer, which hides the state space from the compiler and
+          // made these generic loads (LD.E, about 0.2 ms of the dE pass at config 2).  volatile keeps it behind the tile's
+          // mbarrier wait, which is what makes the offsets valid.
+          if (COLCONST) asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(cq.x), "=f"(cq.y) : "r"(smem_u32(off + 8 * q)));
+          // the same fragment columns of every tile take the polynomial, so a logit's value never depends on scheduling
+          const bool poly = q % 8 < kPolyEighths;
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int col = col0 + 8 * q + e;
-          float va = sacc[4 * q + e], vb = sacc[4 * q + 2 + e];
-          if (COLCONST) {
-            const float cc = e ? cq.y : cq.x;
-            g[e] = ex2f(fmaf(va, kLog2e, cc));
-            g[2 + e] = ex2f(fmaf(vb, kLog2e, cc));
-          } else {
-            const bool in = col < c_end;
-            if (HAS_BIAS && in) {
-              const float bb = __ldg(bias + col);
-              va += bb;
-              vb += bb;
+          for (int e = 0; e < 2; ++e) {
+            const int col = col0 + 8 * q + e;
+            float va = sacc[4 * q + e], vb = sacc[4 * q + 2 + e];
+            if (COLCONST) {
+              const float cc = e ? cq.y : cq.x;
+              g[e] = poly ? ex2_poly(fmaf(va, kLog2e, cc)) : ex2f(fmaf(va, kLog2e, cc));
+              g[2 + e] = poly ? ex2_poly(fmaf(vb, kLog2e, cc)) : ex2f(fmaf(vb, kLog2e, cc));
+            } else {
+              const bool in = !MASKED || col < c_end;
+              if (HAS_BIAS && in) {
+                const float bb = __ldg(bias + col);
+                va += bb;
+                vb += bb;
+              }
+              if (poly) {   // masked through the argument (2^-inf = 0): a select on the result would become a branch
+                g[e] = ex2_poly(in ? fmaf(va, kLog2e, crow_a) : -INFINITY);
+                g[2 + e] = ex2_poly(in ? fmaf(vb, kLog2e, crow_b) : -INFINITY);
+              } else {
+                g[e] = in ? ex2f(fmaf(va, kLog2e, crow_a)) : 0.f;
+                g[2 + e] = in ? ex2f(fmaf(vb, kLog2e, crow_b)) : 0.f;
+              }
             }
-            g[e] = in ? ex2f(fmaf(va, kLog2e, crow_a)) : 0.f;
-            g[2 + e] = in ? ex2f(fmaf(vb, kLog2e, crow_b)) : 0.f;
           }
+          if (FUSED || (COLCONST && HAS_BIAS)) {
+            za += g[0] + g[1];
+            zb += g[2] + g[3];
+          }
+          pk[2 * q] = pack_bf16(g[0], g[1]);
+          pk[2 * q + 1] = pack_bf16(g[2], g[3]);
         }
-        if (FUSED || (COLCONST && HAS_BIAS)) {
-          za += g[0] + g[1];
-          zb += g[2] + g[3];
-        }
-        pk[2 * q] = pack_bf16(g[0], g[1]);
-        pk[2 * q + 1] = pack_bf16(g[2], g[3]);
-      }
+      };
+      if (COLCONST || c_begin + (jl + 1) * TN > c_end) exps(std::true_type{});
+      else exps(std::false_type{});
     }
-    if (kSAhead) named_bar_sync(2 + wg, 256);   // this warpgroup's turn
+    if constexpr (kSAhead && kPolyEighths > 0) {
+      // G is complete before the turn: the barrier's thread count (256 whatever pk holds) depends on every pk word.  Without
+      // it ptxas sinks the polynomial's arithmetic below the barrier, into the window where the other warpgroup waits.
+      uint32_t all = 0;
+#pragma unroll
+      for (int i = 0; i < TN / 4; ++i) all |= pk[i];
+      uint32_t n;
+      asm volatile("{\n\t.reg .u32 t;\n\tor.b32 t, %1, 256;\n\tmin.u32 %0, t, 256;\n\t}" : "=r"(n) : "r"(all));
+      named_bar_sync(2 + wg, (int)n);
+    } else if (kSAhead) {
+      named_bar_sync(2 + wg, 256);   // this warpgroup's turn
+    }
     wg_fence();
 #pragma unroll
     for (int kk = 0; kk < TN / 16; ++kk) {

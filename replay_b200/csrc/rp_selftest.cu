@@ -1,6 +1,8 @@
 // rp_selftest.cu - single-CTA wgmma bring-up test: D[128,128] = A[128,128] * B[128,128]^T in the operand modes the
 // production kernels rely on.  Exposed through the C ABI as rp_selftest_mma so a GPU test can pin the descriptor
 // encodings (K-major / MN-major shared-memory operands, A operand from registers) against a plain matmul.
+// rp_selftest_exp2 applies the two exp2 helpers of the CE passes (ex2_poly, ex2f) to an array, so they can be tested apart
+// from the GEMMs around them.
 #include "rp_host.h"
 #include "rp_sm90.cuh"
 
@@ -70,6 +72,15 @@ mma_selftest_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       d0[0] = acc[4 * j]; d0[1] = acc[4 * j + 1];
       d8[0] = acc[4 * j + 2]; d8[1] = acc[4 * j + 3];
     }
+  }
+}
+
+__global__ void exp2_selftest_kernel(const float* __restrict__ x, float* __restrict__ y_poly, float* __restrict__ y_mufu,
+                                     long long n) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const float v = x[i];
+    y_poly[i] = ex2_poly(v);
+    y_mufu[i] = ex2f(v);
   }
 }
 
@@ -183,6 +194,17 @@ RP_API int rp_selftest_tma_probe(const void* table, long long rows, int d, int b
   const int smem = 6 * 32768 + 1024;
   RP_CUDA_CHECK(cudaFuncSetAttribute(tma_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   tma_probe_kernel<<<grid, 64, smem, stream>>>(tm, (int)(rows / box_rows), d / 64, tiles, box_rows * 128, same_tile);
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+RP_API int rp_selftest_exp2(const float* x, float* y_poly, float* y_mufu, long long n, void* stream_) {
+  using namespace rp;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!x || !y_poly || !y_mufu || n < 0) return RP_EINVAL;
+  if (n == 0) return RP_OK;
+  const long long blocks = (n + 255) / 256;
+  exp2_selftest_kernel<<<(int)(blocks < 4096 ? blocks : 4096), 256, 0, stream>>>(x, y_poly, y_mufu, n);
   RP_LAUNCH_CHECK();
   return RP_OK;
 }

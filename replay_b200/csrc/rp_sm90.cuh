@@ -165,6 +165,27 @@ __device__ __forceinline__ float ex2f(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+// 2^x on the FMA and integer pipes, for loops whose exponentials would otherwise queue on the special-function unit
+// (MUFU.EX2 runs 16 lanes per clock per SM, FFMA 128).  Agrees with ex2f wherever the CE passes evaluate it: exactly +0 for
+// -inf and every x < -126 (ex2f's flushed range), finite and normal on [-126, 127], relative error below 3e-6.
+// x = j + f with j = round(x) from the magic-number add, f in [-1/2, 1/2].  Range reduction stays off F2I / FRND (they issue
+// on the special-function unit as well).  2^f = 1 + f q(f), q a cubic relative-minimax fit; its constant term is exactly 1,
+// so p >= 1 for f >= 0 and p < 1 for f < 0.  2^j is built in the exponent bits of t and the ftz multiply flushes every
+// result below 2^-126 to zero, which is what .ftz does for ex2f.
+__device__ __forceinline__ float ex2_poly(float x) {
+  constexpr float kMagic = 12583039.f;            // 1.5 * 2^23 + 127: the low bits of t hold j + 127, the biased exponent
+  x = fmaxf(x, -127.f);                           // -inf would turn f into NaN; 2^-127 flushes to 0 below
+  const float t = __fadd_rn(x, kMagic);
+  const float f = __fsub_rn(x, __fsub_rn(t, kMagic));
+  float p = fmaf(0x1.3a02ccp-7f, f, 0x1.c9fc46p-5f);
+  p = fmaf(p, f, 0x1.ec0378p-3f);
+  p = fmaf(p, f, 0x1.62e12cp-1f);
+  p = fmaf(p, f, 1.f);
+  const float scale = __int_as_float(__float_as_int(t) << 23);   // 2^j, or 0 for j = -127
+  float y;
+  asm("mul.ftz.f32 %0, %1, %2;" : "=f"(y) : "f"(p), "f"(scale));
+  return y;
+}
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);

@@ -30,6 +30,14 @@ def selftest_mma(mode: int, a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     return d
 
 
+def selftest_exp2(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """(ex2_poly(x), ex2.approx.ftz(x)) elementwise: the two exp2 helpers of the CE head's exponential loops."""
+    _need(x, torch.float32, "x")
+    y_poly, y_mufu = torch.empty_like(x), torch.empty_like(x)
+    check(lib().rp_selftest_exp2(_ptr(x), _ptr(y_poly), _ptr(y_mufu), x.numel(), _stream()), "rp_selftest_exp2")
+    return y_poly, y_mufu
+
+
 # the longest seen list rp_seen_prepare sorts in one block's shared memory
 SEEN_PREPARE_MAX_S = 4096
 
