@@ -160,15 +160,30 @@ int rp_bce_head_multi_bwd(const void* hc, const void* table, const int32_t* labe
  * Operand X is a 2-D bf16 array [x_rows, x_cols] with pitch ldx; x_mn = 0: stored [M or N rows, K cols] (K-major),
  * x_mn = 1: stored [K rows, M or N cols].  Batch element bz = outer*inner + in addresses rows r0 + outer*ro + in*ri and
  * columns c0 + outer*co + in*ci.  C: element offset c_off0 + outer*c_oo + in*c_oi, row pitch ldc.
+ * The contraction runs over whole 64-element chunks of the STORED array: with K % 64 != 0 the tail reads the elements
+ * that follow the batch element's K range inside [x_rows, x_cols] (e.g. the next batch element's rows or columns); only
+ * elements past the stored array read as 0.  Callers that contract over a padded length (the
+ * attention backwards over L with b_off = (0, L, ...)) keep the pad columns of the other operand zero.
  * out_mode 0: bf16 store, 1: fp32 atomic add (split_k >= 1), 2: fp32 store, 3: fp32 store of the split-K partial at
  * C + ksplit * c_split_stride (deterministic two-stage split-K; reduce with rp_reduce_splits), 4: fp32 C += x as a plain
- * read-modify-write (split_k == 1, every element has one owner).
+ * read-modify-write (split_k == 1, every element has one owner).  K split s covers chunks [kc*s/S, kc*(s+1)/S) of the
+ * kc = ceil(K_eff / 64) chunks; a split with no chunk stores (out_mode 3) or adds (out_mode 1) zeros.  Every split runs
+ * the epilogue on its partial sum, so split_k > 1 takes only alpha and rowmask: bias, act, residual, gate, C2, drop_p or
+ * post_drop_p with split_k > 1 is RP_EINVAL.
  * Epilogue order: alpha, bias[N], act (0 none, 1 ReLU, 2 GELU-erf, 3 exp2 with a per-row offset, 4 sigmoid times 2^(per-row
- * offset): x = sigmoid(x) * exp2(row_exp2_offset[m]), exactly 0 where the offset is -inf), Philox dropout(drop_p; seed + *seed_ptr, drop_offset +
- * element offset in C), gate (x *= gate != 0 ? gate_scale : 0, same geometry as C), residual (bf16, same geometry as C),
- * post-residual dropout (post_drop_p, post_drop_offset), rowmask[rowmask_off0 + outer*rowmask_oo + m].
+ * offset): x = sigmoid(x) * exp2(row_exp2_offset[m]), exactly 0 where the offset is -inf; act 4 takes K-major operands
+ * only), Philox dropout (drop_p; seed + *seed_ptr, drop_offset, element (row bz*M + m, column n) of the stream of
+ * csrc/rp_philox.cuh: drop_row_key / drop_col_key / drop_mix), gate (x *= gate != 0 ? gate_scale : 0, same geometry as C),
+ * residual (bf16, same geometry as C), post-residual dropout (post_drop_p, post_drop_offset, same row and column keys),
+ * rowmask[rowmask_off0 + outer*rowmask_oo + m] (indexed by outer, not by in).
+ * row_exp2_offset is indexed by m alone, whatever the batch element.
  * C2 (optional, bf16, geometry of C) receives the value after the bias and before the activation; gate_mode 1 multiplies
- * by gelu'(gate) instead of the (gate != 0) test. */
+ * by gelu'(gate) instead of the (gate != 0) test.
+ * Left untouched: rows >= M, columns >= N, the pitch padding of every row, and all of a 128-row tile that m_limit skips
+ * (in every split's partial too).
+ * Alignment (RP_EALIGN): A, B 16-byte aligned with lda, ldb and the column offsets c0, co, ci multiples of 8; out_mode 0: C 16-byte aligned and ldc, c_off0,
+ * c_oo, c_oi multiples of 8; a residual: 16-byte aligned with ldc and the C offsets multiples of 8; C2: 4-byte aligned with
+ * ldc and the C offsets even. */
 typedef struct rp_gemm_desc {
   const void* A; long long a_rows, a_cols, lda; int a_mn;
   const void* B; long long b_rows, b_cols, ldb; int b_mn;

@@ -27,14 +27,14 @@ struct GemmParams {
   long long c_split_stride;
   float alpha;
   const float* bias;           // [N] or null
-  int act;                     // 0 none, 1 relu, 2 gelu(erf)
+  int act;                     // 0 none, 1 relu, 2 gelu(erf), 3 exp2, 4 sigmoid (row_exp2_offset below)
   const __nv_bfloat16* residual;  // same geometry as C (bf16) or null
-  const uint8_t* rowmask;      // [>= rows] multiply row m by rowmask[row_index] (row_index = c row) or null
+  const uint8_t* rowmask;      // multiply row m by (rowmask[rowmask_off0 + outer*rowmask_oo + m] != 0) or null
   long long rowmask_off0, rowmask_oo;   // row index base per batch: rowmask_off0 + outer*rowmask_oo
   float drop_p;                // dropout prob applied after act, before residual (0 = off)
   unsigned long long seed, drop_offset;
   const unsigned long long* seed_ptr;  // optional device counter added to seed (CUDA-graph replays get fresh masks)
-  int split_k;                 // number of K splits (out_mode 1 only)
+  int split_k;                 // number of K splits (out_mode 1 / 3; alpha and rowmask are the only epilogue stages allowed)
   const __nv_bfloat16* gate;   // same geometry as C: x *= (gate != 0) ? gate_scale : 0   (ReLU+dropout backward) or null
   float gate_scale;
   __nv_bfloat16* C2;           // optional second output (bf16, geometry of C): the value after bias, before the activation
@@ -83,8 +83,10 @@ __device__ __forceinline__ void gemm_epilogue_chunk(const GemmParams& p, const f
       if (p.C2) {
         __nv_bfloat16* o2 = p.C2 + c_base + n0 + c;
 #pragma unroll
-        for (int q = 0; q < 32; q += 2)
-          if (n0 + c + q < p.N) *reinterpret_cast<uint32_t*>(o2 + q) = pack_bf16(x[q], x[q + 1]);
+        for (int q = 0; q < 32; q += 2) {
+          if (n0 + c + q + 1 < p.N) *reinterpret_cast<uint32_t*>(o2 + q) = pack_bf16(x[q], x[q + 1]);
+          else if (n0 + c + q < p.N) o2[q] = __float2bfloat16(x[q]);   // odd N: the last column alone, not column N
+        }
       }
       if (p.act == 1) {
 #pragma unroll
@@ -358,12 +360,32 @@ using namespace rp;
 
 #include "rp_gemm_desc.h"
 
+// every element offset of C's geometry (ldc, c_off0, c_oo, c_oi) is a multiple of `elems`
+static bool c_geom_multiple(const rp_gemm_desc* g, long long elems) {
+  return g->ldc % elems == 0 && g->c_off0 % elems == 0 && g->c_oo % elems == 0 && g->c_oi % elems == 0;
+}
+
+static bool aligned(const void* ptr, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(ptr) & (bytes - 1)) == 0; }
+
 RP_API int rp_gemm(const rp_gemm_desc* g, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  // every argument check comes before the tensor maps are made, so it holds without a driver
   if (!g || !g->A || !g->B || !g->C) return RP_EINVAL;
   if (g->M <= 0 || g->N <= 0 || g->K <= 0 || g->batch <= 0 || g->inner <= 0) return RP_ESHAPE;
   if (g->split_k < 1 || (g->split_k > 1 && g->out_mode != 1 && g->out_mode != 3)) return RP_EINVAL;
-  if (g->out_mode == 0 && (g->ldc % 8 != 0)) return RP_EALIGN;
+  // each K split runs the epilogue on its partial sum: only the linear stages (alpha, rowmask) may be split
+  if (g->split_k > 1 && (g->bias || g->act != 0 || g->residual || g->gate || g->C2 || g->drop_p > 0.f || g->post_drop_p > 0.f))
+    return RP_EINVAL;
+  // TMA boxes start at a 16-byte aligned column of the stored operands
+  if ((g->a_c0 | g->a_co | g->a_ci | g->b_c0 | g->b_co | g->b_ci) & 7) return RP_EALIGN;
+  if ((g->act == 3 || g->act == 4) && !g->row_exp2_offset) return RP_EINVAL;
+  if (g->act == 4 && (g->a_mn || g->b_mn)) return RP_EINVAL;   // split_k > 1 with an act is rejected above
+  if (g->out_mode == 4 && g->split_k != 1) return RP_EINVAL;
+  // out_mode 0 stores 8 bf16 per 16-byte store, and the residual is read the same way at C's geometry; C2 is stored in
+  // bf16 pairs
+  if (g->out_mode == 0 && (!aligned(g->C, 16) || !c_geom_multiple(g, 8))) return RP_EALIGN;
+  if (g->residual && (!aligned(g->residual, 16) || !c_geom_multiple(g, 8))) return RP_EALIGN;
+  if (g->C2 && (!aligned(g->C2, 4) || !c_geom_multiple(g, 2))) return RP_EALIGN;
   GemmParams p;
   p.M = g->M; p.N = g->N; p.K = g->K; p.inner = g->inner;
   p.a_r0 = g->a_r0; p.a_ro = g->a_ro; p.a_ri = g->a_ri; p.a_c0 = g->a_c0; p.a_co = g->a_co; p.a_ci = g->a_ci;
@@ -380,18 +402,14 @@ RP_API int rp_gemm(const rp_gemm_desc* g, void* stream_) {
   p.row_exp2_offset = g->row_exp2_offset;
   p.m_limit_dev = g->m_limit_dev; p.m_limit_base = g->m_limit_base;
   p.k_limit_dev = g->k_limit_dev; p.k_limit_base = g->k_limit_base;
-  if ((g->act == 3 || g->act == 4) && !g->row_exp2_offset) return RP_EINVAL;
-  if (g->out_mode == 4 && g->split_k != 1) return RP_EINVAL;
   CUtensorMap tmA, tmB;
   int rc;
   // K-major operand: box [128 (or BN) rows x 64 cols]; MN-major operand: box [64 k-rows x 64 cols]
   const int bn = (g->N <= 64 && g->act != 4) ? 64 : 128;
   if ((rc = make_tmap_bf16(&tmA, g->A, g->a_rows, g->a_cols, g->lda, g->a_mn ? 64 : 128)) != RP_OK) return rc;
   if ((rc = make_tmap_bf16(&tmB, g->B, g->b_rows, g->b_cols, g->ldb, g->b_mn ? 64 : bn)) != RP_OK) return rc;
-  if (g->act == 4) {   // sigmoid epilogue: one instantiation, K-major operands and 128-column tiles (BCE logit chunks)
-    if (g->a_mn || g->b_mn || g->split_k != 1) return RP_EINVAL;
+  if (g->act == 4)   // sigmoid epilogue: one instantiation, K-major operands and 128-column tiles (BCE logit chunks)
     return launch_gemm_n<128, false, false, 4, true>(tmA, tmB, p, g->batch, stream);
-  }
 #define RP_GEMM_CASE(BN_, AMN_, BMN_) return launch_gemm<BN_, AMN_, BMN_>(tmA, tmB, p, g->batch, stream)
   if (bn == 64) {
     if (!g->a_mn && !g->b_mn) RP_GEMM_CASE(64, false, false);
