@@ -3,13 +3,14 @@ the valid tokens in column tiles of TN and reads each tile's exponent offsets (c
 128) from a shared-memory slot that the tile ring fills together with the tile, so the cases are the token counts around the
 tile and buffer edges (T_v below one tile, not a multiple of 128, up to the end of a capacity that is not one either), fewer
 and more token tiles than ring stages, offsets written by the two-pass forward (-lse, the bound failed) and by the un-fused
-forward, and bitwise repeatability."""
+forward, and bitwise repeatability.  d_table is held to the per-element bounds of tests/ce_reference.py."""
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
+import ce_reference as cr
+from ce_reference import TILE
 
-TILE = {64: (128, 8), 128: (128, 4), 256: (64, 4)}   # (TN, NSTAGE) of ce_bwd_kernel per d (dispatch_ce_bwd)
+pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
@@ -22,7 +23,7 @@ def ops():
 
 
 def _run(ops, T, n_valid, I, d, *, fused=True, scale_h=0.5, scale_e=0.3, seed=0, distinct_labels=False):
-    """forward + backward of the head; d_table [I, d] from the device and its fp64 reference on the same bf16 inputs"""
+    """forward + backward of the head; d_table [I, d] from the device and the fp64 reference on the same bf16 inputs"""
     g = torch.Generator().manual_seed(seed + 31 * T + 7 * n_valid + I + d)
     hc = (torch.randn(T, d, generator=g) * scale_h).to(torch.bfloat16)
     hc[n_valid:] = 0
@@ -31,10 +32,7 @@ def _run(ops, T, n_valid, I, d, *, fused=True, scale_h=0.5, scale_e=0.3, seed=0,
         labels = torch.randperm(I, generator=g)[:T].to(torch.int64)
     else:
         labels = torch.randint(0, I, (T,), generator=g, dtype=torch.int64)
-    h64, e64 = hc[:n_valid].double(), table.double().requires_grad_(True)
-    logits = h64 @ e64.T
-    (torch.logsumexp(logits, -1) - logits.gather(1, labels[:n_valid, None])[:, 0]).mean().backward()
-
+    ref = cr.reference(hc, table, None, labels, n_valid)
     st = ops.CEHeadState(T, I, d, "cuda")
     nv = torch.tensor([n_valid], dtype=torch.int32, device="cuda")
     hc_c, tab_c, lab_c = hc.cuda(), table.cuda(), labels.int().cuda()
@@ -44,15 +42,11 @@ def _run(ops, T, n_valid, I, d, *, fused=True, scale_h=0.5, scale_e=0.3, seed=0,
     taken = ops.ce_head_fused_taken(st) if fused else None
     ops.ce_head_bwd(st, hc_c, tab_c, lab_c, nv, d_hc, d_tab)
     torch.cuda.synchronize()
-    return d_tab.cpu(), e64.grad, taken
+    return d_tab.cpu(), ref, taken
 
 
 def _check(got, ref):
-    assert torch.isfinite(got).all()
-    # G reaches the dE GEMM in bf16: norm-relative tolerance over the table and per touched row
-    assert ((got.double() - ref).norm() / ref.norm()).item() < 1e-2
-    rows = ref.norm(dim=1) > 0.1 * ref.norm(dim=1).max()
-    assert ((got.double() - ref)[rows].norm(dim=1) / ref[rows].norm(dim=1)).max().item() < 3e-2
+    assert cr.worst(got, ref["d_W"], ref["bound_W"]) <= 1.0
 
 
 def _tokens(d, n_tiles, tail):

@@ -3,13 +3,15 @@ head at hidden 512, or at any shape that pads to 512 columns such as 300 / 4.  T
 G of a token chunk in bf16 with the bias inside the exponent / sigmoid.  d_bias is the fixed-order column sums of every
 chunk.
 
-Bounds as in tests/bce_reference.py.  G is a bf16 operand (relative 2^-8 with margin) and d_bias sums the same bf16 G.
+Bounds as in tests/bce_reference.py and tests/ce_reference.py.  G is a bf16 operand (relative 2^-8 with margin) and d_bias
+sums the same bf16 G.
 Rows past n_valid hold finite garbage, as stale rows do in the engine.  Column n_items of d_table / d_bias is a sentinel that
 must stay untouched."""
 import pytest
 import torch
 
-from bce_reference import U_G, U_OUT, reference as bce_reference, worst
+from bce_reference import reference as bce_reference, worst
+from ce_reference import reference as ce_reference
 
 pytestmark = pytest.mark.gpu
 
@@ -25,26 +27,6 @@ def ops():
     from replay_b200 import ops as _ops
 
     return _ops
-
-
-def ce_reference(h, W, b, labels, n_valid):
-    """float64 softmax CE of the valid rows: loss, d_h, d_W, d_b and their bounds (shapes of bce_reference)"""
-    h, W, y = h[:n_valid].double(), W.double(), labels[:n_valid].long()
-    x = h @ W.T + b.double()[None, :]
-    M = max(n_valid, 1)
-    p = torch.softmax(x, -1)
-    lse = torch.logsumexp(x, -1)
-    loss = (lse - x.gather(1, y[:, None])[:, 0]).sum() / M if n_valid else x.new_zeros(())
-    g = p.clone()
-    if n_valid:
-        g[torch.arange(n_valid, device=g.device), y] -= 1.0
-    g /= M
-    d_h, d_W, d_b = g @ W, g.T @ h, g.sum(0)
-    return dict(loss=loss, d_h=d_h, d_W=d_W, d_b=d_b,
-                bound_loss=1e-4 * (lse.abs().sum() + x.gather(1, y[:, None]).abs().sum()) / M + 1e-7 if n_valid else 1e-7,
-                bound_h=U_G * (p @ W.abs() + W[y].abs()) / M + U_OUT * d_h.abs() + 1e-7,
-                bound_W=U_G * (p.T @ h.abs() + torch.zeros_like(W).index_add_(0, y, h.abs())) / M + 1e-7,
-                bound_b=U_G * (p.sum(0) + torch.bincount(y, minlength=W.shape[0]).double()) / M + 1e-7)
 
 
 def _inputs(n_valid, I, seed=0):
