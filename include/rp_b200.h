@@ -301,7 +301,8 @@ int rp_row_plan(const uint8_t* pad_mask, const int64_t* labels, const uint8_t* t
                 int32_t* row_tok, int32_t* valid_rows, void* stream);
 
 /* x[t] = table[ids[t]] * scale + pos[pos0 + t % L] -> dropout -> (zero pad rows)      nn/sequential/sasrec/agg.py:37-53,
- * models/nn/sequential/sasrec/model.py:346-357 ; and its backward (fp32 atomics into d_table, pad row frozen). */
+ * models/nn/sequential/sasrec/model.py:346-357 ; and its backward (fp32 atomics into d_table, pad row frozen).
+ * pos / d_pos NULL: no positional term (TiSASRec's item input, model.py:597-604), and no positional gradient. */
 int rp_embed_fwd(const void* table, const float* pos, const int32_t* ids, const uint8_t* pad_mask, int T, int L, int d,
                  int pos0, float scale, int zero_pad_rows, float drop_p, unsigned long long seed, unsigned long long drop_off,
                  const unsigned long long* seed_ptr, void* out, void* stream);
@@ -773,6 +774,55 @@ int rp_tower_compact(const int32_t* labels, const int32_t* n_valid, int capacity
                      int64_t* negatives_out, void* rows_out, void* workspace, size_t workspace_bytes, void* stream);
 int rp_tower_scatter_rows(const void* dx, const int32_t* item_of_slot, const int32_t* n_slots, int n_rows, int d,
                           float* d_table, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * TiSASRec's time-interval attention (replay/models/nn/sequential/sasrec/model.py:532-800, csrc/rp_tisasrec.cu) without
+ * the reference's [B, L, L] interval matrix or its [B, L, L, d] embeddings.  Per head h (64-wide slot, true width
+ * head_dim), sequence b, query i, key j, with r_ij = min(floor(|t_i - t_j|), time_span) computed in the kernels from the
+ * timestamps in their own dtype (0 int64, 1 float32, 2 float64; int64 skips the floor):
+ *   S_ij = (q_i . k'_j + q_i . TKm_ij) * scale, causal keys j <= i, softmax -> A, Ad = dropout(A) (site att_off, row key
+ *   (b*H + h) * Lp + i, column j: the stream of rp_attn_softmax_bwd), o_i = sum_j Ad_ij (v'_j + TVm_ij)
+ * with k' = k + dropout(pos_k), v' = v + dropout(pos_v) (rp_ti_pos_add) and TKm_ij / TVm_ij = dropout(time_k / time_v
+ * [r_ij]), element (token b*L + i, key j, padded column c) of sites tk_off / tv_off kept iff
+ * drop_mix(drop_row_key(seed + *seed_ptr, off, (b*L + i) * L + j), drop_col_key(c)) >= p * 2^32 - one mask per step,
+ * shared by every block.  A query row with pad_mask 0 attends to nothing (A = Ad = 0, hpre = q_in): the reference gives it
+ * a uniform row and then zeroes the block's output there, so nothing downstream depends on it.
+ * Lp = round_up(L, 64).  q, q_in, hpre, d_o, dq_t: bf16 [B*L, ldq]; time_k / time_v: bf16 [time_span + 1, ld_t] (padded
+ * columns zero); d_time_k / d_time_v: fp32 of the same pitch.  L <= 256, H * 64 <= RP_TI_MAX_COLS, 1 <= time_span <=
+ * RP_TI_MAX_SPAN (the backward keeps both tables' fp32 gradients of one head in shared memory).
+ * rp_ti_attn_fwd: s = q . k'^T fp32 [B*H, Lp, Lp] (rp_gemm) -> a_save, ad bf16 [B*H, Lp, Lp] (ad may alias a_save iff
+ *   drop_p == 0; columns up to Lp written) and hpre = q_in + sum_j Ad_ij TVm_ij, the residual of o = Ad . v' (rp_gemm).
+ * rp_ti_attn_bwd: dpd = dO . v'^T bf16 [B*H, Lp, Lp] (rp_gemm) is overwritten with dS (scale included), ad with Ad (unless
+ *   it aliases a_save), dq_t = sum_j dS_ij TKm_ij (the residual of dQ = dS . k'); d_time_k / d_time_v += the gradients of
+ *   the two tables (true columns only).  Each CTA sums its pairs' table gradients in shared memory with fp32 atomics, then
+ *   the CTAs' partials (workspace rp_ti_attn_bwd_workspace bytes) are added in a fixed order: the time-table gradients are
+ *   NOT bitwise deterministic (the shared-memory sums' order varies); every other output is.
+ * rp_ti_pos_add: kv bf16 [T, ld_kv] columns [0, d) += dropout(pos_k[t % L]), [d, 2d) += dropout(pos_v[t % L]) (sites off_k /
+ *   off_v, row key t, column c of its table); rp_ti_pos_bwd: d_pos_k / d_pos_v fp32 [L, d] += sum over b in order of the
+ *   dropout' of dkv's two halves (deterministic), true columns (c % 64 < head_dim) only. */
+#define RP_TI_MAX_SPAN 320
+#define RP_TI_MAX_COLS 256
+typedef struct rp_ti_attn_desc {
+  const void* q; long long ldq;
+  const uint8_t* pad_mask;
+  const void* times; int times_dtype;
+  const void* time_k; const void* time_v; long long ld_t;
+  int B, H, L, head_dim, time_span;
+  float scale;
+  float drop_p; unsigned long long seed; const unsigned long long* seed_ptr;
+  unsigned long long att_off, tk_off, tv_off;
+} rp_ti_attn_desc;
+int rp_ti_attn_fwd(const rp_ti_attn_desc* p, const float* s, const void* q_in, void* a_save, void* ad, void* hpre,
+                   void* stream);
+size_t rp_ti_attn_bwd_workspace(int B, int H, int time_span);
+int rp_ti_attn_bwd(const rp_ti_attn_desc* p, const void* a_save, void* dpd, void* ad, const void* d_o, void* dq_t, void* ws,
+                   size_t ws_bytes, float* d_time_k, float* d_time_v, void* stream);
+int rp_ti_pos_add(void* kv, long long ld_kv, const float* pos_k, const float* pos_v, int T, int L, int d, float drop_p,
+                  unsigned long long seed, const unsigned long long* seed_ptr, unsigned long long off_k,
+                  unsigned long long off_v, void* stream);
+int rp_ti_pos_bwd(const void* dkv, long long ld_kv, int B, int L, int d, int head_dim, float drop_p, unsigned long long seed,
+                  const unsigned long long* seed_ptr, unsigned long long off_k, unsigned long long off_v, float* d_pos_k,
+                  float* d_pos_v, void* stream);
 
 #ifdef __cplusplus
 }

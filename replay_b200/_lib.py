@@ -253,8 +253,32 @@ MAX_POSITIVES = 32       # RP_MAX_POSITIVES: most positive slots per position of
 CONCAT_MAX_COLS = 1024   # RP_CONCAT_MAX_COLS: widest concatenated input of ConcatAggregator (padded to 64 columns)
 
 
+class TiAttnDesc(ctypes.Structure):
+    """Mirror of ``struct rp_ti_attn_desc`` (include/rp_b200.h): TiSASRec's time-interval attention."""
+
+    _fields_ = [
+        ("q", c_void_p), ("ldq", ctypes.c_longlong),
+        ("pad_mask", c_void_p),
+        ("times", c_void_p), ("times_dtype", c_int),
+        ("time_k", c_void_p), ("time_v", c_void_p), ("ld_t", ctypes.c_longlong),
+        ("B", c_int), ("H", c_int), ("L", c_int), ("head_dim", c_int), ("time_span", c_int),
+        ("scale", c_float),
+        ("drop_p", c_float), ("seed", ctypes.c_ulonglong), ("seed_ptr", c_void_p),
+        ("att_off", ctypes.c_ulonglong), ("tk_off", ctypes.c_ulonglong), ("tv_off", ctypes.c_ulonglong),
+    ]
+
+
+TI_MAX_SPAN = 320   # RP_TI_MAX_SPAN: largest time_span of the time-interval attention kernels
+TI_MAX_COLS = 256   # RP_TI_MAX_COLS: at most four 64-wide head slots
+
+
 _P, _LL, _U64 = c_void_p, ctypes.c_longlong, ctypes.c_ulonglong
 _EXTRA_SIGS: list = [
+    ("rp_ti_attn_fwd", c_int, [ctypes.POINTER(TiAttnDesc), _P, _P, _P, _P, _P, _P]),
+    ("rp_ti_attn_bwd_workspace", c_size_t, [c_int, c_int, c_int]),
+    ("rp_ti_attn_bwd", c_int, [ctypes.POINTER(TiAttnDesc), _P, _P, _P, _P, _P, _P, c_size_t, _P, _P, _P]),
+    ("rp_ti_pos_add", c_int, [_P, _LL, _P, _P, c_int, c_int, c_int, c_float, _U64, _P, _U64, _U64, _P]),
+    ("rp_ti_pos_bwd", c_int, [_P, _LL, c_int, c_int, c_int, c_int, c_float, _U64, _P, _U64, _U64, _P, _P, _P]),
     ("rp_diff_attn_fwd", c_int, [ctypes.POINTER(DiffAttnDesc), _P]),
     ("rp_diff_attn_softmax_bwd", c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int, c_int, c_float,
                                          ctypes.POINTER(DiffLambda), _P, _P, _P, _P, c_float, _LL, c_int, _P]),
@@ -305,4 +329,4 @@ _EXTRA_SIGS: list = [
     ("rp_bce_head_multi_bwd", c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
 ]
 
-__all__ = ["GemmDesc", "DiffAttnDesc", "DiffLambda", "SceDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "RpFeature", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]
+__all__ = ["GemmDesc", "TiAttnDesc", "DiffAttnDesc", "DiffLambda", "SceDesc", "AttnDesc", "AttnBwdDesc", "WgradPair", "RpFeature", "lib", "check", "RpError", "LIB_PATH", "c_float", "c_int", "c_int32", "c_int64", "c_size_t", "c_void_p"]

@@ -893,7 +893,7 @@ RP_API int rp_embed_fwd(const void* table, const float* pos, const int32_t* ids,
                         int d, int pos0, float scale, int zero_pad_rows, float drop_p, unsigned long long seed,
                         unsigned long long drop_off, const unsigned long long* seed_ptr, void* out, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!table || !pos || !ids || !out || T <= 0 || L <= 0) return RP_EINVAL;
+  if (!table || !ids || !out || T <= 0 || L <= 0) return RP_EINVAL;   // pos NULL: no positional term
   if (T % L != 0) return RP_ESHAPE;   // whole sequences (the kernel walks position by position)
   const int grid = grid_for(T, 8);
   RP_DISPATCH_D(d, (embed_fwd_kernel<VEC><<<grid, 256, 0, stream>>>(
@@ -908,14 +908,14 @@ RP_API int rp_embed_bwd(const void* dx, const int32_t* ids, const uint8_t* pad_m
                         unsigned long long drop_off, const unsigned long long* seed_ptr, float* d_table, float* d_pos,
                         void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!dx || !ids || !d_table || !d_pos || B <= 0 || L <= 0) return RP_EINVAL;
+  if (!dx || !ids || !d_table || B <= 0 || L <= 0) return RP_EINVAL;   // d_pos NULL: no positional gradient
   const int T = B * L;
   const int grid = grid_for(T, 8);
   RP_DISPATCH_D(d, (embed_bwd_table_kernel<VEC><<<grid, 256, 0, stream>>>(
                        reinterpret_cast<const __nv_bfloat16*>(dx), ids, pad_mask, T, pad_id, scale, zero_pad_rows, drop_p,
                        seed, drop_off, seed_ptr, nullptr, nullptr, d_table)));
   RP_LAUNCH_CHECK();
-  {
+  if (d_pos) {
     const int rlanes = 256 / (d / 4);
     int G = (B + 31) / 32;
     if (G < 1) G = 1;

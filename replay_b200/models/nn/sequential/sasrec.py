@@ -9,6 +9,7 @@ import torch
 from ....compat import LightningModuleBase
 from ....core import SasRecCore
 from ....engine import EncoderConfig
+from ....engine_tisasrec import TiConfig, TiSasRecCore
 from ..loss import check_sce_params
 from ....schema import item_feature_of
 
@@ -32,8 +33,6 @@ class SasRecModel(torch.nn.Module):
     def __init__(self, schema, num_blocks: int = 2, num_heads: int = 1, hidden_size: int = 50, max_len: int = 200,
                  dropout: float = 0.2, ti_modification: bool = False, time_span: int = 256, device=None, seed: int = 0):
         super().__init__()
-        if ti_modification:
-            raise NotImplementedError("TiSASRec is outside the hot-path scope (SURVEY.md §2)")
         name, card, pad, _ = item_feature_of(schema)
         self.schema = schema
         self.item_feature_name = name
@@ -41,9 +40,26 @@ class SasRecModel(torch.nn.Module):
         self.padding_idx = card
         self.max_len = max_len
         self.hidden_size, self.num_blocks, self.num_heads, self.dropout = hidden_size, num_blocks, num_heads, dropout
-        cfg = EncoderConfig(n_items=card, d=hidden_size, n_heads=num_heads, n_blocks=num_blocks, max_len=max_len,
-                            dropout=dropout, variant="legacy")
-        self.core = SasRecCore(cfg, item_feature=name, device=device, seed=seed)
+        self.ti_modification, self.time_span = ti_modification, time_span
+        if ti_modification:   # TiSASRec (model.py:532-800): the timestamps come with the batch's feature tensors
+            assert schema.timestamp_feature_name
+            self.timestamp_feature_name = schema.timestamp_feature_name
+            cfg = TiConfig(n_items=card, d=hidden_size, n_heads=num_heads, n_blocks=num_blocks, max_len=max_len,
+                           dropout=dropout, time_span=time_span)
+        else:
+            cfg = EncoderConfig(n_items=card, d=hidden_size, n_heads=num_heads, n_blocks=num_blocks, max_len=max_len,
+                                dropout=dropout, variant="legacy")
+        self.core = self._make_core(cfg, device, seed)
+
+    def _make_core(self, cfg, device, seed):
+        if self.ti_modification:
+            return TiSasRecCore(cfg, item_feature=self.item_feature_name, timestamp_feature=self.timestamp_feature_name,
+                                device=device, seed=seed)
+        return SasRecCore(cfg, item_feature=self.item_feature_name, device=device, seed=seed)
+
+    def feats(self, feature_tensor):
+        """What the core stages next to the item ids: the timestamps of TiSASRec, nothing otherwise."""
+        return feature_tensor if self.ti_modification else None
 
     def state_dict(self, *a, **k):
         return self.core.state_dict(*a, **k)
@@ -65,8 +81,7 @@ class SasRecModel(torch.nn.Module):
         sd["item_embedder.item_emb.weight"] = table.detach().to(torch.float32)
         new_count = table.shape[0] - 1
         spec = getattr(self.core, "_loss_spec", None)
-        self.core = SasRecCore(dataclasses.replace(self.core.cfg, n_items=new_count), item_feature=self.item_feature_name,
-                               device=self.core._device, seed=self.core._seed)
+        self.core = self._make_core(dataclasses.replace(self.core.cfg, n_items=new_count), self.core._device, self.core._seed)
         if spec is not None:
             self.core.set_loss(spec[0], **spec[1])
         self.core.load_state_dict(sd)
@@ -74,10 +89,11 @@ class SasRecModel(torch.nn.Module):
 
     def forward_step(self, feature_tensor, padding_mask):
         """Hidden states [B, L, d] (model.py:159-180)."""
-        return self.core.hidden_states(feature_tensor[self.item_feature_name], padding_mask).float()
+        return self.core.hidden_states(feature_tensor[self.item_feature_name], padding_mask, self.feats(feature_tensor)).float()
 
     def get_query_embeddings(self, feature_tensor, padding_mask):
-        return self.core.query_embeddings(feature_tensor[self.item_feature_name], padding_mask).float()
+        return self.core.query_embeddings(feature_tensor[self.item_feature_name], padding_mask,
+                                          self.feats(feature_tensor)).float()
 
     def get_logits(self, out_embeddings, item_ids=None):
         h = out_embeddings.reshape(-1, out_embeddings.shape[-1]).to(torch.bfloat16)
@@ -92,7 +108,8 @@ class SasRecModel(torch.nn.Module):
         return self.get_logits(self.forward_step(feature_tensor, padding_mask))
 
     def predict(self, feature_tensor, padding_mask, candidates_to_score=None):
-        return self.core.logits(feature_tensor[self.item_feature_name], padding_mask, candidates_to_score)
+        return self.core.logits(feature_tensor[self.item_feature_name], padding_mask, candidates_to_score,
+                                self.feats(feature_tensor))
 
 
 class SasRec(LightningModuleBase):
@@ -160,10 +177,11 @@ class SasRec(LightningModuleBase):
             raise ValueError(f"bucket_size_x = {self._sce_params.bucket_size_x} exceeds min(1024, B * L = {ids.numel()}): "
                              "the fused top-K of the SCE head selects at most 1024 rows per bucket")
         neg = (self._sample_negatives(ids) if self._loss_sample_count is not None and self._sce_params is None else None)
+        feats = self._model.feats(batch["feature_tensor"])
         if self.fused_optimizer:
-            loss = core.fused_step(*args, lr=self._fused_lr(), negatives=neg)  # all_reduce="auto": DDP exchange inside
+            loss = core.fused_step(*args, lr=self._fused_lr(), negatives=neg, feats=feats)  # all_reduce="auto": DDP inside
         else:
-            loss = core.loss(*args, negatives=neg)
+            loss = core.loss(*args, negatives=neg, feats=feats)
         self.log("train_loss", loss, on_step=True, on_epoch=True, prog_bar=True, sync_dist=True)
         return loss
 
@@ -182,7 +200,8 @@ class SasRec(LightningModuleBase):
         """Fused predict (no [B, |I|] scores): (item ids [B,k] int64, scores [B,k])."""
         batch = _prepare_prediction_batch(self._schema, self._model.max_len, batch)
         ids = batch["feature_tensor"][self._model.item_feature_name]
-        return self._model.core.predict_topk(ids, batch["padding_mask"], k, seen_ids, candidates_to_score)
+        return self._model.core.predict_topk(ids, batch["padding_mask"], k, seen_ids, candidates_to_score,
+                                             self._model.feats(batch["feature_tensor"]))
 
     def _fused_lr(self) -> float:
         """learning rate of this step: the (possibly scheduled) optimizer Lightning holds, else the factory's."""
@@ -272,6 +291,10 @@ class SasRec(LightningModuleBase):
         if sd is None:
             self._model.item_table_fp32()
             sd = self._model.state_dict()
+        if self._model.ti_modification:   # TiSasRecEmbeddings.get_all_embeddings (model.py:633-646)
+            return {"item_embedding": sd["item_embedder.item_emb.weight"][:-1].detach().clone(),
+                    **{k: sd[f"item_embedder.{k}{'.pe' if k.startswith('abs') else ''}.weight"].detach().clone()
+                       for k in ("abs_pos_k_emb", "abs_pos_v_emb", "time_matrix_k_emb", "time_matrix_v_emb")}}
         return {"item_embedding": sd["item_embedder.item_emb.weight"][:-1].detach().clone(),
                 "positional_embedding": sd["item_embedder.pos_emb.pe.weight"].detach().clone()}
 
