@@ -48,3 +48,47 @@ except Exception:  # noqa: BLE001
 
     class CallbackBase:
         pass
+
+
+class FusedOptimizerModule(LightningModuleBase):
+    """Optimizer plumbing of the engine-backed Lightning modules.  With ``fused_optimizer=True`` the CUDA engine runs Adam
+    itself under manual optimisation: each step reads its learning rate from the optimizer Lightning configured, so an lr
+    scheduler takes effect, and the schedulers are stepped here at epoch end, which Lightning leaves to the module under
+    manual optimisation (the default interval of the reference's factories, replay/nn/lightning/scheduler.py)."""
+
+    def _setup_optimizer(self, core, optimizer_factory, lr_scheduler_factory, fused_optimizer: bool):
+        self._lr_scheduler_factory = lr_scheduler_factory
+        self.fused_optimizer = fused_optimizer
+        if fused_optimizer:
+            self.automatic_optimization = False
+        self._use_optimizer_factory(optimizer_factory, core)
+
+    def _use_optimizer_factory(self, optimizer_factory, core):
+        """``_lr``, the learning rate of a step without a trainer, is the factory's (1e-3 without one); its Adam betas go to
+        ``core`` (optimizer_factory.py:56-63 / nn/lightning/optimizer.py:44-60)."""
+        self._optimizer_factory = optimizer_factory
+        self._lr = getattr(optimizer_factory, "learning_rate", 1e-3)
+        if core is not None:
+            core.adam_betas = tuple(getattr(optimizer_factory, "betas", (0.9, 0.98)))
+
+    def _current_lr(self) -> float:
+        """The learning rate Lightning's (possibly scheduled) optimizer holds right now; ``_lr`` without a trainer."""
+        try:
+            opt = self.optimizers()
+        except Exception:  # noqa: BLE001 - no trainer attached (direct use, tests)
+            opt = None
+        if isinstance(opt, (list, tuple)):
+            opt = opt[0] if opt else None
+        if opt is not None and getattr(opt, "param_groups", None):
+            return float(opt.param_groups[0]["lr"])
+        return float(self._lr)
+
+    def on_train_epoch_end(self):
+        if self.fused_optimizer and self._lr_scheduler_factory is not None:
+            try:
+                sch = self.lr_schedulers()
+            except Exception:  # noqa: BLE001 - no trainer attached
+                sch = None
+            for s_ in (sch if isinstance(sch, (list, tuple)) else [sch]):
+                if s_ is not None:
+                    s_.step()

@@ -8,6 +8,7 @@
 """
 from __future__ import annotations
 
+import dataclasses
 import os
 
 import torch
@@ -92,6 +93,24 @@ class SasRecCore(torch.nn.Module):
         self.adam_betas = (0.9, 0.98)  # optimizer_factory.py:56-63 / nn/lightning/optimizer.py:44-60
         self._keymap = self._key_map()
         self._materialise()
+
+    def _init_args(self) -> dict:
+        """Constructor arguments besides the configuration, device and seed, as ``for_catalog`` passes them on."""
+        return {"item_feature": self.item_feature}
+
+    def for_catalog(self, n_items: int, state: dict) -> SasRecCore:
+        """A core of the same kind for a catalog of ``n_items`` items, holding the reference-keyed weights ``state``.  The
+        loss, the Adam betas, the device and the seed carry over; Adam's moments restart, as they do for the reference's
+        newly created parameters.  This core's captured graphs are released."""
+        self._drop_graphs()
+        core = type(self)(dataclasses.replace(self.cfg, n_items=n_items), device=self._device, seed=self._seed,
+                          **self._init_args())
+        spec = getattr(self, "_loss_spec", None)
+        if spec is not None:
+            core.set_loss(spec[0], **spec[1])
+        core.adam_betas = tuple(self.adam_betas)
+        core.load_state_dict(state)
+        return core
 
     def _key_map(self) -> dict:
         m = reference_key_map(self.cfg.variant, self.cfg.n_blocks, self.item_feature)

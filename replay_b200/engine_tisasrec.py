@@ -319,6 +319,9 @@ class TiSasRecCore(SasRecCore):
         self.timestamp_feature = timestamp_feature
         super().__init__(cfg, item_feature=item_feature, device=device, seed=seed)
 
+    def _init_args(self) -> dict:
+        return {**super()._init_args(), "timestamp_feature": self.timestamp_feature}
+
     def _key_map(self) -> dict:
         return ti_reference_key_map(self.cfg.n_blocks)
 

@@ -5,10 +5,10 @@ from __future__ import annotations
 
 import torch
 
-from ....compat import LightningModuleBase
 from ....core import SasRecCore, _EngineLoss, dist_grad_all_reduce
 from ....engine_bert import Bert4RecEngine, BertConfig
 from ....schema import bert_side_features_of, item_feature_of
+from .lightning_base import LegacyLightningModule
 
 # in the order TransformerBlock registers its parameters (bert4rec/model.py:481-500)
 _BLEAF = {"in_w": "attention.in_proj_weight", "in_b": "attention.in_proj_bias", "out_w": "attention.out_proj.weight",
@@ -90,12 +90,16 @@ class _BertCore(SasRecCore):
                     out[prefix + "_head._item_embedder." + k[len("item_embedder."):]] = v
         return out
 
-    loss_kind = "ce"   # "ce" | "bce": the full-catalog head of every engine this core creates or resizes
+    @property
+    def loss_kind(self) -> str:
+        """The full-catalog head chosen with ``set_loss``: "ce" (the default) or "bce"."""
+        return getattr(self, "_loss_spec", ("ce", {}))[0]
 
     def _apply_loss(self, eng):
-        if getattr(eng, "_loss_applied", None) != self.loss_kind:
-            eng.set_loss(self.loss_kind)
-            eng._loss_applied = self.loss_kind
+        kind = self.loss_kind
+        if getattr(eng, "_loss_applied", None) != kind:
+            eng.set_loss(kind)
+            eng._loss_applied = kind
             self._drop_graphs()   # captured graphs launch the other head's kernels
 
     # ``feats``: the batch's feature tensors by name (its "inputs"); a model with side features stages them, an item-only
@@ -259,12 +263,9 @@ class Bert4RecModel(torch.nn.Module):
         """Rebuild for the catalog of ``table`` [I', d] (I' >= I), keeping every other weight, side tables included
         (lightning.py:612-627): the
         head keeps its first I rows and bias entries and takes fresh ones for the new items - ``Linear(hidden, I')``'s
-        default initialisation untied, N(0, 0.01) bias entries tied.  The new core starts with fresh Adam moments, as the
-        reference's newly created parameters do, and without captured graphs; the loss, the Adam betas, the passes and the
-        positional setting carry over."""
-        import dataclasses
-
-        old, n_new = self.core, int(table.shape[0])
+        default initialisation untied, N(0, 0.01) bias entries tied.  The core is rebuilt for the new catalog size
+        (``SasRecCore.for_catalog``); the passes and the positional setting carry over with its configuration."""
+        n_new = int(table.shape[0])
         sd = {k: v.float().cpu() for k, v in self._weights().items()}
         n_old, d = self.item_count, self.hidden_size
         sd[f"item_embedder.cat_embeddings.{self.item_feature_name}.weight"] = table.detach().float().cpu()
@@ -277,19 +278,14 @@ class Bert4RecModel(torch.nn.Module):
             w, b = lin.weight.detach().clone(), lin.bias.detach().clone()
             w[:n_old], b[:n_old] = sd["_head.linear.weight"], sd["_head.linear.bias"]
             sd["_head.linear.weight"], sd["_head.linear.bias"] = w, b
-        old._drop_graphs()
-        core = _BertCore(dataclasses.replace(old.cfg, n_items=n_new), item_feature=self.item_feature_name, device=old._device,
-                         seed=old._seed)
-        core.loss_kind, core.adam_betas = old.loss_kind, tuple(old.adam_betas)
-        core.load_state_dict(sd)
-        self.core = core
+        self.core = self.core.for_catalog(n_new, sd)
         self.item_count = n_new
 
     def predict(self, inputs, pad_mask, token_mask, candidates_to_score=None):
         return self.core.logits(inputs[self.item_feature_name], pad_mask, token_mask, candidates_to_score, inputs)
 
 
-class Bert4Rec(LightningModuleBase):
+class Bert4Rec(LegacyLightningModule):
     def __init__(self, tensor_schema, block_count: int = 2, head_count: int = 4, hidden_size: int = 256, max_seq_len: int = 100,
                  dropout_rate: float = 0.1, pass_per_transformer_block_count: int = 1, enable_positional_embedding: bool = True,
                  enable_embedding_tying: bool = False, loss_type: str = "CE", loss_sample_count=None,
@@ -301,33 +297,19 @@ class Bert4Rec(LightningModuleBase):
         kind = {"CE": "ce", "CE_restricted": "ce", "BCE": "bce"}.get(loss_type)
         if kind is None or loss_sample_count is not None:
             raise NotImplementedError("Not supported loss_type")
-        self._model = Bert4RecModel(tensor_schema, max_len=max_seq_len, hidden_size=hidden_size, num_blocks=block_count,
-                                    num_heads=head_count, num_passes_over_block=pass_per_transformer_block_count,
-                                    dropout=dropout_rate, enable_positional_embedding=enable_positional_embedding,
-                                    enable_embedding_tying=enable_embedding_tying, device=device)
-        self._model.core.loss_kind = kind
-        self._schema = tensor_schema
-        self._vocab_size = self._model.item_count
-        self._optimizer_factory, self._lr_scheduler_factory = optimizer_factory, lr_scheduler_factory
-        self._candidates_to_score = None
-        self.fused_optimizer = fused_optimizer
-        if fused_optimizer:
-            self.automatic_optimization = False
-        self._lr = getattr(optimizer_factory, "learning_rate", 1e-3)
-        self._model.core.adam_betas = tuple(getattr(optimizer_factory, "betas", (0.9, 0.98)))
-
-    def state_dict(self, *a, prefix="", **k):
-        return {prefix + "_model." + key: v for key, v in self._model.state_dict().items()}
-
-    def load_state_dict(self, sd, strict=True, assign=False):
-        return self._model.load_state_dict({k[len("_model."):]: v for k, v in sd.items() if k.startswith("_model.")}, strict)
+        self._attach(Bert4RecModel(tensor_schema, max_len=max_seq_len, hidden_size=hidden_size, num_blocks=block_count,
+                                   num_heads=head_count, num_passes_over_block=pass_per_transformer_block_count,
+                                   dropout=dropout_rate, enable_positional_embedding=enable_positional_embedding,
+                                   enable_embedding_tying=enable_embedding_tying, device=device),
+                     tensor_schema, optimizer_factory, lr_scheduler_factory, fused_optimizer)
+        self._model.core.set_loss(kind)
 
     def training_step(self, batch: dict, batch_idx: int = 0):
         """batch keys (bert4rec/dataset.py:167-173): query_id, pad_mask, inputs, token_mask, positive_labels."""
         ids = batch["inputs"][self._model.item_feature_name]
         args = (ids, batch["pad_mask"], batch["token_mask"], batch["positive_labels"])
         core, feats = self._model.core, batch["inputs"]
-        loss = core.fused_step(*args, lr=self._fused_lr(), feats=feats) if self.fused_optimizer else core.loss(*args, feats)
+        loss = core.fused_step(*args, lr=self._current_lr(), feats=feats) if self.fused_optimizer else core.loss(*args, feats)
         self.log("train_loss", loss, on_step=True, on_epoch=True, prog_bar=True, sync_dist=True)
         return loss
 
@@ -385,33 +367,6 @@ class Bert4Rec(LightningModuleBase):
         cands = self._candidates_to_score if candidates_to_score is None else candidates_to_score
         return self._model.core.predict_topk(ids, pm, tm, k, seen_ids, cands, feats)
 
-    def _fused_lr(self) -> float:
-        try:
-            opt = self.optimizers()
-        except Exception:  # noqa: BLE001 - no trainer attached
-            opt = None
-        if isinstance(opt, (list, tuple)):
-            opt = opt[0] if opt else None
-        if opt is not None and getattr(opt, "param_groups", None):
-            return float(opt.param_groups[0]["lr"])
-        return float(self._lr)
-
-    def on_train_epoch_end(self):
-        if self.fused_optimizer and self._lr_scheduler_factory is not None:
-            try:
-                sch = self.lr_schedulers()
-            except Exception:  # noqa: BLE001
-                sch = None
-            for s_ in (sch if isinstance(sch, (list, tuple)) else [sch]):
-                if s_ is not None:
-                    s_.step()
-
-    def configure_optimizers(self):
-        params = [self._model.core.flat]
-        opt = self._optimizer_factory.create(params) if self._optimizer_factory is not None else torch.optim.Adam(
-            params, lr=1e-3, betas=(0.9, 0.98))
-        return opt if self._lr_scheduler_factory is None else ([opt], [self._lr_scheduler_factory.create(opt)])
-
     # ---- catalog growth for fine-tuning on new items (bert4rec/lightning.py:501-628)
     def get_all_embeddings(self) -> dict:
         return self._model.get_all_embeddings()
@@ -422,10 +377,7 @@ class Bert4Rec(LightningModuleBase):
 
     def _set_new_item_table(self, table: torch.Tensor):
         self._model.resize_items(table)
-        self._vocab_size = self._model.item_count
-        feats = self._schema.item_id_features
-        feat = feats.item() if hasattr(feats, "item") else feats[self._schema.item_id_feature_name]
-        feat._set_cardinality(self._vocab_size)
+        self._item_count_changed()
 
     def set_item_embeddings_by_size(self, new_vocab_size: int):
         """Keep the fitted item embeddings and add xavier-normal rows (drawn over the whole new table) for the new items."""
@@ -454,29 +406,3 @@ class Bert4Rec(LightningModuleBase):
             raise ValueError("Input tensor second dimension doesn't match embedding dim")
         new = torch.cat([self._model.item_embeddings().cpu(), item_embeddings.detach().float().cpu()])
         self._set_new_item_table(new)
-
-    @property
-    def optimizer_factory(self):
-        return self._optimizer_factory
-
-    @optimizer_factory.setter
-    def optimizer_factory(self, optimizer_factory):
-        if not hasattr(optimizer_factory, "create"):  # lightning.py:614-626 (isinstance check against OptimizerFactory)
-            raise ValueError(f"Expected optimizer_factory of type OptimizerFactory, got {type(optimizer_factory)}")
-        self._optimizer_factory = optimizer_factory
-        self._lr = getattr(optimizer_factory, "learning_rate", 1e-3)
-        self._model.core.adam_betas = tuple(getattr(optimizer_factory, "betas", (0.9, 0.98)))
-
-    @property
-    def candidates_to_score(self):
-        return self._candidates_to_score
-
-    @candidates_to_score.setter
-    def candidates_to_score(self, candidates=None):
-        total = self._model.item_count
-        if isinstance(candidates, torch.Tensor) and candidates.dtype is torch.long:
-            if not (0 < candidates.shape[0] <= total):
-                raise ValueError(f"Expected candidates length to be between 1 and total_item_count={total}")
-        elif candidates is not None:
-            raise ValueError(f"Expected candidates to be of type torch.LongTensor or None, gpt {type(candidates)}")
-        self._candidates_to_score = candidates

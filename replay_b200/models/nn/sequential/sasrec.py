@@ -6,11 +6,11 @@ from __future__ import annotations
 
 import torch
 
-from ....compat import LightningModuleBase
 from ....core import SasRecCore
 from ....engine import EncoderConfig
 from ....engine_tisasrec import TiConfig, TiSasRecCore
 from ..loss import check_sce_params
+from .lightning_base import LegacyLightningModule
 from ....schema import item_feature_of
 
 
@@ -46,16 +46,12 @@ class SasRecModel(torch.nn.Module):
             self.timestamp_feature_name = schema.timestamp_feature_name
             cfg = TiConfig(n_items=card, d=hidden_size, n_heads=num_heads, n_blocks=num_blocks, max_len=max_len,
                            dropout=dropout, time_span=time_span)
+            self.core = TiSasRecCore(cfg, item_feature=name, timestamp_feature=self.timestamp_feature_name, device=device,
+                                     seed=seed)
         else:
             cfg = EncoderConfig(n_items=card, d=hidden_size, n_heads=num_heads, n_blocks=num_blocks, max_len=max_len,
                                 dropout=dropout, variant="legacy")
-        self.core = self._make_core(cfg, device, seed)
-
-    def _make_core(self, cfg, device, seed):
-        if self.ti_modification:
-            return TiSasRecCore(cfg, item_feature=self.item_feature_name, timestamp_feature=self.timestamp_feature_name,
-                                device=device, seed=seed)
-        return SasRecCore(cfg, item_feature=self.item_feature_name, device=device, seed=seed)
+            self.core = SasRecCore(cfg, item_feature=name, device=device, seed=seed)
 
     def feats(self, feature_tensor):
         """What the core stages next to the item ids: the timestamps of TiSASRec, nothing otherwise."""
@@ -74,17 +70,12 @@ class SasRecModel(torch.nn.Module):
         return self.core.state_dict()["item_embedder.item_emb.weight"].detach().clone()
 
     def replace_item_table(self, table: torch.Tensor):
-        """Swap in a table for a (larger) vocabulary, keeping every other weight (lightning.py:612-621): the engine is rebuilt
-        for the new catalog size; optimizer moments restart, as they do for the reference's freshly created Embedding."""
-        import dataclasses
+        """Swap in a table for a (larger) vocabulary, keeping every other weight (lightning.py:612-621): the core is rebuilt
+        for the new catalog size (``SasRecCore.for_catalog``)."""
         sd = {k: v for k, v in self.state_dict().items() if not k.startswith("_head.")}
         sd["item_embedder.item_emb.weight"] = table.detach().to(torch.float32)
         new_count = table.shape[0] - 1
-        spec = getattr(self.core, "_loss_spec", None)
-        self.core = self._make_core(dataclasses.replace(self.core.cfg, n_items=new_count), self.core._device, self.core._seed)
-        if spec is not None:
-            self.core.set_loss(spec[0], **spec[1])
-        self.core.load_state_dict(sd)
+        self.core = self.core.for_catalog(new_count, sd)
         self.item_count = self.padding_idx = new_count
 
     def forward_step(self, feature_tensor, padding_mask):
@@ -112,7 +103,7 @@ class SasRecModel(torch.nn.Module):
                                 self.feats(feature_tensor))
 
 
-class SasRec(LightningModuleBase):
+class SasRec(LegacyLightningModule):
     def __init__(self, tensor_schema, block_count: int = 2, head_count: int = 1, hidden_size: int = 50,
                  max_seq_len: int = 200, dropout_rate: float = 0.2, ti_modification: bool = False, time_span: int = 256,
                  loss_type: str = "CE", loss_sample_count=None, negative_sampling_strategy: str = "global_uniform",
@@ -129,13 +120,12 @@ class SasRec(LightningModuleBase):
             raise AssertionError("negative_sampling_strategy must be 'global_uniform' or 'inbatch'")
         if loss_sample_count is not None and negative_sampling_strategy != "global_uniform":
             raise NotImplementedError("only the 'global_uniform' negative sampling strategy has a fused head")
-        self._model = SasRecModel(tensor_schema, num_blocks=block_count, num_heads=head_count, hidden_size=hidden_size,
-                                  max_len=max_seq_len, dropout=dropout_rate, ti_modification=ti_modification,
-                                  time_span=time_span, device=device)
-        self._schema = tensor_schema
+        self._attach(SasRecModel(tensor_schema, num_blocks=block_count, num_heads=head_count, hidden_size=hidden_size,
+                                 max_len=max_seq_len, dropout=dropout_rate, ti_modification=ti_modification,
+                                 time_span=time_span, device=device),
+                     tensor_schema, optimizer_factory, lr_scheduler_factory, fused_optimizer)
         self._loss_type, self._loss_sample_count = loss_type, loss_sample_count
         self._negative_sampling_strategy, self._negatives_sharing = negative_sampling_strategy, negatives_sharing
-        self._vocab_size = self._model.item_count
         self._sce_params = sce_params if loss_type == "SCE" else None
         if self._sce_params is not None:
             p = self._sce_params
@@ -146,20 +136,6 @@ class SasRec(LightningModuleBase):
                                       bucket_size_y=p.bucket_size_y, mix_x=bool(p.mix_x))
         elif loss_sample_count is not None:
             self._model.core.set_loss("legacy_ce_sampled" if loss_type == "CE" else "legacy_bce_sampled")
-        self._optimizer_factory = optimizer_factory
-        self._lr_scheduler_factory = lr_scheduler_factory
-        self._candidates_to_score = None
-        self.fused_optimizer = fused_optimizer
-        if fused_optimizer:
-            self.automatic_optimization = False
-        self._lr = getattr(optimizer_factory, "learning_rate", 1e-3)
-        self._model.core.adam_betas = tuple(getattr(optimizer_factory, "betas", (0.9, 0.98)))
-
-    def state_dict(self, *a, prefix="", **k):
-        return {prefix + "_model." + key: v for key, v in self._model.state_dict().items()}
-
-    def load_state_dict(self, sd, strict=True, assign=False):
-        return self._model.load_state_dict({k[len("_model."):]: v for k, v in sd.items() if k.startswith("_model.")}, strict)
 
     def _sample_negatives(self, ids):
         """lightning.py:394-472, 'global_uniform': one shared draw without replacement (negatives_sharing) or an independent
@@ -179,7 +155,7 @@ class SasRec(LightningModuleBase):
         neg = (self._sample_negatives(ids) if self._loss_sample_count is not None and self._sce_params is None else None)
         feats = self._model.feats(batch["feature_tensor"])
         if self.fused_optimizer:
-            loss = core.fused_step(*args, lr=self._fused_lr(), negatives=neg, feats=feats)  # all_reduce="auto": DDP inside
+            loss = core.fused_step(*args, lr=self._current_lr(), negatives=neg, feats=feats)  # all_reduce="auto": DDP inside
         else:
             loss = core.loss(*args, negatives=neg, feats=feats)
         self.log("train_loss", loss, on_step=True, on_epoch=True, prog_bar=True, sync_dist=True)
@@ -203,38 +179,6 @@ class SasRec(LightningModuleBase):
         return self._model.core.predict_topk(ids, batch["padding_mask"], k, seen_ids, candidates_to_score,
                                              self._model.feats(batch["feature_tensor"]))
 
-    def _fused_lr(self) -> float:
-        """learning rate of this step: the (possibly scheduled) optimizer Lightning holds, else the factory's."""
-        try:
-            opt = self.optimizers()
-        except Exception:  # noqa: BLE001 - no trainer attached
-            opt = None
-        if isinstance(opt, (list, tuple)):
-            opt = opt[0] if opt else None
-        if opt is not None and getattr(opt, "param_groups", None):
-            return float(opt.param_groups[0]["lr"])
-        return float(self._lr)
-
-    def on_train_epoch_end(self):
-        if self.fused_optimizer and self._lr_scheduler_factory is not None:  # manual optimisation: step the scheduler here
-            try:
-                sch = self.lr_schedulers()
-            except Exception:  # noqa: BLE001
-                sch = None
-            for s_ in (sch if isinstance(sch, (list, tuple)) else [sch]):
-                if s_ is not None:
-                    s_.step()
-
-    def configure_optimizers(self):
-        params = [self._model.core.flat]
-        if self._optimizer_factory is not None:
-            opt = self._optimizer_factory.create(params)
-        else:
-            opt = torch.optim.Adam(params, lr=1e-3, betas=(0.9, 0.98))  # optimizer_factory.py:56-63
-        if self._lr_scheduler_factory is None:
-            return opt
-        return [opt], [self._lr_scheduler_factory.create(opt)]
-
     def validation_step(self, batch: dict, batch_idx: int = 0, dataloader_idx: int = 0):
         """lightning.py:196-220: scores of the validation batch (same computation as predict)."""
         batch = _prepare_prediction_batch(self._schema, self._model.max_len, batch)
@@ -243,10 +187,7 @@ class SasRec(LightningModuleBase):
     # ---- vocabulary growth (lightning.py:493-566, 612-621)
     def _set_new_item_table(self, table: torch.Tensor):
         self._model.replace_item_table(table)
-        self._vocab_size = self._model.item_count
-        feats = self._schema.item_id_features
-        feat = feats.item() if hasattr(feats, "item") else feats[self._schema.item_id_feature_name]
-        feat._set_cardinality(self._model.item_count)
+        self._item_count_changed()
 
     def set_item_embeddings_by_size(self, new_vocab_size: int):
         """Keep the fitted item embeddings and add xavier-normal rows for the new items."""
@@ -297,29 +238,3 @@ class SasRec(LightningModuleBase):
                        for k in ("abs_pos_k_emb", "abs_pos_v_emb", "time_matrix_k_emb", "time_matrix_v_emb")}}
         return {"item_embedding": sd["item_embedder.item_emb.weight"][:-1].detach().clone(),
                 "positional_embedding": sd["item_embedder.pos_emb.pe.weight"].detach().clone()}
-
-    @property
-    def optimizer_factory(self):
-        return self._optimizer_factory
-
-    @optimizer_factory.setter
-    def optimizer_factory(self, optimizer_factory):
-        if not hasattr(optimizer_factory, "create"):  # lightning.py:575-585 (isinstance check against OptimizerFactory)
-            raise ValueError(f"Expected optimizer_factory of type OptimizerFactory, got {type(optimizer_factory)}")
-        self._optimizer_factory = optimizer_factory
-        self._lr = getattr(optimizer_factory, "learning_rate", 1e-3)
-        self._model.core.adam_betas = tuple(getattr(optimizer_factory, "betas", (0.9, 0.98)))
-
-    @property
-    def candidates_to_score(self):
-        return self._candidates_to_score
-
-    @candidates_to_score.setter
-    def candidates_to_score(self, candidates=None):
-        total = self._model.item_count  # lightning.py:594-610
-        if isinstance(candidates, torch.Tensor) and candidates.dtype is torch.long:
-            if not (0 < candidates.shape[0] <= total):
-                raise ValueError(f"Expected candidates length to be between 1 and total_item_count={total}")
-        elif candidates is not None:
-            raise ValueError(f"Expected candidates to be of type torch.LongTensor or None, gpt {type(candidates)}")
-        self._candidates_to_score = candidates

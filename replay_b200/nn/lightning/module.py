@@ -4,7 +4,7 @@ import inspect
 
 import torch
 
-from ...compat import LightningModuleBase
+from ...compat import FusedOptimizerModule
 
 
 class OptimizerFactory:
@@ -65,7 +65,7 @@ class LazyInferenceOutput(dict):
         return self._compute is None
 
 
-class LightningModule(LightningModuleBase):
+class LightningModule(FusedOptimizerModule):
     """replay/nn/lightning/module.py:13-123.  ``fused_optimizer=True`` (default) runs forward+backward+Adam inside the CUDA
     engine (manual optimisation; under ``torch.distributed`` the flat gradient is all-reduced before Adam, which is what
     Lightning's DDP does for the reference); with False the loss goes through autograd and the optimizer from
@@ -77,16 +77,10 @@ class LightningModule(LightningModuleBase):
         super().__init__()
         self.save_hyperparameters(ignore=["model"])
         self.model = model
-        self._optimizer_factory = optimizer_factory or OptimizerFactory()
-        self._lr_scheduler_factory = lr_scheduler_factory
         self._candidates_to_score = None
-        self.fused_optimizer = fused_optimizer
-        if fused_optimizer:
-            self.automatic_optimization = False
+        self._setup_optimizer(getattr(model, "core", None), optimizer_factory or OptimizerFactory(), lr_scheduler_factory,
+                              fused_optimizer)
         self._sig = set(inspect.signature(model.forward).parameters)
-        core = getattr(model, "core", None)
-        if core is not None:
-            core.adam_betas = tuple(getattr(self._optimizer_factory, "betas", (0.9, 0.98)))
 
     def forward(self, batch: dict):
         if "candidates_to_score" in self._sig and self._candidates_to_score is not None and not self.model.training:
@@ -114,18 +108,6 @@ class LightningModule(LightningModuleBase):
         missing = ["model." + k for k in getattr(res, "missing_keys", [])]
         return torch.nn.modules.module._IncompatibleKeys(missing, unexpected)
 
-    def _current_lr(self) -> float:
-        """The learning rate Lightning's (possibly scheduled) optimizer holds right now; the factory's without a Trainer."""
-        try:
-            opt = self.optimizers()
-        except Exception:  # noqa: BLE001 - no trainer attached (direct use, tests)
-            opt = None
-        if isinstance(opt, (list, tuple)):
-            opt = opt[0] if opt else None
-        if opt is not None and getattr(opt, "param_groups", None):
-            return float(opt.param_groups[0]["lr"])
-        return float(self._optimizer_factory.learning_rate)
-
     def training_step(self, batch: dict, batch_idx: int = 0):
         if self.fused_optimizer and hasattr(self.model, "core"):
             core = self.model.core
@@ -150,18 +132,6 @@ class LightningModule(LightningModuleBase):
             loss = self(batch)["loss"]
         self.log("train_loss", loss, on_step=True, on_epoch=True, prog_bar=True, sync_dist=True)
         return loss
-
-    def on_train_epoch_end(self):
-        # manual optimisation: Lightning does not step lr schedulers by itself (default interval of the reference's
-        # factories: once per epoch, replay/nn/lightning/scheduler.py)
-        if self.fused_optimizer and self._lr_scheduler_factory is not None:
-            try:
-                sch = self.lr_schedulers()
-            except Exception:  # noqa: BLE001
-                sch = None
-            for s_ in (sch if isinstance(sch, (list, tuple)) else [sch]):
-                if s_ is not None:
-                    s_.step()
 
     def _inference(self, batch: dict):
         self.model.eval()
