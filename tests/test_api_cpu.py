@@ -288,6 +288,56 @@ def test_c_abi_argument_errors_without_a_gpu():
     buf = ctypes.create_string_buffer(64)
     p = ctypes.cast(buf, ctypes.c_void_p)
     assert L.rp_ce_head_fwd(p, p, None, p, p, 128, 100, 96, p, p, p, None, 0, p, 1 << 40, None) == ESHAPE
+    # TiSASRec's time-interval kernels: the descriptor and the buffers are checked before any launch
+    from replay_b200._lib import TiAttnDesc
+    EALIGN, EWORKSPACE = -3, -5
+
+    def ti(**kw):
+        t = TiAttnDesc()
+        t.q = t.pad_mask = t.times = t.time_k = t.time_v = p.value
+        t.ldq, t.ld_t, t.B, t.H, t.L, t.head_dim, t.time_span, t.scale = 128, 128, 3, 2, 50, 64, 8, 0.125
+        for k, v in kw.items():
+            setattr(t, k, v)
+        return ctypes.byref(t)
+
+    def ws(B, H, span):   # one fp32 [2, span + 1, 64] partial per (CTA, head), min(256 / H, B) CTAs per head
+        return min(256 // H, B) * H * 2 * (span + 1) * 64 * 4
+
+    fwd = lambda d, a=p, ad=p: L.rp_ti_attn_fwd(d, p, p, a, ad, p, None)  # noqa: E731
+    n = L.rp_ti_attn_bwd_workspace(3, 2, 8)
+    bwd = lambda d, ad=p, nbytes=n: L.rp_ti_attn_bwd(d, p, p, ad, p, p, p, nbytes, p, p, None)  # noqa: E731
+    for B, H, span in ((3, 2, 8), (1, 1, 1), (300, 1, 320), (300, 4, 320), (129, 4, 256)):
+        assert L.rp_ti_attn_bwd_workspace(B, H, span) == ws(B, H, span), (B, H, span)
+    assert L.rp_ti_attn_bwd_workspace(0, 2, 8) == 0 and L.rp_ti_attn_bwd_workspace(3, 0, 8) == 0
+    assert L.rp_ti_attn_bwd_workspace(3, 2, 0) == 0 and L.rp_ti_attn_bwd_workspace(3, 2, 321) == 0
+    assert fwd(None) == EINVAL and bwd(None) == EINVAL
+    for f in ("q", "pad_mask", "times", "time_k", "time_v"):
+        assert fwd(ti(**{f: None})) == EINVAL and bwd(ti(**{f: None})) == EINVAL, f
+    assert L.rp_ti_attn_fwd(ti(), None, p, p, p, p, None) == EINVAL
+    assert fwd(ti(), a=None) == EINVAL and fwd(ti(), ad=None) == EINVAL
+    assert L.rp_ti_attn_bwd(ti(), None, p, p, p, p, p, n, p, p, None) == EINVAL
+    assert L.rp_ti_attn_bwd(ti(), p, p, p, p, p, None, n, p, p, None) == EINVAL
+    assert L.rp_ti_attn_bwd(ti(), p, p, p, p, p, p, n, None, p, None) == EINVAL
+    q2 = ctypes.cast(ctypes.create_string_buffer(64), ctypes.c_void_p)          # Ad may alias A only without dropout
+    assert L.rp_ti_attn_fwd(ti(drop_p=0.2), p, p, q2, q2, p, None) == EINVAL
+    assert L.rp_ti_attn_bwd(ti(drop_p=0.2), q2, p, q2, p, p, p, n, p, p, None) == EINVAL
+    assert fwd(ti(drop_p=1.0)) == EINVAL and fwd(ti(times_dtype=3)) == EINVAL
+    for bad in (dict(time_span=0), dict(time_span=321), dict(L=257), dict(H=5, ldq=320, ld_t=320), dict(head_dim=65),
+                dict(ldq=64)):
+        assert fwd(ti(**bad)) == ESHAPE and bwd(ti(**bad)) == ESHAPE, bad
+    assert fwd(ti(ldq=129)) == EALIGN and bwd(ti(ldq=129)) == EALIGN           # odd ldq
+    assert fwd(ti(ld_t=132)) == EALIGN
+    assert bwd(ti(), nbytes=n - 1) == EWORKSPACE                                 # one byte short
+    # positional terms: T a multiple of L, ld_kv >= 2d, head_dim a slot's width at most
+    assert L.rp_ti_pos_add(None, 256, p, p, 100, 50, 128, 0.0, 0, None, 0, 0, None) == EINVAL
+    assert L.rp_ti_pos_add(p, 256, None, p, 100, 50, 128, 0.0, 0, None, 0, 0, None) == EINVAL
+    assert L.rp_ti_pos_add(p, 256, p, p, 100, 50, 128, 1.0, 0, None, 0, 0, None) == EINVAL
+    assert L.rp_ti_pos_add(p, 256, p, p, 101, 50, 128, 0.0, 0, None, 0, 0, None) == ESHAPE      # T % L != 0
+    assert L.rp_ti_pos_add(p, 255, p, p, 100, 50, 128, 0.0, 0, None, 0, 0, None) == ESHAPE
+    assert L.rp_ti_pos_bwd(None, 256, 2, 50, 128, 64, 0.0, 0, None, 0, 0, p, p, None) == EINVAL
+    assert L.rp_ti_pos_bwd(p, 256, 2, 50, 128, 64, 0.0, 0, None, 0, 0, p, None, None) == EINVAL
+    assert L.rp_ti_pos_bwd(p, 256, 2, 50, 128, 65, 0.0, 0, None, 0, 0, p, p, None) == ESHAPE
+    assert L.rp_ti_pos_bwd(p, 256, 0, 50, 128, 64, 0.0, 0, None, 0, 0, p, p, None) == ESHAPE
 
 
 def test_device_loader_sharding_covers_every_window_once():

@@ -82,11 +82,12 @@ CASES = [  # (n_items, d, H, L, span, timestamp dtype)
     (60, 50, 1, 12, 8, torch.int64),
     (300, 64, 2, 50, 256, torch.int64),
     (200, 64, 2, 40, 64, torch.float32),
+    (150, 64, 2, 33, 32, torch.float64),
 ]
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", CASES, ids=["d50h1_span8", "d64h2_span256", "fp32_times"])
+@pytest.mark.parametrize("case", CASES, ids=["d50h1_span8", "d64h2_span256", "fp32_times", "fp64_times"])
 def test_train_step_matches_fp64_oracle(cuda, case):
     n_items, d, H, L, span, ts_dtype = case
     g = torch.Generator().manual_seed(11)
@@ -185,6 +186,31 @@ def test_lightning_training_paths_agree(cuda):
     for _ in range(20):
         last = float(m.training_step(b))
     assert last < first
+
+
+@pytest.mark.gpu
+def test_timestamp_dtype_change_rebuilds_the_captured_step(cuda):
+    """Graph-replayed steps on int64 timestamps, then the same values as float64: the captured launches carry the
+    timestamps' dtype, so the core must drop them.  The float64 step's loss equals an eager step's on the same state."""
+    from replay_b200.core import SasRecCore
+
+    b = _lbatch(cuda, 16, 32, 500, seed=12)
+    b["feature_tensor"]["timestamp"] = b["feature_tensor"]["timestamp"].floor().to(torch.int64)
+    b64 = dict(b, feature_tensor=dict(b["feature_tensor"], timestamp=b["feature_tensor"]["timestamp"].double()))
+    graph, eager = _module(cuda), _module(cuda)
+    old = SasRecCore.use_cuda_graph
+    try:
+        SasRecCore.use_cuda_graph = True
+        for _ in range(3):
+            graph.training_step(b)
+        eager.load_state_dict(graph.state_dict())
+        got = float(graph.training_step(b64))
+        SasRecCore.use_cuda_graph = False
+        want = float(eager.training_step(b64))
+    finally:
+        SasRecCore.use_cuda_graph = old
+    assert graph._model.core.engine.times_dtype == 2
+    assert abs(got - want) <= 1e-4 * abs(want), (got, want)
 
 
 @pytest.mark.gpu
