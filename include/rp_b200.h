@@ -763,7 +763,8 @@ int rp_swiglu_bwd(const void* du, const void* gl, long long n_rows, int F, void*
  * negatives_out int64 (the negatives' layout; per-position rows of invalid targets untouched) as slot ids - negatives equal to
  * ignore_index (>= 0) become `cap` (give the head ignore_index = cap), ids outside [0, n_items) become cap + 1 (the head
  * reads row 0, item 0, as it does for such ids over the whole catalog, and never matches a positive); rows_out bf16 [cap, d]
- * = table[item_of_slot[s]], zero rows from *n_slots on.  cap = min(n_items, capacity + negative entries) bounds the slots.
+ * = table[item_of_slot[s]], zero rows from *n_slots on; rows_out = null skips the rows (rp_item_feature_embed_fwd builds
+ * them with item features).  cap = min(n_items, capacity + negative entries) bounds the slots.
  * No host synchronisation (graph-capturable).  Workspace: rp_tower_compact_workspace(n_items) bytes, need not be zeroed.
  * rp_tower_scatter_rows: d_table fp32 [*, d] row item_of_slot[s] += dx bf16 [n_rows, d] row s, s < min(*n_slots, n_rows);
  * item_of_slot = null: identity over n_rows rows.  Each item has at most one slot: plain stores, deterministic. */
@@ -774,6 +775,36 @@ int rp_tower_compact(const int32_t* labels, const int32_t* n_valid, int capacity
                      int64_t* negatives_out, void* rows_out, void* workspace, size_t workspace_bytes, void* stream);
 int rp_tower_scatter_rows(const void* dx, const int32_t* item_of_slot, const int32_t* n_slots, int n_rows, int d,
                           float* d_table, void* stream);
+
+/* The item tower's input with side features (ItemTower.forward -> embedder -> SumAggregator, csrc/rp_features.cu):
+ *   out[r] = table[i] + sum_f term_f(i)   (bf16 [n_rows, d], summed in fp32, rounded once; no scale, position or dropout)
+ * i = item_of_slot[r] for r < *n_slots (zero rows from there on), or i = item0 + r when item_of_slot is null.  The features
+ * are rp_feature_embed_fwd's kinds with `values` indexed by item id (the item features reader's columns on the device).
+ * rp_item_feature_embed_bwd, from dx = d(out) bf16 [n_rows, d] (the item table's own gradient is rp_tower_scatter_rows'):
+ *   item_of_slot set: each slot's row is added into its categorical d_table rows with fp32 atomics (padding rows frozen,
+ *     mean bags by 1 / count); plan unused.
+ *   item_of_slot null (row r = item r, the whole catalog): the categorical rows are reduced in the fixed order of `plan`,
+ *     bitwise reproducible.  The plan lists, per (feature, table row) group with at least one live entry, the entries
+ *     (item, weight 1 or 1 / count) in chunks; partial fp32 [n_chunks, d] is its workspace.
+ * With numerical features v_rows bf16 [n_rows, v_ld] gets their values at val_col (other columns zero; rows from *n_slots
+ * on untouched), so that rp_wgrad_group over (dx, v_rows) gives dW and column sums of dx give db.  Over the catalog the
+ * values never change, so v_rows may be null there (staged once by the caller); with item_of_slot it is required.  No host
+ * synchronisation.  RP_EINVAL: null pointer, unknown kind; RP_ESHAPE: d, hd_valid, n_feats, widths, val_col, v_ld. */
+typedef struct rp_item_feature_plan {
+  const int32_t* ent_item;   /* [n_ent] item of each entry, grouped by (feature, table row), chunks contiguous */
+  const float* ent_w;        /* [n_ent] 1, or 1 / (live entries of the item's bag) for RP_FEAT_BAG_MEAN */
+  const int32_t* chunk_off;  /* [n_chunks + 1] entry range of each chunk; a chunk lies inside one group */
+  const int32_t* grp_chunk;  /* [n_groups + 1] chunk range of each group */
+  const int32_t* grp_feat;   /* [n_groups] index into feats (a categorical kind) */
+  const int32_t* grp_row;    /* [n_groups] table row, distinct per feature */
+  float* partial;            /* [n_chunks, d] fp32 workspace */
+  int n_chunks, n_groups;
+} rp_item_feature_plan;
+int rp_item_feature_embed_fwd(const void* item_table, const rp_feature* feats, int n_feats, const int32_t* item_of_slot,
+                              const int32_t* n_slots, int n_rows, int item0, int d, int hd_valid, void* out, void* stream);
+int rp_item_feature_embed_bwd(const void* dx, const rp_feature* feats, int n_feats, const int32_t* item_of_slot,
+                              const int32_t* n_slots, int n_rows, int d, int hd_valid, const rp_item_feature_plan* plan,
+                              void* v_rows, int v_ld, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * TiSASRec's time-interval attention (replay/models/nn/sequential/sasrec/model.py:532-800, csrc/rp_tisasrec.cu) without

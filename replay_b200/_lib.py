@@ -247,6 +247,16 @@ class RpFeature(ctypes.Structure):
     ]
 
 
+class ItemFeaturePlan(ctypes.Structure):
+    """Mirror of ``struct rp_item_feature_plan`` (include/rp_b200.h): the fixed-order reduction of the item tower's
+    categorical table gradients over the whole catalog."""
+
+    _fields_ = [
+        ("ent_item", c_void_p), ("ent_w", c_void_p), ("chunk_off", c_void_p), ("grp_chunk", c_void_p), ("grp_feat", c_void_p),
+        ("grp_row", c_void_p), ("partial", c_void_p), ("n_chunks", c_int), ("n_groups", c_int),
+    ]
+
+
 FEAT_CAT, FEAT_BAG_SUM, FEAT_BAG_MEAN, FEAT_NUM, FEAT_IDENT = range(5)   # rp_feature.kind
 FEAT_MAX, FEAT_MAX_NUM_COLS = 16, 64
 MAX_POSITIVES = 32       # RP_MAX_POSITIVES: most positive slots per position of a multi-positive batch
@@ -304,6 +314,9 @@ _EXTRA_SIGS: list = [
     ("rp_tower_compact", c_int, [_P, _P, c_int, _P, c_int, c_int, c_int, _P, c_int, c_int, c_int, _P, c_int, c_int, _P, _P, _P,
                                  _P, _P, _P, c_size_t, _P]),
     ("rp_tower_scatter_rows", c_int, [_P, _P, _P, c_int, c_int, _P, _P]),
+    ("rp_item_feature_embed_fwd", c_int, [_P, ctypes.POINTER(RpFeature), c_int, _P, _P, c_int, c_int, c_int, c_int, _P, _P]),
+    ("rp_item_feature_embed_bwd", c_int, [_P, ctypes.POINTER(RpFeature), c_int, _P, _P, c_int, c_int, c_int,
+                                          ctypes.POINTER(ItemFeaturePlan), _P, c_int, _P]),
     ("rp_feature_embed_fwd", c_int, [_P, _P, _P, ctypes.POINTER(RpFeature), c_int, c_int, c_int, c_int, c_int, c_int, c_float,
                                      c_float, _U64, _U64, _P, _P, _P]),
     ("rp_feature_embed_fwd_rows", c_int, [_P, _P, _P, ctypes.POINTER(RpFeature), c_int, _P, _P, c_int, c_int, c_int, c_int,

@@ -55,6 +55,49 @@ __device__ __forceinline__ void add_row(float* acc, const __nv_bfloat16* row, fl
   }
 }
 
+// acc[0, VEC) += sum_f term_f(t) over columns [c0, c0 + VEC) (the kinds of rp_feature_embed_fwd; BERT: CAT and IDENT)
+template <int VEC, bool BERT>
+__device__ __forceinline__ void add_features(float* acc, const FeatArgs& fa, int t, int c0, int hd_valid) {
+  constexpr int D = VEC * 32;
+  for (int k = 0; k < fa.n; ++k) {
+    const rp_feature& f = fa.f[k];
+    if (f.kind == RP_FEAT_CAT || (!BERT && (f.kind == RP_FEAT_BAG_SUM || f.kind == RP_FEAT_BAG_MEAN))) {
+      const int32_t* v = reinterpret_cast<const int32_t*>(f.values) + (size_t)t * f.width;
+      const __nv_bfloat16* tab = reinterpret_cast<const __nv_bfloat16*>(f.table);
+      float bag[VEC];
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) bag[i] = 0.f;
+      int cnt = 0;
+      for (int j = 0; j < f.width; ++j) {
+        const int id = v[j];
+        if (!feat_live(id, f)) continue;
+        add_row<VEC>(bag, tab + (size_t)id * D + c0, 1.f);
+        ++cnt;
+      }
+      const float w = (f.kind == RP_FEAT_BAG_MEAN && cnt > 0) ? 1.f / (float)cnt : 1.f;
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) acc[i] += bag[i] * w;
+    } else if (!BERT && f.kind == RP_FEAT_NUM) {
+      const float* v = reinterpret_cast<const float*>(f.values) + (size_t)t * f.width;
+      const float* W = reinterpret_cast<const float*>(f.table);
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) acc[i] += f.bias[c0 + i];
+      for (int j = 0; j < f.width; ++j) {
+        const float vj = v[j];
+#pragma unroll
+        for (int i = 0; i < VEC; ++i) acc[i] += vj * W[(size_t)(c0 + i) * f.width + j];
+      }
+    } else {  // RP_FEAT_IDENT: the values are the embedding (true features only; padded columns stay zero)
+      const float* v = reinterpret_cast<const float*>(f.values) + (size_t)t * f.width;
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) {
+        const int tc = feat_true_col(c0 + i, hd_valid);
+        if (tc >= 0) acc[i] += v[tc];
+      }
+    }
+  }
+}
+
 // row r of the output is token row_tok[r] (packed rows, *n_rows_dev of them) or token r (row_tok == null, n_tok rows)
 // BERT: tok_mask / mask_emb replace the masked tokens' sum, pos may be null, scale is not applied (only CAT and IDENT kinds)
 template <int VEC, bool BERT>
@@ -78,43 +121,7 @@ __global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) feature_embed_fwd_kern
     // BERT's <MASK> and pad tokens take mask_emb in place of the whole sum, so nothing else is gathered for them
     const bool masked = BERT && !tok_mask[t];
     add_row<VEC>(acc, masked ? mask_emb + c0 : item + (size_t)ids[t] * D + c0, 1.f);
-    for (int k = 0; k < (masked ? 0 : fa.n); ++k) {
-      const rp_feature& f = fa.f[k];
-      if (f.kind == RP_FEAT_CAT || (!BERT && (f.kind == RP_FEAT_BAG_SUM || f.kind == RP_FEAT_BAG_MEAN))) {
-        const int32_t* v = reinterpret_cast<const int32_t*>(f.values) + (size_t)t * f.width;
-        const __nv_bfloat16* tab = reinterpret_cast<const __nv_bfloat16*>(f.table);
-        float bag[VEC];
-#pragma unroll
-        for (int i = 0; i < VEC; ++i) bag[i] = 0.f;
-        int cnt = 0;
-        for (int j = 0; j < f.width; ++j) {
-          const int id = v[j];
-          if (!feat_live(id, f)) continue;
-          add_row<VEC>(bag, tab + (size_t)id * D + c0, 1.f);
-          ++cnt;
-        }
-        const float w = (f.kind == RP_FEAT_BAG_MEAN && cnt > 0) ? 1.f / (float)cnt : 1.f;
-#pragma unroll
-        for (int i = 0; i < VEC; ++i) acc[i] += bag[i] * w;
-      } else if (!BERT && f.kind == RP_FEAT_NUM) {
-        const float* v = reinterpret_cast<const float*>(f.values) + (size_t)t * f.width;
-        const float* W = reinterpret_cast<const float*>(f.table);
-#pragma unroll
-        for (int i = 0; i < VEC; ++i) acc[i] += f.bias[c0 + i];
-        for (int j = 0; j < f.width; ++j) {
-          const float vj = v[j];
-#pragma unroll
-          for (int i = 0; i < VEC; ++i) acc[i] += vj * W[(size_t)(c0 + i) * f.width + j];
-        }
-      } else {  // RP_FEAT_IDENT: the values are the embedding (true features only; padded columns stay zero)
-        const float* v = reinterpret_cast<const float*>(f.values) + (size_t)t * f.width;
-#pragma unroll
-        for (int i = 0; i < VEC; ++i) {
-          const int tc = feat_true_col(c0 + i, hd_valid);
-          if (tc >= 0) acc[i] += v[tc];
-        }
-      }
-    }
+    if (!masked) add_features<VEC, BERT>(acc, fa, t, c0, hd_valid);
     if (BERT) {
       if (pos) {
         const float* p = pos + (size_t)(t % L) * D + c0;
@@ -346,6 +353,78 @@ __global__ void __launch_bounds__(256) concat_scatter_kernel(
         for (int j = lane; j < f.width; j += 32) v_rows[(size_t)r * v_ld + f.val_col + j] = __float2bfloat16(v[j]);
       }
     }
+  }
+}
+
+
+// ---- TwoTower's item tower input (replay/nn/sequential/twotower/model.py ItemTower.forward -> embedder -> SumAggregator):
+//
+//   X0[r] = E_item[i] + sum_f term_f(reader_f[i]),   i = item_of_slot[r] (compacted candidates) or item0 + r (the catalog)
+//
+// No scale, position or dropout.  The reader's values are indexed by item id, so the feature terms are add_features' own.
+// Rows from *n_slots on are written as zeros, as rp_tower_compact leaves its rows there.
+template <int VEC>
+__global__ void __launch_bounds__(256, VEC >= 16 ? 2 : 4) item_feature_fwd_kernel(
+    const __nv_bfloat16* __restrict__ item, const __grid_constant__ FeatArgs fa, int n_rows, int item0, int hd_valid,
+    const int32_t* __restrict__ item_of_slot, const int32_t* __restrict__ n_slots, __nv_bfloat16* __restrict__ out) {
+  constexpr int D = VEC * 32;
+  const int live = item_of_slot ? min(*n_slots, n_rows) : n_rows;
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  const int c0 = lane * VEC;
+  for (int r = blockIdx.x * wpb + (threadIdx.x >> 5); r < n_rows; r += gridDim.x * wpb) {
+    float acc[VEC];
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) acc[i] = 0.f;
+    if (r < live) {
+      const int t = item_of_slot ? item_of_slot[r] : item0 + r;
+      add_row<VEC>(acc, item + (size_t)t * D + c0, 1.f);
+      add_features<VEC, false>(acc, fa, t, c0, hd_valid);
+    }
+    __nv_bfloat16* o = out + (size_t)r * D + c0;
+#pragma unroll
+    for (int i = 0; i < VEC; i += 2) *reinterpret_cast<uint32_t*>(o + i) = pack_bf16(acc[i], acc[i + 1]);
+  }
+}
+
+// Full-catalog backward of the categorical tables in a fixed order (rp_item_feature_plan): pass 1 sums each chunk's entries,
+// partial[c] = sum_e w_e * dx[item_e]; pass 2 adds each (feature, table row) group's chunk partials, in chunk order, into its
+// d_table row.  Every group has one owner, so the stores are plain and the result is the same bits on every run.
+template <int VEC>
+__global__ void __launch_bounds__(256) item_feature_chunk_kernel(const __nv_bfloat16* __restrict__ dx,
+                                                                 const rp_item_feature_plan plan) {
+  constexpr int D = VEC * 32;
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  const int c0 = lane * VEC;
+  for (int c = blockIdx.x * wpb + (threadIdx.x >> 5); c < plan.n_chunks; c += gridDim.x * wpb) {
+    float acc[VEC];
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) acc[i] = 0.f;
+    for (int e = plan.chunk_off[c]; e < plan.chunk_off[c + 1]; ++e)
+      add_row<VEC>(acc, dx + (size_t)plan.ent_item[e] * D + c0, plan.ent_w[e]);
+    float* p = plan.partial + (size_t)c * D + c0;
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) p[i] = acc[i];
+  }
+}
+
+template <int VEC>
+__global__ void __launch_bounds__(256) item_feature_group_kernel(const __grid_constant__ FeatArgs fa,
+                                                                 const rp_item_feature_plan plan) {
+  constexpr int D = VEC * 32;
+  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  const int c0 = lane * VEC;
+  for (int g = blockIdx.x * wpb + (threadIdx.x >> 5); g < plan.n_groups; g += gridDim.x * wpb) {
+    float acc[VEC];
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) acc[i] = 0.f;
+    for (int c = plan.grp_chunk[g]; c < plan.grp_chunk[g + 1]; ++c) {
+      const float* p = plan.partial + (size_t)c * D + c0;
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) acc[i] += p[i];
+    }
+    float* dst = fa.f[plan.grp_feat[g]].d_table + (size_t)plan.grp_row[g] * D + c0;
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) dst[i] += acc[i];
   }
 }
 
@@ -644,5 +723,66 @@ RP_API int rp_concat_scatter(const void* dx, const int32_t* ids, float* d_item, 
                                                           T, d, d_true, hd_valid, kp, row_tok, n_rows_dev,
                                                           reinterpret_cast<__nv_bfloat16*>(v_rows), v_ld);
   RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+// ---- TwoTower's item tower input: see item_feature_fwd_kernel above and include/rp_b200.h
+RP_API int rp_item_feature_embed_fwd(const void* item_table, const rp_feature* feats, int n_feats, const int32_t* item_of_slot,
+                                     const int32_t* n_slots, int n_rows, int item0, int d, int hd_valid, void* out,
+                                     void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!item_table || !out || n_rows <= 0 || item0 < 0 || (item_of_slot && !n_slots)) return RP_EINVAL;
+  FeatArgs fa;
+  const int rc = feat_args(feats, n_feats, d, hd_valid, false, 0, &fa);
+  if (rc != RP_OK) return rc;
+  const int grid = feat_grid(n_rows);
+  RP_FEAT_DISPATCH(d, (item_feature_fwd_kernel<VEC><<<grid, 256, 0, stream>>>(
+                          reinterpret_cast<const __nv_bfloat16*>(item_table), fa, n_rows, item0, hd_valid, item_of_slot, n_slots,
+                          reinterpret_cast<__nv_bfloat16*>(out))));
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
+RP_API int rp_item_feature_embed_bwd(const void* dx, const rp_feature* feats, int n_feats, const int32_t* item_of_slot,
+                                     const int32_t* n_slots, int n_rows, int d, int hd_valid, const rp_item_feature_plan* plan,
+                                     void* v_rows, int v_ld, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!dx || n_rows <= 0 || (item_of_slot && !n_slots) || (!item_of_slot && !plan)) return RP_EINVAL;
+  FeatArgs fa;
+  const int rc = feat_args(feats, n_feats, d, hd_valid, true, v_ld, &fa);
+  if (rc != RP_OK) return rc;
+  bool has_num = false;
+  for (int k = 0; k < n_feats; ++k) has_num |= feats[k].kind == RP_FEAT_NUM;
+  if (has_num && item_of_slot && !v_rows) return RP_EINVAL;
+  const int grid = feat_grid(n_rows);
+  if (item_of_slot) {   // at most cap rows, one slot per item: fp32 atomics into the table rows, values staged per slot
+    RP_FEAT_DISPATCH(d, (feature_embed_bwd_kernel<VEC, false><<<grid, 256, 0, stream>>>(
+                            reinterpret_cast<const __nv_bfloat16*>(dx), fa, n_rows, 1.f, 0.f, 0ull, 0ull, nullptr, item_of_slot,
+                            n_slots, nullptr, reinterpret_cast<__nv_bfloat16*>(v_rows), v_ld, nullptr, nullptr)));
+    RP_LAUNCH_CHECK();
+    return RP_OK;
+  }
+  if (plan->n_chunks < 0 || plan->n_groups < 0) return RP_ESHAPE;
+  if (plan->n_chunks > 0 && (!plan->ent_item || !plan->ent_w || !plan->chunk_off || !plan->partial)) return RP_EINVAL;
+  if (plan->n_groups > 0 && (!plan->grp_chunk || !plan->grp_feat || !plan->grp_row)) return RP_EINVAL;
+  if (has_num && v_rows) {   // the values of the numerical features only: no table row is touched here
+    FeatArgs nf;
+    nf.n = 0;
+    for (int k = 0; k < n_feats; ++k)
+      if (feats[k].kind == RP_FEAT_NUM) nf.f[nf.n++] = feats[k];
+    RP_FEAT_DISPATCH(d, (feature_embed_bwd_kernel<VEC, false><<<grid, 256, 0, stream>>>(
+                            reinterpret_cast<const __nv_bfloat16*>(dx), nf, n_rows, 1.f, 0.f, 0ull, 0ull, nullptr, nullptr,
+                            nullptr, nullptr, reinterpret_cast<__nv_bfloat16*>(v_rows), v_ld, nullptr, nullptr)));
+    RP_LAUNCH_CHECK();
+  }
+  if (plan->n_chunks > 0) {
+    RP_FEAT_DISPATCH(d, (item_feature_chunk_kernel<VEC><<<feat_grid(plan->n_chunks), 256, 0, stream>>>(
+                            reinterpret_cast<const __nv_bfloat16*>(dx), *plan)));
+    RP_LAUNCH_CHECK();
+  }
+  if (plan->n_groups > 0) {
+    RP_FEAT_DISPATCH(d, (item_feature_group_kernel<VEC><<<feat_grid(plan->n_groups), 256, 0, stream>>>(fa, *plan)));
+    RP_LAUNCH_CHECK();
+  }
   return RP_OK;
 }

@@ -149,7 +149,8 @@ __global__ void __launch_bounds__(kThreads) remap_kernel(CompactArgs a, const in
   });
 }
 
-// rows[s] = table[item_of_slot[s]] for s < n_slots, zero rows up to cap (item_of_slot = -1 there); 8 bf16 per thread
+// rows[s] = table[item_of_slot[s]] for s < n_slots, zero rows up to cap (item_of_slot = -1 there); 8 bf16 per thread.
+// rows == null: only item_of_slot = -1 from n_slots on (the caller builds the rows itself)
 __global__ void __launch_bounds__(kThreads) gather_kernel(const uint4* __restrict__ table, int d8, int cap,
                                                           int32_t* item_of_slot, const int32_t* n_slots, uint4* rows) {
   const int ns = *n_slots;
@@ -157,9 +158,9 @@ __global__ void __launch_bounds__(kThreads) gather_kernel(const uint4* __restric
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
     const int s = (int)(e / d8), c = (int)(e % d8);
     if (s < ns) {
-      rows[e] = table[(long long)item_of_slot[s] * d8 + c];
+      if (rows) rows[e] = table[(long long)item_of_slot[s] * d8 + c];
     } else {
-      rows[e] = make_uint4(0u, 0u, 0u, 0u);
+      if (rows) rows[e] = make_uint4(0u, 0u, 0u, 0u);
       if (c == 0) item_of_slot[s] = -1;
     }
   }
@@ -209,8 +210,7 @@ RP_API int rp_tower_compact(const int32_t* labels, const int32_t* n_valid, int c
                             int neg_mode, int n_neg_rows, const int32_t* valid_idx, int seq_len, int ignore_index, int n_items,
                             const void* table, int d, int cap, int32_t* n_slots, int32_t* item_of_slot, int32_t* labels_out,
                             int64_t* negatives_out, void* rows_out, void* workspace, size_t workspace_bytes, void* stream_) {
-  if (!labels || !n_valid || !negatives || !table || !n_slots || !item_of_slot || !labels_out || !negatives_out || !rows_out ||
-      !workspace)
+  if (!labels || !n_valid || !negatives || !table || !n_slots || !item_of_slot || !labels_out || !negatives_out || !workspace)
     return RP_EINVAL;
   if (neg_mode != 0 && !valid_idx) return RP_EINVAL;
   if (capacity <= 0 || n_items <= 0 || n_neg <= 0 || d <= 0 || d % 8 || cap <= 0 || cap > n_items || seq_len <= 0 ||
@@ -234,8 +234,9 @@ RP_API int rp_tower_compact(const int32_t* labels, const int32_t* n_valid, int c
   RP_LAUNCH_CHECK();
   remap_kernel<<<grid_for(entries), kThreads, 0, stream>>>(a, flag, labels_out, negatives_out);
   RP_LAUNCH_CHECK();
-  gather_kernel<<<grid_for((long long)cap * (d / 8)), kThreads, 0, stream>>>(
-      reinterpret_cast<const uint4*>(table), d / 8, cap, item_of_slot, n_slots, reinterpret_cast<uint4*>(rows_out));
+  const int d8 = rows_out ? d / 8 : 1;
+  gather_kernel<<<grid_for((long long)cap * d8), kThreads, 0, stream>>>(
+      reinterpret_cast<const uint4*>(table), d8, cap, item_of_slot, n_slots, reinterpret_cast<uint4*>(rows_out));
   RP_LAUNCH_CHECK();
   return RP_OK;
 }

@@ -2,9 +2,10 @@
 (replay_b200/engine_twotower.py).
 
 Same construction (``TwoTower(body, loss)`` and ``from_params(schema, item_features_reader, ...)``), the same ``forward`` /
-``forward_train`` / ``forward_inference`` / ``get_logits`` contracts and the same ``state_dict`` keys as the reference, for
-the item-id feature: the query tower is the new-path SASRec body, the item tower SwiGLUEncoder(d, 2d) over the item table
-both towers share."""
+``forward_train`` / ``forward_inference`` / ``get_logits`` contracts and the same ``state_dict`` keys as the reference: the
+query tower is the new-path SASRec body, the item tower SwiGLUEncoder(d, 2d) over the sum of the reader's item features,
+embedded by the tables both towers share.  The query tower reads the schema's side features from ``feature_tensors`` as
+``SasRec`` does; the item tower reads the reader's columns, held on the device."""
 from __future__ import annotations
 
 import torch
@@ -12,13 +13,13 @@ import torch
 from ...core import _LEAF, SasRecCore
 from ...engine import _BLOCK_PARAMS
 from ...engine_twotower import TOWER_LAYERS, TwoTowerConfig, TwoTowerEngine
-from ...schema import item_feature_of
+from ...schema import item_feature_of, side_features_of
 from ..agg import SumAggregator
 from ..embedding import SequenceEmbedding
 from ..ffn import SwiGLUEncoder
 from ..loss import CE
 from ..mask import DefaultAttentionMask
-from .sasrec import PositionAwareAggregator, SasRec, SasRecTransformerLayer
+from .sasrec import PositionAwareAggregator, SasRec, SasRecTransformerLayer, _check_side
 
 _TOWER_LEAF = {"wg": "WG.weight", "bg": "WG.bias", "w1": "W1.weight", "b1": "W1.bias", "w2": "W2.weight", "b2": "W2.bias"}
 
@@ -65,24 +66,38 @@ def _source_is_item_features(info) -> bool:
     return src is not None and str(getattr(src, "source", "")).upper().endswith("ITEM_FEATURES")
 
 
-def twotower_keys(n_blocks: int, item_feature: str = "item_id") -> list:
+def _embedder_keys(pre: str, item_feature: str, features=()) -> list:
+    """the keys of SequenceEmbedding's feature_embedders under ``pre``: the item table, then each side feature's
+    (nn/embedding.py: CategoricalEmbedding.emb, NumericalEmbedding.linear, IdentityEmbedding's _weight buffer)"""
+    keys = [f"{pre}embedder.feature_embedders.{item_feature}.emb.weight"]
+    for f in features:
+        e = f"{pre}embedder.feature_embedders.{f.name}."
+        keys += ([e + "emb.weight"] if f.categorical else [e + "linear.weight", e + "linear.bias"] if f.kind == "num"
+                 else [e + "_weight"])
+    return keys
+
+
+def twotower_keys(n_blocks: int, item_feature: str = "item_id", features=(), item_features=()) -> list:
     """Every parameter / buffer key of the reference's TwoTower in its ``state_dict`` order, without the item tower's
-    ``cache`` (which follows ``body.item_tower.item_reference_<item>`` while the reference holds one)."""
-    emb = f"embedder.feature_embedders.{item_feature}.emb.weight"
+    ``cache`` (which follows the last ``body.item_tower.item_reference_<f>`` while the reference holds one).  ``features``:
+    the embedder's side features (engine.SideFeature, schema order); ``item_features``: the names of those the item
+    features reader holds besides the item id."""
     enc = "body.query_tower.encoder."
-    keys = [f"body.{emb}", f"body.query_tower.{emb}", "body.query_tower.embedding_aggregator.pe.weight"]
+    keys = _embedder_keys("body.", item_feature, features) + _embedder_keys("body.query_tower.", item_feature, features)
+    keys.append("body.query_tower.embedding_aggregator.pe.weight")
     for group in (("in_w", "in_b", "out_w", "out_b"), ("ln1_w", "ln1_b"), ("w1", "b1", "w2", "b2"), ("ln2_w", "ln2_b")):
         keys += [enc + _LEAF[k].format(i=i) for i in range(n_blocks) for k in group]
-    keys += ["body.query_tower.output_normalization.weight", "body.query_tower.output_normalization.bias",
-             f"body.item_tower.item_reference_{item_feature}", f"body.item_tower.{emb}"]
+    keys += ["body.query_tower.output_normalization.weight", "body.query_tower.output_normalization.bias"]
+    keys += [f"body.item_tower.item_reference_{n}" for n in (item_feature, *item_features)]
+    keys += _embedder_keys("body.item_tower.", item_feature, features)
     for layer in (1, 2):
         keys += [f"body.item_tower.encoder.sw{layer}.{_TOWER_LEAF[k]}" for k in ("wg", "bg", "w1", "b1", "w2", "b2")]
         keys.append(f"body.item_tower.encoder.norm{layer}.weight")
     return keys
 
 
-def twotower_key_map(n_blocks: int, item_feature: str = "item_id") -> dict:
-    """engine parameter name -> reference key (the shared item table under ``body.embedder``)"""
+def twotower_key_map(n_blocks: int, item_feature: str = "item_id", features=()) -> dict:
+    """engine parameter name -> reference key (the shared tables under ``body.embedder``)"""
     m = {"item_emb": f"body.embedder.feature_embedders.{item_feature}.emb.weight",
          "pos_emb": "body.query_tower.embedding_aggregator.pe.weight",
          "lnf_w": "body.query_tower.output_normalization.weight", "lnf_b": "body.query_tower.output_normalization.bias"}
@@ -91,6 +106,12 @@ def twotower_key_map(n_blocks: int, item_feature: str = "item_id") -> dict:
     for layer, p in enumerate(TOWER_LAYERS, start=1):
         m.update({p + k: f"body.item_tower.encoder.sw{layer}.{v}" for k, v in _TOWER_LEAF.items()})
         m[p + "norm"] = f"body.item_tower.encoder.norm{layer}.weight"
+    for f in features:
+        pre = f"body.embedder.feature_embedders.{f.name}."
+        if f.categorical:
+            m[f"feat.{f.name}"] = pre + "emb.weight"
+        elif f.kind == "num":
+            m.update({f"feat.{f.name}.w": pre + "linear.weight", f"feat.{f.name}.b": pre + "linear.bias"})
     return m
 
 
@@ -99,59 +120,91 @@ class TwoTowerCore(SasRecCore):
     until the parameters change.  ``cache_live`` follows the reference's ``item_tower.cache`` (set by an eval forward over
     the whole catalog, cleared by a training forward): the ``state_dict`` carries the cache while it is live."""
 
-    def __init__(self, cfg: TwoTowerConfig, item_feature: str = "item_id", device=None, seed: int = 0):
+    def __init__(self, cfg: TwoTowerConfig, item_feature: str = "item_id", device=None, seed: int = 0, item_values=None):
         self.cache_live = False
+        # the item features reader's side columns (cfg.item_features) as it gave them: the state_dict's item_reference_<f>
+        self.item_values = {n: torch.as_tensor(item_values[n]).detach().cpu().clone() for n in cfg.item_features}
         super().__init__(cfg, item_feature=item_feature, device=device, seed=seed)
 
+    def _init_args(self) -> dict:
+        return {**super()._init_args(), "item_values": self.item_values}
+
     def _key_map(self):
-        return twotower_key_map(self.cfg.n_blocks, self.item_feature)
+        return twotower_key_map(self.cfg.n_blocks, self.item_feature, self.cfg.features)
 
     def _make_engine(self, batch, seq_len, with_grad):
-        return TwoTowerEngine(self.cfg, batch, seq_len, self._device, seed=self._seed, with_grad=with_grad)
+        return TwoTowerEngine(self.cfg, batch, seq_len, self._device, seed=self._seed, with_grad=with_grad,
+                              item_values=self.item_values)
 
-    def _item_keys(self):
-        emb = f"embedder.feature_embedders.{self.item_feature}.emb.weight"
-        return f"body.{emb}", f"body.query_tower.{emb}", f"body.item_tower.{emb}"
+    def _keys(self):
+        return twotower_keys(self.cfg.n_blocks, self.item_feature, self.cfg.features, self.cfg.item_features)
 
-    def _ref_key(self):
-        return f"body.item_tower.item_reference_{self.item_feature}"
+    def _shared_keys(self):
+        """reference key under body.embedder -> its two aliases (the query and item towers share the embedder)"""
+        main = _embedder_keys("body.", self.item_feature, self.cfg.features)
+        q = _embedder_keys("body.query_tower.", self.item_feature, self.cfg.features)
+        it = _embedder_keys("body.item_tower.", self.item_feature, self.cfg.features)
+        return {m: (a, b) for m, a, b in zip(main, q, it)}
+
+    def _ref_keys(self):
+        return {f"body.item_tower.item_reference_{n}": n for n in (self.item_feature, *self.cfg.item_features)}
 
     def _cache_key(self):
         return "body.item_tower.cache"
 
+    def _reference_buffer(self, name):
+        return torch.arange(self.cfg.n_items, dtype=torch.int64) if name == self.item_feature else self.item_values[name]
+
     def state_dict(self, *args, destination=None, prefix="", keep_vars=False):  # noqa: D102
         src = self._export() if self.engine is not None else dict(self._pending_state or {})
-        main, q, it = self._item_keys()
-        if main in src:
-            src[q] = src[it] = src[main]
-        src[self._ref_key()] = torch.arange(self.cfg.n_items, dtype=torch.int64)
+        for f in self.cfg.features:   # IdentityEmbedding's buffer (nn/embedding.py): eye(d), no parameter
+            if f.kind == "ident":
+                src[f"body.embedder.feature_embedders.{f.name}._weight"] = torch.eye(self.cfg.d)
+        for main, aliases in self._shared_keys().items():
+            if main in src:
+                for a in aliases:
+                    src[a] = src[main]
+        refs = self._ref_keys()
+        for k, n in refs.items():
+            src[k] = self._reference_buffer(n)
+        last_ref = list(refs)[-1]
         out = destination if destination is not None else {}
-        for k in twotower_keys(self.cfg.n_blocks, self.item_feature):
+        for k in self._keys():
             if k in src:
                 out[prefix + k] = src[k]
-            if k == self._ref_key() and self.cache_live and self.engine is not None:
+            if k == last_ref and self.cache_live and self.engine is not None:
                 out[prefix + self._cache_key()] = self.engine.unpad_features(self.item_table()).float().cpu()
         return out
 
     def load_state_dict(self, state_dict, strict: bool = True, assign: bool = False):  # noqa: D102
-        """The reference's keys; the shared item table is read from whichever of its three keys comes last in the
-        reference's order.  ``body.item_tower.cache`` is optional and, when present, is the tower output the next eval
-        forward uses (the reference's shape checks apply)."""
-        keys = twotower_keys(self.cfg.n_blocks, self.item_feature)
+        """The reference's keys; a shared table is read from whichever of its three keys comes last in the reference's
+        order.  The item_reference_<f> buffers must hold the reader the model was built with (the item id's: arange).
+        ``body.item_tower.cache`` is optional and, when present, is the tower output the next eval forward uses (the
+        reference's shape checks apply)."""
+        keys = self._keys()
         missing = [k for k in keys if k not in state_dict]
         if strict and missing:
             raise RuntimeError(f"missing keys in state_dict: {missing[:5]} ...")
-        ref = state_dict.get(self._ref_key())
-        if ref is not None and not torch.equal(torch.as_tensor(ref).cpu().long(), torch.arange(self.cfg.n_items)):
-            raise ValueError(f"{self._ref_key()} must equal arange({self.cfg.n_items}) (logit column i is item i)")
+        for k, n in self._ref_keys().items():
+            ref = state_dict.get(k)
+            if ref is None:
+                continue
+            mine = self._reference_buffer(n)
+            ref = torch.as_tensor(ref).cpu()
+            if ref.shape != mine.shape or not torch.equal(ref.to(mine.dtype), mine):
+                if n == self.item_feature:
+                    raise ValueError(f"{k} must equal arange({self.cfg.n_items}) (logit column i is item i)")
+                raise ValueError(f"{k} differs from the item features reader this model was built with")
         cache = state_dict.get(self._cache_key())
         if cache is not None and (cache.dim() != 2 or cache.shape[0] != self.cfg.n_items or cache.shape[1] != self.cfg.d):
             raise AssertionError(f"cache of shape {tuple(cache.shape)} does not fit [{self.cfg.n_items}, {self.cfg.d}]")
         inv = {v: k for k, v in self._keymap.items()}
-        main, q, it = self._item_keys()
-        inv[q] = inv[it] = "item_emb"
+        for main, aliases in self._shared_keys().items():
+            for a in aliases:
+                if main in inv:
+                    inv[a] = inv[main]
         ordered = {}
-        for k in keys:   # the reference's order: the last of the three item-table keys wins
+        for k in keys:   # the reference's order: the last of a shared table's three keys wins
             if k in state_dict and k in inv:
                 ordered[self._keymap[inv[k]]] = state_dict[k]
         if self.engine is None:
@@ -209,11 +262,11 @@ class TwoTowerCore(SasRecCore):
         return t if candidates is None else t[candidates].contiguous()
 
     @torch.no_grad()
-    def predict_topk(self, ids, pad_mask, k: int, seen_ids=None, candidates=None):
+    def predict_topk(self, ids, pad_mask, k: int, seen_ids=None, candidates=None, feats=None):
         # the tower runs outside any captured predict graph, which then reads its (stable) output buffer
         self._eval_engine(ids)
         self.item_table()
-        return super().predict_topk(ids, pad_mask, k, seen_ids, candidates)
+        return super().predict_topk(ids, pad_mask, k, seen_ids, candidates, feats=feats)
 
 
 class TwoTowerBody:
@@ -246,14 +299,15 @@ class TwoTowerBody:
         name, card, pad, feat_dim = item_feature_of(self.schema)
         if pad != card:
             raise ValueError("the item feature's padding_value must equal its cardinality (replay/data/nn/schema.py:89-90)")
-        side = sorted(set(_embedder_features(emb)) - {name})
-        if side:
-            raise ValueError(f"side features {side} are not supported in the query tower; exclude them from the SequenceEmbedding")
-        if set(self.query_tower_feature_names) != {name}:
-            raise ValueError(f"the query tower must use the item feature {name!r} only, got {sorted(self.query_tower_feature_names)}")
-        if list(reader.feature_names) != [name]:
-            raise ValueError(f"the item tower supports the item feature {name!r} only (side features "
-                             f"{sorted(set(reader.feature_names) - {name})} are not supported)")
+        skip = set(emb.excluded_features) | {self.schema.query_id_feature_name, self.schema.timestamp_feature_name}
+        side = side_features_of(emb.schema, skip, emb.categorical_list_feature_aggregation_method)
+        unused = sorted({name, *(f.name for f in side)} - set(self.query_tower_feature_names))
+        if unused:   # the query tower's input sums every embedder table (the CUDA path has no per-tower feature subset)
+            raise ValueError(f"side features {unused} are in the embedder but not in query_tower_feature_names; the query tower "
+                             "must embed every feature of the embedder (exclude the others from the SequenceEmbedding)")
+        if name not in reader.feature_names:
+            raise ValueError(f"the item features reader must hold the item feature {name!r}")
+        item_side = [f.name for f in side if f.name in set(reader.feature_names)]
         ref = torch.as_tensor(reader[name]).cpu()
         if ref.dim() != 1 or not torch.equal(ref.long(), torch.arange(card)):
             raise ValueError(f"the item features reader's {name!r} column must equal arange({card}): the rows of a complete, "
@@ -269,6 +323,7 @@ class TwoTowerBody:
         if enc.activation != "relu":
             raise ValueError(f"SasRecTransformerLayer supports activation='relu' only, got {enc.activation!r}")
         d = enc.embedding_dim
+        _check_side(emb.schema, side, d)
         if qagg.embedding_aggregator.embedding_dim != d or iagg.embedding_dim != d or (feat_dim is not None and feat_dim != d):
             raise ValueError("the embedder, the aggregators and the encoders must share one embedding_dim")
         if mask.num_heads != enc.num_heads:
@@ -286,8 +341,10 @@ class TwoTowerBody:
             raise ValueError(f"item_encoder must be SwiGLUEncoder(embedding_dim={d}, hidden_dim={2 * d}), got "
                              f"({ienc.embedding_dim}, {ienc.hidden_dim})")
         cfg = TwoTowerConfig(n_items=card, d=d, n_heads=enc.num_heads, n_blocks=enc.num_blocks, max_len=qagg.max_sequence_length,
-                             dropout=qagg.dropout, variant="new", lnf_eps=norm.eps)
-        return TwoTowerCore(cfg, item_feature=name, device=device, seed=seed)
+                             dropout=qagg.dropout, variant="new", lnf_eps=norm.eps, features=tuple(side),
+                             item_features=tuple(item_side))
+        return TwoTowerCore(cfg, item_feature=name, device=device, seed=seed,
+                            item_values={n: reader[n] for n in item_side})
 
 
 def _embedder_features(emb) -> list:
