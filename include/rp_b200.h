@@ -718,8 +718,8 @@ typedef struct rp_diff_attn_desc {
   rp_diff_lambda lam;
   const float* rms_scale;                           /* fp32 [v_slot], zero beyond 2*head_dim */
   void* out; long long ldo;                         /* bf16 normalised output */
-  /* training saves (all NULL in eval): o_pre = O before the per-head RMSNorm (geometry of out); e1 / e2 bf16
-   * [B*H, Lp, Lp] = exp(s - rowmax) of either map (zero where masked; Lp = round_up(L, 64); rows >= L are not written,
+  /* training saves (all NULL in eval; a NULL e1_save switches every save off): o_pre = O before the per-head RMSNorm
+   * (geometry of out); e1 / e2 bf16 [B*H, Lp, Lp] = exp(s - rowmax) of either map (zero where masked; Lp = round_up(L, 64); rows >= L are not written,
    * so the buffers are zero-initialised once); inv1 / inv2 fp32 [B*H, Lp] the reciprocal row sums */
   void* o_pre; void* e1_save; void* e2_save; float* inv1; float* inv2;
   float* o32_save; float* o2_save;                  /* fp32, geometry of out: O_pre and A2 . V (inputs of the lambda gradient) */

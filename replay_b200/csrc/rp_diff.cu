@@ -165,7 +165,8 @@ __global__ void __launch_bounds__(kFwdWarps * 32) diff_attn_fwd_kernel(rp_diff_a
     for (int t = 0; t < VS / 32; ++t) ss += o[t] * o[t];
     const float rstd = rsqrtf(warp_sum(ss) / (float)(2 * hd) + a.eps);
     __nv_bfloat16* orow = reinterpret_cast<__nv_bfloat16*>(a.out) + tok * a.ldo + h * VS;
-    __nv_bfloat16* prow = a.o_pre ? reinterpret_cast<__nv_bfloat16*>(a.o_pre) + tok * a.ldo + h * VS : nullptr;
+    // e1_save switches every save (as rp_diff_attn_fwd validates them): a set o_pre alone must not be written
+    __nv_bfloat16* prow = e1s ? reinterpret_cast<__nv_bfloat16*>(a.o_pre) + tok * a.ldo + h * VS : nullptr;
 #pragma unroll
     for (int t = 0; t < VS / 32; ++t) {
       const int c = lane + 32 * t;
