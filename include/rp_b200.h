@@ -445,8 +445,6 @@ int rp_colsum(const void* dy, int rows, int cols, long long ld, float* db, void*
 /* the same for n <= 6 tensors sharing the row count, one launch (the bias gradients of one block's backward) */
 int rp_colsum_multi(int n, const void* const* dy, const int* cols, const long long* ld, float* const* db, int rows, void* stream);
 
-/* torch.optim.Adam (models/nn/optimizer_utils/optimizer_factory.py:71-87; no weight decay) on flat fp32 buffers; refreshes
- * the bf16 shadow, optionally zeroes the gradient; lr and the step counter live in device memory. */
 /* BERT4Rec embedding: where(token_mask, table[ids], mask_emb) + pos[t % L] (bert4rec/model.py:239-296) and its backward;
  * row gather / scatter with a device-side row count (dst[r] = src[idx[r]] or dst[idx[r]] = src[r]).
  * pos == NULL (forward) / d_pos == NULL (backward): the model has no positional embedding (enable_positional_embedding
@@ -548,6 +546,23 @@ int rp_wgrad_group(const rp_wgrad_pair* pairs, int n_pairs, int T, int accumulat
 int rp_wgrad_group_rows(const rp_wgrad_pair* pairs, int n_pairs, int T, int accumulate, const int32_t* n_rows_dev,
                         void* workspace, size_t workspace_bytes, void* stream);
 
+/* The optimizer step of models/nn/optimizer_utils/optimizer_factory.py:71-87 / nn/lightning/optimizer.py:44-60 on flat
+ * fp32 buffers of n elements (n % 4 == 0, 16-byte aligned); refreshes the bf16 shadow (if not NULL), optionally zeroes the
+ * gradient.  lr and the step counter live in device memory (graph-replayable); every call first adds 1 to *step_dev.
+ * The gradient is g * grad_scale (1/world after a sum all-reduce), and weight_decay != 0 adds weight_decay * p to it.
+ *   RP_OPT_ADAM  torch.optim.Adam(lr, betas, eps, weight_decay): state0 = exp_avg, state1 = exp_avg_sq, bias corrections
+ *                from the incremented step.
+ *   RP_OPT_SGD   torch.optim.SGD(lr, momentum, weight_decay), dampening 0, no Nesterov; the step counter is not read.
+ *                momentum 0: no state (state0 and state1 unused).  momentum != 0: state0 = momentum_buffer, state1 unused.
+ *                A buffer that was never written must be zero: its first step then gives momentum * 0 + d = d, which is
+ *                torch's clone of d.  A restored buffer is simply used.
+ * frozen: per-element mask (or NULL) of parameters the step leaves unchanged; their state still advances.
+ * rp_adam_step is rp_optimizer_step(RP_OPT_ADAM, ..., weight_decay 0, momentum 0, ...). */
+#define RP_OPT_ADAM 0
+#define RP_OPT_SGD 1
+int rp_optimizer_step(int kind, float* p, float* g, float* state0, float* state1, void* shadow_bf16, long long n,
+                      const float* lr_dev, int32_t* step_dev, float beta1, float beta2, float eps, float weight_decay,
+                      float momentum, float grad_scale, const uint8_t* frozen, int zero_grad, void* stream);
 int rp_adam_step(float* p, float* g, float* m, float* v, void* shadow_bf16, long long n, const float* lr_dev,
                  int32_t* step_dev, float beta1, float beta2, float eps, float grad_scale, const uint8_t* frozen,
                  int zero_grad, void* stream);

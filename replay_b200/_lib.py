@@ -74,6 +74,8 @@ def lib():
     _sig(L.rp_dropout_bwd, c_int, [P, P, LL, c_int, P, c_float, U64, U64, P, P])
     _sig(L.rp_colsum, c_int, [P, c_int, c_int, LL, P, P])
     _sig(L.rp_adam_step, c_int, [P, P, P, P, P, LL, P, P, c_float, c_float, c_float, c_float, P, c_int, P])
+    _sig(L.rp_optimizer_step, c_int, [c_int, P, P, P, P, P, LL, P, P, c_float, c_float, c_float, c_float, c_float, c_float, P,
+                                      c_int, P])
     _sig(L.rp_peer_allreduce_state_bytes, c_size_t, [])
     _sig(L.rp_peer_allreduce, c_int, [P, P, c_int, c_int, LL, P])
     _sig(L.rp_cast_bf16, c_int, [P, P, LL, P])

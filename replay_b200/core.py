@@ -4,7 +4,7 @@
   REFERENCE's key names (SURVEY.md Appendix B) so checkpoints interchange with RePlay's modules;
 * the loss is produced by an ``autograd.Function`` whose backward runs the engine's hand-written backward kernels and
   hands the flat gradient to autograd, so ``loss.backward()`` + any torch optimizer (or Lightning's automatic
-  optimization) work unchanged; ``fused_step()`` instead runs forward+backward+Adam entirely in the engine.
+  optimization) work unchanged; ``fused_step()`` instead runs forward+backward+the optimizer step entirely in the engine.
 """
 from __future__ import annotations
 
@@ -13,7 +13,7 @@ import os
 
 import torch
 
-from .engine import _BLOCK_PARAMS, EncoderConfig, SasRecEngine
+from .engine import _BLOCK_PARAMS, EncoderConfig, OptimizerConfig, SasRecEngine
 
 _LEAF = {"ln1_w": "attention_layernorms.{i}.weight", "ln1_b": "attention_layernorms.{i}.bias",
          "in_w": "attention_layers.{i}.in_proj_weight", "in_b": "attention_layers.{i}.in_proj_bias",
@@ -89,8 +89,9 @@ class SasRecCore(torch.nn.Module):
         self.engine: SasRecEngine | None = None
         self.flat: torch.nn.Parameter | None = None
         self._pending_state = None
+        self._pending_opt_state = None   # optimizer state loaded before the engine had its gradient state
         self._shadow_dirty = True
-        self.adam_betas = (0.9, 0.98)  # optimizer_factory.py:56-63 / nn/lightning/optimizer.py:44-60
+        self.optimizer = OptimizerConfig()  # optimizer_factory.py:56-63 / nn/lightning/optimizer.py:44-60
         self._keymap = self._key_map()
         self._materialise()
 
@@ -100,17 +101,36 @@ class SasRecCore(torch.nn.Module):
 
     def for_catalog(self, n_items: int, state: dict) -> SasRecCore:
         """A core of the same kind for a catalog of ``n_items`` items, holding the reference-keyed weights ``state``.  The
-        loss, the Adam betas, the device and the seed carry over; Adam's moments restart, as they do for the reference's
-        newly created parameters.  This core's captured graphs are released."""
+        loss, the optimizer configuration, the device and the seed carry over; the optimizer state restarts, as it does for
+        the reference's newly created parameters.  This core's captured graphs are released."""
         self._drop_graphs()
         core = type(self)(dataclasses.replace(self.cfg, n_items=n_items), device=self._device, seed=self._seed,
                           **self._init_args())
         spec = getattr(self, "_loss_spec", None)
         if spec is not None:
             core.set_loss(spec[0], **spec[1])
-        core.adam_betas = tuple(self.adam_betas)
+        core.optimizer = self.optimizer
         core.load_state_dict(state)
         return core
+
+    @property
+    def adam_betas(self) -> tuple:
+        """The betas of ``optimizer`` (what Adam would use)."""
+        return self.optimizer.betas
+
+    @adam_betas.setter
+    def adam_betas(self, betas):
+        self.optimizer = dataclasses.replace(self.optimizer, betas=tuple(betas))
+
+    def load_optimizer_state(self, state: dict):
+        """Restore the fused optimizer's state from torch.optim's per-parameter format (``SasRecEngine.load_optimizer_state``).
+        Applied when the engine has its gradient state; the captured step graphs are released."""
+        e = self.engine
+        if e is None or not e.with_grad:
+            self._pending_opt_state = state
+            return
+        e.load_optimizer_state(state)
+        self._drop_graphs()
 
     def _key_map(self) -> dict:
         m = reference_key_map(self.cfg.variant, self.cfg.n_blocks, self.item_feature)
@@ -161,6 +181,9 @@ class SasRecCore(torch.nn.Module):
             e.resize(max(batch, e.B) if seq_len == e.L else batch, seq_len, with_grad or e.with_grad)
             e._loss_applied = None
             self._drop_graphs()
+        if e.with_grad and self._pending_opt_state is not None:
+            e.load_optimizer_state(self._pending_opt_state)
+            self._pending_opt_state = None
         return e
 
     # ---- the fused step replays two CUDA graphs (forward + backward | Adam) around the gradient exchange, exactly like
@@ -178,9 +201,9 @@ class SasRecCore(torch.nn.Module):
 
         tr = getattr(self, "_trainer", None)
         if tr is None or tr.engine is not eng:
-            tr = self._trainer = Trainer(eng, use_graph=self.use_cuda_graph, betas=self.adam_betas)
-        if tr.betas != tuple(self.adam_betas):
-            tr.betas = tuple(self.adam_betas)
+            tr = self._trainer = Trainer(eng, use_graph=self.use_cuda_graph, opt=self.optimizer)
+        if tr.opt != self.optimizer:
+            tr.opt = self.optimizer
             tr.invalidate()
         return tr
 
@@ -283,7 +306,7 @@ class SasRecCore(torch.nn.Module):
 
     def fused_step(self, ids, pad_mask, labels, target_mask, all_reduce="auto", lr: float | None = None,
                    negatives=None, row_weights=None, feats=None) -> torch.Tensor:
-        """forward + backward + Adam entirely inside the engine (no autograd, no torch optimizer).  ``all_reduce="auto"``
+        """forward + backward + the optimizer step entirely inside the engine (no autograd, no torch optimizer).  ``all_reduce="auto"``
         exchanges the gradient over ``torch.distributed`` whenever a process group with more than one rank is initialised
         (Lightning ``strategy="ddp"``): this path has no autograd backward for DDP's hooks to fire on."""
         B, L = ids.shape
@@ -301,7 +324,7 @@ class SasRecCore(torch.nn.Module):
             self._drop_graphs()  # another loss head or positive count: different kernels / buffers
         if isinstance(all_reduce, str):  # "auto": torch.distributed when initialised (inside Trainer.run)
             return self._graph_trainer(eng).run()[0]
-        return eng.train_step(all_reduce, betas=self.adam_betas)[0]
+        return eng.train_step(all_reduce, opt=self.optimizer)[0]
 
     def _set_lr(self, eng, lr):
         if lr is not None and lr != getattr(eng, "_lr_host", None):

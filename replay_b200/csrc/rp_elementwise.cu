@@ -1,11 +1,12 @@
 // rp_elementwise.cu - the HBM-bound kernels of the transformer body and of the optimizer: batch preparation / target
 // compaction, embedding gather + positional add (+dropout) and its backward, LayerNorm forward/backward (optionally
-// gathering / scattering the valid-target rows), dropout backward, bias-gradient column sums, Adam.
+// gathering / scattering the valid-target rows), dropout backward, bias-gradient column sums, the optimizer step.
 // All are coalesced, vectorised (8/16-byte accesses) row-per-warp kernels sized in multiples of the SM count.
 //
 // Reference call sites: replay/nn/sequential/sasrec/agg.py:37-53, replay/models/nn/sequential/sasrec/model.py:346-357
 // (embedding), transformer.py:47-49,60-62 + model.py:415-417,463 (LayerNorm eps 1e-8 / 1e-5),
-// replay/models/nn/optimizer_utils/optimizer_factory.py:71-87 (torch.optim.Adam).
+// replay/models/nn/optimizer_utils/optimizer_factory.py:71-87 (torch.optim.Adam / SGD).
+#include "rp_b200.h"
 #include "rp_host.h"
 #include "rp_philox.cuh"
 #include "rp_sm90.cuh"
@@ -737,35 +738,60 @@ __global__ void colsum_multi_kernel(const ColsumBatch b) {
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// Adam (torch.optim.Adam, no weight decay / amsgrad) over one flat fp32 parameter buffer; also refreshes the bf16 shadow
-// copy the kernels consume and zeroes the gradient for the next step.  The step counter and lr live in device memory so
-// the launch is CUDA-graph replayable.  grad_scale multiplies the gradient (1/world_size after a sum all-reduce).
+// The optimizer step over one flat fp32 parameter buffer; also refreshes the bf16 shadow copy the kernels consume and
+// zeroes the gradient for the next step.  The step counter and lr live in device memory so the launch is CUDA-graph
+// replayable.  grad_scale multiplies the gradient (1/world_size after a sum all-reduce) before the L2 decay term is added,
+// as torch.optim sees Lightning's averaged gradient.  Kinds (rp_b200.h RP_OPT_*):
+//   Adam          torch.optim.Adam(betas, eps, weight_decay): s0 = exp_avg, s1 = exp_avg_sq
+//   SGD           torch.optim.SGD(momentum=0, weight_decay): no state
+//   SGD momentum  torch.optim.SGD(momentum, weight_decay), dampening 0, no Nesterov: s0 = momentum_buffer.  A buffer that
+//                 was never written is zero, so its first step gives momentum * 0 + d = d: torch's clone of d
 // ------------------------------------------------------------------------------------------------------------------
-__global__ void adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                            __nv_bfloat16* __restrict__ shadow, long long n, const float* __restrict__ lr_dev,
-                            const int32_t* __restrict__ step_dev, float beta1, float beta2, float eps, float grad_scale,
-                            const uint8_t* __restrict__ frozen /* per-element freeze mask or null */, int zero_grad) {
+constexpr int RP_OPT_SGD_MOMENTUM = 2;   // RP_OPT_SGD with momentum != 0: the kernel variant that keeps a buffer
+
+template <int kKind, bool kDecay>
+__global__ void optimizer_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                                 __nv_bfloat16* __restrict__ shadow, long long n, const float* __restrict__ lr_dev,
+                                 const int32_t* __restrict__ step_dev, float beta1, float beta2, float eps, float weight_decay,
+                                 float momentum, float grad_scale,
+                                 const uint8_t* __restrict__ frozen /* per-element freeze mask or null */, int zero_grad) {
   const float lr = *lr_dev;
-  const int step = *step_dev;  // 1-based, already incremented by adam_tick_kernel
-  const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
-  const float step_size = lr / bc1, inv_sqrt_bc2 = rsqrtf(bc2);
+  float step_size = 0.f, inv_sqrt_bc2 = 0.f;
+  if constexpr (kKind == RP_OPT_ADAM) {
+    const int step = *step_dev;  // 1-based, already incremented by adam_tick_kernel
+    const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
+    step_size = lr / bc1;
+    inv_sqrt_bc2 = rsqrtf(bc2);
+  }
   for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4; i < n;
        i += (long long)gridDim.x * blockDim.x * 4) {
     float4 pp = *reinterpret_cast<float4*>(p + i), gg = *reinterpret_cast<float4*>(g + i);
-    float4 mm = *reinterpret_cast<float4*>(m + i), vv = *reinterpret_cast<float4*>(v + i);
+    float4 mm = make_float4(0.f, 0.f, 0.f, 0.f), vv = mm;
+    if constexpr (kKind != RP_OPT_SGD) mm = *reinterpret_cast<float4*>(m + i);
+    if constexpr (kKind == RP_OPT_ADAM) vv = *reinterpret_cast<float4*>(v + i);
     float* pa = &pp.x; float* ga = &gg.x; float* ma = &mm.x; float* va = &vv.x;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      const float gk = ga[k] * grad_scale;
-      ma[k] = beta1 * ma[k] + (1.f - beta1) * gk;
-      va[k] = beta2 * va[k] + (1.f - beta2) * gk * gk;
-      const float denom = sqrtf(va[k]) * inv_sqrt_bc2 + eps;
-      const float upd = step_size * ma[k] / denom;
+      float gk = ga[k] * grad_scale;
+      if constexpr (kDecay) gk = fmaf(weight_decay, pa[k], gk);   // grad.add(param, alpha=weight_decay)
+      float upd;
+      if constexpr (kKind == RP_OPT_ADAM) {
+        ma[k] = beta1 * ma[k] + (1.f - beta1) * gk;
+        va[k] = beta2 * va[k] + (1.f - beta2) * gk * gk;
+        const float denom = sqrtf(va[k]) * inv_sqrt_bc2 + eps;
+        upd = step_size * ma[k] / denom;
+      } else if constexpr (kKind == RP_OPT_SGD_MOMENTUM) {
+        // buf.mul_(momentum).add_(d): two roundings, as torch's two passes
+        ma[k] = __fadd_rn(__fmul_rn(momentum, ma[k]), gk);
+        upd = lr * ma[k];
+      } else {
+        upd = lr * gk;
+      }
       if (!frozen || !frozen[i + k]) pa[k] -= upd;
     }
     *reinterpret_cast<float4*>(p + i) = pp;
-    *reinterpret_cast<float4*>(m + i) = mm;
-    *reinterpret_cast<float4*>(v + i) = vv;
+    if constexpr (kKind != RP_OPT_SGD) *reinterpret_cast<float4*>(m + i) = mm;
+    if constexpr (kKind == RP_OPT_ADAM) *reinterpret_cast<float4*>(v + i) = vv;
     if (zero_grad) *reinterpret_cast<float4*>(g + i) = make_float4(0.f, 0.f, 0.f, 0.f);
     if (shadow) {
       uint2 w;
@@ -1102,16 +1128,42 @@ RP_API int rp_colsum_multi(int n, const void* const* dy, const int* cols, const 
   return RP_OK;
 }
 
+template <int kKind>
+static void launch_optimizer(float* p, float* g, float* s0, float* s1, void* shadow_bf16, long long n, const float* lr_dev,
+                             const int32_t* step_dev, float beta1, float beta2, float eps, float weight_decay, float momentum,
+                             float grad_scale, const uint8_t* frozen, int zero_grad, cudaStream_t stream) {
+  auto* shadow = reinterpret_cast<__nv_bfloat16*>(shadow_bf16);
+  auto kernel = weight_decay != 0.f ? optimizer_kernel<kKind, true> : optimizer_kernel<kKind, false>;
+  kernel<<<grid_for(n / 4, 256), 256, 0, stream>>>(p, g, s0, s1, shadow, n, lr_dev, step_dev, beta1, beta2, eps, weight_decay,
+                                                   momentum, grad_scale, frozen, zero_grad);
+}
+
+RP_API int rp_optimizer_step(int kind, float* p, float* g, float* state0, float* state1, void* shadow_bf16, long long n,
+                             const float* lr_dev, int32_t* step_dev, float beta1, float beta2, float eps, float weight_decay,
+                             float momentum, float grad_scale, const uint8_t* frozen, int zero_grad, void* stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (!p || !g || !lr_dev || !step_dev || n <= 0 || (n & 3) || (kind != RP_OPT_ADAM && kind != RP_OPT_SGD)) return RP_EINVAL;
+  if (kind == RP_OPT_SGD && momentum != 0.f) kind = RP_OPT_SGD_MOMENTUM;
+  if ((kind == RP_OPT_ADAM && (!state0 || !state1)) || (kind == RP_OPT_SGD_MOMENTUM && !state0)) return RP_EINVAL;
+  adam_tick_kernel<<<1, 1, 0, stream>>>(step_dev);
+  if (kind == RP_OPT_ADAM)
+    launch_optimizer<RP_OPT_ADAM>(p, g, state0, state1, shadow_bf16, n, lr_dev, step_dev, beta1, beta2, eps, weight_decay,
+                                  momentum, grad_scale, frozen, zero_grad, stream);
+  else if (kind == RP_OPT_SGD)
+    launch_optimizer<RP_OPT_SGD>(p, g, state0, state1, shadow_bf16, n, lr_dev, step_dev, beta1, beta2, eps, weight_decay,
+                                 momentum, grad_scale, frozen, zero_grad, stream);
+  else
+    launch_optimizer<RP_OPT_SGD_MOMENTUM>(p, g, state0, state1, shadow_bf16, n, lr_dev, step_dev, beta1, beta2, eps,
+                                          weight_decay, momentum, grad_scale, frozen, zero_grad, stream);
+  RP_LAUNCH_CHECK();
+  return RP_OK;
+}
+
 RP_API int rp_adam_step(float* p, float* g, float* m, float* v, void* shadow_bf16, long long n, const float* lr_dev,
                         int32_t* step_dev, float beta1, float beta2, float eps, float grad_scale, const uint8_t* frozen,
                         int zero_grad, void* stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (!p || !g || !m || !v || !lr_dev || !step_dev || n <= 0 || (n & 3)) return RP_EINVAL;
-  adam_tick_kernel<<<1, 1, 0, stream>>>(step_dev);
-  adam_kernel<<<grid_for(n / 4, 256), 256, 0, stream>>>(p, g, m, v, reinterpret_cast<__nv_bfloat16*>(shadow_bf16), n, lr_dev,
-                                                        step_dev, beta1, beta2, eps, grad_scale, frozen, zero_grad);
-  RP_LAUNCH_CHECK();
-  return RP_OK;
+  return rp_optimizer_step(RP_OPT_ADAM, p, g, m, v, shadow_bf16, n, lr_dev, step_dev, beta1, beta2, eps, 0.f, 0.f, grad_scale,
+                           frozen, zero_grad, stream_);
 }
 
 RP_API int rp_cast_bf16(const float* src, void* dst, long long n, void* stream_) {

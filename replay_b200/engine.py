@@ -30,6 +30,31 @@ def _ru(x, m):
     return (x + m - 1) // m * m
 
 
+@dataclass(frozen=True)
+class OptimizerConfig:
+    """The optimizer of the fused step, as the reference's factories build it (models/nn/optimizer_utils/
+    optimizer_factory.py:71-87, nn/lightning/optimizer.py:44-60): ``torch.optim.Adam(lr, betas, eps, weight_decay)`` or
+    ``torch.optim.SGD(lr, momentum, weight_decay)``.  The learning rate is the engine's device-resident ``lr``."""
+
+    kind: str = "adam"            # "adam" | "sgd"
+    betas: tuple = (0.9, 0.98)
+    eps: float = 1e-8
+    weight_decay: float = 0.0
+    momentum: float = 0.0
+
+    def __post_init__(self):
+        object.__setattr__(self, "betas", tuple(self.betas))
+
+    def validate(self) -> OptimizerConfig:
+        """The reference factories raise for an unknown name from ``create()``, not from their constructor: so does a step."""
+        if self.kind not in _OPT_KINDS:
+            raise ValueError("Unexpected optimizer")
+        return self
+
+
+_OPT_KINDS = {"adam": 0, "sgd": 1}   # RP_OPT_ADAM / RP_OPT_SGD
+
+
 @dataclass
 class BaseConfig:
     """What SASRec (EncoderConfig) and BERT4Rec (BertConfig) share: the transformer's sizes, the feature-slot geometry
@@ -256,7 +281,7 @@ class _CountingLib:
 
     KERNELS = {"rp_gemm": 1, "rp_attn_fwd": 1, "rp_attn_bwd": 1, "rp_attn_last": 1, "rp_attn_softmax_bwd": 1, "rp_prepare_batch": 2, "rp_embed_fwd": 1,
                "rp_embed_bwd": 2, "rp_layernorm_fwd": 1, "rp_layernorm_fwd_compact": 1, "rp_layernorm_bwd": 1, "rp_dropout_bwd": 1, "rp_colsum": 1, "rp_colsum_multi": 1,
-               "rp_adam_step": 2, "rp_cast_bf16": 1, "rp_counter_add": 1, "rp_reduce_splits": 1, "rp_ce_head_fwd": 2, "rp_ce_head_bwd": 3,
+               "rp_adam_step": 2, "rp_optimizer_step": 2, "rp_cast_bf16": 1, "rp_counter_add": 1, "rp_reduce_splits": 1, "rp_ce_head_fwd": 2, "rp_ce_head_bwd": 3,
                "rp_score_topk": 2, "rp_seen_prepare": 1, "rp_sampled_head_fwd": 4, "rp_sampled_head_bwd": 4, "rp_post_attn_fused": 1,
                "rp_post_attn_train": 1, "rp_wgrad_group": 2, "rp_ln_qkv_fused": 1, "rp_pre_attn_bwd": 1,
                "rp_post_attn_bwd": 1, "rp_row_plan": 3, "rp_embed_fwd_rows": 1, "rp_embed_bwd_rows": 2, "rp_ln_qkv_fused_rows": 1,
@@ -343,7 +368,8 @@ class SasRecEngine:
 
     # ------------------------------------------------------------------------------------------------ state that outlives a batch geometry
     def _alloc_grad_state(self):
-        """Flat gradient, Adam moments, learning rate and step counter: sized by the configuration only, allocated once."""
+        """Flat gradient, optimizer state, learning rate and step counter: sized by the configuration only, allocated once.
+        ``adam_m`` / ``adam_v`` are Adam's moments; SGD keeps its momentum buffer in ``adam_m``."""
         f32 = dict(device=self.dev, dtype=torch.float32)
         n = self.n_flat
         # data-parallel runs on one NVLink node: the gradient lives in a symmetric (peer-mapped) allocation so that the
@@ -357,6 +383,7 @@ class SasRecEngine:
         self.grads = {k: self.g32[o:o + math.prod(s)].view(s) for k, (o, s) in self.layout.items()}
         self.lr = torch.full((1,), 1e-3, **f32)
         self.step_count = torch.zeros(1, device=self.dev, dtype=torch.int32)
+        self.opt_kind = "adam"   # the optimizer the state belongs to
 
     def _check_geometry(self, seq_len: int):
         cfg = self.cfg
@@ -1532,26 +1559,65 @@ class SasRecEngine:
                                     pos0, math.sqrt(cfg.d), int(legacy), drop, self.seed, 0, self.rng_counter.data_ptr(),
                                     G["item_emb"].data_ptr(), G["pos_emb"].data_ptr(), st()), "rp_embed_bwd")
 
-    def optimizer_step(self, grad_scale: float = 1.0, beta1=0.9, beta2=0.98, eps=1e-8):
-        """torch.optim.Adam(lr, betas=(0.9, 0.98)) (optimizer_factory.py:56-63,79-80) on the flat buffers; also refreshes
-        the bf16 shadow weights and zeroes the gradients."""
-        check(self.lib.rp_adam_step(self.p32.data_ptr(), self.g32.data_ptr(), self.adam_m.data_ptr(), self.adam_v.data_ptr(),
-                                    self.p16.data_ptr(), self.n_flat, self.lr.data_ptr(), self.step_count.data_ptr(), beta1,
-                                    beta2, eps, grad_scale, None, 1, self._stream()), "rp_adam_step")
+    def optimizer_step(self, grad_scale: float = 1.0, opt: OptimizerConfig = OptimizerConfig()):
+        """One step of ``opt`` (default: torch.optim.Adam(lr, betas=(0.9, 0.98)), optimizer_factory.py:56-63,79-80) on the
+        flat buffers; also refreshes the bf16 shadow weights and zeroes the gradients.  A step of another kind than the
+        state's starts from fresh state, as a newly built torch optimizer does."""
+        if opt.validate().kind != self.opt_kind:
+            self.reset_optimizer_state(opt.kind)
+        adam = opt.kind == "adam"
+        check(self.lib.rp_optimizer_step(_OPT_KINDS[opt.kind], self.p32.data_ptr(), self.g32.data_ptr(),
+                                         self.adam_m.data_ptr(), self.adam_v.data_ptr() if adam else None, self.p16.data_ptr(),
+                                         self.n_flat, self.lr.data_ptr(), self.step_count.data_ptr(), opt.betas[0],
+                                         opt.betas[1], opt.eps, opt.weight_decay, opt.momentum, grad_scale, None, 1,
+                                         self._stream()), "rp_optimizer_step")
+
+    def reset_optimizer_state(self, kind: str = "adam"):
+        """Zero the moments (or momentum buffer) and the step counter: the state of a newly built optimizer of ``kind``."""
+        self.adam_m.zero_()
+        self.adam_v.zero_()
+        self.step_count.zero_()
+        self.opt_kind = kind
+
+    def optimizer_state(self, opt: OptimizerConfig) -> dict:
+        """The state of ``opt`` for the flat parameter in torch.optim's per-parameter format (host copies): Adam's ``step`` /
+        ``exp_avg`` / ``exp_avg_sq``, SGD's ``momentum_buffer``; empty where a newly built torch optimizer's is (no step
+        taken, momentum 0, or state of the other kind, which the next step discards)."""
+        steps = int(self.step_count.item())
+        if opt.kind != self.opt_kind or steps == 0:
+            return {}
+        if opt.kind == "adam":
+            return {"step": torch.tensor(float(steps)), "exp_avg": self.adam_m.cpu(), "exp_avg_sq": self.adam_v.cpu()}
+        return {"momentum_buffer": self.adam_m.cpu()} if opt.momentum != 0 else {}
+
+    def load_optimizer_state(self, state: dict):
+        """Restore what ``optimizer_state`` returns (or a torch Adam / SGD state of the flat parameter)."""
+        if "exp_avg" in state:
+            self.reset_optimizer_state("adam")
+            self.adam_m.copy_(state["exp_avg"])
+            self.adam_v.copy_(state["exp_avg_sq"])
+            self.step_count.fill_(int(state["step"]))
+        elif state.get("momentum_buffer") is not None:
+            self.reset_optimizer_state("sgd")
+            self.adam_m.copy_(state["momentum_buffer"])
+            self.step_count.fill_(1)   # torch's SGD keeps no step count: the restored buffer stands for one or more steps
+        else:
+            self.reset_optimizer_state(self.opt_kind)
 
     def tick_rng(self):
         check(self.lib.rp_counter_add(self.rng_counter.data_ptr(), 0x9E3779B97F4A7C15 & 0xFFFFFFFFFFFF, self._stream()),
               "rp_counter_add")
 
-    def train_step(self, all_reduce=None, betas=(0.9, 0.98)):
-        """forward + backward + (optional gradient all-reduce callback on the flat fp32 gradient) + Adam."""
+    def train_step(self, all_reduce=None, opt: OptimizerConfig = OptimizerConfig()):
+        """forward + backward + (optional gradient all-reduce callback on the flat fp32 gradient) + the optimizer step."""
+        opt.validate()   # before the backward accumulates a gradient that no step would consume
         self.tick_rng()
         loss = self.forward_train()
         self.backward()
         scale = 1.0
         if all_reduce is not None:
             scale = all_reduce(self.g32)
-        self.optimizer_step(grad_scale=scale, beta1=betas[0], beta2=betas[1])
+        self.optimizer_step(grad_scale=scale, opt=opt)
         return loss
 
     # ------------------------------------------------------------------------------------------------ inference

@@ -121,7 +121,7 @@ class _BertCore(SasRecCore):
         eng.set_batch(ids, pad_mask, token_mask, labels)
         if isinstance(all_reduce, str):
             return self._graph_trainer(eng).run()[0]
-        return eng.train_step(all_reduce, betas=self.adam_betas)[0]
+        return eng.train_step(all_reduce, opt=self.optimizer)[0]
 
     @torch.no_grad()
     def _query_padded(self, ids, pad_mask, token_mask, feats=None):

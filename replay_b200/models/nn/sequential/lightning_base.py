@@ -22,12 +22,11 @@ class LegacyLightningModule(FusedOptimizerModule):
     def load_state_dict(self, sd, strict=True, assign=False):
         return self._model.load_state_dict({k[len("_model."):]: v for k, v in sd.items() if k.startswith("_model.")}, strict)
 
+    def _fused_core(self):
+        return self._model.core
+
     def configure_optimizers(self):
-        params = [self._model.core.flat]
-        if self._optimizer_factory is not None:
-            opt = self._optimizer_factory.create(params)
-        else:
-            opt = torch.optim.Adam(params, lr=1e-3, betas=(0.9, 0.98))  # optimizer_factory.py:56-63
+        opt = self._create_optimizer([self._model.core.flat])
         if self._lr_scheduler_factory is None:
             return opt
         return [opt], [self._lr_scheduler_factory.create(opt)]

@@ -8,16 +8,24 @@ from ...compat import FusedOptimizerModule
 
 
 class OptimizerFactory:
-    """replay/nn/lightning/optimizer.py:24-60 - Adam(lr 1e-3, betas (0.9, 0.98)) by default."""
+    """replay/nn/lightning/optimizer.py:24-60 - Adam(lr 1e-3, betas (0.9, 0.98)) by default, or SGD.  The fused step runs
+    the same optimizer (``optimizer``, ``learning_rate``, ``weight_decay``, ``sgd_momentum``, ``betas``) on the GPU."""
 
     def __init__(self, optimizer: str = "adam", learning_rate: float = 0.001, weight_decay: float = 0.0,
-                 betas: tuple = (0.9, 0.98)):
-        if optimizer != "adam" or weight_decay != 0.0:
-            raise NotImplementedError("the fused path implements Adam without weight decay (the reference default)")
-        self.learning_rate, self.betas = learning_rate, betas
+                 sgd_momentum: float = 0.0, betas: tuple = (0.9, 0.98)):
+        self.optimizer = optimizer
+        self.learning_rate = learning_rate
+        self.weight_decay = weight_decay
+        self.sgd_momentum = sgd_momentum
+        self.betas = betas
 
     def create(self, parameters):
-        return torch.optim.Adam(parameters, lr=self.learning_rate, betas=self.betas)
+        if self.optimizer == "adam":
+            return torch.optim.Adam(parameters, lr=self.learning_rate, weight_decay=self.weight_decay, betas=self.betas)
+        if self.optimizer == "sgd":
+            return torch.optim.SGD(parameters, lr=self.learning_rate, weight_decay=self.weight_decay,
+                                   momentum=self.sgd_momentum)
+        raise ValueError("Unexpected optimizer")
 
 
 class LazyInferenceOutput(dict):
@@ -66,11 +74,11 @@ class LazyInferenceOutput(dict):
 
 
 class LightningModule(FusedOptimizerModule):
-    """replay/nn/lightning/module.py:13-123.  ``fused_optimizer=True`` (default) runs forward+backward+Adam inside the CUDA
-    engine (manual optimisation; under ``torch.distributed`` the flat gradient is all-reduced before Adam, which is what
-    Lightning's DDP does for the reference); with False the loss goes through autograd and the optimizer from
-    ``optimizer_factory``.  In fused mode the learning rate of every step is read from the optimizer Lightning configured
-    (so an lr scheduler takes effect), ``betas`` come from the factory."""
+    """replay/nn/lightning/module.py:13-123.  ``fused_optimizer=True`` (default) runs forward+backward+the factory's
+    optimizer inside the CUDA engine (manual optimisation; under ``torch.distributed`` the flat gradient is all-reduced
+    before the optimizer step, which is what Lightning's DDP does for the reference); with False the loss goes through
+    autograd and the optimizer from ``optimizer_factory``.  In fused mode the learning rate of every step is read from the
+    optimizer Lightning configured (so an lr scheduler takes effect), the rest comes from the factory."""
 
     def __init__(self, model, optimizer_factory: OptimizerFactory | None = None, lr_scheduler_factory=None,
                  fused_optimizer: bool = True):
@@ -81,6 +89,9 @@ class LightningModule(FusedOptimizerModule):
         self._setup_optimizer(getattr(model, "core", None), optimizer_factory or OptimizerFactory(), lr_scheduler_factory,
                               fused_optimizer)
         self._sig = set(inspect.signature(model.forward).parameters)
+
+    def _fused_core(self):
+        return getattr(self.model, "core", None)
 
     def forward(self, batch: dict):
         if "candidates_to_score" in self._sig and self._candidates_to_score is not None and not self.model.training:

@@ -2,7 +2,7 @@
 
 Mirrors what ``lightning.Trainer(strategy="ddp")`` does around the reference's ``training_step`` (SURVEY.md §5, §8e):
 every rank runs forward/backward on its own shard of the batch, the flat fp32 gradient is sum-reduced over NVLink with
-one ``ncclAllReduce`` and Adam applies it scaled by 1/world_size on every rank."""
+one ``ncclAllReduce`` and the optimizer step applies it scaled by 1/world_size on every rank."""
 from __future__ import annotations
 
 import os
@@ -10,11 +10,12 @@ import os
 import torch
 import torch.distributed as dist
 
-from .engine import SasRecEngine
+from .engine import OptimizerConfig, SasRecEngine
 
 
 class Trainer:
-    def __init__(self, engine: SasRecEngine, use_graph: bool = True, betas=(0.9, 0.98), one_graph: bool | None = None):
+    def __init__(self, engine: SasRecEngine, use_graph: bool = True, opt: OptimizerConfig = OptimizerConfig(),
+                 one_graph: bool | None = None):
         self.engine = engine
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         self.use_graph = use_graph
@@ -26,7 +27,7 @@ class Trainer:
             self.one_graph = False   # gloo stages CUDA tensors through the host: not capturable
         # the engine's gradient sits in a symmetric allocation: the exchange is rp_peer_allreduce, a kernel of the step graph
         self.peer = getattr(engine, "peer", None) if self.world > 1 else None
-        self.betas = tuple(betas)
+        self.opt = opt
         # the step reads only the loss and the gradients, so the body runs on packed rows where that is exact
         # (SasRecEngine.packed_eligible); RP_PACKED_BODY=0 keeps the padded rows for A/B runs
         engine.packed_body = os.environ.get("RP_PACKED_BODY", "1") != "0"
@@ -34,7 +35,7 @@ class Trainer:
         self.invalidate()
 
     def invalidate(self):
-        """Drop the captured graphs (the engine's workspace was re-allocated, the loss head or the Adam betas changed)."""
+        """Drop the captured graphs (the engine's workspace was re-allocated, the loss head or the optimizer changed)."""
         self._g_fb = None
         self._g_opt = None
         self._warm = 0
@@ -55,7 +56,7 @@ class Trainer:
         e.backward()
 
     def _opt(self, scale):
-        self.engine.optimizer_step(grad_scale=scale, beta1=self.betas[0], beta2=self.betas[1])
+        self.engine.optimizer_step(grad_scale=scale, opt=self.opt)
 
     def step(self, *batch):
         """One optimisation step on this rank's shard; ``batch`` is what the engine's ``set_batch`` takes (SASRec: ids,
@@ -67,6 +68,7 @@ class Trainer:
     def run(self):
         """The step on the batch already staged in the engine's static input buffers (``set_batch`` / ``set_negatives``)."""
         e = self.engine
+        self.opt.validate()   # before the backward accumulates a gradient that no step would consume
         if not self.use_graph:
             c0 = e.lib.count
             self._fwd_bwd()
