@@ -691,6 +691,38 @@ int rp_build_batch(const int64_t* offsets, const int32_t* items, long long n_seq
                    unsigned long long seed, unsigned long long draw0, const int64_t* query_ids, int64_t* ids,
                    uint8_t* pad_mask, int64_t* labels, uint8_t* aux_mask, int64_t* query_out, void* stream);
 
+/* Feature columns of the same store, cut in the same launch (rp_build_batch_features).  A column holds one entry per
+ * event of every history, aligned with `items` (event e of history s is offsets[s] + k):
+ *   RP_BATCH_COL_INT   one integer per event, values int32 or int64 (in_bytes 4 / 8)           -> out int64 [B, L]
+ *   RP_BATCH_COL_FLOAT `width` floats per event ([n_events, width]), float32 or float64        -> out [B, L, width]
+ *                      (width 1: a scalar, out [B, L]); out_bytes 4 = float32 (rounded to nearest), 8 = float64
+ *   RP_BATCH_COL_LIST  a list of any length per event: list_offsets [n_events + 1] into values (int32 / int64);
+ *                      out int64 [B, L, width]: each event's LAST `width` entries left-padded to width with the padding
+ *                      value (Array2DColumn.__getitem__, replay/data/nn/parquet/impl/array_2d_column.py:72-92)
+ * Every column uses the ids' window, offset and shift: a position that is padding in the ids (and the last position of
+ * RP_BATCH_BERT_PREDICT) is pad_int / pad_float in every element.  Integer outputs take pad_int, float outputs pad_float
+ * converted to the output type.  At most RP_BATCH_MAX_COLUMNS columns.  Other arguments as rp_build_batch, which this
+ * call runs in the same kernel; n_cols == 0 is rp_build_batch.  RP_EINVAL: null pointer, unknown kind, byte widths
+ * other than 4 / 8 (int out_bytes must be 8), width < 1, n_cols outside [0, RP_BATCH_MAX_COLUMNS].  No host
+ * synchronisation: the descriptors are passed by value to the kernel. */
+#define RP_BATCH_MAX_COLUMNS 16
+#define RP_BATCH_COL_INT 0
+#define RP_BATCH_COL_FLOAT 1
+#define RP_BATCH_COL_LIST 2
+typedef struct rp_batch_column {
+  int kind, in_bytes, out_bytes, width;
+  const void* values;
+  const int64_t* list_offsets;
+  void* out;
+  long long pad_int;
+  double pad_float;
+} rp_batch_column;
+int rp_build_batch_features(const int64_t* offsets, const int32_t* items, long long n_seq, const int32_t* seq_index,
+                            const int32_t* seq_offset, int B, int L, int mode, int pad_value, float mask_prob,
+                            const float* uniforms, unsigned long long seed, unsigned long long draw0,
+                            const int64_t* query_ids, int64_t* ids, uint8_t* pad_mask, int64_t* labels, uint8_t* aux_mask,
+                            int64_t* query_out, const rp_batch_column* cols, int n_cols, void* stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Bring-up self test of the wgmma operand encodings (used by tests/, not by the product path).
  * A, B: bf16 [128,128]; D: fp32 [128,128].  mode bit0: B given as Bt[K,N]; bit1: A read into registers;

@@ -284,8 +284,24 @@ TI_MAX_SPAN = 320   # RP_TI_MAX_SPAN: largest time_span of the time-interval att
 TI_MAX_COLS = 256   # RP_TI_MAX_COLS: at most four 64-wide head slots
 
 
+class BatchColumn(ctypes.Structure):
+    """Mirror of ``struct rp_batch_column`` (include/rp_b200.h): one feature column of the device sequence store."""
+
+    _fields_ = [
+        ("kind", c_int), ("in_bytes", c_int), ("out_bytes", c_int), ("width", c_int),
+        ("values", c_void_p), ("list_offsets", c_void_p), ("out", c_void_p),
+        ("pad_int", ctypes.c_longlong), ("pad_float", ctypes.c_double),
+    ]
+
+
+BATCH_COL_INT, BATCH_COL_FLOAT, BATCH_COL_LIST = range(3)   # rp_batch_column.kind
+BATCH_MAX_COLUMNS = 16   # RP_BATCH_MAX_COLUMNS: most feature columns one batch launch takes
+
+
 _P, _LL, _U64 = c_void_p, ctypes.c_longlong, ctypes.c_ulonglong
 _EXTRA_SIGS: list = [
+    ("rp_build_batch_features", c_int, [_P, _P, _LL, _P, _P, c_int, c_int, c_int, c_int, c_float, _P, _U64, _U64, _P, _P, _P,
+                                        _P, _P, _P, ctypes.POINTER(BatchColumn), c_int, _P]),
     ("rp_ti_attn_fwd", c_int, [ctypes.POINTER(TiAttnDesc), _P, _P, _P, _P, _P, _P]),
     ("rp_ti_attn_bwd_workspace", c_size_t, [c_int, c_int, c_int]),
     ("rp_ti_attn_bwd", c_int, [ctypes.POINTER(TiAttnDesc), _P, _P, _P, _P, _P, _P, c_size_t, _P, _P, _P]),

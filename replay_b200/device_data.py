@@ -6,15 +6,198 @@ path (``TorchSequentialDataset.__getitem__`` -> ``SasRecTrainingDataset.__getite
 default collate -> H2D copy; replay/data/nn/torch_sequential_dataset.py:69-171, sasrec/dataset.py:104-126,
 bert4rec/dataset.py:71-92,163-177,322-351).  The produced batch dictionaries carry the reference's key names, dtypes and
 shapes, so they feed ``training_step`` / ``predict_step`` of the modules in ``replay_b200.models`` / ``replay_b200.nn``
-unchanged.  There is no CPU fallback: building a batch needs the CUDA library."""
+unchanged.  There is no CPU fallback: building a batch needs the CUDA library.
+
+Next to the item ids the store holds sequence feature columns, one entry per event and aligned with the item history,
+cut in the same launch (``rp_build_batch_features``) through the same window, offset and shift as the ids, each left-padded
+with its own padding value.  Four kinds: an integer scalar (stored as int32 when every value fits, else int64), a float
+scalar (stored in its source dtype, float32 or float64), a float vector of one ``dim`` for every event (``[n_events,
+dim]``) and an integer list of any length per event (a second level of offsets plus flat values; output width ``K``).
+Legacy builders emit every integer as int64 and every float as float32 (TorchSequentialDataset._get_tensor_dtype); the
+new-path builders emit integers as int64 and keep each float column's dtype."""
 from __future__ import annotations
 
 import numpy as np
 import torch
 
-from ._lib import check, lib
+from ._lib import BATCH_COL_FLOAT, BATCH_COL_INT, BATCH_COL_LIST, BATCH_MAX_COLUMNS, BatchColumn, check, lib
 
 SASREC_TRAIN, PREDICT, BERT_TRAIN, BERT_PREDICT = 0, 1, 2, 3
+_INT32 = np.iinfo(np.int32)
+
+
+class FeatureColumn:
+    """One sequence feature of a ``DeviceSequenceStore`` on the store's device.  ``kind``: ``"int"``, ``"float"`` or
+    ``"list"``; ``tail``: the per-event output shape (``()`` for a scalar, ``(dim,)`` for a vector, ``(K,)`` for a list);
+    ``values``: the flat event values; ``list_offsets``: ``[n_events + 1]`` for a list column, else None."""
+
+    def __init__(self, name, kind, values, tail, padding_value, list_offsets=None):
+        self.name, self.kind, self.tail, self.list_offsets = name, kind, tuple(tail), list_offsets
+        self.values = values
+        self.padding_value = padding_value
+        self.width = int(np.prod(self.tail)) if self.tail else 1
+
+
+def _narrow_int(values: np.ndarray) -> np.ndarray:
+    values = np.asarray(values, dtype=np.int64)
+    if len(values) == 0 or (values.min() >= _INT32.min and values.max() <= _INT32.max):
+        return values.astype(np.int32)
+    return values
+
+
+def _float_dtype(dtypes) -> np.dtype:
+    return np.dtype(np.float64) if any(np.dtype(d) == np.float64 for d in dtypes) else np.dtype(np.float32)
+
+
+def _make_column(name, kind, values, seq_lengths, item_lengths, padding_value, *, dim=None, event_lengths=None,
+                 list_width=None, device="cuda"):
+    """Checks one column against the item history and moves it to the device.  ``values``: flat event values (float
+    vectors flattened row-major, list entries concatenated); ``seq_lengths``: events per sequence; ``event_lengths``: entries
+    per event of a list column."""
+    seq_lengths = np.asarray(seq_lengths, dtype=np.int64)
+    if len(seq_lengths) != len(item_lengths) or np.any(seq_lengths != item_lengths):
+        bad = np.flatnonzero(seq_lengths != item_lengths)[:1] if len(seq_lengths) == len(item_lengths) else []
+        where = f" (sequence {int(bad[0])}: {int(seq_lengths[bad[0]])} events, {int(item_lengths[bad[0]])} items)" if len(bad) \
+            else f" ({len(seq_lengths)} sequences, {len(item_lengths)} histories)"
+        raise ValueError(f"feature {name!r}: per-sequence lengths differ from the item column's{where}")
+    dev = torch.device(device)
+    list_offsets = None
+    if kind == "int":
+        vals, tail = _narrow_int(values), ()
+        pad = int(padding_value)
+    elif kind == "float":
+        vals = np.asarray(values)
+        vals = vals.astype(_float_dtype([vals.dtype]))
+        tail = () if dim is None else (int(dim),)
+        pad = float(padding_value)
+    else:
+        k = list_width
+        if k is None:
+            k = max(1, int(np.max(event_lengths))) if len(event_lengths) else 1
+        if int(k) < 1:
+            raise ValueError(f"feature {name!r}: list width K must be >= 1, got {k}")
+        vals, tail = _narrow_int(values), (int(k),)
+        pad = int(padding_value)
+        offs = np.zeros(len(event_lengths) + 1, dtype=np.int64)
+        np.cumsum(event_lengths, out=offs[1:])
+        list_offsets = torch.from_numpy(offs).to(dev)
+    t = torch.from_numpy(np.require(vals, requirements=["C", "W"])).to(dev)
+    if t.numel() == 0:  # keep a valid pointer
+        t = torch.zeros(1, dtype=t.dtype, device=dev)
+    return FeatureColumn(name, kind, t, tail, pad, list_offsets)
+
+
+def _column_from_sequences(name, col, item_lengths, padding_value, list_width, device):
+    """One raw column: a per-sequence list of 1-D integer / float arrays (scalars), ``[n, dim]`` float arrays (vectors)
+    or lists of integer lists (lists; ``[n, k]`` integer arrays count as lists of k entries)."""
+    if len(col) != len(item_lengths):
+        raise ValueError(f"feature {name!r}: {len(col)} sequences, the store has {len(item_lengths)}")
+    seq_lengths, parts, nested = [], [], False
+    for x in col:
+        try:
+            a = np.asarray(x)
+        except ValueError:  # ragged nested lists
+            a = None
+        if a is None or a.dtype == object:
+            nested = True
+            a = list(x)
+        seq_lengths.append(len(a))
+        parts.append(a)
+    if not nested:
+        live = [a for a in parts if len(a)]
+        kinds = {a.dtype.kind for a in live}
+        if kinds - set("biuf"):
+            raise ValueError(f"feature {name!r}: unsupported dtype {sorted(kinds)}")
+        ndims = {a.ndim for a in live}
+        if len(ndims) > 1 or (ndims and ndims.pop() > 2):
+            raise ValueError(f"feature {name!r}: events must all be scalars or all be vectors")
+        two_d = bool(live) and live[0].ndim == 2
+        is_float = "f" in kinds
+        if not two_d:
+            values = np.concatenate(live) if live else np.zeros(0, np.float32 if is_float else np.int64)
+            if is_float:
+                values = values.astype(_float_dtype(a.dtype for a in live if a.dtype.kind == "f"))
+                return _make_column(name, "float", values, seq_lengths, item_lengths, padding_value, device=device)
+            return _make_column(name, "int", values.astype(np.int64), seq_lengths, item_lengths, padding_value,
+                                device=device)
+        dims = {a.shape[1] for a in live}
+        if is_float:
+            if len(dims) > 1:
+                raise ValueError(f"feature {name!r}: ragged vectors (dims {sorted(dims)})")
+            values = np.concatenate([a.reshape(-1) for a in live])
+            values = values.astype(_float_dtype(a.dtype for a in live if a.dtype.kind == "f"))
+            return _make_column(name, "float", values, seq_lengths, item_lengths, padding_value, dim=dims.pop(),
+                                device=device)
+        ev_len = np.concatenate([np.full(len(a), a.shape[1], np.int64) for a in live])
+        return _make_column(name, "list", np.concatenate([a.reshape(-1) for a in live]), seq_lengths, item_lengths,
+                            padding_value, event_lengths=ev_len, list_width=list_width, device=device)
+    # nested: one list per event
+    ev_len, flat, is_float, scalar_events = [], [], False, False
+    for a in parts:
+        for e in a:
+            ev = None if e is None else np.asarray(e)
+            if ev is None or ev.dtype == object:
+                raise ValueError(f"feature {name!r} holds null values")
+            if ev.ndim != 1:
+                scalar_events = True
+                continue
+            if len(ev) and ev.dtype.kind not in "biuf":
+                raise ValueError(f"feature {name!r}: unsupported dtype {ev.dtype}")
+            is_float |= len(ev) > 0 and ev.dtype.kind == "f"
+            ev_len.append(len(ev))
+            flat.append(ev)
+    if scalar_events:
+        raise ValueError(f"feature {name!r}: mixes scalar and list events")
+    ev_len = np.asarray(ev_len, dtype=np.int64)
+    if is_float:
+        if len(set(ev_len.tolist())) > 1:
+            raise ValueError(f"feature {name!r}: ragged vectors (dims {sorted(set(ev_len.tolist()))})")
+        values = np.concatenate(flat).astype(_float_dtype(f.dtype for f in flat if len(f)))
+        return _make_column(name, "float", values, seq_lengths, item_lengths, padding_value, dim=int(ev_len[0]),
+                            device=device)
+    values = np.concatenate(flat).astype(np.int64) if flat else np.zeros(0, np.int64)
+    return _make_column(name, "list", values, seq_lengths, item_lengths, padding_value, event_lengths=ev_len,
+                        list_width=list_width, device=device)
+
+
+def _column_from_arrow(name, col, item_lengths, padding_value, list_width, device):
+    """A ``list<T>`` (scalars) or ``list<list<T>>`` / ``list<fixed_size_list<T>>`` (float vectors, integer lists) arrow
+    column, read with pyarrow compute: null rows count as empty like the item column's, null events or values raise."""
+    import pyarrow as pa
+    import pyarrow.compute as pc
+
+    if not (pa.types.is_list(col.type) or pa.types.is_large_list(col.type)):
+        raise ValueError(f"column {name!r} must be a list column, got {col.type}")
+    seq_lengths = pc.fill_null(pc.list_value_length(col), 0).to_numpy(zero_copy_only=False).astype(np.int64)
+    events = pc.list_flatten(col)
+    if events.null_count:
+        raise ValueError(f"column {name!r} holds null values")
+    t = events.type
+    nested = pa.types.is_list(t) or pa.types.is_large_list(t) or pa.types.is_fixed_size_list(t)
+    if nested:
+        ev_len = pc.list_value_length(events).to_numpy(zero_copy_only=False).astype(np.int64)
+        values = pc.list_flatten(events)
+        t = values.type
+    else:
+        values = events
+    if values.null_count:
+        raise ValueError(f"column {name!r} holds null values")
+    if not (pa.types.is_integer(t) or pa.types.is_floating(t)):
+        raise ValueError(f"column {name!r}: unsupported value type {t}")
+    vals = values.to_numpy(zero_copy_only=False)
+    if pa.types.is_floating(t):
+        vals = vals.astype(_float_dtype([vals.dtype]))
+        dim = None
+        if nested:
+            dims = np.unique(ev_len)
+            if len(dims) > 1:
+                raise ValueError(f"column {name!r}: ragged vectors (dims {dims.tolist()})")
+            dim = int(dims[0]) if len(dims) else (events.type.list_size if pa.types.is_fixed_size_list(events.type) else 1)
+        return _make_column(name, "float", vals, seq_lengths, item_lengths, padding_value, dim=dim, device=device)
+    if nested:
+        return _make_column(name, "list", vals, seq_lengths, item_lengths, padding_value, event_lengths=ev_len,
+                            list_width=list_width, device=device)
+    return _make_column(name, "int", vals, seq_lengths, item_lengths, padding_value, device=device)
 
 
 def window_index(lengths, window: int, sliding_window_step: int | None = None):
@@ -41,9 +224,17 @@ def window_index(lengths, window: int, sliding_window_step: int | None = None):
 
 class DeviceSequenceStore:
     """CSR store of item-id histories in HBM.  ``sequences``: list of 1-D integer arrays (one per query, item ids already
-    label-encoded to 0..|I|-1 as the reference's SequenceTokenizer does), or pass ``offsets``/``items`` directly."""
+    label-encoded to 0..|I|-1 as the reference's SequenceTokenizer does), or pass ``offsets``/``items`` directly.
 
-    def __init__(self, sequences=None, *, offsets=None, items=None, query_ids=None, device="cuda"):
+    ``features``: ``{name: column}``, each column one entry per sequence with one entry per event of that sequence: a
+    1-D integer or float array (scalars), an ``[n, dim]`` float array or list of equal-length float lists (vectors), or a
+    list of integer lists of any length (lists).  ``padding_values``: ``{name: value}`` (default 0); ``list_widths``:
+    ``{name: K}``, the output width of a list column (default: its longest list).  ValueError for a column whose
+    per-sequence lengths differ from the item column's, ragged vectors, null values, ``K < 1`` or more than
+    ``BATCH_MAX_COLUMNS`` (16) columns."""
+
+    def __init__(self, sequences=None, *, offsets=None, items=None, query_ids=None, device="cuda", features=None,
+                 padding_values=None, list_widths=None):
         if sequences is not None:
             lens = np.fromiter((len(s) for s in sequences), dtype=np.int64, count=len(sequences))
             offsets = np.zeros(len(lens) + 1, dtype=np.int64)
@@ -63,27 +254,51 @@ class DeviceSequenceStore:
         if len(items) == 0:  # keep a valid pointer
             self.items = torch.zeros(1, dtype=torch.int32, device=self.device)
         self.query_ids = None if query_ids is None else torch.from_numpy(np.array(query_ids, dtype=np.int64)).to(self.device)
+        features = dict(features or {})
+        self._check_column_count(len(features))
+        padding_values, list_widths = dict(padding_values or {}), dict(list_widths or {})
+        self.columns = [c if isinstance(c, FeatureColumn) else
+                        _column_from_sequences(n, c, self.lengths, padding_values.get(n, 0), list_widths.get(n), self.device)
+                        for n, c in features.items()]
+
+    @staticmethod
+    def _check_column_count(n):
+        if n > BATCH_MAX_COLUMNS:
+            raise ValueError(f"{n} feature columns: one batch launch takes at most {BATCH_MAX_COLUMNS}")
+
+    @property
+    def feature_names(self):
+        return [c.name for c in self.columns]
 
     @classmethod
-    def from_sequential_dataset(cls, sequential, feature_name: str | None = None, device="cuda"):
+    def from_sequential_dataset(cls, sequential, feature_name: str | None = None, device="cuda", list_widths=None):
         """Duck-typed ``SequentialDataset`` (replay/data/nn/sequential_dataset.py:18-105): ``__len__``, ``get_query_id``,
-        ``get_sequence`` and ``schema.item_id_feature_name``."""
-        name = feature_name or sequential.schema.item_id_feature_name
+        ``get_sequence`` and ``schema``.  Every other ``is_seq`` feature of the schema becomes a feature column with the
+        schema's ``padding_value``; per-query (non-sequential) features are not read."""
+        schema = sequential.schema
+        name = feature_name or schema.item_id_feature_name
         n = len(sequential)
+        side = [(k, f) for k, f in schema.items() if k != name and getattr(f, "is_seq", True)]
         return cls([np.asarray(sequential.get_sequence(i, name)) for i in range(n)],
-                   query_ids=[sequential.get_query_id(i) for i in range(n)], device=device)
+                   query_ids=[sequential.get_query_id(i) for i in range(n)], device=device,
+                   features={k: [sequential.get_sequence(i, k) for i in range(n)] for k, _ in side},
+                   padding_values={k: getattr(f, "padding_value", 0) for k, f in side}, list_widths=list_widths)
 
     @classmethod
-    def from_parquet(cls, source, item_column: str = "item_id", query_column: str | None = None, device="cuda"):
+    def from_parquet(cls, source, item_column: str = "item_id", query_column: str | None = None, device="cuda",
+                     feature_columns=(), padding_values=None, list_widths=None):
         """Sequence-per-row parquet (the layout the reference's ParquetDataset / ParquetModule reads: one row per query, the
         item ids in a list<int> column; replay/data/nn/parquet/impl/array_1d_column.py:87-140): the list column's offsets and
         flat values become the CSR store without a Python loop (null lists count as empty).  ``source``: a path, a list of
-        paths or a ``pyarrow.Table``."""
+        paths or a ``pyarrow.Table``.  ``feature_columns``: ``list<T>`` (scalars) and ``list<list<T>>`` (float vectors,
+        integer lists) columns read the same way, with ``padding_values`` / ``list_widths`` as in the constructor."""
         import pyarrow as pa
         import pyarrow.compute as pc
         import pyarrow.parquet as pq
 
-        cols = [item_column] + ([query_column] if query_column else [])
+        feature_columns = list(feature_columns)
+        cls._check_column_count(len(feature_columns))
+        cols = [item_column] + ([query_column] if query_column else []) + feature_columns
         if isinstance(source, pa.Table):
             table = source.select(cols)
         elif isinstance(source, (list, tuple)):
@@ -100,14 +315,19 @@ class DeviceSequenceStore:
         offsets = np.zeros(len(lengths) + 1, dtype=np.int64)
         np.cumsum(lengths, out=offsets[1:])
         q = table.column(query_column).combine_chunks().to_numpy(zero_copy_only=False) if query_column else None
-        return cls(offsets=offsets, items=values.to_numpy(zero_copy_only=False), query_ids=q, device=device)
+        padding_values, list_widths = dict(padding_values or {}), dict(list_widths or {})
+        feats = {n: _column_from_arrow(n, table.column(n).combine_chunks(), lengths, padding_values.get(n, 0),
+                                       list_widths.get(n), device) for n in feature_columns}
+        return cls(offsets=offsets, items=values.to_numpy(zero_copy_only=False), query_ids=q, device=device, features=feats)
 
     def __len__(self):
         return self.n_seq
 
     # --------------------------------------------------------------------------------------------- batch builders
     def _build(self, mode, seq_index, seq_offset, L, pad_value, *, mask_prob=0.0, uniforms=None, seed=0, draw0=0,
-               with_labels=False, with_aux=False):
+               with_labels=False, with_aux=False, new_path=False, feature_name="item_id"):
+        """ids, pad, labels, aux, query [B, 1] and ``{name: tensor}`` of the feature columns (empty for an item-only
+        store, which runs the item-only launch)."""
         dev = self.device
         seq_index = torch.as_tensor(seq_index, device=dev).to(torch.int32).contiguous()
         B = seq_index.numel()
@@ -125,66 +345,119 @@ class DeviceSequenceStore:
             if tuple(uniforms.shape) != (B, L):
                 raise ValueError("uniforms must be [B, L]")
         p = lambda t: None if t is None else t.data_ptr()  # noqa: E731
-        check(lib().rp_build_batch(self.offsets.data_ptr(), self.items.data_ptr(), self.n_seq, seq_index.data_ptr(),
-                                   p(seq_offset), B, L, mode, int(pad_value), float(mask_prob), p(uniforms), int(seed),
-                                   int(draw0), p(self.query_ids), ids.data_ptr(), pad.data_ptr(), p(labels), p(aux),
-                                   q.data_ptr(), torch.cuda.current_stream().cuda_stream), "rp_build_batch")
-        return ids, pad, labels, aux, q.view(-1, 1)
+        args = (self.offsets.data_ptr(), self.items.data_ptr(), self.n_seq, seq_index.data_ptr(), p(seq_offset), B, L, mode,
+                int(pad_value), float(mask_prob), p(uniforms), int(seed), int(draw0), p(self.query_ids), ids.data_ptr(),
+                pad.data_ptr(), p(labels), p(aux), q.data_ptr())
+        stream = torch.cuda.current_stream().cuda_stream
+        if not self.columns:
+            check(lib().rp_build_batch(*args, stream), "rp_build_batch")
+            return ids, pad, labels, aux, q.view(-1, 1), {}
+        feats, desc = self._feature_outputs(B, L, new_path, feature_name)
+        check(lib().rp_build_batch_features(*args, desc, len(desc), stream), "rp_build_batch_features")
+        return ids, pad, labels, aux, q.view(-1, 1), feats
+
+    def _feature_outputs(self, B, L, new_path, feature_name):
+        if feature_name in self.feature_names:
+            raise ValueError(f"feature column {feature_name!r} has the item feature's name")
+        if not new_path:
+            lists = [c.name for c in self.columns if c.kind == "list"]
+            if lists:
+                raise ValueError(f"list features {lists} need the new-path builders: the legacy datasets stack one tensor "
+                                 "per feature and cannot stack ragged lists")
+        feats, desc = {}, (BatchColumn * len(self.columns))()
+        for c, d in zip(self.columns, desc):
+            if c.kind == "float":
+                dt = c.values.dtype if new_path else torch.float32
+            else:
+                dt = torch.int64
+            out = torch.empty((B, L, *c.tail), dtype=dt, device=self.device)
+            feats[c.name] = out
+            d.kind = {"int": BATCH_COL_INT, "float": BATCH_COL_FLOAT, "list": BATCH_COL_LIST}[c.kind]
+            d.in_bytes, d.out_bytes, d.width = c.values.element_size(), out.element_size(), c.width
+            d.values, d.out = c.values.data_ptr(), out.data_ptr()
+            d.list_offsets = None if c.list_offsets is None else c.list_offsets.data_ptr()
+            if c.kind == "float":
+                d.pad_float = float(c.padding_value)
+            else:
+                d.pad_int = int(c.padding_value)
+        return feats, desc
 
     def sasrec_training_batch(self, seq_index, max_len: int, pad_value: int, seq_offset=None, feature_name="item_id"):
-        """Reference keys (sasrec/dataset.py:120-126): query_id [B,1], feature_tensor{item_id [B,L]}, padding_mask,
-        positive_labels, target_padding_mask - all on the device."""
-        ids, pad, labels, tmask, q = self._build(SASREC_TRAIN, seq_index, seq_offset, max_len, pad_value, with_labels=True,
-                                                 with_aux=True)
-        return {"query_id": q, "feature_tensor": {feature_name: ids}, "padding_mask": pad, "positive_labels": labels,
+        """Reference keys (sasrec/dataset.py:120-126): query_id [B,1], feature_tensor{item_id [B,L], features...},
+        padding_mask, positive_labels, target_padding_mask - all on the device."""
+        ids, pad, labels, tmask, q, feats = self._build(SASREC_TRAIN, seq_index, seq_offset, max_len, pad_value,
+                                                        with_labels=True, with_aux=True, feature_name=feature_name)
+        return {"query_id": q, "feature_tensor": {feature_name: ids, **feats}, "padding_mask": pad, "positive_labels": labels,
                 "target_padding_mask": tmask}
 
-    def sasrec_new_path_batch(self, seq_index, max_len: int, pad_value: int, feature_name="item_id", with_seen: bool = True):
+    def sasrec_new_path_batch(self, seq_index, max_len: int, pad_value: int, feature_name="item_id", with_seen: bool = True,
+                              seq_offset=None):
         """The new path's model inputs: Array1DColumn.__getitem__ with shape max_len + 1 (left-padded gather of the last
-        elements, parquet/impl/indexing.py:42-78) + NextTokenTransform(shift=1) (nn/transform/next_token.py:65-96) +
-        the unsqueeze of the default SASRec transform template -> feature_tensors, padding_mask, positive_labels [B,L,1],
-        target_padding_mask [B,L,1] (+ seen_ids = the window)."""
-        ids, pad, labels, tmask, q = self._build(SASREC_TRAIN, seq_index, None, max_len, pad_value, with_labels=True,
-                                                 with_aux=True)
-        out = {"query_id": q, "feature_tensors": {feature_name: ids}, "padding_mask": pad,
+        elements, parquet/impl/indexing.py:42-78; Array2DColumn.__getitem__ for lists, array_2d_column.py:72-92) +
+        NextTokenTransform(shift=1) (nn/transform/next_token.py:65-96) + the unsqueeze of the default SASRec transform
+        template -> feature_tensors{item_id, features...}, padding_mask, positive_labels [B,L,1], target_padding_mask
+        [B,L,1] (+ seen_ids = the window).  ``seq_offset``: window starts (default: the last L + 1 events)."""
+        ids, pad, labels, tmask, q, feats = self._build(SASREC_TRAIN, seq_index, seq_offset, max_len, pad_value,
+                                                        with_labels=True, with_aux=True, new_path=True,
+                                                        feature_name=feature_name)
+        out = {"query_id": q, "feature_tensors": {feature_name: ids, **feats}, "padding_mask": pad,
                "positive_labels": labels.unsqueeze(-1), "target_padding_mask": tmask.unsqueeze(-1)}
         if with_seen:
             out["seen_ids"] = ids
         return out
 
+    def sasrec_new_path_prediction_batch(self, seq_index, max_len: int, pad_value: int, feature_name="item_id",
+                                         with_seen: bool = True):
+        """The predict transforms of the default SASRec template (nn/transform/template/sasrec.py): every column read at
+        max_len (the last events, left-padded), no shift -> query_id, feature_tensors{item_id, features...}, padding_mask
+        (+ seen_ids = the window)."""
+        ids, pad, _, _, q, feats = self._build(PREDICT, seq_index, None, max_len, pad_value, new_path=True,
+                                               feature_name=feature_name)
+        out = {"query_id": q, "feature_tensors": {feature_name: ids, **feats}, "padding_mask": pad}
+        if with_seen:
+            out["seen_ids"] = ids
+        return out
+
     def sasrec_prediction_batch(self, seq_index, max_len: int, pad_value: int, feature_name="item_id"):
-        ids, pad, _, _, q = self._build(PREDICT, seq_index, None, max_len, pad_value)
-        return {"query_id": q, "padding_mask": pad, "feature_tensor": {feature_name: ids}}
+        ids, pad, _, _, q, feats = self._build(PREDICT, seq_index, None, max_len, pad_value, feature_name=feature_name)
+        return {"query_id": q, "padding_mask": pad, "feature_tensor": {feature_name: ids, **feats}}
 
     def bert4rec_training_batch(self, seq_index, max_len: int, pad_value: int, mask_prob: float = 0.15, seq_offset=None,
                                 seed: int = 0, draw0: int = 0, uniforms=None, feature_name="item_id"):
-        """Reference keys (bert4rec/dataset.py:167-173).  ``token_mask`` False = masked.  Random draws: Philox keyed by
-        (seed, draw0 + row); pass ``uniforms`` [B, L] to reproduce a given masker stream exactly."""
-        ids, pad, labels, tok, q = self._build(BERT_TRAIN, seq_index, seq_offset, max_len, pad_value, mask_prob=mask_prob,
-                                               uniforms=uniforms, seed=seed, draw0=draw0, with_labels=True, with_aux=True)
-        return {"query_id": q, "pad_mask": pad, "inputs": {feature_name: ids}, "token_mask": tok, "positive_labels": labels}
+        """Reference keys (bert4rec/dataset.py:167-173), the feature columns unmasked under ``inputs``.  ``token_mask``
+        False = masked.  Random draws: Philox keyed by (seed, draw0 + row); pass ``uniforms`` [B, L] to reproduce a given
+        masker stream exactly."""
+        ids, pad, labels, tok, q, feats = self._build(BERT_TRAIN, seq_index, seq_offset, max_len, pad_value,
+                                                      mask_prob=mask_prob, uniforms=uniforms, seed=seed, draw0=draw0,
+                                                      with_labels=True, with_aux=True, feature_name=feature_name)
+        return {"query_id": q, "pad_mask": pad, "inputs": {feature_name: ids, **feats}, "token_mask": tok,
+                "positive_labels": labels}
 
     def bert4rec_prediction_batch(self, seq_index, max_len: int, pad_value: int, feature_name="item_id"):
-        ids, pad, _, tok, q = self._build(BERT_PREDICT, seq_index, None, max_len, pad_value, with_aux=True)
-        return {"query_id": q, "pad_mask": pad, "inputs": {feature_name: ids}, "token_mask": tok}
+        """_shift_features (bert4rec/dataset.py:322-351): every column shifted left, its padding value in the last slot."""
+        ids, pad, _, tok, q, feats = self._build(BERT_PREDICT, seq_index, None, max_len, pad_value, with_aux=True,
+                                                 feature_name=feature_name)
+        return {"query_id": q, "pad_mask": pad, "inputs": {feature_name: ids, **feats}, "token_mask": tok}
 
 
 class DeviceBatchLoader:
     """Iterates device-built training batches the way ``DataLoader(SasRecTrainingDataset(...), shuffle=True)`` +
     ``DistributedSampler`` would: the window index is built once (host, vectorised), permuted per epoch with a seeded
     generator shared by all ranks, padded by wrap-around to a multiple of the world size (DistributedSampler semantics) and
-    strided over the ranks; every batch is then one kernel launch on HBM-resident data."""
+    strided over the ranks; every batch is then one kernel launch on HBM-resident data.  ``kind``: ``"sasrec"`` (the
+    legacy SasRec's batches), ``"sasrec_new"`` (new-path training batches for ``LightningModule(SasRec | TwoTower)``) or
+    ``"bert4rec"``."""
 
     def __init__(self, store: DeviceSequenceStore, max_len: int, batch_size: int, pad_value: int, kind: str = "sasrec",
                  sliding_window_step: int | None = None, shuffle: bool = True, drop_last: bool = False, seed: int = 0,
                  rank: int = 0, world_size: int = 1, mask_prob: float = 0.15, partitioning: str = "sampler"):
-        if kind not in ("sasrec", "bert4rec"):
+        if kind not in ("sasrec", "sasrec_new", "bert4rec"):
             raise ValueError(f"unknown kind {kind!r}")
         if partitioning not in ("sampler", "replay"):
             raise ValueError(f"unknown partitioning {partitioning!r}")
         self.partitioning = partitioning
         self.store, self.L, self.bs, self.pad, self.kind = store, int(max_len), int(batch_size), int(pad_value), kind
-        window = self.L + (1 if kind == "sasrec" else 0)
+        window = self.L + (1 if kind in ("sasrec", "sasrec_new") else 0)
         seq, off = window_index(store.lengths, window, sliding_window_step)
         self.win_seq = torch.from_numpy(seq).to(store.device)
         self.win_off = torch.from_numpy(off).to(store.device)
@@ -228,6 +501,8 @@ class DeviceBatchLoader:
             s, o = self.win_seq[idx], self.win_off[idx]
             if self.kind == "sasrec":
                 yield self.store.sasrec_training_batch(s, self.L, self.pad, seq_offset=o)
+            elif self.kind == "sasrec_new":
+                yield self.store.sasrec_new_path_batch(s, self.L, self.pad, seq_offset=o)
             else:
                 draw0 = (self.epoch * self.per_rank * self.world) + self.rank * self.per_rank + i * self.bs
                 yield self.store.bert4rec_training_batch(s, self.L, self.pad, self.mask_prob, seq_offset=o,
