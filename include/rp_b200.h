@@ -701,14 +701,25 @@ int rp_build_batch(const int64_t* offsets, const int32_t* items, long long n_seq
  *                      value (Array2DColumn.__getitem__, replay/data/nn/parquet/impl/array_2d_column.py:72-92)
  * Every column uses the ids' window, offset and shift: a position that is padding in the ids (and the last position of
  * RP_BATCH_BERT_PREDICT) is pad_int / pad_float in every element.  Integer outputs take pad_int, float outputs pad_float
- * converted to the output type.  At most RP_BATCH_MAX_COLUMNS columns.  Other arguments as rp_build_batch, which this
- * call runs in the same kernel; n_cols == 0 is rp_build_batch.  RP_EINVAL: null pointer, unknown kind, byte widths
- * other than 4 / 8 (int out_bytes must be 8), width < 1, n_cols outside [0, RP_BATCH_MAX_COLUMNS].  No host
- * synchronisation: the descriptors are passed by value to the kernel. */
+ * converted to the output type.
+ * Query lists hold one integer list per stored history instead of one entry per event (a user's ground-truth or train
+ * items): list_offsets [n_seq + 1] into values (int32 / int64), out int64 [B, width] from the list of seq_index[b],
+ * independent of the window and of every mode's shift:
+ *   RP_BATCH_COL_QUERY_LIST       the list's FIRST `width` entries, right-padded with pad_int
+ *                                 (TorchSequentialValidationDataset._get_ground_truth / _get_train,
+ *                                 replay/data/nn/torch_sequential_dataset.py:263-285)
+ *   RP_BATCH_COL_QUERY_LIST_LAST  the list's LAST `width` entries, left-padded with pad_int (Array1DColumn.__getitem__,
+ *                                 replay/data/nn/parquet/impl/array_1d_column.py:70-84, indexing.py:42-78)
+ * At most RP_BATCH_MAX_COLUMNS columns of all kinds together.  Other arguments as rp_build_batch, which this call runs in
+ * the same kernel; n_cols == 0 is rp_build_batch.  RP_EINVAL: null pointer, unknown kind, byte widths other than 4 / 8
+ * (integer out_bytes must be 8), width < 1, n_cols outside [0, RP_BATCH_MAX_COLUMNS].  No host synchronisation: the
+ * descriptors are passed by value to the kernel. */
 #define RP_BATCH_MAX_COLUMNS 16
 #define RP_BATCH_COL_INT 0
 #define RP_BATCH_COL_FLOAT 1
 #define RP_BATCH_COL_LIST 2
+#define RP_BATCH_COL_QUERY_LIST 3
+#define RP_BATCH_COL_QUERY_LIST_LAST 4
 typedef struct rp_batch_column {
   int kind, in_bytes, out_bytes, width;
   const void* values;

@@ -294,7 +294,7 @@ class BatchColumn(ctypes.Structure):
     ]
 
 
-BATCH_COL_INT, BATCH_COL_FLOAT, BATCH_COL_LIST = range(3)   # rp_batch_column.kind
+BATCH_COL_INT, BATCH_COL_FLOAT, BATCH_COL_LIST, BATCH_COL_QUERY_LIST, BATCH_COL_QUERY_LIST_LAST = range(5)   # .kind
 BATCH_MAX_COLUMNS = 16   # RP_BATCH_MAX_COLUMNS: most feature columns one batch launch takes
 
 

@@ -15,7 +15,8 @@
 // rp_build_batch_features adds the store's feature columns (one entry per event, aligned with the item ids) to the same
 // launch: after the row's ids, every column's [L(, width)] slab of the row is written through the same window, offset and
 // shift, with the column's own padding value.  Loads and stores run along the flattened (position, element) axis, so
-// consecutive threads touch consecutive events' values.
+// consecutive threads touch consecutive events' values.  Query lists (one list per history: ground-truth and train items
+// of validation batches) ride in the same launch as [width] rows read by the row's history index.
 #include "rp_b200.h"
 #include "rp_host.h"
 #include "rp_philox.cuh"
@@ -186,6 +187,27 @@ __device__ __forceinline__ void copy_list(const rp_batch_column& c, const RowWin
   }
 }
 
+// query lists: one list per history, cut by the row's history index alone; head = first entries right-padded (legacy),
+// else last entries left-padded (new path)
+template <typename In>
+__device__ __forceinline__ void copy_query_list(const rp_batch_column& c, int s, size_t row, bool head) {
+  const In* __restrict__ v = reinterpret_cast<const In*>(c.values);
+  const int K = c.width;
+  int64_t* out = reinterpret_cast<int64_t*>(c.out) + row * (size_t)K;
+  const long long lo = c.list_offsets[s], hi = c.list_offsets[s + 1];
+  const int m = (int)min(hi - lo, (long long)K);
+  for (int j = threadIdx.x; j < K; j += blockDim.x) {
+    int64_t x = (int64_t)c.pad_int;
+    if (head) {
+      if (j < m) x = (int64_t)v[lo + j];
+    } else {
+      const int kk = j - (K - m);
+      if (kk >= 0) x = (int64_t)v[hi - m + kk];
+    }
+    out[j] = x;
+  }
+}
+
 __global__ void __launch_bounds__(128) build_batch_features_kernel(const BatchArgs a, const ColumnArgs cols) {
   const int b = blockIdx.x;
   build_row(a, b);
@@ -214,9 +236,13 @@ __global__ void __launch_bounds__(128) build_batch_features_kernel(const BatchAr
         if (c.out_bytes == 4) copy_dense<double, float>(c, w, b);
         else copy_dense<double, double>(c, w, b);
       }
-    } else {
+    } else if (c.kind == RP_BATCH_COL_LIST) {
       if (c.in_bytes == 4) copy_list<int32_t>(c, w, b);
       else copy_list<int64_t>(c, w, b);
+    } else {
+      const bool head = c.kind == RP_BATCH_COL_QUERY_LIST;
+      if (c.in_bytes == 4) copy_query_list<int32_t>(c, s, b, head);
+      else copy_query_list<int64_t>(c, s, b, head);
     }
   }
 }
@@ -272,8 +298,10 @@ RP_API int rp_build_batch_features(const int64_t* offsets, const int32_t* items,
     if (!c.values || !c.out || c.width < 1) return RP_EINVAL;
     if ((c.in_bytes != 4 && c.in_bytes != 8) || (c.out_bytes != 4 && c.out_bytes != 8)) return RP_EINVAL;
     if (c.kind == RP_BATCH_COL_INT && (c.out_bytes != 8 || c.width != 1)) return RP_EINVAL;
-    if (c.kind == RP_BATCH_COL_LIST && (c.out_bytes != 8 || !c.list_offsets)) return RP_EINVAL;
-    if (c.kind != RP_BATCH_COL_INT && c.kind != RP_BATCH_COL_FLOAT && c.kind != RP_BATCH_COL_LIST) return RP_EINVAL;
+    const bool lists = c.kind == RP_BATCH_COL_LIST || c.kind == RP_BATCH_COL_QUERY_LIST ||
+                       c.kind == RP_BATCH_COL_QUERY_LIST_LAST;
+    if (lists && (c.out_bytes != 8 || !c.list_offsets)) return RP_EINVAL;
+    if (c.kind != RP_BATCH_COL_INT && c.kind != RP_BATCH_COL_FLOAT && !lists) return RP_EINVAL;
     ca.c[i] = c;
   }
   return launch_batch(offsets, items, n_seq, seq_index, seq_offset, B, L, mode, pad_value, mask_prob, uniforms, seed, draw0,

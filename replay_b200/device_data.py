@@ -14,16 +14,27 @@ with its own padding value.  Four kinds: an integer scalar (stored as int32 when
 scalar (stored in its source dtype, float32 or float64), a float vector of one ``dim`` for every event (``[n_events,
 dim]``) and an integer list of any length per event (a second level of offsets plus flat values; output width ``K``).
 Legacy builders emit every integer as int64 and every float as float32 (TorchSequentialDataset._get_tensor_dtype); the
-new-path builders emit integers as int64 and keep each float column's dtype."""
+new-path builders emit integers as int64 and keep each float column's dtype.
+
+Query lists hold one integer list per stored sequence instead of one entry per event: the ground-truth and train items of
+a validation or test user (``TorchSequentialValidationDataset``, replay/data/nn/torch_sequential_dataset.py:183-285).
+They are stored as CSR (int64 offsets, int32 values when every value fits, else int64) and cut in the same launch as
+int64 ``[B, width]``: the legacy validation builders take each list's first ``width`` entries right-padded (``width`` is
+the dataset-wide longest list, as the reference's placeholders are), the new path's take its last ``width`` entries
+left-padded (Array1DColumn.__getitem__, replay/data/nn/parquet/impl/array_1d_column.py:70-84)."""
 from __future__ import annotations
 
 import numpy as np
 import torch
 
-from ._lib import BATCH_COL_FLOAT, BATCH_COL_INT, BATCH_COL_LIST, BATCH_MAX_COLUMNS, BatchColumn, check, lib
+from ._lib import (BATCH_COL_FLOAT, BATCH_COL_INT, BATCH_COL_LIST, BATCH_COL_QUERY_LIST, BATCH_COL_QUERY_LIST_LAST,
+                   BATCH_MAX_COLUMNS, BatchColumn, check, lib)
 
 SASREC_TRAIN, PREDICT, BERT_TRAIN, BERT_PREDICT = 0, 1, 2, 3
 _INT32 = np.iinfo(np.int32)
+# DEFAULT_GROUND_TRUTH_PADDING_VALUE / DEFAULT_TRAIN_PADDING_VALUE (torch_sequential_dataset.py:179-180); other query
+# lists default to -1, which no item id, metric or seen filter takes for an item
+QUERY_LIST_PADDING = {"ground_truth": -1, "train": -2}
 
 
 class FeatureColumn:
@@ -36,6 +47,47 @@ class FeatureColumn:
         self.values = values
         self.padding_value = padding_value
         self.width = int(np.prod(self.tail)) if self.tail else 1
+
+
+class QueryList:
+    """One integer list per stored sequence of a ``DeviceSequenceStore``: ``offsets`` int64 ``[n_seq + 1]`` into
+    ``values`` (int32 or int64) on the store's device; ``width``: the output width; ``padding_value``: the pad of both
+    layouts."""
+
+    def __init__(self, name, values, offsets, width, padding_value):
+        self.name, self.values, self.offsets = name, values, offsets
+        self.width, self.padding_value = int(width), int(padding_value)
+
+
+def _make_query_list(name, values, lengths, n_seq, width, padding_value, device):
+    """``values``: the lists concatenated; ``lengths``: entries per stored sequence.  ``width`` None: the longest list."""
+    lengths = np.asarray(lengths, dtype=np.int64)
+    if len(lengths) != n_seq:
+        raise ValueError(f"query list {name!r}: {len(lengths)} lists, the store has {n_seq} sequences")
+    if width is None:
+        width = max(1, int(lengths.max())) if len(lengths) else 1
+    if int(width) < 1:
+        raise ValueError(f"query list {name!r}: width must be >= 1, got {width}")
+    if padding_value is None:
+        padding_value = QUERY_LIST_PADDING.get(name, -1)
+    dev = torch.device(device)
+    offs = np.zeros(n_seq + 1, dtype=np.int64)
+    np.cumsum(lengths, out=offs[1:])
+    t = torch.from_numpy(np.require(_narrow_int(values), requirements=["C", "W"])).to(dev)
+    if t.numel() == 0:  # keep a valid pointer
+        t = torch.zeros(1, dtype=t.dtype, device=dev)
+    return QueryList(name, t, torch.from_numpy(offs).to(dev), width, padding_value)
+
+
+def _query_list_from_sequences(name, lists, n_seq, width, padding_value, device):
+    parts = []
+    for x in lists:
+        a = np.asarray(x)
+        if a.ndim != 1 or (len(a) and a.dtype.kind not in "biu"):
+            raise ValueError(f"query list {name!r}: every entry must be a 1-D integer array, got {a.dtype} {a.shape}")
+        parts.append(a.astype(np.int64))
+    values = np.concatenate(parts) if parts else np.zeros(0, np.int64)
+    return _make_query_list(name, values, [len(a) for a in parts], n_seq, width, padding_value, device)
 
 
 def _narrow_int(values: np.ndarray) -> np.ndarray:
@@ -200,6 +252,38 @@ def _column_from_arrow(name, col, item_lengths, padding_value, list_width, devic
     return _make_column(name, "int", vals, seq_lengths, item_lengths, padding_value, device=device)
 
 
+def _check_validation_datasets(sequential, given, label_feature_name):
+    """TorchSequentialValidationDataset.__init__ / _check_if_schema_match (torch_sequential_dataset.py:211-233,
+    288-302), with its messages."""
+    seq_item = sequential.schema.item_id_features.item()
+    for ds in given.values():
+        other = ds.schema.item_id_features.item()
+        if seq_item.name != other.name:
+            raise ValueError("Schema mismatch: item feature name does not match ground truth")
+        if seq_item.cardinality != other.cardinality:
+            raise ValueError("Schema mismatch: item feature cardinality does not match ground truth")
+    gt = given.get("ground_truth")
+    if label_feature_name:
+        for k, ds in given.items():
+            if label_feature_name not in dict(ds.schema.items()):
+                raise ValueError(f"Label feature name not found in {k.replace('_', ' ')} schema")
+        if gt is not None:
+            if not gt.schema[label_feature_name].is_cat:
+                raise ValueError("Label feature must be categorical")
+            if not gt.schema[label_feature_name].is_seq:
+                raise ValueError("Label feature must be sequential")
+    if gt is not None and len(np.intersect1d(sequential.get_all_query_ids(), gt.get_all_query_ids())) == 0:
+        raise ValueError("Sequential data and ground truth must contain the same query IDs")
+
+
+def _join_by_query_id(ds, query_ids, label):
+    """The label sequence of every query id in ``ds`` (empty when absent), looked up once per dataset row."""
+    row = {q: i for i, q in enumerate(np.asarray(ds.get_all_query_ids()).tolist())}
+    empty = np.zeros(0, np.int64)
+    return [np.asarray(ds.get_sequence(row[q], label)) if q in row else empty
+            for q in np.asarray(query_ids).tolist()]
+
+
 def window_index(lengths, window: int, sliding_window_step: int | None = None):
     """(sequence_index int32 [n], offset int32 [n]) in the reference's iteration order
     (TorchSequentialDataset._iter_with_window, torch_sequential_dataset.py:154-171), vectorised: without a step one
@@ -229,12 +313,18 @@ class DeviceSequenceStore:
     ``features``: ``{name: column}``, each column one entry per sequence with one entry per event of that sequence: a
     1-D integer or float array (scalars), an ``[n, dim]`` float array or list of equal-length float lists (vectors), or a
     list of integer lists of any length (lists).  ``padding_values``: ``{name: value}`` (default 0); ``list_widths``:
-    ``{name: K}``, the output width of a list column (default: its longest list).  ValueError for a column whose
-    per-sequence lengths differ from the item column's, ragged vectors, null values, ``K < 1`` or more than
-    ``BATCH_MAX_COLUMNS`` (16) columns."""
+    ``{name: K}``, the output width of a list column (default: its longest list).
+
+    ``query_lists``: ``{name: lists}``, one 1-D integer array per sequence (e.g. ``ground_truth`` and ``train``), emitted
+    by the validation builders.  ``padding_values`` / ``list_widths`` apply to them too; their padding defaults to -1 for
+    ``ground_truth``, -2 for ``train`` (the reference's) and -1 otherwise, their width to the longest list.
+
+    ValueError for a column whose per-sequence lengths differ from the item column's, ragged vectors, null values,
+    ``K < 1``, a query list whose count differs from the store's, or more than ``BATCH_MAX_COLUMNS`` (16) feature columns
+    and query lists together."""
 
     def __init__(self, sequences=None, *, offsets=None, items=None, query_ids=None, device="cuda", features=None,
-                 padding_values=None, list_widths=None):
+                 padding_values=None, list_widths=None, query_lists=None):
         if sequences is not None:
             lens = np.fromiter((len(s) for s in sequences), dtype=np.int64, count=len(sequences))
             offsets = np.zeros(len(lens) + 1, dtype=np.int64)
@@ -254,51 +344,82 @@ class DeviceSequenceStore:
         if len(items) == 0:  # keep a valid pointer
             self.items = torch.zeros(1, dtype=torch.int32, device=self.device)
         self.query_ids = None if query_ids is None else torch.from_numpy(np.array(query_ids, dtype=np.int64)).to(self.device)
-        features = dict(features or {})
-        self._check_column_count(len(features))
+        features, query_lists = dict(features or {}), dict(query_lists or {})
+        self._check_column_count(len(features) + len(query_lists))
+        both = set(features) & set(query_lists)
+        if both:
+            raise ValueError(f"{sorted(both)} are both feature columns and query lists")
         padding_values, list_widths = dict(padding_values or {}), dict(list_widths or {})
         self.columns = [c if isinstance(c, FeatureColumn) else
                         _column_from_sequences(n, c, self.lengths, padding_values.get(n, 0), list_widths.get(n), self.device)
                         for n, c in features.items()]
+        self.query_lists = [c if isinstance(c, QueryList) else
+                            _query_list_from_sequences(n, c, self.n_seq, list_widths.get(n), padding_values.get(n),
+                                                       self.device)
+                            for n, c in query_lists.items()]
 
     @staticmethod
     def _check_column_count(n):
         if n > BATCH_MAX_COLUMNS:
-            raise ValueError(f"{n} feature columns: one batch launch takes at most {BATCH_MAX_COLUMNS}")
+            raise ValueError(f"{n} feature columns and query lists: one batch launch takes at most {BATCH_MAX_COLUMNS}")
 
     @property
     def feature_names(self):
         return [c.name for c in self.columns]
 
+    @property
+    def query_list_names(self):
+        return [c.name for c in self.query_lists]
+
     @classmethod
-    def from_sequential_dataset(cls, sequential, feature_name: str | None = None, device="cuda", list_widths=None):
+    def from_sequential_dataset(cls, sequential, feature_name: str | None = None, device="cuda", list_widths=None,
+                                ground_truth=None, train=None, label_feature_name: str | None = None):
         """Duck-typed ``SequentialDataset`` (replay/data/nn/sequential_dataset.py:18-105): ``__len__``, ``get_query_id``,
         ``get_sequence`` and ``schema``.  Every other ``is_seq`` feature of the schema becomes a feature column with the
-        schema's ``padding_value``; per-query (non-sequential) features are not read."""
+        schema's ``padding_value``; per-query (non-sequential) features are not model inputs and are not read.
+
+        ``ground_truth`` / ``train``: the validation datasets of ``TorchSequentialValidationDataset``
+        (torch_sequential_dataset.py:183-285), joined by query id once, here: each stored query gets the label feature's
+        sequence of its query id as the query list ``ground_truth`` / ``train`` (an empty list when the id is absent, as
+        ``get_sequence_by_query_id`` gives), padded -1 / -2 to the dataset's ``get_max_sequence_length()``.  ValueError,
+        with the reference's messages, for an item feature whose name or cardinality differs from ``sequential``'s, a
+        label feature missing from either schema or not categorical and sequential, and no query id shared with
+        ``ground_truth``."""
         schema = sequential.schema
         name = feature_name or schema.item_id_feature_name
         n = len(sequential)
         side = [(k, f) for k, f in schema.items() if k != name and getattr(f, "is_seq", True)]
-        return cls([np.asarray(sequential.get_sequence(i, name)) for i in range(n)],
-                   query_ids=[sequential.get_query_id(i) for i in range(n)], device=device,
+        qids = [sequential.get_query_id(i) for i in range(n)]
+        lists, widths = {}, dict(list_widths or {})
+        given = {k: v for k, v in (("ground_truth", ground_truth), ("train", train)) if v is not None}
+        if given:
+            _check_validation_datasets(sequential, given, label_feature_name)
+            label = label_feature_name or next(iter(given.values())).schema.item_id_feature_name
+            for k, ds in given.items():
+                lists[k] = _join_by_query_id(ds, qids, label)
+                widths[k] = int(ds.get_max_sequence_length())
+        return cls([np.asarray(sequential.get_sequence(i, name)) for i in range(n)], query_ids=qids, device=device,
                    features={k: [sequential.get_sequence(i, k) for i in range(n)] for k, _ in side},
-                   padding_values={k: getattr(f, "padding_value", 0) for k, f in side}, list_widths=list_widths)
+                   padding_values={k: getattr(f, "padding_value", 0) for k, f in side}, list_widths=widths,
+                   query_lists=lists)
 
     @classmethod
     def from_parquet(cls, source, item_column: str = "item_id", query_column: str | None = None, device="cuda",
-                     feature_columns=(), padding_values=None, list_widths=None):
+                     feature_columns=(), padding_values=None, list_widths=None, query_list_columns=()):
         """Sequence-per-row parquet (the layout the reference's ParquetDataset / ParquetModule reads: one row per query, the
         item ids in a list<int> column; replay/data/nn/parquet/impl/array_1d_column.py:87-140): the list column's offsets and
         flat values become the CSR store without a Python loop (null lists count as empty).  ``source``: a path, a list of
         paths or a ``pyarrow.Table``.  ``feature_columns``: ``list<T>`` (scalars) and ``list<list<T>>`` (float vectors,
-        integer lists) columns read the same way, with ``padding_values`` / ``list_widths`` as in the constructor."""
+        integer lists) columns read the same way, with ``padding_values`` / ``list_widths`` as in the constructor.
+        ``query_list_columns``: ``list<int>`` columns held as query lists (one list per row: ground truth, train or seen
+        items), with the width and padding of the reader's metadata given in ``list_widths`` / ``padding_values``."""
         import pyarrow as pa
         import pyarrow.compute as pc
         import pyarrow.parquet as pq
 
-        feature_columns = list(feature_columns)
-        cls._check_column_count(len(feature_columns))
-        cols = [item_column] + ([query_column] if query_column else []) + feature_columns
+        feature_columns, query_list_columns = list(feature_columns), list(query_list_columns)
+        cls._check_column_count(len(feature_columns) + len(query_list_columns))
+        cols = [item_column] + ([query_column] if query_column else []) + feature_columns + query_list_columns
         if isinstance(source, pa.Table):
             table = source.select(cols)
         elif isinstance(source, (list, tuple)):
@@ -318,16 +439,29 @@ class DeviceSequenceStore:
         padding_values, list_widths = dict(padding_values or {}), dict(list_widths or {})
         feats = {n: _column_from_arrow(n, table.column(n).combine_chunks(), lengths, padding_values.get(n, 0),
                                        list_widths.get(n), device) for n in feature_columns}
-        return cls(offsets=offsets, items=values.to_numpy(zero_copy_only=False), query_ids=q, device=device, features=feats)
+        lists = {}
+        for n in query_list_columns:
+            c = table.column(n).combine_chunks()
+            if not ((pa.types.is_list(c.type) or pa.types.is_large_list(c.type)) and pa.types.is_integer(c.type.value_type)):
+                raise ValueError(f"query list column {n!r} must be a list<int> column, got {c.type}")
+            flat = pc.list_flatten(c)
+            if flat.null_count:
+                raise ValueError(f"query list column {n!r} holds null values")
+            lists[n] = _make_query_list(n, flat.to_numpy(zero_copy_only=False),
+                                        pc.fill_null(pc.list_value_length(c), 0).to_numpy(zero_copy_only=False),
+                                        len(lengths), list_widths.get(n), padding_values.get(n), device)
+        return cls(offsets=offsets, items=values.to_numpy(zero_copy_only=False), query_ids=q, device=device, features=feats,
+                   query_lists=lists)
 
     def __len__(self):
         return self.n_seq
 
     # --------------------------------------------------------------------------------------------- batch builders
     def _build(self, mode, seq_index, seq_offset, L, pad_value, *, mask_prob=0.0, uniforms=None, seed=0, draw0=0,
-               with_labels=False, with_aux=False, new_path=False, feature_name="item_id"):
-        """ids, pad, labels, aux, query [B, 1] and ``{name: tensor}`` of the feature columns (empty for an item-only
-        store, which runs the item-only launch)."""
+               with_labels=False, with_aux=False, new_path=False, feature_name="item_id", query_layout=None):
+        """ids, pad, labels, aux, query [B, 1], ``{name: tensor}`` of the feature columns and ``{name: [B, width]}`` of the
+        query lists (empty unless ``query_layout`` is ``"first"`` (legacy) or ``"last"`` (new path)).  With neither, the
+        item-only launch runs."""
         dev = self.device
         seq_index = torch.as_tensor(seq_index, device=dev).to(torch.int32).contiguous()
         B = seq_index.numel()
@@ -349,12 +483,26 @@ class DeviceSequenceStore:
                 int(pad_value), float(mask_prob), p(uniforms), int(seed), int(draw0), p(self.query_ids), ids.data_ptr(),
                 pad.data_ptr(), p(labels), p(aux), q.data_ptr())
         stream = torch.cuda.current_stream().cuda_stream
-        if not self.columns:
+        if not self.columns and query_layout is None:
             check(lib().rp_build_batch(*args, stream), "rp_build_batch")
-            return ids, pad, labels, aux, q.view(-1, 1), {}
+            return ids, pad, labels, aux, q.view(-1, 1), {}, {}
         feats, desc = self._feature_outputs(B, L, new_path, feature_name)
+        lists, ldesc = self._query_list_outputs(B, query_layout)
+        desc = (BatchColumn * (len(desc) + len(ldesc)))(*desc, *ldesc)
         check(lib().rp_build_batch_features(*args, desc, len(desc), stream), "rp_build_batch_features")
-        return ids, pad, labels, aux, q.view(-1, 1), feats
+        return ids, pad, labels, aux, q.view(-1, 1), feats, lists
+
+    def _query_list_outputs(self, B, layout):
+        if layout is None:
+            return {}, []
+        kind = {"first": BATCH_COL_QUERY_LIST, "last": BATCH_COL_QUERY_LIST_LAST}[layout]
+        lists, desc = {}, []
+        for c in self.query_lists:
+            out = lists[c.name] = torch.empty(B, c.width, dtype=torch.int64, device=self.device)
+            desc.append(BatchColumn(kind=kind, in_bytes=c.values.element_size(), out_bytes=8, width=c.width,
+                                    values=c.values.data_ptr(), list_offsets=c.offsets.data_ptr(), out=out.data_ptr(),
+                                    pad_int=c.padding_value))
+        return lists, desc
 
     def _feature_outputs(self, B, L, new_path, feature_name):
         if feature_name in self.feature_names:
@@ -385,7 +533,7 @@ class DeviceSequenceStore:
     def sasrec_training_batch(self, seq_index, max_len: int, pad_value: int, seq_offset=None, feature_name="item_id"):
         """Reference keys (sasrec/dataset.py:120-126): query_id [B,1], feature_tensor{item_id [B,L], features...},
         padding_mask, positive_labels, target_padding_mask - all on the device."""
-        ids, pad, labels, tmask, q, feats = self._build(SASREC_TRAIN, seq_index, seq_offset, max_len, pad_value,
+        ids, pad, labels, tmask, q, feats, _ = self._build(SASREC_TRAIN, seq_index, seq_offset, max_len, pad_value,
                                                         with_labels=True, with_aux=True, feature_name=feature_name)
         return {"query_id": q, "feature_tensor": {feature_name: ids, **feats}, "padding_mask": pad, "positive_labels": labels,
                 "target_padding_mask": tmask}
@@ -397,7 +545,7 @@ class DeviceSequenceStore:
         NextTokenTransform(shift=1) (nn/transform/next_token.py:65-96) + the unsqueeze of the default SASRec transform
         template -> feature_tensors{item_id, features...}, padding_mask, positive_labels [B,L,1], target_padding_mask
         [B,L,1] (+ seen_ids = the window).  ``seq_offset``: window starts (default: the last L + 1 events)."""
-        ids, pad, labels, tmask, q, feats = self._build(SASREC_TRAIN, seq_index, seq_offset, max_len, pad_value,
+        ids, pad, labels, tmask, q, feats, _ = self._build(SASREC_TRAIN, seq_index, seq_offset, max_len, pad_value,
                                                         with_labels=True, with_aux=True, new_path=True,
                                                         feature_name=feature_name)
         out = {"query_id": q, "feature_tensors": {feature_name: ids, **feats}, "padding_mask": pad,
@@ -411,7 +559,7 @@ class DeviceSequenceStore:
         """The predict transforms of the default SASRec template (nn/transform/template/sasrec.py): every column read at
         max_len (the last events, left-padded), no shift -> query_id, feature_tensors{item_id, features...}, padding_mask
         (+ seen_ids = the window)."""
-        ids, pad, _, _, q, feats = self._build(PREDICT, seq_index, None, max_len, pad_value, new_path=True,
+        ids, pad, _, _, q, feats, _ = self._build(PREDICT, seq_index, None, max_len, pad_value, new_path=True,
                                                feature_name=feature_name)
         out = {"query_id": q, "feature_tensors": {feature_name: ids, **feats}, "padding_mask": pad}
         if with_seen:
@@ -419,7 +567,7 @@ class DeviceSequenceStore:
         return out
 
     def sasrec_prediction_batch(self, seq_index, max_len: int, pad_value: int, feature_name="item_id"):
-        ids, pad, _, _, q, feats = self._build(PREDICT, seq_index, None, max_len, pad_value, feature_name=feature_name)
+        ids, pad, _, _, q, feats, _ = self._build(PREDICT, seq_index, None, max_len, pad_value, feature_name=feature_name)
         return {"query_id": q, "padding_mask": pad, "feature_tensor": {feature_name: ids, **feats}}
 
     def bert4rec_training_batch(self, seq_index, max_len: int, pad_value: int, mask_prob: float = 0.15, seq_offset=None,
@@ -427,7 +575,7 @@ class DeviceSequenceStore:
         """Reference keys (bert4rec/dataset.py:167-173), the feature columns unmasked under ``inputs``.  ``token_mask``
         False = masked.  Random draws: Philox keyed by (seed, draw0 + row); pass ``uniforms`` [B, L] to reproduce a given
         masker stream exactly."""
-        ids, pad, labels, tok, q, feats = self._build(BERT_TRAIN, seq_index, seq_offset, max_len, pad_value,
+        ids, pad, labels, tok, q, feats, _ = self._build(BERT_TRAIN, seq_index, seq_offset, max_len, pad_value,
                                                       mask_prob=mask_prob, uniforms=uniforms, seed=seed, draw0=draw0,
                                                       with_labels=True, with_aux=True, feature_name=feature_name)
         return {"query_id": q, "pad_mask": pad, "inputs": {feature_name: ids, **feats}, "token_mask": tok,
@@ -435,9 +583,54 @@ class DeviceSequenceStore:
 
     def bert4rec_prediction_batch(self, seq_index, max_len: int, pad_value: int, feature_name="item_id"):
         """_shift_features (bert4rec/dataset.py:322-351): every column shifted left, its padding value in the last slot."""
-        ids, pad, _, tok, q, feats = self._build(BERT_PREDICT, seq_index, None, max_len, pad_value, with_aux=True,
+        ids, pad, _, tok, q, feats, _ = self._build(BERT_PREDICT, seq_index, None, max_len, pad_value, with_aux=True,
                                                  feature_name=feature_name)
         return {"query_id": q, "pad_mask": pad, "inputs": {feature_name: ids, **feats}, "token_mask": tok}
+
+    # ------------------------------------------------------------------------------------ validation / test builders
+    def _legacy_lists(self, lists):
+        missing = [k for k in ("ground_truth", "train") if k not in lists]
+        if missing:
+            raise ValueError(f"the legacy validation batches need the query lists 'ground_truth' and 'train'; the store "
+                             f"lacks {missing}")
+        return lists
+
+    def sasrec_validation_batch(self, seq_index, max_len: int, pad_value: int, feature_name="item_id"):
+        """SasRecValidationDataset.__getitem__ + default collate (sasrec/dataset.py:218-268): the prediction window and
+        every query list, first entries right-padded -> query_id, padding_mask, feature_tensor, ground_truth, train."""
+        ids, pad, _, _, q, feats, lists = self._build(PREDICT, seq_index, None, max_len, pad_value,
+                                                      feature_name=feature_name, query_layout="first")
+        return {"query_id": q, "padding_mask": pad, "feature_tensor": {feature_name: ids, **feats},
+                **self._legacy_lists(lists)}
+
+    def bert4rec_validation_batch(self, seq_index, max_len: int, pad_value: int, feature_name="item_id"):
+        """Bert4RecValidationDataset.__getitem__ + default collate (bert4rec/dataset.py:264-320): the shifted prediction
+        window and every query list, first entries right-padded -> query_id, pad_mask, inputs, token_mask, ground_truth,
+        train."""
+        ids, pad, _, tok, q, feats, lists = self._build(BERT_PREDICT, seq_index, None, max_len, pad_value, with_aux=True,
+                                                        feature_name=feature_name, query_layout="first")
+        return {"query_id": q, "pad_mask": pad, "inputs": {feature_name: ids, **feats}, "token_mask": tok,
+                **self._legacy_lists(lists)}
+
+    def sasrec_new_path_validation_batch(self, seq_index, max_len: int, pad_value: int, feature_name="item_id",
+                                         seen_list: str | None = "train"):
+        """The validate / test transforms of the default SASRec template (nn/transform/template/sasrec.py:27-31) on the
+        columns the reader cuts at their metadata's shape: every column read at max_len, no shift, and every query list's
+        last ``width`` entries left-padded -> query_id [B] (the reader's query column), feature_tensors, padding_mask,
+        the query lists under their names
+        and ``seen_ids`` for ``SeenItemsFilter``: the query list named ``seen_ids`` when the store has one, else the
+        list ``seen_list`` (None: the window, as the prediction batch)."""
+        ids, pad, _, _, q, feats, lists = self._build(PREDICT, seq_index, None, max_len, pad_value, new_path=True,
+                                                      feature_name=feature_name, query_layout="last")
+        out = {"query_id": q.view(-1), "feature_tensors": {feature_name: ids, **feats}, "padding_mask": pad, **lists}
+        if "seen_ids" not in out:
+            if seen_list is not None and seen_list not in lists:
+                raise ValueError(f"seen_list {seen_list!r} is not a query list of the store {self.query_list_names}")
+            out["seen_ids"] = ids if seen_list is None else lists[seen_list]
+        return out
+
+
+VALIDATION_KINDS = ("sasrec_validate", "bert4rec_validate", "sasrec_new_validate")
 
 
 class DeviceBatchLoader:
@@ -446,17 +639,31 @@ class DeviceBatchLoader:
     generator shared by all ranks, padded by wrap-around to a multiple of the world size (DistributedSampler semantics) and
     strided over the ranks; every batch is then one kernel launch on HBM-resident data.  ``kind``: ``"sasrec"`` (the
     legacy SasRec's batches), ``"sasrec_new"`` (new-path training batches for ``LightningModule(SasRec | TwoTower)``) or
-    ``"bert4rec"``."""
+    ``"bert4rec"``.
+
+    The validation / test kinds ``"sasrec_validate"``, ``"bert4rec_validate"`` and ``"sasrec_new_validate"`` yield the
+    store's validation batches instead: every stored query exactly once, in store order, the last batch kept partial.
+    Under ``world_size > 1`` each rank takes its contiguous shard of ``trainer.user_shard``, so the ranks together visit
+    every query once with no wrap-around duplicates; ``shuffle``, ``drop_last``, ``sliding_window_step`` and
+    ``partitioning`` do not apply."""
 
     def __init__(self, store: DeviceSequenceStore, max_len: int, batch_size: int, pad_value: int, kind: str = "sasrec",
                  sliding_window_step: int | None = None, shuffle: bool = True, drop_last: bool = False, seed: int = 0,
                  rank: int = 0, world_size: int = 1, mask_prob: float = 0.15, partitioning: str = "sampler"):
-        if kind not in ("sasrec", "sasrec_new", "bert4rec"):
+        if kind not in ("sasrec", "sasrec_new", "bert4rec") + VALIDATION_KINDS:
             raise ValueError(f"unknown kind {kind!r}")
         if partitioning not in ("sampler", "replay"):
             raise ValueError(f"unknown partitioning {partitioning!r}")
         self.partitioning = partitioning
         self.store, self.L, self.bs, self.pad, self.kind = store, int(max_len), int(batch_size), int(pad_value), kind
+        self.rank, self.world, self.epoch = rank, world_size, 0
+        if kind in VALIDATION_KINDS:
+            from .trainer import user_shard
+
+            self.lo, hi = user_shard(store.n_seq, rank, world_size)
+            self.n = self.per_rank = hi - self.lo
+            self.drop_last = False
+            return
         window = self.L + (1 if kind in ("sasrec", "sasrec_new") else 0)
         seq, off = window_index(store.lengths, window, sliding_window_step)
         self.win_seq = torch.from_numpy(seq).to(store.device)
@@ -495,6 +702,15 @@ class DeviceBatchLoader:
         return order[self.rank: total: self.world]
 
     def __iter__(self):
+        if self.kind in VALIDATION_KINDS:
+            build = {"sasrec_validate": self.store.sasrec_validation_batch,
+                     "bert4rec_validate": self.store.bert4rec_validation_batch,
+                     "sasrec_new_validate": self.store.sasrec_new_path_validation_batch}[self.kind]
+            for i in range(len(self)):
+                lo = self.lo + i * self.bs
+                s = torch.arange(lo, min(lo + self.bs, self.lo + self.n), dtype=torch.int32, device=self.store.device)
+                yield build(s, self.L, self.pad)
+            return
         mine = self.epoch_indices()
         for i in range(len(self)):
             idx = mine[i * self.bs: (i + 1) * self.bs]
